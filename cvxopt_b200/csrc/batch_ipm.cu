@@ -328,8 +328,8 @@ struct cvxb_batch {
     int iters_run = 0;
     double solve_ms = 0;
     // single large problem: SYRK on the int8 tensor path (ozaki_syrk.cu), same rule as cvxb_kkt_factor:
-    // mode 1 when B == 1, n >= 4096, m >= 8192; 2: whenever B == 1; 0 (default): never.  CVXB_OZAKI (or the
-    // older CVXB_OZAKI_IPM) = 0/1/2 read at create.
+    // mode 1 when B == 1, n >= 4096, m >= 8192; 2: whenever B == 1; 0 (default): never.  CVXB_OZAKI = 0/1/2
+    // read at create.
     int i8_mode = 0;
     int syrk_path = 0;
     void *oz_work = nullptr;
@@ -419,7 +419,6 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     cvxb_batch *b = new cvxb_batch();
     b->device = device; b->B = nprob; b->n = n; b->m = m;
     if (const char *e = getenv("CVXB_OZAKI")) b->i8_mode = (e[0] == '0') ? 0 : (e[0] == '2') ? 2 : 1;
-    if (const char *e = getenv("CVXB_OZAKI_IPM")) b->i8_mode = (e[0] == '1') ? 1 : (e[0] == '2') ? 2 : 0;
     b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
     b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;

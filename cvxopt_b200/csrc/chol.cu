@@ -74,10 +74,6 @@ potf2_inv_kernel(double *A, long long lda, int jb, double *inv, double *invT, in
         unsigned long long t_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_));       \
         trace[8 * 2048 + (SLOT)] = t_;                                                      \
     }
-    // Programmatic dependent launch (CVXB_CHOL_PDL): the next diagonal-block kernel of the chain may be scheduled while
-    // this one runs; it blocks here until its predecessor has completed and flushed.  No-ops for ordinary launches.
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    asm volatile("griddepcontrol.launch_dependents;");
     A += (long long)blockIdx.x * sA; inv += (long long)blockIdx.x * sInv;
     invT += (long long)blockIdx.x * sInv; info += blockIdx.x;
     double *M = sm;                    // NB x LDM, column-major
@@ -387,277 +383,6 @@ potf2_inv_kernel(double *A, long long lda, int jb, double *inv, double *invT, in
     }
 }
 
-// ---- trailing update of the blocked factorisation:  A22(lower) -= L21 L21'  for one 128-wide panel ----
-// In the generic DMMA GEMM this K = 128 update runs well below the DMMA peak: every 128x64
-// tile is its own CTA with a pipeline prologue and an epilogue for only eight k steps.  Here a CTA (one per SM at a
-// time) walks a few consecutive 128x128 tiles strip by strip (strip = block column cb of the trailing matrix, rb >= cb):
-//   * the strip's column operand L21[cb rows, 0:128] (128 KB) stays in shared memory for all tiles of the strip;
-//   * the row operand streams through two 32-column buffers, the copy of the next chunk -- of the next TILE after
-//     the last chunk -- in flight under the DMMAs of the current one, so there is no per-tile prologue;
-//   * the tile of A22 goes straight into the accumulator fragments (acc = C, a-fragments negated: acc = C - L L')
-//     and is stored from them: no shared-memory staging, no epilogue barrier.
-// STATUS: validated correct (tests/test_kkt_gpu.py, tests/test_fullsize_gpu.py with CVXB_CHOL_TU=1) but SLOWER than the
-// generic kernel when it was tuned (one 8-warp CTA per SM without register double-buffering of the fragments and
-// with the C tile's load/store latency exposed at every tile boundary does not keep the DMMA pipe as busy as two
-// 4-warp CTAs of the generic kernel do; not re-measured on H100).  Opt-in: CVXB_CHOL_TU=1.
-// W = L21 (m x 128, column-major, ld ldw); tiles of block column 0 are left to the caller (the panel stream updates
-// the next block column itself).  Requires even ldc / 16-byte aligned C (the caller falls back to dmma_gemm otherwise).
-constexpr int TU_LD = NB + 4;                   // 132: row stride of the [k][idx] operand buffers (conflict-free LDS.64)
-constexpr int TU_CH = 32;                       // k columns per streamed chunk
-constexpr int TU_NCH = NB / TU_CH;
-constexpr int TU_SMEM = (NB * TU_LD + 2 * TU_CH * TU_LD) * 8;      // 202752 B
-
-__global__ void __launch_bounds__(256, 1)
-chol_trailing_kernel(int m, const double *__restrict__ W, long long ldw, double *C, long long ldc, int nbk, int cb0,
-                     long long T, unsigned long long *trace) {
-    extern __shared__ __align__(16) double sm[];
-    double *Bs = sm;                            // [128 k][TU_LD]  rows of block column cb
-    double *As = sm + NB * TU_LD;               // 2 x [32 k][TU_LD]  rows of block rb
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wr = warp & 1, wc = warp >> 1;
-    const int g4 = lane >> 2, t4 = lane & 3;
-    if (trace && tid == 0) {
-        unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        atomicCAS(trace, 0ULL, t);
-    }
-    const long long t0 = T * blockIdx.x / gridDim.x, t1 = T * (blockIdx.x + 1) / gridDim.x;
-    if (t0 >= t1) return;
-    // tile t -> (cb, rb): strips cb = cb0 .. nbk-1, strip cb holds rb = cb .. nbk-1
-    int cb = cb0, rb;
-    {
-        long long t = t0;
-        while (t >= nbk - cb) { t -= nbk - cb; ++cb; }
-        rb = cb + (int)t;
-    }
-    auto issue_rows = [&](double *dst, int blk, int k0, int nk) {       // dst[kk][r] = W[blk*128 + r, k0 + kk]
-        for (int q = tid; q < nk * (NB / 2); q += 256) {
-            const int kk = q >> 6, rr = (q & 63) * 2;
-            const long long row = (long long)blk * NB + rr;
-            const int bytes = (row + 1 < m) ? 16 : (row < m ? 8 : 0);
-            cp_async16(dst + kk * TU_LD + rr, bytes ? W + row + (long long)(k0 + kk) * ldw : W, bytes);
-        }
-    };
-    int cur_cb = -1, buf = 0;
-    issue_rows(As, rb, 0, TU_CH);
-    cp_async_commit();
-    for (long long t = t0; t < t1; ++t) {
-        if (cb != cur_cb) {                     // new strip: every warp is past the previous tile's last barrier
-            issue_rows(Bs, cb, 0, NB);
-            cp_async_commit();
-            cur_cb = cb;
-        }
-        // ---- the tile of A22 -> accumulators ----
-        const long long r0 = (long long)rb * NB, c0 = (long long)cb * NB;
-        const bool interior = (rb > cb) && (r0 + NB <= m);
-        double acc[4][8][2];
-        double *Ct = C + r0 + c0 * ldc;
-#pragma unroll
-        for (int cf = 0; cf < 4; ++cf) {
-            const int cl = wc * 32 + cf * 8 + g4;
-#pragma unroll
-            for (int rf = 0; rf < 8; ++rf) {
-                const int rl = wr * 64 + rf * 8 + t4 * 2;
-                if (interior) {
-                    const double2 v = *reinterpret_cast<const double2 *>(Ct + rl + cl * ldc);
-                    acc[cf][rf][0] = v.x; acc[cf][rf][1] = v.y;
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const long long r = r0 + rl + e, c = c0 + cl;
-                        acc[cf][rf][e] = (r < m && c < m && r >= c) ? Ct[rl + e + cl * ldc] : 0.0;
-                    }
-                }
-            }
-        }
-        // next tile (for the cross-tile prefetch)
-        int ncb = cb, nrb = rb + 1;
-        if (nrb >= nbk) { ++ncb; nrb = ncb; }
-        const bool has_next = (t + 1 < t1);
-#pragma unroll 1
-        for (int ch = 0; ch < TU_NCH; ++ch) {
-            if (ch + 1 < TU_NCH) issue_rows(As + (buf ^ 1) * TU_CH * TU_LD, rb, (ch + 1) * TU_CH, TU_CH);
-            else if (has_next) issue_rows(As + (buf ^ 1) * TU_CH * TU_LD, nrb, 0, TU_CH);
-            cp_async_commit();
-            cp_async_wait<1>();                 // everything but the chunk just issued has landed (incl. a new Bs)
-            __syncthreads();
-            const double *Ab = As + buf * TU_CH * TU_LD + (wr * 64 + g4) + t4 * TU_LD;
-            const double *Bb = Bs + (ch * TU_CH) * TU_LD + (wc * 32 + g4) + t4 * TU_LD;
-#pragma unroll
-            for (int kk = 0; kk < TU_CH / 4; ++kk) {
-                double a[4], bf[8];
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf) a[cf] = -Bb[cf * 8 + kk * 4 * TU_LD];
-#pragma unroll
-                for (int rf = 0; rf < 8; ++rf) bf[rf] = Ab[rf * 8 + kk * 4 * TU_LD];
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf)
-#pragma unroll
-                    for (int rf = 0; rf < 8; ++rf) dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf], bf[rf]);
-            }
-            __syncthreads();                    // the buffer may be refilled by the next issue
-            buf ^= 1;
-        }
-        // ---- accumulators -> A22 ----
-#pragma unroll
-        for (int cf = 0; cf < 4; ++cf) {
-            const int cl = wc * 32 + cf * 8 + g4;
-#pragma unroll
-            for (int rf = 0; rf < 8; ++rf) {
-                const int rl = wr * 64 + rf * 8 + t4 * 2;
-                if (interior) {
-                    *reinterpret_cast<double2 *>(Ct + rl + cl * ldc) = make_double2(acc[cf][rf][0], acc[cf][rf][1]);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const long long r = r0 + rl + e, c = c0 + cl;
-                        if (r < m && c < m && r >= c) Ct[rl + e + cl * ldc] = acc[cf][rf][e];
-                    }
-                }
-            }
-        }
-        cb = ncb; rb = nrb;
-    }
-    cp_async_wait<0>();
-    if (trace && tid == 0) {
-        unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        atomicMax(trace + 1, t);
-    }
-}
-
-// Second form of the strip kernel (CVXB_CHOL_TU=2; validated, also slower when it was tuned): the generic GEMM's geometry -- 128x64 tiles, four warps, two CTAs per
-// SM so that one CTA's tile boundary (store C, load the next C into the accumulators) runs under the other's DMMAs --
-// but a CTA walks several consecutive tiles of a 64-column strip and its 3-stage operand ring never drains: the chunks
-// of the next tile follow the last chunk of the current one.
-constexpr int T2_BC = 64, T2_LDA = NB + 4, T2_LDB = T2_BC + 4, T2_CH = 16, T2_ST = 3;
-constexpr int T2_STAGE = T2_CH * (T2_LDA + T2_LDB);            // doubles per stage: A chunk then B chunk
-constexpr int T2_SMEM = T2_ST * T2_STAGE * 8;                  // 76800 B
-constexpr int T2_NCH = NB / T2_CH;                             // 8 chunks per tile
-
-__global__ void __launch_bounds__(128, 2)
-chol_trailing2_kernel(int m, const double *__restrict__ W, long long ldw, double *C, long long ldc, int nbk, long long T,
-                      unsigned long long *trace) {
-    extern __shared__ __align__(16) double sm[];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int wr = warp & 1, wc = warp >> 1;
-    const int g4 = lane >> 2, t4 = lane & 3;
-    if (trace && tid == 0) {
-        unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        atomicCAS(trace, 0ULL, t);
-    }
-    const long long t0 = T * blockIdx.x / gridDim.x, t1 = T * (blockIdx.x + 1) / gridDim.x;
-    if (t0 >= t1) return;
-    // tile t -> (cs, rb): 64-column strips cs = 2 .. 2*nbk-1 (the first 128 columns belong to the panel stream),
-    // strip cs holds the 128-row blocks rb = cs/2 .. nbk-1
-    int cs = 2, rb;
-    {
-        long long t = t0;
-        while (t >= nbk - (cs >> 1)) { t -= nbk - (cs >> 1); ++cs; }
-        rb = (cs >> 1) + (int)t;
-    }
-    auto issue = [&](int stage, int rblk, int cstrip, int k0) {
-        double *As = sm + stage * T2_STAGE, *Bs = As + T2_CH * T2_LDA;
-        for (int q = tid; q < T2_CH * (NB / 2); q += 128) {           // A: rows of block rblk
-            const int kk = q >> 6, rr = (q & 63) * 2;
-            const long long row = (long long)rblk * NB + rr;
-            const int bytes = (row + 1 < m) ? 16 : (row < m ? 8 : 0);
-            cp_async16(As + kk * T2_LDA + rr, bytes ? W + row + (long long)(k0 + kk) * ldw : W, bytes);
-        }
-        for (int q = tid; q < T2_CH * (T2_BC / 2); q += 128) {        // B: rows of strip cstrip
-            const int kk = q >> 5, rr = (q & 31) * 2;
-            const long long row = (long long)cstrip * T2_BC + rr;
-            const int bytes = (row + 1 < m) ? 16 : (row < m ? 8 : 0);
-            cp_async16(Bs + kk * T2_LDB + rr, bytes ? W + row + (long long)(k0 + kk) * ldw : W, bytes);
-        }
-    };
-    // the chunk stream of this CTA: chunk q of tile i; `pf_*` walks two chunks ahead of the compute position
-    int pf_cs = cs, pf_rb = rb, pf_ch = 0;
-    long long pf_t = t0;
-    int pf_stage = 0;
-    auto prefetch = [&]() {
-        if (pf_t < t1) {
-            issue(pf_stage, pf_rb, pf_cs, pf_ch * T2_CH);
-            if (++pf_ch == T2_NCH) {
-                pf_ch = 0; ++pf_t;
-                if (++pf_rb >= nbk) { ++pf_cs; pf_rb = pf_cs >> 1; }
-            }
-        }
-        cp_async_commit();
-        if (++pf_stage == T2_ST) pf_stage = 0;
-    };
-    prefetch();
-    prefetch();
-    int stage = 0;
-    for (long long t = t0; t < t1; ++t) {
-        const long long r0 = (long long)rb * NB, c0 = (long long)cs * T2_BC;
-        const bool interior = (r0 >= c0 + T2_BC) && (r0 + NB <= m);
-        double acc[4][8][2];
-        double *Ct = C + r0 + c0 * ldc;
-#pragma unroll
-        for (int cf = 0; cf < 4; ++cf) {
-            const int cl = wc * 32 + cf * 8 + g4;
-#pragma unroll
-            for (int rf = 0; rf < 8; ++rf) {
-                const int rl = wr * 64 + rf * 8 + t4 * 2;
-                if (interior) {
-                    const double2 v = *reinterpret_cast<const double2 *>(Ct + rl + cl * ldc);
-                    acc[cf][rf][0] = v.x; acc[cf][rf][1] = v.y;
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const long long r = r0 + rl + e, c = c0 + cl;
-                        acc[cf][rf][e] = (r < m && c < m && r >= c) ? Ct[rl + e + cl * ldc] : 0.0;
-                    }
-                }
-            }
-        }
-#pragma unroll 1
-        for (int ch = 0; ch < T2_NCH; ++ch) {
-            cp_async_wait<T2_ST - 2>();         // this chunk has landed (one newer group may be in flight)
-            __syncthreads();                    // ... for every thread; the stage read last iteration is free
-            prefetch();                         // two chunks ahead, into the stage freed by the barrier above
-            const double *As = sm + stage * T2_STAGE, *Bs = As + T2_CH * T2_LDA;
-            const double *Ab = As + (wr * 64 + g4) + t4 * T2_LDA;
-            const double *Bb = Bs + (wc * 32 + g4) + t4 * T2_LDB;
-#pragma unroll
-            for (int kk = 0; kk < T2_CH / 4; ++kk) {
-                double a[4], bf[8];
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf) a[cf] = -Bb[cf * 8 + kk * 4 * T2_LDB];
-#pragma unroll
-                for (int rf = 0; rf < 8; ++rf) bf[rf] = Ab[rf * 8 + kk * 4 * T2_LDA];
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf)
-#pragma unroll
-                    for (int rf = 0; rf < 8; ++rf) dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf], bf[rf]);
-            }
-            if (++stage == T2_ST) stage = 0;
-        }
-#pragma unroll
-        for (int cf = 0; cf < 4; ++cf) {
-            const int cl = wc * 32 + cf * 8 + g4;
-#pragma unroll
-            for (int rf = 0; rf < 8; ++rf) {
-                const int rl = wr * 64 + rf * 8 + t4 * 2;
-                if (interior) {
-                    *reinterpret_cast<double2 *>(Ct + rl + cl * ldc) = make_double2(acc[cf][rf][0], acc[cf][rf][1]);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const long long r = r0 + rl + e, c = c0 + cl;
-                        if (r < m && c < m && r >= c) Ct[rl + e + cl * ldc] = acc[cf][rf][e];
-                    }
-                }
-            }
-        }
-        if (++rb >= nbk) { ++cs; rb = cs >> 1; }
-    }
-    cp_async_wait<0>();
-    if (trace && tid == 0) {
-        unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        atomicMax(trace + 1, t);
-    }
-}
-
 // ---- blocked triangular solve with one right-hand side ------------------------
 // forward:  L x = b ;  backward: L' x = b.   In place on b.  One CTA per 128-row block.
 // flags[i] == epoch  <=>  x_i is final in b.
@@ -829,10 +554,7 @@ int chol_work_create(CholWork &w) {
     CVXB_CUDA(cudaStreamCreateWithPriority(&w.trsm_stream, cudaStreamNonBlocking, greatest));
     CVXB_CUDA(cudaStreamCreateWithPriority(&w.update_stream, cudaStreamNonBlocking, least));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_t, cudaEventDisableTiming));
-    w.r_valid[0] = w.r_valid[1] = -1;
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_start, cudaEventDisableTiming));
-    CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_panel, cudaEventDisableTiming));
-    CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_rest, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_p, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_u, cudaEventDisableTiming));
     CVXB_CUDA(cudaMalloc(&w.d_info, sizeof(int)));
@@ -841,8 +563,6 @@ int chol_work_create(CholWork &w) {
     CVXB_CUDA(cudaMalloc(&w.d_flags, 4096 * sizeof(int)));
     CVXB_CUDA(cudaMemset(w.d_flags, 0, 4096 * sizeof(int)));
     CVXB_CUDA(cudaMalloc(&w.splitk_ws, dmma_gemm_splitk_ws_doubles() * sizeof(double)));
-    CVXB_CUDA(cudaFuncSetAttribute(chol_trailing_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TU_SMEM));
-    CVXB_CUDA(cudaFuncSetAttribute(chol_trailing2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T2_SMEM));
     CVXB_CUDA(cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    POTF2_SMEM));
     CVXB_CUDA(cudaFuncSetAttribute(trsv_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TRSV_SMEM));
@@ -862,8 +582,6 @@ void chol_work_destroy(CholWork &w) {
     for (auto *v : {&w.ev_dg, &w.ev_tr, &w.ev_c0, &w.ev_r})
         for (cudaEvent_t e : *v) cudaEventDestroy(e);
     if (w.ev_start) cudaEventDestroy(w.ev_start);
-    if (w.ev_panel) cudaEventDestroy(w.ev_panel);
-    if (w.ev_rest) cudaEventDestroy(w.ev_rest);
     if (w.ev_end_p) cudaEventDestroy(w.ev_end_p);
     if (w.ev_end_u) cudaEventDestroy(w.ev_end_u);
     if (w.d_info) cudaFree(w.d_info);
@@ -894,10 +612,10 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             if (w.panel[i]) CVXB_CUDA(cudaFree(w.panel[i]));
             w.panel[i] = nullptr;
         }
-        // two group buffers, each holding the TRSM results of a PAIR of consecutive panels side by side
-        // (rows x 2 NB), so that the bulk trailing update of a pair is one K = 256 product
+        // two panel buffers (rows x NB): the TRSM result of step jb goes to panel[jb & 1], so it can be
+        // written while the bulk update of step jb-1 still reads the other one
         const int rows = (n + 1) & ~1;
-        for (int i = 0; i < 2; ++i) CVXB_CUDA(cudaMalloc(&w.panel[i], (size_t)rows * 2 * NB * sizeof(double)));
+        for (int i = 0; i < 2; ++i) CVXB_CUDA(cudaMalloc(&w.panel[i], (size_t)rows * NB * sizeof(double)));
         w.panel_rows = rows;
     }
     while ((int)w.ev_dg.size() < nblk) {
@@ -917,25 +635,6 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
     CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_start, 0));
     CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_start, 0));
     CVXB_CUDA(cudaStreamWaitEvent(U, w.ev_start, 0));
-    // Pair aggregation of the bulk update (opt-in, CVXB_CHOL_PAIR=1; slower when it was tuned, not re-measured on
-    // H100: the K = 256 column update of the odd steps lengthens the panel path while the chain, not the bulk
-    // rate, sets the pace):
-    //   even step 2g  : TRSM -> group buffer columns [0, NB);  C0 (K = NB) completes block column 2g+1;
-    //                   D0: diagonal tile (2g+2, 2g+2) -= its panel-2g part (the only tile of block column 2g+2
-    //                   the diagonal chain needs before the pair's bulk update exists); NO bulk update.
-    //   odd step 2g+1 : TRSM -> columns [NB, 2 NB);  C0 with K = 2 NB (panels 2g and 2g+1) completes block
-    //                   column 2g+2 below its diagonal tile;  bulk R with K = 2 NB on block columns >= 2g+3.
-    // A K = 128 update leaves the DMMA pipe partly idle (prologue + read-modify-write epilogue per 8 k steps);
-    // K = 256 halves the C traffic and the per-tile overhead of the bulk flops.
-    // CVXB_CHOL_PAIR = 0 off (default), 1 every step, k >= 2: the first k (even) steps only — the pair form helps
-    // where the bulk update sets the pace (large trailing matrix) and hurts once the diagonal chain does.
-    static int pair_mode = -1;
-    if (pair_mode < 0) {
-        const char *e = getenv("CVXB_CHOL_PAIR");
-        pair_mode = e ? atoi(e) : 0;
-        if (pair_mode < 0) pair_mode = 0;
-    }
-    const int pair_limit = pair_mode == 1 ? (1 << 30) : (pair_mode & ~1);
     int last_r = -1;                       // last step that recorded ev_r
     int prev_r = -1;                       // the one before
     for (int jb = 0; jb < nblk; ++jb) {
@@ -945,49 +644,21 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         double *Ajj = A + j + (long long)j * lda;
         double *invj = inv + (long long)jb * NB * NB;
         double *invTj = inv + (long long)(nblk + jb) * NB * NB;
-        const bool pair = jb < pair_limit;
-        const bool pair_prev = (jb - 1) < pair_limit;
-        const bool odd = pair && (jb & 1);
-        // Group buffer of this step.  Its row r is global row R0 + r, R0 = first row below the EVEN panel's
-        // diagonal block, for both panels of the pair: the odd panel's TRSM result therefore sits at column
-        // offset NB and row offset NB.  `Wo` = buffer row of this step's first trailing row (A22).
-        double *Wg = pair ? w.panel[(jb >> 1) & 1] : w.panel[jb & 1];
-        double *Wp = Wg + (odd ? (long long)NB * ldw + NB : 0);
-        double *Wo = Wg + (odd ? NB : 0);
+        double *Wp = w.panel[jb & 1];
         // ---- D: diagonal block.  Needs A(jb,jb) updated through panel jb-2 and the raw tile A(jb,jb-1)
-        // (block column jb-1 complete through panel jb-2): C0(jb-2) [which follows D0(jb-2) on T] and the
-        // last bulk update that touched block column jb.
-        static int nowait = -1;      // timing experiment only (WRONG results): chain stream without its cross-stream waits
-        if (nowait < 0) { const char *e = getenv("CVXB_CHOL_NOWAIT_EXPERIMENT"); nowait = (e && e[0] == '1') ? 1 : 0; }
-        if (jb >= 2 && !nowait) {
+        // (block column jb-1 complete through panel jb-2): C0(jb-2) and the last bulk update that touched
+        // block column jb.
+        if (jb >= 2) {
             CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_c0[jb - 2], 0));
             // the latest bulk update issued at a step <= jb-2 (a later one belongs to panels the prologue
             // applies itself, waiting for it would serialise the chain behind the bulk work)
-            // (pair region, odd step: the pair's own bulk update (step jb-2) does not touch this step's diagonal
-            // tile — the odd step's column update C1 did — so the one before it is the one to wait for)
-            const int rd = (pair_prev && (jb & 1) && last_r == jb - 2) ? prev_r : ((last_r <= jb - 2) ? last_r : prev_r);
+            const int rd = (last_r <= jb - 2) ? last_r : prev_r;
             if (rd >= 0) CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_r[rd], 0));
         }
         const double *Tprev = jb > 0 ? A + j + (long long)(j - NB) * lda : nullptr;
         const double *invprev = jb > 0 ? inv + (long long)(jb - 1) * NB * NB : nullptr;
-        static int pdl = -1;
-        if (pdl < 0) { const char *e = getenv("CVXB_CHOL_PDL"); pdl = (e && e[0] == '1') ? 1 : 0; }
-        if (pdl && jb > 0) {
-            // the edge potf2(jb-1) -> potf2(jb) on the chain stream becomes a programmatic dependency: the launch
-            // latency (a visible share of a chain step) overlaps the predecessor
-            cudaLaunchConfig_t cfg = {};
-            cfg.gridDim = dim3(1); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = POTF2_SMEM; cfg.stream = D;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            at[0].val.programmaticStreamSerializationAllowed = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
-            unsigned long long *tr = w.trace ? w.trace + 8 * jb : nullptr;
-            CVXB_CUDA(cudaLaunchKernelEx(&cfg, potf2_inv_kernel, Ajj, (long long)lda, wj, invj, invTj, w.d_info, j,
-                                         (long long)0, (long long)0, Tprev, (long long)lda, invprev, tr));
-        } else {
-            potf2_inv_kernel<<<1, 256, POTF2_SMEM, D>>>(Ajj, lda, wj, invj, invTj, w.d_info, j, 0, 0, Tprev,
-                                                         lda, invprev, w.trace ? w.trace + 8 * jb : nullptr);
-        }
+        potf2_inv_kernel<<<1, 256, POTF2_SMEM, D>>>(Ajj, lda, wj, invj, invTj, w.d_info, j, 0, 0, Tprev,
+                                                     lda, invprev, w.trace ? w.trace + 8 * jb : nullptr);
         count_launch();
         CVXB_LAUNCH_CHECK();
         CVXB_CUDA(cudaEventRecord(w.ev_dg[jb], D));
@@ -996,10 +667,8 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         auto copy_back_prev = [&]() -> int {
             if (jb == 0) return 0;
             const int jp = j - NB, mp = n - j;
-            const int pb = jb - 1;
-            const double *src = pair_prev ? w.panel[(pb >> 1) & 1] + ((pb & 1) ? (long long)NB * ldw + NB : 0) : w.panel[pb & 1];
             CVXB_CUDA(cudaMemcpy2DAsync(A + j + (long long)jp * lda, (size_t)lda * sizeof(double),
-                                        src, (size_t)ldw * sizeof(double),
+                                        w.panel[(jb - 1) & 1], (size_t)ldw * sizeof(double),
                                         (size_t)mp * sizeof(double), NB, cudaMemcpyDeviceToDevice, T));
             return 0;
         };
@@ -1012,9 +681,8 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         double *A22 = A21 + (long long)wj * lda;
         // ---- T: panel TRSM as a GEMM with the block inverse (out of place) ----
         CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_dg[jb], 0));
-        // the group buffer about to be overwritten was read by the bulk update two groups (steps) ago
-        if (!odd && prev_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[prev_r], 0));
-        if (!pair && pair_prev && last_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[last_r], 0));   // mode switch
+        // the panel buffer about to be overwritten was read by the bulk update two steps ago
+        if (prev_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[prev_r], 0));
         {
             GemmDesc g;
             g.M = m; g.N = wj; g.K = wj;
@@ -1028,29 +696,11 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         // every later write of this step into block columns >= jb+1 is ordered behind the last bulk update
         if (last_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[last_r], 0));
         const int wn = (m < NB) ? m : NB;          // width of block column jb+1
-        // ---- T (even step of a pair): diagonal tile of block column jb+2 gets its panel-jb part now ----
-        if (pair && !odd && m > NB) {
-            const int w2 = (m - NB < NB) ? (m - NB) : NB;
-            GemmDesc d0;
-            d0.M = w2; d0.N = w2; d0.K = wj;
-            d0.X = Wp + NB; d0.ldx = ldw; d0.x_kmajor = false;
-            d0.Y = Wp + NB; d0.ldy = ldw; d0.y_kmajor = false;
-            double *tile = A22 + NB + (long long)NB * lda;
-            d0.D = tile; d0.ldd = lda; d0.C = tile; d0.ldc = lda;
-            d0.alpha = -1.0; d0.beta = 1.0; d0.lower_only = true;
-            CVXB_TRY(dmma_gemm(d0, T));
-        }
         // ---- T: next block column, rows below its diagonal block ----
         if (m > wn) {
             GemmDesc c;
-            c.M = m - wn; c.N = wn;
-            if (odd) {          // both panels of the pair: rows of the group buffer, K = NB + wj
-                c.K = NB + wj;
-                c.X = Wo + wn; c.Y = Wo;
-            } else {
-                c.K = wj;
-                c.X = Wp + wn; c.Y = Wp;
-            }
+            c.M = m - wn; c.N = wn; c.K = wj;
+            c.X = Wp + wn; c.Y = Wp;
             c.ldx = ldw; c.x_kmajor = false;
             c.ldy = ldw; c.y_kmajor = false;
             c.D = A22 + wn; c.ldd = lda; c.C = A22 + wn; c.ldc = lda;
@@ -1058,77 +708,25 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             c.trace = w.trace ? w.trace + 8 * jb + 4 : nullptr;
             CVXB_TRY(dmma_gemm(c, T));
         }
-        // ---- T (odd step of a pair): block column jb+2 INCLUDING its diagonal tile gets both panels now, so that
-        // the diagonal chain two steps ahead does not wait for this pair's bulk update
-        if (odd && m > NB) {
-            GemmDesc c1;
-            c1.M = m; c1.N = m; c1.K = NB + wj;
-            c1.X = Wo; c1.Y = Wo; c1.ldx = ldw; c1.x_kmajor = false; c1.ldy = ldw; c1.y_kmajor = false;
-            c1.D = A22; c1.ldd = lda; c1.C = A22; c1.ldc = lda;
-            c1.alpha = -1.0; c1.beta = 1.0; c1.lower_only = true;
-            c1.ct_begin = panel_tiles; c1.ct_end = 2 * panel_tiles;
-            CVXB_TRY(dmma_gemm(c1, T));
-        }
         CVXB_CUDA(cudaEventRecord(w.ev_c0[jb], T));
         CVXB_TRY(copy_back_prev());
         // ---- U: the rest of the trailing matrix ----
-        if ((pair ? (odd && m > 2 * NB) : (m > NB))) {
+        if (m > NB) {
             CVXB_CUDA(cudaStreamWaitEvent(U, w.ev_tr[jb], 0));
             GemmDesc u;
-            u.M = m; u.N = m;
-            if (odd) { u.K = NB + wj; u.X = Wo; u.Y = Wo; }
-            else { u.K = wj; u.X = Wp; u.Y = Wp; }
-            u.ldx = ldw; u.x_kmajor = false;
-            u.ldy = ldw; u.y_kmajor = false;
+            u.M = m; u.N = m; u.K = wj;
+            u.X = Wp; u.ldx = ldw; u.x_kmajor = false;
+            u.Y = Wp; u.ldy = ldw; u.y_kmajor = false;
             u.D = A22; u.ldd = lda; u.C = A22; u.ldc = lda;
             u.alpha = -1.0; u.beta = 1.0; u.lower_only = true;
-            u.ct_begin = odd ? 2 * panel_tiles : panel_tiles; u.ct_end = 1 << 30;
+            u.ct_begin = panel_tiles; u.ct_end = 1 << 30;
             u.trace = w.trace ? w.trace + 8 * jb + 6 : nullptr;
-            static int tu_on = -1;
-            // correct, but slower than the generic GEMM when it was tuned (not re-measured on H100), so it is an
-            // opt-in experiment (CVXB_CHOL_TU=1), the generic GEMM stays default
-            if (tu_on < 0) { const char *e = getenv("CVXB_CHOL_TU"); tu_on = (e && (e[0] == '1' || e[0] == '2')) ? e[0] - '0' : 0; }
-            const bool tu = tu_on && !odd && !pair && wj == NB && (lda & 1) == 0 && (ldw & 1) == 0 &&
-                            ((reinterpret_cast<uintptr_t>(A22) & 15) == 0) && ((reinterpret_cast<uintptr_t>(Wp) & 15) == 0);
-            if (tu) {
-                // persistent strip kernel (chol_trailing_kernel): block columns 1 .. nbk-1 of the trailing matrix
-                const int nbk = (m + NB - 1) / NB;
-                const long long Tt = (long long)(nbk - 1) * nbk / 2;
-                if (tu_on == 2) {
-                    // 128 x 64 tiles, two CTAs per SM, ~6 tiles (~3 of the 128 x 128 ones) per CTA
-                    long long T2 = 0;
-                    for (int c2 = 2; c2 < 2 * nbk; ++c2) T2 += nbk - (c2 >> 1);
-                    if (T2 > 0) {
-                        static int tpc2 = -1;
-                        if (tpc2 < 0) { const char *e = getenv("CVXB_CHOL_TU_TILES"); tpc2 = e ? std::max(1, atoi(e)) : 6; }
-                        const long long slots = 2LL * kNumSMs;
-                        const long long waves = (T2 + slots * tpc2 - 1) / (slots * tpc2);
-                        const int grid = (int)std::min<long long>(T2, waves * slots);
-                        chol_trailing2_kernel<<<grid, 128, T2_SMEM, U>>>(m, Wp, ldw, A22, lda, nbk, T2, u.trace);
-                        count_launch();
-                        CVXB_LAUNCH_CHECK();
-                    }
-                } else if (Tt > 0) {
-                    // CTAs of ~3 tiles (~50 us): long enough to amortise the strip operand and the pipeline fill, short
-                    // enough that the SMs keep coming free for the chain / panel streams' kernels (a CTA of this
-                    // kernel fills an SM's shared memory: nothing else can be resident beside it)
-                    static int tpc = -1;
-                    if (tpc < 0) { const char *e = getenv("CVXB_CHOL_TU_TILES"); tpc = e ? std::max(1, atoi(e)) : 3; }
-                    const long long waves = (Tt + (long long)kNumSMs * tpc - 1) / ((long long)kNumSMs * tpc);
-                    const int grid = (int)std::min<long long>(Tt, waves * kNumSMs);
-                    chol_trailing_kernel<<<grid, 256, TU_SMEM, U>>>(m, Wp, ldw, A22, lda, nbk, 1, Tt, u.trace);
-                    count_launch();
-                    CVXB_LAUNCH_CHECK();
-                }
-            } else {
-                CVXB_TRY(dmma_gemm(u, U));
-            }
+            CVXB_TRY(dmma_gemm(u, U));
             CVXB_CUDA(cudaEventRecord(w.ev_r[jb], U));
             prev_r = last_r;
             last_r = jb;
         }
     }
-    w.r_valid[0] = w.r_valid[1] = -1;
     CVXB_CUDA(cudaEventRecord(w.ev_end_p, D));
     CVXB_CUDA(cudaEventRecord(w.ev_end_u, U));
     CVXB_CUDA(cudaEventRecord(w.ev_end_t, T));
@@ -1143,18 +741,12 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
 // kernels then start without host-side launch latency, which is what the diagonal chain of
 // small kernels is sensitive to.  First call with a new key runs eagerly (allocations, function
 // attributes), the second one is captured; any capture failure falls back to eager launches.
-// CVXB_GRAPH=0 disables.
 int potrf_lower(int n, double *A, int lda, double *inv, CholWork &w, cudaStream_t st) {
     if (n <= 0) return 0;
-    static int enabled = -1;
-    if (enabled < 0) {
-        const char *e = getenv("CVXB_GRAPH");
-        enabled = (e && e[0] == '0') ? 0 : 1;
-    }
     // replay removes ~450 host API calls per factorisation; large factorisations stay on the eager path because
     // graph kernel nodes do not keep the panel streams' priority over the bulk update (threshold chosen when the
     // kernels were tuned, not re-measured on H100)
-    if (!enabled || w.graph_failed || n > 4096) return potrf_enqueue(n, A, lda, inv, w, st);
+    if (w.graph_failed || n > 4096) return potrf_enqueue(n, A, lda, inv, w, st);
     CholWork::GraphEntry *ent = nullptr;
     for (auto &g : w.graphs)
         if (g.n == n && g.A == A && g.lda == lda && g.inv == inv) { ent = &g; break; }

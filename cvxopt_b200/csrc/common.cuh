@@ -164,9 +164,7 @@ struct CholWork {
     };
     std::vector<GraphEntry> graphs;
     bool graph_failed = false;
-    int r_valid[2] = {-1, -1};            // which steps recorded ev_r (steps without bulk work do not)
-    cudaEvent_t ev_start = nullptr, ev_panel = nullptr, ev_rest = nullptr, ev_end_p = nullptr,
-                ev_end_u = nullptr;
+    cudaEvent_t ev_start = nullptr, ev_end_p = nullptr, ev_end_u = nullptr;
     int *d_info = nullptr;                // device flag
     int *d_flags = nullptr;               // trsv progress flags (batch * ceil(n/NB) ints)
     long long flags_cap = 0;

@@ -26,8 +26,6 @@
 // (Y operand), the "n" index over C's rows (X operand), so each thread's accumulator
 // pair is two consecutive ROWS of a column-major C (one 16-byte access).
 #include "common.cuh"
-#include <cuda.h>
-#include <cstdlib>
 
 namespace cvxb {
 
@@ -491,312 +489,6 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const KParams p) {
     }
 }
 
-// =====================================================================================
-// TMA + mbarrier, warp-specialised, persistent variant for the long-K, K-major x K-major case
-// (the normal-equations SYRK: 96 % of the factor's flops at the north-star size).
-//
-//   * one CTA per SM, 256 threads: two independent groups of 4 warps (each owns a 128x64 tile at
-//     a time, exactly the 64x32 warp tiling of the kernel above).  Lane 0 of a group's first warp
-//     is also its producer: it keeps the group's ring TS-1 stages ahead (a ninth, dedicated
-//     producer warp would cap the CTA at 168 registers/thread; the accumulators alone need 128)
-//   * operands arrive by cp.async.bulk.tensor.2d (SASS UTMALDG) with the 128-byte swizzle into a
-//     4-stage ring per group; full/empty mbarriers replace __syncthreads, no consumer warp ever
-//     computes a global address or issues a copy
-//   * swizzled tiles are read conflict-free by permuting which tile row a lane's fragment row
-//     maps to: rho(g) = 2*(g&3) + (g>>2), so each half-warp touches rows {0,2,4,6} or {1,3,5,7}
-//     of an 8-row group, whose 16-byte chunks the XOR swizzle sends to distinct bank groups
-//   * K tail / ragged n rely on TMA's out-of-bounds zero fill
-// =====================================================================================
-constexpr int TS = 4;                                   // ring stages per consumer group
-constexpr int T_XB = BR * BK * 8;                       // 16384 B
-constexpr int T_YB = BC * BK * 8;                       //  8192 B
-constexpr int T_STAGE = T_XB + T_YB + 1024;             // + scaling chunk, keeps 1024-B alignment
-constexpr int T_GROUP = TS * T_STAGE;
-constexpr int T_SMEM = 2 * T_GROUP + 1024 /*align slack*/ + 256 /*barriers*/;
-constexpr int T_THREADS = 256;
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ bool mbar_test(uint64_t *bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-        ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-        : "memory");
-}
-__device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-        ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
-        : "memory");
-}
-
-__global__ void __launch_bounds__(T_THREADS, 1)
-dmma_syrk_tma_kernel(const KParams p, const __grid_constant__ CUtensorMap mapX,
-                     const __grid_constant__ CUtensorMap mapY, int units) {
-    extern __shared__ __align__(1024) unsigned char tsm_raw[];
-    unsigned char *tsm = reinterpret_cast<unsigned char *>(
-        (reinterpret_cast<uintptr_t>(tsm_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-    uint64_t *bars = reinterpret_cast<uint64_t *>(tsm + 2 * T_GROUP);   // [g][full TS | empty TS]
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-    if (tid == 0) {
-        for (int g = 0; g < 2; ++g)
-            for (int s = 0; s < TS; ++s) {
-                mbar_init(bars + g * 2 * TS + s, 1);            // full: producer's expect_tx arrive
-                mbar_init(bars + g * 2 * TS + TS + s, 4);       // empty: one arrive per consumer warp
-            }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    const bool has_w = (p.w != nullptr);
-
-    // ------------------------------ consumers ------------------------------
-    const int g = warp >> 2, wl = warp & 3;
-    const int wr = wl & 1, wc = wl >> 1;
-    const int g4 = lane >> 2, t4 = lane & 3;
-    const int rho = ((g4 & 3) << 1) | (g4 >> 2);             // tile row (mod 8) this lane's fragment row maps to
-    const int hsel = t4 >> 1, lo8 = (t4 & 1) * 8;
-    unsigned char *ring = tsm + g * T_GROUP;
-    uint64_t *full = bars + g * 2 * TS, *empty = full + TS;
-    // byte offsets of this lane's fragment rows inside the X / Y tiles
-    int xrow[8], yrow[4];
-#pragma unroll
-    for (int rf = 0; rf < 8; ++rf) xrow[rf] = (wr * 64 + rf * 8 + rho) * 128 + lo8;
-#pragma unroll
-    for (int cf = 0; cf < 4; ++cf) yrow[cf] = T_XB + (wc * 32 + cf * 8 + rho) * 128 + lo8;
-    int kxor[4];                                             // swizzled 16-byte chunk of k = kk*4 + t4
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) kxor[kk] = ((kk * 2 + hsel) ^ rho) << 4;
-
-    // ---- producer state (lane 0 of the group's first warp): a cursor that runs TS-1 k tiles
-    // ahead of the consumers across tile boundaries
-    const bool is_producer = (wl == 0) && (lane == 0);
-    const uint32_t tx = T_XB + T_YB + (has_w ? BK * 8 : 0);
-    int pu = blockIdx.x * 2 + g, pkt = 0, pktiles = 0, pk0 = 0, ptr_ = 0, ptc_ = 0;
-    uint32_t pit = 0;
-    auto p_open_unit = [&]() {                       // decode unit `pu` for the producer cursor
-        if (pu >= units) { pktiles = 0; return; }
-        int tile, split = 0;
-        if (pu < p.full_tiles) tile = pu;
-        else { tile = p.full_tiles + (pu - p.full_tiles) / p.S; split = (pu - p.full_tiles) % p.S; }
-        decode_tile(p, tile, ptr_, ptc_);
-        int kb = 0, ke = p.K;
-        if (pu >= p.full_tiles && p.S > 1) { kb = split * p.kchunk; ke = min(p.K, kb + p.kchunk); }
-        pk0 = kb; pktiles = (ke - kb + BK - 1) / BK; pkt = 0;
-    };
-    // blocking == false: give up (and retry at the next poll point) when the stage is still in use,
-    // so the producer lane never stalls the DMMA stream of its own warp
-    auto p_issue_one = [&](bool blocking) {          // issue the next k tile of the cursor, if any
-        while (pu < units && pkt >= pktiles) { pu += 2 * gridDim.x; p_open_unit(); }
-        if (pu >= units) return;
-        const int st = pit % TS;
-        if (blocking) mbar_wait(empty + st, ((pit / TS) & 1) ^ 1);
-        else if (!mbar_test(empty + st, ((pit / TS) & 1) ^ 1)) return;
-        unsigned char *sb = ring + st * T_STAGE;
-        mbar_expect_tx(full + st, tx);
-        const int k0 = pk0 + pkt * BK;
-        tma_load_2d(sb, &mapX, k0, ptr_ * BR, full + st);
-        tma_load_2d(sb + T_XB, &mapY, k0, ptc_ * BC, full + st);
-        if (has_w) bulk_load_1d(sb + T_XB + T_YB, p.w + k0, BK * 8, full + st);
-        ++pkt; ++pit;
-    };
-    if (is_producer) {
-        p_open_unit();
-        for (int i = 0; i < TS; ++i) p_issue_one(true);        // fill the ring
-    }
-
-    uint32_t it = 0;
-    for (int u = blockIdx.x * 2 + g; u < units; u += 2 * gridDim.x) {
-        int tile, split = 0;
-        if (u < p.full_tiles) tile = u;
-        else { tile = p.full_tiles + (u - p.full_tiles) / p.S; split = (u - p.full_tiles) % p.S; }
-        int tr, tc;
-        decode_tile(p, tile, tr, tc);
-        const bool is_split = (u >= p.full_tiles) && (p.S > 1);
-        int kbeg = 0, kend = p.K;
-        if (is_split) { kbeg = split * p.kchunk; kend = min(p.K, kbeg + p.kchunk); }
-        const int ktiles = (kend - kbeg + BK - 1) / BK;
-
-        double acc[4][8][2];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
-
-        for (int kt = 0; kt < ktiles; ++kt, ++it) {
-            const int st = it % TS;
-            if (is_producer) {                                          // poll point 1
-                if (pit <= it) p_issue_one(true);                       // tile `it` itself: must go out
-                else if (pit < it + TS) p_issue_one(false);
-            }
-            mbar_wait(full + st, (it / TS) & 1);
-            const unsigned char *sb = ring + st * T_STAGE;
-            const double *sw = reinterpret_cast<const double *>(sb + T_XB + T_YB);
-            const int kvalid = kend - kbeg - kt * BK;        // >= BK except in the last tile
-            double a[2][4], bf[2][8];
-#pragma unroll
-            for (int cf = 0; cf < 4; ++cf) a[0][cf] = *reinterpret_cast<const double *>(sb + yrow[cf] + kxor[0]);
-#pragma unroll
-            for (int rf = 0; rf < 8; ++rf) bf[0][rf] = *reinterpret_cast<const double *>(sb + xrow[rf] + kxor[0]);
-            if (has_w) {
-                const double wv = (t4 < kvalid) ? sw[t4] : 0.0;
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf) a[0][cf] *= wv;
-            }
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const int cur = kk & 1, nxt = cur ^ 1;
-                if (kk + 1 < 4) {
-#pragma unroll
-                    for (int cf = 0; cf < 4; ++cf)
-                        a[nxt][cf] = *reinterpret_cast<const double *>(sb + yrow[cf] + kxor[kk + 1]);
-#pragma unroll
-                    for (int rf = 0; rf < 8; ++rf)
-                        bf[nxt][rf] = *reinterpret_cast<const double *>(sb + xrow[rf] + kxor[kk + 1]);
-                    if (has_w) {
-                        const int k = (kk + 1) * 4 + t4;
-                        const double wn = (k < kvalid) ? sw[k] : 0.0;
-#pragma unroll
-                        for (int cf = 0; cf < 4; ++cf) a[nxt][cf] *= wn;
-                    }
-                }
-#pragma unroll
-                for (int cf = 0; cf < 4; ++cf)
-#pragma unroll
-                    for (int rf = 0; rf < 8; ++rf)
-                        dmma(acc[cf][rf][0], acc[cf][rf][1], a[cur][cf], bf[cur][rf]);
-                if (kk == 1 && is_producer && pit < it + TS) p_issue_one(false);   // poll point 2
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(empty + st);          // this warp is done with the stage
-            if (is_producer && pit < it + 1 + TS) p_issue_one(false);              // poll point 3
-        }
-
-
-        // ---- epilogue: D[m = g4][n = 2*t4 + e]  ->  C[r0 + .. + rho'(2*t4+e), c0 + .. + rho(g4)]
-        const int r0 = tr * BR, c0 = tc * BC;
-        const int nr = min(BR, p.M - r0), nc = min(BC, p.N - c0);
-        if (is_split) {
-            double *ws = p.ws + ((long long)(tile - p.full_tiles) * p.S + split) * TILE_ELEMS;
-#pragma unroll
-            for (int cf = 0; cf < 4; ++cf)
-#pragma unroll
-                for (int rf = 0; rf < 8; ++rf)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int n8 = t4 * 2 + e;
-                        const int rl = wr * 64 + rf * 8 + (((n8 & 3) << 1) | (n8 >> 2));
-                        const int cl = wc * 32 + cf * 8 + rho;
-                        ws[rl + cl * BR] = acc[cf][rf][e];
-                    }
-        } else {
-            const bool use_d = (p.beta != 0.0);
-#pragma unroll
-            for (int cf = 0; cf < 4; ++cf) {
-                const int cl = wc * 32 + cf * 8 + rho;
-                if (cl >= nc) continue;
-                const long long c = c0 + cl;
-#pragma unroll
-                for (int rf = 0; rf < 8; ++rf)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int n8 = t4 * 2 + e;
-                        const int rl = wr * 64 + rf * 8 + (((n8 & 3) << 1) | (n8 >> 2));
-                        if (rl >= nr) continue;
-                        const long long r = r0 + rl;
-                        if (p.lower_only && r < c) continue;
-                        double v = p.alpha * acc[cf][rf][e];
-                        if (use_d) v += p.beta * p.D[r + c * p.ldd];
-                        p.C[r + c * p.ldc] = v;
-                    }
-            }
-        }
-    }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-
-// returns 0 on launch, 1 when this path does not apply (caller falls back to the cp.async kernel)
-int launch_syrk_tma(const KParams &p, int units, cudaStream_t st) {
-    static std::atomic<int> state{0};  // 0 untested, 1 usable, -1 unusable
-    static std::atomic<EncodeTiledFn> encode_fn{nullptr};
-    static DeviceOnce once;
-    if (state.load() == 0) {
-        int ns = -1;
-        // opt-in (CVXB_TMA=1): parity-green, but it kept the DMMA pipe less busy than the cp.async kernel
-        // on the north-star SYRK when the kernels were tuned (not re-measured on H100)
-        const char *on = getenv("CVXB_TMA");
-        if (on && on[0] == '1') {
-            void *fn = nullptr;
-            cudaDriverEntryPointQueryResult q;
-            if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess &&
-                q == cudaDriverEntryPointSuccess && fn) {
-                encode_fn.store(reinterpret_cast<EncodeTiledFn>(fn));
-                ns = 1;
-            }
-            cudaGetLastError();
-        }
-        state.store(ns);
-    }
-    if (state.load() != 1) return 1;
-    if (const unsigned long long bit = once.pending()) {
-        if (cudaFuncSetAttribute(dmma_syrk_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM) !=
-            cudaSuccess) { cudaGetLastError(); return 1; }
-        once.mark(bit);
-    }
-    const EncodeTiledFn encode = encode_fn.load();
-    // the matrix as TMA sees it: dim0 = k (contiguous), dim1 = row/column index of C
-    CUtensorMap mx, my;
-    const cuuint64_t gdimx[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
-    const cuuint64_t gdimy[2] = {(cuuint64_t)p.K, (cuuint64_t)p.N};
-    const cuuint64_t gsx[1] = {(cuuint64_t)p.ldx * 8}, gsy[1] = {(cuuint64_t)p.ldy * 8};
-    const cuuint32_t boxx[2] = {BK, BR}, boxy[2] = {BK, BC}, es[2] = {1, 1};
-    if (encode(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, const_cast<double *>(p.X), gdimx, gsx, boxx, es,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return 1;
-    if (encode(&my, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, const_cast<double *>(p.Y), gdimy, gsy, boxy, es,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return 1;
-    int grid = kNumSMs;
-    if (grid * 2 > units) grid = (units + 1) / 2;
-    dmma_syrk_tma_kernel<<<grid, T_THREADS, T_SMEM, st>>>(p, mx, my, units);
-    count_launch();
-    CVXB_LAUNCH_CHECK();
-    return 0;
-}
-
 template <bool XK, bool YK, bool VEC>
 int launch_inst(const KParams &p, dim3 grid, cudaStream_t st) {
     static DeviceOnce once;              // per instantiation, per device
@@ -889,14 +581,7 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
                      (g.batch == 1 || (g.sX % 2 == 0 && g.sY % 2 == 0));
     p.vec_c = aligned(g.C, g.ldc) && (!g.D || aligned(g.D, g.ldd)) &&
               (g.batch == 1 || (g.sC % 2 == 0 && g.sD % 2 == 0));
-    int rc = 1;
-    // long-K SYRK-shaped launches go to the TMA / mbarrier kernel when its preconditions hold
-    if (g.x_kmajor && g.y_kmajor && g.batch == 1 && vec && g.K >= 1024 &&
-        (!g.w || (uintptr_t)g.w % 16 == 0)) {
-        rc = launch_syrk_tma(p, units, st);
-        if (rc < 0) return rc;
-    }
-    if (rc == 1) {
+    int rc;
 #define DISPATCH(XK, YK)                                                   \
     rc = vec ? launch_inst<XK, YK, true>(p, grid, st) : launch_inst<XK, YK, false>(p, grid, st)
     if (g.x_kmajor && g.y_kmajor) DISPATCH(true, true);
@@ -904,7 +589,6 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     else if (!g.x_kmajor && g.y_kmajor) DISPATCH(false, true);
     else DISPATCH(false, false);
 #undef DISPATCH
-    }
     if (rc) return rc;
     if (p.S > 1) {
         dim3 rg(rem_tiles, 8);

@@ -21,8 +21,6 @@
 // run the epilogue, warp 8 is the producer (cp.async.bulk + mbarrier ring).
 #include "common.cuh"
 #include <cstdint>
-#include <cstdlib>
-#include <cstdio>
 #include <cmath>
 #include <vector>
 #include <algorithm>
@@ -66,7 +64,7 @@ struct OzParams {
     // and writes its 128 x 128 partial (tile-local, column-major) to part + b * 128*128; oz_tail_reduce_kernel sums them
     int nchunk, kper;
     double *part;
-    int kb2, kb5;              // k steps per ring stage for passes with <= 2 / <= 5 slices (CVXB_OZ_KB=a,b)
+    int kb2, kb5;              // k steps per ring stage for passes with <= 2 / <= 5 slices (ozaki_syrk sets 4 / 1)
 };
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
@@ -419,10 +417,7 @@ int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, co
     // pageable-source copy is staged before cudaMemcpyAsync returns)
     std::vector<unsigned int> order;
     order.reserve((size_t)tiles);
-    int band = 12;
-    if (const char *e = getenv("CVXB_OZ_BAND")) band = std::max(1, atoi(e));
-    static int tail_on = -1;
-    if (tail_on < 0) { const char *e = getenv("CVXB_OZ_TAIL"); tail_on = (e && e[0] == '0') ? 0 : 1; }
+    const int band = 12;
     for (int r0 = 0; r0 < nblk; r0 += band) {
         const int r1 = std::min(nblk, r0 + band);
         for (int J = 0; J < r1; ++J)
@@ -438,10 +433,6 @@ int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, co
     p.n = n; p.nblk = nblk; p.nk = nk; p.S = S; p.layout = layout; p.tiles = dtiles;
     p.nchunk = 1; p.kper = nk; p.part = nullptr;
     p.kb2 = 4; p.kb5 = 1;
-    if (const char *e = getenv("CVXB_OZ_KB")) {
-        int a = 0, b = 0;
-        if (sscanf(e, "%d,%d", &a, &b) == 2 && a >= 1 && a <= 6 && b >= 1 && b <= 2) { p.kb2 = a; p.kb5 = b; }
-    }
     p.npass = 0;
     for (int d0 = 0; d0 < S; d0 += 2, ++p.npass) { p.pd0[p.npass] = d0; p.pd1[p.npass] = std::min(S - 1, d0 + 1); }
     cudaEvent_t tev0 = g_oz_ev0, tev1 = g_oz_ev1;
@@ -449,10 +440,10 @@ int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, co
     if (tev0) CVXB_CUDA(cudaEventRecord(tev0, st));
     // The last, partial wave of tiles (2080 = 15 x 132 + 100 at n = 8192) would leave SMs idle for a whole tile
     // time: when it fills at most half the SMs, its tiles are split along K over all SMs (partials + ordered
-    // reduce).  CVXB_OZ_TAIL=0 disables.
+    // reduce).
     long long tmain = tiles;
     int ntail = (int)(tiles % kNumSMs), nchunk = 1;
-    if (tail_on && tiles > kNumSMs && ntail > 0 && ntail <= kNumSMs / 2) {
+    if (tiles > kNumSMs && ntail > 0 && ntail <= kNumSMs / 2) {
         nchunk = std::min(kNumSMs / ntail, nk);
         if (nchunk >= 2) tmain = tiles - ntail; else nchunk = 1;
     }
