@@ -408,14 +408,7 @@ extern "C" {
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
     *out = nullptr;
-    int cnt = 0;
-    if (cudaGetDeviceCount(&cnt) != cudaSuccess || cnt == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device available: cvxopt_b200 has no CPU fallback");
-        return CVXB_E_NOGPU;
-    }
-    if (device < 0 || device >= cnt) { set_error("device out of range"); return CVXB_E_ARG; }
-    CVXB_CUDA(cudaSetDevice(device));
+    CVXB_TRY(check_device(device));
     cvxb_batch *b = new cvxb_batch();
     b->device = device; b->B = nprob; b->n = n; b->m = m;
     if (const char *e = getenv("CVXB_OZAKI")) b->i8_mode = (e[0] == '0') ? 0 : (e[0] == '2') ? 2 : 1;
@@ -425,27 +418,21 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     b->nblk = (n + NB - 1) / NB;
     b->sInv = (long long)2 * b->nblk * NB * NB;
     auto fail = [&](int r) { cvxb_batch_destroy(b); return r; };
-#define BCUDA(expr) do { cudaError_t _e = (expr); \
-        /* out of memory: give the scratch-buffer cache (common.cuh) back to the driver and try once more */ \
-        if (_e == cudaErrorMemoryAllocation) { cudaGetLastError(); tmp_cache_release(); _e = (expr); } \
-        if (_e != cudaSuccess) { \
-        set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
-        return fail(_e == cudaErrorMemoryAllocation ? CVXB_E_NOMEM : CVXB_E_CUDA); } } while (0)
     const size_t B = nprob;
-    BCUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
-    BCUDA(cudaEventCreate(&b->e0)); BCUDA(cudaEventCreate(&b->e1));
+    CVXB_CUDA_RETRY(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
+    CVXB_CUDA_RETRY(cudaEventCreate(&b->e0)); CVXB_CUDA_RETRY(cudaEventCreate(&b->e1));
     { int r = chol_work_create(b->cw); if (r) return fail(r); }
-    BCUDA(cudaMalloc(&b->P, B * b->sP * sizeof(double)));
-    BCUDA(cudaMalloc(&b->G, B * b->sG * sizeof(double)));
-    BCUDA(cudaMalloc(&b->K, B * b->sK * sizeof(double)));
-    BCUDA(cudaMalloc(&b->inv, B * b->sInv * sizeof(double)));
-    BCUDA(cudaMalloc(&b->panel, B * (size_t)((n + 1) & ~1) * NB * sizeof(double)));
-    BCUDA(cudaMalloc(&b->gemv_ws, B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n) * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->P, B * b->sP * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->G, B * b->sG * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->K, B * b->sK * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->inv, B * b->sInv * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->panel, B * (size_t)((n + 1) & ~1) * NB * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->gemv_ws, B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n) * sizeof(double)));
     // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
     const size_t nv = 4, mv = 13;
     const size_t me = (size_t)(m > 0 ? m : 1);
-    BCUDA(cudaMalloc(&b->vecs, B * (nv * n + mv * me) * sizeof(double)));
-    BCUDA(cudaMemset(b->vecs, 0, B * (nv * n + mv * me) * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->vecs, B * (nv * n + mv * me) * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMemset(b->vecs, 0, B * (nv * n + mv * me) * sizeof(double)));
     double *v = b->vecs;
     auto take = [&](size_t len) { double *r = v; v += B * len; return r; };
     b->q = take(n); b->p.x = take(n); b->p.rx = take(n); b->p.dx = take(n);
@@ -453,18 +440,17 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     b->p.dz = take(me); b->p.lmbda = take(me); b->p.lmbdasq = take(me); b->p.d = take(me);
     b->p.di = take(me); b->p.di2 = take(me); b->p.ws3 = take(me); b->p.bzp = take(me);
     b->p.q = b->q; b->p.h = b->h; b->p.n = n; b->p.m = m;
-    BCUDA(cudaMalloc(&b->sc, B * sizeof(Scal)));
-    BCUDA(cudaMemset(b->sc, 0, B * sizeof(Scal)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->sc, B * sizeof(Scal)));
+    CVXB_CUDA_RETRY(cudaMemset(b->sc, 0, B * sizeof(Scal)));
     b->p.sc = b->sc;
-    BCUDA(cudaMalloc(&b->d_info, B * sizeof(int)));
-    BCUDA(cudaMalloc(&b->d_ndone, sizeof(int)));
-    BCUDA(cudaMalloc(&b->d_done, B * sizeof(int)));
-    BCUDA(cudaMalloc(&b->d_pairs, 2 * B * sizeof(int)));
-    BCUDA(cudaMalloc(&b->d_perm, B * sizeof(int)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->d_info, B * sizeof(int)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->d_ndone, sizeof(int)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->d_done, B * sizeof(int)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->d_pairs, 2 * B * sizeof(int)));
+    CVXB_CUDA_RETRY(cudaMalloc(&b->d_perm, B * sizeof(int)));
     b->perm.resize(B);
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
-#undef BCUDA
     *out = b;
     return 0;
 }

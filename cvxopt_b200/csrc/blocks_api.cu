@@ -1,7 +1,8 @@
 // C ABI, part 2: dense building blocks on device pointers (the BLAS/LAPACK calls the
 // reference path makes: blas.syrk blas.c:3039, lapack.potrf lapack.c:1471,
 // lapack.potrs lapack.c:1553, blas.gemm blas.c:2602) and the misc_solvers mirror
-// (src/C/misc_solvers.c:1155-1173) on flat buffers.
+// (src/C/misc_solvers.c:1155-1173) on flat buffers.  Also the per-device context (CallCtx, common.cuh)
+// of every entry point that takes no handle.
 #include "cone.cuh"
 #include <map>
 #include <mutex>
@@ -9,137 +10,91 @@
 using namespace cvxb;
 
 namespace {
-
-// One context (stream + Cholesky workspace) per device, shared by the stateless entry points of this
-// file.  Calls on the same device are serialised by the context's mutex (held until the entry point
-// returns), calls on different devices run concurrently; the map itself is guarded by g_ctx_mu.
+// check_device has passed and the stream and CholWork exist once ok is set
 struct DevCtx {
     cudaStream_t st = nullptr;
     CholWork cw;
     bool ok = false;
     std::mutex mu;
 };
-std::map<int, DevCtx> g_ctx;
+std::map<int, DevCtx> g_ctx;     // std::map nodes are address-stable; the map itself is guarded by g_ctx_mu
 std::mutex g_ctx_mu;
+}  // namespace
 
-struct CtxRef {
-    DevCtx *c = nullptr;
-    std::unique_lock<std::mutex> lk;
-    DevCtx *operator->() const { return c; }
-};
-
-int get_ctx(int device, CtxRef *out) {
-    int cnt = 0;
-    if (cudaGetDeviceCount(&cnt) != cudaSuccess || cnt == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device available: cvxopt_b200 has no CPU fallback");
-        return CVXB_E_NOGPU;
-    }
-    if (device < 0 || device >= cnt) { set_error("device %d out of range", device); return CVXB_E_ARG; }
-    CVXB_CUDA(cudaSetDevice(device));
-    DevCtx *cp;
+int cvxb::CallCtx::acquire(int device) {
+    DevCtx *c;
     {
         std::lock_guard<std::mutex> g(g_ctx_mu);
-        cp = &g_ctx[device];             // std::map nodes are address-stable
+        c = &g_ctx[device];
     }
-    std::unique_lock<std::mutex> lk(cp->mu);
-    DevCtx &c = *cp;
-    if (!c.ok) {
-        CVXB_CUDA(cudaStreamCreateWithFlags(&c.st, cudaStreamNonBlocking));
-        CVXB_TRY(chol_work_create(c.cw));
-        c.ok = true;
+    lock = std::unique_lock<std::mutex>(c->mu);
+    if (c->ok) {
+        CVXB_CUDA(cudaSetDevice(device));
+    } else {
+        CVXB_TRY(check_device(device));
+        CVXB_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
+        CVXB_TRY(chol_work_create(c->cw));
+        c->ok = true;
     }
-    out->c = cp;
-    out->lk = std::move(lk);
+    st = c->st;
+    cw = &c->cw;
     return 0;
 }
-
-// RAII device temp
-struct DBuf {
-    double *p = nullptr;
-    ~DBuf() { if (p) tmp_free(p); }
-    int alloc(size_t n) {
-        CVXB_CUDA(tmp_malloc(&p, (n ? n : 1) * sizeof(double)));
-        return 0;
-    }
-};
-
-// stage a host buffer on the device for the misc_solvers mirror (space == HOST) or
-// use the pointer directly (space == DEVICE)
-struct Staged {
-    double *dev = nullptr; double *host = nullptr; size_t n = 0; bool owned = false;
-    ~Staged() { if (owned && dev) tmp_free(dev); }
-    int in(const double *src, size_t count, int space, cudaStream_t st) {
-        n = count; host = const_cast<double *>(src);
-        if (space == CVXB_DEVICE) { dev = host; owned = false; return 0; }
-        CVXB_CUDA(tmp_malloc(&dev, (n ? n : 1) * sizeof(double)));
-        owned = true;
-        if (n) CVXB_CUDA(cudaMemcpyAsync(dev, src, n * sizeof(double), cudaMemcpyHostToDevice, st));
-        return 0;
-    }
-    int out(cudaStream_t st) {
-        if (owned && n) CVXB_CUDA(cudaMemcpyAsync(host, dev, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-        return 0;
-    }
-};
-
-}  // namespace
 
 extern "C" {
 
 int cvxb_syrk_scaled(int n, int k, const double *A, int lda, const double *rowscale,
                      const double *H, int ldh, double *C, int ldc, int device) {
-    CtxRef ctx; CVXB_TRY(get_ctx(device, &ctx));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
     GemmDesc g;
     g.M = n; g.N = n; g.K = k;
     g.X = A; g.ldx = lda; g.x_kmajor = true;
     g.Y = A; g.ldy = lda; g.y_kmajor = true;
     g.w = rowscale;
     g.D = H; g.ldd = ldh; g.beta = 1.0;
-    g.C = C; g.ldc = ldc; g.lower_only = true; g.splitk_ws = ctx->cw.splitk_ws;
-    CVXB_TRY(dmma_gemm(g, ctx->st));
-    CVXB_CUDA(cudaStreamSynchronize(ctx->st));
+    g.C = C; g.ldc = ldc; g.lower_only = true; g.splitk_ws = ctx.cw->splitk_ws;
+    CVXB_TRY(dmma_gemm(g, ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     return 0;
 }
 
 int cvxb_syrk_scaled_i8(int n, int k, const double *A, int lda, const double *d, const double *H, int ldh,
                         double *C, int ldc, int slices, int device) {
-    CtxRef ctx; CVXB_TRY(get_ctx(device, &ctx));
-    void *work = nullptr;
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
     if (slices < 1 || slices > 9) { set_error("syrk_scaled_i8: slices must be 1..9"); return CVXB_E_ARG; }
-    if (tmp_malloc(&work, ozaki_workspace_bytes(n, k, slices)) != cudaSuccess) {
+    Scratch<char> work;
+    if (work.alloc(ozaki_workspace_bytes(n, k, slices))) {
         cudaGetLastError();
         set_error("syrk_scaled_i8: out of device memory for the slice workspace");
         return CVXB_E_NOMEM;
     }
-    int rc = ozaki_syrk(n, k, A, lda, d, H, ldh, 1.0, C, ldc, slices, 0, work, ctx->st);
-    cudaError_t e = cudaStreamSynchronize(ctx->st);
-    tmp_free(work);
+    int rc = ozaki_syrk(n, k, A, lda, d, H, ldh, 1.0, C, ldc, slices, 0, work.p, ctx.st);
+    cudaError_t e = cudaStreamSynchronize(ctx.st);
     if (rc) return rc;
     if (e != cudaSuccess) { set_error("syrk_scaled_i8: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
     return 0;
 }
 
 int cvxb_potrf(int n, double *A, int lda, double *work_inv, int device) {
-    CtxRef ctx; CVXB_TRY(get_ctx(device, &ctx));
-    CVXB_TRY(potrf_lower(n, A, lda, work_inv, ctx->cw, ctx->st));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    CVXB_TRY(potrf_lower(n, A, lda, work_inv, *ctx.cw, ctx.st));
     int info = 0;
-    CVXB_CUDA(cudaMemcpyAsync(&info, ctx->cw.d_info, sizeof(int), cudaMemcpyDeviceToHost, ctx->st));
-    CVXB_CUDA(cudaStreamSynchronize(ctx->st));
+    CVXB_CUDA(cudaMemcpyAsync(&info, ctx.cw->d_info, sizeof(int), cudaMemcpyDeviceToHost, ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     if (info > 0) set_error("potrf: leading minor of order %d is not positive definite", info);
     return info;
 }
 
 int cvxb_potrs(int n, const double *L, int ldl, const double *inv, double *b, int device) {
-    CtxRef ctx; CVXB_TRY(get_ctx(device, &ctx));
-    CVXB_TRY(potrs_lower(n, L, ldl, inv, b, ctx->cw, ctx->st));
-    CVXB_CUDA(cudaStreamSynchronize(ctx->st));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    CVXB_TRY(potrs_lower(n, L, ldl, inv, b, *ctx.cw, ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     return 0;
 }
 
 int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const double *A, int lda,
               const double *B, int ldb, double beta, double *C, int ldc, int device) {
-    CtxRef ctx; CVXB_TRY(get_ctx(device, &ctx));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
     const bool ta = (transa == 'T' || transa == 't'), tb = (transb == 'T' || transb == 't');
     GemmDesc g;
     g.M = m; g.N = n; g.K = k;
@@ -149,76 +104,61 @@ int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const d
     g.Y = B; g.ldy = ldb; g.y_kmajor = !tb;
     g.D = (beta != 0.0) ? C : nullptr; g.ldd = ldc; g.beta = beta;
     g.C = C; g.ldc = ldc; g.alpha = alpha;
-    CVXB_TRY(dmma_gemm(g, ctx->st));
-    CVXB_CUDA(cudaStreamSynchronize(ctx->st));
+    CVXB_TRY(dmma_gemm(g, ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     return 0;
 }
 
 // ---------------------------------------------------------------- misc_solvers mirror
 int cvxb_scale(double *x, int xr, int xc, const cvxb_dims *dims, const cvxb_scaling *W, int trans,
                int inverse, int space) {
-    CtxRef ctx; CVXB_TRY(get_ctx(0, &ctx));
-    cudaStream_t st = ctx->st;
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
     ConeLayout c;
-    int rc = c.init(dims);
-    if (rc) { c.destroy(); return rc; }
-    if (xr < c.cdim) { c.destroy(); set_error("scale: x has fewer rows than the cone dimension"); return CVXB_E_ARG; }
+    CVXB_TRY(c.init(dims));
+    if (xr < c.cdim) { set_error("scale: x has fewer rows than the cone dimension"); return CVXB_E_ARG; }
     DevScaling S;
+    CVXB_TRY(S.alloc(c));
+    CVXB_TRY(S.upload(c, W, space, st));
     Staged X;
-    DBuf work;
-    auto body = [&]() -> int {
-        CVXB_TRY(S.alloc(c));
-        CVXB_TRY(S.upload(c, W, space, st));
-        CVXB_TRY(X.in(x, (size_t)xr * xc, space, st));
-        const bool inv = (inverse == 'I');
-        double *xd = X.dev;
-        if (c.mnl) CVXB_TRY(scale_rows(xd, xr, xd, xr, c.mnl, xc, inv ? S.dnli : S.dnl, st));
-        if (c.ml) CVXB_TRY(scale_rows(xd + c.mnl, xr, xd + c.mnl, xr, c.ml, xc, inv ? S.di : S.d, st));
-        if (c.nq) CVXB_TRY(scale_q(c, S, xd + c.mnl + c.ml, xr, xd + c.mnl + c.ml, xr, xc, inv, st));
-        if (c.ns && c.maxs) {
-            size_t per = (size_t)2 * c.maxs * c.maxs;
-            size_t cols = (size_t)xc;
-            size_t cap = (size_t)1 << 28;
-            size_t want = per * cols;
-            if (want > cap) want = (cap / per ? cap / per : 1) * per;
-            CVXB_TRY(work.alloc(want));
-            double *base = xd + c.mnl + c.ml + c.sumq;
-            CVXB_TRY(scale_s(c, S, base, xr, base, xr, xc, trans, inverse, work.p, want, st));
-        }
-        CVXB_TRY(X.out(st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        return 0;
-    };
-    rc = body();
-    cudaStreamSynchronize(st);
-    S.destroy();
-    c.destroy();
-    return rc;
+    CVXB_TRY(X.in(x, (size_t)xr * xc, space, st));
+    const bool inv = (inverse == 'I');
+    double *xd = X.dev;
+    if (c.mnl) CVXB_TRY(scale_rows(xd, xr, xd, xr, c.mnl, xc, inv ? S.dnli : S.dnl, st));
+    if (c.ml) CVXB_TRY(scale_rows(xd + c.mnl, xr, xd + c.mnl, xr, c.ml, xc, inv ? S.di : S.d, st));
+    if (c.nq) CVXB_TRY(scale_q(c, S, xd + c.mnl + c.ml, xr, xd + c.mnl + c.ml, xr, xc, inv, st));
+    Scratch<double> work;
+    if (c.ns && c.maxs) {
+        size_t per = (size_t)2 * c.maxs * c.maxs;
+        size_t cols = (size_t)xc;
+        size_t cap = (size_t)1 << 28;
+        size_t want = per * cols;
+        if (want > cap) want = (cap / per ? cap / per : 1) * per;
+        CVXB_TRY(work.alloc(want));
+        double *base = xd + c.mnl + c.ml + c.sumq;
+        CVXB_TRY(scale_s(c, S, base, xr, base, xr, xc, trans, inverse, work.p, want, st));
+    }
+    CVXB_TRY(X.out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 static int pack_common(const double *x, double *y, const cvxb_dims *dims, int space, bool do_pack) {
-    CtxRef ctx; CVXB_TRY(get_ctx(0, &ctx));
-    cudaStream_t st = ctx->st;
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
     ConeLayout c;
-    int rc = c.init(dims);
-    if (rc) { c.destroy(); return rc; }
+    CVXB_TRY(c.init(dims));
+    const size_t nin = do_pack ? c.cdim : c.cdim_pckd, nout = do_pack ? c.cdim_pckd : c.cdim;
     Staged X, Y;
-    auto body = [&]() -> int {
-        const size_t nin = do_pack ? c.cdim : c.cdim_pckd, nout = do_pack ? c.cdim_pckd : c.cdim;
-        CVXB_TRY(X.in(x, nin, space, st));
-        CVXB_TRY(Y.in(y, nout, space, st));   // unpack leaves the strict upper triangles untouched
-        const int nlq = c.mnl + c.ml + c.sumq;
-        if (nlq) CVXB_CUDA(cudaMemcpyAsync(Y.dev, X.dev, (size_t)nlq * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        if (do_pack) CVXB_TRY(pack_s(c, X.dev + nlq, c.cdim, Y.dev + nlq, c.cdim_pckd, 1, true, st));
-        else         CVXB_TRY(unpack_s(c, X.dev + nlq, c.cdim_pckd, Y.dev + nlq, c.cdim, 1, st));
-        CVXB_TRY(Y.out(st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        return 0;
-    };
-    rc = body();
-    cudaStreamSynchronize(st);
-    c.destroy();
-    return rc;
+    CVXB_TRY(X.in(x, nin, space, st));
+    CVXB_TRY(Y.in(y, nout, space, st));   // unpack leaves the strict upper triangles untouched
+    const int nlq = c.mnl + c.ml + c.sumq;
+    if (nlq) CVXB_CUDA(cudaMemcpyAsync(Y.dev, X.dev, (size_t)nlq * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (do_pack) CVXB_TRY(pack_s(c, X.dev + nlq, c.cdim, Y.dev + nlq, c.cdim_pckd, 1, true, st));
+    else         CVXB_TRY(unpack_s(c, X.dev + nlq, c.cdim_pckd, Y.dev + nlq, c.cdim, 1, st));
+    CVXB_TRY(Y.out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 int cvxb_pack(const double *x, double *y, const cvxb_dims *dims, int space) {
@@ -229,40 +169,33 @@ int cvxb_unpack(const double *x, double *y, const cvxb_dims *dims, int space) {
 }
 
 int cvxb_pack2(double *x, int xr, int xc, const cvxb_dims *dims, int space) {
-    CtxRef ctx; CVXB_TRY(get_ctx(0, &ctx));
-    cudaStream_t st = ctx->st;
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
     ConeLayout c;
-    int rc = c.init(dims);
-    if (rc) { c.destroy(); return rc; }
+    CVXB_TRY(c.init(dims));
+    if (c.ns == 0 || c.maxs == 0) return 0;
     Staged X;
-    DBuf tmp;
-    auto body = [&]() -> int {
-        if (c.ns == 0 || c.maxs == 0) return 0;
-        CVXB_TRY(X.in(x, (size_t)xr * xc, space, st));
-        const int nlq = c.mnl + c.ml + c.sumq;
-        // in place in the reference (rows compacted towards the top); go through a copy
-        CVXB_TRY(tmp.alloc((size_t)c.sump * xc));
-        CVXB_TRY(pack_s(c, X.dev + nlq, xr, tmp.p, c.sump, xc, false, st));
-        CVXB_CUDA(cudaMemcpy2DAsync(X.dev + nlq, (size_t)xr * sizeof(double), tmp.p,
-                                    (size_t)c.sump * sizeof(double), (size_t)c.sump * sizeof(double),
-                                    xc, cudaMemcpyDeviceToDevice, st));
-        CVXB_TRY(X.out(st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        return 0;
-    };
-    rc = body();
-    cudaStreamSynchronize(st);
-    c.destroy();
-    return rc;
+    CVXB_TRY(X.in(x, (size_t)xr * xc, space, st));
+    const int nlq = c.mnl + c.ml + c.sumq;
+    // in place in the reference (rows compacted towards the top); go through a copy
+    Scratch<double> tmp;
+    CVXB_TRY(tmp.alloc((size_t)c.sump * xc));
+    CVXB_TRY(pack_s(c, X.dev + nlq, xr, tmp.p, c.sump, xc, false, st));
+    CVXB_CUDA(cudaMemcpy2DAsync(X.dev + nlq, (size_t)xr * sizeof(double), tmp.p,
+                                (size_t)c.sump * sizeof(double), (size_t)c.sump * sizeof(double),
+                                xc, cudaMemcpyDeviceToDevice, st));
+    CVXB_TRY(X.out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 int cvxb_symm(double *x, int n, int space) {
-    CtxRef ctx; CVXB_TRY(get_ctx(0, &ctx));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
     Staged X;
-    CVXB_TRY(X.in(x, (size_t)n * n, space, ctx->st));
-    CVXB_TRY(symmetrize_lower(n, X.dev, n, 1, 0, ctx->st));
-    CVXB_TRY(X.out(ctx->st));
-    CVXB_CUDA(cudaStreamSynchronize(ctx->st));
+    CVXB_TRY(X.in(x, (size_t)n * n, space, ctx.st));
+    CVXB_TRY(symmetrize_lower(n, X.dev, n, 1, 0, ctx.st));
+    CVXB_TRY(X.out(ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     return 0;
 }
 

@@ -7,6 +7,7 @@
 #include <string>
 #include <vector>
 #include <atomic>
+#include <mutex>
 #include "../../include/cvxopt_b200.h"
 
 namespace cvxb {
@@ -67,6 +68,58 @@ cudaError_t tmp_malloc_bytes(void **p, size_t bytes);
 void tmp_free(void *p);
 void tmp_cache_release();          // free every cached block of every device
 template <class T> inline cudaError_t tmp_malloc(T **p, size_t bytes) { return tmp_malloc_bytes(reinterpret_cast<void **>(p), bytes); }
+
+// n elements of device scratch from the cache, returned to it when the Scratch goes out of scope
+template <class T> struct Scratch {
+    T *p = nullptr;
+    Scratch() = default;
+    Scratch(const Scratch &) = delete;
+    Scratch &operator=(const Scratch &) = delete;
+    ~Scratch() { tmp_free(p); }
+    int alloc(size_t n) {
+        CVXB_CUDA(tmp_malloc(&p, (n ? n : 1) * sizeof(T)));
+        return 0;
+    }
+};
+
+// n doubles of a caller's buffer on the device: a host buffer (space == CVXB_HOST) is staged in scratch, a device
+// pointer (CVXB_DEVICE) is used in place.  upload == false skips the host-to-device copy of output-only buffers.
+struct Staged {
+    double *dev = nullptr, *host = nullptr; size_t n = 0; bool owned = false;
+    Staged() = default;
+    Staged(const Staged &) = delete;
+    Staged &operator=(const Staged &) = delete;
+    ~Staged() { if (owned) tmp_free(dev); }
+    int in(const double *src, size_t count, int space, cudaStream_t st, bool upload = true) {
+        n = count; host = const_cast<double *>(src);
+        if (space == CVXB_DEVICE) { dev = host; return 0; }
+        CVXB_CUDA(tmp_malloc(&dev, (n ? n : 1) * sizeof(double)));
+        owned = true;
+        if (n && upload) CVXB_CUDA(cudaMemcpyAsync(dev, src, n * sizeof(double), cudaMemcpyHostToDevice, st));
+        return 0;
+    }
+    int out(cudaStream_t st) {
+        if (owned && n) CVXB_CUDA(cudaMemcpyAsync(host, dev, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+        return 0;
+    }
+};
+
+// For cvxb_kkt_create / cvxb_batch_create: an allocation that fails for lack of memory is tried once more after
+// the scratch-buffer cache is given back to the driver.  Any failure returns fail(code), a lambda of the caller
+// that releases what was built so far.
+#define CVXB_CUDA_RETRY(expr)                                                                       \
+    do {                                                                                            \
+        cudaError_t _e = (expr);                                                                    \
+        if (_e == cudaErrorMemoryAllocation) { cudaGetLastError(); cvxb::tmp_cache_release(); _e = (expr); } \
+        if (_e != cudaSuccess) {                                                                    \
+            cvxb::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));  \
+            return fail(_e == cudaErrorMemoryAllocation ? CVXB_E_NOMEM : CVXB_E_CUDA);              \
+        }                                                                                           \
+    } while (0)
+
+// CVXB_JACOBI_COOP (default on, =0 for one launch per round) allows a cooperative launch, and `ctas` CTAs of
+// `threads` threads of `kernel` can be resident on the current device at once
+bool coop_launch_fits(const void *kernel, int threads, long long ctas);
 
 constexpr int kNumSMs = 132;       // H100 SXM
 constexpr int NB = 128;            // Cholesky block size == GEMM tile edge
@@ -185,5 +238,20 @@ int trsv_lower(int n, const double *L, int ldl, const double *inv, double *b, bo
                long long sb = 0);
 int potrf_lower_batched(int n, double *A, int lda, long long sA, double *inv, long long sInv,
                         int batch, int *d_info, double *panel, int ldw, cudaStream_t st);
+
+// ---- device selection ----------------------------------------------------------
+// CVXB_E_NOGPU unless `device` exists and is sm_90; selects it.
+int check_device(int device);
+
+// The entry points that take no cvxb_kkt / cvxb_batch handle (misc_solvers mirror, NT scaling, dense blocks)
+// share one stream and one CholWork per device.  acquire() selects the device and holds its lock until the
+// CallCtx goes out of scope, so calls on one device are serialised.  The lock is not recursive: such an entry
+// point must not call another one.  Declare the CallCtx before the buffers it frees.
+struct CallCtx {
+    cudaStream_t st = nullptr;
+    CholWork *cw = nullptr;
+    std::unique_lock<std::mutex> lock;
+    int acquire(int device);
+};
 
 }  // namespace cvxb

@@ -18,7 +18,7 @@ int ConeLayout::init(const cvxb_dims *dims) {
     mnl = dims->mnl; ml = dims->ml; nq = dims->nq; ns = dims->ns;
     q.assign(dims->q, dims->q + nq);
     s.assign(dims->s, dims->s + ns);
-    sumq = sums2 = sump = maxs = 0;
+    sumq = sums = sums2 = sump = maxs = 0;
     q_off.resize(nq); v_off.resize(nq); s_off.resize(ns); s_poff.resize(ns); r_off.resize(ns);
     for (int k = 0; k < nq; ++k) {
         if (q[k] < 1) { set_error("dims['q'] entries must be >= 1"); return CVXB_E_ARG; }
@@ -27,7 +27,7 @@ int ConeLayout::init(const cvxb_dims *dims) {
     for (int k = 0; k < ns; ++k) {
         if (s[k] < 0) { set_error("dims['s'] entries must be >= 0"); return CVXB_E_ARG; }
         s_off[k] = sums2; s_poff[k] = sump; r_off[k] = sums2;
-        sums2 += s[k] * s[k]; sump += s[k] * (s[k] + 1) / 2;
+        sums += s[k]; sums2 += s[k] * s[k]; sump += s[k] * (s[k] + 1) / 2;
         if (s[k] > maxs) maxs = s[k];
     }
     cdim = mnl + ml + sumq + sums2;
@@ -44,9 +44,8 @@ int ConeLayout::init(const cvxb_dims *dims) {
     return 0;
 }
 
-void ConeLayout::destroy() {
-    int **ptrs[] = {&d_q, &d_qoff, &d_voff, &d_s, &d_soff, &d_spoff, &d_roff};
-    for (auto pp : ptrs) { if (*pp) tmp_free(*pp); *pp = nullptr; }
+ConeLayout::~ConeLayout() {
+    for (int *p : {d_q, d_qoff, d_voff, d_s, d_soff, d_spoff, d_roff}) tmp_free(p);
 }
 
 // ------------------------------------------------------------------ scaling storage
@@ -61,7 +60,6 @@ int DevScaling::alloc(const ConeLayout &c) {
     r = p; p += c.sums2; rti = p; p += c.sums2;
     return 0;
 }
-void DevScaling::destroy() { if (store) tmp_free(store); store = nullptr; }
 cvxb_scaling DevScaling::view() const {
     cvxb_scaling w;
     w.dnl = dnl; w.dnli = dnli; w.d = d; w.di = di; w.v = v; w.beta = beta; w.r = r; w.rti = rti;

@@ -5,11 +5,11 @@
 
 namespace cvxb {
 
-// Host + device description of a cone product  [mnl | l | q.. | s..]
+// Host + device description of a cone product  [mnl | l | q.. | s..]; owns its device arrays
 struct ConeLayout {
     int mnl = 0, ml = 0, nq = 0, ns = 0;
     std::vector<int> q, s;
-    int sumq = 0, sums2 = 0, sump = 0, maxs = 0;
+    int sumq = 0, sums = 0, sums2 = 0, sump = 0, maxs = 0;   // sums: sum of the 's' orders
     int cdim = 0, cdim_pckd = 0;
     // per-cone offsets (host)
     std::vector<int> q_off;    // row offset of q cone k in an (unpacked or packed) cone vector
@@ -20,8 +20,11 @@ struct ConeLayout {
     // device copies: [q sizes | q_off | v_off] and [s sizes | s_off | s_poff | r_off]
     int *d_q = nullptr, *d_qoff = nullptr, *d_voff = nullptr;
     int *d_s = nullptr, *d_soff = nullptr, *d_spoff = nullptr, *d_roff = nullptr;
-    int init(const cvxb_dims *dims);
-    void destroy();
+    ConeLayout() = default;
+    ConeLayout(const ConeLayout &) = delete;
+    ConeLayout &operator=(const ConeLayout &) = delete;
+    ~ConeLayout();
+    int init(const cvxb_dims *dims);   // call once; what a failed init allocated is freed by the destructor
 };
 
 // Device-resident copy of the scaling W (flat mirror of the reference dict)
@@ -31,9 +34,12 @@ struct DevScaling {
     double *di2 = nullptr;      // di .* di  (weight of the fused SYRK)
     double *store = nullptr;    // single allocation backing all of the above
     size_t total = 0;
+    DevScaling() = default;
+    DevScaling(const DevScaling &) = delete;
+    DevScaling &operator=(const DevScaling &) = delete;
+    ~DevScaling() { tmp_free(store); }
     int alloc(const ConeLayout &c);
     int upload(const ConeLayout &c, const cvxb_scaling *W, int space, cudaStream_t st);
-    void destroy();
     cvxb_scaling view() const;
 };
 

@@ -8,8 +8,6 @@
 // round is a single race-free pass.
 #include "cone.cuh"
 #include <cooperative_groups.h>
-#include <mutex>
-#include <map>
 #include <vector>
 #include <algorithm>
 #include <cfloat>
@@ -421,62 +419,20 @@ __global__ void max_step_s_kernel(double *out, const double *sigma, const int *s
     *out = t;
 }
 
-struct VCtx { cudaStream_t st = nullptr; bool ok = false; };
-VCtx g_v;
-int vctx(cudaStream_t *st) {
-    int cnt = 0;
-    if (cudaGetDeviceCount(&cnt) != cudaSuccess || cnt == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device available: cvxopt_b200 has no CPU fallback");
-        return CVXB_E_NOGPU;
-    }
-    CVXB_CUDA(cudaSetDevice(0));
-    static std::mutex mu;               // creation only; a CUDA stream itself may be shared by threads
-    std::lock_guard<std::mutex> g(mu);
-    if (!g_v.ok) { CVXB_CUDA(cudaStreamCreateWithFlags(&g_v.st, cudaStreamNonBlocking)); g_v.ok = true; }
-    *st = g_v.st;
-    return 0;
-}
-
-struct Buf {       // host buffer staged on the device (or a device pointer used in place)
-    double *dev = nullptr, *host = nullptr; size_t n = 0; bool owned = false;
-    ~Buf() { if (owned && dev) tmp_free(dev); }
-    int in(const double *src, size_t count, int space, cudaStream_t st) {
-        n = count; host = const_cast<double *>(src);
-        if (space == CVXB_DEVICE) { dev = host; return 0; }
-        CVXB_CUDA(tmp_malloc(&dev, (n ? n : 1) * sizeof(double)));
-        owned = true;
-        if (n) CVXB_CUDA(cudaMemcpyAsync(dev, src, n * sizeof(double), cudaMemcpyHostToDevice, st));
-        return 0;
-    }
-    int out(cudaStream_t st) {
-        if (owned && n) CVXB_CUDA(cudaMemcpyAsync(host, dev, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-        return 0;
-    }
-};
-
-struct Lay {
-    ConeLayout c; Cones k;
-    int init(const cvxb_dims *dims) {
-        int rc = c.init(dims);
-        if (rc) return rc;
-        k.nl = c.mnl + c.ml; k.nq = c.nq; k.q = c.d_q; k.ns = c.ns; k.s = c.d_s;
-        return 0;
-    }
-    ~Lay() { c.destroy(); }
-};
+Cones cones_of(const ConeLayout &c) { return Cones{c.mnl + c.ml, c.nq, c.d_q, c.ns, c.d_s}; }
 
 }  // namespace
 
 extern "C" {
 
 int cvxb_scale2(const double *lmbda, double *x, const cvxb_dims *dims, int inverse, int space) {
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
-    Buf l, xb;
-    CVXB_TRY(l.in(lmbda, (size_t)L.c.mnl + L.c.ml + L.c.sumq + [&] { int t = 0; for (int v : L.c.s) t += v; return t; }(), space, st));
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
-    scale2_kernel<<<1, 256, 0, st>>>(l.dev, xb.dev, L.k, inverse == 'I');
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
+    Staged l, xb;
+    CVXB_TRY(l.in(lmbda, (size_t)c.mnl + c.ml + c.sumq + c.sums, space, st));
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
+    scale2_kernel<<<1, 256, 0, st>>>(l.dev, xb.dev, cones_of(c), inverse == 'I');
     count_launch(); CVXB_LAUNCH_CHECK();
     CVXB_TRY(xb.out(st));
     CVXB_CUDA(cudaStreamSynchronize(st));
@@ -484,44 +440,39 @@ int cvxb_scale2(const double *lmbda, double *x, const cvxb_dims *dims, int inver
 }
 
 int cvxb_sprod(double *x, const double *y, const cvxb_dims *dims, int diag, int space) {
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
     const bool dd = (diag == 'D');
-    size_t ny = dd ? (size_t)L.c.mnl + L.c.ml + L.c.sumq + [&] { int t = 0; for (int v : L.c.s) t += v; return t; }()
-                   : (size_t)L.c.cdim;
-    Buf xb, yb;
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
+    size_t ny = dd ? (size_t)c.mnl + c.ml + c.sumq + c.sums : (size_t)c.cdim;
+    Staged xb, yb;
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
     CVXB_TRY(yb.in(y, ny, space, st));
-    sprod_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, L.k, dd ? 1 : 0);
+    sprod_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, cones_of(c), dd ? 1 : 0);
     count_launch(); CVXB_LAUNCH_CHECK();
-    if (!dd && L.c.ns > 0) {
+    if (!dd && c.ns > 0) {
         // 0.5 (A Y + Y A) with A = sym(x_k), Y = sym(y_k): T = A Y on the DMMA GEMM
-        const int nlq = L.c.mnl + L.c.ml + L.c.sumq;
-        for (int k = 0; k < L.c.ns; ++k) {
-            const int mk = L.c.s[k];
+        const int nlq = c.mnl + c.ml + c.sumq;
+        for (int k = 0; k < c.ns; ++k) {
+            const int mk = c.s[k];
             if (mk == 0) continue;
             const long long m2 = (long long)mk * mk;
-            double *tmp = nullptr;
-            CVXB_CUDA(tmp_malloc(&tmp, 3 * m2 * sizeof(double)));
-            double *As = tmp, *Ys = tmp + m2, *T = tmp + 2 * m2;
-            int rc = 0;
-            do {
-                if (cudaMemcpyAsync(As, xb.dev + nlq + L.c.s_off[k], m2 * sizeof(double), cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
-                    cudaMemcpyAsync(Ys, yb.dev + nlq + L.c.s_off[k], m2 * sizeof(double), cudaMemcpyDeviceToDevice, st) != cudaSuccess) { rc = CVXB_E_CUDA; break; }
-                if ((rc = symmetrize_lower(mk, As, mk, 1, 0, st))) break;
-                if ((rc = symmetrize_lower(mk, Ys, mk, 1, 0, st))) break;
-                GemmDesc g;
-                g.M = mk; g.N = mk; g.K = mk;
-                g.X = As; g.ldx = mk; g.x_kmajor = false;
-                g.Y = Ys; g.ldy = mk; g.y_kmajor = true;       // Y[c,k] = Ys[k, c]
-                g.C = T; g.ldc = mk;
-                if ((rc = dmma_gemm(g, st))) break;
-                sprod_s_finish_kernel<<<(int)((m2 + 255) / 256), 256, 0, st>>>(xb.dev + nlq + L.c.s_off[k], T, mk);
-                count_launch();
-            } while (0);
-            cudaStreamSynchronize(st);
-            tmp_free(tmp);
-            if (rc) return rc;
+            Scratch<double> tmp;
+            CVXB_TRY(tmp.alloc(3 * m2));
+            double *As = tmp.p, *Ys = tmp.p + m2, *T = tmp.p + 2 * m2;
+            CVXB_CUDA(cudaMemcpyAsync(As, xb.dev + nlq + c.s_off[k], m2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            CVXB_CUDA(cudaMemcpyAsync(Ys, yb.dev + nlq + c.s_off[k], m2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+            CVXB_TRY(symmetrize_lower(mk, As, mk, 1, 0, st));
+            CVXB_TRY(symmetrize_lower(mk, Ys, mk, 1, 0, st));
+            GemmDesc g;
+            g.M = mk; g.N = mk; g.K = mk;
+            g.X = As; g.ldx = mk; g.x_kmajor = false;
+            g.Y = Ys; g.ldy = mk; g.y_kmajor = true;       // Y[c,k] = Ys[k, c]
+            g.C = T; g.ldc = mk;
+            CVXB_TRY(dmma_gemm(g, st));
+            sprod_s_finish_kernel<<<(int)((m2 + 255) / 256), 256, 0, st>>>(xb.dev + nlq + c.s_off[k], T, mk);
+            count_launch();
+            CVXB_CUDA(cudaStreamSynchronize(st));    // before tmp is freed
         }
     }
     CVXB_TRY(xb.out(st));
@@ -530,13 +481,13 @@ int cvxb_sprod(double *x, const double *y, const cvxb_dims *dims, int diag, int 
 }
 
 int cvxb_sinv(double *x, const double *y, const cvxb_dims *dims, int space) {
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
-    size_t ny = (size_t)L.c.mnl + L.c.ml + L.c.sumq + [&] { int t = 0; for (int v : L.c.s) t += v; return t; }();
-    Buf xb, yb;
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
-    CVXB_TRY(yb.in(y, ny, space, st));
-    sinv_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, L.k);
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
+    Staged xb, yb;
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
+    CVXB_TRY(yb.in(y, (size_t)c.mnl + c.ml + c.sumq + c.sums, space, st));
+    sinv_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, cones_of(c));
     count_launch(); CVXB_LAUNCH_CHECK();
     CVXB_TRY(xb.out(st));
     CVXB_CUDA(cudaStreamSynchronize(st));
@@ -544,11 +495,12 @@ int cvxb_sinv(double *x, const double *y, const cvxb_dims *dims, int space) {
 }
 
 static int trisc_common(double *x, const cvxb_dims *dims, int space, int mode) {
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
-    Buf xb;
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
-    trisc_kernel<<<1, 256, 0, st>>>(xb.dev, L.k, L.c.mnl + L.c.ml + L.c.sumq, mode);
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
+    Staged xb;
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
+    trisc_kernel<<<1, 256, 0, st>>>(xb.dev, cones_of(c), c.mnl + c.ml + c.sumq, mode);
     count_launch(); CVXB_LAUNCH_CHECK();
     CVXB_TRY(xb.out(st));
     CVXB_CUDA(cudaStreamSynchronize(st));
@@ -559,18 +511,18 @@ int cvxb_triusc(double *x, const cvxb_dims *dims, int space) { return trisc_comm
 
 int cvxb_sdot(const double *x, const double *y, const cvxb_dims *dims, double *result, int space) {
     if (!result) { set_error("sdot: result is NULL"); return CVXB_E_ARG; }
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
-    Buf xb, yb;
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
-    CVXB_TRY(yb.in(y, L.c.cdim, space, st));
-    double *d = nullptr;
-    CVXB_CUDA(tmp_malloc(&d, sizeof(double)));
-    sdot_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, L.k, L.c.mnl + L.c.ml + L.c.sumq, d);
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
+    Staged xb, yb;
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
+    CVXB_TRY(yb.in(y, c.cdim, space, st));
+    Scratch<double> d;
+    CVXB_TRY(d.alloc(1));
+    sdot_kernel<<<1, 256, 0, st>>>(xb.dev, yb.dev, cones_of(c), c.mnl + c.ml + c.sumq, d.p);
     count_launch();
-    cudaError_t e = cudaMemcpyAsync(result, d, sizeof(double), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(result, d.p, sizeof(double), cudaMemcpyDeviceToHost, st);
     cudaStreamSynchronize(st);
-    tmp_free(d);
     if (e != cudaSuccess) { set_error("sdot: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
     return 0;
 }
@@ -581,45 +533,35 @@ int cvxb_sdot(const double *x, const double *y, const cvxb_dims *dims, double *r
 static int sym_eig_blocks(const ConeLayout &c, double *xs, double *sigma_dev, const int *d_sigoff,
                           bool with_vectors, cudaStream_t st) {
     const int MAX_SWEEPS = 40;
-    int sums = 0;
-    for (int v : c.s) sums += v;
     if (c.maxs == 0) return 0;
     const size_t m2 = (size_t)c.sums2;
-    double *work = nullptr, *stats = nullptr;
-    int *perm = nullptr, *fail = nullptr;
     std::vector<double> hstats(2 * (size_t)c.ns), prev(c.ns, 1e300);
-    int rc = 0;
-    auto done = [&](int r) {
-        cudaStreamSynchronize(st);
-        tmp_free(work); tmp_free(stats); tmp_free(perm); tmp_free(fail);
-        return r;
-    };
-    if (tmp_malloc(&work, (with_vectors ? 3 : 2) * m2 * sizeof(double)) != cudaSuccess ||
-        tmp_malloc(&stats, 2 * (size_t)c.ns * sizeof(double)) != cudaSuccess ||
-        tmp_malloc(&perm, (size_t)(sums ? sums : 1) * sizeof(int)) != cudaSuccess ||
-        tmp_malloc(&fail, sizeof(int)) != cudaSuccess) {
+    Scratch<double> work, stats;
+    Scratch<int> perm, fail;
+    if (work.alloc((with_vectors ? 3 : 2) * m2) || stats.alloc(2 * (size_t)c.ns) || perm.alloc(c.sums) ||
+        fail.alloc(1)) {
         cudaGetLastError();
         set_error("max_step: out of device memory for the eigensolver workspace");
-        return done(CVXB_E_NOMEM);
+        return CVXB_E_NOMEM;
     }
     JacArgs a;
-    a.x = xs; a.w0 = work; a.w1 = work + m2; a.V = with_vectors ? work + 2 * m2 : nullptr;
+    a.x = xs; a.w0 = work.p; a.w1 = work.p + m2; a.V = with_vectors ? work.p + 2 * m2 : nullptr;
     a.s = c.d_s; a.soff = c.d_soff; a.sigoff = d_sigoff;
-    a.sigma = sigma_dev; a.xout = with_vectors ? xs : nullptr; a.stats = stats; a.perm = perm;
+    a.sigma = sigma_dev; a.xout = with_vectors ? xs : nullptr; a.stats = stats.p; a.perm = perm.p;
     a.N = std::max(2, c.maxs + (c.maxs & 1));
     const int h = a.N / 2;
     if (c.maxs <= 64) {
-        if (cudaMemsetAsync(fail, 0, sizeof(int), st) != cudaSuccess) return done(CVXB_E_CUDA);
+        CVXB_CUDA(cudaMemsetAsync(fail.p, 0, sizeof(int), st));
         const int nt = std::max(32, (h * h + 31) / 32 * 32);
-        if (with_vectors) jac_small_kernel<true><<<c.ns, nt, 0, st>>>(a, MAX_SWEEPS, fail);
-        else jac_small_kernel<false><<<c.ns, nt, 0, st>>>(a, MAX_SWEEPS, fail);
+        if (with_vectors) jac_small_kernel<true><<<c.ns, nt, 0, st>>>(a, MAX_SWEEPS, fail.p);
+        else jac_small_kernel<false><<<c.ns, nt, 0, st>>>(a, MAX_SWEEPS, fail.p);
         count_launch();
         int hfail = 0;
-        cudaError_t e = cudaMemcpyAsync(&hfail, fail, sizeof(int), cudaMemcpyDeviceToHost, st);
+        cudaError_t e = cudaMemcpyAsync(&hfail, fail.p, sizeof(int), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return done(CVXB_E_CUDA); }
-        if (hfail) { set_error("max_step: Jacobi eigensolver did not converge (non-finite input?)"); rc = 1; }
-        return done(rc);
+        if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
+        if (hfail) { set_error("max_step: Jacobi eigensolver did not converge (non-finite input?)"); return 1; }
+        return 0;
     }
     {
         const int gx = (int)std::min<size_t>(((size_t)c.maxs * c.maxs + 255) / 256, 1184);
@@ -628,38 +570,27 @@ static int sym_eig_blocks(const ConeLayout &c, double *xs, double *sigma_dev, co
     }
     int flip = 0;
     bool ok = false;
-    // one cooperative launch per sweep when all its CTAs can be resident at once (CVXB_JACOBI_COOP=0: per-round launches)
-    bool coop = false;
-    {
-        static int coop_on = -1;
-        if (coop_on < 0) { const char *e = getenv("CVXB_JACOBI_COOP"); coop_on = (e && e[0] == '0') ? 0 : 1; }
-        int dev = 0, can = 0, per_sm = 0, sms = 0;
-        const void *fn = with_vectors ? (const void *)jac_sweep_kernel<true> : (const void *)jac_sweep_kernel<false>;
-        if (coop_on && cudaGetDevice(&dev) == cudaSuccess &&
-            cudaDeviceGetAttribute(&can, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && can &&
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0) == cudaSuccess)
-            coop = (long long)per_sm * sms >= (long long)((h + 15) / 16) * ((h + 15) / 16) * c.ns;
-    }
+    const void *sweep_fn = with_vectors ? (const void *)jac_sweep_kernel<true> : (const void *)jac_sweep_kernel<false>;
+    const dim3 blk(16, 16), grd((h + 15) / 16, (h + 15) / 16, c.ns);
+    // one cooperative launch per sweep when all its CTAs can be resident at once, else one launch per round
+    const bool coop = coop_launch_fits(sweep_fn, 256, (long long)grd.x * grd.y * grd.z);
     for (int sweep = 0; sweep <= MAX_SWEEPS; ++sweep) {
         jac_off_kernel<<<c.ns, 256, 0, st>>>(a, flip);
         count_launch();
-        cudaError_t e = cudaMemcpyAsync(hstats.data(), stats, hstats.size() * sizeof(double), cudaMemcpyDeviceToHost, st);
+        cudaError_t e = cudaMemcpyAsync(hstats.data(), stats.p, hstats.size() * sizeof(double), cudaMemcpyDeviceToHost, st);
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return done(CVXB_E_CUDA); }
+        if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
         ok = true;
         for (int k = 0; k < c.ns; ++k) {
             if (c.s[k] && !jac_done(hstats[2 * k], hstats[2 * k + 1], prev[k], c.s[k])) ok = false;
             prev[k] = hstats[2 * k];
         }
         if (ok || sweep == MAX_SWEEPS) break;
-        const dim3 blk(16, 16), grd((h + 15) / 16, (h + 15) / 16, c.ns);
         if (coop) {
             void *args[] = {&a, &flip};
-            const void *fn = with_vectors ? (const void *)jac_sweep_kernel<true> : (const void *)jac_sweep_kernel<false>;
-            if (cudaLaunchCooperativeKernel(fn, grd, blk, args, 0, st) != cudaSuccess) {
+            if (cudaLaunchCooperativeKernel(sweep_fn, grd, blk, args, 0, st) != cudaSuccess) {
                 set_error("max_step: cooperative launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-                return done(CVXB_E_CUDA);
+                return CVXB_E_CUDA;
             }
             count_launch();
             flip ^= 1;                                   // N - 1 (odd) buffer swaps
@@ -672,7 +603,7 @@ static int sym_eig_blocks(const ConeLayout &c, double *xs, double *sigma_dev, co
             }
         }
     }
-    if (!ok) { set_error("max_step: Jacobi eigensolver did not converge (non-finite input?)"); return done(1); }
+    if (!ok) { set_error("max_step: Jacobi eigensolver did not converge (non-finite input?)"); return 1; }
     jac_sort_kernel<<<c.ns, 256, 0, st>>>(a, flip);
     count_launch();
     if (with_vectors) {
@@ -681,54 +612,51 @@ static int sym_eig_blocks(const ConeLayout &c, double *xs, double *sigma_dev, co
         count_launch();
     }
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return done(CVXB_E_CUDA); }
-    return done(0);
+    cudaStreamSynchronize(st);                           // before the scratch is freed
+    if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
+    return 0;
 }
 
 int cvxb_max_step(double *x, const cvxb_dims *dims, double *sigma, double *result, int space) {
     if (!result) { set_error("max_step: result is NULL"); return CVXB_E_ARG; }
-    cudaStream_t st; CVXB_TRY(vctx(&st));
-    Lay L; CVXB_TRY(L.init(dims));
-    const int nlq = L.c.mnl + L.c.ml + L.c.sumq;
-    int sums = 0;
-    std::vector<int> sigoff(L.c.ns);
-    for (int k = 0; k < L.c.ns; ++k) { sigoff[k] = sums; sums += L.c.s[k]; }
-    Buf xb;
-    CVXB_TRY(xb.in(x, L.c.cdim, space, st));
-    double *d = nullptr, *dsig = nullptr;
-    int *dsigoff = nullptr;
-    auto done = [&](int r) { tmp_free(d); tmp_free(dsig); tmp_free(dsigoff); return r; };
-    CVXB_CUDA(tmp_malloc(&d, sizeof(double)));
-    max_step_kernel<<<1, 256, 0, st>>>(xb.dev, L.k, d);
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
+    ConeLayout c; CVXB_TRY(c.init(dims));
+    const int nlq = c.mnl + c.ml + c.sumq;
+    std::vector<int> sigoff(c.ns);
+    for (int k = 0, o = 0; k < c.ns; ++k) { sigoff[k] = o; o += c.s[k]; }
+    Staged xb;
+    CVXB_TRY(xb.in(x, c.cdim, space, st));
+    Scratch<double> d, dsig;
+    Scratch<int> dsigoff;
+    CVXB_TRY(d.alloc(1));
+    max_step_kernel<<<1, 256, 0, st>>>(xb.dev, cones_of(c), d.p);
     count_launch();
-    if (L.c.maxs > 0) {
+    if (c.maxs > 0) {
         // 's' blocks: lambda_min of each block (reference dsyevr_ range 'I' 1..1, or dsyevd_ 'V' when
         // sigma is given: eigenvalues -> sigma, eigenvectors -> x; misc_solvers.c:1099-1150)
-        if (tmp_malloc(&dsig, (size_t)sums * sizeof(double)) != cudaSuccess ||
-            tmp_malloc(&dsigoff, (size_t)L.c.ns * sizeof(int)) != cudaSuccess ||
-            cudaMemcpyAsync(dsigoff, sigoff.data(), (size_t)L.c.ns * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        if (dsig.alloc(c.sums) || dsigoff.alloc(c.ns) ||
+            cudaMemcpyAsync(dsigoff.p, sigoff.data(), (size_t)c.ns * sizeof(int), cudaMemcpyHostToDevice, st) != cudaSuccess) {
             cudaGetLastError();
             set_error("max_step: device allocation failed");
-            return done(CVXB_E_NOMEM);
+            return CVXB_E_NOMEM;
         }
-        int rc = sym_eig_blocks(L.c, xb.dev + nlq, dsig, dsigoff, sigma != nullptr, st);
-        if (rc) return done(rc);
-        max_step_s_kernel<<<1, 1, 0, st>>>(d, dsig, L.c.d_s, dsigoff, L.c.ns, nlq > 0);
+        CVXB_TRY(sym_eig_blocks(c, xb.dev + nlq, dsig.p, dsigoff.p, sigma != nullptr, st));
+        max_step_s_kernel<<<1, 1, 0, st>>>(d.p, dsig.p, c.d_s, dsigoff.p, c.ns, nlq > 0);
         count_launch();
         if (sigma) {
-            if (cudaMemcpyAsync(sigma, dsig, (size_t)sums * sizeof(double),
+            if (cudaMemcpyAsync(sigma, dsig.p, (size_t)c.sums * sizeof(double),
                                 space == CVXB_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st) != cudaSuccess) {
                 set_error("max_step: copy of sigma failed");
-                return done(CVXB_E_CUDA);
+                return CVXB_E_CUDA;
             }
-            int rc2 = xb.out(st);
-            if (rc2) return done(rc2);
+            CVXB_TRY(xb.out(st));
         }
     }
-    cudaError_t e = cudaMemcpyAsync(result, d, sizeof(double), cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaMemcpyAsync(result, d.p, sizeof(double), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return done(CVXB_E_CUDA); }
-    return done(0);
+    if (e != cudaSuccess) { set_error("max_step: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
+    return 0;
 }
 
 }  // extern "C"

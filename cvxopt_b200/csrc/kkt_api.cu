@@ -121,7 +121,7 @@ void set_error(const char *fmt, ...) {
     g_err = buf;
 }
 
-static int check_device(int device) {
+int check_device(int device) {
     int cnt = 0;
     cudaError_t e = cudaGetDeviceCount(&cnt);
     if (e != cudaSuccess || cnt == 0) {
@@ -285,17 +285,11 @@ int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const d
     }
     auto fail = [&](int r) { cvxb_kkt_destroy(k); return r; };
 #define KTRY(expr) do { int _r = (expr); if (_r) return fail(_r); } while (0)
-#define KCUDA(expr) do { cudaError_t _e = (expr); \
-        /* out of memory: give the scratch-buffer cache (common.cuh) back to the driver and try once more */ \
-        if (_e == cudaErrorMemoryAllocation) { cudaGetLastError(); tmp_cache_release(); _e = (expr); } \
-        if (_e != cudaSuccess) { \
-        set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e)); \
-        return fail(_e == cudaErrorMemoryAllocation ? CVXB_E_NOMEM : CVXB_E_CUDA); } } while (0)
-    KCUDA(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
-    KCUDA(cudaEventCreate(&k->e0)); KCUDA(cudaEventCreate(&k->e1));
-    KCUDA(cudaEventCreate(&k->e2)); KCUDA(cudaEventCreate(&k->e3));
-    KCUDA(cudaEventCreate(&k->t0)); KCUDA(cudaEventCreate(&k->t1));
-    KCUDA(cudaEventCreate(&k->m0)); KCUDA(cudaEventCreate(&k->m1));
+    CVXB_CUDA_RETRY(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
+    CVXB_CUDA_RETRY(cudaEventCreate(&k->e0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->e1));
+    CVXB_CUDA_RETRY(cudaEventCreate(&k->e2)); CVXB_CUDA_RETRY(cudaEventCreate(&k->e3));
+    CVXB_CUDA_RETRY(cudaEventCreate(&k->t0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->t1));
+    CVXB_CUDA_RETRY(cudaEventCreate(&k->m0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->m1));
     KTRY(chol_work_create(k->cw));
     const size_t nn = (size_t)(n > 0 ? n : 1);
     if (space == CVXB_DEVICE) {
@@ -304,21 +298,21 @@ int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const d
         double *g = nullptr;
         k->ldg = (c.cdim + 1) & ~1;     // even leading dimension: 16-byte aligned columns
         if (k->ldg < 2) k->ldg = 2;
-        KCUDA(cudaMalloc(&g, (size_t)k->ldg * nn * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&g, (size_t)k->ldg * nn * sizeof(double)));
         k->G = g; k->own_G = true;
         KTRY(upload_matrix(g, k->ldg, G, ldg, c.cdim, n, CVXB_HOST, k->st));
     }
     const long long ldk = (n + 1) & ~1;
-    KCUDA(cudaMalloc(&k->Kmat, (size_t)(ldk > 2 ? ldk : 2) * nn * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->Kmat, (size_t)(ldk > 2 ? ldk : 2) * nn * sizeof(double)));
     const int nblk = (n + NB - 1) / NB + 1;
-    KCUDA(cudaMalloc(&k->inv, (size_t)2 * nblk * NB * NB * sizeof(double)));   // inv + inv' blocks
+    CVXB_CUDA_RETRY(cudaMalloc(&k->inv, (size_t)2 * nblk * NB * NB * sizeof(double)));   // inv + inv' blocks
     k->nrest = c.mnl + c.sumq + c.sump;
     if (k->nrest > 0) {
         k->ldgs = (k->nrest + 1) & ~1;
-        KCUDA(cudaMalloc(&k->Gs, (size_t)k->ldgs * nn * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->Gs, (size_t)k->ldgs * nn * sizeof(double)));
     }
     if (c.sums2 > 0) {
-        KCUDA(cudaMalloc(&k->Gunp, (size_t)c.sums2 * nn * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->Gunp, (size_t)c.sums2 * nn * sizeof(double)));
         // workspace for the congruences: symmetric copies + intermediate, chunked over columns
         size_t per_col = (size_t)2 * c.maxs * c.maxs;
         size_t cols = (size_t)n < 1 ? 1 : (size_t)n;
@@ -326,36 +320,35 @@ int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const d
         const size_t cap = (size_t)1 << 29;            // 4 GiB of doubles at most
         if (want > cap) want = (cap / per_col ? cap / per_col : 1) * per_col;
         k->swork_doubles = want;
-        KCUDA(cudaMalloc(&k->swork, want * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->swork, want * sizeof(double)));
     }
-    if (c.mnl > 0) KCUDA(cudaMalloc(&k->Dfbuf, (size_t)c.mnl * nn * sizeof(double)));
+    if (c.mnl > 0) CVXB_CUDA_RETRY(cudaMalloc(&k->Dfbuf, (size_t)c.mnl * nn * sizeof(double)));
     if (p > 0) {
         k->lda_eq = (p + 1) & ~1;
         k->ldas = (n + 1) & ~1;
         k->ldkp = (p + 1) & ~1;
-        KCUDA(cudaMalloc(&k->Aeq, (size_t)k->lda_eq * nn * sizeof(double)));
-        KCUDA(cudaMalloc(&k->Asct, (size_t)k->ldas * p * sizeof(double)));
-        KCUDA(cudaMalloc(&k->Kp, (size_t)k->ldkp * p * sizeof(double)));
-        KCUDA(cudaMalloc(&k->invp, (size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB * sizeof(double)));
-        KCUDA(cudaMalloc(&k->yd, (size_t)p * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->Aeq, (size_t)k->lda_eq * nn * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->Asct, (size_t)k->ldas * p * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->Kp, (size_t)k->ldkp * p * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->invp, (size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->yd, (size_t)p * sizeof(double)));
         KTRY(upload_matrix(k->Aeq, k->lda_eq, A, lda, p, n, space, k->st));
     }
     KTRY(k->W.alloc(c));
     const size_t cd = (size_t)(c.cdim > 0 ? c.cdim : 1);
-    KCUDA(cudaMalloc(&k->bzp, cd * sizeof(double)));
-    KCUDA(cudaMalloc(&k->zin, cd * sizeof(double)));
-    KCUDA(cudaMalloc(&k->zt, cd * sizeof(double)));
-    KCUDA(cudaMalloc(&k->xv, nn * sizeof(double)));
-    KCUDA(cudaMalloc(&k->yv, (cd > nn ? cd : nn) * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->bzp, cd * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->zin, cd * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->zt, cd * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->xv, nn * sizeof(double)));
+    CVXB_CUDA_RETRY(cudaMalloc(&k->yv, (cd > nn ? cd : nn) * sizeof(double)));
     {
         size_t w1 = cd * (size_t)gemv_n_chunks(n), w2 = nn * (size_t)gemv_n_chunks(p > 0 ? p : 1);
         const size_t w3 = (size_t)(p > 0 ? p : 1) * (size_t)gemv_n_chunks(n);      // A operator
         if (w3 > w1) w1 = w3;
-        KCUDA(cudaMalloc(&k->gemv_ws, (w1 > w2 ? w1 : w2) * sizeof(double)));
+        CVXB_CUDA_RETRY(cudaMalloc(&k->gemv_ws, (w1 > w2 ? w1 : w2) * sizeof(double)));
     }
-    KCUDA(cudaStreamSynchronize(k->st));
+    CVXB_CUDA_RETRY(cudaStreamSynchronize(k->st));
 #undef KTRY
-#undef KCUDA
     *out = k;
     return 0;
 }
@@ -370,8 +363,6 @@ void cvxb_kkt_destroy(cvxb_kkt *k) {
     for (double *b : bufs) if (b) cudaFree(b);
     if (k->oz_work) cudaFree(k->oz_work);
     if (k->ext && k->ext_destroy) k->ext_destroy(k->ext);
-    k->W.destroy();
-    k->cone.destroy();
     chol_work_destroy(k->cw);
     cudaEvent_t evs[] = {k->e0, k->e1, k->e2, k->e3, k->t0, k->t1, k->m0, k->m1};
     for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);

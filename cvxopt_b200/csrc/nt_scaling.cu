@@ -15,7 +15,6 @@
 #include <cooperative_groups.h>
 #include <cmath>
 #include <cstdlib>
-#include <mutex>
 
 using namespace cvxb;
 
@@ -322,24 +321,6 @@ __global__ void transpose_small_kernel(int m, const double *src, double *dst) {
     dst[(size_t)i * m + j] = src[e];
 }
 
-struct NtCtx {
-    cudaStream_t st = nullptr;
-    CholWork cw;
-    bool ok = false;
-    std::mutex mu;
-};
-NtCtx g_nt;
-
-struct DTemp {
-    void *p = nullptr;
-    ~DTemp() { if (p) tmp_free(p); }
-    int alloc(size_t bytes) {
-        CVXB_CUDA(tmp_malloc(&p, bytes ? bytes : 8));
-        return 0;
-    }
-    double *d() const { return static_cast<double *>(p); }
-};
-
 int gemm_mm(int transa, int transb, int m, const double *A, const double *B, double *C, cudaStream_t st) {
     GemmDesc g;
     g.M = m; g.N = m; g.K = m;
@@ -366,18 +347,8 @@ int svd_jacobi(int m, double *B, double *Vw, double *U, double *V, double *sig, 
     set_identity_kernel<<<nb, T, 0, st>>>(m, Vw);
     count_launch();
     const int m2 = (m + 1) & ~1;
-    // one cooperative launch per sweep when every pair's CTA can be resident at once (CVXB_JACOBI_COOP=0: per-round launches)
-    bool coop = false;
-    {
-        static int coop_on = -1;
-        if (coop_on < 0) { const char *e = getenv("CVXB_JACOBI_COOP"); coop_on = (e && e[0] == '0') ? 0 : 1; }
-        int dev = 0, can = 0, per_sm = 0, sms = 0;
-        if (coop_on && cudaGetDevice(&dev) == cudaSuccess &&
-            cudaDeviceGetAttribute(&can, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && can &&
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, jacobi_sweep_kernel, 128, 0) == cudaSuccess)
-            coop = (long long)per_sm * sms >= m2 / 2;
-    }
+    // one cooperative launch per sweep when every pair's CTA can be resident at once, else one launch per round
+    const bool coop = coop_launch_fits((const void *)jacobi_sweep_kernel, 128, m2 / 2);
     for (int sweep = 0; sweep < 30; ++sweep) {
         CVXB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(int), st));
         if (coop) {
@@ -403,61 +374,26 @@ int svd_jacobi(int m, double *B, double *Vw, double *U, double *V, double *sig, 
     return 0;
 }
 
-int nt_ctx(NtCtx **out, std::unique_lock<std::mutex> &lk) {
-    int cnt = 0;
-    if (cudaGetDeviceCount(&cnt) != cudaSuccess || cnt == 0) {
-        cudaGetLastError();
-        set_error("no CUDA device available: cvxopt_b200 has no CPU fallback");
-        return CVXB_E_NOGPU;
-    }
-    CVXB_CUDA(cudaSetDevice(0));
-    lk = std::unique_lock<std::mutex>(g_nt.mu);
-    if (!g_nt.ok) {
-        CVXB_CUDA(cudaStreamCreateWithFlags(&g_nt.st, cudaStreamNonBlocking));
-        CVXB_TRY(chol_work_create(g_nt.cw));
-        g_nt.ok = true;
-    }
-    *out = &g_nt;
-    return 0;
-}
-
-// stage host <-> device
-struct HBuf {
-    double *dev = nullptr, *host = nullptr; size_t n = 0; bool owned = false;
-    ~HBuf() { if (owned && dev) tmp_free(dev); }
-    int in(double *src, size_t count, int space, cudaStream_t st, bool copy = true) {
-        n = count; host = src;
-        if (space == CVXB_DEVICE) { dev = src; return 0; }
-        CVXB_CUDA(tmp_malloc(&dev, (n ? n : 1) * sizeof(double)));
-        owned = true;
-        if (n && copy) CVXB_CUDA(cudaMemcpyAsync(dev, src, n * sizeof(double), cudaMemcpyHostToDevice, st));
-        return 0;
-    }
-    int out(cudaStream_t st) {
-        if (owned && n) CVXB_CUDA(cudaMemcpyAsync(host, dev, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-        return 0;
-    }
-};
-
 // the 's' part shared by compute (need_chol) and update: blocks of s/z are overwritten
-int nt_s_blocks(const ConeLayout &c, NtCtx *ctx, double *sS, double *zS, double *r, double *rti, double *lam_s,
+int nt_s_blocks(const ConeLayout &c, double *sS, double *zS, double *r, double *rti, double *lam_s,
                 bool is_update, cudaStream_t st) {
     if (c.ns == 0) return 0;
     const size_t mm = (size_t)c.maxs * c.maxs;
-    DTemp t[7], ti, tc;
-    for (int i = 0; i < 7; ++i) CVXB_TRY(t[i].alloc(mm * sizeof(double)));
-    CVXB_TRY(ti.alloc((size_t)c.maxs * sizeof(int)));
-    CVXB_TRY(tc.alloc(sizeof(int)));
-    double *Ls = t[0].d(), *Lz = t[1].d(), *M = t[2].d(), *Vw = t[3].d(), *U = t[4].d(), *V = t[5].d(), *tmp = t[6].d();
-    DTemp tn, tinv;
-    CVXB_TRY(tn.alloc((size_t)c.maxs * sizeof(double)));
+    Scratch<double> t[7];
+    Scratch<int> ti, tc;
+    for (int i = 0; i < 7; ++i) CVXB_TRY(t[i].alloc(mm));
+    CVXB_TRY(ti.alloc(c.maxs));
+    CVXB_TRY(tc.alloc(1));
+    double *Ls = t[0].p, *Lz = t[1].p, *M = t[2].p, *Vw = t[3].p, *U = t[4].p, *V = t[5].p, *tmp = t[6].p;
+    Scratch<double> tn, tinv;
+    CVXB_TRY(tn.alloc(c.maxs));
     const int nbk = (c.maxs + NB - 1) / NB + 1;
-    CVXB_TRY(tinv.alloc((size_t)2 * nbk * NB * NB * sizeof(double)));
-    DTemp tpanel;
+    CVXB_TRY(tinv.alloc((size_t)2 * nbk * NB * NB));
+    Scratch<double> tpanel;
     const int ldw = (c.maxs + 1) & ~1;
-    CVXB_TRY(tpanel.alloc((size_t)ldw * NB * sizeof(double)));
-    DTemp tinfo;
-    CVXB_TRY(tinfo.alloc(sizeof(int)));
+    CVXB_TRY(tpanel.alloc((size_t)ldw * NB));
+    Scratch<int> tinfo;
+    CVXB_TRY(tinfo.alloc(1));
     int lam_off = 0;
     for (int k = 0; k < c.ns; ++k) {
         const int m = c.s[k];
@@ -471,7 +407,7 @@ int nt_s_blocks(const ConeLayout &c, NtCtx *ctx, double *sS, double *zS, double 
                 double *L = w ? Lz : Ls;
                 tril_copy_kernel<<<nb, T, 0, st>>>(m, w ? zk : sk, L);
                 count_launch();
-                CVXB_TRY(potrf_lower_batched(m, L, m, 0, tinv.d(), 0, 1, static_cast<int *>(tinfo.p), tpanel.d(), ldw, st));
+                CVXB_TRY(potrf_lower_batched(m, L, m, 0, tinv.p, 0, 1, tinfo.p, tpanel.p, ldw, st));
                 int info = 0;
                 CVXB_CUDA(cudaMemcpyAsync(&info, tinfo.p, sizeof(int), cudaMemcpyDeviceToHost, st));
                 CVXB_CUDA(cudaStreamSynchronize(st));
@@ -486,7 +422,7 @@ int nt_s_blocks(const ConeLayout &c, NtCtx *ctx, double *sS, double *zS, double 
         }
         // M = Lz' Ls;  M V = U diag(lambda)
         CVXB_TRY(gemm_mm('T', 'N', m, Lz, Ls, M, st));
-        CVXB_TRY(svd_jacobi(m, M, Vw, U, V, lam_s + lam_off, tn.d(), static_cast<int *>(ti.p), static_cast<int *>(tc.p), st));
+        CVXB_TRY(svd_jacobi(m, M, Vw, U, V, lam_s + lam_off, tn.p, ti.p, tc.p, st));
         if (!is_update) {
             // r = Ls V lambda^-1/2,  rti = Lz U lambda^-1/2                         (= misc.py:402-414)
             CVXB_TRY(gemm_mm('N', 'N', m, Ls, V, rk, st));
@@ -514,6 +450,16 @@ int nt_s_blocks(const ConeLayout &c, NtCtx *ctx, double *sS, double *zS, double 
 
 }  // namespace
 
+bool cvxb::coop_launch_fits(const void *kernel, int threads, long long ctas) {
+    static const bool allowed = [] { const char *e = getenv("CVXB_JACOBI_COOP"); return !(e && e[0] == '0'); }();
+    int dev = 0, can = 0, per_sm = 0, sms = 0;
+    return allowed && cudaGetDevice(&dev) == cudaSuccess &&
+           cudaDeviceGetAttribute(&can, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && can &&
+           cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
+           cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0) == cudaSuccess &&
+           (long long)per_sm * sms >= ctas;
+}
+
 extern "C" {
 
 // misc.compute_scaling(s, z, lmbda, dims, mnl)  (misc.py:250-419).  s, z: cdim; lmbda: mnl + ml + sum q + sum s;
@@ -521,58 +467,49 @@ extern "C" {
 int cvxb_compute_scaling(const double *s, const double *z, double *lmbda, const cvxb_dims *dims,
                          const cvxb_scaling *Wout, int space) {
     if (!s || !z || !lmbda || !dims || !Wout) { set_error("compute_scaling: NULL argument"); return CVXB_E_ARG; }
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
     ConeLayout c;
     CVXB_TRY(c.init(dims));
-    NtCtx *ctx; std::unique_lock<std::mutex> lk;
-    int rc = nt_ctx(&ctx, lk);
-    if (rc) { c.destroy(); return rc; }
-    cudaStream_t st = ctx->st;
     const int nl = c.mnl + c.ml, nlam = nl + c.sumq;
-    int sums = 0;
-    for (int k = 0; k < c.ns; ++k) sums += c.s[k];
-    auto body = [&]() -> int {
-        HBuf S, Z, L, Dnl, Dnli, D, Di, V, Beta, R, Rti;
-        CVXB_TRY(S.in(const_cast<double *>(s), c.cdim, space, st));
-        CVXB_TRY(Z.in(const_cast<double *>(z), c.cdim, space, st));
-        CVXB_TRY(L.in(lmbda, (size_t)nlam + sums, space, st, false));
-        CVXB_TRY(Dnl.in(const_cast<double *>(Wout->dnl), c.mnl, space, st, false));
-        CVXB_TRY(Dnli.in(const_cast<double *>(Wout->dnli), c.mnl, space, st, false));
-        CVXB_TRY(D.in(const_cast<double *>(Wout->d), c.ml, space, st, false));
-        CVXB_TRY(Di.in(const_cast<double *>(Wout->di), c.ml, space, st, false));
-        CVXB_TRY(V.in(const_cast<double *>(Wout->v), c.sumq, space, st, false));
-        CVXB_TRY(Beta.in(const_cast<double *>(Wout->beta), c.nq, space, st, false));
-        CVXB_TRY(R.in(const_cast<double *>(Wout->r), c.sums2, space, st, false));
-        CVXB_TRY(Rti.in(const_cast<double *>(Wout->rti), c.sums2, space, st, false));
-        const int T = 256;
-        if (c.mnl > 0) { nt_l_compute_kernel<<<(c.mnl + T - 1) / T, T, 0, st>>>(c.mnl, S.dev, Z.dev, Dnl.dev, Dnli.dev, L.dev); count_launch(); }
-        if (c.ml > 0) {
-            nt_l_compute_kernel<<<(c.ml + T - 1) / T, T, 0, st>>>(c.ml, S.dev + c.mnl, Z.dev + c.mnl, D.dev, Di.dev, L.dev + c.mnl);
-            count_launch();
-        }
-        if (c.nq > 0) {
-            nt_q_compute_kernel<<<c.nq, 128, 0, st>>>(c.d_q, c.d_qoff, c.d_voff, nl, S.dev + nl, Z.dev + nl, V.dev,
-                                                       Beta.dev, L.dev);
-            count_launch();
-        }
-        CVXB_LAUNCH_CHECK();
-        if (c.ns > 0) {
-            // private copies of the 's' blocks (the inputs are const)
-            DTemp cs, cz;
-            CVXB_TRY(cs.alloc((size_t)c.sums2 * sizeof(double)));
-            CVXB_TRY(cz.alloc((size_t)c.sums2 * sizeof(double)));
-            const size_t so = (size_t)nl + c.sumq;
-            CVXB_CUDA(cudaMemcpyAsync(cs.p, S.dev + so, (size_t)c.sums2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-            CVXB_CUDA(cudaMemcpyAsync(cz.p, Z.dev + so, (size_t)c.sums2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-            CVXB_TRY(nt_s_blocks(c, ctx, cs.d(), cz.d(), R.dev, Rti.dev, L.dev + nlam, false, st));
-        }
-        CVXB_TRY(L.out(st)); CVXB_TRY(Dnl.out(st)); CVXB_TRY(Dnli.out(st)); CVXB_TRY(D.out(st)); CVXB_TRY(Di.out(st));
-        CVXB_TRY(V.out(st)); CVXB_TRY(Beta.out(st)); CVXB_TRY(R.out(st)); CVXB_TRY(Rti.out(st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        return 0;
-    };
-    rc = body();
-    c.destroy();
-    return rc;
+    Staged S, Z, L, Dnl, Dnli, D, Di, V, Beta, R, Rti;
+    CVXB_TRY(S.in(s, c.cdim, space, st));
+    CVXB_TRY(Z.in(z, c.cdim, space, st));
+    CVXB_TRY(L.in(lmbda, (size_t)nlam + c.sums, space, st, false));
+    CVXB_TRY(Dnl.in(Wout->dnl, c.mnl, space, st, false));
+    CVXB_TRY(Dnli.in(Wout->dnli, c.mnl, space, st, false));
+    CVXB_TRY(D.in(Wout->d, c.ml, space, st, false));
+    CVXB_TRY(Di.in(Wout->di, c.ml, space, st, false));
+    CVXB_TRY(V.in(Wout->v, c.sumq, space, st, false));
+    CVXB_TRY(Beta.in(Wout->beta, c.nq, space, st, false));
+    CVXB_TRY(R.in(Wout->r, c.sums2, space, st, false));
+    CVXB_TRY(Rti.in(Wout->rti, c.sums2, space, st, false));
+    const int T = 256;
+    if (c.mnl > 0) { nt_l_compute_kernel<<<(c.mnl + T - 1) / T, T, 0, st>>>(c.mnl, S.dev, Z.dev, Dnl.dev, Dnli.dev, L.dev); count_launch(); }
+    if (c.ml > 0) {
+        nt_l_compute_kernel<<<(c.ml + T - 1) / T, T, 0, st>>>(c.ml, S.dev + c.mnl, Z.dev + c.mnl, D.dev, Di.dev, L.dev + c.mnl);
+        count_launch();
+    }
+    if (c.nq > 0) {
+        nt_q_compute_kernel<<<c.nq, 128, 0, st>>>(c.d_q, c.d_qoff, c.d_voff, nl, S.dev + nl, Z.dev + nl, V.dev,
+                                                   Beta.dev, L.dev);
+        count_launch();
+    }
+    CVXB_LAUNCH_CHECK();
+    if (c.ns > 0) {
+        // private copies of the 's' blocks (the inputs are const)
+        Scratch<double> cs, cz;
+        CVXB_TRY(cs.alloc(c.sums2));
+        CVXB_TRY(cz.alloc(c.sums2));
+        const size_t so = (size_t)nl + c.sumq;
+        CVXB_CUDA(cudaMemcpyAsync(cs.p, S.dev + so, (size_t)c.sums2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_CUDA(cudaMemcpyAsync(cz.p, Z.dev + so, (size_t)c.sums2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(nt_s_blocks(c, cs.p, cz.p, R.dev, Rti.dev, L.dev + nlam, false, st));
+    }
+    CVXB_TRY(L.out(st)); CVXB_TRY(Dnl.out(st)); CVXB_TRY(Dnli.out(st)); CVXB_TRY(D.out(st)); CVXB_TRY(Di.out(st));
+    CVXB_TRY(V.out(st)); CVXB_TRY(Beta.out(st)); CVXB_TRY(R.out(st)); CVXB_TRY(Rti.out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 // misc.update_scaling(W, lmbda, s, z)  (misc.py:422-634): W and lmbda are updated in place; s, z are overwritten
@@ -580,53 +517,44 @@ int cvxb_compute_scaling(const double *s, const double *z, double *lmbda, const 
 int cvxb_update_scaling(const cvxb_scaling *W, double *lmbda, double *s, double *z, const cvxb_dims *dims,
                         int space) {
     if (!s || !z || !lmbda || !dims || !W) { set_error("update_scaling: NULL argument"); return CVXB_E_ARG; }
+    CallCtx ctx; CVXB_TRY(ctx.acquire(0));
+    cudaStream_t st = ctx.st;
     ConeLayout c;
     CVXB_TRY(c.init(dims));
-    NtCtx *ctx; std::unique_lock<std::mutex> lk;
-    int rc = nt_ctx(&ctx, lk);
-    if (rc) { c.destroy(); return rc; }
-    cudaStream_t st = ctx->st;
     const int nl = c.mnl + c.ml, nlam = nl + c.sumq;
-    int sums = 0;
-    for (int k = 0; k < c.ns; ++k) sums += c.s[k];
-    auto body = [&]() -> int {
-        HBuf S, Z, L, Dnl, Dnli, D, Di, V, Beta, R, Rti;
-        CVXB_TRY(S.in(s, c.cdim, space, st));
-        CVXB_TRY(Z.in(z, c.cdim, space, st));
-        CVXB_TRY(L.in(lmbda, (size_t)nlam + sums, space, st));
-        CVXB_TRY(Dnl.in(const_cast<double *>(W->dnl), c.mnl, space, st));
-        CVXB_TRY(Dnli.in(const_cast<double *>(W->dnli), c.mnl, space, st, false));
-        CVXB_TRY(D.in(const_cast<double *>(W->d), c.ml, space, st));
-        CVXB_TRY(Di.in(const_cast<double *>(W->di), c.ml, space, st, false));
-        CVXB_TRY(V.in(const_cast<double *>(W->v), c.sumq, space, st));
-        CVXB_TRY(Beta.in(const_cast<double *>(W->beta), c.nq, space, st));
-        CVXB_TRY(R.in(const_cast<double *>(W->r), c.sums2, space, st));
-        CVXB_TRY(Rti.in(const_cast<double *>(W->rti), c.sums2, space, st));
-        const int T = 256;
-        if (c.mnl > 0) { nt_l_update_kernel<<<(c.mnl + T - 1) / T, T, 0, st>>>(c.mnl, S.dev, Z.dev, Dnl.dev, Dnli.dev, L.dev); count_launch(); }
-        if (c.ml > 0) {
-            nt_l_update_kernel<<<(c.ml + T - 1) / T, T, 0, st>>>(c.ml, S.dev + c.mnl, Z.dev + c.mnl, D.dev, Di.dev, L.dev + c.mnl);
-            count_launch();
-        }
-        if (c.nq > 0) {
-            nt_q_update_kernel<<<c.nq, 128, 0, st>>>(c.d_q, c.d_qoff, c.d_voff, nl, S.dev + nl, Z.dev + nl, V.dev, Beta.dev,
-                                                      L.dev);
-            count_launch();
-        }
-        CVXB_LAUNCH_CHECK();
-        if (c.ns > 0) {
-            const size_t so = (size_t)nl + c.sumq;
-            CVXB_TRY(nt_s_blocks(c, ctx, S.dev + so, Z.dev + so, R.dev, Rti.dev, L.dev + nlam, true, st));
-        }
-        CVXB_TRY(S.out(st)); CVXB_TRY(Z.out(st)); CVXB_TRY(L.out(st));
-        CVXB_TRY(Dnl.out(st)); CVXB_TRY(Dnli.out(st)); CVXB_TRY(D.out(st)); CVXB_TRY(Di.out(st));
-        CVXB_TRY(V.out(st)); CVXB_TRY(Beta.out(st)); CVXB_TRY(R.out(st)); CVXB_TRY(Rti.out(st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        return 0;
-    };
-    rc = body();
-    c.destroy();
-    return rc;
+    Staged S, Z, L, Dnl, Dnli, D, Di, V, Beta, R, Rti;
+    CVXB_TRY(S.in(s, c.cdim, space, st));
+    CVXB_TRY(Z.in(z, c.cdim, space, st));
+    CVXB_TRY(L.in(lmbda, (size_t)nlam + c.sums, space, st));
+    CVXB_TRY(Dnl.in(W->dnl, c.mnl, space, st));
+    CVXB_TRY(Dnli.in(W->dnli, c.mnl, space, st, false));
+    CVXB_TRY(D.in(W->d, c.ml, space, st));
+    CVXB_TRY(Di.in(W->di, c.ml, space, st, false));
+    CVXB_TRY(V.in(W->v, c.sumq, space, st));
+    CVXB_TRY(Beta.in(W->beta, c.nq, space, st));
+    CVXB_TRY(R.in(W->r, c.sums2, space, st));
+    CVXB_TRY(Rti.in(W->rti, c.sums2, space, st));
+    const int T = 256;
+    if (c.mnl > 0) { nt_l_update_kernel<<<(c.mnl + T - 1) / T, T, 0, st>>>(c.mnl, S.dev, Z.dev, Dnl.dev, Dnli.dev, L.dev); count_launch(); }
+    if (c.ml > 0) {
+        nt_l_update_kernel<<<(c.ml + T - 1) / T, T, 0, st>>>(c.ml, S.dev + c.mnl, Z.dev + c.mnl, D.dev, Di.dev, L.dev + c.mnl);
+        count_launch();
+    }
+    if (c.nq > 0) {
+        nt_q_update_kernel<<<c.nq, 128, 0, st>>>(c.d_q, c.d_qoff, c.d_voff, nl, S.dev + nl, Z.dev + nl, V.dev, Beta.dev,
+                                                  L.dev);
+        count_launch();
+    }
+    CVXB_LAUNCH_CHECK();
+    if (c.ns > 0) {
+        const size_t so = (size_t)nl + c.sumq;
+        CVXB_TRY(nt_s_blocks(c, S.dev + so, Z.dev + so, R.dev, Rti.dev, L.dev + nlam, true, st));
+    }
+    CVXB_TRY(S.out(st)); CVXB_TRY(Z.out(st)); CVXB_TRY(L.out(st));
+    CVXB_TRY(Dnl.out(st)); CVXB_TRY(Dnli.out(st)); CVXB_TRY(D.out(st)); CVXB_TRY(Di.out(st));
+    CVXB_TRY(V.out(st)); CVXB_TRY(Beta.out(st)); CVXB_TRY(R.out(st)); CVXB_TRY(Rti.out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 }  // extern "C"

@@ -149,6 +149,10 @@ int cvxb_kkt_symv_H(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
 int cvxb_kkt_gemv_A(cvxb_kkt *k, const double *x, double *y, double alpha, double beta,
                     int trans, int space);
 
+/* The calls from here to cvxb_gemm take no handle.  The cone algebra and the NT scaling run on device 0, the dense
+ * building blocks on their `device` argument, and calls on one device are serialised across host threads (each
+ * call holds that device's one stream until it returns). */
+
 /* ---- cone algebra: mirror of src/C/misc_solvers.c (12 entry points,
  * misc_solvers.c:1155-1173).  x is xr x xc column-major with leading
  * dimension xr; everything in place as in the reference. */

@@ -30,10 +30,35 @@ def test_no_cpu_fallback():
     """Without a GPU every compute entry point must fail loudly, never fall back."""
     import numpy as np
     import cvxopt_b200
+    from cvxopt_b200 import _lib, misc_solvers as ms, scaling
     if cvxopt_b200.device_count() > 0:
         pytest.skip("a GPU is visible")
     with pytest.raises(RuntimeError):
         cvxopt_b200.kkt_chol(np.zeros((4, 2), order="F"), {"l": 4, "q": [], "s": []})
+    # the entry points without a handle check for the device before they touch it
+    dims = {"l": 2, "q": [3], "s": [2]}           # cdim 9, packed 8, lmbda 7
+    W = {"d": np.ones(2), "di": np.ones(2), "v": [np.array([1.0, 0.0, 0.0])], "beta": [1.0],
+         "r": [np.eye(2, order="F")], "rti": [np.eye(2, order="F")]}
+    calls = [
+        lambda: ms.scale(np.ones(9), W), lambda: ms.scale2(np.ones(7), np.ones(9), dims),
+        lambda: ms.pack(np.ones(9), np.zeros(8), dims), lambda: ms.unpack(np.ones(8), np.zeros(9), dims),
+        lambda: ms.pack2(np.ones(9), dims), lambda: ms.symm(np.ones(4), 2),
+        lambda: ms.sprod(np.ones(9), np.ones(9), dims), lambda: ms.sinv(np.ones(9), np.ones(7), dims),
+        lambda: ms.trisc(np.ones(9), dims), lambda: ms.triusc(np.ones(9), dims),
+        lambda: ms.sdot(np.ones(9), np.ones(9), dims), lambda: ms.max_step(np.ones(9), dims),
+        lambda: scaling.compute_scaling(np.ones(9), np.ones(9), np.zeros(7), dims),
+        lambda: scaling.update_scaling(W, np.ones(7), np.ones(9), np.ones(9)),
+    ]
+    for call in calls:
+        with pytest.raises(RuntimeError, match="no CUDA device available"):
+            call()
+    lib = _lib.load()
+    a, c, inv = np.eye(2, order="F"), np.zeros((2, 2), order="F"), np.zeros(2 * 128 * 128)
+    assert lib.cvxb_potrf(2, a.ctypes.data, 2, inv.ctypes.data, 0) == _lib.E_NOGPU
+    assert "no CUDA device available" in _lib.last_error()
+    assert lib.cvxb_gemm(ord("N"), ord("N"), 2, 2, 2, 1.0, a.ctypes.data, 2, a.ctypes.data, 2, 0.0,
+                         c.ctypes.data, 2, 0) == _lib.E_NOGPU
+    assert "no CUDA device available" in _lib.last_error()
 
 
 def test_product_does_not_import_oracle():

@@ -5,11 +5,12 @@ CPU part: the module imports next to the reference (import_cvxopt() finds the ba
 functions with the reference's keyword lists, rejects bad arguments with the reference's exception types, and
 fails loudly (RuntimeError) when asked to compute without a GPU.
 GPU part: the 12 functions are swapped into cvxopt.misc and the UNMODIFIED solvers run to the reference's
-iteration count with the reference's own kktsolver names ('chol', 'qr', 'ldl')."""
+iteration count with the reference's own kktsolver names ('chol', 'qr', 'ldl'); concurrent host threads get the
+results of one thread."""
 import numpy as np
 import pytest
 
-from problems import cone_lp, dense_qp
+from problems import cone_lp, cone_point, dense_qp
 
 NAMES = ["scale", "scale2", "pack", "pack2", "unpack", "symm", "sprod", "sinv", "trisc", "triusc", "sdot",
          "max_step"]
@@ -149,3 +150,56 @@ def test_unmodified_sdp_and_socp_with_the_extension_swapped_in(ref, solver):
     want, got = _solve_both(ref, lambda: solvers.socp(matrix(c), Gm[:3, :], hm[:3], Gq, hq, kktsolver=solver))
     assert want["status"] == got["status"] == "optimal" and want["iterations"] == got["iterations"]
     np.testing.assert_allclose(got["primal objective"], want["primal objective"], rtol=1e-7)
+
+
+@pytest.mark.gpu
+def test_concurrent_host_threads_get_single_thread_results():
+    """The entry points without a handle share one stream per device and hold its lock for the whole call.  Two
+    host threads calling cvxopt_b200.misc_solvers at once (ctypes releases the GIL, so the calls overlap in the
+    library) must get, bit for bit, what the same calls give from one thread."""
+    import threading
+    from cvxopt_b200 import misc_solvers as ms
+    dims = {"l": 5, "q": [4, 3], "s": [3, 70]}       # 70: the multi-launch Jacobi eigensolver of max_step
+
+    def inputs(seed):
+        rng = np.random.Generator(np.random.PCG64(seed))
+        lam = [rng.uniform(0.5, 2.0, dims["l"])]
+        lam += [np.concatenate([[2.0], rng.uniform(-0.5, 0.5, k - 1) / k]) for k in dims["q"]]
+        lam += [rng.uniform(0.5, 2.0, k) for k in dims["s"]]
+        return cone_point(dims, rng), cone_point(dims, rng), np.concatenate(lam)
+
+    def calls(x, y, lam):
+        out = []
+        v = x.copy()
+        ms.scale2(lam, v, dims)
+        out.append(v)
+        out.append(np.array([ms.sdot(x, y, dims)]))
+        v = x.copy()
+        ms.sprod(v, y, dims)
+        out.append(v)
+        v, sig = x.copy(), np.zeros(sum(dims["s"]))
+        out += [np.array([ms.max_step(v, dims, sigma=sig)]), v, sig]
+        return out
+
+    data = [inputs(31), inputs(32)]                  # each thread its own inputs
+    want = [calls(*d) for d in data]
+    errors, start = [], threading.Barrier(2)
+
+    def worker(t):
+        try:
+            start.wait()
+            for it in range(40):
+                got = calls(*data[t])
+                for k, (g, w) in enumerate(zip(got, want[t])):
+                    if g.tobytes() != w.tobytes():
+                        errors.append("thread %d, iteration %d, result %d differs" % (t, it, k))
+                        return
+        except Exception as e:           # noqa: BLE001 - reported by the main thread
+            errors.append("thread %d: %r" % (t, e))
+
+    threads = [threading.Thread(target=worker, args=(t,)) for t in range(2)]
+    for th in threads:
+        th.start()
+    for th in threads:
+        th.join()
+    assert not errors, errors
