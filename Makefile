@@ -11,7 +11,7 @@ PYINC := $(shell $(PYTHON) -c "import sysconfig; print(sysconfig.get_paths()['in
 PYEXT := $(shell $(PYTHON) -c "import sysconfig; print(sysconfig.get_config_var('EXT_SUFFIX'))")
 EXT := cvxopt_b200/_misc_solvers$(PYEXT)
 
-all: $(LIB) $(EXT)
+all: $(LIB) $(EXT) tools/dmma_rate
 
 $(EXT): $(SRC)/_misc_solvers.c include/cvxopt_b200.h $(LIB)
 	gcc -O2 -fPIC -shared -Wall -I$(PYINC) $< -o $@ -Lcvxopt_b200 -lcvxopt_b200 -Wl,-rpath,'$$ORIGIN'
@@ -22,6 +22,10 @@ $(SRC)/%.o: $(SRC)/%.cu $(SRC)/common.cuh $(SRC)/cone.cuh $(SRC)/kkt_internal.cu
 $(LIB): $(OBJ)
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJ) -lcudart
 
+# standalone probe of the fp64 mma.sync shapes (fragment layouts, issue rate); see tools/README.md
+tools/dmma_rate: tools/dmma_rate.cu
+	$(NVCC) $(ARCH) -O3 -std=c++17 -o $@ $<
+
 clean:
-	rm -f $(OBJ) $(LIB) $(EXT)
+	rm -f $(OBJ) $(LIB) $(EXT) tools/dmma_rate
 .PHONY: all clean

@@ -29,7 +29,9 @@ constexpr int LDM = NB + 4;            // column stride (doubles) of the shared-
 constexpr int POTF2_SMEM = (NB * LDM + NB * SP + 4 * 80) * 8;
 
 // acc[cf][rf] -= sum_k Lt[c, k] Lt[r, k] over k = 0..127 for the tiles rf >= S_cf of each column
-// fragment cf (Lt in shared memory, column-major with stride LDM; Ma/Mb already offset by lane)
+// fragment cf (Lt in shared memory, column-major with stride LDM; Ma/Mb already offset by lane).
+// Column fragments 2mf and 2mf+1 go through one m16n8k4, so where only the first of the pair is live the
+// second, strictly upper tile gets a product too; nothing reads an upper tile's accumulators.
 template <int PAT>      // 0: every tile, 1: rf >= cf, 2: rf >= 4 + cf
 __device__ __forceinline__ void sym_update(double (&acc)[4][8][2], const double *Ma, const double *Mb) {
 #pragma unroll 2
@@ -40,13 +42,13 @@ __device__ __forceinline__ void sym_update(double (&acc)[4][8][2], const double 
 #pragma unroll
         for (int rf = 0; rf < 8; ++rf) bfr[rf] = Mb[rf * 8 + kk * 4 * LDM];
 #pragma unroll
-        for (int cf = 0; cf < 4; ++cf)
+        for (int mf = 0; mf < 2; ++mf)
 #pragma unroll
             for (int rf = 0; rf < 8; ++rf) {
-                constexpr bool dummy = true; (void)dummy;
-                if (PAT == 1 && rf < cf) continue;           // compile-time after unrolling
-                if (PAT == 2 && rf < 4 + cf) continue;
-                dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf], bfr[rf]);
+                if (PAT == 1 && rf < 2 * mf) continue;           // compile-time after unrolling
+                if (PAT == 2 && rf < 4 + 2 * mf) continue;
+                dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0], acc[2 * mf + 1][rf][1],
+                           a[2 * mf], a[2 * mf + 1], bfr[rf]);
             }
     }
 }
@@ -136,9 +138,11 @@ potf2_inv_kernel(double *A, long long lda, int jb, double *inv, double *invT, in
 #pragma unroll
             for (int rf = 0; rf < 8; ++rf) bfr[rf] = tq[rf * 8 + kk * 4 * LDM];
 #pragma unroll
-            for (int cf = 0; cf < 4; ++cf)
+            for (int mf = 0; mf < 2; ++mf)
 #pragma unroll
-                for (int rf = 0; rf < 8; ++rf) dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf], bfr[rf]);
+                for (int rf = 0; rf < 8; ++rf)
+                    dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0],
+                               acc[2 * mf + 1][rf][1], a[2 * mf], a[2 * mf + 1], bfr[rf]);
         }
         __syncthreads();                                // every warp is done reading Tprev from M
 #pragma unroll
@@ -269,13 +273,17 @@ potf2_inv_kernel(double *A, long long lda, int jb, double *inv, double *invT, in
 #pragma unroll
                 for (int rf = 0; rf < 8; ++rf) bfr[rf][kk] = P[(wr * 64 + rf * 8 + g4) * SP + kk * 4 + t4];
             }
+            // column fragments 2mf and 2mf+1 share one m16n8k4; when only the first is final (it is column
+            // block t, published above) its accumulators take a product nobody reads
 #pragma unroll
-            for (int cf = 0; cf < 4; ++cf) {
-                if (wc * 4 + cf <= t) continue;            // column block already final
+            for (int mf = 0; mf < 2; ++mf) {
+                if (wc * 4 + 2 * mf + 1 <= t) continue;    // both column blocks already final
 #pragma unroll
                 for (int rf = 0; rf < 8; ++rf) {
-                    dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf][0], bfr[rf][0]);
-                    dmma(acc[cf][rf][0], acc[cf][rf][1], a[cf][1], bfr[rf][1]);
+                    dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0], acc[2 * mf + 1][rf][1],
+                               a[2 * mf][0], a[2 * mf + 1][0], bfr[rf][0]);
+                    dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0], acc[2 * mf + 1][rf][1],
+                               a[2 * mf][1], a[2 * mf + 1][1], bfr[rf][1]);
                 }
             }
         }

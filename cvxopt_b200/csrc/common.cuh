@@ -126,12 +126,25 @@ constexpr int NB = 128;            // Cholesky block size == GEMM tile edge
 
 // ---- device helpers ---------------------------------------------------------
 #ifdef __CUDACC__
-// fp64 tensor-core MMA: D(8x8) += A(8x4,row) * B(4x8,col).  SASS: DMMA.8x8x4.
+// fp64 tensor-core MMA, Ampere shape: D(8x8) += A(8x4,row) * B(4x8,col).  SASS: DMMA.8x8x4.
 // lane -> A[lane>>2][lane&3], B[k=lane&3][n=lane>>2], D[lane>>2][2*(lane&3)+{0,1}]
+// Only for 8-wide tiles: on sm_90 it runs at half the fp64 tensor rate of dmma16x8x4 (128 against 256 flop per
+// clock and SM, tools/dmma_rate).
 __device__ __forceinline__ void dmma(double &d0, double &d1, double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                  : "+d"(d0), "+d"(d1)
                  : "d"(a), "d"(b));
+}
+// fp64 tensor-core MMA, sm_90 shape: D(16x8) += A(16x4,row) * B(4x8,col).  SASS: DMMA.16x8x4.
+// lane -> A[lane>>2][lane&3] (a0), A[8+(lane>>2)][lane&3] (a1), B[k=lane&3][n=lane>>2],
+//         D[lane>>2][2*(lane&3)+{0,1}] (d0,d1), D[8+(lane>>2)][2*(lane&3)+{0,1}] (d2,d3)
+// so it is the two products dmma(d0,d1,a0,b) and dmma(d2,d3,a1,b) of 8-row blocks that share b, in one instruction
+// (fragment map checked on the device by tools/dmma_rate).
+__device__ __forceinline__ void dmma16x8x4(double &d0, double &d1, double &d2, double &d3, double a0, double a1,
+                                           double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                 : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
+                 : "d"(a0), "d"(a1), "d"(b));
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {

@@ -9,8 +9,10 @@
 //   * Cholesky trailing update A22 -= L21 L21'                   (X=Y=L21, M-major, lower)
 //   * the 's'-cone congruences r' X r                            (batched general GEMMs)
 //
-// wgmma has no fp64 form, so the fp64 tensor path is warp-level DMMA.8x8x4
-// (mma.sync.m8n8k4.f64); the H100 SXM data sheet gives 67 TF/s for it (132 SMs).
+// wgmma has no fp64 form, so the fp64 tensor path is warp-level mma.sync.  sm_90 runs the
+// 16x8 shapes (DMMA.16x8x4/8/16) at 256 flop/clk/SM, the data-sheet 67 TF/s at 1.98 GHz, and
+// the Ampere shape DMMA.8x8x4 at half that (tools/dmma_rate), so the kernel issues
+// m16n8k4 (dmma16x8x4): same fragments as two m8n8k4, half the instructions.
 // A 128x64x16 tile step moves 24 KB for 131072 FMAs, so operand traffic is small next to
 // the tensor work; the design goal is to keep the DMMA pipe issuing:
 //   * 128-thread CTAs (4 warps, 64x32 warp tiles, 64 accumulator doubles / thread),
@@ -24,7 +26,8 @@
 //
 // MMA roles are swapped w.r.t. the matrix: the MMA "m" index runs over C's columns
 // (Y operand), the "n" index over C's rows (X operand), so each thread's accumulator
-// pair is two consecutive ROWS of a column-major C (one 16-byte access).
+// pair is two consecutive ROWS of a column-major C (one 16-byte access).  One m16n8k4
+// covers the column fragments cf = 2mf and 2mf+1 (8 columns apart) of a row fragment.
 #include "common.cuh"
 
 namespace cvxb {
@@ -342,10 +345,11 @@ __global__ void __launch_bounds__(THREADS, 2) dmma_gemm_kernel(const KParams p) 
                 }
             }
 #pragma unroll
-            for (int cf = 0; cf < 4; ++cf)
+            for (int mf = 0; mf < 2; ++mf)
 #pragma unroll
                 for (int rf = 0; rf < 8; ++rf)
-                    dmma(acc[cf][rf][0], acc[cf][rf][1], a[cur][cf], bf[cur][rf]);
+                    dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0],
+                               acc[2 * mf + 1][rf][1], a[cur][2 * mf], a[cur][2 * mf + 1], bf[cur][rf]);
         }
     }
     cp_async_wait<0>();

@@ -127,7 +127,7 @@ int cvxb_kkt_trace(cvxb_kkt *k, unsigned long long *out, int nsteps);
 /* per-kernel-class CUDA-event breakdown of the last factor (syrk, potrf, scale) */
 int cvxb_kkt_last_breakdown(cvxb_kkt *k, double *ms3);
 /* which kernel computed the 'l'-row SYRK of the last factor: 0 none (ml == 0), 1 fp64 DMMA
- * (mma.sync.m8n8k4.f64, the default), 2 int8 slices on wgmma s8 (CVXB_OZAKI=2 always, =1 for large problems;
+ * (mma.sync.m16n8k4.f64, the default), 2 int8 slices on wgmma s8 (CVXB_OZAKI=2 always, =1 for large problems;
  * falls back to 1 when the slice workspace does not fit in device memory) */
 int cvxb_kkt_syrk_path(cvxb_kkt *k);
 /* int8-slice path only: CUDA-event time of the MMA launches of the last factor's SYRK, without the two slicing kernels
