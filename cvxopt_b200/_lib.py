@@ -33,6 +33,7 @@ _SIGS = {
     "cvxb_device_count": (C.c_int, []),
     "cvxb_version": (C.c_int, []),
     "cvxb_launch_count": (C.c_ulonglong, []),
+    "cvxb_device_bytes": (C.c_ulonglong, []),
     "cvxb_malloc": (C.c_int, [C.POINTER(C.c_void_p), C.c_ulonglong]),
     "cvxb_free": (C.c_int, [C.c_void_p]),
     "cvxb_memcpy_h2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_ulonglong]),

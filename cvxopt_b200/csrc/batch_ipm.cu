@@ -13,6 +13,7 @@
 // Nothing leaves the device between iterations except one int ("how many are done").
 #include "cone.cuh"
 #include <cstdlib>
+#include <memory>
 
 using namespace cvxb;
 
@@ -310,13 +311,13 @@ struct cvxb_batch {
     long long ldg = 0, ldp = 0, ldk = 0;
     long long sG = 0, sP = 0, sK = 0, sInv = 0;
     int nblk = 0;
-    double *P = nullptr, *G = nullptr, *q = nullptr, *h = nullptr;
-    double *K = nullptr, *inv = nullptr, *panel = nullptr, *gemv_ws = nullptr;
-    double *vecs = nullptr;          // all n- and m-vectors
+    DevBuf<double> P, G, K, inv, panel, gemv_ws;
+    DevBuf<double> vecs;             // all n- and m-vectors
+    double *q = nullptr, *h = nullptr;   // in vecs
     Ptrs p;
-    Scal *sc = nullptr;
-    int *d_info = nullptr, *d_ndone = nullptr;
-    int *d_done = nullptr, *d_pairs = nullptr, *d_perm = nullptr;     // compaction: done flags, swap list, slot -> problem
+    DevBuf<Scal> sc;
+    DevBuf<int> d_info, d_ndone;
+    DevBuf<int> d_done, d_pairs, d_perm;     // compaction: done flags, swap list, slot -> problem
     std::vector<int> perm;           // slot -> original problem index (identity unless the last solve compacted)
     bool permuted = false;
     int compact = 1;                 // CVXB_BATCH_COMPACT=0 disables
@@ -327,62 +328,48 @@ struct cvxb_batch {
     bool loaded = false;
     int iters_run = 0;
     double solve_ms = 0;
-    // single large problem: SYRK on the int8 tensor path (ozaki_syrk.cu), same rule as cvxb_kkt_factor:
-    // mode 1 when B == 1, n >= 4096, m >= 8192; 2: whenever B == 1; 0 (default): never.  CVXB_OZAKI = 0/1/2
-    // read at create.
+    // single large problem: SYRK on the int8 tensor path (ozaki_syrk.cu), same rule as cvxb_kkt_factor
+    // (ozaki_use) when B == 1; ozaki_mode() at create
     int i8_mode = 0;
     int syrk_path = 0;
-    void *oz_work = nullptr;
-    size_t oz_bytes = 0;
+    DevBuf<char> oz_work;
+    ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
+        if (st) cudaStreamSynchronize(st);
+        for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
+        if (st) cudaStreamDestroy(st);
+    }
 };
 
 namespace {
 
 int batch_factor(cvxb_batch *b) {
     cudaStream_t st = b->st;
-    bool i8 = b->B == 1 && b->m > 0 && (b->i8_mode == 2 || (b->i8_mode == 1 && b->n >= 4096 && b->m >= 8192));
-    if (i8) {
-        // K = P + G' diag(di)^2 G from nine int8 slices per entry (fp64-accurate, ~1.8x the DMMA SYRK);
-        // same size rule and same fallback (workspace does not fit -> DMMA kernel) as cvxb_kkt_factor
-        const size_t need = ozaki_workspace_bytes(b->n, b->m, 9);
-        if (need > b->oz_bytes) {
-            if (b->oz_work) cudaFree(b->oz_work);
-            b->oz_work = nullptr; b->oz_bytes = 0;
-            cudaError_t ae = cudaMalloc(&b->oz_work, need);
-            if (ae == cudaErrorMemoryAllocation) { cudaGetLastError(); tmp_cache_release(); ae = cudaMalloc(&b->oz_work, need); }
-            if (ae != cudaSuccess) {
-                cudaGetLastError();
-                b->oz_work = nullptr;
-                i8 = false;
-            } else {
-                b->oz_bytes = need;
-            }
-        }
-    }
+    // K = P + G' diag(di)^2 G from nine int8 slices per entry (fp64-accurate, ~1.8x the DMMA SYRK)
+    const bool i8 = b->B == 1 && b->m > 0 && ozaki_use(b->i8_mode, b->n, b->m, b->oz_work);
     b->syrk_path = i8 ? 2 : 1;
     if (i8) {
-        CVXB_TRY(ozaki_syrk(b->n, b->m, b->G, b->ldg, b->p.di, b->P, b->ldp, 1.0, b->K, b->ldk, 9, 0,
-                            b->oz_work, st));
-        CVXB_TRY(potrf_lower(b->n, b->K, (int)b->ldk, b->inv, b->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(b->d_info, b->cw.d_info, sizeof(int), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(ozaki_syrk(b->n, b->m, b->G.p, b->ldg, b->p.di, b->P.p, b->ldp, 1.0, b->K.p, b->ldk, 9, 0,
+                            b->oz_work.p, st));
+        CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
         return 0;
     }
     GemmDesc g;
     g.M = b->n; g.N = b->n; g.K = b->m;
-    g.X = b->G; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
-    g.Y = b->G; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
+    g.X = b->G.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
+    g.Y = b->G.p; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
     g.w = b->p.di2; g.sW = b->m;
-    g.D = b->P; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
-    g.C = b->K; g.ldc = (int)b->ldk; g.sC = b->sK;
+    g.D = b->P.p; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
+    g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
     g.lower_only = true; g.batch = b->Bact;
-    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws;
+    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
     CVXB_TRY(dmma_gemm(g, st));
     if (b->B == 1) {
-        CVXB_TRY(potrf_lower(b->n, b->K, (int)b->ldk, b->inv, b->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(b->d_info, b->cw.d_info, sizeof(int), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
     } else {
-        CVXB_TRY(potrf_lower_batched(b->n, b->K, (int)b->ldk, b->sK, b->inv, b->sInv, b->Bact, b->d_info,
-                                     b->panel, (b->n + 1) & ~1, st));
+        CVXB_TRY(potrf_lower_batched(b->n, b->K.p, (int)b->ldk, b->sK, b->inv.p, b->sInv, b->Bact, b->d_info.p,
+                                     b->panel.p, (b->n + 1) & ~1, st));
     }
     return 0;
 }
@@ -393,11 +380,11 @@ int batch_solve(cvxb_batch *b) {
     const int n = b->n, m = b->m, B = b->Bact;
     GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sw = m; gt.sx = m; gt.sy = n;
     // x := x + G' (di .* bzp)
-    CVXB_TRY(gemv_t(m, n, b->G, b->ldg, b->p.di, b->p.bzp, 1.0, 1.0, b->p.dx, st, gt));
-    CVXB_TRY(potrs_lower(n, b->K, (int)b->ldk, b->inv, b->p.dx, b->cw, st, B, b->sK, b->sInv, n));
+    CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, b->p.di, b->p.bzp, 1.0, 1.0, b->p.dx, st, gt));
+    CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, b->p.dx, b->cw, st, B, b->sK, b->sInv, n));
     // bzp := di .* (G x) - bzp
     GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sw = m; gn.sx = n; gn.sy = m;
-    CVXB_TRY(gemv_n(m, n, b->G, b->ldg, b->p.di, b->p.dx, 1.0, -1.0, b->p.bzp, b->gemv_ws, st, gn));
+    CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, b->p.di, b->p.dx, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
     return 0;
 }
 
@@ -409,69 +396,54 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
     *out = nullptr;
     CVXB_TRY(check_device(device));
-    cvxb_batch *b = new cvxb_batch();
+    std::unique_ptr<cvxb_batch> b(new cvxb_batch());
     b->device = device; b->B = nprob; b->n = n; b->m = m;
-    if (const char *e = getenv("CVXB_OZAKI")) b->i8_mode = (e[0] == '0') ? 0 : (e[0] == '2') ? 2 : 1;
+    b->i8_mode = ozaki_mode();
     b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
     b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;
     b->nblk = (n + NB - 1) / NB;
     b->sInv = (long long)2 * b->nblk * NB * NB;
-    auto fail = [&](int r) { cvxb_batch_destroy(b); return r; };
     const size_t B = nprob;
-    CVXB_CUDA_RETRY(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
-    CVXB_CUDA_RETRY(cudaEventCreate(&b->e0)); CVXB_CUDA_RETRY(cudaEventCreate(&b->e1));
-    { int r = chol_work_create(b->cw); if (r) return fail(r); }
-    CVXB_CUDA_RETRY(cudaMalloc(&b->P, B * b->sP * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->G, B * b->sG * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->K, B * b->sK * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->inv, B * b->sInv * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->panel, B * (size_t)((n + 1) & ~1) * NB * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->gemv_ws, B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n) * sizeof(double)));
+    CVXB_CUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
+    CVXB_CUDA(cudaEventCreate(&b->e0)); CVXB_CUDA(cudaEventCreate(&b->e1));
+    CVXB_TRY(chol_work_create(b->cw));
+    CVXB_TRY(b->P.alloc(B * b->sP));
+    CVXB_TRY(b->G.alloc(B * b->sG));
+    CVXB_TRY(b->K.alloc(B * b->sK));
+    CVXB_TRY(b->inv.alloc(B * b->sInv));
+    CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
+    CVXB_TRY(b->gemv_ws.alloc(B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n)));
     // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
     const size_t nv = 4, mv = 13;
     const size_t me = (size_t)(m > 0 ? m : 1);
-    CVXB_CUDA_RETRY(cudaMalloc(&b->vecs, B * (nv * n + mv * me) * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMemset(b->vecs, 0, B * (nv * n + mv * me) * sizeof(double)));
-    double *v = b->vecs;
+    CVXB_TRY(b->vecs.alloc(B * (nv * n + mv * me)));
+    CVXB_CUDA(cudaMemset(b->vecs.p, 0, B * (nv * n + mv * me) * sizeof(double)));
+    double *v = b->vecs.p;
     auto take = [&](size_t len) { double *r = v; v += B * len; return r; };
     b->q = take(n); b->p.x = take(n); b->p.rx = take(n); b->p.dx = take(n);
     b->h = take(me); b->p.s = take(me); b->p.z = take(me); b->p.rz = take(me); b->p.ds = take(me);
     b->p.dz = take(me); b->p.lmbda = take(me); b->p.lmbdasq = take(me); b->p.d = take(me);
     b->p.di = take(me); b->p.di2 = take(me); b->p.ws3 = take(me); b->p.bzp = take(me);
     b->p.q = b->q; b->p.h = b->h; b->p.n = n; b->p.m = m;
-    CVXB_CUDA_RETRY(cudaMalloc(&b->sc, B * sizeof(Scal)));
-    CVXB_CUDA_RETRY(cudaMemset(b->sc, 0, B * sizeof(Scal)));
-    b->p.sc = b->sc;
-    CVXB_CUDA_RETRY(cudaMalloc(&b->d_info, B * sizeof(int)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->d_ndone, sizeof(int)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->d_done, B * sizeof(int)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->d_pairs, 2 * B * sizeof(int)));
-    CVXB_CUDA_RETRY(cudaMalloc(&b->d_perm, B * sizeof(int)));
+    CVXB_TRY(b->sc.alloc(B));
+    CVXB_CUDA(cudaMemset(b->sc.p, 0, B * sizeof(Scal)));
+    b->p.sc = b->sc.p;
+    CVXB_TRY(b->d_info.alloc(B));
+    CVXB_TRY(b->d_ndone.alloc(1));
+    CVXB_TRY(b->d_done.alloc(B));
+    CVXB_TRY(b->d_pairs.alloc(2 * B));
+    CVXB_TRY(b->d_perm.alloc(B));
     b->perm.resize(B);
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
-    *out = b;
+    *out = b.release();
     return 0;
 }
 
 void cvxb_batch_destroy(cvxb_batch *b) {
     if (!b) return;
     cudaSetDevice(b->device);
-    if (b->st) cudaStreamSynchronize(b->st);
-    double *bufs[] = {b->P, b->G, b->K, b->inv, b->panel, b->gemv_ws, b->vecs};
-    for (double *x : bufs) if (x) cudaFree(x);
-    if (b->sc) cudaFree(b->sc);
-    if (b->oz_work) cudaFree(b->oz_work);
-    if (b->d_info) cudaFree(b->d_info);
-    if (b->d_ndone) cudaFree(b->d_ndone);
-    if (b->d_done) cudaFree(b->d_done);
-    if (b->d_pairs) cudaFree(b->d_pairs);
-    if (b->d_perm) cudaFree(b->d_perm);
-    chol_work_destroy(b->cw);
-    if (b->e0) cudaEventDestroy(b->e0);
-    if (b->e1) cudaEventDestroy(b->e1);
-    if (b->st) cudaStreamDestroy(b->st);
     delete b;
 }
 
@@ -483,16 +455,16 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t B = b->B, n = b->n, m = b->m;
     // one strided 2-D copy per operand: rows of the "matrix of columns" are the matrix columns
-    CVXB_CUDA(cudaMemcpy2DAsync(b->P, b->ldp * sizeof(double), P, n * sizeof(double), n * sizeof(double),
+    CVXB_CUDA(cudaMemcpy2DAsync(b->P.p, b->ldp * sizeof(double), P, n * sizeof(double), n * sizeof(double),
                                 n * B, kind, b->st));
     if (m > 0) {
-        CVXB_CUDA(cudaMemcpy2DAsync(b->G, b->ldg * sizeof(double), G, m * sizeof(double),
+        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double),
                                     m * sizeof(double), n * B, kind, b->st));
         CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
     }
     CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
     // only tril(P) is significant in the reference; make the resident copies symmetric
-    CVXB_TRY(symmetrize_lower(b->n, b->P, b->ldp, b->B, b->sP, b->st));
+    CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->loaded = true;
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
@@ -504,11 +476,11 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
 static int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     const int np = (int)pairs.size() / 2;
     if (np == 0) return 0;
-    CVXB_CUDA(cudaMemcpyAsync(b->d_pairs, pairs.data(), pairs.size() * sizeof(int), cudaMemcpyHostToDevice, b->st));
+    CVXB_CUDA(cudaMemcpyAsync(b->d_pairs.p, pairs.data(), pairs.size() * sizeof(int), cudaMemcpyHostToDevice, b->st));
     SwapArgs a;
-    a.P = b->P; a.G = b->G; a.vecs = b->vecs; a.sc = b->sc; a.sP = b->sP; a.sG = b->sG;
+    a.P = b->P.p; a.G = b->G.p; a.vecs = b->vecs.p; a.sc = b->sc.p; a.sP = b->sP; a.sG = b->sG;
     a.n = b->n; a.me = b->m > 0 ? b->m : 1; a.Btot = b->B;
-    k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs);
+    k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs.p);
     count_launch();
     // `pairs` is pageable host memory: the copy above is staged before cudaMemcpyAsync returns
     return 0;
@@ -543,7 +515,7 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
     GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
     GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
-    CVXB_CUDA(cudaMemsetAsync(b->sc, 0, (size_t)B * sizeof(Scal), st));
+    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I ----
     k_init_rhs<<<B, T, 0, st>>>(p); count_launch();
@@ -556,7 +528,7 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     {
         // a singular first factorisation is the reference's "Rank([P; G]) < n" ValueError
         std::vector<int> info(B);
-        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaStreamSynchronize(st));
         for (int i = 0; i < B; ++i) if (info[i] > 0) { info_fail = i + 1; break; }
         if (info_fail) {
@@ -569,17 +541,17 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     for (it = 0; it <= maxiters; ++it) {
         // residuals (:2169-2186)
         k_res_begin<<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(gemv_t(n, n, b->P, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
         k_res_dots<<<B, T, 0, st>>>(p); count_launch();
         if (m > 0) {
-            CVXB_TRY(gemv_t(m, n, b->G, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
-            CVXB_TRY(gemv_n(m, n, b->G, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws, st, gGn));
+            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
+            CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
         }
-        CVXB_CUDA(cudaMemsetAsync(b->d_ndone, 0, sizeof(int), st));
-        k_stats<<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone, b->d_done); count_launch();
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_stats<<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p); count_launch();
         int ndone = 0;
-        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaStreamSynchronize(st));
         if (ndone >= B) break;
         if (ndone > 0 && b->compact && b->B > 1) {
@@ -607,7 +579,7 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
             CVXB_TRY(batch_solve(b));
             k_dir_post<<<B, T, 0, st>>>(p, i); count_launch();
         }
-        k_update<<<B, T, 0, st>>>(p, b->d_info, it); count_launch();
+        k_update<<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -627,12 +599,12 @@ int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *stat
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     const size_t B = b->B;
     // slot -> problem (identity unless the solve compacted finished problems away)
-    if (b->permuted) CVXB_CUDA(cudaMemcpy(b->d_perm, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice));
+    if (b->permuted) CVXB_CUDA(cudaMemcpy(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice));
     auto give = [&](double *dst, const double *src, int len) -> int {
         if (!b->permuted) { CVXB_CUDA(cudaMemcpy(dst, src, B * len * sizeof(double), kind)); return 0; }
         double *tmp = (space == CVXB_DEVICE) ? dst : nullptr;
         if (!tmp) CVXB_CUDA(tmp_malloc(&tmp, B * len * sizeof(double)));
-        k_unpermute_rows<<<(unsigned)B, 256, 0, b->st>>>(src, tmp, b->d_perm, len);
+        k_unpermute_rows<<<(unsigned)B, 256, 0, b->st>>>(src, tmp, b->d_perm.p, len);
         count_launch();
         cudaError_t e = cudaStreamSynchronize(b->st);
         if (e == cudaSuccess && tmp != dst) e = cudaMemcpy(dst, tmp, B * len * sizeof(double), kind);
@@ -646,7 +618,7 @@ int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *stat
     if (status || iters || pobj || dobj) {
         if (space == CVXB_DEVICE) { set_error("batch_results: scalars are returned to host memory only"); return CVXB_E_ARG; }
         std::vector<Scal> sc(B);
-        CVXB_CUDA(cudaMemcpy(sc.data(), b->sc, B * sizeof(Scal), cudaMemcpyDeviceToHost));
+        CVXB_CUDA(cudaMemcpy(sc.data(), b->sc.p, B * sizeof(Scal), cudaMemcpyDeviceToHost));
         for (size_t slot = 0; slot < B; ++slot) {
             const size_t i = (size_t)b->perm[slot];
             if (status) status[i] = sc[slot].status;

@@ -5,6 +5,7 @@
 // of every entry point that takes no handle.
 #include "cone.cuh"
 #include <map>
+#include <memory>
 #include <mutex>
 
 using namespace cvxb;
@@ -13,11 +14,13 @@ namespace {
 // check_device has passed and the stream and CholWork exist once ok is set
 struct DevCtx {
     cudaStream_t st = nullptr;
-    CholWork cw;
+    std::unique_ptr<CholWork> cw;
     bool ok = false;
     std::mutex mu;
 };
-std::map<int, DevCtx> g_ctx;     // std::map nodes are address-stable; the map itself is guarded by g_ctx_mu
+// Contexts are created on first use and never destroyed: CUDA calls are not safe during static destruction.
+// The map itself is guarded by g_ctx_mu.
+std::map<int, DevCtx *> g_ctx;
 std::mutex g_ctx_mu;
 }  // namespace
 
@@ -25,19 +28,22 @@ int cvxb::CallCtx::acquire(int device) {
     DevCtx *c;
     {
         std::lock_guard<std::mutex> g(g_ctx_mu);
-        c = &g_ctx[device];
+        DevCtx *&slot = g_ctx[device];
+        if (!slot) slot = new DevCtx;
+        c = slot;
     }
     lock = std::unique_lock<std::mutex>(c->mu);
     if (c->ok) {
         CVXB_CUDA(cudaSetDevice(device));
     } else {
         CVXB_TRY(check_device(device));
-        CVXB_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
-        CVXB_TRY(chol_work_create(c->cw));
+        if (!c->st) CVXB_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
+        c->cw.reset(new CholWork());      // frees what an earlier attempt that failed part-way created
+        CVXB_TRY(chol_work_create(*c->cw));
         c->ok = true;
     }
     st = c->st;
-    cw = &c->cw;
+    cw = c->cw.get();
     return 0;
 }
 
@@ -52,7 +58,7 @@ int cvxb_syrk_scaled(int n, int k, const double *A, int lda, const double *rowsc
     g.Y = A; g.ldy = lda; g.y_kmajor = true;
     g.w = rowscale;
     g.D = H; g.ldd = ldh; g.beta = 1.0;
-    g.C = C; g.ldc = ldc; g.lower_only = true; g.splitk_ws = ctx.cw->splitk_ws;
+    g.C = C; g.ldc = ldc; g.lower_only = true; g.splitk_ws = ctx.cw->splitk_ws.p;
     CVXB_TRY(dmma_gemm(g, ctx.st));
     CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     return 0;
@@ -79,7 +85,7 @@ int cvxb_potrf(int n, double *A, int lda, double *work_inv, int device) {
     CallCtx ctx; CVXB_TRY(ctx.acquire(device));
     CVXB_TRY(potrf_lower(n, A, lda, work_inv, *ctx.cw, ctx.st));
     int info = 0;
-    CVXB_CUDA(cudaMemcpyAsync(&info, ctx.cw->d_info, sizeof(int), cudaMemcpyDeviceToHost, ctx.st));
+    CVXB_CUDA(cudaMemcpyAsync(&info, ctx.cw->d_info.p, sizeof(int), cudaMemcpyDeviceToHost, ctx.st));
     CVXB_CUDA(cudaStreamSynchronize(ctx.st));
     if (info > 0) set_error("potrf: leading minor of order %d is not positive definite", info);
     return info;

@@ -565,12 +565,11 @@ int chol_work_create(CholWork &w) {
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_start, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_p, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_u, cudaEventDisableTiming));
-    CVXB_CUDA(cudaMalloc(&w.d_info, sizeof(int)));
-    CVXB_CUDA(cudaMemset(w.d_info, 0, sizeof(int)));
-    w.flags_cap = 4096;
-    CVXB_CUDA(cudaMalloc(&w.d_flags, 4096 * sizeof(int)));
-    CVXB_CUDA(cudaMemset(w.d_flags, 0, 4096 * sizeof(int)));
-    CVXB_CUDA(cudaMalloc(&w.splitk_ws, dmma_gemm_splitk_ws_doubles() * sizeof(double)));
+    CVXB_TRY(w.d_info.alloc(1));
+    CVXB_CUDA(cudaMemset(w.d_info.p, 0, sizeof(int)));
+    CVXB_TRY(w.d_flags.alloc(4096));
+    CVXB_CUDA(cudaMemset(w.d_flags.p, 0, 4096 * sizeof(int)));
+    CVXB_TRY(w.splitk_ws.alloc(dmma_gemm_splitk_ws_doubles()));
     CVXB_CUDA(cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    POTF2_SMEM));
     CVXB_CUDA(cudaFuncSetAttribute(trsv_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TRSV_SMEM));
@@ -580,24 +579,12 @@ int chol_work_create(CholWork &w) {
     return 0;
 }
 
-void chol_work_destroy(CholWork &w) {
-    if (w.panel_stream) cudaStreamDestroy(w.panel_stream);
-    if (w.update_stream) cudaStreamDestroy(w.update_stream);
-    if (w.trsm_stream) cudaStreamDestroy(w.trsm_stream);
-    for (auto &g : w.graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    w.graphs.clear();
-    if (w.ev_end_t) cudaEventDestroy(w.ev_end_t);
-    for (auto *v : {&w.ev_dg, &w.ev_tr, &w.ev_c0, &w.ev_r})
+CholWork::~CholWork() {
+    for (cudaStream_t s : {panel_stream, update_stream, trsm_stream}) if (s) cudaStreamDestroy(s);
+    for (auto &g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+    for (cudaEvent_t e : {ev_end_t, ev_start, ev_end_p, ev_end_u}) if (e) cudaEventDestroy(e);
+    for (auto *v : {&ev_dg, &ev_tr, &ev_c0, &ev_r})
         for (cudaEvent_t e : *v) cudaEventDestroy(e);
-    if (w.ev_start) cudaEventDestroy(w.ev_start);
-    if (w.ev_end_p) cudaEventDestroy(w.ev_end_p);
-    if (w.ev_end_u) cudaEventDestroy(w.ev_end_u);
-    if (w.d_info) cudaFree(w.d_info);
-    if (w.d_flags) cudaFree(w.d_flags);
-    if (w.splitk_ws) cudaFree(w.splitk_ws);
-    if (w.panel[0]) cudaFree(w.panel[0]);
-    if (w.panel[1]) cudaFree(w.panel[1]);
-    w = CholWork();
 }
 
 // Look-ahead schedule (three streams, per-step events):
@@ -616,14 +603,11 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         // captured graphs bake in the panel addresses and their leading dimension: drop them
         for (auto &g : w.graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
         w.graphs.clear();
-        for (int i = 0; i < 2; ++i) {
-            if (w.panel[i]) CVXB_CUDA(cudaFree(w.panel[i]));
-            w.panel[i] = nullptr;
-        }
+        for (DevBuf<double> &pb : w.panel) pb.reset();
         // two panel buffers (rows x NB): the TRSM result of step jb goes to panel[jb & 1], so it can be
         // written while the bulk update of step jb-1 still reads the other one
         const int rows = (n + 1) & ~1;
-        for (int i = 0; i < 2; ++i) CVXB_CUDA(cudaMalloc(&w.panel[i], (size_t)rows * NB * sizeof(double)));
+        for (DevBuf<double> &pb : w.panel) CVXB_TRY(pb.alloc((size_t)rows * NB));
         w.panel_rows = rows;
     }
     while ((int)w.ev_dg.size() < nblk) {
@@ -631,14 +615,13 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         for (int i = 0; i < 4; ++i) CVXB_CUDA(cudaEventCreateWithFlags(&e[i], cudaEventDisableTiming));
         w.ev_dg.push_back(e[0]); w.ev_tr.push_back(e[1]); w.ev_c0.push_back(e[2]); w.ev_r.push_back(e[3]);
     }
-    if (getenv("CVXB_TRACE") && !w.trace) {
-        CVXB_CUDA(cudaMalloc(&w.trace, 8 * 4096 * sizeof(unsigned long long)));
-    }
-    if (w.trace) CVXB_CUDA(cudaMemsetAsync(w.trace, 0, 8 * 4096 * sizeof(unsigned long long), st));
+    if (getenv("CVXB_TRACE") && !w.trace.p) CVXB_TRY(w.trace.alloc(8 * 4096));
+    unsigned long long *trace = w.trace.p;
+    if (trace) CVXB_CUDA(cudaMemsetAsync(trace, 0, 8 * 4096 * sizeof(unsigned long long), st));
     const int ldw = w.panel_rows;
     const int panel_tiles = NB / dmma_gemm_tile_cols();      // c tiles that make up one block column
     cudaStream_t D = w.panel_stream, T = w.trsm_stream, U = w.update_stream;
-    CVXB_CUDA(cudaMemsetAsync(w.d_info, 0, sizeof(int), st));
+    CVXB_CUDA(cudaMemsetAsync(w.d_info.p, 0, sizeof(int), st));
     CVXB_CUDA(cudaEventRecord(w.ev_start, st));
     CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_start, 0));
     CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_start, 0));
@@ -652,7 +635,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         double *Ajj = A + j + (long long)j * lda;
         double *invj = inv + (long long)jb * NB * NB;
         double *invTj = inv + (long long)(nblk + jb) * NB * NB;
-        double *Wp = w.panel[jb & 1];
+        double *Wp = w.panel[jb & 1].p;
         // ---- D: diagonal block.  Needs A(jb,jb) updated through panel jb-2 and the raw tile A(jb,jb-1)
         // (block column jb-1 complete through panel jb-2): C0(jb-2) and the last bulk update that touched
         // block column jb.
@@ -665,8 +648,8 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         }
         const double *Tprev = jb > 0 ? A + j + (long long)(j - NB) * lda : nullptr;
         const double *invprev = jb > 0 ? inv + (long long)(jb - 1) * NB * NB : nullptr;
-        potf2_inv_kernel<<<1, 256, POTF2_SMEM, D>>>(Ajj, lda, wj, invj, invTj, w.d_info, j, 0, 0, Tprev,
-                                                     lda, invprev, w.trace ? w.trace + 8 * jb : nullptr);
+        potf2_inv_kernel<<<1, 256, POTF2_SMEM, D>>>(Ajj, lda, wj, invj, invTj, w.d_info.p, j, 0, 0, Tprev,
+                                                     lda, invprev, trace ? trace + 8 * jb : nullptr);
         count_launch();
         CVXB_LAUNCH_CHECK();
         CVXB_CUDA(cudaEventRecord(w.ev_dg[jb], D));
@@ -676,7 +659,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             if (jb == 0) return 0;
             const int jp = j - NB, mp = n - j;
             CVXB_CUDA(cudaMemcpy2DAsync(A + j + (long long)jp * lda, (size_t)lda * sizeof(double),
-                                        w.panel[(jb - 1) & 1], (size_t)ldw * sizeof(double),
+                                        w.panel[(jb - 1) & 1].p, (size_t)ldw * sizeof(double),
                                         (size_t)mp * sizeof(double), NB, cudaMemcpyDeviceToDevice, T));
             return 0;
         };
@@ -697,7 +680,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             g.X = A21; g.ldx = lda; g.x_kmajor = false;
             g.Y = invj; g.ldy = NB; g.y_kmajor = false;
             g.C = Wp; g.ldc = ldw;
-            g.trace = w.trace ? w.trace + 8 * jb + 2 : nullptr;
+            g.trace = trace ? trace + 8 * jb + 2 : nullptr;
             CVXB_TRY(dmma_gemm(g, T));
         }
         CVXB_CUDA(cudaEventRecord(w.ev_tr[jb], T));
@@ -713,7 +696,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             c.ldy = ldw; c.y_kmajor = false;
             c.D = A22 + wn; c.ldd = lda; c.C = A22 + wn; c.ldc = lda;
             c.alpha = -1.0; c.beta = 1.0;
-            c.trace = w.trace ? w.trace + 8 * jb + 4 : nullptr;
+            c.trace = trace ? trace + 8 * jb + 4 : nullptr;
             CVXB_TRY(dmma_gemm(c, T));
         }
         CVXB_CUDA(cudaEventRecord(w.ev_c0[jb], T));
@@ -728,7 +711,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             u.D = A22; u.ldd = lda; u.C = A22; u.ldc = lda;
             u.alpha = -1.0; u.beta = 1.0; u.lower_only = true;
             u.ct_begin = panel_tiles; u.ct_end = 1 << 30;
-            u.trace = w.trace ? w.trace + 8 * jb + 6 : nullptr;
+            u.trace = trace ? trace + 8 * jb + 6 : nullptr;
             CVXB_TRY(dmma_gemm(u, U));
             CVXB_CUDA(cudaEventRecord(w.ev_r[jb], U));
             prev_r = last_r;
@@ -810,17 +793,17 @@ int trsv_lower(int n, const double *L, int ldl, const double *inv, double *b, bo
                CholWork &w, cudaStream_t st, int batch, long long sL, long long sInv, long long sb) {
     if (n <= 0 || batch <= 0) return 0;
     const int nblk = (n + NB - 1) / NB;
-    if ((long long)nblk * batch > w.flags_cap) {
-        if (w.d_flags) CVXB_CUDA(cudaFree(w.d_flags));
-        w.flags_cap = (long long)nblk * batch;
-        CVXB_CUDA(cudaMalloc(&w.d_flags, (size_t)w.flags_cap * sizeof(int)));
-        CVXB_CUDA(cudaMemset(w.d_flags, 0, (size_t)w.flags_cap * sizeof(int)));
+    const size_t nflags = (size_t)nblk * batch;
+    if (nflags > w.d_flags.n) {
+        w.d_flags.reset();
+        CVXB_TRY(w.d_flags.alloc(nflags));
+        CVXB_CUDA(cudaMemset(w.d_flags.p, 0, nflags * sizeof(int)));
     }
     const int epoch = g_trsv_epoch.fetch_add(1) + 1;
     const double *invT = inv + (long long)nblk * NB * NB;
     const bool vec = ((uintptr_t)L % 16 == 0) && (ldl % 2 == 0) && (batch == 1 || sL % 2 == 0);
     dim3 grid(nblk, batch);
-#define TRSV_LAUNCH(T, V) trsv_kernel<T, V><<<grid, 256, TRSV_SMEM, st>>>(n, L, ldl, inv, invT, b, w.d_flags, epoch, sL, sInv, sb)
+#define TRSV_LAUNCH(T, V) trsv_kernel<T, V><<<grid, 256, TRSV_SMEM, st>>>(n, L, ldl, inv, invT, b, w.d_flags.p, epoch, sL, sInv, sb)
     if (trans) { if (vec) TRSV_LAUNCH(true, true); else TRSV_LAUNCH(true, false); }
     else       { if (vec) TRSV_LAUNCH(false, true); else TRSV_LAUNCH(false, false); }
 #undef TRSV_LAUNCH

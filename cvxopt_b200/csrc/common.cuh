@@ -104,18 +104,51 @@ struct Staged {
     }
 };
 
-// For cvxb_kkt_create / cvxb_batch_create: an allocation that fails for lack of memory is tried once more after
-// the scratch-buffer cache is given back to the driver.  Any failure returns fail(code), a lambda of the caller
-// that releases what was built so far.
-#define CVXB_CUDA_RETRY(expr)                                                                       \
-    do {                                                                                            \
-        cudaError_t _e = (expr);                                                                    \
-        if (_e == cudaErrorMemoryAllocation) { cudaGetLastError(); cvxb::tmp_cache_release(); _e = (expr); } \
-        if (_e != cudaSuccess) {                                                                    \
-            cvxb::set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(_e));  \
-            return fail(_e == cudaErrorMemoryAllocation ? CVXB_E_NOMEM : CVXB_E_CUDA);              \
-        }                                                                                           \
-    } while (0)
+// ---- long-lived device memory ---------------------------------------------------
+// Bytes currently held by DevBufs, all devices together (cvxb_device_bytes).
+extern std::atomic<unsigned long long> g_device_bytes;
+
+// n elements of cudaMalloc memory owned by the handle (or workspace) it is a member of, freed with it.
+template <class T> struct DevBuf {
+    T *p = nullptr;
+    size_t n = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    DevBuf(DevBuf &&o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+    DevBuf &operator=(DevBuf &&o) noexcept {
+        if (this != &o) { reset(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+        return *this;
+    }
+    ~DevBuf() { reset(); }
+    // Frees what it held, then allocates count elements.  An allocation that fails for lack of memory is tried
+    // once more after the scratch-buffer cache is given back to the driver.  Leaves no CUDA error pending and no
+    // error text: for callers that have a fallback.
+    cudaError_t try_alloc(size_t count) {
+        reset();
+        const size_t bytes = count * sizeof(T);
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaErrorMemoryAllocation) { cudaGetLastError(); tmp_cache_release(); e = cudaMalloc(&p, bytes); }
+        if (e != cudaSuccess) { cudaGetLastError(); p = nullptr; return e; }
+        n = count;
+        g_device_bytes.fetch_add(bytes, std::memory_order_relaxed);
+        return cudaSuccess;
+    }
+    // try_alloc; a failure returns CVXB_E_NOMEM (out of memory) or CVXB_E_CUDA with the error text set
+    int alloc(size_t count) {
+        const cudaError_t e = try_alloc(count);
+        if (e == cudaSuccess) return 0;
+        set_error("cudaMalloc(%zu bytes) -> %s", count * sizeof(T), cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? CVXB_E_NOMEM : CVXB_E_CUDA;
+    }
+    void reset() {
+        if (!p) return;
+        cudaFree(p);
+        g_device_bytes.fetch_sub(n * sizeof(T), std::memory_order_relaxed);
+        p = nullptr;
+        n = 0;
+    }
+};
 
 // CVXB_JACOBI_COOP (default on, =0 for one launch per round) allows a cooperative launch, and `ctas` CTAs of
 // `threads` threads of `kernel` can be resident on the current device at once
@@ -208,6 +241,12 @@ int dmma_gemm_tile_cols();              // width of a c tile (units of ct_begin 
 
 // ozaki_syrk.cu (opt-in): C(lower) = A' diag(d)^2 A + beta*D through int8 slices on wgmma
 size_t ozaki_workspace_bytes(int n, int m, int S);
+// CVXB_OZAKI (read when a handle is created): 0 or unset never, 1 for large problems, 2 always
+int ozaki_mode();
+// whether the SYRK of an m x n operand runs on the int8 slices (nine of them) under `mode`: 2 always, 1 when
+// n >= 4096 and m >= 8192.  Keeps the slice workspace in `work`; when it does not fit, the answer is no (the
+// DMMA kernel, which needs none, computes the same result), with no CUDA error pending and no error text.
+bool ozaki_use(int mode, int n, int m, DevBuf<char> &work);
 void ozaki_time_mma(cudaEvent_t a, cudaEvent_t b);   // events recorded around the MMA launches of this thread's next call
 int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, const double *D,
                long long ldd, double beta, double *C, long long ldc, int S, int layout, void *work,
@@ -222,7 +261,7 @@ struct CholWork {
     cudaStream_t update_stream = nullptr;  // low-priority: bulk trailing update
     cudaEvent_t ev_end_t = nullptr;
     std::vector<cudaEvent_t> ev_dg, ev_tr, ev_c0, ev_r;   // one per block step
-    unsigned long long *trace = nullptr;  // CVXB_TRACE=1: per step {Dg, Tr, C0, R} x {start, end}
+    DevBuf<unsigned long long> trace;      // CVXB_TRACE=1: per step {Dg, Tr, C0, R} x {start, end}
     struct GraphEntry {                    // captured factorisation, keyed by its arguments
         int n = 0, lda = 0, launches = 0;
         const void *A = nullptr, *inv = nullptr;
@@ -231,15 +270,14 @@ struct CholWork {
     std::vector<GraphEntry> graphs;
     bool graph_failed = false;
     cudaEvent_t ev_start = nullptr, ev_end_p = nullptr, ev_end_u = nullptr;
-    int *d_info = nullptr;                // device flag
-    int *d_flags = nullptr;               // trsv progress flags (batch * ceil(n/NB) ints)
-    long long flags_cap = 0;
-    double *splitk_ws = nullptr;
-    double *panel[2] = {nullptr, nullptr};   // out-of-place TRSM results (double-buffered)
+    DevBuf<int> d_info;                    // device flag
+    DevBuf<int> d_flags;                   // trsv progress flags (batch * ceil(n/NB) ints)
+    DevBuf<double> splitk_ws;
+    DevBuf<double> panel[2];               // out-of-place TRSM results (double-buffered)
     int panel_rows = 0;
+    ~CholWork();                           // also right after a chol_work_create that failed part-way
 };
 int chol_work_create(CholWork &w);
-void chol_work_destroy(CholWork &w);
 int potrf_lower(int n, double *A, int lda, double *inv, CholWork &w, cudaStream_t st);
 // b := L^{-T} L^{-1} b  (potrs with one right-hand side)
 // batched variants: problem p uses L + p*sL, inv + p*sInv, b + p*sb

@@ -8,18 +8,16 @@
 #include "cone.cuh"
 #include <cstdlib>
 #include <cstdarg>
-#include <mutex>
-
 #include <map>
 #include <unordered_map>
 #include <mutex>
 #include <iterator>
-#include <cstdlib>
 
 namespace cvxb {
 
 static thread_local std::string g_err;
 std::atomic<unsigned long long> g_launches{0};
+std::atomic<unsigned long long> g_device_bytes{0};
 
 
 // ---- scratch-buffer cache (common.cuh) ----
@@ -175,15 +173,15 @@ int kkt_pack_bz(cvxb_kkt *k, const double *zd) {
     const ConeLayout &c = k->cone;
     cudaStream_t st = k->st;
     const int nlq = c.mnl + c.ml + c.sumq;
-    if (c.mnl > 0) CVXB_TRY(scale_rows(zd, c.cdim, k->bzp, c.cdim, c.mnl, 1, k->W.dnli, st));
+    double *bzp = k->bzp.p;
+    if (c.mnl > 0) CVXB_TRY(scale_rows(zd, c.cdim, bzp, c.cdim, c.mnl, 1, k->W.dnli, st));
     if (c.ml > 0)
-        CVXB_TRY(scale_rows(zd + c.mnl, c.cdim, k->bzp + c.mnl, c.cdim, c.ml, 1, k->W.di, st));
+        CVXB_TRY(scale_rows(zd + c.mnl, c.cdim, bzp + c.mnl, c.cdim, c.ml, 1, k->W.di, st));
     if (c.nq > 0)
-        CVXB_TRY(scale_q(c, k->W, zd + c.mnl + c.ml, c.cdim, k->bzp + c.mnl + c.ml, c.cdim, 1, true, st));
+        CVXB_TRY(scale_q(c, k->W, zd + c.mnl + c.ml, c.cdim, bzp + c.mnl + c.ml, c.cdim, 1, true, st));
     if (c.ns > 0) {
-        CVXB_TRY(scale_s(c, k->W, zd + nlq, c.cdim, k->zt + nlq, c.cdim, 1, 'T', 'I', k->swork,
-                         k->swork_doubles, st));
-        CVXB_TRY(pack_s(c, k->zt + nlq, c.cdim, k->bzp + nlq, c.cdim, 1, true, st));
+        CVXB_TRY(scale_s(c, k->W, zd + nlq, c.cdim, k->zt.p + nlq, c.cdim, 1, 'T', 'I', k->swork.p, k->swork.n, st));
+        CVXB_TRY(pack_s(c, k->zt.p + nlq, c.cdim, bzp + nlq, c.cdim, 1, true, st));
     }
     return 0;
 }
@@ -194,8 +192,60 @@ int kkt_unpack_z(cvxb_kkt *k, double *zd) {
     cudaStream_t st = k->st;
     const int nlq = c.mnl + c.ml + c.sumq;
     if (nlq > 0)
-        CVXB_CUDA(cudaMemcpyAsync(zd, k->bzp, (size_t)nlq * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (c.ns > 0) CVXB_TRY(unpack_s(c, k->bzp + nlq, c.cdim, zd + nlq, c.cdim, 1, st));
+        CVXB_CUDA(cudaMemcpyAsync(zd, k->bzp.p, (size_t)nlq * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (c.ns > 0) CVXB_TRY(unpack_s(c, k->bzp.p + nlq, c.cdim, zd + nlq, c.cdim, 1, st));
+    return 0;
+}
+
+// 'q' and 's' rows of Gs = pack(W^{-T} G)                       (misc.py:1267-1272, :1614-1616)
+int kkt_scale_pack_G(cvxb_kkt *k, double *dst, long long ldd) {
+    const ConeLayout &c = k->cone;
+    const double *Gq = k->G + c.mnl + c.ml;
+    if (c.nq > 0) CVXB_TRY(scale_q(c, k->W, Gq, k->ldg, dst, ldd, k->n, true, k->st));
+    if (c.ns > 0) {
+        // W^{-T} on an 's' block: rti' * mat(x) * rti  (trans 'T', inverse 'I'), then pack2
+        CVXB_TRY(scale_s(c, k->W, Gq + c.sumq, k->ldg, k->Gunp.p, c.sums2, k->n, 'T', 'I', k->swork.p, k->swork.n,
+                         k->st));
+        CVXB_TRY(pack_s(c, k->Gunp.p, c.sums2, dst + c.sumq, ldd, k->n, false, k->st));
+    }
+    return 0;
+}
+
+// solve of the Cholesky and LDL' routes, in place on device vectors; on entry bzp = pack(W^{-T} bz)
+static int chol_solve(cvxb_kkt *k, double *xd, double *ydv) {
+    const ConeLayout &c = k->cone;
+    const int n = k->n;
+    cudaStream_t st = k->st;
+    const long long ldk = kkt_ldk(k);
+    const double *K = k->Kmat.p, *inv = k->inv.p, *Gs = k->Gs.p;
+    double *bzp = k->bzp.p, *ws = k->gemv_ws.p;
+    // x := x + Gs' bzp                                            (misc.py:1311)
+    if (c.ml > 0) CVXB_TRY(gemv_t(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, bzp + c.mnl, 1.0, 1.0, xd, st));
+    if (c.mnl > 0) CVXB_TRY(gemv_t(c.mnl, n, Gs, k->ldgs, nullptr, bzp, 1.0, 1.0, xd, st));
+    if (k->nrest - c.mnl > 0)
+        CVXB_TRY(gemv_t(k->nrest - c.mnl, n, Gs + c.mnl, k->ldgs, nullptr, bzp + c.mnl + c.ml, 1.0, 1.0, xd, st));
+    if (k->method == 2 && k->p > 0) {
+        // [x; y] := (L D L')^{-1} [x; y]                          (lapack.sytrs, misc.py:1196)
+        CVXB_TRY(kkt_ldl_solve(k, xd, ydv));
+    } else if (k->p == 0) {
+        // x := K^{-1} x                                           (misc.py:1327)
+        CVXB_TRY(potrs_lower(n, K, (int)ldk, inv, xd, k->cw, st));
+    } else {
+        // kkt_chol2-style elimination of the equality constraints  (misc.py:1526-1558)
+        const int p = k->p;
+        if (k->singular)      // x += A' by
+            CVXB_TRY(gemv_t(p, n, k->Aeq.p, k->lda_eq, nullptr, ydv, 1.0, 1.0, xd, st));
+        CVXB_TRY(trsv_lower(n, K, (int)ldk, inv, xd, false, k->cw, st));                   // x := L^{-1} x
+        CVXB_TRY(gemv_t(n, p, k->Asct.p, k->ldas, nullptr, xd, 1.0, -1.0, ydv, st));       // y := Asct' x - y
+        CVXB_TRY(potrs_lower(p, k->Kp.p, (int)k->ldkp, k->invp.p, ydv, k->cw, st));        // y := Kp^{-1} y
+        CVXB_TRY(gemv_n(n, p, k->Asct.p, k->ldas, nullptr, ydv, -1.0, 1.0, xd, ws, st));   // x -= Asct y
+        CVXB_TRY(trsv_lower(n, K, (int)ldk, inv, xd, true, k->cw, st));                    // x := L^{-T} x
+    }
+    // bzp := Gs x - bzp                                           (misc.py:1344)
+    if (c.ml > 0) CVXB_TRY(gemv_n(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, xd, 1.0, -1.0, bzp + c.mnl, ws, st));
+    if (c.mnl > 0) CVXB_TRY(gemv_n(c.mnl, n, Gs, k->ldgs, nullptr, xd, 1.0, -1.0, bzp, ws, st));
+    if (k->nrest - c.mnl > 0)
+        CVXB_TRY(gemv_n(k->nrest - c.mnl, n, Gs + c.mnl, k->ldgs, nullptr, xd, 1.0, -1.0, bzp + c.mnl + c.ml, ws, st));
     return 0;
 }
 
@@ -231,11 +281,18 @@ int trsm_lower_left(int n, const double *L, long long ldl, const double *inv, do
 
 }  // namespace cvxb
 
+cvxb_kkt::~cvxb_kkt() {
+    if (st) cudaStreamSynchronize(st);
+    for (cudaEvent_t e : {e0, e1, e2, e3, t0, t1, m0, m1}) if (e) cudaEventDestroy(e);
+    if (st) cudaStreamDestroy(st);
+}
+
 extern "C" {
 
 const char *cvxb_last_error(void) { return g_err.c_str(); }
 int cvxb_version(void) { return 100; }
 unsigned long long cvxb_launch_count(void) { return g_launches.load(); }
+unsigned long long cvxb_device_bytes(void) { return g_device_bytes.load(); }
 
 int cvxb_device_count(void) {
     int cnt = 0;
@@ -272,101 +329,80 @@ int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const d
     if (p > 0 && (!A || lda < p)) { set_error("kkt_create: A must be p x n with lda >= p"); return CVXB_E_ARG; }
     if (p > n) { set_error("kkt_create: Rank(A) < p (p > n)"); return CVXB_E_ARG; }
     CVXB_TRY(check_device(device));
-    cvxb_kkt *k = new cvxb_kkt();
+    std::unique_ptr<cvxb_kkt> k(new cvxb_kkt());
     k->device = device; k->n = n; k->p = p;
-    if (const char *e = getenv("CVXB_OZAKI")) k->i8_mode = (e[0] == '0') ? 0 : (e[0] == '2') ? 2 : 1;
-    int rc = k->cone.init(dims);
-    if (rc) { delete k; return rc; }
+    k->i8_mode = ozaki_mode();
+    CVXB_TRY(k->cone.init(dims));
     const ConeLayout &c = k->cone;
     if (c.cdim > 0 && (!G || ldg < (c.cdim > 1 ? c.cdim : 1))) {
         set_error("kkt_create: G must be cdim x n with ldg >= cdim (cdim=%d, ldg=%d)", c.cdim, ldg);
-        cvxb_kkt_destroy(k);
         return CVXB_E_ARG;
     }
-    auto fail = [&](int r) { cvxb_kkt_destroy(k); return r; };
-#define KTRY(expr) do { int _r = (expr); if (_r) return fail(_r); } while (0)
-    CVXB_CUDA_RETRY(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
-    CVXB_CUDA_RETRY(cudaEventCreate(&k->e0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->e1));
-    CVXB_CUDA_RETRY(cudaEventCreate(&k->e2)); CVXB_CUDA_RETRY(cudaEventCreate(&k->e3));
-    CVXB_CUDA_RETRY(cudaEventCreate(&k->t0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->t1));
-    CVXB_CUDA_RETRY(cudaEventCreate(&k->m0)); CVXB_CUDA_RETRY(cudaEventCreate(&k->m1));
-    KTRY(chol_work_create(k->cw));
+    CVXB_CUDA(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
+    for (cudaEvent_t *e : {&k->e0, &k->e1, &k->e2, &k->e3, &k->t0, &k->t1, &k->m0, &k->m1})
+        CVXB_CUDA(cudaEventCreate(e));
+    CVXB_TRY(chol_work_create(k->cw));
     const size_t nn = (size_t)(n > 0 ? n : 1);
     if (space == CVXB_DEVICE) {
-        k->G = G; k->ldg = ldg; k->own_G = false;
+        k->G = G; k->ldg = ldg;
     } else {
-        double *g = nullptr;
         k->ldg = (c.cdim + 1) & ~1;     // even leading dimension: 16-byte aligned columns
         if (k->ldg < 2) k->ldg = 2;
-        CVXB_CUDA_RETRY(cudaMalloc(&g, (size_t)k->ldg * nn * sizeof(double)));
-        k->G = g; k->own_G = true;
-        KTRY(upload_matrix(g, k->ldg, G, ldg, c.cdim, n, CVXB_HOST, k->st));
+        CVXB_TRY(k->Gown.alloc((size_t)k->ldg * nn));
+        k->G = k->Gown.p;
+        CVXB_TRY(upload_matrix(k->Gown.p, k->ldg, G, ldg, c.cdim, n, CVXB_HOST, k->st));
     }
-    const long long ldk = (n + 1) & ~1;
-    CVXB_CUDA_RETRY(cudaMalloc(&k->Kmat, (size_t)(ldk > 2 ? ldk : 2) * nn * sizeof(double)));
+    CVXB_TRY(k->Kmat.alloc((size_t)kkt_ldk(k.get()) * nn));
     const int nblk = (n + NB - 1) / NB + 1;
-    CVXB_CUDA_RETRY(cudaMalloc(&k->inv, (size_t)2 * nblk * NB * NB * sizeof(double)));   // inv + inv' blocks
+    CVXB_TRY(k->inv.alloc((size_t)2 * nblk * NB * NB));   // inv + inv' blocks
     k->nrest = c.mnl + c.sumq + c.sump;
     if (k->nrest > 0) {
         k->ldgs = (k->nrest + 1) & ~1;
-        CVXB_CUDA_RETRY(cudaMalloc(&k->Gs, (size_t)k->ldgs * nn * sizeof(double)));
+        CVXB_TRY(k->Gs.alloc((size_t)k->ldgs * nn));
     }
     if (c.sums2 > 0) {
-        CVXB_CUDA_RETRY(cudaMalloc(&k->Gunp, (size_t)c.sums2 * nn * sizeof(double)));
+        CVXB_TRY(k->Gunp.alloc((size_t)c.sums2 * nn));
         // workspace for the congruences: symmetric copies + intermediate, chunked over columns
         size_t per_col = (size_t)2 * c.maxs * c.maxs;
         size_t cols = (size_t)n < 1 ? 1 : (size_t)n;
         size_t want = per_col * cols;
         const size_t cap = (size_t)1 << 29;            // 4 GiB of doubles at most
         if (want > cap) want = (cap / per_col ? cap / per_col : 1) * per_col;
-        k->swork_doubles = want;
-        CVXB_CUDA_RETRY(cudaMalloc(&k->swork, want * sizeof(double)));
+        CVXB_TRY(k->swork.alloc(want));
     }
-    if (c.mnl > 0) CVXB_CUDA_RETRY(cudaMalloc(&k->Dfbuf, (size_t)c.mnl * nn * sizeof(double)));
+    if (c.mnl > 0) CVXB_TRY(k->Dfbuf.alloc((size_t)c.mnl * nn));
     if (p > 0) {
         k->lda_eq = (p + 1) & ~1;
         k->ldas = (n + 1) & ~1;
         k->ldkp = (p + 1) & ~1;
-        CVXB_CUDA_RETRY(cudaMalloc(&k->Aeq, (size_t)k->lda_eq * nn * sizeof(double)));
-        CVXB_CUDA_RETRY(cudaMalloc(&k->Asct, (size_t)k->ldas * p * sizeof(double)));
-        CVXB_CUDA_RETRY(cudaMalloc(&k->Kp, (size_t)k->ldkp * p * sizeof(double)));
-        CVXB_CUDA_RETRY(cudaMalloc(&k->invp, (size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB * sizeof(double)));
-        CVXB_CUDA_RETRY(cudaMalloc(&k->yd, (size_t)p * sizeof(double)));
-        KTRY(upload_matrix(k->Aeq, k->lda_eq, A, lda, p, n, space, k->st));
+        CVXB_TRY(k->Aeq.alloc((size_t)k->lda_eq * nn));
+        CVXB_TRY(k->Asct.alloc((size_t)k->ldas * p));
+        CVXB_TRY(k->Kp.alloc((size_t)k->ldkp * p));
+        CVXB_TRY(k->invp.alloc((size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB));
+        CVXB_TRY(k->yd.alloc((size_t)p));
+        CVXB_TRY(upload_matrix(k->Aeq.p, k->lda_eq, A, lda, p, n, space, k->st));
     }
-    KTRY(k->W.alloc(c));
+    CVXB_TRY(k->W.alloc(c));
     const size_t cd = (size_t)(c.cdim > 0 ? c.cdim : 1);
-    CVXB_CUDA_RETRY(cudaMalloc(&k->bzp, cd * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&k->zin, cd * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&k->zt, cd * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&k->xv, nn * sizeof(double)));
-    CVXB_CUDA_RETRY(cudaMalloc(&k->yv, (cd > nn ? cd : nn) * sizeof(double)));
+    CVXB_TRY(k->bzp.alloc(cd));
+    CVXB_TRY(k->zin.alloc(cd));
+    CVXB_TRY(k->zt.alloc(cd));
+    CVXB_TRY(k->xv.alloc(nn));
+    CVXB_TRY(k->yv.alloc(cd > nn ? cd : nn));
     {
         size_t w1 = cd * (size_t)gemv_n_chunks(n), w2 = nn * (size_t)gemv_n_chunks(p > 0 ? p : 1);
         const size_t w3 = (size_t)(p > 0 ? p : 1) * (size_t)gemv_n_chunks(n);      // A operator
         if (w3 > w1) w1 = w3;
-        CVXB_CUDA_RETRY(cudaMalloc(&k->gemv_ws, (w1 > w2 ? w1 : w2) * sizeof(double)));
+        CVXB_TRY(k->gemv_ws.alloc(w1 > w2 ? w1 : w2));
     }
-    CVXB_CUDA_RETRY(cudaStreamSynchronize(k->st));
-#undef KTRY
-    *out = k;
+    CVXB_CUDA(cudaStreamSynchronize(k->st));
+    *out = k.release();
     return 0;
 }
 
 void cvxb_kkt_destroy(cvxb_kkt *k) {
     if (!k) return;
     cudaSetDevice(k->device);
-    if (k->st) cudaStreamSynchronize(k->st);
-    if (k->own_G && k->G) cudaFree(const_cast<double *>(k->G));
-    double *bufs[] = {k->Aeq, k->Asct, k->Kp, k->invp, k->yd, k->Hres, k->Hbuf, k->Kmat, k->inv, k->Gs, k->Gunp, k->Dfbuf, k->bzp,
-                      k->zin, k->zt, k->xv, k->yv, k->gemv_ws, k->swork};
-    for (double *b : bufs) if (b) cudaFree(b);
-    if (k->oz_work) cudaFree(k->oz_work);
-    if (k->ext && k->ext_destroy) k->ext_destroy(k->ext);
-    chol_work_destroy(k->cw);
-    cudaEvent_t evs[] = {k->e0, k->e1, k->e2, k->e3, k->t0, k->t1, k->m0, k->m1};
-    for (cudaEvent_t e : evs) if (e) cudaEventDestroy(e);
-    if (k->st) cudaStreamDestroy(k->st);
     delete k;
 }
 
@@ -396,17 +432,16 @@ int cvxb_kkt_set_H(cvxb_kkt *k, const double *H, int ldh, int space) {
     if (!k) { set_error("kkt is NULL"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(k->device));
     if (!H) {
-        if (k->Hres) cudaFree(k->Hres);
-        k->Hres = nullptr;
+        k->Hres.reset();
         return 0;
     }
     if (ldh < (k->n > 1 ? k->n : 1)) { set_error("set_H: ldh < n"); return CVXB_E_ARG; }
     const long long ldk = kkt_ldk(k);
-    if (!k->Hres) CVXB_CUDA(cudaMalloc(&k->Hres, (size_t)ldk * (k->n > 0 ? k->n : 1) * sizeof(double)));
-    CVXB_TRY(upload_matrix(k->Hres, ldk, H, ldh, k->n, k->n, space, k->st));
+    if (!k->Hres.p) CVXB_TRY(k->Hres.alloc((size_t)ldk * (k->n > 0 ? k->n : 1)));
+    CVXB_TRY(upload_matrix(k->Hres.p, ldk, H, ldh, k->n, k->n, space, k->st));
     // only tril(H) is significant in the reference (misc.py:1276-1277); make the resident
     // copy fully symmetric so it also serves the P(x, y) operator
-    CVXB_TRY(symmetrize_lower(k->n, k->Hres, ldk, 1, 0, k->st));
+    CVXB_TRY(symmetrize_lower(k->n, k->Hres.p, ldk, 1, 0, k->st));
     CVXB_CUDA(cudaStreamSynchronize(k->st));
     return 0;
 }
@@ -436,113 +471,73 @@ int cvxb_kkt_factor(cvxb_kkt *k, const cvxb_scaling *Wp, const double *H, int ld
         if (ldh < (n > 1 ? n : 1)) { set_error("factor: ldh < n"); return CVXB_E_ARG; }
         if (space == CVXB_DEVICE) { Hptr = H; ldH = ldh; }
         else {
-            if (!k->Hbuf) CVXB_CUDA(cudaMalloc(&k->Hbuf, (size_t)ldk * (n > 0 ? n : 1) * sizeof(double)));
-            CVXB_TRY(upload_matrix(k->Hbuf, ldk, H, ldh, n, n, CVXB_HOST, st));
-            Hptr = k->Hbuf;
+            if (!k->Hbuf.p) CVXB_TRY(k->Hbuf.alloc((size_t)ldk * (n > 0 ? n : 1)));
+            CVXB_TRY(upload_matrix(k->Hbuf.p, ldk, H, ldh, n, n, CVXB_HOST, st));
+            Hptr = k->Hbuf.p;
         }
-    } else if (use_resident_H && k->Hres) {
-        Hptr = k->Hres;
+    } else if (use_resident_H && k->Hres.p) {
+        Hptr = k->Hres.p;
     }
+    double *K = k->Kmat.p;
     // ---- Gs rows that cannot be folded into the SYRK operand load: [Df | q | s] ----
     if (c.mnl > 0) {
         if (!Df) { set_error("factor: Df is required when mnl > 0"); return CVXB_E_ARG; }
         const double *Dfd = Df; long long ldd = lddf;
         if (space != CVXB_DEVICE) {
-            CVXB_TRY(upload_matrix(k->Dfbuf, c.mnl, Df, lddf, c.mnl, n, CVXB_HOST, st));
-            Dfd = k->Dfbuf; ldd = c.mnl;
+            CVXB_TRY(upload_matrix(k->Dfbuf.p, c.mnl, Df, lddf, c.mnl, n, CVXB_HOST, st));
+            Dfd = k->Dfbuf.p; ldd = c.mnl;
         }
-        CVXB_TRY(scale_rows(Dfd, ldd, k->Gs, k->ldgs, c.mnl, n, k->W.dnli, st));
+        CVXB_TRY(scale_rows(Dfd, ldd, k->Gs.p, k->ldgs, c.mnl, n, k->W.dnli, st));
     }
-    if (c.nq > 0)
-        CVXB_TRY(scale_q(c, k->W, k->G + c.mnl + c.ml, k->ldg, k->Gs + c.mnl, k->ldgs, n, true, st));
-    if (c.ns > 0) {
-        // W^{-T} on an 's' block: rti' * mat(x) * rti  (trans 'T', inverse 'I'), then pack2
-        CVXB_TRY(scale_s(c, k->W, k->G + c.mnl + c.ml + c.sumq, k->ldg, k->Gunp, c.sums2, n, 'T',
-                         'I', k->swork, k->swork_doubles, st));
-        CVXB_TRY(pack_s(c, k->Gunp, c.sums2, k->Gs + c.mnl + c.sumq, k->ldgs, n, false, st));
-    }
+    CVXB_TRY(kkt_scale_pack_G(k, k->Gs.p + c.mnl, k->ldgs));
     CVXB_CUDA(cudaEventRecord(k->e1, st));
     // ---- K = H + G_l' diag(di^2) G_l + Gs' Gs (+ A'A)  (lower triangle), then Cholesky ----
     int info = 0;
     auto assemble_and_factor = [&](bool add_ata) -> int {
-        bool have = false;
-        bool i8 = k->i8_mode == 2 || (k->i8_mode == 1 && n >= 4096 && c.ml >= 8192);
-        if (c.ml > 0 && n > 0 && i8) {
-            // the slice workspace is ~1.125 x sizeof(G_l): when it does not fit, the DMMA kernel (no
-            // workspace) computes the same K
-            const size_t need = ozaki_workspace_bytes(n, c.ml, 9);
-            if (need > k->oz_bytes) {
-                if (k->oz_work) cudaFree(k->oz_work);
-                k->oz_work = nullptr; k->oz_bytes = 0;
-                cudaError_t ae = cudaMalloc(&k->oz_work, need);
-                if (ae == cudaErrorMemoryAllocation) { cudaGetLastError(); tmp_cache_release(); ae = cudaMalloc(&k->oz_work, need); }
-                if (ae != cudaSuccess) {
-                    cudaGetLastError();
-                    k->oz_work = nullptr;
-                    i8 = false;
-                } else {
-                    k->oz_bytes = need;
-                }
-            }
-        }
+        bool have = false;        // K holds a partial sum; until then the first term is added to H
+        // K += X' diag(w) X for the kdim x n matrix X (ld ldx)
+        auto syrk_add = [&](const double *X, long long ldx, int kdim, const double *w) -> int {
+            GemmDesc g;
+            g.M = n; g.N = n; g.K = kdim;
+            g.X = X; g.ldx = (int)ldx; g.x_kmajor = true;
+            g.Y = X; g.ldy = (int)ldx; g.y_kmajor = true;
+            g.w = w;
+            g.D = have ? K : Hptr; g.ldd = have ? (int)ldk : (int)ldH; g.beta = 1.0;
+            g.C = K; g.ldc = (int)ldk;
+            g.lower_only = true; g.splitk_ws = k->cw.splitk_ws.p;
+            CVXB_TRY(dmma_gemm(g, st));
+            have = true;
+            return 0;
+        };
         k->syrk_path = 0;
-        if (c.ml > 0 && n > 0 && i8) {
+        if (c.ml > 0 && n > 0 && ozaki_use(k->i8_mode, n, c.ml, k->oz_work)) {
             // G_l' diag(di)^2 G_l + H from nine int8 slices per entry (exact products, fp64-level result)
             ozaki_time_mma(k->m0, k->m1);
-            CVXB_TRY(ozaki_syrk(n, c.ml, k->G + c.mnl, k->ldg, k->W.di, Hptr, ldH, 1.0, k->Kmat, ldk, 9, 0,
-                                k->oz_work, st));
+            CVXB_TRY(ozaki_syrk(n, c.ml, k->G + c.mnl, k->ldg, k->W.di, Hptr, ldH, 1.0, K, ldk, 9, 0,
+                                k->oz_work.p, st));
             have = true;
             k->syrk_path = 2;
         } else if (c.ml > 0 && n > 0) {
-            GemmDesc g;
-            g.M = n; g.N = n; g.K = c.ml;
-            g.X = k->G + c.mnl; g.ldx = (int)k->ldg; g.x_kmajor = true;
-            g.Y = g.X; g.ldy = g.ldx; g.y_kmajor = true;
-            g.w = k->W.di2;
-            g.D = Hptr; g.ldd = (int)ldH; g.beta = 1.0;
-            g.C = k->Kmat; g.ldc = (int)ldk;
-            g.lower_only = true; g.splitk_ws = k->cw.splitk_ws;
-            CVXB_TRY(dmma_gemm(g, st));
-            have = true;
+            CVXB_TRY(syrk_add(k->G + c.mnl, k->ldg, c.ml, k->W.di2));
             k->syrk_path = 1;
         }
-        if (k->nrest > 0 && n > 0) {
-            GemmDesc g;
-            g.M = n; g.N = n; g.K = k->nrest;
-            g.X = k->Gs; g.ldx = (int)k->ldgs; g.x_kmajor = true;
-            g.Y = g.X; g.ldy = g.ldx; g.y_kmajor = true;
-            g.D = have ? k->Kmat : Hptr; g.ldd = have ? (int)ldk : (int)ldH; g.beta = 1.0;
-            g.C = k->Kmat; g.ldc = (int)ldk;
-            g.lower_only = true; g.splitk_ws = k->cw.splitk_ws;
-            CVXB_TRY(dmma_gemm(g, st));
-            have = true;
-        }
-        if (add_ata && k->p > 0 && n > 0) {
-            GemmDesc g;                                   // S += A'A   (misc.py:1440)
-            g.M = n; g.N = n; g.K = k->p;
-            g.X = k->Aeq; g.ldx = (int)k->lda_eq; g.x_kmajor = true;
-            g.Y = g.X; g.ldy = g.ldx; g.y_kmajor = true;
-            g.D = have ? k->Kmat : Hptr; g.ldd = have ? (int)ldk : (int)ldH; g.beta = 1.0;
-            g.C = k->Kmat; g.ldc = (int)ldk;
-            g.lower_only = true; g.splitk_ws = k->cw.splitk_ws;
-            CVXB_TRY(dmma_gemm(g, st));
-            have = true;
-        }
+        if (k->nrest > 0 && n > 0) CVXB_TRY(syrk_add(k->Gs.p, k->ldgs, k->nrest, nullptr));
+        if (add_ata && k->p > 0 && n > 0) CVXB_TRY(syrk_add(k->Aeq.p, k->lda_eq, k->p, nullptr));   // S += A'A   (misc.py:1440)
         if (!have && n > 0) {
             if (!Hptr) { set_error("factor: no cone rows and no H: KKT matrix is singular"); return 1; }
-            CVXB_TRY(upload_matrix(k->Kmat, ldk, Hptr, ldH, n, n, CVXB_DEVICE, st));
+            CVXB_TRY(upload_matrix(K, ldk, Hptr, ldH, n, n, CVXB_DEVICE, st));
         }
         CVXB_CUDA(cudaEventRecord(k->e2, st));
         if (k->method == 2 && k->p > 0) {
             // kkt_ldl2: Kmat now holds S = H + GG' W^-1 W^-T GG (lower); the 2x2 system [S A'; A 0] is factored
             // with Bunch-Kaufman pivoting (lapack.sytrf, misc.py:1172).  p == 0 is a plain Cholesky there too (:1173).
             CVXB_TRY(kkt_ldl_factor(k));
-            CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info, sizeof(int), cudaMemcpyDeviceToHost, st));
+            CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToHost, st));
             CVXB_CUDA(cudaStreamSynchronize(st));
             return 0;
         }
-        CVXB_TRY(potrf_lower(n, k->Kmat, (int)ldk, k->inv, k->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_TRY(potrf_lower(n, K, (int)ldk, k->inv.p, k->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaStreamSynchronize(st));
         return 0;
     };
@@ -558,18 +553,18 @@ int cvxb_kkt_factor(cvxb_kkt *k, const cvxb_scaling *Wp, const double *H, int ld
         // Asct := L^{-1} A'  (blocked forward substitution with the diagonal-block inverses),
         // Kp := Asct' Asct,  Kp = Lp Lp'                               (misc.py:1464-1472)
         const int p = k->p;
-        CVXB_TRY(transpose_copy(k->Aeq, k->lda_eq, k->Asct, k->ldas, p, n, st));
-        CVXB_TRY(trsm_lower_left(n, k->Kmat, ldk, k->inv, k->Asct, k->ldas, p, st));
+        CVXB_TRY(transpose_copy(k->Aeq.p, k->lda_eq, k->Asct.p, k->ldas, p, n, st));
+        CVXB_TRY(trsm_lower_left(n, K, ldk, k->inv.p, k->Asct.p, k->ldas, p, st));
         {
             GemmDesc g;
             g.M = p; g.N = p; g.K = n;
-            g.X = k->Asct; g.ldx = (int)k->ldas; g.x_kmajor = true;
-            g.Y = k->Asct; g.ldy = (int)k->ldas; g.y_kmajor = true;
-            g.C = k->Kp; g.ldc = (int)k->ldkp; g.lower_only = true;
+            g.X = k->Asct.p; g.ldx = (int)k->ldas; g.x_kmajor = true;
+            g.Y = k->Asct.p; g.ldy = (int)k->ldas; g.y_kmajor = true;
+            g.C = k->Kp.p; g.ldc = (int)k->ldkp; g.lower_only = true;
             CVXB_TRY(dmma_gemm(g, st));
         }
-        CVXB_TRY(potrf_lower(p, k->Kp, (int)k->ldkp, k->invp, k->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_TRY(potrf_lower(p, k->Kp.p, (int)k->ldkp, k->invp.p, k->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaStreamSynchronize(st));
     }
     CVXB_CUDA(cudaEventRecord(k->e3, st));
@@ -595,60 +590,25 @@ int cvxb_kkt_solve(cvxb_kkt *k, double *x, double *y, double *z, int space) {
     if (!k) { set_error("kkt is NULL"); return CVXB_E_ARG; }
     if (!k->factored) { set_error("solve called before a successful factor"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(k->device));
-    if (k->method == 1) return kkt_qr_solve(k, x, y, z, space);
     const ConeLayout &c = k->cone;
-    const int n = k->n;
+    const int n = k->n, p = k->p;
     cudaStream_t st = k->st;
-    const long long ldk = kkt_ldk(k);
-    const int nlq = c.mnl + c.ml + c.sumq;     // rows that are identical packed / unpacked
     CVXB_CUDA(cudaEventRecord(k->e0, st));
     double *xd = x, *zd = z, *ydv = y;
-    if (k->p > 0 && !y) { set_error("solve: y is required when p > 0"); return CVXB_E_ARG; }
+    if (p > 0 && !y) { set_error("solve: y is required when p > 0"); return CVXB_E_ARG; }
     if (space != CVXB_DEVICE) {
-        CVXB_TRY(xfer_vec(k->xv, x, n, CVXB_HOST, true, st));
-        CVXB_TRY(xfer_vec(k->zin, z, c.cdim, CVXB_HOST, true, st));
-        xd = k->xv; zd = k->zin;
-        if (k->p > 0) { CVXB_TRY(xfer_vec(k->yd, y, k->p, CVXB_HOST, true, st)); ydv = k->yd; }
+        CVXB_TRY(xfer_vec(k->xv.p, x, n, CVXB_HOST, true, st));
+        CVXB_TRY(xfer_vec(k->zin.p, z, c.cdim, CVXB_HOST, true, st));
+        xd = k->xv.p; zd = k->zin.p;
+        if (p > 0) { CVXB_TRY(xfer_vec(k->yd.p, y, p, CVXB_HOST, true, st)); ydv = k->yd.p; }
     }
     CVXB_TRY(kkt_pack_bz(k, zd));
-    // x := x + Gs' bzp                                            (misc.py:1311)
-    if (c.ml > 0)
-        CVXB_TRY(gemv_t(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, k->bzp + c.mnl, 1.0, 1.0, xd, st));
-    if (c.mnl > 0) CVXB_TRY(gemv_t(c.mnl, n, k->Gs, k->ldgs, nullptr, k->bzp, 1.0, 1.0, xd, st));
-    if (k->nrest - c.mnl > 0)
-        CVXB_TRY(gemv_t(k->nrest - c.mnl, n, k->Gs + c.mnl, k->ldgs, nullptr,
-                        k->bzp + c.mnl + c.ml, 1.0, 1.0, xd, st));
-    if (k->method == 2 && k->p > 0) {
-        // [x; y] := (L D L')^{-1} [x; y]                          (lapack.sytrs, misc.py:1196)
-        CVXB_TRY(kkt_ldl_solve(k, xd, ydv));
-    } else if (k->p == 0) {
-        // x := K^{-1} x                                           (misc.py:1327)
-        CVXB_TRY(potrs_lower(n, k->Kmat, (int)ldk, k->inv, xd, k->cw, st));
-    } else {
-        // kkt_chol2-style elimination of the equality constraints  (misc.py:1526-1558)
-        const int p = k->p;
-        if (k->singular)      // x += A' by
-            CVXB_TRY(gemv_t(p, n, k->Aeq, k->lda_eq, nullptr, ydv, 1.0, 1.0, xd, st));
-        CVXB_TRY(trsv_lower(n, k->Kmat, (int)ldk, k->inv, xd, false, k->cw, st));          // x := L^{-1} x
-        CVXB_TRY(gemv_t(n, p, k->Asct, k->ldas, nullptr, xd, 1.0, -1.0, ydv, st));         // y := Asct' x - y
-        CVXB_TRY(potrs_lower(p, k->Kp, (int)k->ldkp, k->invp, ydv, k->cw, st));            // y := Kp^{-1} y
-        CVXB_TRY(gemv_n(n, p, k->Asct, k->ldas, nullptr, ydv, -1.0, 1.0, xd, k->gemv_ws, st));   // x -= Asct y
-        CVXB_TRY(trsv_lower(n, k->Kmat, (int)ldk, k->inv, xd, true, k->cw, st));           // x := L^{-T} x
-    }
-    // bzp := Gs x - bzp                                           (misc.py:1344)
-    if (c.ml > 0)
-        CVXB_TRY(gemv_n(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, xd, 1.0, -1.0, k->bzp + c.mnl,
-                        k->gemv_ws, st));
-    if (c.mnl > 0)
-        CVXB_TRY(gemv_n(c.mnl, n, k->Gs, k->ldgs, nullptr, xd, 1.0, -1.0, k->bzp, k->gemv_ws, st));
-    if (k->nrest - c.mnl > 0)
-        CVXB_TRY(gemv_n(k->nrest - c.mnl, n, k->Gs + c.mnl, k->ldgs, nullptr, xd, 1.0, -1.0,
-                        k->bzp + c.mnl + c.ml, k->gemv_ws, st));
+    CVXB_TRY(k->method == 1 ? kkt_qr_solve(k, xd, ydv) : chol_solve(k, xd, ydv));
     CVXB_TRY(kkt_unpack_z(k, zd));
     if (space != CVXB_DEVICE) {
-        CVXB_TRY(xfer_vec(x, k->xv, n, CVXB_HOST, false, st));
-        CVXB_TRY(xfer_vec(z, k->zin, c.cdim, CVXB_HOST, false, st));
-        if (k->p > 0) CVXB_TRY(xfer_vec(y, k->yd, k->p, CVXB_HOST, false, st));
+        CVXB_TRY(xfer_vec(x, k->xv.p, n, CVXB_HOST, false, st));
+        CVXB_TRY(xfer_vec(z, k->zin.p, c.cdim, CVXB_HOST, false, st));
+        if (p > 0) CVXB_TRY(xfer_vec(y, k->yd.p, p, CVXB_HOST, false, st));
     }
     CVXB_CUDA(cudaEventRecord(k->e1, st));
     CVXB_CUDA(cudaStreamSynchronize(st));
@@ -661,7 +621,7 @@ int cvxb_kkt_solve(cvxb_kkt *k, double *x, double *y, double *z, int space) {
 int cvxb_kkt_get_L(cvxb_kkt *k, double *L_host, int ldl) {
     if (!k || !L_host || ldl < k->n) { set_error("get_L: bad arguments"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(k->device));
-    CVXB_CUDA(cudaMemcpy2D(L_host, (size_t)ldl * sizeof(double), k->Kmat, kkt_ldk(k) * sizeof(double),
+    CVXB_CUDA(cudaMemcpy2D(L_host, (size_t)ldl * sizeof(double), k->Kmat.p, kkt_ldk(k) * sizeof(double),
                            (size_t)k->n * sizeof(double), k->n, cudaMemcpyDeviceToHost));
     return 0;
 }
@@ -691,12 +651,12 @@ int cvxb_kkt_timer_stop(cvxb_kkt *k, double *ms) {
 }
 /* debug: copy the CVXB_TRACE timeline of the last potrf (8 values per block step) */
 int cvxb_kkt_trace(cvxb_kkt *k, unsigned long long *out, int nsteps) {
-    if (!k || !out || !k->cw.trace) return CVXB_E_ARG;
-    CVXB_CUDA(cudaMemcpy(out, k->cw.trace, (size_t)nsteps * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (!k || !out || !k->cw.trace.p) return CVXB_E_ARG;
+    CVXB_CUDA(cudaMemcpy(out, k->cw.trace.p, (size_t)nsteps * 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return 0;
 }
 int cvxb_kkt_syrk_path(cvxb_kkt *k) { return k ? k->syrk_path : CVXB_E_ARG; }
-int cvxb_kkt_qr_passes(cvxb_kkt *k) { return (k && k->method == 1) ? kkt_qr_passes(k) : CVXB_E_ARG; }
+int cvxb_kkt_qr_passes(cvxb_kkt *k) { return (k && k->method == 1) ? k->qr->npass : CVXB_E_ARG; }
 int cvxb_kkt_last_breakdown(cvxb_kkt *k, double *ms3) {
     if (!k || !ms3) return CVXB_E_ARG;
     ms3[0] = k->br[1]; ms3[1] = k->br[2]; ms3[2] = k->br[0];
@@ -722,13 +682,13 @@ int cvxb_kkt_gemv_G(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
     const double *xd = x; double *yd = y;
     if (space != CVXB_DEVICE) {
         // zin/yv are cdim long, xv is n long: pick by role
-        double *xb = tr ? k->zin : k->xv, *yb = tr ? k->xv : k->yv;
+        double *xb = tr ? k->zin.p : k->xv.p, *yb = tr ? k->xv.p : k->yv.p;
         CVXB_TRY(xfer_vec(xb, x, nx, CVXB_HOST, true, st));
         if (beta != 0.0) CVXB_TRY(xfer_vec(yb, y, ny, CVXB_HOST, true, st));
         xd = xb; yd = yb;
     }
     if (tr) CVXB_TRY(gemv_t(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, st));
-    else    CVXB_TRY(gemv_n(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, k->gemv_ws, st));
+    else    CVXB_TRY(gemv_n(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, k->gemv_ws.p, st));
     if (space != CVXB_DEVICE) CVXB_TRY(xfer_vec(y, yd, ny, CVXB_HOST, false, st));
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;
@@ -746,14 +706,14 @@ int cvxb_kkt_gemv_A(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
     const double *xd = x; double *yd = y;
     if (space != CVXB_DEVICE) {
         // xv (n) / yd (p) by role; yv is max(cdim, n) long and serves as the second n- or p-vector
-        double *xb = tr ? k->yd : k->xv, *yb = k->yv;
+        double *xb = tr ? k->yd.p : k->xv.p, *yb = k->yv.p;
         if (!tr && p > n) { set_error("gemv_A: p > n"); return CVXB_E_ARG; }
         CVXB_TRY(xfer_vec(xb, x, nx, CVXB_HOST, true, st));
         if (beta != 0.0) CVXB_TRY(xfer_vec(yb, y, ny, CVXB_HOST, true, st));
         xd = xb; yd = yb;
     }
-    if (tr) CVXB_TRY(gemv_t(p, n, k->Aeq, k->lda_eq, nullptr, xd, alpha, beta, yd, st));
-    else    CVXB_TRY(gemv_n(p, n, k->Aeq, k->lda_eq, nullptr, xd, alpha, beta, yd, k->gemv_ws, st));
+    if (tr) CVXB_TRY(gemv_t(p, n, k->Aeq.p, k->lda_eq, nullptr, xd, alpha, beta, yd, st));
+    else    CVXB_TRY(gemv_n(p, n, k->Aeq.p, k->lda_eq, nullptr, xd, alpha, beta, yd, k->gemv_ws.p, st));
     if (space != CVXB_DEVICE) CVXB_TRY(xfer_vec(y, yd, ny, CVXB_HOST, false, st));
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;
@@ -761,17 +721,17 @@ int cvxb_kkt_gemv_A(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
 
 int cvxb_kkt_symv_H(cvxb_kkt *k, const double *x, double *y, double alpha, double beta, int space) {
     if (!k || !x || !y) { set_error("symv_H: bad arguments"); return CVXB_E_ARG; }
-    if (!k->Hres) { set_error("symv_H: no resident H (call cvxb_kkt_set_H)"); return CVXB_E_ARG; }
+    if (!k->Hres.p) { set_error("symv_H: no resident H (call cvxb_kkt_set_H)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(k->device));
     const int n = k->n;
     cudaStream_t st = k->st;
     const double *xd = x; double *yd = y;
     if (space != CVXB_DEVICE) {
-        CVXB_TRY(xfer_vec(k->xv, x, n, CVXB_HOST, true, st));
-        if (beta != 0.0) CVXB_TRY(xfer_vec(k->yv, y, n, CVXB_HOST, true, st));
-        xd = k->xv; yd = k->yv;
+        CVXB_TRY(xfer_vec(k->xv.p, x, n, CVXB_HOST, true, st));
+        if (beta != 0.0) CVXB_TRY(xfer_vec(k->yv.p, y, n, CVXB_HOST, true, st));
+        xd = k->xv.p; yd = k->yv.p;
     }
-    CVXB_TRY(gemv_t(n, n, k->Hres, kkt_ldk(k), nullptr, xd, alpha, beta, yd, st));
+    CVXB_TRY(gemv_t(n, n, k->Hres.p, kkt_ldk(k), nullptr, xd, alpha, beta, yd, st));
     if (space != CVXB_DEVICE) CVXB_TRY(xfer_vec(y, yd, n, CVXB_HOST, false, st));
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;

@@ -2,43 +2,76 @@
 // kkt_qr.cu (misc.kkt_qr) and kkt_ldl.cu (misc.kkt_ldl2).
 #pragma once
 #include "cone.cuh"
+#include <memory>
 
 using cvxb::ConeLayout;
 using cvxb::DevScaling;
 using cvxb::CholWork;
+using cvxb::DevBuf;
+
+namespace cvxb {
+// state of the QR route (kkt_qr.cu)
+struct QrState {
+    int nq = 0;                 // n - p: columns of Gs2
+    DevBuf<double> Q;           // n x n orthogonal factor of A' (p > 0)
+    long long ldQ = 0;
+    DevBuf<double> R1;          // p x p upper triangular (ld p)
+    DevBuf<double> tau;
+    DevBuf<double> GsF;         // cdim_pckd x n: Gs, then Gs [Q1 Q2] (p > 0: second buffer)
+    DevBuf<double> GsQ;
+    long long ldf = 0;
+    DevBuf<double> Q3t;         // nq x cdim_pckd: Q3'
+    long long ldq = 0;
+    DevBuf<double> C[3], inv[3];
+    long long ldc = 0;
+    int npass = 2;
+    DevBuf<double> w, u, vv, xt, ws, norm2;
+};
+
+// state of the LDL' route (kkt_ldl.cu)
+struct LdlState {
+    int N = 0;
+    DevBuf<double> K2;          // N x N
+    long long ld = 0;
+    DevBuf<int> ipiv;           // LAPACK convention, 1-based, negative for 2x2 blocks
+    DevBuf<int> state;          // [0] k  [1] kstep  [2] kp  [3] info  [4] pending (step to finish)
+    DevBuf<double> w1, w2;      // multipliers of the current step
+    DevBuf<double> u;           // N right-hand side
+    double kktreg = 0.0;
+};
+}  // namespace cvxb
 
 struct cvxb_kkt {
     int device = 0;
     int n = 0, p = 0;
     ConeLayout cone;
     const double *G = nullptr;   // cdim x n, rows [mnl, cdim) hold G (rows [0,mnl) belong to Df)
+    DevBuf<double> Gown;         // backs G when it came from the host; a device G stays the caller's
     long long ldg = 0;
-    bool own_G = false;
-    double *Hres = nullptr;      // resident H (symmetrised), or null
-    double *Hbuf = nullptr;      // per-call H upload buffer (lazy)
-    double *Kmat = nullptr;      // n x n: normal equations, then its Cholesky factor (lower)
-    double *inv = nullptr;       // inverses of the diagonal blocks of L
-    double *Gs = nullptr;        // scaled+packed rows that are not 'l': [mnl | q | s packed] x n
+    DevBuf<double> Hres;         // resident H (symmetrised), or empty
+    DevBuf<double> Hbuf;         // per-call H upload buffer (lazy)
+    DevBuf<double> Kmat;         // n x n: normal equations, then its Cholesky factor (lower)
+    DevBuf<double> inv;          // inverses of the diagonal blocks of L
+    DevBuf<double> Gs;           // scaled+packed rows that are not 'l': [mnl | q | s packed] x n
     long long ldgs = 0;
     int nrest = 0;
-    double *Gunp = nullptr;      // unpacked scaled 's' rows (sums2 x n) — only when ns > 0
-    double *Dfbuf = nullptr;     // mnl x n upload buffer
+    DevBuf<double> Gunp;         // unpacked scaled 's' rows (sums2 x n) — only when ns > 0
+    DevBuf<double> Dfbuf;        // mnl x n upload buffer
     // equality constraints (p > 0), kkt_chol2-style elimination (reference misc.py:1464-1472):
-    double *Aeq = nullptr;       // p x n (ld lda_eq)
+    DevBuf<double> Aeq;          // p x n (ld lda_eq)
     long long lda_eq = 0;
-    double *Asct = nullptr;      // n x p: L^{-1} A'
+    DevBuf<double> Asct;         // n x p: L^{-1} A'
     long long ldas = 0;
-    double *Kp = nullptr;        // p x p: Asct' Asct, then its Cholesky factor
+    DevBuf<double> Kp;           // p x p: Asct' Asct, then its Cholesky factor
     long long ldkp = 0;
-    double *invp = nullptr;      // diagonal-block inverses of chol(Kp)
-    double *yd = nullptr;        // p
+    DevBuf<double> invp;         // diagonal-block inverses of chol(Kp)
+    DevBuf<double> yd;           // p
     bool singular = false;       // first factorisation failed -> S += A'A from then on (misc.py:1433-1447)
     bool first_factor = true;
     DevScaling W;
-    double *bzp = nullptr, *zin = nullptr, *zt = nullptr, *xv = nullptr, *yv = nullptr;
-    double *gemv_ws = nullptr;
-    double *swork = nullptr;
-    size_t swork_doubles = 0;
+    DevBuf<double> bzp, zin, zt, xv, yv;
+    DevBuf<double> gemv_ws;
+    DevBuf<double> swork;        // congruence workspace of the 's' rows
     CholWork cw;
     cudaStream_t st = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr, e2 = nullptr, e3 = nullptr, t0 = nullptr, t1 = nullptr;
@@ -46,18 +79,17 @@ struct cvxb_kkt {
     double mma_ms = 0.0;
     double factor_ms = 0, solve_ms = 0, br[3] = {0, 0, 0};
     bool factored = false;
-    // SYRK of the 'l' rows on the int8 tensor path (ozaki_syrk.cu): 0 off (DMMA kernel), 1 for large
-    // problems, 2 always.  CVXB_OZAKI=0/1/2 read at create; unset = 0: on H100 the fp64 DMMA kernel is the
-    // faster of the two at every size measured (DESIGN.md).
+    // SYRK of the 'l' rows on the int8 tensor path (ozaki_syrk.cu): ozaki_mode() at create; by default off: on
+    // H100 the fp64 DMMA kernel is the faster of the two at every size measured (DESIGN.md).
     int i8_mode = 0;
-    void *oz_work = nullptr;
-    size_t oz_bytes = 0;
+    DevBuf<char> oz_work;
     int syrk_path = 0;           // kernel of the last factor's 'l'-row SYRK: 0 none, 1 fp64 DMMA, 2 int8 slices
     // factorisation route: 0 Cholesky of the reduced system (kkt_chol / kkt_chol2), 1 QR (kkt_qr), 2 LDL' of the
-    // 2x2 system (kkt_ldl2).  Set once after create (cvxb_kkt_set_method); state of routes 1/2 lives in `ext`.
+    // 2x2 system (kkt_ldl2).  Set once after create (cvxb_kkt_set_method), with the state of that route.
     int method = 0;
-    void *ext = nullptr;
-    void (*ext_destroy)(void *) = nullptr;
+    std::unique_ptr<cvxb::QrState> qr;
+    std::unique_ptr<cvxb::LdlState> ldl;
+    ~cvxb_kkt();                 // synchronises the stream, then releases it and the events; the members free the rest
 };
 
 
@@ -72,13 +104,16 @@ int trsm_lower_left(int n, const double *L, long long ldl, const double *inv, do
                     cudaStream_t st);
 int kkt_pack_bz(cvxb_kkt *k, const double *zd);      // k->bzp := pack(W^{-T} bz)
 int kkt_unpack_z(cvxb_kkt *k, double *zd);           // z := unpack(k->bzp)
-// route-specific factor / solve (kkt_qr.cu, kkt_ldl.cu)
+// the 'q' and 's' rows of pack(W^{-T} G): dst is where the first 'q' row goes (ld ldd), the packed 's' rows follow
+// at dst + sumq
+int kkt_scale_pack_G(cvxb_kkt *k, double *dst, long long ldd);
+// route-specific factor / solve (kkt_qr.cu, kkt_ldl.cu); the solves work in place on device vectors, between
+// cvxb_kkt_solve's kkt_pack_bz and kkt_unpack_z
 int kkt_qr_factor(cvxb_kkt *k, const cvxb_scaling *W, int space);
-int kkt_qr_solve(cvxb_kkt *k, double *x, double *y, double *z, int space);
+int kkt_qr_solve(cvxb_kkt *k, double *xd, double *yd);
 int kkt_qr_setup(cvxb_kkt *k);
-int kkt_qr_passes(const cvxb_kkt *k);
 // LDL' route: Kmat holds S (lower) on entry of factor; info (k->cw.d_info) = first exactly-zero pivot, 1-based
 int kkt_ldl_factor(cvxb_kkt *k);
-int kkt_ldl_solve(cvxb_kkt *k, double *xd, double *yd);        // device vectors, in place
+int kkt_ldl_solve(cvxb_kkt *k, double *xd, double *yd);
 int kkt_ldl_setup(cvxb_kkt *k, double kktreg);
 }  // namespace cvxb

@@ -26,29 +26,7 @@ namespace cvxb {
 
 namespace {
 
-struct LdlState {
-    int N = 0;
-    double *K2 = nullptr;       // N x N
-    long long ld = 0;
-    int *ipiv = nullptr;        // LAPACK convention, 1-based, negative for 2x2 blocks
-    int *state = nullptr;       // [0] k  [1] kstep  [2] kp  [3] info  [4] pending (step to finish)
-    double *w1 = nullptr, *w2 = nullptr;   // multipliers of the current step
-    double *u = nullptr;        // N right-hand side
-    double kktreg = 0.0;
-};
-
-void ldl_destroy(void *p) {
-    LdlState *s = static_cast<LdlState *>(p);
-    if (s->K2) cudaFree(s->K2);
-    if (s->ipiv) cudaFree(s->ipiv);
-    if (s->state) cudaFree(s->state);
-    if (s->w1) cudaFree(s->w1);
-    if (s->w2) cudaFree(s->w2);
-    if (s->u) cudaFree(s->u);
-    delete s;
-}
-
-// K2 = [S 0; A 0] (lower), diagonal regularisation
+// K2 =[S 0; A 0] (lower), diagonal regularisation
 __global__ void ldl_build_kernel(int n, int p, const double *S, long long lds, const double *A, long long lda,
                                  double *K2, long long ld, double reg) {
     const int N = n + p;
@@ -296,64 +274,67 @@ __global__ void __launch_bounds__(1024) ldl_solve_kernel(int N, const double *A,
 }  // namespace
 
 int kkt_ldl_setup(cvxb_kkt *k, double kktreg) {
-    LdlState *s = new LdlState();
-    k->ext = s; k->ext_destroy = ldl_destroy;
+    auto s = std::make_unique<LdlState>();
     s->N = k->n + k->p;
     s->kktreg = kktreg;
     s->ld = (s->N + 1) & ~1;
     if (s->ld < 2) s->ld = 2;
     const size_t NN = (size_t)(s->N > 0 ? s->N : 1);
-    CVXB_CUDA(cudaMalloc(&s->K2, (size_t)s->ld * NN * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&s->ipiv, NN * sizeof(int)));
-    CVXB_CUDA(cudaMalloc(&s->state, 8 * sizeof(int)));
-    CVXB_CUDA(cudaMalloc(&s->w1, NN * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&s->w2, NN * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&s->u, NN * sizeof(double)));
+    CVXB_TRY(s->K2.alloc((size_t)s->ld * NN));
+    CVXB_TRY(s->ipiv.alloc(NN));
+    CVXB_TRY(s->state.alloc(8));
+    CVXB_TRY(s->w1.alloc(NN));
+    CVXB_TRY(s->w2.alloc(NN));
+    CVXB_TRY(s->u.alloc(NN));
+    k->ldl = std::move(s);
     return 0;
 }
 
 int kkt_ldl_factor(cvxb_kkt *k) {
-    LdlState *s = static_cast<LdlState *>(k->ext);
+    const LdlState *s = k->ldl.get();
     const int n = k->n, p = k->p, N = s->N;
     cudaStream_t st = k->st;
     const long long ldk = kkt_ldk(k);
-    ldl_build_kernel<<<(unsigned)(((long long)N * N + 255) / 256), 256, 0, st>>>(n, p, k->Kmat, ldk, k->Aeq, k->lda_eq,
-                                                                               s->K2, s->ld, s->kktreg);
+    double *K2 = s->K2.p, *w1 = s->w1.p, *w2 = s->w2.p;
+    int *ipiv = s->ipiv.p, *state = s->state.p;
+    ldl_build_kernel<<<(unsigned)(((long long)N * N + 255) / 256), 256, 0, st>>>(n, p, k->Kmat.p, ldk, k->Aeq.p,
+                                                                               k->lda_eq, K2, s->ld, s->kktreg);
     count_launch();
-    CVXB_CUDA(cudaMemsetAsync(s->state, 0, 8 * sizeof(int), st));
+    CVXB_CUDA(cudaMemsetAsync(state, 0, 8 * sizeof(int), st));
     for (int it = 0; it < N; ++it) {
         // after `it` completed steps k >= it: the trailing matrix has at most N - it - 1 rows beyond the pivot
         const int rem = N - it - 1;
-        ldl_pivot_kernel<<<1, 512, 0, st>>>(N, s->K2, s->ld, s->ipiv, s->state, s->w1, s->w2);
+        ldl_pivot_kernel<<<1, 512, 0, st>>>(N, K2, s->ld, ipiv, state, w1, w2);
         count_launch();
         if (rem <= 0) continue;
         int sb = (rem + 255) / 256; if (sb > 64) sb = 64;
-        ldl_swap_kernel<<<sb, 256, 0, st>>>(N, s->K2, s->ld, s->state);
-        ldl_mult_kernel<<<(rem + 255) / 256, 256, 0, st>>>(N, s->K2, s->ld, s->state, s->w1, s->w2);
+        ldl_swap_kernel<<<sb, 256, 0, st>>>(N, K2, s->ld, state);
+        ldl_mult_kernel<<<(rem + 255) / 256, 256, 0, st>>>(N, K2, s->ld, state, w1, w2);
         int gx = (rem + 255) / 256; if (gx > 32) gx = 32;
         dim3 grid(gx, (rem + 7) / 8);
-        ldl_update_kernel<<<grid, 256, 0, st>>>(N, s->K2, s->ld, s->state, s->w1, s->w2);
+        ldl_update_kernel<<<grid, 256, 0, st>>>(N, K2, s->ld, state, w1, w2);
         count_launch(3);
     }
-    ldl_pivot_kernel<<<1, 512, 0, st>>>(N, s->K2, s->ld, s->ipiv, s->state, s->w1, s->w2);     // finish the last step
+    ldl_pivot_kernel<<<1, 512, 0, st>>>(N, K2, s->ld, ipiv, state, w1, w2);     // finish the last step
     count_launch();
     CVXB_LAUNCH_CHECK();
     // dsytrf's info > 0: D(info, info) is exactly zero -> the reference raises ArithmeticError
-    CVXB_CUDA(cudaMemcpyAsync(k->cw.d_info, s->state + 3, sizeof(int), cudaMemcpyDeviceToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(k->cw.d_info.p, state + 3, sizeof(int), cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
 int kkt_ldl_solve(cvxb_kkt *k, double *xd, double *yd) {
-    LdlState *s = static_cast<LdlState *>(k->ext);
+    const LdlState *s = k->ldl.get();
     const int n = k->n, p = k->p, N = s->N;
     cudaStream_t st = k->st;
-    CVXB_CUDA(cudaMemcpyAsync(s->u, xd, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    CVXB_CUDA(cudaMemcpyAsync(s->u + n, yd, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    ldl_solve_kernel<<<1, 1024, 0, st>>>(N, s->K2, s->ld, s->ipiv, s->u);
+    double *u = s->u.p;
+    CVXB_CUDA(cudaMemcpyAsync(u, xd, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(u + n, yd, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    ldl_solve_kernel<<<1, 1024, 0, st>>>(N, s->K2.p, s->ld, s->ipiv.p, u);
     count_launch();
     CVXB_LAUNCH_CHECK();
-    CVXB_CUDA(cudaMemcpyAsync(xd, s->u, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    CVXB_CUDA(cudaMemcpyAsync(yd, s->u + n, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(xd, u, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(yd, u + n, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 

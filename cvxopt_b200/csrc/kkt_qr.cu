@@ -22,31 +22,6 @@ namespace cvxb {
 
 namespace {
 
-struct QrState {
-    int nq = 0;                 // n - p: columns of Gs2
-    double *Q = nullptr;        // n x n orthogonal factor of A' (p > 0)
-    long long ldQ = 0;
-    double *R1 = nullptr;       // p x p upper triangular (ld p)
-    double *tau = nullptr;
-    double *GsF = nullptr;      // cdim_pckd x n: Gs, then Gs [Q1 Q2] (p > 0: second buffer)
-    double *GsQ = nullptr;
-    long long ldf = 0;
-    double *Q3t = nullptr;      // nq x cdim_pckd: Q3'
-    long long ldq = 0;
-    double *C[3] = {nullptr, nullptr, nullptr}, *inv[3] = {nullptr, nullptr, nullptr};
-    long long ldc = 0;
-    int npass = 2;
-    double *w = nullptr, *u = nullptr, *vv = nullptr, *xt = nullptr, *ws = nullptr, *norm2 = nullptr;
-};
-
-void qr_destroy(void *p) {
-    QrState *q = static_cast<QrState *>(p);
-    double *bufs[] = {q->Q, q->R1, q->tau, q->GsF, q->GsQ, q->Q3t, q->C[0], q->C[1], q->C[2], q->inv[0], q->inv[1],
-                      q->inv[2], q->w, q->u, q->vv, q->xt, q->ws, q->norm2};
-    for (double *b : bufs) if (b) cudaFree(b);
-    delete q;
-}
-
 __device__ __forceinline__ double cta_sum256(double v, double *sh) {
     v = warp_sum(v);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -154,121 +129,118 @@ int kkt_qr_setup(cvxb_kkt *k) {
     const int n = k->n, p = k->p, Kp = c.cdim_pckd;
     if (c.mnl) { set_error("kkt_qr: nonlinear rows are not part of this route (the reference's kkt_qr takes no mnl)"); return CVXB_E_ARG; }
     if (Kp < n - p) { set_error("kkt_qr: Rank([A; G]) < n (fewer cone rows than free variables)"); return CVXB_E_ARG; }
-    QrState *q = new QrState();
-    k->ext = q; k->ext_destroy = qr_destroy;
+    auto q = std::make_unique<QrState>();
     cudaStream_t st = k->st;
     q->nq = n - p;
     const size_t nn = (size_t)(n > 0 ? n : 1);
     q->ldf = ((Kp + 1) & ~1) > 2 ? ((Kp + 1) & ~1) : 2;
     q->ldq = ((q->nq + 1) & ~1) > 2 ? ((q->nq + 1) & ~1) : 2;
     q->ldc = q->ldq;
-    CVXB_CUDA(cudaMalloc(&q->GsF, (size_t)q->ldf * nn * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&q->Q3t, (size_t)q->ldq * (Kp > 0 ? Kp : 1) * sizeof(double)));
+    CVXB_TRY(q->GsF.alloc((size_t)q->ldf * nn));
+    CVXB_TRY(q->Q3t.alloc((size_t)q->ldq * (Kp > 0 ? Kp : 1)));
     const int nbk = (q->nq + NB - 1) / NB + 1;
     for (int i = 0; i < 3; ++i) {
-        CVXB_CUDA(cudaMalloc(&q->C[i], (size_t)q->ldc * (q->nq > 0 ? q->nq : 1) * sizeof(double)));
-        CVXB_CUDA(cudaMalloc(&q->inv[i], (size_t)2 * nbk * NB * NB * sizeof(double)));
+        CVXB_TRY(q->C[i].alloc((size_t)q->ldc * (q->nq > 0 ? q->nq : 1)));
+        CVXB_TRY(q->inv[i].alloc((size_t)2 * nbk * NB * NB));
     }
     const size_t kp1 = (size_t)(Kp > 0 ? Kp : 1);
-    CVXB_CUDA(cudaMalloc(&q->w, kp1 * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&q->u, (kp1 > nn ? kp1 : nn) * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&q->vv, nn * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&q->xt, nn * sizeof(double)));
-    CVXB_CUDA(cudaMalloc(&q->norm2, sizeof(double)));
+    CVXB_TRY(q->w.alloc(kp1));
+    CVXB_TRY(q->u.alloc(kp1 > nn ? kp1 : nn));
+    CVXB_TRY(q->vv.alloc(nn));
+    CVXB_TRY(q->xt.alloc(nn));
+    CVXB_TRY(q->norm2.alloc(1));
     {
         size_t a = nn * (size_t)gemv_n_chunks(Kp > n ? Kp : n), b = kp1 * (size_t)gemv_n_chunks(n);
-        CVXB_CUDA(cudaMalloc(&q->ws, (a > b ? a : b) * sizeof(double)));
+        CVXB_TRY(q->ws.alloc(a > b ? a : b));
     }
     if (p > 0) {
         // A' = [Q1 Q2][R1; 0]: p Householder reflectors of the n x p matrix, then Q = H_0 ... H_{p-1} applied to I
         q->ldQ = (n + 1) & ~1;
-        CVXB_CUDA(cudaMalloc(&q->Q, (size_t)q->ldQ * nn * sizeof(double)));
-        CVXB_CUDA(cudaMalloc(&q->R1, (size_t)p * p * sizeof(double)));
-        CVXB_CUDA(cudaMalloc(&q->tau, (size_t)p * sizeof(double)));
-        CVXB_CUDA(cudaMalloc(&q->GsQ, (size_t)q->ldf * nn * sizeof(double)));
-        double *QA = nullptr;                       // n x p
+        CVXB_TRY(q->Q.alloc((size_t)q->ldQ * nn));
+        CVXB_TRY(q->R1.alloc((size_t)p * p));
+        CVXB_TRY(q->tau.alloc((size_t)p));
+        CVXB_TRY(q->GsQ.alloc((size_t)q->ldf * nn));
+        DevBuf<double> QAbuf;                       // n x p
         const long long ldqa = (n + 1) & ~1;
-        CVXB_CUDA(cudaMalloc(&QA, (size_t)ldqa * p * sizeof(double)));
-        int rc = transpose_copy(k->Aeq, k->lda_eq, QA, ldqa, p, n, st);
+        CVXB_TRY(QAbuf.alloc((size_t)ldqa * p));
+        double *QA = QAbuf.p, *tau = q->tau.p;
+        int rc = transpose_copy(k->Aeq.p, k->lda_eq, QA, ldqa, p, n, st);
         for (int j = 0; j < p && rc == 0; ++j) {
-            house_kernel<<<1, 256, 0, st>>>(n, j, QA, ldqa, q->tau);
-            if (j + 1 < p) house_apply_kernel<<<p - j - 1, 256, 0, st>>>(n, j, QA, ldqa, q->tau, QA, ldqa, j + 1);
+            house_kernel<<<1, 256, 0, st>>>(n, j, QA, ldqa, tau);
+            if (j + 1 < p) house_apply_kernel<<<p - j - 1, 256, 0, st>>>(n, j, QA, ldqa, tau, QA, ldqa, j + 1);
             count_launch(2);
         }
         if (rc == 0) {
-            identity_kernel<<<(unsigned)(((long long)n * n + 255) / 256), 256, 0, st>>>(n, q->Q, q->ldQ);
+            identity_kernel<<<(unsigned)(((long long)n * n + 255) / 256), 256, 0, st>>>(n, q->Q.p, q->ldQ);
             for (int j = p - 1; j >= 0; --j) {
                 // H_j touches rows j.. only and columns < j of the partial product are still unit vectors e_c with
                 // c < j: apply to columns j .. n-1
-                house_apply_kernel<<<n - j, 256, 0, st>>>(n, j, QA, ldqa, q->tau, q->Q, q->ldQ, j);
+                house_apply_kernel<<<n - j, 256, 0, st>>>(n, j, QA, ldqa, tau, q->Q.p, q->ldQ, j);
                 count_launch();
             }
-            extract_r_kernel<<<(p * p + 255) / 256, 256, 0, st>>>(p, QA, ldqa, q->R1);
+            extract_r_kernel<<<(p * p + 255) / 256, 256, 0, st>>>(p, QA, ldqa, q->R1.p);
             count_launch(2);
         }
         cudaError_t e = cudaStreamSynchronize(st);
-        cudaFree(QA);
         if (rc) return rc;
         if (e != cudaSuccess) { set_error("kkt_qr setup: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
         CVXB_LAUNCH_CHECK();
     }
+    k->qr = std::move(q);
     return 0;
 }
 
 int kkt_qr_factor(cvxb_kkt *k, const cvxb_scaling *Wp, int space) {
-    QrState *q = static_cast<QrState *>(k->ext);
+    QrState *q = k->qr.get();
     const ConeLayout &c = k->cone;
     const int n = k->n, p = k->p, Kp = c.cdim_pckd, nq = q->nq;
     cudaStream_t st = k->st;
     CVXB_CUDA(cudaEventRecord(k->e0, st));
     CVXB_TRY(k->W.upload(c, Wp, space, st));
     // ---- Gs = pack(W^{-T} G), every row materialised                            (misc.py:1614-1616)
-    if (c.ml > 0) CVXB_TRY(scale_rows(k->G, k->ldg, q->GsF, q->ldf, c.ml, n, k->W.di, st));
-    if (c.nq > 0) CVXB_TRY(scale_q(c, k->W, k->G + c.ml, k->ldg, q->GsF + c.ml, q->ldf, n, true, st));
-    if (c.ns > 0) {
-        CVXB_TRY(scale_s(c, k->W, k->G + c.ml + c.sumq, k->ldg, k->Gunp, c.sums2, n, 'T', 'I', k->swork,
-                         k->swork_doubles, st));
-        CVXB_TRY(pack_s(c, k->Gunp, c.sums2, q->GsF + c.ml + c.sumq, q->ldf, n, false, st));
-    }
+    if (c.ml > 0) CVXB_TRY(scale_rows(k->G, k->ldg, q->GsF.p, q->ldf, c.ml, n, k->W.di, st));
+    CVXB_TRY(kkt_scale_pack_G(k, q->GsF.p + c.ml, q->ldf));
     CVXB_CUDA(cudaEventRecord(k->e1, st));
-    const double *Gs2 = q->GsF;
+    const double *Gs2 = q->GsF.p;
     if (p > 0) {                                   // [Gs1 Gs2] = Gs [Q1 Q2]          (:1619)
         GemmDesc g;
         g.M = Kp; g.N = n; g.K = n;
-        g.X = q->GsF; g.ldx = (int)q->ldf; g.x_kmajor = false;
-        g.Y = q->Q; g.ldy = (int)q->ldQ; g.y_kmajor = true;
-        g.C = q->GsQ; g.ldc = (int)q->ldf;
+        g.X = q->GsF.p; g.ldx = (int)q->ldf; g.x_kmajor = false;
+        g.Y = q->Q.p; g.ldy = (int)q->ldQ; g.y_kmajor = true;
+        g.C = q->GsQ.p; g.ldc = (int)q->ldf;
         CVXB_TRY(dmma_gemm(g, st));
-        Gs2 = q->GsQ + (long long)p * q->ldf;
+        Gs2 = q->GsQ.p + (long long)p * q->ldf;
     }
     int info = 0;
     if (nq > 0) {
         // ---- Gs2 = Q3 R3 by Cholesky-QR passes; Q3' is built in place in Q3t
+        double *Q3t = q->Q3t.p, *norm2 = q->norm2.p;
         auto run = [&](bool shifted) -> int {
             q->npass = shifted ? 3 : 2;
-            CVXB_TRY(transpose_copy(Gs2, q->ldf, q->Q3t, q->ldq, Kp, nq, st));
+            CVXB_TRY(transpose_copy(Gs2, q->ldf, Q3t, q->ldq, Kp, nq, st));
             if (shifted) {
-                CVXB_CUDA(cudaMemsetAsync(q->norm2, 0, sizeof(double), st));
-                sumsq_kernel<<<nq, 256, 0, st>>>(Kp, nq, Gs2, q->ldf, q->norm2);
+                CVXB_CUDA(cudaMemsetAsync(norm2, 0, sizeof(double), st));
+                sumsq_kernel<<<nq, 256, 0, st>>>(Kp, nq, Gs2, q->ldf, norm2);
                 count_launch();
             }
             for (int ps = 0; ps < q->npass; ++ps) {
+                double *C = q->C[ps].p, *inv = q->inv[ps].p;
                 GemmDesc g;                        // C = B B'  (B = Q3t, nq x Kp), lower triangle
                 g.M = nq; g.N = nq; g.K = Kp;
-                g.X = q->Q3t; g.ldx = (int)q->ldq; g.x_kmajor = false;
-                g.Y = q->Q3t; g.ldy = (int)q->ldq; g.y_kmajor = false;
-                g.C = q->C[ps]; g.ldc = (int)q->ldc; g.lower_only = true; g.splitk_ws = k->cw.splitk_ws;
+                g.X = Q3t; g.ldx = (int)q->ldq; g.x_kmajor = false;
+                g.Y = Q3t; g.ldy = (int)q->ldq; g.y_kmajor = false;
+                g.C = C; g.ldc = (int)q->ldc; g.lower_only = true; g.splitk_ws = k->cw.splitk_ws.p;
                 CVXB_TRY(dmma_gemm(g, st));
                 if (shifted && ps == 0) {
                     const double fac = 11.0 * ((double)Kp * nq + (double)nq * (nq + 1)) * 1.1102230246251565e-16;
-                    add_diag_kernel<<<(nq + 255) / 256, 256, 0, st>>>(nq, q->C[0], q->ldc, q->norm2, fac);
+                    add_diag_kernel<<<(nq + 255) / 256, 256, 0, st>>>(nq, C, q->ldc, norm2, fac);
                     count_launch();
                 }
-                CVXB_TRY(potrf_lower(nq, q->C[ps], (int)q->ldc, q->inv[ps], k->cw, st));
-                CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info, sizeof(int), cudaMemcpyDeviceToHost, st));
+                CVXB_TRY(potrf_lower(nq, C, (int)q->ldc, inv, k->cw, st));
+                CVXB_CUDA(cudaMemcpyAsync(&info, k->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToHost, st));
                 CVXB_CUDA(cudaStreamSynchronize(st));
                 if (info > 0) return 0;
-                CVXB_TRY(trsm_lower_left(nq, q->C[ps], q->ldc, q->inv[ps], q->Q3t, q->ldq, Kp, st));
+                CVXB_TRY(trsm_lower_left(nq, C, q->ldc, inv, Q3t, q->ldq, Kp, st));
             }
             return 0;
         };
@@ -289,72 +261,51 @@ int kkt_qr_factor(cvxb_kkt *k, const cvxb_scaling *Wp, int space) {
     return 0;
 }
 
-int kkt_qr_passes(const cvxb_kkt *k) { return k->ext ? static_cast<const QrState *>(k->ext)->npass : 0; }
-
-int kkt_qr_solve(cvxb_kkt *k, double *x, double *y, double *z, int space) {
-    QrState *q = static_cast<QrState *>(k->ext);
+// on entry w = bzp = W^{-T} bz, packed (:1626-1627); on return it holds W*uz, packed, for kkt_unpack_z (:1675)
+int kkt_qr_solve(cvxb_kkt *k, double *xd, double *yd) {
+    const QrState *q = k->qr.get();
     const ConeLayout &c = k->cone;
     const int n = k->n, p = k->p, Kp = c.cdim_pckd, nq = q->nq;
     cudaStream_t st = k->st;
     const int T = 256;
-    CVXB_CUDA(cudaEventRecord(k->e0, st));
-    double *xd = x, *zd = z, *yd = y;
-    if (p > 0 && !y) { set_error("solve: y is required when p > 0"); return CVXB_E_ARG; }
-    if (space != CVXB_DEVICE) {
-        CVXB_TRY(xfer_vec(k->xv, x, n, CVXB_HOST, true, st));
-        CVXB_TRY(xfer_vec(k->zin, z, c.cdim, CVXB_HOST, true, st));
-        xd = k->xv; zd = k->zin;
-        if (p > 0) { CVXB_TRY(xfer_vec(k->yd, y, p, CVXB_HOST, true, st)); yd = k->yd; }
-    }
-    // w := W^{-T} bz, packed                                                      (:1626-1627)
-    CVXB_TRY(kkt_pack_bz(k, zd));
-    double *w = k->bzp;
+    double *w = k->bzp.p;
+    double *vv = q->vv.p, *xt = q->xt.p, *u = q->u.p, *ws = q->ws.p;
+    const double *Q = q->Q.p, *R1 = q->R1.p, *GsQ = q->GsQ.p, *Q3t = q->Q3t.p;
     // vv := [Q1'bx; R3^{-T} Q2'bx]                                                (:1630-1633)
-    if (p > 0) CVXB_TRY(gemv_t(n, n, q->Q, q->ldQ, nullptr, xd, 1.0, 0.0, q->vv, st));
-    else CVXB_CUDA(cudaMemcpyAsync(q->vv, xd, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (p > 0) CVXB_TRY(gemv_t(n, n, Q, q->ldQ, nullptr, xd, 1.0, 0.0, vv, st));
+    else CVXB_CUDA(cudaMemcpyAsync(vv, xd, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
     for (int ps = 0; ps < q->npass; ++ps)       // R3^{-T} = L_np^{-1} ... L_1^{-1}
-        CVXB_TRY(trsv_lower(nq, q->C[ps], (int)q->ldc, q->inv[ps], q->vv + p, false, k->cw, st));
+        CVXB_TRY(trsv_lower(nq, q->C[ps].p, (int)q->ldc, q->inv[ps].p, vv + p, false, k->cw, st));
     if (p > 0) {
         // xt[:p] := R1^{-T} by;   w := w - Gs1 xt[:p]                             (:1636-1642)
-        CVXB_CUDA(cudaMemcpyAsync(q->xt, yd, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        trsv_upper_small_kernel<<<1, 256, 0, st>>>(p, q->R1, q->xt, 1);
+        CVXB_CUDA(cudaMemcpyAsync(xt, yd, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        trsv_upper_small_kernel<<<1, 256, 0, st>>>(p, R1, xt, 1);
         count_launch();
-        CVXB_TRY(gemv_n(Kp, p, q->GsQ, q->ldf, nullptr, q->xt, -1.0, 1.0, w, q->ws, st));
+        CVXB_TRY(gemv_n(Kp, p, GsQ, q->ldf, nullptr, xt, -1.0, 1.0, w, ws, st));
     }
     // u := Q3'w + vv[p:]                                                          (:1646-1650)
     if (nq > 0) {
-        CVXB_CUDA(cudaMemcpyAsync(q->u, q->vv + p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        CVXB_TRY(gemv_n(nq, Kp, q->Q3t, q->ldq, nullptr, w, 1.0, 1.0, q->u, q->ws, st));
+        CVXB_CUDA(cudaMemcpyAsync(u, vv + p, (size_t)nq * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(gemv_n(nq, Kp, Q3t, q->ldq, nullptr, w, 1.0, 1.0, u, ws, st));
         // xt[p:] := R3^{-1} u = L_1^{-T} ... L_np^{-T} u                          (:1653-1655)
-        CVXB_CUDA(cudaMemcpyAsync(q->xt + p, q->u, (size_t)nq * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_CUDA(cudaMemcpyAsync(xt + p, u, (size_t)nq * sizeof(double), cudaMemcpyDeviceToDevice, st));
         for (int ps = q->npass - 1; ps >= 0; --ps)
-            CVXB_TRY(trsv_lower(nq, q->C[ps], (int)q->ldc, q->inv[ps], q->xt + p, true, k->cw, st));
+            CVXB_TRY(trsv_lower(nq, q->C[ps].p, (int)q->ldc, q->inv[ps].p, xt + p, true, k->cw, st));
     }
     // x := [Q1 Q2] xt                                                             (:1659)
-    if (p > 0) CVXB_TRY(gemv_n(n, n, q->Q, q->ldQ, nullptr, q->xt, 1.0, 0.0, xd, q->ws, st));
-    else CVXB_CUDA(cudaMemcpyAsync(xd, q->xt, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    if (p > 0) CVXB_TRY(gemv_n(n, n, Q, q->ldQ, nullptr, xt, 1.0, 0.0, xd, ws, st));
+    else CVXB_CUDA(cudaMemcpyAsync(xd, xt, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
     // W*uz (packed) := Q3 u - w, kept in bzp                                       (:1663-1665)
-    if (nq > 0) CVXB_TRY(gemv_t(nq, Kp, q->Q3t, q->ldq, nullptr, q->u, 1.0, -1.0, w, st));
-    else if (Kp > 0) { axmy_kernel<<<(Kp + T - 1) / T, T, 0, st>>>(Kp, q->u, w); count_launch(); }
+    if (nq > 0) CVXB_TRY(gemv_t(nq, Kp, Q3t, q->ldq, nullptr, u, 1.0, -1.0, w, st));
+    else if (Kp > 0) { axmy_kernel<<<(Kp + T - 1) / T, T, 0, st>>>(Kp, u, w); count_launch(); }
     if (p > 0) {
         // y := R1^{-1} (Q1'bx - Gs1' (W uz))                                       (:1669-1673)
-        CVXB_CUDA(cudaMemcpyAsync(yd, q->vv, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        CVXB_TRY(gemv_t(Kp, p, q->GsQ, q->ldf, nullptr, w, -1.0, 1.0, yd, st));
-        trsv_upper_small_kernel<<<1, 256, 0, st>>>(p, q->R1, yd, 0);
+        CVXB_CUDA(cudaMemcpyAsync(yd, vv, (size_t)p * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(gemv_t(Kp, p, GsQ, q->ldf, nullptr, w, -1.0, 1.0, yd, st));
+        trsv_upper_small_kernel<<<1, 256, 0, st>>>(p, R1, yd, 0);
         count_launch();
     }
     CVXB_LAUNCH_CHECK();
-    CVXB_TRY(kkt_unpack_z(k, zd));                                              // (:1675)
-    if (space != CVXB_DEVICE) {
-        CVXB_TRY(xfer_vec(x, k->xv, n, CVXB_HOST, false, st));
-        CVXB_TRY(xfer_vec(z, k->zin, c.cdim, CVXB_HOST, false, st));
-        if (p > 0) CVXB_TRY(xfer_vec(y, k->yd, p, CVXB_HOST, false, st));
-    }
-    CVXB_CUDA(cudaEventRecord(k->e1, st));
-    CVXB_CUDA(cudaStreamSynchronize(st));
-    float t;
-    cudaEventElapsedTime(&t, k->e0, k->e1);
-    k->solve_ms = t;
     return 0;
 }
 

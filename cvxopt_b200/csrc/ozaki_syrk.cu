@@ -21,6 +21,7 @@
 // run the epilogue, warp 8 is the producer (cp.async.bulk + mbarrier ring).
 #include "common.cuh"
 #include <cstdint>
+#include <cstdlib>
 #include <cmath>
 #include <vector>
 #include <algorithm>
@@ -390,6 +391,18 @@ size_t ozaki_workspace_bytes(int n, int m, int S) {
     const size_t nblk = (n + OZ_T - 1) / OZ_T, nk = std::max(1, (m + OZ_KS - 1) / OZ_KS);
     return nblk * nk * (size_t)S * OZ_UNIT + 2 * (size_t)n * sizeof(double) + nblk * (nblk + 1) / 2 * sizeof(unsigned int) + 1024
            + (size_t)kNumSMs * OZ_T * OZ_T * sizeof(double) + 256;         // partial tiles of the split-K tail wave
+}
+
+int ozaki_mode() {
+    const char *e = getenv("CVXB_OZAKI");
+    return !e ? 0 : (e[0] == '0') ? 0 : (e[0] == '2') ? 2 : 1;
+}
+
+bool ozaki_use(int mode, int n, int m, DevBuf<char> &work) {
+    if (!(mode == 2 || (mode == 1 && n >= 4096 && m >= 8192))) return false;
+    // the slice workspace is ~1.125 x sizeof(A)
+    const size_t need = ozaki_workspace_bytes(n, m, 9);
+    return need <= work.n || work.try_alloc(need) == cudaSuccess;
 }
 
 int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, const double *D, long long ldd,

@@ -66,6 +66,10 @@ int  cvxb_device_count(void);                 /* sm_90 devices visible          
 int  cvxb_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches) */
 unsigned long long cvxb_launch_count(void);
+/* bytes of device memory the library's handles and per-device workspaces hold right now (all devices); back to
+ * its earlier value once a handle is destroyed.  The scratch-buffer cache of the calls without a handle is not
+ * counted. */
+unsigned long long cvxb_device_bytes(void);
 /* cudaMalloc/cudaFree/cudaMemcpy shims so a ctypes-only host needs no CUDA binding */
 int  cvxb_malloc(void **dptr, unsigned long long bytes);
 int  cvxb_free(void *dptr);

@@ -103,6 +103,38 @@ def test_distributed_entry_single_process_matches_qp_batch():
         assert set(tm) >= {"setup_ms", "scatter_ms", "solve_ms", "gather_ms"}
 
 
+@pytest.mark.parametrize("B,ozaki", [(3, "0"), (1, "2")])
+def test_batch_handle_frees_its_device_memory(B, ozaki, monkeypatch):
+    """every byte of device memory a batch handle holds is freed with it: a batch that compacts finished problems
+    away, and a single problem whose SYRK runs on the int8 slices (CVXB_OZAKI=2: its workspace)"""
+    from cvxopt_b200 import _lib
+    from cvxopt_b200.batch import QPBatch
+    lib = _lib.load()
+    monkeypatch.setenv("CVXB_OZAKI", ozaki)
+    monkeypatch.setenv("CVXB_BATCH_COMPACT", "1")
+    n, m = 40, 90
+    P, q, G, h = make_batch(B, n, m, seed0=500)
+    q[0] *= 1e3                     # the first problem takes a different number of iterations
+    h[0] *= 1e-2
+
+    def run():
+        b = QPBatch(B, n, m, 0)
+        b.load(P, q, G, h)
+        b.solve()
+        return b, b.results()
+
+    b, _ = run()                    # warm-up
+    b.close()
+    base = lib.cvxb_device_bytes()
+    b, r = run()
+    assert lib.cvxb_device_bytes() > base
+    assert b.stats()["syrk_path"] == ("int8" if ozaki == "2" else "dmma")
+    if B > 1:
+        assert len(set(r["iterations"])) > 1          # finished problems were swapped out of the active prefix
+    b.close()
+    assert lib.cvxb_device_bytes() == base
+
+
 def test_compaction_of_finished_problems(monkeypatch):
     """The lock-step loop swaps finished problems out of the active prefix (csrc/batch_ipm.cu): per-problem results
     are those of the uncompacted loop, come back in the caller's order, and a second solve on the same loaded batch

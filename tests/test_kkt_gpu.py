@@ -352,9 +352,78 @@ def test_max_step_s_blocks_special_matrices():
         ms.max_step(bad.reshape(-1, order="F").copy(), {"l": 0, "q": [], "s": [5]})
 
 
-def test_no_cone_rows_and_handle_lifecycle():
-    """cdim == 0 (unconstrained QP step: K = H) and repeated create/destroy (no leaks, no stale state)."""
+def open_factory(case, rng):
+    """create, factor and solve one KKT factory of the kind `case`; returned still open"""
+    import cvxopt_b200
+    n, p, dims = 30, 5, {"l": 40, "q": [5, 8], "s": [4, 3]}
+    if case in ("l", "ozaki2", "trace"):
+        n, p, dims = 300, 0, {"l": 900, "q": [], "s": []}
+    K = cone_dim(dims)
+    G = np.asfortranarray(rng.standard_normal((K, n)))
+    A = np.asfortranarray(rng.standard_normal((p, n))) if p else None
+    B = rng.standard_normal((n, n))
+    H = np.asfortranarray(B @ B.T / n + np.eye(n))
+    W, _ = random_scaling(dims, 3)
+    mnl = 0
+    if case == "qs_A_H":
+        f = cvxopt_b200.kkt_chol(G, dims, A, H=H)
+        f.set_H(H)                      # the resident H a second time
+        f(W)
+        f(W, H.copy())                  # a per-call H: the lazily allocated upload buffer
+    elif case == "mnl_Df":
+        mnl = 3
+        W = dict(W, dnl=rng.uniform(0.5, 2.0, mnl))
+        W["dnli"] = 1.0 / W["dnl"]
+        f = cvxopt_b200.kkt_chol(G, dims, A, mnl)
+        f(W, H, np.asfortranarray(rng.standard_normal((mnl, n))))
+    elif case == "qr_A":
+        f = cvxopt_b200.kkt_qr(G, dims, A)
+        f(W)
+    elif case == "ldl2_A":
+        f = cvxopt_b200.kkt_ldl2(G, dims, A)
+        f(W, H)
+    else:
+        f = cvxopt_b200.kkt_chol(G, dims)
+        f(W)
+        assert f.syrk_path() == ("int8" if case == "ozaki2" else "dmma")
+    f.solve(rng.standard_normal(n), rng.standard_normal(p) if p else None, rng.standard_normal(mnl + K))
+    return f
+
+
+def check_lifecycle(case, rng, monkeypatch):
+    """20 create/factor/solve/close rounds of one kind of factory: cvxb_device_bytes() is above its baseline while the
+    factory is open and back to it exactly after close(), and the card's free memory does not drift"""
     import torch
+    from cvxopt_b200 import _lib
+    lib = _lib.load()
+    monkeypatch.delenv("CVXB_OZAKI", raising=False)
+    monkeypatch.delenv("CVXB_TRACE", raising=False)
+    if case == "ozaki2":
+        monkeypatch.setenv("CVXB_OZAKI", "2")
+    if case == "trace":
+        monkeypatch.setenv("CVXB_TRACE", "1")
+    free0 = torch.cuda.mem_get_info()[0]
+    open_factory(case, rng).close()     # warm-up
+    base = lib.cvxb_device_bytes()
+    for _ in range(20):
+        f = open_factory(case, rng)
+        assert lib.cvxb_device_bytes() > base
+        f.close()
+        assert lib.cvxb_device_bytes() == base
+    free1 = torch.cuda.mem_get_info()[0]
+    assert free0 - free1 < 64 << 20, (free0, free1)
+
+
+@pytest.mark.parametrize("case", ["qs_A_H", "mnl_Df", "qr_A", "ldl2_A", "ozaki2", "trace"])
+def test_factory_lifecycle_frees_device_memory(case, monkeypatch):
+    """every byte of device memory a factory holds is freed with it, for each route and each lazily allocated
+    buffer (the per-call H upload, the int8-slice workspace with CVXB_OZAKI=2, the Cholesky timeline with
+    CVXB_TRACE=1); the 'l'-only Cholesky case is test_no_cone_rows_and_handle_lifecycle's"""
+    check_lifecycle(case, np.random.Generator(np.random.PCG64(2)), monkeypatch)
+
+
+def test_no_cone_rows_and_handle_lifecycle(monkeypatch):
+    """cdim == 0 (unconstrained QP step: K = H) and repeated create/destroy (no leaks, no stale state)."""
     import cvxopt_b200
     n = 70
     rng = np.random.Generator(np.random.PCG64(2))
@@ -369,12 +438,4 @@ def test_no_cone_rows_and_handle_lifecycle():
     solve(x, None, np.zeros(0))
     assert relerr(x, np.linalg.solve(H, x0)) < 1e-11
     fac.close()
-    free0 = torch.cuda.mem_get_info()[0]
-    G = np.asfortranarray(rng.standard_normal((900, 300)))
-    Wl, _ = random_scaling({"l": 900, "q": [], "s": []}, 3)
-    for _ in range(20):
-        f = cvxopt_b200.kkt_chol(G, {"l": 900, "q": [], "s": []})
-        f(Wl)
-        f.close()
-    free1 = torch.cuda.mem_get_info()[0]
-    assert free0 - free1 < 64 << 20, (free0, free1)
+    check_lifecycle("l", rng, monkeypatch)
