@@ -1,11 +1,13 @@
 """Batch of independent dense QPs solved in lock-step on the device (BASELINE config 4).
 
-    minimize 1/2 x'P x + q'x   subject to   G x <= h        (one 'l' cone of m rows, no A)
+    minimize 1/2 x'P x + q'x   subject to   G x + s = h,  s in K      (no A)
 
-The per-problem algorithm is coneprog.coneqp restricted to dims={'l': m} (reference
-src/python/coneprog.py:1998-2547) — same start, stopping rule, Mehrotra steps — so every
-problem converges in the same number of iterations as `solvers.qp(P, q, G, h)` does.
-The reference has no batch API; its counterpart is a Python loop over `solvers.qp`.
+K is one 'l' cone of m rows by default, or dims = {'l': ml, 'q': [...]} shared by every problem.
+The per-problem algorithm is coneprog.coneqp (reference src/python/coneprog.py:1998-2547) with
+kktsolver='chol' and default options — same start, stopping rule, Mehrotra steps and iterative
+refinement — so every problem converges in the same number of iterations as
+`solvers.coneqp(P, q, G, h, dims)` (for dims={'l': m}: `solvers.qp(P, q, G, h)`) does.
+The reference has no batch API; its counterpart is a Python loop over those calls.
 """
 import ctypes as C
 
@@ -15,6 +17,20 @@ from . import _lib
 
 STATUS = {0: "running", 1: "optimal", 2: "unknown", 3: "unknown"}
 DEFAULTS = dict(maxiters=100, abstol=1e-7, reltol=1e-6, feastol=1e-7)   # coneprog.py:436-456
+
+
+def _batch_dims(dims, m=None):
+    """dims -> (ctypes Dims or None, keep-alive, cdim).  None is {'l': m}.  's' cones are not built for the batch."""
+    if dims is None:
+        return None, None, m
+    from . import kkt
+    dims = {"l": dims.get("l", 0), "q": list(dims.get("q", [])), "s": list(dims.get("s", []))}
+    d, keep, cdim, _ = kkt.make_dims(dims)
+    if dims["s"]:
+        raise NotImplementedError("the batch solver has no 's' cones")
+    if m is not None and int(m) != cdim:
+        raise TypeError("m = %d does not match the cone dimension %d of dims" % (int(m), cdim))
+    return d, keep, cdim
 
 
 def _stack(P, q, G, h):
@@ -40,11 +56,20 @@ def _stack(P, q, G, h):
 
 
 class QPBatch:
-    def __init__(self, nprob, n, m, device=0):
+    """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}."""
+
+    def __init__(self, nprob, n, m, device=0, dims=None):
+        d, keep, cdim = _batch_dims(dims, m)
         self._lib = _lib.load()
         self._h = C.c_void_p()
-        self.B, self.n, self.m = int(nprob), int(n), int(m)
-        _lib.check(self._lib.cvxb_batch_create(C.byref(self._h), self.B, self.n, self.m, device), "batch")
+        self.B, self.n, self.m = int(nprob), int(n), int(cdim)
+        if d is None:
+            rc = self._lib.cvxb_batch_create(C.byref(self._h), self.B, self.n, self.m, device)
+        else:
+            rc = self._lib.cvxb_batch_create_cones(C.byref(self._h), self.B, self.n, C.byref(d), device)
+        del keep
+        _lib.check(rc, "batch")
+        self._refinement = None
 
     def load(self, P, q, G, h):
         Pcm, q, Gcm, h, B, n, m = _stack(P, q, G, h)
@@ -58,9 +83,16 @@ class QPBatch:
         """raw addresses of already laid-out buffers (device-resident callers)"""
         _lib.check(self._lib.cvxb_batch_load(self._h, P, q, G, h, space), "batch_load")
 
-    def solve(self, **options):
+    def solve(self, refinement=None, **options):
+        """refinement: steps of iterative refinement per Newton solve (coneqp's option); None keeps the default
+        (1 with 'q' cones, else 0)"""
         o = dict(DEFAULTS)
         o.update(options)
+        if refinement is not None and refinement != self._refinement:
+            if not isinstance(refinement, (int, np.integer)) or isinstance(refinement, bool) or refinement < 0:
+                raise ValueError("refinement must be a nonnegative integer")
+            _lib.check(self._lib.cvxb_batch_set_refinement(self._h, int(refinement)), "batch_set_refinement")
+            self._refinement = refinement
         rc = self._lib.cvxb_batch_solve(self._h, int(o["maxiters"]), float(o["abstol"]),
                                         float(o["reltol"]), float(o["feastol"]))
         if rc == _lib.E_ARG and "Rank(" in _lib.last_error():
@@ -118,7 +150,7 @@ class QPBatchGroup:
     as ITS slowest problem is done.  Interleaved slices (problem i -> sub-batch i mod nsub) spread hard and easy
     problems evenly."""
 
-    def __init__(self, nprob, n, m, device=0, nsub=None):
+    def __init__(self, nprob, n, m, device=0, nsub=None, dims=None):
         if nsub is None:
             # a few sub-batches let the finished problems of one leave the lock-step loop early (counts chosen
             # when the kernels were tuned, not re-measured on H100; CVXB_BATCH_NSUB overrides)
@@ -127,7 +159,13 @@ class QPBatchGroup:
         self.nsub = max(1, min(int(nsub), nprob))
         self.B, self.n, self.m = int(nprob), int(n), int(m)
         self.idx = [np.arange(r, self.B, self.nsub) for r in range(self.nsub)]
-        self.parts = [QPBatch(len(ix), n, m, device) for ix in self.idx]
+        self.parts = []
+        try:
+            for ix in self.idx:
+                self.parts.append(QPBatch(len(ix), n, m, device, dims))
+        except BaseException:
+            self.close()
+            raise
 
     def load_ptr_sliced(self, loader):
         """loader(part_index, indices, QPBatch) loads one sub-batch (device-resident callers)"""
@@ -183,12 +221,17 @@ class QPBatchGroup:
             b.close()
 
 
-def qp_batch(P, q, G, h, device=0, nsub=None, **options):
-    """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,m,n), h (B,m).
-    nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches)."""
+def qp_batch(P, q, G, h, device=0, nsub=None, dims=None, **options):
+    """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,cdim,n), h (B,cdim).
+    nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches).
+    dims: cone dimensions shared by every problem ({'l': ml, 'q': [...]}); None is {'l': cdim}.
+    options: maxiters, abstol, reltol, feastol, refinement (as coneqp's)."""
     P = np.asarray(P)
     G = np.asarray(G)
-    b = QPBatchGroup(P.shape[0], P.shape[1], G.shape[1], device, nsub)
+    if P.ndim != 3 or G.ndim != 3:
+        raise TypeError("P must have shape (B, n, n) and G (B, cdim, n)")
+    _, _, cdim = _batch_dims(dims, G.shape[1])
+    b = QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims)
     try:
         b.load(P, q, G, h)
         import time
@@ -238,9 +281,10 @@ def _p2p(ops):
 
 
 def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interleaved", timings=None,
-                         nsub=None, **options):
+                         nsub=None, dims=None, **options):
     """Rank 0 passes the full batch (other ranks pass None); every rank returns its shard's results and
     rank 0 additionally gets the gathered batch, in the original problem order, under key 'all'.
+    Every rank passes the same `dims` (and options); shards are (k, cdim, n).
 
     `timings` (dict, optional) receives scatter_ms / solve_ms / gather_ms of this rank, measured with
     device events on the current stream (wall clock on CPU)."""
@@ -281,6 +325,7 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
     if rank == 0:
         # the batch in the layout QPBatch loads: column-major n x n / m x n per problem
         Pcm, qh, Gcm, hh, Btot, n, m = _stack(P, q, G, h)
+        _batch_dims(dims, m)
         meta = torch.tensor([Btot, n, m], dtype=torch.int64, device=dev)
         full = [torch.from_numpy(a).to(dev) for a in (Pcm, qh, Gcm, hh)]       # one H2D of the whole batch
     if world > 1:
@@ -294,7 +339,7 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
     # ---- setup (not data path): this rank's batch object = its device allocations ----
     local_dev = torch.cuda.current_device() if on_gpu else 0
     clk.start("setup_ms")
-    bobj = QPBatchGroup(k, n, m, local_dev, nsub) if (solver is None and k) else None
+    bobj = QPBatchGroup(k, n, m, local_dev, nsub, dims) if (solver is None and k) else None
     clk.stop()
 
     # ---- scatter ----

@@ -11,6 +11,7 @@
 // (misc.py:450-464).  Every KKT solve is the same path as cvxb_kkt_*: fused-scaling SYRK,
 // Cholesky, GEMV/TRSV — here batched over the problems through blockIdx.z / blockIdx.y.
 // Nothing leaves the device between iterations except one int ("how many are done").
+// Batches with 'q' cones or iterative refinement run the cone path further down (kc_* kernels, cone_batch_solve).
 #include "cone.cuh"
 #include <cstdlib>
 #include <memory>
@@ -304,6 +305,428 @@ __global__ void k_update(Ptrs p, const int *info, int iter) {
     if (tid == 0) S.gap = gap;
 }
 
+// ---- the cone path: dims = {'l': ml, 'q': [...]} and/or iterative refinement ----
+// Same IPM as above, restated for coneqp with 'q' cones (coneprog.py:1998-2547) and `refinement` steps of
+// iterative refinement per Newton solve (:2330-2347).  The 'l' rows [0, ml) keep d / di / lmbda in the vectors
+// above; cone k occupies rows [qoff[k], qoff[k+1]) and its NT scaling W_k = beta_k (2 v_k v_k' - J) lives in the
+// per-slot state row `cst` (misc.py:290-352).  'l' rows are spread over the threads of the CTA, 'q' cones over its
+// warps: lane i of the warp owns entries i, i+32, ... of the cone in every pass, and the entry-0 values every lane
+// needs are formed from warp sums, so no pass reads what another lane wrote.
+struct CPtrs {
+    Ptrs p;
+    int ml, nq, refinement;
+    const int *qoff;                 // nq + 1 row offsets; qoff[nq] = m
+    long long L;                     // doubles per slot in the state row
+    // inside a slot's row: v (sum q, indexed by row - ml), beta (nq), then the refinement vectors
+    double *v, *beta, *wx, *wx2, *wz, *ws, *wz2, *ws2, *wz3;
+};
+#define CB_SETUP                                                           \
+    const Ptrs &p = cp.p;                                                  \
+    PB_SETUP                                                               \
+    const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;           \
+    const long long oc = (long long)b * cp.L;                              \
+    (void)lane; (void)warp; (void)nwarp; (void)oc;
+#define FOR_CONES(o, len)                                                  \
+    for (int k_ = warp; k_ < cp.nq; k_ += nwarp)                           \
+        if (const int o = cp.qoff[k_], len = cp.qoff[k_ + 1] - cp.qoff[k_]; true)
+#define FOR_LANE(i, len) for (int i = lane; i < len; i += 32)
+
+// y := W_k x (inverse = 0) or W_k^{-1} x (inverse = 1) for one cone, x and y of this lane's entries (misc_solvers.c:144-183)
+__device__ __forceinline__ void q_scale(const double *v, double beta, const double *x, double *y, int len, int lane,
+                                        bool inverse) {
+    double a = 0;
+    FOR_LANE(i, len) a += (inverse && i > 0 ? -v[i] : v[i]) * x[i];
+    a = warp_sum(a);                                      // v'x, or v'Jx for the inverse
+    const double bb = inverse ? 1.0 / beta : beta;
+    __syncwarp();
+    FOR_LANE(i, len) {
+        const double xi = x[i];
+        double r;
+        if (!inverse) r = (i == 0) ? 2.0 * v[i] * a - xi : 2.0 * v[i] * a + xi;
+        else          r = (i == 0) ? 2.0 * v[i] * a - xi : xi - 2.0 * v[i] * a;
+        y[i] = bb * r;
+    }
+}
+// x := lmbda o\ x for one cone (misc_solvers.c:813-836)
+__device__ __forceinline__ void q_sinv(const double *l, double *x, int len, int lane) {
+    const double x0 = x[0], l0 = l[0];
+    double nl = 0, d = 0;
+    FOR_LANE(i, len) if (i > 0) { nl += l[i] * l[i]; d += x[i] * l[i]; }
+    nl = sqrt(warp_sum(nl)); d = warp_sum(d);
+    const double a = (l0 + nl) * (l0 - nl), ai = 1.0 / a;
+    const double al1 = a / l0, al2 = d / l0 - x0;
+    __syncwarp();
+    FOR_LANE(i, len) x[i] = (i == 0) ? (x0 * l0 - d) * ai : (al1 * x[i] + al2 * l[i]) * ai;
+}
+// x := H(lmbda^{1/2}) x (inverse = 0) or H(lmbda^{-1/2}) x (inverse = 1) for one cone (misc_solvers.c:315-342);
+// returns the new x[0]
+__device__ __forceinline__ double q_scale2(const double *l, double *x, int len, int lane, bool inverse) {
+    const double x0 = x[0], l0 = l[0];
+    double nl = 0, lx = 0;
+    FOR_LANE(i, len) {
+        if (i > 0) nl += l[i] * l[i];
+        lx += (i > 0 && !inverse) ? -l[i] * x[i] : l[i] * x[i];
+    }
+    nl = sqrt(warp_sum(nl)); lx = warp_sum(lx);
+    double a = sqrt(l0 + nl) * sqrt(l0 - nl);
+    lx /= a;
+    double bb = (x0 + lx) / (l0 / a + 1.0) / a;
+    if (!inverse) { bb = -bb; a = 1.0 / a; }
+    __syncwarp();
+    FOR_LANE(i, len) x[i] = (i == 0) ? lx * a : (x[i] + bb * l[i]) * a;
+    return lx * a;
+}
+// sqrt(x' J x) of this lane's entries, x0 given
+__device__ __forceinline__ double q_jnrm2(const double *x, double x0, int len, int lane) {
+    double a = 0;
+    FOR_LANE(i, len) if (i > 0) a += x[i] * x[i];
+    a = sqrt(warp_sum(a));
+    return sqrt(x0 - a) * sqrt(x0 + a);
+}
+// min over the cone of the 'l'-style margin: x0 - ||x1|| (max_step is its negative, misc_solvers.c:1073-1085)
+__device__ __forceinline__ double q_margin(const double *x, double x0, int len, int lane) {
+    double a = 0;
+    FOR_LANE(i, len) if (i > 0) a += x[i] * x[i];
+    return x0 - sqrt(warp_sum(a));
+}
+
+// W = I: v = e1, beta = 1 (coneprog.py:2055-2064); the 'l' part is k_init_rhs's
+__global__ void kc_init_w(CPtrs cp) {
+    CB_SETUP
+    (void)sh; (void)S; (void)on; (void)om;
+    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    FOR_CONES(o, len) {
+        FOR_LANE(i, len) v[o + i] = (i == 0) ? 1.0 : 0.0;
+        if (lane == 0) beta[k_] = 1.0;
+    }
+}
+// Gs = W^{-T} G, one warp per column (misc.py:1268-1271): 'l' rows times di, each 'q' block times W_k^{-1}
+__global__ void kc_build_gs(CPtrs cp, const double *G, double *Gs, long long ldg, long long sG) {
+    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+    const int j = blockIdx.x * nwarp + warp;
+    if (j >= cp.p.n) return;
+    const long long off = (long long)b * sG + (long long)j * ldg;
+    const double *g = G + off, *di = cp.p.di + (long long)b * cp.p.m;
+    double *o = Gs + off;
+    for (int i = lane; i < cp.ml; i += 32) o[i] = di[i] * g[i];
+    const double *v = cp.v + (long long)b * cp.L - cp.ml, *beta = cp.beta + (long long)b * cp.L;
+    for (int k = 0; k < cp.nq; ++k) {
+        const int r = cp.qoff[k], len = cp.qoff[k + 1] - r;
+        q_scale(v + r, beta[k], g + r, o + r, len, lane, true);
+    }
+}
+// dst = W^{-T} src over all rows
+__device__ __forceinline__ void cone_scale_inv(const CPtrs &cp, int b, const double *src, double *dst) {
+    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
+    const double *di = cp.p.di + (long long)b * cp.p.m;
+    const double *v = cp.v + (long long)b * cp.L - cp.ml, *beta = cp.beta + (long long)b * cp.L;
+    for (int i = tid; i < cp.ml; i += nt) dst[i] = di[i] * src[i];
+    FOR_CONES(o, len) q_scale(v + o, beta[k_], src + o, dst + o, len, lane, true);
+}
+// bzp = W^{-T} dz (the starting point's right-hand side)
+__global__ void kc_scale_bz(CPtrs cp) {
+    const long long om = (long long)blockIdx.x * cp.p.m;
+    cone_scale_inv(cp, blockIdx.x, cp.p.dz + om, cp.p.bzp + om);
+}
+// starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both
+__global__ void kc_init_point(CPtrs cp) {
+    CB_SETUP
+    double *s = p.s + om, *z = p.z + om;
+    const double *zn = p.bzp + om;
+    double ns = 0, mins = INFINITY, minz = INFINITY;
+    for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
+    for (int i = tid; i < p.m; i += nt) {
+        const double zv = zn[i];
+        z[i] = zv; s[i] = -zv;
+        ns += zv * zv;
+        if (i < cp.ml) { mins = fmin(mins, -zv); minz = fmin(minz, zv); }
+    }
+    FOR_CONES(o, len) {                                  // s = -z: ||s1|| = ||z1||, s0 = -z0
+        const double z0 = zn[o], mz = q_margin(zn + o, z0, len, lane);
+        mins = fmin(mins, -z0 - (z0 - mz));
+        minz = fmin(minz, mz);
+    }
+    ns = sqrt(block_sum(ns, sh));
+    mins = block_min(mins, sh);
+    minz = block_min(minz, sh);
+    const double ts = -mins, tz = -minz;
+    const double as = (ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
+    const double az = (tz >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + tz : 0.0;
+    __syncthreads();
+    for (int i = tid; i < cp.ml; i += nt) { s[i] += as; z[i] += az; }
+    for (int k = tid; k < cp.nq; k += nt) { s[cp.qoff[k]] += as; z[cp.qoff[k]] += az; }
+    __syncthreads();
+    double gap = 0;
+    for (int i = tid; i < p.m; i += nt) gap += s[i] * z[i];
+    gap = block_sum(gap, sh);
+    if (tid == 0) S.gap = gap;
+}
+// NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357)
+__global__ void kc_scaling(CPtrs cp, int first) {
+    CB_SETUP
+    (void)on;
+    if (S.done) return;
+    double *l = p.lmbda + om, *lsq = p.lmbdasq + om;
+    const double *s = p.s + om, *z = p.z + om;
+    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    for (int i = tid; i < cp.ml; i += nt) {
+        if (first) {
+            const double d = sqrt(s[i] / z[i]);
+            p.d[om + i] = d;
+            p.di[om + i] = 1.0 / d;
+            l[i] = sqrt(s[i] * z[i]);
+        }
+        lsq[i] = l[i] * l[i];
+    }
+    FOR_CONES(o, len) {
+        if (first) {
+            const double s0 = s[o], z0 = z[o];
+            const double aa = q_jnrm2(s + o, s0, len, lane), bb = q_jnrm2(z + o, z0, len, lane);
+            double sz = 0;
+            FOR_LANE(i, len) sz += s[o + i] * z[o + i];
+            sz = warp_sum(sz);
+            const double cc = sqrt((sz / aa / bb + 1.0) / 2.0);
+            // v = (s/a + J z/b) / (2c), then v := (v + e) / sqrt(2 (v0 + 1))
+            const double v0 = (z0 / bb + s0 / aa) * (1.0 / 2.0 / cc) + 1.0;
+            const double sc = 1.0 / sqrt(2.0 * v0);
+            const double dd = 2 * cc + s0 / aa + z0 / bb;
+            const double cs = (cc + z0 / bb) / dd / aa, cz = (cc + s0 / aa) / dd / bb, r = sqrt(aa * bb);
+            FOR_LANE(i, len) {
+                if (i == 0) { v[o] = v0 * sc; l[o] = cc * r; }
+                else {
+                    v[o + i] = (-z[o + i] / bb + s[o + i] / aa) * (1.0 / 2.0 / cc) * sc;
+                    l[o + i] = (s[o + i] * cs + z[o + i] * cz) * r;
+                }
+            }
+            if (lane == 0) beta[k_] = sqrt(aa / bb);
+            __syncwarp();
+        }
+        double nl = 0;
+        FOR_LANE(i, len) nl += l[o + i] * l[o + i];
+        nl = warp_sum(nl);
+        const double l0 = l[o];
+        FOR_LANE(i, len) lsq[o + i] = (i == 0) ? nl : 2.0 * l0 * l[o + i];
+    }
+    if (tid == 0) { S.mu = S.gap / (cp.ml + cp.nq); S.sigma = 0.0; S.eta = 0.0; }
+}
+// right-hand side of the i-th Newton system (coneprog.py:2373-2399); a copy of it for the refinement (:2331-2335)
+__global__ void kc_dir_rhs(CPtrs cp, int i) {
+    CB_SETUP
+    (void)sh;
+    const double sm = S.sigma * S.mu, c = -1.0 + S.eta;
+    for (int k = tid; k < p.n; k += nt) {
+        const double dx = c * p.rx[on + k];
+        p.dx[on + k] = dx;
+        if (cp.refinement) cp.wx[oc + k] = dx;
+    }
+    for (int k = tid; k < p.m; k += nt) {
+        double ds = (i == 1) ? -p.ws3[om + k] : 0.0;     // Mehrotra correction
+        ds -= p.lmbdasq[om + k];
+        const double dz = c * p.rz[om + k];
+        p.dz[om + k] = dz;
+        if (cp.refinement) { cp.wz[oc + k] = dz; cp.ws[oc + k] = ds; }
+        p.ds[om + k] = ds;
+    }
+    __syncthreads();
+    for (int k = tid; k < cp.ml; k += nt) { p.ds[om + k] += sm; if (cp.refinement) cp.ws[oc + k] += sm; }
+    for (int k = tid; k < cp.nq; k += nt) {
+        const int r = cp.qoff[k];
+        p.ds[om + r] += sm;
+        if (cp.refinement) cp.ws[oc + r] += sm;
+    }
+}
+// f4_no_ir, before the solve (coneprog.py:2301-2309): s := lmbda o\ s; z := z - W's; bzp := W^{-T} z.
+// z and s are slot b's vectors at z + b*sz, s + b*ss
+__global__ void kc_f4_pre(CPtrs cp, double *z, long long sz, double *s, long long ss) {
+    CB_SETUP
+    (void)sh; (void)S; (void)on;
+    z += b * sz; s += b * ss;
+    const double *l = p.lmbda + om;
+    for (int i = tid; i < cp.ml; i += nt) {
+        const double sv = s[i] / l[i];
+        s[i] = sv;
+        const double zv = z[i] - p.d[om + i] * sv;
+        z[i] = zv;
+        p.bzp[om + i] = p.di[om + i] * zv;
+    }
+    const double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    double *t = cp.wz3 + oc;                              // W's, then W^{-T} z
+    FOR_CONES(o, len) {
+        q_sinv(l + o, s + o, len, lane);
+        q_scale(v + o, beta[k_], s + o, t + o, len, lane, false);
+        FOR_LANE(i, len) z[o + i] -= t[o + i];
+        q_scale(v + o, beta[k_], z + o, p.bzp + om + o, len, lane, true);
+    }
+}
+// f4_no_ir, after the solve (:2316): z := W uz (bzp), s := s - z.  acc: the refinement step, (dx, dz, ds) += (x, z, s)
+__global__ void kc_f4_post(CPtrs cp, double *x, long long sx, double *z, long long sz, double *s, long long ss,
+                           int acc) {
+    CB_SETUP
+    (void)sh; (void)S;
+    x += b * sx; z += b * sz; s += b * ss;
+    for (int i = tid; i < p.m; i += nt) {
+        const double zv = p.bzp[om + i], sv = s[i] - zv;
+        z[i] = zv; s[i] = sv;
+        if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
+    }
+    if (acc) for (int i = tid; i < p.n; i += nt) p.dx[on + i] += x[i];
+}
+// refinement residual, the elementwise part of res() (coneprog.py:1930-1960): wx2 = wx, wz3 = W^{-1} dz,
+// wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds).  The P, G and G' products follow as batched GEMVs.
+__global__ void kc_res(CPtrs cp) {
+    CB_SETUP
+    (void)sh; (void)S;
+    const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om;
+    for (int i = tid; i < p.n; i += nt) cp.wx2[oc + i] = cp.wx[oc + i];
+    double *wz3 = cp.wz3 + oc, *wz2 = cp.wz2 + oc, *ws2 = cp.ws2 + oc;
+    for (int i = tid; i < cp.ml; i += nt) {
+        wz3[i] = p.di[om + i] * dz[i];
+        wz2[i] = cp.wz[oc + i] - p.d[om + i] * ds[i];
+        ws2[i] = cp.ws[oc + i] - l[i] * (dz[i] + ds[i]);
+    }
+    const double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    FOR_CONES(o, len) {
+        q_scale(v + o, beta[k_], dz + o, wz3 + o, len, lane, true);
+        q_scale(v + o, beta[k_], ds + o, wz2 + o, len, lane, false);
+        double a = 0;
+        FOR_LANE(i, len) a += l[o + i] * (ds[o + i] + dz[o + i]);
+        a = warp_sum(a);
+        const double u0 = ds[o] + dz[o], l0 = l[o];
+        FOR_LANE(i, len) {
+            wz2[o + i] = cp.wz[oc + o + i] - wz2[o + i];
+            ws2[o + i] = cp.ws[oc + o + i] - ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]);
+        }
+    }
+}
+// after the i-th direction: ds o dz, scale2 of ds and dz, step length, sigma (coneprog.py:2423-2456)
+__global__ void kc_dir_post(CPtrs cp, int i) {
+    CB_SETUP
+    (void)on;
+    double *ds = p.ds + om, *dz = p.dz + om;
+    const double *l = p.lmbda + om;
+    double dsdz = 0, mins = INFINITY, minz = INFINITY;
+    for (int k = tid; k < cp.ml; k += nt) {
+        const double s = ds[k], z = dz[k];
+        dsdz += s * z;
+        if (i == 0) p.ws3[om + k] = s * z;
+        const double ss = s / l[k], zs = z / l[k];
+        ds[k] = ss; dz[k] = zs;
+        mins = fmin(mins, ss); minz = fmin(minz, zs);
+    }
+    FOR_CONES(o, len) {
+        double a = 0;
+        FOR_LANE(k, len) a += ds[o + k] * dz[o + k];
+        a = warp_sum(a);
+        if (lane == 0) dsdz += a;
+        if (i == 0) {
+            const double s0 = ds[o], z0 = dz[o];
+            FOR_LANE(k, len) p.ws3[om + o + k] = (k == 0) ? a : z0 * ds[o + k] + s0 * dz[o + k];
+        }
+        __syncwarp();
+        const double s0 = q_scale2(l + o, ds + o, len, lane, false);
+        const double z0 = q_scale2(l + o, dz + o, len, lane, false);
+        mins = fmin(mins, q_margin(ds + o, s0, len, lane));
+        minz = fmin(minz, q_margin(dz + o, z0, len, lane));
+    }
+    dsdz = block_sum(dsdz, sh);
+    mins = block_min(mins, sh);
+    minz = block_min(minz, sh);
+    if (tid == 0) {
+        const double t = fmax(0.0, fmax(-mins, -minz));
+        double step;
+        if (t == 0.0) step = 1.0;
+        else step = (i == 0) ? fmin(1.0, 1.0 / t) : fmin(1.0, 0.99 / t);
+        S.step = step; S.dsdz = dsdz;
+        if (i == 0) {
+            const double v = fmin(1.0, fmax(0.0, 1.0 - step + dsdz / S.gap * step * step));
+            S.sigma = v * v * v;
+            S.eta = 0.0;
+        }
+    }
+}
+// x += step dx; ds, dz := e + step d; scale2 inverse; update_scaling (misc.py:439-573); s = W' lmbda,
+// z = W^{-1} lmbda; gap (coneprog.py:2459-2547)
+__global__ void kc_update(CPtrs cp, const int *info, int iter) {
+    CB_SETUP
+    if (S.done) return;
+    if (info[b] > 0) {      // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
+        if (tid == 0) { S.done = 1; S.status = 3; S.iters = iter; }
+        return;
+    }
+    const double step = S.step;
+    for (int k = tid; k < p.n; k += nt) p.x[on + k] += step * p.dx[on + k];
+    double *ds = p.ds + om, *dz = p.dz + om, *l = p.lmbda + om, *s = p.s + om, *z = p.z + om;
+    double gap = 0;
+    for (int k = tid; k < cp.ml; k += nt) {
+        const double lk = l[k];
+        const double ss = sqrt((1.0 + step * ds[k]) * lk), sz = sqrt((1.0 + step * dz[k]) * lk);
+        const double d = p.d[om + k] * ss / sz;
+        const double ln = ss * sz;
+        p.d[om + k] = d; p.di[om + k] = 1.0 / d;
+        l[k] = ln;
+        s[k] = d * ln;
+        z[k] = (1.0 / d) * ln;
+        gap += ln * ln;
+    }
+    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    FOR_CONES(o, len) {
+        FOR_LANE(k, len) {
+            ds[o + k] = step * ds[o + k] + (k == 0 ? 1.0 : 0.0);
+            dz[o + k] = step * dz[o + k] + (k == 0 ? 1.0 : 0.0);
+        }
+        __syncwarp();
+        const double s0r = q_scale2(l + o, ds + o, len, lane, true);
+        const double z0r = q_scale2(l + o, dz + o, len, lane, true);
+        // update_scaling: st = ds / a, zt = dz / b
+        const double aa = q_jnrm2(ds + o, s0r, len, lane), bb = q_jnrm2(dz + o, z0r, len, lane);
+        const double s0 = s0r / aa, z0 = z0r / bb, v0 = v[o];
+        double sz = 0, vs = 0, vz = 0;
+        FOR_LANE(k, len) {
+            const double sk = ds[o + k] / aa, zk = dz[o + k] / bb;
+            ds[o + k] = sk; dz[o + k] = zk;
+            sz += sk * zk;
+            vs += v[o + k] * sk;
+            vz += (k == 0) ? v[o + k] * zk : -v[o + k] * zk;
+        }
+        sz = warp_sum(sz); vs = warp_sum(vs); vz = warp_sum(vz);
+        const double cc = sqrt((1.0 + sz) / 2.0);
+        const double vq = (vs + vz) / 2.0 / cc, vu = vs - vz;
+        const double wk0 = 2 * v0 * vq - (s0 + z0) / 2.0 / cc;
+        const double dd = (v0 * vu - s0 / 2.0 + z0 / 2.0) / (wk0 + 1.0);
+        const double r = sqrt(aa * bb);
+        const double nv0 = 2.0 * vq * v0 - s0 / 2.0 / cc - 0.5 / cc * z0 + 1.0, sc = 1.0 / sqrt(2.0 * nv0);
+        __syncwarp();                                     // every lane has read v[o] and l[o]
+        FOR_LANE(k, len) {
+            const double sk = ds[o + k], zk = dz[o + k], vk = v[o + k];
+            if (k == 0) { l[o] = cc * r; v[o] = nv0 * sc; }
+            else {
+                l[o + k] = (vk * (2.0 * (-dd * vq + 0.5 * vu)) + sk * (0.5 * (1.0 - dd / cc)) +
+                            zk * (0.5 * (1.0 + dd / cc))) * r;
+                v[o + k] = (2.0 * vq * vk + 0.5 / cc * sk - 0.5 / cc * zk) * sc;
+            }
+        }
+        const double bk = beta[k_] * sqrt(aa / bb);
+        __syncwarp();
+        if (lane == 0) beta[k_] = bk;
+        // unscale with the new W and lambda
+        q_scale(v + o, bk, l + o, s + o, len, lane, false);
+        q_scale(v + o, bk, l + o, z + o, len, lane, true);
+        double g = 0;
+        FOR_LANE(k, len) g += l[o + k] * l[o + k];
+        g = warp_sum(g);
+        if (lane == 0) gap += g;
+    }
+    gap = block_sum(gap, sh);
+    if (tid == 0) S.gap = gap;
+}
+// swap rows i and j of a [slots x L] buffer for each pair
+__global__ void kc_swap_rows(double *a, long long L, const int *pairs) {
+    const long long i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < L; e += (long long)gridDim.x * blockDim.x) {
+        const double t = a[i * L + e]; a[i * L + e] = a[j * L + e]; a[j * L + e] = t;
+    }
+}
+
 }  // namespace
 
 struct cvxb_batch {
@@ -333,6 +756,14 @@ struct cvxb_batch {
     int i8_mode = 0;
     int syrk_path = 0;
     DevBuf<char> oz_work;
+    // cone path (cvxb_batch_create_cones / cvxb_batch_set_refinement): rows [0, ml) are 'l', then the 'q' cones
+    int ml = 0, refinement = 0;
+    std::vector<int> qdims;          // dims['q']
+    DevBuf<int> qoff;                // nq + 1 row offsets
+    DevBuf<double> Gs;               // W^{-T} G per slot (ld ldg), rebuilt every factorisation
+    DevBuf<double> cst;              // per-slot state row: v, beta, refinement vectors (moves with its problem)
+    long long L = 0;
+    CPtrs cp;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -388,6 +819,100 @@ int batch_solve(cvxb_batch *b) {
     return 0;
 }
 
+// ---- cone path ----
+bool cone_path(const cvxb_batch *b) { return !b->qdims.empty() || (b->refinement > 0 && b->m > 0); }
+
+// the offset table and the buffers only the cone path uses
+int cone_alloc(cvxb_batch *b) {
+    if (b->cst.p) return 0;
+    const int nq = (int)b->qdims.size();
+    std::vector<int> off(nq + 1, b->ml);
+    for (int k = 0; k < nq; ++k) off[k + 1] = off[k] + b->qdims[k];
+    CVXB_TRY(b->qoff.alloc(nq + 1));
+    CVXB_CUDA(cudaMemcpy(b->qoff.p, off.data(), (nq + 1) * sizeof(int), cudaMemcpyHostToDevice));
+    CVXB_TRY(b->Gs.alloc((size_t)b->B * b->sG));
+    // state row: v (sum q) | beta (nq) | wx wx2 (n) | wz ws wz2 ws2 wz3 (m); every piece starts 16-byte aligned
+    auto ev = [](long long x) { return (x + 1) & ~1LL; };
+    const long long sumq = b->m - b->ml, n2 = ev(b->n), m2 = ev(b->m);
+    b->L = ev(sumq) + ev(nq) + 2 * n2 + 5 * m2;
+    CVXB_TRY(b->cst.alloc((size_t)b->B * b->L));
+    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * b->L * sizeof(double)));
+    CPtrs &c = b->cp;
+    double *r = b->cst.p;
+    c.v = r; r += ev(sumq);
+    c.beta = r; r += ev(nq);
+    c.wx = r; r += n2; c.wx2 = r; r += n2;
+    c.wz = r; r += m2; c.ws = r; r += m2; c.wz2 = r; r += m2; c.ws2 = r; r += m2; c.wz3 = r;
+    c.ml = b->ml; c.nq = nq; c.qoff = b->qoff.p; c.L = b->L;
+    return 0;
+}
+
+// K = P + Gs' Gs with Gs = W^{-T} G (misc.py:1267-1282), then its Cholesky factor
+int cone_factor(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    kc_build_gs<<<dim3((b->n + 7) / 8, b->Bact), 256, 0, st>>>(b->cp, b->G.p, b->Gs.p, b->ldg, b->sG);
+    count_launch();
+    b->syrk_path = 1;
+    GemmDesc g;
+    g.M = b->n; g.N = b->n; g.K = b->m;
+    g.X = b->Gs.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
+    g.Y = b->Gs.p; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
+    g.D = b->P.p; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
+    g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
+    g.lower_only = true; g.batch = b->Bact;
+    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
+    CVXB_TRY(dmma_gemm(g, st));
+    if (b->B == 1) {
+        CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
+    } else {
+        CVXB_TRY(potrf_lower_batched(b->n, b->K.p, (int)b->ldk, b->sK, b->inv.p, b->sInv, b->Bact, b->d_info.p,
+                                     b->panel.p, (b->n + 1) & ~1, st));
+    }
+    return 0;
+}
+
+// (x, bzp) := solution of the reduced KKT system on Gs; on entry x = bx (slot k at x + k*sx), bzp = W^{-T} bz
+int cone_solve(cvxb_batch *b, double *x, long long sx) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact;
+    GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = m; gt.sy = sx;
+    CVXB_TRY(gemv_t(m, n, b->Gs.p, b->ldg, nullptr, b->p.bzp, 1.0, 1.0, x, st, gt));
+    CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, b->cw, st, B, b->sK, b->sInv, sx));
+    GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = sx; gn.sy = m;
+    CVXB_TRY(gemv_n(m, n, b->Gs.p, b->ldg, nullptr, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
+    return 0;
+}
+
+// f4_no_ir (coneprog.py:2288-2316) on (x, z, s); acc: add the result to (dx, dz, ds) (the refinement step)
+int cone_f4_no_ir(cvxb_batch *b, double *x, long long sx, double *z, long long sz, double *s, long long ss, int acc) {
+    const int B = b->Bact;
+    kc_f4_pre<<<B, 256, 0, b->st>>>(b->cp, z, sz, s, ss); count_launch();
+    CVXB_TRY(cone_solve(b, x, sx));
+    kc_f4_post<<<B, 256, 0, b->st>>>(b->cp, x, sx, z, sz, s, ss, acc); count_launch();
+    return 0;
+}
+
+// f4 (coneprog.py:2330-2347): f4_no_ir on (dx, dz, ds), then `refinement` correction steps from the residual
+int cone_f4(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact;
+    const CPtrs &c = b->cp;
+    const long long L = b->L;
+    CVXB_TRY(cone_f4_no_ir(b, c.p.dx, n, c.p.dz, m, c.p.ds, m, 0));
+    for (int r = 0; r < b->refinement; ++r) {
+        kc_res<<<B, 256, 0, st>>>(c); count_launch();
+        GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, c.p.dx, -1.0, 1.0, c.wx2, st, gP));
+        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, c.wz3, -1.0, 1.0, c.wx2, st, gt));
+        GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, c.p.dx, -1.0, 1.0, c.wz2, b->gemv_ws.p, st, gn));
+        CVXB_TRY(cone_f4_no_ir(b, c.wx2, L, c.wz2, L, c.ws2, L, 1));
+    }
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -397,7 +922,7 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     *out = nullptr;
     CVXB_TRY(check_device(device));
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
-    b->device = device; b->B = nprob; b->n = n; b->m = m;
+    b->device = device; b->B = nprob; b->n = n; b->m = m; b->ml = m;
     b->i8_mode = ozaki_mode();
     b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
@@ -438,6 +963,39 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
     *out = b.release();
+    return 0;
+}
+
+int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
+    if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
+    *out = nullptr;
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("batch_create_cones: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
+        return CVXB_E_ARG;
+    }
+    long long m = dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("batch_create_cones: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
+        m += dims->q[k];
+    }
+    if (m > (1LL << 30)) { set_error("batch_create_cones: too many cone rows"); return CVXB_E_ARG; }
+    if (dims->ns > 0) { set_error("batch_create_cones: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    cvxb_batch *b = nullptr;
+    CVXB_TRY(cvxb_batch_create(&b, nprob, n, (int)m, device));
+    std::unique_ptr<cvxb_batch> own(b);
+    b->ml = dims->ml;
+    b->qdims.assign(dims->q, dims->q + dims->nq);
+    b->refinement = dims->nq > 0 ? 1 : 0;        // coneqp's default (coneprog.py:1862-1865)
+    if (cone_path(b)) CVXB_TRY(cone_alloc(b));
+    *out = own.release();
+    return 0;
+}
+
+int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
+    if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    b->refinement = refinement;
+    if (cone_path(b)) CVXB_TRY(cone_alloc(b));
     return 0;
 }
 
@@ -482,6 +1040,10 @@ static int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     a.n = b->n; a.me = b->m > 0 ? b->m : 1; a.Btot = b->B;
     k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs.p);
     count_launch();
+    if (b->cst.p) {
+        kc_swap_rows<<<dim3(8, np), 256, 0, b->st>>>(b->cst.p, b->L, b->d_pairs.p);
+        count_launch();
+    }
     // `pairs` is pageable host memory: the copy above is staged before cudaMemcpyAsync returns
     return 0;
 }
@@ -503,11 +1065,99 @@ static int restore_order(cvxb_batch *b) {
     return 0;
 }
 
+// the lock-step loop of cvxb_batch_solve for the cone path: same residuals, stopping rule and compaction; the
+// scaling, the Newton directions (with refinement) and the update are the kc_* kernels
+static int cone_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, T = 256;
+    int B = b->B;
+    b->Bact = B;
+    Ptrs &p = b->p;
+    CPtrs &cp = b->cp;
+    cp.p = p; cp.refinement = b->refinement;
+    GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
+    GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
+    GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
+    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
+    CVXB_CUDA(cudaEventRecord(b->e0, st));
+    // ---- starting point: W = I ----
+    k_init_rhs<<<B, T, 0, st>>>(p); count_launch();
+    kc_init_w<<<B, T, 0, st>>>(cp); count_launch();
+    CVXB_TRY(cone_factor(b));
+    kc_scale_bz<<<B, T, 0, st>>>(cp); count_launch();
+    CVXB_TRY(cone_solve(b, p.dx, n));
+    kc_init_point<<<B, T, 0, st>>>(cp); count_launch();
+    CVXB_LAUNCH_CHECK();
+    {
+        // a singular first factorisation is the reference's "Rank([P; G]) < n" ValueError
+        std::vector<int> info(B);
+        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaStreamSynchronize(st));
+        for (int i = 0; i < B; ++i)
+            if (info[i] > 0) {
+                set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
+                return CVXB_E_ARG;
+            }
+    }
+    std::vector<int> flags(B), pairs;
+    int it = 0;
+    for (it = 0; it <= maxiters; ++it) {
+        // residuals (:2169-2186): row-wise, so the 'l' kernels serve every cone row
+        k_res_begin<<<B, T, 0, st>>>(p); count_launch();
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
+        k_res_dots<<<B, T, 0, st>>>(p); count_launch();
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_stats<<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p); count_launch();
+        int ndone = 0;
+        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaStreamSynchronize(st));
+        if (ndone >= B) break;
+        if (ndone > 0 && b->compact && b->B > 1) {
+            const int nb = B - ndone;
+            pairs.clear();
+            int j = B - 1;
+            for (int i = 0; i < nb; ++i) {
+                if (!flags[i]) continue;
+                while (flags[j]) --j;
+                pairs.push_back(i); pairs.push_back(j);
+                std::swap(b->perm[i], b->perm[j]);
+                --j;
+            }
+            CVXB_TRY(swap_slots(b, pairs));
+            b->permuted = true;
+            B = nb;
+            b->Bact = B;
+            gP.batch = gGt.batch = gGn.batch = B;
+        }
+        kc_scaling<<<B, T, 0, st>>>(cp, it == 0 ? 1 : 0); count_launch();
+        CVXB_TRY(cone_factor(b));
+        for (int i = 0; i < 2; ++i) {
+            kc_dir_rhs<<<B, T, 0, st>>>(cp, i); count_launch();
+            CVXB_TRY(cone_f4(b));
+            kc_dir_post<<<B, T, 0, st>>>(cp, i); count_launch();
+        }
+        kc_update<<<B, T, 0, st>>>(cp, b->d_info.p, it); count_launch();
+        CVXB_LAUNCH_CHECK();
+    }
+    b->iters_run = it;
+    b->Bact = b->B;
+    CVXB_CUDA(cudaEventRecord(b->e1, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    float t = 0;
+    cudaEventElapsedTime(&t, b->e0, b->e1);
+    b->solve_ms = t;
+    return 0;
+}
+
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     if (!b || !b->loaded) { set_error("batch_solve: load the problems first"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     cudaStream_t st = b->st;
     CVXB_TRY(restore_order(b));
+    if (cone_path(b)) return cone_batch_solve(b, maxiters, abstol, reltol, feastol);
     const int n = b->n, m = b->m, T = 256;
     int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
     b->Bact = B;

@@ -213,10 +213,20 @@ int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const d
 
 /* ---- batch of independent dense QPs (BASELINE config 4): one problem per
  * CTA-group, lock-step primal-dual IPM fully on device (oracle: a Python loop
- * over solvers.qp).  Problems are  min 1/2 x'P x + q'x  s.t.  G x <= h. */
+ * over coneqp).  Problems are  min 1/2 x'P x + q'x  s.t.  G x + s = h, s in the
+ * cone product  'l' x 'q'[0] x ... ; all problems share n and the dims.
+ * cvxb_batch_create(.., m, ..) is dims = {'l': m}: G x <= h.
+ * A batch with 'q' cones or refinement > 0 runs the cone path (Gs = W^{-T} G is
+ * materialised per problem: nprob * cdim * n more doubles); an 'l'-only batch
+ * without refinement runs the fused-scaling path. */
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device);
+/* batch of  min 1/2 x'Px + q'x  s.t.  G x + s = h,  s in 'l' x 'q' cones  (B x coneqp, coneprog.py:1440).
+ * dims->mnl != 0, a cone order q[k] < 1: CVXB_E_ARG; dims->ns > 0: CVXB_E_UNSUP. */
+int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device);
+/* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
+int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);
-/* P: nprob x (n x n, ld n); q: nprob x n; G: nprob x (m x n column-major, ld m); h: nprob x m */
+/* P: nprob x (n x n, ld n); q: nprob x n; G: nprob x (m x n column-major, ld m); h: nprob x m; m = cdim */
 int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
                     const double *h, int space);
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol);
