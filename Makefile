@@ -11,7 +11,7 @@ PYINC := $(shell $(PYTHON) -c "import sysconfig; print(sysconfig.get_paths()['in
 PYEXT := $(shell $(PYTHON) -c "import sysconfig; print(sysconfig.get_config_var('EXT_SUFFIX'))")
 EXT := cvxopt_b200/_misc_solvers$(PYEXT)
 
-all: $(LIB) $(EXT) tools/dmma_rate
+all: $(LIB) $(EXT) tools/dmma_rate tools/syrk_feed
 
 $(EXT): $(SRC)/_misc_solvers.c include/cvxopt_b200.h $(LIB)
 	gcc -O2 -fPIC -shared -Wall -I$(PYINC) $< -o $@ -Lcvxopt_b200 -lcvxopt_b200 -Wl,-rpath,'$$ORIGIN'
@@ -26,6 +26,10 @@ $(LIB): $(OBJ)
 tools/dmma_rate: tools/dmma_rate.cu
 	$(NVCC) $(ARCH) -O3 -std=c++17 -o $@ $<
 
+# standalone probe of the SYRK's L2 -> shared-memory operand feed (no DMMAs); see tools/README.md
+tools/syrk_feed: tools/syrk_feed.cu
+	$(NVCC) $(ARCH) -O3 -std=c++17 -o $@ $<
+
 clean:
-	rm -f $(OBJ) $(LIB) $(EXT) tools/dmma_rate
+	rm -f $(OBJ) $(LIB) $(EXT) tools/dmma_rate tools/syrk_feed
 .PHONY: all clean

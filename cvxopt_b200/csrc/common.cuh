@@ -198,6 +198,51 @@ __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N));
 }
 
+// mbarrier ring of a producer / consumer pipeline: `full` barriers complete when their bulk / TMA copies have
+// landed (expect_tx), `empty` ones when every consumer has arrived; waiters pass the parity of the phase they wait for
+__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
+                 : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "WAIT_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE_%=;\n\t"
+        "bra WAIT_%=;\n\t"
+        "DONE_%=:\n\t}" ::"r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+}
+// contiguous global -> shared copy (16-byte aligned, multiple of 16 bytes) that completes `bytes` on bar
+__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+        ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
+        : "memory");
+}
+// TMA box loads through a CUtensorMap kernel parameter (`map` is its generic address); the box lands in shared
+// memory as the map's swizzle lays it out, elements outside the tensor are zero, and the whole box's bytes
+// complete on bar
+__device__ __forceinline__ void tma_load_1d(void *dst, const void *map, int c0, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.1d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2}], [%3];"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(smem_u32(bar))
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(void *dst, const void *map, int c0, int c1, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+        : "memory");
+}
+
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -24,11 +24,18 @@
 //     issue before the DMMAs of step kk (no DMUL->DMMA dependency stall)
 //   * per-thread copy descriptors hoisted out of the k loop
 //
+// Single K-major lower-triangle SYRKs with 16-byte aligned operands and even leading dimensions (the KKT
+// normal equations, A'A, Asct'Asct, cvxb_syrk_scaled) run on syrk_tma_kernel instead: 128x128 tiles, one
+// CTA per SM, operands fed by TMA through an mbarrier ring by a producer warpgroup (see its comment).  It keeps
+// this kernel's warp tiles, fragments and k order, so the two agree bit for bit outside the split-K tail.
+//
 // MMA roles are swapped w.r.t. the matrix: the MMA "m" index runs over C's columns
 // (Y operand), the "n" index over C's rows (X operand), so each thread's accumulator
 // pair is two consecutive ROWS of a column-major C (one 16-byte access).  One m16n8k4
 // covers the column fragments cf = 2mf and 2mf+1 (8 columns apart) of a row fragment.
 #include "common.cuh"
+#include <cuda.h>
+#include <cudaTypedefs.h>
 
 namespace cvxb {
 
@@ -69,9 +76,11 @@ struct KParams {
     int band;               // > 0: band-major tile order (lower_only, long K), width in c tiles
 };
 
-// first r tile that intersects the lower triangle for c tile `tc`
-__device__ __host__ __forceinline__ int first_tr(int tc) { return (tc * BC) / BR; }
+// first r tile that intersects the lower triangle for c tile `tc` of width `tcols`
+__device__ __host__ __forceinline__ int first_tr(int tc, int tcols) { return (tc * tcols) / BR; }
 
+// unit t -> (r tile, c tile) for c tiles TC columns wide
+template <int TC>
 __device__ __forceinline__ void decode_tile(const KParams &p, int t, int &tr, int &tc) {
     int c = p.ct_begin;
     if (p.lower_only && p.band > 0) {
@@ -83,13 +92,13 @@ __device__ __forceinline__ void decode_tile(const KParams &p, int t, int &tr, in
         while (true) {
             cb_end = min(c + p.band, p.ct_end);
             int cnt = 0;
-            for (int cc = c; cc < cb_end; ++cc) cnt += max(0, p.nTr - first_tr(cc));
+            for (int cc = c; cc < cb_end; ++cc) cnt += max(0, p.nTr - first_tr(cc, TC));
             if (t < cnt) break;
             t -= cnt;
             c = cb_end;
         }
-        for (int r = first_tr(c);; ++r) {
-            const int cmax = min(cb_end - 1, (r * BR + BR - 1) / BC);   // last live c tile of this row
+        for (int r = first_tr(c, TC);; ++r) {
+            const int cmax = min(cb_end - 1, (r * BR + BR - 1) / TC);   // last live c tile of this row
             const int cntr = cmax - c + 1;
             if (t < cntr) { tr = r; tc = c + t; return; }
             t -= cntr;
@@ -97,12 +106,12 @@ __device__ __forceinline__ void decode_tile(const KParams &p, int t, int &tr, in
     }
     if (p.lower_only) {
         while (true) {
-            int cnt = p.nTr - first_tr(c);
+            int cnt = p.nTr - first_tr(c, TC);
             if (t < cnt) break;
             t -= cnt;
             ++c;
         }
-        tr = first_tr(c) + t;
+        tr = first_tr(c, TC) + t;
         tc = c;
     } else {
         tc = c + t / p.nTr;
@@ -183,7 +192,7 @@ __global__ void __launch_bounds__(THREADS, 2) dmma_gemm_kernel(const KParams p) 
         split = (u - p.full_tiles) % p.S;
     }
     int tr, tc;
-    decode_tile(p, tile, tr, tc);
+    decode_tile<BC>(p, tile, tr, tc);
     const bool is_split = (u >= p.full_tiles) && (p.S > 1);
     int kbeg = 0, kend = p.K;
     if (is_split) {
@@ -472,21 +481,260 @@ __global__ void __launch_bounds__(THREADS, 2) dmma_gemm_kernel(const KParams p) 
     }
 }
 
-// sums the S split-K partials of the remainder tiles in a fixed order (deterministic)
+// ---- K-major lower-triangle SYRK on 128x128 tiles: TMA-fed, warp-specialised ----
+// One CTA per SM owns a 128x128 tile of C: warps 0-7 are the 2x4 grid of 64x32 warp tiles of dmma_gemm_kernel
+// (same fragments, same k order, w applied to the column fragments, same pre_d start), so every element outside
+// the split-K tail is bit-identical to the 128x64 kernel's; warps 8-11 are the producer warpgroup, which hands
+// its registers to the consumers (setmaxnreg: 64 accumulators and two fragment sets per consumer thread do not fit
+// the 168 registers a 9-warp CTA gets, because one SM sub-partition holds 3 of its warps).  Per 16-wide k tile it
+// issues one 2D TMA box {16 k, 128 rows} per operand and a 1D box of w into a T_STAGES-deep mbarrier ring;
+// consumers release a stage through its empty barrier, so the main loop has no CTA-wide barrier, and TMA's zero
+// fill outside the tensor replaces CopyPlan's row and k-tail masking.  A 128x128 tile moves 256 operand rows
+// per k for 2*128*128 flop (16 flop/B against 10.7 for 128x64), so a SYRK reads a third less from L2.
+//
+// Shared-memory map of an operand panel (128-byte swizzle): row r (a tile row of X, or column of Y) is 128 bytes
+// = its 16 k values, and the 16-byte chunk c = k/2 of row r sits at chunk c ^ (r & 7).  A fragment load of one
+// warp reads rows idx = 8j + g4 (g4 = lane/4) at k = 4kk + t4 (t4 = lane%4): lanes t4 < 2 read chunk 2kk and
+// lanes t4 >= 2 chunk 2kk+1, which the eight g4 spread over all eight chunk positions, so each half-warp is
+// one 128-byte wavefront (2 per load, the minimum for 256 bytes).  The double offset is
+//   16 idx + 4 (kk ^ (g4 >> 1)) + 2 ((t4 >> 1) ^ (g4 & 1)) + (t4 & 1).
+constexpr int TB = 128;                                  // tile edge (rows and columns of C)
+constexpr int T_STAGES = 6;
+constexpr int T_CONSUMERS = 8;                           // 2 x 4 warps of 64 x 32
+constexpr int T_THREADS = 32 * (T_CONSUMERS + 4);        // + the producer warpgroup
+constexpr int T_REGS_PRODUCER = 40, T_REGS_CONSUMER = 232;   // 128 * 40 + 256 * 232 <= 65536
+constexpr int T_PANEL = TB * BK;                         // doubles of one operand panel (16 KB)
+constexpr int T_SMEM = T_STAGES * (2 * T_PANEL + BK) * 8 + 2 * T_STAGES * 8 + 1024;   // + barriers, alignment
+constexpr int T_TILE_ELEMS = TB * TB;
+constexpr int T_WS_TILES = 4 * kNumSMs;                  // split-K workspace capacity (tiles)
+
+__global__ void __launch_bounds__(T_THREADS, 1)
+syrk_tma_kernel(const KParams p, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmY,
+                const __grid_constant__ CUtensorMap tmW) {
+    extern __shared__ unsigned char t_smem_raw[];
+    // 1024-byte aligned (the 128-byte swizzle repeats every 8 rows); offset from the array so that the compiler
+    // keeps shared-memory loads
+    double *sm = reinterpret_cast<double *>(t_smem_raw + ((1024u - (smem_u32(t_smem_raw) & 1023u)) & 1023u));
+    double *sw = sm + T_STAGES * 2 * T_PANEL;            // w of stage s at sw + s * BK
+    uint64_t *full = reinterpret_cast<uint64_t *>(sw + T_STAGES * BK), *empty = full + T_STAGES;
+    // warp index through a shuffle, so the compiler knows the role branches are warp-uniform
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+
+    const int u = blockIdx.x;
+    int tile, split = 0;
+    if (u < p.full_tiles) {
+        tile = u;
+    } else {
+        tile = p.full_tiles + (u - p.full_tiles) / p.S;
+        split = (u - p.full_tiles) % p.S;
+    }
+    int tr, tc;
+    decode_tile<TB>(p, tile, tr, tc);
+    const bool is_split = ((int)blockIdx.x >= p.full_tiles) && (p.S > 1);
+    int kbeg = 0, kend = p.K;
+    if (is_split) {
+        kbeg = split * p.kchunk;
+        kend = min(p.K, kbeg + p.kchunk);
+    }
+    const int r0 = tr * TB, c0 = tc * TB;
+    const int nr = min(TB, p.M - r0), nc = min(TB, p.N - c0);
+    const bool has_w = (p.w != nullptr);
+    const int ktiles = (kend - kbeg + BK - 1) / BK;
+
+    if (tid == 0) {
+        for (int s = 0; s < T_STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, T_CONSUMERS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp >= T_CONSUMERS) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T_REGS_PRODUCER));
+        if (warp == T_CONSUMERS && lane == 0) {
+            // ===== producer: one box per operand (and one of w) per k tile =====
+            const uint32_t bytes = (uint32_t)(2 * T_PANEL + (has_w ? BK : 0)) * 8u;
+            for (int kt = 0; kt < ktiles; ++kt) {
+                const int s = kt % T_STAGES;
+                if (kt >= T_STAGES) mbar_wait(empty + s, (uint32_t)(kt / T_STAGES - 1) & 1u);
+                mbar_expect_tx(full + s, bytes);
+                const int k = kbeg + kt * BK;
+                tma_load_2d(sm + s * 2 * T_PANEL, &tmX, k, r0, full + s);
+                tma_load_2d(sm + s * 2 * T_PANEL + T_PANEL, &tmY, k, c0, full + s);
+                if (has_w) tma_load_1d(sw + s * BK, &tmW, k, full + s);
+            }
+        }
+        return;
+    }
+
+    // ===== consumers: warp (wr, wc) owns rows 64 wr .. +63 and columns 32 wc .. +31 of the tile =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T_REGS_CONSUMER));
+    const int wr = warp & 1, wc = warp >> 1;
+    const int g4 = lane >> 2, t4 = lane & 3;
+    double acc[4][8][2];
+    const bool pre_d = p.vec_c && (nr == TB) && (nc == TB) && !(c0 + TB - 1 > r0) && !is_split &&
+                       p.beta != 0.0 && p.D != nullptr && (p.alpha == 1.0 || p.alpha == -1.0) && ((p.ldd & 1) == 0);
+    if (pre_d) {
+        const double sc = p.beta / p.alpha;
+        const double *Dt = p.D + r0 + (long long)c0 * p.ldd;
+#pragma unroll
+        for (int cf = 0; cf < 4; ++cf) {
+            const int cl = wc * 32 + cf * 8 + g4;
+#pragma unroll
+            for (int rf = 0; rf < 8; ++rf) {
+                const int rl = wr * 64 + rf * 8 + t4 * 2;
+                const double2 dv = *reinterpret_cast<const double2 *>(Dt + rl + (long long)cl * p.ldd);
+                acc[cf][rf][0] = sc * dv.x; acc[cf][rf][1] = sc * dv.y;
+            }
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+    }
+
+    if (r0 + wr * 64 + 63 < c0 + wc * 32) {
+        // this warp's 64x32 block lies strictly above the diagonal: it only takes part in the stage releases
+        for (int kt = 0; kt < ktiles; ++kt) {
+            const int s = kt % T_STAGES;
+            mbar_wait(full + s, (uint32_t)(kt / T_STAGES) & 1u);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty + s);
+        }
+    } else if (ktiles > 0) {
+        // swizzled fragment offsets (see the address map above) at kk = 0; kk adds 4 (kk ^ q)
+        const int q = g4 >> 1;
+        const int lo = 2 * ((t4 >> 1) ^ (g4 & 1)) + (t4 & 1);
+        const int xo = (wr * 64 + g4) * BK + lo;
+        const int yo = T_PANEL + (wc * 32 + g4) * BK + lo;
+        double a[2][4], bf[2][8];
+        // fragments of step kk of stage s into buffer b (the column fragments scaled by w)
+        auto load = [&](int s, int kk, int b) {
+            const double *st = sm + s * 2 * T_PANEL + 4 * (kk ^ q);
+#pragma unroll
+            for (int cf = 0; cf < 4; ++cf) a[b][cf] = st[yo + cf * 8 * BK];
+#pragma unroll
+            for (int rf = 0; rf < 8; ++rf) bf[b][rf] = st[xo + rf * 8 * BK];
+            if (has_w) {
+                const double wv = sw[s * BK + kk * 4 + t4];
+#pragma unroll
+                for (int cf = 0; cf < 4; ++cf) a[b][cf] *= wv;
+            }
+        };
+        mbar_wait(full, 0u);
+        load(0, 0, 0);
+        for (int kt = 0; kt < ktiles; ++kt) {
+            const int s = kt % T_STAGES;
+#pragma unroll
+            for (int kk = 0; kk < BK / 4; ++kk) {
+                const int cur = kk & 1, nxt = cur ^ 1;
+                if (kk + 1 < BK / 4) load(s, kk + 1, nxt);
+#pragma unroll
+                for (int mf = 0; mf < 2; ++mf)
+#pragma unroll
+                    for (int rf = 0; rf < 8; ++rf)
+                        dmma16x8x4(acc[2 * mf][rf][0], acc[2 * mf][rf][1], acc[2 * mf + 1][rf][0],
+                                   acc[2 * mf + 1][rf][1], a[cur][2 * mf], a[cur][2 * mf + 1], bf[cur][rf]);
+                if (kk + 1 == BK / 4 && kt + 1 < ktiles) {
+                    // the next stage's first fragments load under this step's DMMAs
+                    const int s1 = (kt + 1) % T_STAGES;
+                    mbar_wait(full + s1, (uint32_t)((kt + 1) / T_STAGES) & 1u);
+                    load(s1, 0, nxt);
+                }
+            }
+            // every fragment of stage s is in registers (this tile's last DMMAs consumed them)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty + s);
+        }
+    }
+
+    // ---- epilogue (the expressions of dmma_gemm_kernel's, so that the results match it bit for bit) ----
+    if (is_split) {
+        double *ws = p.ws + ((long long)(tile - p.full_tiles) * p.S + split) * T_TILE_ELEMS;
+#pragma unroll
+        for (int cf = 0; cf < 4; ++cf)
+#pragma unroll
+            for (int rf = 0; rf < 8; ++rf) {
+                const int rl = wr * 64 + rf * 8 + t4 * 2;
+                const int cl = wc * 32 + cf * 8 + g4;
+                *reinterpret_cast<double2 *>(ws + rl + cl * TB) = make_double2(acc[cf][rf][0], acc[cf][rf][1]);
+            }
+        return;
+    }
+    double *C = p.C;
+    const double *D = p.D;
+    const bool diag = (c0 + TB - 1 > r0);                 // tile touches the diagonal
+    const bool use_d = (p.beta != 0.0);
+    if (p.vec_c && (nr == TB) && (nc == TB) && !diag) {
+        // full interior tile, 16-byte accesses
+#pragma unroll
+        for (int cf = 0; cf < 4; ++cf) {
+            const int cl = wc * 32 + cf * 8 + g4;
+#pragma unroll
+            for (int rf = 0; rf < 8; ++rf) {
+                const int rl = wr * 64 + rf * 8 + t4 * 2;
+                double2 v;
+                if (use_d && !pre_d) {
+                    const double2 dv = *reinterpret_cast<const double2 *>(D + (r0 + rl) + (long long)(c0 + cl) * p.ldd);
+                    v = make_double2(p.alpha * acc[cf][rf][0] + p.beta * dv.x,
+                                     p.alpha * acc[cf][rf][1] + p.beta * dv.y);
+                } else {
+                    v = make_double2(p.alpha * acc[cf][rf][0], p.alpha * acc[cf][rf][1]);
+                }
+                *reinterpret_cast<double2 *>(C + (r0 + rl) + (long long)(c0 + cl) * p.ldc) = v;
+            }
+        }
+        return;
+    }
+    // edge / diagonal tiles (C may alias D: a column fragment's D values are all loaded before it is stored)
+#pragma unroll
+    for (int cf = 0; cf < 4; ++cf) {
+        const int cl = wc * 32 + cf * 8 + g4;
+        if (cl >= nc) continue;
+        const long long c = c0 + cl;
+        double dv[8][2];
+#pragma unroll
+        for (int rf = 0; rf < 8; ++rf) {
+            const int rl = wr * 64 + rf * 8 + t4 * 2;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const long long r = r0 + rl + e;
+                const bool ok = use_d && (rl + e < nr) && !(diag && r < c);
+                dv[rf][e] = ok ? D[r + c * p.ldd] : 0.0;
+            }
+        }
+#pragma unroll
+        for (int rf = 0; rf < 8; ++rf) {
+            const int rl = wr * 64 + rf * 8 + t4 * 2;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                if (rl + e >= nr) continue;
+                const long long r = r0 + rl + e;
+                if (diag && r < c) continue;
+                double v = p.alpha * acc[cf][rf][e];
+                if (use_d) v += p.beta * dv[rf][e];
+                C[r + c * p.ldc] = v;
+            }
+        }
+    }
+}
+
+// sums the S split-K partials of the remainder tiles (BR x TC each) in a fixed order (deterministic)
+template <int TC>
 __global__ void __launch_bounds__(256) splitk_reduce_kernel(const KParams p) {
+    constexpr int ELEMS = BR * TC;
     const int tile = p.full_tiles + blockIdx.x;
     int tr, tc;
-    decode_tile(p, tile, tr, tc);
-    const int r0 = tr * BR, c0 = tc * BC;
-    const int nr = min(BR, p.M - r0), nc = min(BC, p.N - c0);
-    const double *ws = p.ws + (long long)blockIdx.x * p.S * TILE_ELEMS;
-    for (int e = blockIdx.y * blockDim.x + threadIdx.x; e < TILE_ELEMS; e += gridDim.y * blockDim.x) {
+    decode_tile<TC>(p, tile, tr, tc);
+    const int r0 = tr * BR, c0 = tc * TC;
+    const int nr = min(BR, p.M - r0), nc = min(TC, p.N - c0);
+    const double *ws = p.ws + (long long)blockIdx.x * p.S * ELEMS;
+    for (int e = blockIdx.y * blockDim.x + threadIdx.x; e < ELEMS; e += gridDim.y * blockDim.x) {
         const int rl = e % BR, cl = e / BR;
         if (rl >= nr || cl >= nc) continue;
         const long long r = r0 + rl, c = c0 + cl;
         if (p.lower_only && r < c) continue;
         double s = 0.0;
-        for (int k = 0; k < p.S; ++k) s += ws[(long long)k * TILE_ELEMS + e];
+        for (int k = 0; k < p.S; ++k) s += ws[(long long)k * ELEMS + e];
         double v = p.alpha * s;
         if (p.beta != 0.0) v += p.beta * p.D[r + c * p.ldd];
         p.C[r + c * p.ldc] = v;
@@ -509,9 +757,67 @@ int launch_inst(const KParams &p, dim3 grid, cudaStream_t st) {
     return 0;
 }
 
+// cuTensorMapEncodeTiled from the driver the runtime loaded (the library links the runtime only)
+PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+    static PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
+        void *f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess) {
+            cudaGetLastError();
+            f = nullptr;
+        }
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+    }();
+    return fn;
+}
+
+// tensor map of a K-major operand (rows x K, row stride ld doubles) in boxes of {BK k, TB rows}, 128-byte swizzle;
+// rank 1 (rows == 0): the K-vector w in boxes of BK
+int encode_operand(CUtensorMap &m, const double *base, long long ld, int K, int rows) {
+    PFN_cuTensorMapEncodeTiled_v12000 enc = tensor_map_encoder();
+    if (!enc) {
+        set_error("dmma_gemm: cuTensorMapEncodeTiled is not available from the driver");
+        return CVXB_E_CUDA;
+    }
+    const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(double)};
+    const cuuint32_t box[2] = {BK, TB};
+    const cuuint32_t estr[2] = {1, 1};
+    const CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, rows ? 2 : 1, const_cast<double *>(base), dims, strides,
+                           box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                           rows ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("dmma_gemm: cuTensorMapEncodeTiled -> CUresult %d", (int)r);
+        return CVXB_E_CUDA;
+    }
+    return 0;
+}
+
+int launch_tma(const KParams &p, dim3 grid, cudaStream_t st) {
+    CUtensorMap tx, ty, tw;
+    CVXB_TRY(encode_operand(tx, p.X, p.ldx, p.K, p.M));
+    CVXB_TRY(encode_operand(ty, p.Y, p.ldy, p.K, p.N));
+    if (p.w) CVXB_TRY(encode_operand(tw, p.w, 0, p.K, 0));
+    else tw = tx;                                        // not read
+    static DeviceOnce once;
+    if (const unsigned long long bit = once.pending()) {
+        CVXB_CUDA(cudaFuncSetAttribute(syrk_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM));
+        once.mark(bit);
+    }
+    syrk_tma_kernel<<<grid, T_THREADS, T_SMEM, st>>>(p, tx, ty, tw);
+    count_launch();
+    CVXB_LAUNCH_CHECK();
+    return 0;
+}
+
 }  // namespace
 
-size_t dmma_gemm_splitk_ws_doubles() { return (size_t)SPLITK_WS_TILES * TILE_ELEMS; }
+size_t dmma_gemm_splitk_ws_doubles() {
+    const size_t a = (size_t)SPLITK_WS_TILES * TILE_ELEMS, b = (size_t)T_WS_TILES * T_TILE_ELEMS;
+    return a > b ? a : b;
+}
 int dmma_gemm_tile_cols() { return BC; }
 
 int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
@@ -520,6 +826,16 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
         set_error("dmma_gemm: bad arguments");
         return CVXB_E_ARG;
     }
+    auto aligned = [](const void *ptr, long long ld) {
+        return ((uintptr_t)ptr % 16 == 0) && (ld % 2 == 0);
+    };
+    const int nTc = (g.N + BC - 1) / BC;
+    // single K-major lower-triangle SYRKs over the whole matrix run on the TMA kernel, which needs 16-byte aligned
+    // operands and row strides; the rest (odd leading dimensions, batches, Cholesky updates) on dmma_gemm_kernel
+    const bool tma = g.x_kmajor && g.y_kmajor && g.lower_only && g.batch == 1 && g.K > 0 && g.ct_begin <= 0 &&
+                     g.ct_end >= nTc && aligned(g.X, g.ldx) && aligned(g.Y, g.ldy) && ((uintptr_t)g.w % 16 == 0);
+    const int tcols = tma ? TB : BC;                     // c-tile width
+    const int wave = tma ? kNumSMs : CTAS_PER_WAVE;      // resident CTAs
     KParams p;
     p.M = g.M; p.N = g.N; p.K = g.K;
     p.X = g.X; p.ldx = g.ldx; p.Y = g.Y; p.ldy = g.ldy; p.w = g.w;
@@ -527,16 +843,17 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     p.alpha = g.alpha; p.beta = (g.D ? g.beta : 0.0);
     p.lower_only = g.lower_only ? 1 : 0;
     p.nTr = (g.M + BR - 1) / BR;
-    const int nTc = (g.N + BC - 1) / BC;
     p.ct_begin = g.ct_begin < 0 ? 0 : g.ct_begin;
     p.ct_end = g.ct_end > nTc ? nTc : g.ct_end;
     if (p.ct_begin >= p.ct_end) return 0;
+    if (tma) p.ct_end = (g.N + TB - 1) / TB;
     p.sX = g.sX; p.sY = g.sY; p.sW = g.sW; p.sD = g.sD; p.sC = g.sC;
-    p.band = (p.lower_only && g.K >= 1024 && g.batch == 1) ? 16 : 0;
+    // bands of 1024 columns
+    p.band = (p.lower_only && g.K >= 1024 && g.batch == 1) ? 1024 / tcols : 0;
     long long T = 0;
     if (p.lower_only) {
         for (int c = p.ct_begin; c < p.ct_end; ++c) {
-            int cnt = p.nTr - first_tr(c);
+            int cnt = p.nTr - first_tr(c, tcols);
             T += cnt > 0 ? cnt : 0;
         }
     } else {
@@ -548,17 +865,17 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     if (g.splitk_ws && g.batch == 1 && g.K >= 1024) {
         // the tiles of the last, partial wave are split along K so that the tail costs
         // ceil(rem*S / wave) / S of a tile time instead of a whole one
-        int full = (int)(T / CTAS_PER_WAVE) * CTAS_PER_WAVE;
+        int full = (int)(T / wave) * wave;
         int rem = (int)T - full;
         if (rem > 0) {
             int maxS = g.K / 512;
             if (maxS > 18) maxS = 18;
-            const int cap_units = SPLITK_WS_TILES;           // workspace capacity in tiles
+            const int cap_units = tma ? T_WS_TILES : SPLITK_WS_TILES;   // workspace capacity in tiles
             int bestS = 1;
             double best = 1.0;
             for (int S = 2; S <= maxS; ++S) {
                 if ((long long)rem * S > cap_units) break;
-                const double cost = (double)((rem * S + CTAS_PER_WAVE - 1) / CTAS_PER_WAVE) / S;
+                const double cost = (double)((rem * S + wave - 1) / wave) / S;
                 if (cost < best - 1e-9) { best = cost; bestS = S; }
             }
             if (bestS >= 2) {
@@ -574,13 +891,10 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     // DMMA pipe: ~2.1 us per 16-wide k step)
     p.stagger_ns = 0;
     p.trace = g.trace;
-    if (g.K <= 512 && T > CTAS_PER_WAVE) p.stagger_ns = ((g.K + BK - 1) / BK) * 1050;
+    if (!tma && g.K <= 512 && T > CTAS_PER_WAVE) p.stagger_ns = ((g.K + BK - 1) / BK) * 1050;
     const int rem_tiles = (int)T - p.full_tiles;
     const int units = p.full_tiles + rem_tiles * p.S;
     dim3 grid(units, 1, g.batch);
-    auto aligned = [](const void *ptr, long long ld) {
-        return ((uintptr_t)ptr % 16 == 0) && (ld % 2 == 0);
-    };
     const bool vec = aligned(g.X, g.ldx) && aligned(g.Y, g.ldy) &&
                      (g.batch == 1 || (g.sX % 2 == 0 && g.sY % 2 == 0));
     p.vec_c = aligned(g.C, g.ldc) && (!g.D || aligned(g.D, g.ldd)) &&
@@ -588,7 +902,8 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     int rc;
 #define DISPATCH(XK, YK)                                                   \
     rc = vec ? launch_inst<XK, YK, true>(p, grid, st) : launch_inst<XK, YK, false>(p, grid, st)
-    if (g.x_kmajor && g.y_kmajor) DISPATCH(true, true);
+    if (tma) rc = launch_tma(p, grid, st);
+    else if (g.x_kmajor && g.y_kmajor) DISPATCH(true, true);
     else if (g.x_kmajor && !g.y_kmajor) DISPATCH(true, false);
     else if (!g.x_kmajor && g.y_kmajor) DISPATCH(false, true);
     else DISPATCH(false, false);
@@ -596,7 +911,8 @@ int dmma_gemm(const GemmDesc &g, cudaStream_t st) {
     if (rc) return rc;
     if (p.S > 1) {
         dim3 rg(rem_tiles, 8);
-        splitk_reduce_kernel<<<rg, 256, 0, st>>>(p);
+        if (tma) splitk_reduce_kernel<TB><<<rg, 256, 0, st>>>(p);
+        else splitk_reduce_kernel<BC><<<rg, 256, 0, st>>>(p);
         count_launch();
         CVXB_LAUNCH_CHECK();
     }
