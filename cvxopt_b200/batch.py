@@ -17,6 +17,7 @@ from . import _lib
 
 STATUS = {0: "running", 1: "optimal", 2: "unknown", 3: "unknown"}
 DEFAULTS = dict(maxiters=100, abstol=1e-7, reltol=1e-6, feastol=1e-7)   # coneprog.py:436-456
+BATCH_MAX = 65535        # CVXB_BATCH_MAX: problems per cvxb_batch handle
 
 
 def _batch_dims(dims, m=None):
@@ -156,7 +157,8 @@ class QPBatchGroup:
             # when the kernels were tuned, not re-measured on H100; CVXB_BATCH_NSUB overrides)
             nsub = int(__import__("os").environ.get("CVXB_BATCH_NSUB", "0")) or (
                 2 if nprob >= 256 else (max(1, min(8, nprob // 8)) if nprob >= 16 else 1))
-        self.nsub = max(1, min(int(nsub), nprob))
+        # one library batch holds at most BATCH_MAX problems (include/cvxopt_b200.h): larger batches take more parts
+        self.nsub = max(1, min(int(nsub), nprob), -(-int(nprob) // BATCH_MAX))
         self.B, self.n, self.m = int(nprob), int(n), int(m)
         self.idx = [np.arange(r, self.B, self.nsub) for r in range(self.nsub)]
         self.parts = []
@@ -223,7 +225,8 @@ class QPBatchGroup:
 
 def qp_batch(P, q, G, h, device=0, nsub=None, dims=None, **options):
     """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,cdim,n), h (B,cdim).
-    nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches).
+    nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches), and never fewer
+    than ceil(B / 65535), the most problems one library batch holds.
     dims: cone dimensions shared by every problem ({'l': ml, 'q': [...]}); None is {'l': cdim}.
     options: maxiters, abstol, reltol, feastol, refinement (as coneqp's)."""
     P = np.asarray(P)

@@ -919,6 +919,10 @@ extern "C" {
 
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
+    if (nprob > CVXB_BATCH_MAX) {
+        set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
     *out = nullptr;
     CVXB_TRY(check_device(device));
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
@@ -968,6 +972,11 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
 
 int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
     if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
+    if (nprob > CVXB_BATCH_MAX) {
+        set_error("batch_create_cones: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob,
+                  CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
     *out = nullptr;
     if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
         set_error("batch_create_cones: bad dims (mnl must be 0, ml and the cone counts nonnegative)");

@@ -218,10 +218,14 @@ int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const d
  * cvxb_batch_create(.., m, ..) is dims = {'l': m}: G x <= h.
  * A batch with 'q' cones or refinement > 0 runs the cone path (Gs = W^{-T} G is
  * materialised per problem: nprob * cdim * n more doubles); an 'l'-only batch
- * without refinement runs the fused-scaling path. */
+ * without refinement runs the fused-scaling path.
+ * nprob is at most CVXB_BATCH_MAX: the batched kernels put the problem index in gridDim.y / gridDim.z, which
+ * are limited to 65535.  A larger nprob is CVXB_E_ARG (checked before the device); split larger batches
+ * (qp_batch's sub-batches do). */
+#define CVXB_BATCH_MAX 65535
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device);
 /* batch of  min 1/2 x'Px + q'x  s.t.  G x + s = h,  s in 'l' x 'q' cones  (B x coneqp, coneprog.py:1440).
- * dims->mnl != 0, a cone order q[k] < 1: CVXB_E_ARG; dims->ns > 0: CVXB_E_UNSUP. */
+ * dims->mnl != 0, a cone order q[k] < 1, nprob > CVXB_BATCH_MAX: CVXB_E_ARG; dims->ns > 0: CVXB_E_UNSUP. */
 int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);

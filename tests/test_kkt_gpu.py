@@ -23,7 +23,9 @@ def packed(z, dims):
     return out
 
 
-def run_case(dims, n, seed, with_H=True, resident=False):
+def run_case(dims, n, seed, with_H=True, resident=False, factors=1):
+    """`factors` factorisations of one factory with different scalings W, each solve against the oracle: the
+    handle's Cholesky runs eagerly the first time, is captured into a CUDA graph the second and replayed after"""
     import cvxopt_b200
     rng = np.random.Generator(np.random.PCG64(seed))
     K = cone_dim(dims)
@@ -32,25 +34,26 @@ def run_case(dims, n, seed, with_H=True, resident=False):
     if with_H:
         B = rng.standard_normal((n, n))
         H = np.asfortranarray(B @ B.T / n + np.eye(n))
-    W, _ = random_scaling(dims, seed=seed + 1)
     fac = cvxopt_b200.kkt_chol(G, dims, None, H=H if resident else None)
-    solve = fac(W) if (resident or H is None) else fac(W, H)
-    f_or = ko.KktChol(G, dims).factor(W, H)
-    for rep in range(2):
-        x, z = rng.standard_normal(n), rng.standard_normal(K)
-        xo, zo = x.copy(), z.copy()
-        solve(x, None, z)
-        f_or(xo, None, zo)
-        assert relerr(x, xo) < TOL, ("x", relerr(x, xo))
-        assert relerr(packed(z, dims), packed(zo, dims)) < TOL, ("z", relerr(packed(z, dims), packed(zo, dims)))
-    L = fac.get_L()
-    assert relerr(L, f_or.__self__.L) < 1e-9
+    for f in range(factors):
+        W, _ = random_scaling(dims, seed=seed + 1 + f)
+        solve = fac(W) if (resident or H is None) else fac(W, H)
+        f_or = ko.KktChol(G, dims).factor(W, H)
+        for rep in range(2):
+            x, z = rng.standard_normal(n), rng.standard_normal(K)
+            xo, zo = x.copy(), z.copy()
+            solve(x, None, z)
+            f_or(xo, None, zo)
+            assert relerr(x, xo) < TOL, (f, "x", relerr(x, xo))
+            assert relerr(packed(z, dims), packed(zo, dims)) < TOL, (f, "z", relerr(packed(z, dims), packed(zo, dims)))
+        L = fac.get_L()
+        assert relerr(L, f_or.__self__.L) < 1e-9, f
     fac.close()
 
 
 @pytest.mark.parametrize("n,m,seed", [(1, 1, 0), (3, 7, 1), (64, 100, 2), (200, 400, 3), (257, 391, 4), (513, 1100, 5)])
 def test_l_cones(n, m, seed):
-    run_case({"l": m, "q": [], "s": []}, n, seed)
+    run_case({"l": m, "q": [], "s": []}, n, seed, factors=4)
 
 
 def test_l_cones_no_H():
@@ -63,17 +66,17 @@ def test_l_cones_resident_H():
 
 @pytest.mark.parametrize("q,n,seed", [([5], 4, 0), ([64] * 8, 128, 1), ([3, 1, 70, 33], 50, 2)])
 def test_q_cones(q, n, seed):
-    run_case({"l": 0, "q": q, "s": []}, n, seed)
+    run_case({"l": 0, "q": q, "s": []}, n, seed, factors=4)
 
 
 @pytest.mark.parametrize("s,n,seed", [([3], 4, 0), ([1, 10, 33], 40, 1), ([64], 48, 2), ([130], 20, 3)])
 def test_s_cones(s, n, seed):
-    run_case({"l": 0, "q": [], "s": s}, n, seed)
+    run_case({"l": 0, "q": [], "s": s}, n, seed, factors=4)
 
 
 def test_mixed_cones():
-    run_case({"l": 37, "q": [9, 64, 2], "s": [5, 17]}, 90, 11)
-    run_case({"l": 5, "q": [4], "s": [3]}, 3, 12, with_H=False)
+    run_case({"l": 37, "q": [9, 64, 2], "s": [5, 17]}, 90, 11, factors=4)
+    run_case({"l": 5, "q": [4], "s": [3]}, 3, 12, with_H=False, factors=4)
 
 
 @pytest.mark.parametrize("dims,n,p,with_H", [
@@ -175,40 +178,6 @@ def test_ill_conditioned_scaling():
     # KKT residual of each instead of against each other when conditioning is extreme
     assert relerr(x, xo) < 1e-6
     assert relerr(z, zo) < 1e-6
-
-
-def test_building_blocks_gemm_potrf():
-    """cvxb_gemm / cvxb_potrf / cvxb_potrs on device pointers vs numpy (torch only moves memory)."""
-    import ctypes as C
-    import torch
-    from cvxopt_b200 import _lib
-    lib = _lib.load()
-    rng = np.random.Generator(np.random.PCG64(4))
-    for (m, n, k, ta, tb) in [(130, 70, 45, "N", "N"), (257, 129, 300, "T", "N"), (64, 200, 33, "N", "T"), (100, 100, 100, "T", "T")]:
-        A = rng.standard_normal((k, m) if ta == "T" else (m, k))
-        B = rng.standard_normal((n, k) if tb == "T" else (k, n))
-        Cm = rng.standard_normal((m, n))
-        dA = torch.from_numpy(np.ascontiguousarray(A.T)).cuda()      # column-major buffers
-        dB = torch.from_numpy(np.ascontiguousarray(B.T)).cuda()
-        dC = torch.from_numpy(np.ascontiguousarray(Cm.T)).cuda()
-        rc = lib.cvxb_gemm(ord(ta), ord(tb), m, n, k, 0.7, dA.data_ptr(), A.shape[0], dB.data_ptr(), B.shape[0], -0.3, dC.data_ptr(), m, 0)
-        assert rc == 0, _lib.last_error()
-        ref = 0.7 * (A.T if ta == "T" else A) @ (B.T if tb == "T" else B) - 0.3 * Cm
-        assert relerr(dC.cpu().numpy().T, ref) < 1e-13
-    for n in (1, 100, 128, 129, 700, 1333):
-        B = rng.standard_normal((n, n))
-        S = B @ B.T + n * np.eye(n)
-        dS = torch.from_numpy(S.copy()).cuda()                         # symmetric: layout-agnostic
-        inv = torch.zeros(2 * ((n + 127) // 128) * 128 * 128, dtype=torch.float64, device="cuda")
-        rc = lib.cvxb_potrf(n, dS.data_ptr(), n, inv.data_ptr(), 0)
-        assert rc == 0, _lib.last_error()
-        L = np.tril(dS.cpu().numpy().T)
-        assert relerr(L, np.linalg.cholesky(S)) < 1e-12
-        b = rng.standard_normal(n)
-        db = torch.from_numpy(b.copy()).cuda()
-        rc = lib.cvxb_potrs(n, dS.data_ptr(), n, inv.data_ptr(), db.data_ptr(), 0)
-        assert rc == 0
-        assert relerr(db.cpu().numpy(), np.linalg.solve(S, b)) < 1e-11
 
 
 @pytest.mark.parametrize("dims", [{"l": 5, "q": [4, 9], "s": [3, 7]}, {"l": 0, "q": [], "s": [20]}, {"l": 11, "q": [], "s": []}])

@@ -4,9 +4,9 @@ the same sums with the deterministic bound of an fp64 sum of K products, (K + 2)
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from ld_check import check_syrk as _check                 # columns of C's lower triangle against long double
 
-EPS = 2.0 ** -53
+pytestmark = pytest.mark.gpu
 
 
 def _run(n, k, lda, w, H, seed):
@@ -26,25 +26,6 @@ def _run(n, k, lda, w, H, seed):
                               dH.data_ptr() if dH is not None else None, n, dC.data_ptr(), n, 0)
     assert rc == 0, _lib.last_error()
     return A, dC.cpu().numpy().T
-
-
-def _check(A, w, H, C, cols):
-    """columns `cols` of C's lower triangle against long double"""
-    k, n = A.shape
-    Aw = A * (w[:, None] if w is not None else 1.0)        # fl(w * a) in fp64 first, like the kernels
-    AL, AwL = A.astype(np.longdouble), Aw.astype(np.longdouble)
-    worst = 0.0
-    for j in cols:
-        ref = AL[:, j:].T @ AwL[:, j]
-        mag = np.abs(AL[:, j:]).T @ np.abs(AwL[:, j])
-        if H is not None:
-            ref = ref + H[j:, j].astype(np.longdouble)
-            mag = mag + np.abs(H[j:, j]).astype(np.longdouble)
-        err = np.abs(C[j:, j].astype(np.longdouble) - ref)
-        bound = (k + 2) * EPS * mag
-        assert np.all(err <= bound), (j, float(np.max(err / np.maximum(mag, 1e-300))))
-        worst = max(worst, float(np.max(err / np.maximum(mag, 1e-300))))
-    return worst
 
 
 def _inputs(n, k, with_w, with_H, seed):
