@@ -1,17 +1,16 @@
 // Device-resident primal-dual interior-point method for a BATCH of independent dense QPs
 //
-//      minimize  1/2 x'P x + q'x    subject to  G x + s = h,  s >= 0          ('l' cone, no A)
+//      minimize  1/2 x'P x + q'x    subject to  G x + s = h,  s in 'l' x 'q'[0] x ...          (no A)
 //
 // run in lock-step, one problem per CTA-group, with per-problem convergence masks
 // (BASELINE config 4; the reference has no batch API — its counterpart is a Python loop over
-// solvers.qp).  The algorithm is a restatement of coneprog.coneqp for dims = {'l': m}
-// (reference src/python/coneprog.py:1998-2547): same starting point (:2055-2106), residuals
-// and stopping rule (:2169-2234), Nesterov-Todd scaling d = sqrt(s/z) (misc.py:284-287),
-// Mehrotra predictor/corrector with STEP 0.99 / EXPON 3 (:2357-2456) and scaling update
-// (misc.py:450-464).  Every KKT solve is the same path as cvxb_kkt_*: fused-scaling SYRK,
-// Cholesky, GEMV/TRSV — here batched over the problems through blockIdx.z / blockIdx.y.
+// solvers.coneqp).  The algorithm is a restatement of coneprog.coneqp (reference src/python/coneprog.py:1998-2547):
+// same starting point (:2055-2106), residuals and stopping rule (:2169-2234), Nesterov-Todd scaling (misc.py:284-352),
+// Mehrotra predictor/corrector with STEP 0.99 / EXPON 3 (:2357-2456), `refinement` steps of iterative refinement per
+// Newton solve (:2330-2347) and scaling update (misc.py:439-573).  Every KKT solve is the same path as cvxb_kkt_*:
+// SYRK, Cholesky, GEMV/TRSV — here batched over the problems through blockIdx.z / blockIdx.y.  Without 'q' cones
+// di² is fused into the SYRK operand and W^{-T} G is never formed; with them each factorisation writes Gs = W^{-T} G.
 // Nothing leaves the device between iterations except one int ("how many are done").
-// Batches with 'q' cones or iterative refinement run the cone path further down (kc_* kernels, cone_batch_solve).
 #include "cone.cuh"
 #include <cstdlib>
 #include <memory>
@@ -26,309 +25,32 @@ struct Scal {                       // per-problem scalars, device resident
     int relgap_valid, done, iters, status;   // status: 0 running, 1 optimal, 2 maxiters, 3 singular
 };
 
-__device__ __forceinline__ double block_sum(double v, double *sh) {
-    v = warp_sum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.0;
-    if (warp == 0) t = warp_sum(t);
-    if (threadIdx.x == 0) sh[0] = t;
-    __syncthreads();
-    return sh[0];
-}
-__device__ __forceinline__ double block_min(double v, double *sh) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : INFINITY;
-    if (warp == 0) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) t = fmin(t, __shfl_xor_sync(0xffffffffu, t, o));
-    }
-    if (threadIdx.x == 0) sh[0] = t;
-    __syncthreads();
-    return sh[0];
-}
-
+// The 'l' rows [0, ml) keep d / di / lmbda in the m-vectors; cone k occupies rows [qoff[k], qoff[k+1]) and its NT
+// scaling W_k = beta_k (2 v_k v_k' - J) lives in the per-slot state row (misc.py:290-352).  'l' rows are spread over
+// the threads of the CTA, 'q' cones over its warps: lane i of the warp owns entries i, i+32, ... of the cone in every
+// pass, and the entry-0 values every lane needs are formed from warp sums; a pass that reads an entry another lane
+// wrote follows a __syncwarp().  Kernels templated on CONES compile the cone loops out for batches without cones.
 struct Ptrs {
-    int n, m;
+    int n, m, ml, nq, refinement;
     const double *q, *h;
     double *x, *s, *z, *rx, *rz, *dx, *ds, *dz, *lmbda, *lmbdasq, *d, *di, *di2, *ws3, *bzp;
     Scal *sc;
-};
-#define PB_SETUP                                                  \
-    const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x; \
-    const long long on = (long long)b * p.n, om = (long long)b * p.m; \
-    __shared__ double sh[32];                                     \
-    Scal &S = p.sc[b];
-
-// starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2076-2080)
-__global__ void k_init_rhs(Ptrs p) {
-    PB_SETUP
-    double nq = 0, nh = 0;
-    for (int i = tid; i < p.n; i += nt) { double v = p.q[on + i]; p.dx[on + i] = -v; nq += v * v; }
-    for (int i = tid; i < p.m; i += nt) {
-        double v = p.h[om + i];
-        p.dz[om + i] = v;
-        p.d[om + i] = 1.0; p.di[om + i] = 1.0; p.di2[om + i] = 1.0;
-        nh += v * v;
-    }
-    nq = block_sum(nq, sh);
-    nh = block_sum(nh, sh);
-    if (tid == 0) {
-        S.resx0 = fmax(1.0, sqrt(nq));                  // :1998
-        S.resz0 = fmax(1.0, sqrt(nh));                  // :2000 (snrm2 == 2-norm for 'l')
-        S.done = 0; S.iters = 0; S.status = 0; S.sigma = 0; S.eta = 0; S.step = 0;
-    }
-}
-// bzp = di .* bz  (W^{-T} bz for the 'l' cone)
-__global__ void k_scale_bz(Ptrs p, const double *bz) {
-    PB_SETUP
-    (void)sh; (void)S; (void)on;
-    for (int i = tid; i < p.m; i += nt) p.bzp[om + i] = p.di[om + i] * bz[om + i];
-}
-// starting point, part 2: x = dx, z = dz (solution), s = -z, shifts (:2083-2106), gap (:2165)
-__global__ void k_init_point(Ptrs p) {
-    PB_SETUP
-    double ns = 0, mins = INFINITY;
-    for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
-    for (int i = tid; i < p.m; i += nt) {
-        double zv = p.bzp[om + i];      // solve leaves W*uz in bzp
-        p.z[om + i] = zv;
-        p.s[om + i] = -zv;
-        ns += zv * zv;
-        mins = fmin(mins, -zv);
-    }
-    ns = sqrt(block_sum(ns, sh));
-    mins = block_min(mins, sh);
-    const double ts = -mins;                             // max_step(s) = -min(s) for 'l'
-    double minz = INFINITY;
-    for (int i = tid; i < p.m; i += nt) minz = fmin(minz, p.z[om + i]);
-    minz = block_min(minz, sh);
-    const double tz = -minz;
-    const double as = (ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
-    const double az = (tz >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + tz : 0.0;   // nrmz == nrms here
-    double gap = 0;
-    for (int i = tid; i < p.m; i += nt) {
-        double sv = p.s[om + i] + as, zv = p.z[om + i] + az;
-        p.s[om + i] = sv; p.z[om + i] = zv;
-        gap += sv * zv;
-    }
-    gap = block_sum(gap, sh);
-    if (tid == 0) S.gap = gap;
-}
-// rx = q  (then rx += P x by GEMV)
-__global__ void k_res_begin(Ptrs p) {
-    PB_SETUP
-    (void)sh; (void)S;
-    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = p.q[on + i];
-    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i] - p.h[om + i];      // :2183-2184
-}
-// f0 pieces once rx = P x + q   (:2172)
-__global__ void k_res_dots(Ptrs p) {
-    PB_SETUP
-    double a = 0, c = 0;
-    for (int i = tid; i < p.n; i += nt) { double xv = p.x[on + i]; a += xv * p.rx[on + i]; c += xv * p.q[on + i]; }
-    a = block_sum(a, sh); c = block_sum(c, sh);
-    if (tid == 0) { S.xPxq = a; S.xq = c; }
-}
-// statistics + stopping rule (:2175-2234)
-__global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol, double feastol,
-                        int *ndone, int *doneflags) {
-    PB_SETUP
-    double rx2 = 0, rz2 = 0, zrz = 0;
-    for (int i = tid; i < p.n; i += nt) { double v = p.rx[on + i]; rx2 += v * v; }
-    for (int i = tid; i < p.m; i += nt) { double v = p.rz[om + i]; rz2 += v * v; zrz += p.z[om + i] * v; }
-    rx2 = block_sum(rx2, sh); rz2 = block_sum(rz2, sh); zrz = block_sum(zrz, sh);
-    if (tid == 0) {
-        if (!S.done) {
-            const double f0 = 0.5 * (S.xPxq + S.xq);
-            S.resx = sqrt(rx2); S.resz = sqrt(rz2); S.zrz = zrz;
-            S.pcost = f0;
-            S.dcost = f0 + zrz - S.gap;
-            if (S.pcost < 0.0) { S.relgap = S.gap / -S.pcost; S.relgap_valid = 1; }
-            else if (S.dcost > 0.0) { S.relgap = S.gap / S.dcost; S.relgap_valid = 1; }
-            else { S.relgap = 0.0; S.relgap_valid = 0; }
-            S.pres = S.resz / S.resz0;
-            S.dres = S.resx / S.resx0;
-            const bool opt = S.pres <= feastol && S.dres <= feastol &&
-                             (S.gap <= abstol || (S.relgap_valid && S.relgap <= reltol));
-            if (opt || iter == maxiters) {
-                S.done = 1; S.iters = iter; S.status = opt ? 1 : 2;
-            }
-        }
-        if (S.done) atomicAdd(ndone, 1);
-        doneflags[b] = S.done;
-    }
-}
-
-// ---- compaction of finished problems ----
-// The lock-step loop launches every batched kernel over the first `Bact` slots.  When problems finish, each finished
-// slot below the new active count trades places with an active slot from the tail: everything a problem owns between
-// iterations (P, G, its 17 vectors, its scalars; K / inv / info are rebuilt every iteration) is swapped, so the active
-// problems stay a contiguous prefix and finished ones keep their final iterates in the tail.  ~6.3 MB per swap at
-// n=512, m=1024, at most one swap per problem per solve.
-struct SwapArgs {
-    double *P, *G, *vecs; Scal *sc;
-    long long sP, sG;
-    int n, me, Btot;
-};
-__global__ void k_swap_slots(SwapArgs a, const int *pairs) {
-    const int i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
-    const long long eP = a.sP, eG = a.sG, eN = 4LL * a.n, eM = 13LL * a.me, eS = (long long)(sizeof(Scal) / sizeof(double));
-    const long long total = eP + eG + eN + eM + eS;
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        double *x, *y;
-        long long r = e;
-        if (r < eP) { x = a.P + i * a.sP + r; y = a.P + j * a.sP + r; }
-        else if ((r -= eP) < eG) { x = a.G + i * a.sG + r; y = a.G + j * a.sG + r; }
-        else if ((r -= eG) < eN) {
-            const long long arr = r / a.n, k = r % a.n;
-            double *base = a.vecs + arr * (long long)a.Btot * a.n;
-            x = base + (long long)i * a.n + k; y = base + (long long)j * a.n + k;
-        } else if ((r -= eN) < eM) {
-            const long long arr = r / a.me, k = r % a.me;
-            double *base = a.vecs + 4LL * a.Btot * a.n + arr * (long long)a.Btot * a.me;
-            x = base + (long long)i * a.me + k; y = base + (long long)j * a.me + k;
-        } else {
-            r -= eM;
-            x = reinterpret_cast<double *>(a.sc + i) + r; y = reinterpret_cast<double *>(a.sc + j) + r;
-        }
-        const double t = *x; *x = *y; *y = t;
-    }
-}
-// out[perm[slot], :] = in[slot, :]
-__global__ void k_unpermute_rows(const double *in, double *out, const int *perm, int len) {
-    const int slot = blockIdx.x;
-    const double *src = in + (long long)slot * len;
-    double *dst = out + (long long)perm[slot] * len;
-    for (int k = threadIdx.x; k < len; k += blockDim.x) dst[k] = src[k];
-}
-static_assert(sizeof(Scal) % sizeof(double) == 0, "Scal is swapped as doubles");
-// NT scaling at iteration 0 (misc.py:284-287) and lambda^2 (:2244)
-__global__ void k_scaling(Ptrs p, int first) {
-    PB_SETUP
-    (void)sh; (void)on;
-    if (S.done) return;
-    for (int i = tid; i < p.m; i += nt) {
-        if (first) {
-            const double sv = p.s[om + i], zv = p.z[om + i];
-            const double d = sqrt(sv / zv);
-            p.d[om + i] = d;
-            const double di = 1.0 / d;
-            p.di[om + i] = di;
-            p.di2[om + i] = di * di;
-            p.lmbda[om + i] = sqrt(sv * zv);
-        }
-        const double l = p.lmbda[om + i];
-        p.lmbdasq[om + i] = l * l;
-    }
-    if (tid == 0) { S.mu = S.gap / p.m; S.sigma = 0.0; S.eta = 0.0; }       // :2357-2358
-}
-// right-hand side of the i-th Newton system and the f4_no_ir preamble (:2376-2309)
-__global__ void k_dir_prep(Ptrs p, int i) {
-    PB_SETUP
-    (void)sh;
-    const double sm = S.sigma * S.mu, c = -1.0 + S.eta;
-    for (int k = tid; k < p.n; k += nt) p.dx[on + k] = c * p.rx[on + k];
-    for (int k = tid; k < p.m; k += nt) {
-        double ds = -p.lmbdasq[om + k] + sm;
-        if (i == 1) ds -= p.ws3[om + k];                 // Mehrotra correction
-        ds = ds / p.lmbda[om + k];                       // sinv
-        p.ds[om + k] = ds;
-        const double dz = c * p.rz[om + k] - p.d[om + k] * ds;   // z := z - W' s
-        p.dz[om + k] = dz;
-        p.bzp[om + k] = p.di[om + k] * dz;               // W^{-T} bz for the solve
-    }
-}
-// after the solve: dz = bzp (= W uz); ds := ds - dz; step length, sigma (:2316, :2423-2456)
-__global__ void k_dir_post(Ptrs p, int i) {
-    PB_SETUP
-    double dsdz = 0, mins = INFINITY, minz = INFINITY;
-    for (int k = tid; k < p.m; k += nt) {
-        const double dz = p.bzp[om + k];
-        const double ds = p.ds[om + k] - dz;
-        dsdz += ds * dz;
-        if (i == 0) p.ws3[om + k] = ds * dz;
-        const double l = p.lmbda[om + k];
-        const double dss = ds / l, dzs = dz / l;        // scale2
-        p.ds[om + k] = dss; p.dz[om + k] = dzs;
-        mins = fmin(mins, dss); minz = fmin(minz, dzs);
-    }
-    dsdz = block_sum(dsdz, sh);
-    mins = block_min(mins, sh);
-    minz = block_min(minz, sh);
-    if (tid == 0) {
-        const double t = fmax(0.0, fmax(-mins, -minz));
-        double step;
-        if (t == 0.0) step = 1.0;
-        else step = (i == 0) ? fmin(1.0, 1.0 / t) : fmin(1.0, 0.99 / t);
-        S.step = step; S.dsdz = dsdz;
-        if (i == 0) {
-            const double v = fmin(1.0, fmax(0.0, 1.0 - step + dsdz / S.gap * step * step));
-            S.sigma = v * v * v;
-            S.eta = 0.0;
-        }
-    }
-}
-// x += step dx; new scaled iterates, scaling update, unscaled s, z, gap (:2459-2547, misc.py:450-464)
-__global__ void k_update(Ptrs p, const int *info, int iter) {
-    PB_SETUP
-    if (S.done) return;
-    if (info[b] > 0) {      // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
-        if (tid == 0) { S.done = 1; S.status = 3; S.iters = iter; }
-        return;
-    }
-    const double step = S.step;
-    for (int k = tid; k < p.n; k += nt) p.x[on + k] += step * p.dx[on + k];
-    double gap = 0;
-    for (int k = tid; k < p.m; k += nt) {
-        const double l = p.lmbda[om + k];
-        const double ds = (1.0 + step * p.ds[om + k]) * l;      // scale2 inverse
-        const double dz = (1.0 + step * p.dz[om + k]) * l;
-        const double ss = sqrt(ds), sz = sqrt(dz);
-        const double d = p.d[om + k] * ss / sz;
-        const double di = 1.0 / d;
-        const double ln = ss * sz;
-        p.d[om + k] = d; p.di[om + k] = di; p.di2[om + k] = di * di;
-        p.lmbda[om + k] = ln;
-        p.s[om + k] = d * ln;                                   // W' lambda
-        p.z[om + k] = di * ln;                                  // W^{-1} lambda
-        gap += ln * ln;
-    }
-    gap = block_sum(gap, sh);
-    if (tid == 0) S.gap = gap;
-}
-
-// ---- the cone path: dims = {'l': ml, 'q': [...]} and/or iterative refinement ----
-// Same IPM as above, restated for coneqp with 'q' cones (coneprog.py:1998-2547) and `refinement` steps of
-// iterative refinement per Newton solve (:2330-2347).  The 'l' rows [0, ml) keep d / di / lmbda in the vectors
-// above; cone k occupies rows [qoff[k], qoff[k+1]) and its NT scaling W_k = beta_k (2 v_k v_k' - J) lives in the
-// per-slot state row `cst` (misc.py:290-352).  'l' rows are spread over the threads of the CTA, 'q' cones over its
-// warps: lane i of the warp owns entries i, i+32, ... of the cone in every pass, and the entry-0 values every lane
-// needs are formed from warp sums, so no pass reads what another lane wrote.
-struct CPtrs {
-    Ptrs p;
-    int ml, nq, refinement;
     const int *qoff;                 // nq + 1 row offsets; qoff[nq] = m
     long long L;                     // doubles per slot in the state row
-    // inside a slot's row: v (sum q, indexed by row - ml), beta (nq), then the refinement vectors
+    // inside a slot's row: v (sum q, indexed by row - ml) and beta (nq) with cones, the refinement vectors with
+    // refinement > 0
     double *v, *beta, *wx, *wx2, *wz, *ws, *wz2, *ws2, *wz3;
 };
-#define CB_SETUP                                                           \
-    const Ptrs &p = cp.p;                                                  \
-    PB_SETUP                                                               \
-    const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;           \
-    const long long oc = (long long)b * cp.L;                              \
-    (void)lane; (void)warp; (void)nwarp; (void)oc;
+#define PB_SETUP                                                                                       \
+    const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;                                      \
+    const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;                                       \
+    const long long on = (long long)b * p.n, om = (long long)b * p.m, oc = (long long)b * p.L;         \
+    __shared__ double sh[32];                                                                          \
+    Scal &S = p.sc[b];                                                                                 \
+    (void)lane; (void)warp; (void)nwarp; (void)on; (void)om; (void)oc; (void)sh; (void)S;
 #define FOR_CONES(o, len)                                                  \
-    for (int k_ = warp; k_ < cp.nq; k_ += nwarp)                           \
-        if (const int o = cp.qoff[k_], len = cp.qoff[k_ + 1] - cp.qoff[k_]; true)
+    for (int k_ = warp; k_ < p.nq; k_ += nwarp)                            \
+        if (const int o = p.qoff[k_], len = p.qoff[k_ + 1] - p.qoff[k_]; true)
 #define FOR_LANE(i, len) for (int i = lane; i < len; i += 32)
 
 // y := W_k x (inverse = 0) or W_k^{-1} x (inverse = 1) for one cone, x and y of this lane's entries (misc_solvers.c:144-183)
@@ -390,58 +112,54 @@ __device__ __forceinline__ double q_margin(const double *x, double x0, int len, 
     return x0 - sqrt(warp_sum(a));
 }
 
-// W = I: v = e1, beta = 1 (coneprog.py:2055-2064); the 'l' part is k_init_rhs's
-__global__ void kc_init_w(CPtrs cp) {
-    CB_SETUP
-    (void)sh; (void)S; (void)on; (void)om;
-    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+// starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2055-2080): d = di = 1,
+// v = e1 and beta = 1 for each cone
+__global__ void k_init_rhs(Ptrs p) {
+    PB_SETUP
+    double nq = 0, nh = 0;
+    for (int i = tid; i < p.n; i += nt) { double v = p.q[on + i]; p.dx[on + i] = -v; nq += v * v; }
+    for (int i = tid; i < p.m; i += nt) {
+        double v = p.h[om + i];
+        p.dz[om + i] = v;
+        p.d[om + i] = 1.0; p.di[om + i] = 1.0; p.di2[om + i] = 1.0;
+        nh += v * v;
+    }
+    double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) {
         FOR_LANE(i, len) v[o + i] = (i == 0) ? 1.0 : 0.0;
         if (lane == 0) beta[k_] = 1.0;
     }
-}
-// Gs = W^{-T} G, one warp per column (misc.py:1268-1271): 'l' rows times di, each 'q' block times W_k^{-1}
-__global__ void kc_build_gs(CPtrs cp, const double *G, double *Gs, long long ldg, long long sG) {
-    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
-    const int j = blockIdx.x * nwarp + warp;
-    if (j >= cp.p.n) return;
-    const long long off = (long long)b * sG + (long long)j * ldg;
-    const double *g = G + off, *di = cp.p.di + (long long)b * cp.p.m;
-    double *o = Gs + off;
-    for (int i = lane; i < cp.ml; i += 32) o[i] = di[i] * g[i];
-    const double *v = cp.v + (long long)b * cp.L - cp.ml, *beta = cp.beta + (long long)b * cp.L;
-    for (int k = 0; k < cp.nq; ++k) {
-        const int r = cp.qoff[k], len = cp.qoff[k + 1] - r;
-        q_scale(v + r, beta[k], g + r, o + r, len, lane, true);
+    nq = block_sum(nq, sh);
+    nh = block_sum(nh, sh);
+    if (tid == 0) {
+        S.resx0 = fmax(1.0, sqrt(nq));                  // :1998
+        S.resz0 = fmax(1.0, sqrt(nh));                  // :2000 (snrm2 == 2-norm for 'l' and 'q')
+        S.done = 0; S.iters = 0; S.status = 0; S.sigma = 0; S.eta = 0; S.step = 0;
     }
 }
-// dst = W^{-T} src over all rows
-__device__ __forceinline__ void cone_scale_inv(const CPtrs &cp, int b, const double *src, double *dst) {
-    const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
-    const double *di = cp.p.di + (long long)b * cp.p.m;
-    const double *v = cp.v + (long long)b * cp.L - cp.ml, *beta = cp.beta + (long long)b * cp.L;
-    for (int i = tid; i < cp.ml; i += nt) dst[i] = di[i] * src[i];
+// bzp = W^{-T} dz (the starting point's right-hand side): 'l' rows times di, each 'q' block times W_k^{-1}
+__global__ void k_scale_bz(Ptrs p) {
+    PB_SETUP
+    const double *src = p.dz + om;
+    double *dst = p.bzp + om;
+    for (int i = tid; i < p.ml; i += nt) dst[i] = p.di[om + i] * src[i];
+    const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) q_scale(v + o, beta[k_], src + o, dst + o, len, lane, true);
 }
-// bzp = W^{-T} dz (the starting point's right-hand side)
-__global__ void kc_scale_bz(CPtrs cp) {
-    const long long om = (long long)blockIdx.x * cp.p.m;
-    cone_scale_inv(cp, blockIdx.x, cp.p.dz + om, cp.p.bzp + om);
-}
-// starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both
-__global__ void kc_init_point(CPtrs cp) {
-    CB_SETUP
+// starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both, gap
+template <bool CONES> __global__ void k_init_point(Ptrs p) {
+    PB_SETUP
     double *s = p.s + om, *z = p.z + om;
-    const double *zn = p.bzp + om;
+    const double *zn = p.bzp + om;                      // the solve leaves W uz in bzp
     double ns = 0, mins = INFINITY, minz = INFINITY;
     for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
     for (int i = tid; i < p.m; i += nt) {
         const double zv = zn[i];
         z[i] = zv; s[i] = -zv;
         ns += zv * zv;
-        if (i < cp.ml) { mins = fmin(mins, -zv); minz = fmin(minz, zv); }
+        if (i < p.ml) { mins = fmin(mins, -zv); minz = fmin(minz, zv); }
     }
-    FOR_CONES(o, len) {                                  // s = -z: ||s1|| = ||z1||, s0 = -z0
+    if (CONES) FOR_CONES(o, len) {                      // s = -z: ||s1|| = ||z1||, s0 = -z0
         const double z0 = zn[o], mz = q_margin(zn + o, z0, len, lane);
         mins = fmin(mins, -z0 - (z0 - mz));
         minz = fmin(minz, mz);
@@ -451,34 +169,146 @@ __global__ void kc_init_point(CPtrs cp) {
     minz = block_min(minz, sh);
     const double ts = -mins, tz = -minz;
     const double as = (ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
-    const double az = (tz >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + tz : 0.0;
-    __syncthreads();
-    for (int i = tid; i < cp.ml; i += nt) { s[i] += as; z[i] += az; }
-    for (int k = tid; k < cp.nq; k += nt) { s[cp.qoff[k]] += as; z[cp.qoff[k]] += az; }
-    __syncthreads();
+    const double az = (tz >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + tz : 0.0;   // nrmz == nrms here
+    for (int i = tid; i < p.ml; i += nt) { s[i] += as; z[i] += az; }
+    if (CONES) {
+        for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
+        __syncthreads();
+    }
     double gap = 0;
     for (int i = tid; i < p.m; i += nt) gap += s[i] * z[i];
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
-// NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357)
-__global__ void kc_scaling(CPtrs cp, int first) {
-    CB_SETUP
-    (void)on;
+// rx = q  (then rx += P x by GEMV)
+__global__ void k_res_begin(Ptrs p) {
+    PB_SETUP
+    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = p.q[on + i];
+    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i] - p.h[om + i];      // :2183-2184
+}
+// f0 pieces once rx = P x + q   (:2172)
+__global__ void k_res_dots(Ptrs p) {
+    PB_SETUP
+    double a = 0, c = 0;
+    for (int i = tid; i < p.n; i += nt) { double xv = p.x[on + i]; a += xv * p.rx[on + i]; c += xv * p.q[on + i]; }
+    a = block_sum(a, sh); c = block_sum(c, sh);
+    if (tid == 0) { S.xPxq = a; S.xq = c; }
+}
+// statistics + stopping rule (:2175-2234); row-wise, so every cone row is treated alike
+__global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol, double feastol,
+                        int *ndone, int *doneflags) {
+    PB_SETUP
+    double rx2 = 0, rz2 = 0, zrz = 0;
+    for (int i = tid; i < p.n; i += nt) { double v = p.rx[on + i]; rx2 += v * v; }
+    for (int i = tid; i < p.m; i += nt) { double v = p.rz[om + i]; rz2 += v * v; zrz += p.z[om + i] * v; }
+    rx2 = block_sum(rx2, sh); rz2 = block_sum(rz2, sh); zrz = block_sum(zrz, sh);
+    if (tid == 0) {
+        if (!S.done) {
+            const double f0 = 0.5 * (S.xPxq + S.xq);
+            S.resx = sqrt(rx2); S.resz = sqrt(rz2); S.zrz = zrz;
+            S.pcost = f0;
+            S.dcost = f0 + zrz - S.gap;
+            if (S.pcost < 0.0) { S.relgap = S.gap / -S.pcost; S.relgap_valid = 1; }
+            else if (S.dcost > 0.0) { S.relgap = S.gap / S.dcost; S.relgap_valid = 1; }
+            else { S.relgap = 0.0; S.relgap_valid = 0; }
+            S.pres = S.resz / S.resz0;
+            S.dres = S.resx / S.resx0;
+            const bool opt = S.pres <= feastol && S.dres <= feastol &&
+                             (S.gap <= abstol || (S.relgap_valid && S.relgap <= reltol));
+            if (opt || iter == maxiters) {
+                S.done = 1; S.iters = iter; S.status = opt ? 1 : 2;
+            }
+        }
+        if (S.done) atomicAdd(ndone, 1);
+        doneflags[b] = S.done;
+    }
+}
+
+// ---- compaction of finished problems ----
+// The lock-step loop launches every batched kernel over the first `Bact` slots.  When problems finish, each finished
+// slot below the new active count trades places with an active slot from the tail: everything a problem owns between
+// iterations (P, G, its 17 vectors, its scalars, its state row; K / inv / info / Gs are rebuilt every iteration) is
+// swapped, so the active problems stay a contiguous prefix and finished ones keep their final iterates in the tail.
+// ~6.3 MB per swap at n=512, m=1024, at most one swap per problem per solve.
+struct SwapArgs {
+    double *P, *G, *vecs; Scal *sc;
+    long long sP, sG;
+    int n, me, Btot;
+};
+__global__ void k_swap_slots(SwapArgs a, const int *pairs) {
+    const int i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
+    const long long eP = a.sP, eG = a.sG, eN = 4LL * a.n, eM = 13LL * a.me, eS = (long long)(sizeof(Scal) / sizeof(double));
+    const long long total = eP + eG + eN + eM + eS;
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+        double *x, *y;
+        long long r = e;
+        if (r < eP) { x = a.P + i * a.sP + r; y = a.P + j * a.sP + r; }
+        else if ((r -= eP) < eG) { x = a.G + i * a.sG + r; y = a.G + j * a.sG + r; }
+        else if ((r -= eG) < eN) {
+            const long long arr = r / a.n, k = r % a.n;
+            double *base = a.vecs + arr * (long long)a.Btot * a.n;
+            x = base + (long long)i * a.n + k; y = base + (long long)j * a.n + k;
+        } else if ((r -= eN) < eM) {
+            const long long arr = r / a.me, k = r % a.me;
+            double *base = a.vecs + 4LL * a.Btot * a.n + arr * (long long)a.Btot * a.me;
+            x = base + (long long)i * a.me + k; y = base + (long long)j * a.me + k;
+        } else {
+            r -= eM;
+            x = reinterpret_cast<double *>(a.sc + i) + r; y = reinterpret_cast<double *>(a.sc + j) + r;
+        }
+        const double t = *x; *x = *y; *y = t;
+    }
+}
+// swap rows i and j of a [slots x L] buffer for each pair
+__global__ void k_swap_rows(double *a, long long L, const int *pairs) {
+    const long long i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
+    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < L; e += (long long)gridDim.x * blockDim.x) {
+        const double t = a[i * L + e]; a[i * L + e] = a[j * L + e]; a[j * L + e] = t;
+    }
+}
+// out[perm[slot], :] = in[slot, :]
+__global__ void k_unpermute_rows(const double *in, double *out, const int *perm, int len) {
+    const int slot = blockIdx.x;
+    const double *src = in + (long long)slot * len;
+    double *dst = out + (long long)perm[slot] * len;
+    for (int k = threadIdx.x; k < len; k += blockDim.x) dst[k] = src[k];
+}
+static_assert(sizeof(Scal) % sizeof(double) == 0, "Scal is swapped as doubles");
+
+// Gs = W^{-T} G, one warp per column (misc.py:1268-1271): 'l' rows times di, each 'q' block times W_k^{-1}
+__global__ void k_build_gs(Ptrs p, const double *G, double *Gs, long long ldg, long long sG) {
+    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+    const int j = blockIdx.x * nwarp + warp;
+    if (j >= p.n) return;
+    const long long off = (long long)b * sG + (long long)j * ldg;
+    const double *g = G + off, *di = p.di + (long long)b * p.m;
+    double *o = Gs + off;
+    for (int i = lane; i < p.ml; i += 32) o[i] = di[i] * g[i];
+    const double *v = p.v + (long long)b * p.L - p.ml, *beta = p.beta + (long long)b * p.L;
+    for (int k = 0; k < p.nq; ++k) {
+        const int r = p.qoff[k], len = p.qoff[k + 1] - r;
+        q_scale(v + r, beta[k], g + r, o + r, len, lane, true);
+    }
+}
+// NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357).
+// di2 = di² is the SYRK's weight when W^{-T} G is not formed
+template <bool CONES> __global__ void k_scaling(Ptrs p, int first) {
+    PB_SETUP
     if (S.done) return;
     double *l = p.lmbda + om, *lsq = p.lmbdasq + om;
     const double *s = p.s + om, *z = p.z + om;
-    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
-    for (int i = tid; i < cp.ml; i += nt) {
+    for (int i = tid; i < p.ml; i += nt) {
         if (first) {
-            const double d = sqrt(s[i] / z[i]);
+            const double d = sqrt(s[i] / z[i]), di = 1.0 / d;
             p.d[om + i] = d;
-            p.di[om + i] = 1.0 / d;
+            p.di[om + i] = di;
+            if (!CONES) p.di2[om + i] = di * di;
             l[i] = sqrt(s[i] * z[i]);
         }
         lsq[i] = l[i] * l[i];
     }
-    FOR_CONES(o, len) {
+    double *v = p.v + oc - p.ml, *beta = p.beta + oc;
+    if (CONES) FOR_CONES(o, len) {
         if (first) {
             const double s0 = s[o], z0 = z[o];
             const double aa = q_jnrm2(s + o, s0, len, lane), bb = q_jnrm2(z + o, z0, len, lane);
@@ -507,65 +337,92 @@ __global__ void kc_scaling(CPtrs cp, int first) {
         const double l0 = l[o];
         FOR_LANE(i, len) lsq[o + i] = (i == 0) ? nl : 2.0 * l0 * l[o + i];
     }
-    if (tid == 0) { S.mu = S.gap / (cp.ml + cp.nq); S.sigma = 0.0; S.eta = 0.0; }
+    if (tid == 0) { S.mu = S.gap / (p.ml + p.nq); S.sigma = 0.0; S.eta = 0.0; }
 }
-// right-hand side of the i-th Newton system (coneprog.py:2373-2399); a copy of it for the refinement (:2331-2335)
-__global__ void kc_dir_rhs(CPtrs cp, int i) {
-    CB_SETUP
-    (void)sh;
+
+// f4_no_ir before the solve (coneprog.py:2301-2309): s := lmbda o\ s; z := z - W's; bzp := W^{-T} z.
+// 'l' row r (of the m-vectors), z and s in registers
+__device__ __forceinline__ void f4_pre_row(const Ptrs &p, long long r, double &z, double &s) {
+    s = s / p.lmbda[r];
+    z = z - p.d[r] * s;
+    p.bzp[r] = p.di[r] * z;
+}
+// cone k at rows [o, o + len) of slot b's z and s, one warp; bzp holds W's until it receives W^{-T} z
+__device__ __forceinline__ void f4_pre_cone(const Ptrs &p, long long om, long long oc, int k, int o, int len,
+                                            int lane, double *z, double *s) {
+    const double *v = p.v + oc - p.ml;
+    double *t = p.bzp + om;
+    q_sinv(p.lmbda + om + o, s + o, len, lane);
+    q_scale(v + o, p.beta[oc + k], s + o, t + o, len, lane, false);
+    FOR_LANE(i, len) z[o + i] -= t[o + i];
+    q_scale(v + o, p.beta[oc + k], z + o, t + o, len, lane, true);
+}
+// f4_no_ir after the solve (coneprog.py:2316), row r: z := W uz (the solve leaves it in bzp), s := s - z; returns z
+__device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double &s) {
+    const double z = p.bzp[r];
+    s -= z;
+    return z;
+}
+
+// right-hand side of the i-th Newton system (coneprog.py:2373-2399), a copy of it for the refinement (:2331-2335),
+// then f4_no_ir's steps before the solve.  Cone rows are formed row-wise over the CTA; after a barrier the warp that
+// owns a cone adds sigma mu to its entry 0 and runs the cone part.
+template <bool CONES> __global__ void k_dir_rhs(Ptrs p, int i) {
+    PB_SETUP
     const double sm = S.sigma * S.mu, c = -1.0 + S.eta;
     for (int k = tid; k < p.n; k += nt) {
         const double dx = c * p.rx[on + k];
         p.dx[on + k] = dx;
-        if (cp.refinement) cp.wx[oc + k] = dx;
+        if (p.refinement) p.wx[oc + k] = dx;
     }
-    for (int k = tid; k < p.m; k += nt) {
-        double ds = (i == 1) ? -p.ws3[om + k] : 0.0;     // Mehrotra correction
-        ds -= p.lmbdasq[om + k];
-        const double dz = c * p.rz[om + k];
-        p.dz[om + k] = dz;
-        if (cp.refinement) { cp.wz[oc + k] = dz; cp.ws[oc + k] = ds; }
-        p.ds[om + k] = ds;
+    // row r: z = c rz, s = -ws3 (the Mehrotra correction, i = 1) - lmbda o lmbda (+ sigma mu where e is 1)
+    auto rhs = [&](int r, bool e, double &z, double &s) {
+        s = (i == 1) ? -p.ws3[om + r] : 0.0;
+        s -= p.lmbdasq[om + r];
+        if (e) s += sm;
+        z = c * p.rz[om + r];
+        if (p.refinement) { p.wz[oc + r] = z; p.ws[oc + r] = s; }
+    };
+#pragma unroll 1                                         // unrolled, the 'l'-only kernel needs more registers
+    for (int k = tid; k < p.ml; k += nt) {
+        double z, s;
+        rhs(k, true, z, s);
+        f4_pre_row(p, om + k, z, s);
+        p.dz[om + k] = z; p.ds[om + k] = s;
     }
-    __syncthreads();
-    for (int k = tid; k < cp.ml; k += nt) { p.ds[om + k] += sm; if (cp.refinement) cp.ws[oc + k] += sm; }
-    for (int k = tid; k < cp.nq; k += nt) {
-        const int r = cp.qoff[k];
-        p.ds[om + r] += sm;
-        if (cp.refinement) cp.ws[oc + r] += sm;
+    if (CONES) {
+        for (int k = p.ml + tid; k < p.m; k += nt) {
+            double z, s;
+            rhs(k, false, z, s);
+            p.dz[om + k] = z; p.ds[om + k] = s;
+        }
+        __syncthreads();
+        FOR_CONES(o, len) {
+            if (lane == 0) { p.ds[om + o] += sm; if (p.refinement) p.ws[oc + o] += sm; }
+            __syncwarp();
+            f4_pre_cone(p, om, oc, k_, o, len, lane, p.dz + om, p.ds + om);
+        }
     }
 }
-// f4_no_ir, before the solve (coneprog.py:2301-2309): s := lmbda o\ s; z := z - W's; bzp := W^{-T} z.
-// z and s are slot b's vectors at z + b*sz, s + b*ss
-__global__ void kc_f4_pre(CPtrs cp, double *z, long long sz, double *s, long long ss) {
-    CB_SETUP
-    (void)sh; (void)S; (void)on;
+// f4_no_ir before the solve of a refinement step, on slot b's z and s at z + b*sz, s + b*ss
+__global__ void k_f4_pre(Ptrs p, double *z, long long sz, double *s, long long ss) {
+    PB_SETUP
     z += b * sz; s += b * ss;
-    const double *l = p.lmbda + om;
-    for (int i = tid; i < cp.ml; i += nt) {
-        const double sv = s[i] / l[i];
-        s[i] = sv;
-        const double zv = z[i] - p.d[om + i] * sv;
-        z[i] = zv;
-        p.bzp[om + i] = p.di[om + i] * zv;
+    for (int i = tid; i < p.ml; i += nt) {
+        double zv = z[i], sv = s[i];
+        f4_pre_row(p, om + i, zv, sv);
+        z[i] = zv; s[i] = sv;
     }
-    const double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
-    double *t = cp.wz3 + oc;                              // W's, then W^{-T} z
-    FOR_CONES(o, len) {
-        q_sinv(l + o, s + o, len, lane);
-        q_scale(v + o, beta[k_], s + o, t + o, len, lane, false);
-        FOR_LANE(i, len) z[o + i] -= t[o + i];
-        q_scale(v + o, beta[k_], z + o, p.bzp + om + o, len, lane, true);
-    }
+    FOR_CONES(o, len) f4_pre_cone(p, om, oc, k_, o, len, lane, z, s);
 }
-// f4_no_ir, after the solve (:2316): z := W uz (bzp), s := s - z.  acc: the refinement step, (dx, dz, ds) += (x, z, s)
-__global__ void kc_f4_post(CPtrs cp, double *x, long long sx, double *z, long long sz, double *s, long long ss,
-                           int acc) {
-    CB_SETUP
-    (void)sh; (void)S;
+// f4_no_ir after a solve that refinement follows or that is a refinement step.  acc: the refinement step,
+// (dx, dz, ds) += (x, z, s)
+__global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long sz, double *s, long long ss, int acc) {
+    PB_SETUP
     x += b * sx; z += b * sz; s += b * ss;
     for (int i = tid; i < p.m; i += nt) {
-        const double zv = p.bzp[om + i], sv = s[i] - zv;
+        double sv = s[i];
+        const double zv = f4_post_row(p, om + i, sv);
         z[i] = zv; s[i] = sv;
         if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
     }
@@ -573,18 +430,17 @@ __global__ void kc_f4_post(CPtrs cp, double *x, long long sx, double *z, long lo
 }
 // refinement residual, the elementwise part of res() (coneprog.py:1930-1960): wx2 = wx, wz3 = W^{-1} dz,
 // wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds).  The P, G and G' products follow as batched GEMVs.
-__global__ void kc_res(CPtrs cp) {
-    CB_SETUP
-    (void)sh; (void)S;
+__global__ void k_res(Ptrs p) {
+    PB_SETUP
     const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om;
-    for (int i = tid; i < p.n; i += nt) cp.wx2[oc + i] = cp.wx[oc + i];
-    double *wz3 = cp.wz3 + oc, *wz2 = cp.wz2 + oc, *ws2 = cp.ws2 + oc;
-    for (int i = tid; i < cp.ml; i += nt) {
+    for (int i = tid; i < p.n; i += nt) p.wx2[oc + i] = p.wx[oc + i];
+    double *wz3 = p.wz3 + oc, *wz2 = p.wz2 + oc, *ws2 = p.ws2 + oc;
+    for (int i = tid; i < p.ml; i += nt) {
         wz3[i] = p.di[om + i] * dz[i];
-        wz2[i] = cp.wz[oc + i] - p.d[om + i] * ds[i];
-        ws2[i] = cp.ws[oc + i] - l[i] * (dz[i] + ds[i]);
+        wz2[i] = p.wz[oc + i] - p.d[om + i] * ds[i];
+        ws2[i] = p.ws[oc + i] - l[i] * (dz[i] + ds[i]);
     }
-    const double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
+    const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) {
         q_scale(v + o, beta[k_], dz + o, wz3 + o, len, lane, true);
         q_scale(v + o, beta[k_], ds + o, wz2 + o, len, lane, false);
@@ -593,27 +449,33 @@ __global__ void kc_res(CPtrs cp) {
         a = warp_sum(a);
         const double u0 = ds[o] + dz[o], l0 = l[o];
         FOR_LANE(i, len) {
-            wz2[o + i] = cp.wz[oc + o + i] - wz2[o + i];
-            ws2[o + i] = cp.ws[oc + o + i] - ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]);
+            wz2[o + i] = p.wz[oc + o + i] - wz2[o + i];
+            ws2[o + i] = p.ws[oc + o + i] - ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]);
         }
     }
 }
-// after the i-th direction: ds o dz, scale2 of ds and dz, step length, sigma (coneprog.py:2423-2456)
-__global__ void kc_dir_post(CPtrs cp, int i) {
-    CB_SETUP
-    (void)on;
+// after the i-th direction: ds o dz, scale2 of ds and dz, step length, sigma (coneprog.py:2423-2456).
+// f4_post: the solve has just run without refinement, so f4_no_ir's step after it is done here first
+template <bool CONES> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
+    PB_SETUP
     double *ds = p.ds + om, *dz = p.dz + om;
     const double *l = p.lmbda + om;
     double dsdz = 0, mins = INFINITY, minz = INFINITY;
-    for (int k = tid; k < cp.ml; k += nt) {
-        const double s = ds[k], z = dz[k];
+#pragma unroll 1                                         // as in k_dir_rhs
+    for (int k = tid; k < p.ml; k += nt) {
+        double s = ds[k];
+        const double z = f4_post ? f4_post_row(p, om + k, s) : dz[k];
         dsdz += s * z;
         if (i == 0) p.ws3[om + k] = s * z;
         const double ss = s / l[k], zs = z / l[k];
         ds[k] = ss; dz[k] = zs;
         mins = fmin(mins, ss); minz = fmin(minz, zs);
     }
-    FOR_CONES(o, len) {
+    if (CONES && f4_post) {
+        for (int k = p.ml + tid; k < p.m; k += nt) dz[k] = f4_post_row(p, om + k, ds[k]);
+        __syncthreads();
+    }
+    if (CONES) FOR_CONES(o, len) {
         double a = 0;
         FOR_LANE(k, len) a += ds[o + k] * dz[o + k];
         a = warp_sum(a);
@@ -646,8 +508,8 @@ __global__ void kc_dir_post(CPtrs cp, int i) {
 }
 // x += step dx; ds, dz := e + step d; scale2 inverse; update_scaling (misc.py:439-573); s = W' lmbda,
 // z = W^{-1} lmbda; gap (coneprog.py:2459-2547)
-__global__ void kc_update(CPtrs cp, const int *info, int iter) {
-    CB_SETUP
+template <bool CONES> __global__ void k_update(Ptrs p, const int *info, int iter) {
+    PB_SETUP
     if (S.done) return;
     if (info[b] > 0) {      // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
         if (tid == 0) { S.done = 1; S.status = 3; S.iters = iter; }
@@ -657,19 +519,20 @@ __global__ void kc_update(CPtrs cp, const int *info, int iter) {
     for (int k = tid; k < p.n; k += nt) p.x[on + k] += step * p.dx[on + k];
     double *ds = p.ds + om, *dz = p.dz + om, *l = p.lmbda + om, *s = p.s + om, *z = p.z + om;
     double gap = 0;
-    for (int k = tid; k < cp.ml; k += nt) {
+    for (int k = tid; k < p.ml; k += nt) {
         const double lk = l[k];
         const double ss = sqrt((1.0 + step * ds[k]) * lk), sz = sqrt((1.0 + step * dz[k]) * lk);
-        const double d = p.d[om + k] * ss / sz;
+        const double d = p.d[om + k] * ss / sz, di = 1.0 / d;
         const double ln = ss * sz;
-        p.d[om + k] = d; p.di[om + k] = 1.0 / d;
+        p.d[om + k] = d; p.di[om + k] = di;
+        if (!CONES) p.di2[om + k] = di * di;
         l[k] = ln;
         s[k] = d * ln;
-        z[k] = (1.0 / d) * ln;
+        z[k] = di * ln;
         gap += ln * ln;
     }
-    double *v = cp.v + oc - cp.ml, *beta = cp.beta + oc;
-    FOR_CONES(o, len) {
+    double *v = p.v + oc - p.ml, *beta = p.beta + oc;
+    if (CONES) FOR_CONES(o, len) {
         FOR_LANE(k, len) {
             ds[o + k] = step * ds[o + k] + (k == 0 ? 1.0 : 0.0);
             dz[o + k] = step * dz[o + k] + (k == 0 ? 1.0 : 0.0);
@@ -719,13 +582,6 @@ __global__ void kc_update(CPtrs cp, const int *info, int iter) {
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
-// swap rows i and j of a [slots x L] buffer for each pair
-__global__ void kc_swap_rows(double *a, long long L, const int *pairs) {
-    const long long i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < L; e += (long long)gridDim.x * blockDim.x) {
-        const double t = a[i * L + e]; a[i * L + e] = a[j * L + e]; a[j * L + e] = t;
-    }
-}
 
 }  // namespace
 
@@ -737,7 +593,7 @@ struct cvxb_batch {
     DevBuf<double> P, G, K, inv, panel, gemv_ws;
     DevBuf<double> vecs;             // all n- and m-vectors
     double *q = nullptr, *h = nullptr;   // in vecs
-    Ptrs p;
+    Ptrs p;                          // also holds the dims ('l' rows p.ml, p.nq cones) and p.refinement
     DevBuf<Scal> sc;
     DevBuf<int> d_info, d_ndone;
     DevBuf<int> d_done, d_pairs, d_perm;     // compaction: done flags, swap list, slot -> problem
@@ -752,18 +608,15 @@ struct cvxb_batch {
     int iters_run = 0;
     double solve_ms = 0;
     // single large problem: SYRK on the int8 tensor path (ozaki_syrk.cu), same rule as cvxb_kkt_factor
-    // (ozaki_use) when B == 1; ozaki_mode() at create
+    // (ozaki_use) when B == 1 and there are no 'q' cones; ozaki_mode() at create
     int i8_mode = 0;
     int syrk_path = 0;
     DevBuf<char> oz_work;
-    // cone path (cvxb_batch_create_cones / cvxb_batch_set_refinement): rows [0, ml) are 'l', then the 'q' cones
-    int ml = 0, refinement = 0;
-    std::vector<int> qdims;          // dims['q']
+    // 'q' cones (cvxb_batch_create_cones): rows [0, p.ml) are 'l', then the cones
     DevBuf<int> qoff;                // nq + 1 row offsets
-    DevBuf<double> Gs;               // W^{-T} G per slot (ld ldg), rebuilt every factorisation
-    DevBuf<double> cst;              // per-slot state row: v, beta, refinement vectors (moves with its problem)
+    DevBuf<double> Gs;               // W^{-T} G per slot (ld ldg), rebuilt every factorisation; only with 'q' cones
+    DevBuf<double> cst;              // per-slot state row (moves with its problem); empty without cones and refinement
     long long L = 0;
-    CPtrs cp;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -773,28 +626,57 @@ struct cvxb_batch {
 
 namespace {
 
+// The per-slot state row: v (sum q) | beta (nq) with cones, wx wx2 (n) | wz ws wz2 ws2 wz3 (m) with refinement;
+// every piece starts 16-byte aligned.  Reallocated when the layout changes: nothing in it outlives a solve.
+int state_alloc(cvxb_batch *b) {
+    Ptrs &p = b->p;
+    auto ev = [](long long x) { return (x + 1) & ~1LL; };
+    const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m);
+    const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 : 0;
+    if (b->L == cone + ref) return 0;
+    b->L = p.L = 0;
+    b->cst.reset();
+    p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = nullptr;
+    if (cone + ref == 0) return 0;
+    CVXB_TRY(b->cst.alloc((size_t)b->B * (cone + ref)));
+    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * (cone + ref) * sizeof(double)));
+    b->L = p.L = cone + ref;
+    double *r = b->cst.p;
+    if (cone) { p.v = r; r += ev(sumq); p.beta = r; r += ev(p.nq); }
+    if (ref) {
+        p.wx = r; r += n2; p.wx2 = r; r += n2;
+        p.wz = r; r += m2; p.ws = r; r += m2; p.wz2 = r; r += m2; p.ws2 = r; r += m2; p.wz3 = r;
+    }
+    return 0;
+}
+
+// K = P + Gs' Gs with Gs = W^{-T} G (misc.py:1267-1282), then its Cholesky factor.  With 'q' cones Gs is formed;
+// without, diag(di)² is applied inside the SYRK (w = di2), or by the int8 slicing for a single large problem.
 int batch_factor(cvxb_batch *b) {
     cudaStream_t st = b->st;
+    const bool cones = b->p.nq > 0;
+    if (cones) {
+        k_build_gs<<<dim3((b->n + 7) / 8, b->Bact), 256, 0, st>>>(b->p, b->G.p, b->Gs.p, b->ldg, b->sG);
+        count_launch();
+    }
     // K = P + G' diag(di)^2 G from nine int8 slices per entry (fp64-accurate, ~1.8x the DMMA SYRK)
-    const bool i8 = b->B == 1 && b->m > 0 && ozaki_use(b->i8_mode, b->n, b->m, b->oz_work);
+    const bool i8 = !cones && b->B == 1 && b->m > 0 && ozaki_use(b->i8_mode, b->n, b->m, b->oz_work);
     b->syrk_path = i8 ? 2 : 1;
     if (i8) {
         CVXB_TRY(ozaki_syrk(b->n, b->m, b->G.p, b->ldg, b->p.di, b->P.p, b->ldp, 1.0, b->K.p, b->ldk, 9, 0,
                             b->oz_work.p, st));
-        CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
-        return 0;
+    } else {
+        GemmDesc g;
+        g.M = b->n; g.N = b->n; g.K = b->m;
+        g.X = cones ? b->Gs.p : b->G.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
+        g.Y = g.X; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
+        if (!cones) { g.w = b->p.di2; g.sW = b->m; }
+        g.D = b->P.p; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
+        g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
+        g.lower_only = true; g.batch = b->Bact;
+        if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
+        CVXB_TRY(dmma_gemm(g, st));
     }
-    GemmDesc g;
-    g.M = b->n; g.N = b->n; g.K = b->m;
-    g.X = b->G.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
-    g.Y = b->G.p; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
-    g.w = b->p.di2; g.sW = b->m;
-    g.D = b->P.p; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
-    g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
-    g.lower_only = true; g.batch = b->Bact;
-    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
-    CVXB_TRY(dmma_gemm(g, st));
     if (b->B == 1) {
         CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
         CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -805,242 +687,52 @@ int batch_factor(cvxb_batch *b) {
     return 0;
 }
 
-// (dx, bzp) := solution of the reduced KKT system; on entry dx = bx, bzp = W^{-T} bz
-int batch_solve(cvxb_batch *b) {
+// (x, bzp) := solution of the reduced KKT system; on entry x = bx (slot k at x + k*sx), bzp = W^{-T} bz.
+// Gs is G with the weights di when it is not formed.
+int batch_solve(cvxb_batch *b, double *x, long long sx) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, B = b->Bact;
-    GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sw = m; gt.sx = m; gt.sy = n;
-    // x := x + G' (di .* bzp)
-    CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, b->p.di, b->p.bzp, 1.0, 1.0, b->p.dx, st, gt));
-    CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, b->p.dx, b->cw, st, B, b->sK, b->sInv, n));
-    // bzp := di .* (G x) - bzp
-    GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sw = m; gn.sx = n; gn.sy = m;
-    CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, b->p.di, b->p.dx, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
-    return 0;
-}
-
-// ---- cone path ----
-bool cone_path(const cvxb_batch *b) { return !b->qdims.empty() || (b->refinement > 0 && b->m > 0); }
-
-// the offset table and the buffers only the cone path uses
-int cone_alloc(cvxb_batch *b) {
-    if (b->cst.p) return 0;
-    const int nq = (int)b->qdims.size();
-    std::vector<int> off(nq + 1, b->ml);
-    for (int k = 0; k < nq; ++k) off[k + 1] = off[k] + b->qdims[k];
-    CVXB_TRY(b->qoff.alloc(nq + 1));
-    CVXB_CUDA(cudaMemcpy(b->qoff.p, off.data(), (nq + 1) * sizeof(int), cudaMemcpyHostToDevice));
-    CVXB_TRY(b->Gs.alloc((size_t)b->B * b->sG));
-    // state row: v (sum q) | beta (nq) | wx wx2 (n) | wz ws wz2 ws2 wz3 (m); every piece starts 16-byte aligned
-    auto ev = [](long long x) { return (x + 1) & ~1LL; };
-    const long long sumq = b->m - b->ml, n2 = ev(b->n), m2 = ev(b->m);
-    b->L = ev(sumq) + ev(nq) + 2 * n2 + 5 * m2;
-    CVXB_TRY(b->cst.alloc((size_t)b->B * b->L));
-    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * b->L * sizeof(double)));
-    CPtrs &c = b->cp;
-    double *r = b->cst.p;
-    c.v = r; r += ev(sumq);
-    c.beta = r; r += ev(nq);
-    c.wx = r; r += n2; c.wx2 = r; r += n2;
-    c.wz = r; r += m2; c.ws = r; r += m2; c.wz2 = r; r += m2; c.ws2 = r; r += m2; c.wz3 = r;
-    c.ml = b->ml; c.nq = nq; c.qoff = b->qoff.p; c.L = b->L;
-    return 0;
-}
-
-// K = P + Gs' Gs with Gs = W^{-T} G (misc.py:1267-1282), then its Cholesky factor
-int cone_factor(cvxb_batch *b) {
-    cudaStream_t st = b->st;
-    kc_build_gs<<<dim3((b->n + 7) / 8, b->Bact), 256, 0, st>>>(b->cp, b->G.p, b->Gs.p, b->ldg, b->sG);
-    count_launch();
-    b->syrk_path = 1;
-    GemmDesc g;
-    g.M = b->n; g.N = b->n; g.K = b->m;
-    g.X = b->Gs.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
-    g.Y = b->Gs.p; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
-    g.D = b->P.p; g.ldd = (int)b->ldp; g.sD = b->sP; g.beta = 1.0;
-    g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
-    g.lower_only = true; g.batch = b->Bact;
-    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
-    CVXB_TRY(dmma_gemm(g, st));
-    if (b->B == 1) {
-        CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
-        CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
-    } else {
-        CVXB_TRY(potrf_lower_batched(b->n, b->K.p, (int)b->ldk, b->sK, b->inv.p, b->sInv, b->Bact, b->d_info.p,
-                                     b->panel.p, (b->n + 1) & ~1, st));
-    }
-    return 0;
-}
-
-// (x, bzp) := solution of the reduced KKT system on Gs; on entry x = bx (slot k at x + k*sx), bzp = W^{-T} bz
-int cone_solve(cvxb_batch *b, double *x, long long sx) {
-    cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact;
-    GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = m; gt.sy = sx;
-    CVXB_TRY(gemv_t(m, n, b->Gs.p, b->ldg, nullptr, b->p.bzp, 1.0, 1.0, x, st, gt));
+    const bool cones = b->p.nq > 0;
+    const double *A = cones ? b->Gs.p : b->G.p, *w = cones ? nullptr : b->p.di;
+    const long long sw = w ? m : 0;
+    // x := x + Gs' bzp
+    GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sw = sw; gt.sx = m; gt.sy = sx;
+    CVXB_TRY(gemv_t(m, n, A, b->ldg, w, b->p.bzp, 1.0, 1.0, x, st, gt));
     CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, b->cw, st, B, b->sK, b->sInv, sx));
-    GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = sx; gn.sy = m;
-    CVXB_TRY(gemv_n(m, n, b->Gs.p, b->ldg, nullptr, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
+    // bzp := Gs x - bzp
+    GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sw = sw; gn.sx = sx; gn.sy = m;
+    CVXB_TRY(gemv_n(m, n, A, b->ldg, w, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
     return 0;
 }
 
-// f4_no_ir (coneprog.py:2288-2316) on (x, z, s); acc: add the result to (dx, dz, ds) (the refinement step)
-int cone_f4_no_ir(cvxb_batch *b, double *x, long long sx, double *z, long long sz, double *s, long long ss, int acc) {
-    const int B = b->Bact;
-    kc_f4_pre<<<B, 256, 0, b->st>>>(b->cp, z, sz, s, ss); count_launch();
-    CVXB_TRY(cone_solve(b, x, sx));
-    kc_f4_post<<<B, 256, 0, b->st>>>(b->cp, x, sx, z, sz, s, ss, acc); count_launch();
-    return 0;
-}
-
-// f4 (coneprog.py:2330-2347): f4_no_ir on (dx, dz, ds), then `refinement` correction steps from the residual
-int cone_f4(cvxb_batch *b) {
+// the i-th Newton direction: f4 (coneprog.py:2288-2347) on the right-hand side, i.e. f4_no_ir and then `refinement`
+// correction steps from the residual, followed by the step length and sigma
+template <bool CONES> int direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact;
-    const CPtrs &c = b->cp;
+    const int n = b->n, m = b->m, B = b->Bact, T = 256;
+    const Ptrs &p = b->p;
     const long long L = b->L;
-    CVXB_TRY(cone_f4_no_ir(b, c.p.dx, n, c.p.dz, m, c.p.ds, m, 0));
-    for (int r = 0; r < b->refinement; ++r) {
-        kc_res<<<B, 256, 0, st>>>(c); count_launch();
+    k_dir_rhs<CONES><<<B, T, 0, st>>>(p, i); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n));
+    if (p.refinement) { k_f4_post<<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
+    for (int r = 0; r < p.refinement; ++r) {
+        k_res<<<B, T, 0, st>>>(p); count_launch();
         GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
-        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, c.p.dx, -1.0, 1.0, c.wx2, st, gP));
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
         GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, c.wz3, -1.0, 1.0, c.wx2, st, gt));
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
         GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
-        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, c.p.dx, -1.0, 1.0, c.wz2, b->gemv_ws.p, st, gn));
-        CVXB_TRY(cone_f4_no_ir(b, c.wx2, L, c.wz2, L, c.ws2, L, 1));
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
+        k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
+        CVXB_TRY(batch_solve(b, p.wx2, L));
+        k_f4_post<<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1); count_launch();
     }
-    return 0;
-}
-
-}  // namespace
-
-extern "C" {
-
-int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
-    if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
-    if (nprob > CVXB_BATCH_MAX) {
-        set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    *out = nullptr;
-    CVXB_TRY(check_device(device));
-    std::unique_ptr<cvxb_batch> b(new cvxb_batch());
-    b->device = device; b->B = nprob; b->n = n; b->m = m; b->ml = m;
-    b->i8_mode = ozaki_mode();
-    b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
-    b->ldp = b->ldk = (n + 1) & ~1;
-    b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;
-    b->nblk = (n + NB - 1) / NB;
-    b->sInv = (long long)2 * b->nblk * NB * NB;
-    const size_t B = nprob;
-    CVXB_CUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
-    CVXB_CUDA(cudaEventCreate(&b->e0)); CVXB_CUDA(cudaEventCreate(&b->e1));
-    CVXB_TRY(chol_work_create(b->cw));
-    CVXB_TRY(b->P.alloc(B * b->sP));
-    CVXB_TRY(b->G.alloc(B * b->sG));
-    CVXB_TRY(b->K.alloc(B * b->sK));
-    CVXB_TRY(b->inv.alloc(B * b->sInv));
-    CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
-    CVXB_TRY(b->gemv_ws.alloc(B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n)));
-    // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
-    const size_t nv = 4, mv = 13;
-    const size_t me = (size_t)(m > 0 ? m : 1);
-    CVXB_TRY(b->vecs.alloc(B * (nv * n + mv * me)));
-    CVXB_CUDA(cudaMemset(b->vecs.p, 0, B * (nv * n + mv * me) * sizeof(double)));
-    double *v = b->vecs.p;
-    auto take = [&](size_t len) { double *r = v; v += B * len; return r; };
-    b->q = take(n); b->p.x = take(n); b->p.rx = take(n); b->p.dx = take(n);
-    b->h = take(me); b->p.s = take(me); b->p.z = take(me); b->p.rz = take(me); b->p.ds = take(me);
-    b->p.dz = take(me); b->p.lmbda = take(me); b->p.lmbdasq = take(me); b->p.d = take(me);
-    b->p.di = take(me); b->p.di2 = take(me); b->p.ws3 = take(me); b->p.bzp = take(me);
-    b->p.q = b->q; b->p.h = b->h; b->p.n = n; b->p.m = m;
-    CVXB_TRY(b->sc.alloc(B));
-    CVXB_CUDA(cudaMemset(b->sc.p, 0, B * sizeof(Scal)));
-    b->p.sc = b->sc.p;
-    CVXB_TRY(b->d_info.alloc(B));
-    CVXB_TRY(b->d_ndone.alloc(1));
-    CVXB_TRY(b->d_done.alloc(B));
-    CVXB_TRY(b->d_pairs.alloc(2 * B));
-    CVXB_TRY(b->d_perm.alloc(B));
-    b->perm.resize(B);
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
-    *out = b.release();
-    return 0;
-}
-
-int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
-    if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
-    if (nprob > CVXB_BATCH_MAX) {
-        set_error("batch_create_cones: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob,
-                  CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    *out = nullptr;
-    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("batch_create_cones: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
-        return CVXB_E_ARG;
-    }
-    long long m = dims->ml;
-    for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("batch_create_cones: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
-        m += dims->q[k];
-    }
-    if (m > (1LL << 30)) { set_error("batch_create_cones: too many cone rows"); return CVXB_E_ARG; }
-    if (dims->ns > 0) { set_error("batch_create_cones: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
-    cvxb_batch *b = nullptr;
-    CVXB_TRY(cvxb_batch_create(&b, nprob, n, (int)m, device));
-    std::unique_ptr<cvxb_batch> own(b);
-    b->ml = dims->ml;
-    b->qdims.assign(dims->q, dims->q + dims->nq);
-    b->refinement = dims->nq > 0 ? 1 : 0;        // coneqp's default (coneprog.py:1862-1865)
-    if (cone_path(b)) CVXB_TRY(cone_alloc(b));
-    *out = own.release();
-    return 0;
-}
-
-int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
-    if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
-    CVXB_CUDA(cudaSetDevice(b->device));
-    b->refinement = refinement;
-    if (cone_path(b)) CVXB_TRY(cone_alloc(b));
-    return 0;
-}
-
-void cvxb_batch_destroy(cvxb_batch *b) {
-    if (!b) return;
-    cudaSetDevice(b->device);
-    delete b;
-}
-
-// P: nprob x (n x n, ld n) ; q: nprob x n ; G: nprob x (m x n column-major, ld m) ; h: nprob x m
-int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
-                    const double *h, int space) {
-    if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
-    CVXB_CUDA(cudaSetDevice(b->device));
-    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const size_t B = b->B, n = b->n, m = b->m;
-    // one strided 2-D copy per operand: rows of the "matrix of columns" are the matrix columns
-    CVXB_CUDA(cudaMemcpy2DAsync(b->P.p, b->ldp * sizeof(double), P, n * sizeof(double), n * sizeof(double),
-                                n * B, kind, b->st));
-    if (m > 0) {
-        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double),
-                                    m * sizeof(double), n * B, kind, b->st));
-        CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
-    }
-    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
-    // only tril(P) is significant in the reference; make the resident copies symmetric
-    CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
+    k_dir_post<CONES><<<B, T, 0, st>>>(p, i, p.refinement == 0); count_launch();
     return 0;
 }
 
 // swap the slots of each pair (disjoint pairs: one launch)
-static int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
+int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     const int np = (int)pairs.size() / 2;
     if (np == 0) return 0;
     CVXB_CUDA(cudaMemcpyAsync(b->d_pairs.p, pairs.data(), pairs.size() * sizeof(int), cudaMemcpyHostToDevice, b->st));
@@ -1050,7 +742,7 @@ static int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs.p);
     count_launch();
     if (b->cst.p) {
-        kc_swap_rows<<<dim3(8, np), 256, 0, b->st>>>(b->cst.p, b->L, b->d_pairs.p);
+        k_swap_rows<<<dim3(8, np), 256, 0, b->st>>>(b->cst.p, b->L, b->d_pairs.p);
         count_launch();
     }
     // `pairs` is pageable host memory: the copy above is staged before cudaMemcpyAsync returns
@@ -1058,7 +750,7 @@ static int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
 }
 
 // put every problem back into its own slot (a solve that compacted left them permuted)
-static int restore_order(cvxb_batch *b) {
+int restore_order(cvxb_batch *b) {
     if (!b->permuted) return 0;
     std::vector<int> pr(2);
     for (int i = 0; i < b->B; ++i) {
@@ -1074,16 +766,13 @@ static int restore_order(cvxb_batch *b) {
     return 0;
 }
 
-// the lock-step loop of cvxb_batch_solve for the cone path: same residuals, stopping rule and compaction; the
-// scaling, the Newton directions (with refinement) and the update are the kc_* kernels
-static int cone_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+// the lock-step IPM over the active slots; CONES: the batch has 'q' cones
+template <bool CONES> int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256;
-    int B = b->B;
+    int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
     b->Bact = B;
-    Ptrs &p = b->p;
-    CPtrs &cp = b->cp;
-    cp.p = p; cp.refinement = b->refinement;
+    const Ptrs &p = b->p;
     GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
     GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
     GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
@@ -1091,11 +780,10 @@ static int cone_batch_solve(cvxb_batch *b, int maxiters, double abstol, double r
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I ----
     k_init_rhs<<<B, T, 0, st>>>(p); count_launch();
-    kc_init_w<<<B, T, 0, st>>>(cp); count_launch();
-    CVXB_TRY(cone_factor(b));
-    kc_scale_bz<<<B, T, 0, st>>>(cp); count_launch();
-    CVXB_TRY(cone_solve(b, p.dx, n));
-    kc_init_point<<<B, T, 0, st>>>(cp); count_launch();
+    CVXB_TRY(batch_factor(b));
+    k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n));
+    k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
     CVXB_LAUNCH_CHECK();
     {
         // a singular first factorisation is the reference's "Rank([P; G]) < n" ValueError
@@ -1107,93 +795,6 @@ static int cone_batch_solve(cvxb_batch *b, int maxiters, double abstol, double r
                 set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
                 return CVXB_E_ARG;
             }
-    }
-    std::vector<int> flags(B), pairs;
-    int it = 0;
-    for (it = 0; it <= maxiters; ++it) {
-        // residuals (:2169-2186): row-wise, so the 'l' kernels serve every cone row
-        k_res_begin<<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
-        k_res_dots<<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
-        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
-        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_stats<<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p); count_launch();
-        int ndone = 0;
-        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        if (ndone >= B) break;
-        if (ndone > 0 && b->compact && b->B > 1) {
-            const int nb = B - ndone;
-            pairs.clear();
-            int j = B - 1;
-            for (int i = 0; i < nb; ++i) {
-                if (!flags[i]) continue;
-                while (flags[j]) --j;
-                pairs.push_back(i); pairs.push_back(j);
-                std::swap(b->perm[i], b->perm[j]);
-                --j;
-            }
-            CVXB_TRY(swap_slots(b, pairs));
-            b->permuted = true;
-            B = nb;
-            b->Bact = B;
-            gP.batch = gGt.batch = gGn.batch = B;
-        }
-        kc_scaling<<<B, T, 0, st>>>(cp, it == 0 ? 1 : 0); count_launch();
-        CVXB_TRY(cone_factor(b));
-        for (int i = 0; i < 2; ++i) {
-            kc_dir_rhs<<<B, T, 0, st>>>(cp, i); count_launch();
-            CVXB_TRY(cone_f4(b));
-            kc_dir_post<<<B, T, 0, st>>>(cp, i); count_launch();
-        }
-        kc_update<<<B, T, 0, st>>>(cp, b->d_info.p, it); count_launch();
-        CVXB_LAUNCH_CHECK();
-    }
-    b->iters_run = it;
-    b->Bact = b->B;
-    CVXB_CUDA(cudaEventRecord(b->e1, st));
-    CVXB_CUDA(cudaStreamSynchronize(st));
-    float t = 0;
-    cudaEventElapsedTime(&t, b->e0, b->e1);
-    b->solve_ms = t;
-    return 0;
-}
-
-int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
-    if (!b || !b->loaded) { set_error("batch_solve: load the problems first"); return CVXB_E_ARG; }
-    CVXB_CUDA(cudaSetDevice(b->device));
-    cudaStream_t st = b->st;
-    CVXB_TRY(restore_order(b));
-    if (cone_path(b)) return cone_batch_solve(b, maxiters, abstol, reltol, feastol);
-    const int n = b->n, m = b->m, T = 256;
-    int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
-    b->Bact = B;
-    Ptrs &p = b->p;
-    GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
-    GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
-    GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
-    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
-    CVXB_CUDA(cudaEventRecord(b->e0, st));
-    // ---- starting point: W = I ----
-    k_init_rhs<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_factor(b));
-    k_scale_bz<<<B, T, 0, st>>>(p, p.dz); count_launch();
-    CVXB_TRY(batch_solve(b));
-    k_init_point<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_LAUNCH_CHECK();
-    int info_fail = 0;
-    {
-        // a singular first factorisation is the reference's "Rank([P; G]) < n" ValueError
-        std::vector<int> info(B);
-        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        for (int i = 0; i < B; ++i) if (info[i] > 0) { info_fail = i + 1; break; }
-        if (info_fail) {
-            set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", info_fail - 1);
-            return CVXB_E_ARG;
-        }
     }
     std::vector<int> flags(B), pairs;
     int it = 0;
@@ -1231,14 +832,10 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
             b->Bact = B;
             gP.batch = gGt.batch = gGn.batch = B;
         }
-        k_scaling<<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
+        k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         CVXB_TRY(batch_factor(b));
-        for (int i = 0; i < 2; ++i) {
-            k_dir_prep<<<B, T, 0, st>>>(p, i); count_launch();
-            CVXB_TRY(batch_solve(b));
-            k_dir_post<<<B, T, 0, st>>>(p, i); count_launch();
-        }
-        k_update<<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
+        for (int i = 0; i < 2; ++i) CVXB_TRY(direction<CONES>(b, i));
+        k_update<CONES><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -1249,6 +846,149 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     cudaEventElapsedTime(&t, b->e0, b->e1);
     b->solve_ms = t;
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
+    if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
+    if (nprob > CVXB_BATCH_MAX) {
+        set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    *out = nullptr;
+    CVXB_TRY(check_device(device));
+    std::unique_ptr<cvxb_batch> b(new cvxb_batch());
+    b->device = device; b->B = nprob; b->n = n; b->m = m;
+    b->i8_mode = ozaki_mode();
+    b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
+    b->ldp = b->ldk = (n + 1) & ~1;
+    b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;
+    b->nblk = (n + NB - 1) / NB;
+    b->sInv = (long long)2 * b->nblk * NB * NB;
+    const size_t B = nprob;
+    CVXB_CUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
+    CVXB_CUDA(cudaEventCreate(&b->e0)); CVXB_CUDA(cudaEventCreate(&b->e1));
+    CVXB_TRY(chol_work_create(b->cw));
+    CVXB_TRY(b->P.alloc(B * b->sP));
+    CVXB_TRY(b->G.alloc(B * b->sG));
+    CVXB_TRY(b->K.alloc(B * b->sK));
+    CVXB_TRY(b->inv.alloc(B * b->sInv));
+    CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
+    CVXB_TRY(b->gemv_ws.alloc(B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n)));
+    // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
+    const size_t nv = 4, mv = 13;
+    const size_t me = (size_t)(m > 0 ? m : 1);
+    CVXB_TRY(b->vecs.alloc(B * (nv * n + mv * me)));
+    CVXB_CUDA(cudaMemset(b->vecs.p, 0, B * (nv * n + mv * me) * sizeof(double)));
+    double *v = b->vecs.p;
+    auto take = [&](size_t len) { double *r = v; v += B * len; return r; };
+    Ptrs &p = b->p;
+    p = Ptrs{};
+    b->q = take(n); p.x = take(n); p.rx = take(n); p.dx = take(n);
+    b->h = take(me); p.s = take(me); p.z = take(me); p.rz = take(me); p.ds = take(me);
+    p.dz = take(me); p.lmbda = take(me); p.lmbdasq = take(me); p.d = take(me);
+    p.di = take(me); p.di2 = take(me); p.ws3 = take(me); p.bzp = take(me);
+    p.q = b->q; p.h = b->h; p.n = n; p.m = m; p.ml = m;
+    CVXB_TRY(b->sc.alloc(B));
+    CVXB_CUDA(cudaMemset(b->sc.p, 0, B * sizeof(Scal)));
+    p.sc = b->sc.p;
+    CVXB_TRY(b->d_info.alloc(B));
+    CVXB_TRY(b->d_ndone.alloc(1));
+    CVXB_TRY(b->d_done.alloc(B));
+    CVXB_TRY(b->d_pairs.alloc(2 * B));
+    CVXB_TRY(b->d_perm.alloc(B));
+    b->perm.resize(B);
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
+    *out = b.release();
+    return 0;
+}
+
+int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
+    if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
+    if (nprob > CVXB_BATCH_MAX) {
+        set_error("batch_create_cones: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob,
+                  CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    *out = nullptr;
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("batch_create_cones: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
+        return CVXB_E_ARG;
+    }
+    long long m = dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("batch_create_cones: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
+        m += dims->q[k];
+    }
+    if (m > (1LL << 30)) { set_error("batch_create_cones: too many cone rows"); return CVXB_E_ARG; }
+    if (dims->ns > 0) { set_error("batch_create_cones: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    cvxb_batch *b = nullptr;
+    CVXB_TRY(cvxb_batch_create(&b, nprob, n, (int)m, device));
+    std::unique_ptr<cvxb_batch> own(b);
+    if (dims->nq > 0) {
+        const int nq = dims->nq;
+        std::vector<int> off(nq + 1, dims->ml);
+        for (int k = 0; k < nq; ++k) off[k + 1] = off[k] + dims->q[k];
+        CVXB_TRY(b->qoff.alloc(nq + 1));
+        CVXB_CUDA(cudaMemcpy(b->qoff.p, off.data(), (nq + 1) * sizeof(int), cudaMemcpyHostToDevice));
+        CVXB_TRY(b->Gs.alloc((size_t)b->B * b->sG));
+        b->p.ml = dims->ml; b->p.nq = nq; b->p.qoff = b->qoff.p;
+        b->p.refinement = 1;                      // coneqp's default with 'q' cones (coneprog.py:1862-1865)
+        CVXB_TRY(state_alloc(b));
+    }
+    *out = own.release();
+    return 0;
+}
+
+int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
+    if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    b->p.refinement = b->m > 0 ? refinement : 0;     // a batch without constraint rows takes unrefined steps
+    CVXB_TRY(state_alloc(b));
+    return 0;
+}
+
+void cvxb_batch_destroy(cvxb_batch *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    delete b;
+}
+
+// P: nprob x (n x n, ld n) ; q: nprob x n ; G: nprob x (m x n column-major, ld m) ; h: nprob x m
+int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
+                    const double *h, int space) {
+    if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const size_t B = b->B, n = b->n, m = b->m;
+    // one strided 2-D copy per operand: rows of the "matrix of columns" are the matrix columns
+    CVXB_CUDA(cudaMemcpy2DAsync(b->P.p, b->ldp * sizeof(double), P, n * sizeof(double), n * sizeof(double),
+                                n * B, kind, b->st));
+    if (m > 0) {
+        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double),
+                                    m * sizeof(double), n * B, kind, b->st));
+        CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
+    }
+    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
+    // only tril(P) is significant in the reference; make the resident copies symmetric
+    CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    b->permuted = false;
+    return 0;
+}
+
+int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+    if (!b || !b->loaded) { set_error("batch_solve: load the problems first"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    CVXB_TRY(restore_order(b));
+    return b->p.nq > 0 ? solve_lockstep<true>(b, maxiters, abstol, reltol, feastol)
+                       : solve_lockstep<false>(b, maxiters, abstol, reltol, feastol);
 }
 
 int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *status, int *iters,

@@ -248,6 +248,41 @@ __device__ __forceinline__ double warp_sum(double v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
+__device__ __forceinline__ double warp_min(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+// Sum / min over the CTA (blockDim.x a multiple of 32), returned to every thread: warp reductions, then warp 0
+// reduces the per-warp values.  sh holds 32 doubles of shared memory and is free again when the call returns.
+__device__ __forceinline__ double block_sum(double v, double *sh) {
+    v = warp_sum(v);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.0;
+    if (warp == 0) t = warp_sum(t);
+    if (threadIdx.x == 0) sh[0] = t;
+    __syncthreads();
+    const double r = sh[0];
+    __syncthreads();
+    return r;
+}
+__device__ __forceinline__ double block_min(double v, double *sh) {
+    v = warp_min(v);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : INFINITY;
+    if (warp == 0) t = warp_min(t);
+    if (threadIdx.x == 0) sh[0] = t;
+    __syncthreads();
+    const double r = sh[0];
+    __syncthreads();
+    return r;
+}
 __device__ __forceinline__ int ld_acquire(const int *p) {
     int v;
     asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");

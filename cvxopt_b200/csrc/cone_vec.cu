@@ -16,18 +16,6 @@ using namespace cvxb;
 
 namespace {
 
-__device__ __forceinline__ double blk_sum(double v, double *sh) {
-    v = warp_sum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.0;
-    if (threadIdx.x < 32) t = warp_sum(t);
-    if (threadIdx.x == 0) sh[0] = t;
-    __syncthreads();
-    return sh[0];
-}
-
 struct Cones {
     int nl;                     // mnl + ml
     int nq; const int *q;       // device arrays
@@ -44,7 +32,7 @@ __global__ void scale2_kernel(const double *lm, double *x, Cones c, int inverse)
         const int mk = c.q[k];
         double n2 = 0, dot = 0;
         for (int i = 1 + tid; i < mk; i += nt) { n2 += lm[m + i] * lm[m + i]; dot += lm[m + i] * x[m + i]; }
-        n2 = blk_sum(n2, sh); dot = blk_sum(dot, sh);
+        n2 = block_sum(n2, sh); dot = block_sum(dot, sh);
         const double nrm = sqrt(n2), l0 = lm[m], x0 = x[m];
         double a = sqrt(l0 + nrm) * sqrt(l0 - nrm);
         const double lx = inverse ? (l0 * x0 + dot) / a : (l0 * x0 - dot) / a;
@@ -79,7 +67,7 @@ __global__ void sprod_kernel(double *x, const double *y, Cones c, int diag_d) {
         const int mk = c.q[k];
         double d = 0;
         for (int i = tid; i < mk; i += nt) d += y[m + i] * x[m + i];
-        d = blk_sum(d, sh);
+        d = block_sum(d, sh);
         const double y0 = y[m], x0 = x[m];
         __syncthreads();
         for (int i = 1 + tid; i < mk; i += nt) x[m + i] = y0 * x[m + i] + x0 * y[m + i];
@@ -115,7 +103,7 @@ __global__ void sinv_kernel(double *x, const double *y, Cones c) {
         const int mk = c.q[k];
         double n2 = 0, d = 0;
         for (int i = 1 + tid; i < mk; i += nt) { n2 += y[m + i] * y[m + i]; d += x[m + i] * y[m + i]; }
-        n2 = blk_sum(n2, sh); d = blk_sum(d, sh);
+        n2 = block_sum(n2, sh); d = block_sum(d, sh);
         const double nrm = sqrt(n2), y0 = y[m], cx = x[m];
         const double a = (y0 + nrm) * (y0 - nrm);
         const double al1 = a / y0, al2 = d / y0 - cx, ia = 1.0 / a;
@@ -165,7 +153,7 @@ __global__ void sdot_kernel(const double *x, const double *y, Cones c, int nlq, 
         }
         m += mk * mk;
     }
-    a = blk_sum(a, sh);
+    a = block_sum(a, sh);
     if (tid == 0) *out = a;
 }
 
@@ -187,7 +175,7 @@ __global__ void max_step_kernel(const double *x, Cones c, double *out) {
         const int mk = c.q[k];
         double n2 = 0;
         for (int i = 1 + tid; i < mk; i += nt) n2 += x[m + i] * x[m + i];
-        n2 = blk_sum(n2, sh);
+        n2 = block_sum(n2, sh);
         t = fmax(t, sqrt(n2) - x[m]);
         m += mk;
         __syncthreads();
@@ -318,7 +306,7 @@ __global__ void jac_off_kernel(JacArgs a, int flip) {
         tot += v;
         if (e % mk != e / mk) off += v;
     }
-    off = blk_sum(off, sh); tot = blk_sum(tot, sh);
+    off = block_sum(off, sh); tot = block_sum(tot, sh);
     if (threadIdx.x == 0) { a.stats[2 * k] = off; a.stats[2 * k + 1] = tot; }
 }
 
@@ -381,7 +369,7 @@ __global__ void __launch_bounds__(1024) jac_small_kernel(JacArgs a, int max_swee
             tot += v;
             if (e % mk != e / mk) off += v;
         }
-        off = blk_sum(off, sh); tot = blk_sum(tot, sh);
+        off = block_sum(off, sh); tot = block_sum(tot, sh);
         if (jac_done(off, tot, prev, mk)) { ok = true; break; }
         if (sweep == max_sweeps) break;
         prev = off;

@@ -22,21 +22,6 @@ namespace cvxb {
 
 namespace {
 
-__device__ __forceinline__ double cta_sum256(double v, double *sh) {
-    v = warp_sum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.0;
-    if (warp == 0) t = warp_sum(t);
-    if (threadIdx.x == 0) sh[0] = t;
-    __syncthreads();
-    const double r = sh[0];
-    __syncthreads();
-    return r;
-}
-
 // Householder reflector k of the n x p matrix X (ld ldx): H = I - tau v v', v[k] = 1, v[k+1:] stored below the
 // diagonal, H X[k:, k] = [beta; 0]   (dlarfg's conventions)
 __global__ void __launch_bounds__(256) house_kernel(int n, int k, double *X, long long ldx, double *tau) {
@@ -44,7 +29,7 @@ __global__ void __launch_bounds__(256) house_kernel(int n, int k, double *X, lon
     double *x = X + (long long)k * ldx;
     double t = 0.0;
     for (int i = k + 1 + threadIdx.x; i < n; i += blockDim.x) t += x[i] * x[i];
-    const double xn2 = cta_sum256(t, sh);
+    const double xn2 = block_sum(t, sh);
     const double alpha = x[k];
     if (xn2 == 0.0) { if (threadIdx.x == 0) tau[k] = 0.0; return; }
     const double beta = -copysign(sqrt(alpha * alpha + xn2), alpha);
@@ -63,7 +48,7 @@ __global__ void __launch_bounds__(256) house_apply_kernel(int n, int k, const do
     double *t = T + (long long)(c0 + blockIdx.x) * ldt;
     double a = 0.0;
     for (int i = k + 1 + threadIdx.x; i < n; i += blockDim.x) a += v[i] * t[i];
-    const double wv = (cta_sum256(a, sh) + t[k]) * tk;
+    const double wv = (block_sum(a, sh) + t[k]) * tk;
     __syncthreads();
     for (int i = k + 1 + threadIdx.x; i < n; i += blockDim.x) t[i] -= wv * v[i];
     if (threadIdx.x == 0) t[k] -= wv;
@@ -106,7 +91,7 @@ __global__ void sumsq_kernel(long long rows, int cols, const double *X, long lon
     double t = 0.0;
     const double *x = X + (long long)blockIdx.x * ld;
     for (long long i = threadIdx.x; i < rows; i += blockDim.x) t += x[i] * x[i];
-    t = cta_sum256(t, sh);
+    t = block_sum(t, sh);
     if (threadIdx.x == 0) atomicAdd(out, t);
 }
 __global__ void add_diag_kernel(int n, double *C, long long ld, const double *norm2, double factor) {

@@ -44,25 +44,11 @@ __global__ void nt_l_update_kernel(int m, double *s, double *z, double *d, doubl
 }
 
 // ---------------------------------------------------------------- 'q' cones
-__device__ __forceinline__ double cta_sum(double v, double *sh) {
-    v = warp_sum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    __syncthreads();
-    if (lane == 0) sh[warp] = v;
-    __syncthreads();
-    double t = (threadIdx.x < (blockDim.x >> 5)) ? sh[threadIdx.x] : 0.0;
-    if (warp == 0) t = warp_sum(t);
-    if (threadIdx.x == 0) sh[0] = t;
-    __syncthreads();
-    const double r = sh[0];
-    __syncthreads();
-    return r;
-}
 // sqrt(x' J x) the way misc.jnrm2 evaluates it (misc.py:848-856): a = |x[1:]|, sqrt(x0 - a) * sqrt(x0 + a)
 __device__ __forceinline__ double jnrm2_dev(const double *x, int m, double *sh) {
     double t = 0.0;
     for (int i = 1 + threadIdx.x; i < m; i += blockDim.x) t += x[i] * x[i];
-    const double a = sqrt(cta_sum(t, sh));
+    const double a = sqrt(block_sum(t, sh));
     return sqrt(x[0] - a) * sqrt(x[0] + a);
 }
 
@@ -76,7 +62,7 @@ __global__ void nt_q_compute_kernel(const int *q, const int *qoff, const int *vo
     const double aa = jnrm2_dev(sk, m, sh), bb = jnrm2_dev(zk, m, sh);
     double t = 0.0;
     for (int i = threadIdx.x; i < m; i += blockDim.x) t += sk[i] * zk[i];
-    const double dot = cta_sum(t, sh);
+    const double dot = block_sum(t, sh);
     const double cc = sqrt((dot / aa / bb + 1.0) / 2.0);
     // vk = 1/(2c) ( sk/a + J zk/b ),  then  v = (vk + e) / sqrt(2 (vk0 + 1))
     const double v0 = ((sk[0] / aa) + (zk[0] / bb)) / 2.0 / cc + 1.0;
@@ -114,7 +100,7 @@ __global__ void nt_q_update_kernel(const int *q, const int *qoff, const int *vof
         t2 += v[i] * sk[i];
         t3 += (i == 0 ? v[i] * zk[i] : -v[i] * zk[i]);     // jdot: v' J z
     }
-    const double dot = cta_sum(t1, sh), vs = cta_sum(t2, sh), vz = cta_sum(t3, sh);
+    const double dot = block_sum(t1, sh), vs = block_sum(t2, sh), vz = block_sum(t3, sh);
     const double cc = sqrt((1.0 + dot) / 2.0);
     const double vq = (vs + vz) / 2.0 / cc, vu = vs - vz;
     const double s0 = sk[0], z0 = zk[0], vk0 = v[0];
@@ -172,7 +158,7 @@ __global__ void __launch_bounds__(128) jacobi_round_kernel(int m, int m2, int r,
         const double x = bp[i], y = bq[i];
         a += x * x; b += y * y; g += x * y;
     }
-    a = cta_sum(a, sh); b = cta_sum(b, sh); g = cta_sum(g, sh);
+    a = block_sum(a, sh); b = block_sum(b, sh); g = block_sum(g, sh);
     // orthogonal to working accuracy: the computed dot product carries ~sqrt(m) eps |p||q| of rounding noise
     if (!(fabs(g) > (2.0 * 2.220446049250313e-16 * sqrt((double)m)) * sqrt(a * b)) || g == 0.0) return;
     const double zeta = (b - a) / (2.0 * g);
@@ -285,7 +271,7 @@ __global__ void __launch_bounds__(256) svd_finish_kernel(int m, const double *B,
     for (int j = 0; j < m; ++j) {               // column norms (m <= a few hundred: a serial loop of CTA reductions)
         double t = 0.0;
         for (int i = threadIdx.x; i < m; i += blockDim.x) { const double x = B[(size_t)j * m + i]; t += x * x; }
-        t = cta_sum(t, sh);
+        t = block_sum(t, sh);
         if (threadIdx.x == 0) norms[j] = sqrt(t);
     }
     __syncthreads();

@@ -216,9 +216,9 @@ int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const d
  * over coneqp).  Problems are  min 1/2 x'P x + q'x  s.t.  G x + s = h, s in the
  * cone product  'l' x 'q'[0] x ... ; all problems share n and the dims.
  * cvxb_batch_create(.., m, ..) is dims = {'l': m}: G x <= h.
- * A batch with 'q' cones or refinement > 0 runs the cone path (Gs = W^{-T} G is
- * materialised per problem: nprob * cdim * n more doubles); an 'l'-only batch
- * without refinement runs the fused-scaling path.
+ * A batch with 'q' cones materialises Gs = W^{-T} G per problem (nprob * cdim * n
+ * more doubles); an 'l'-only batch, with or without refinement, folds the 'l'
+ * scaling into the SYRK and the GEMVs instead.
  * nprob is at most CVXB_BATCH_MAX: the batched kernels put the problem index in gridDim.y / gridDim.z, which
  * are limited to 65535.  A larger nprob is CVXB_E_ARG (checked before the device); split larger batches
  * (qp_batch's sub-batches do). */

@@ -1,4 +1,4 @@
-"""Batch solver with second-order cones (csrc/batch_ipm.cu, the cone path) vs the reference: a Python loop over
+"""Batch solver with second-order cones (csrc/batch_ipm.cu) vs the reference: a Python loop over
 solvers.coneqp(P, q, G, h, dims, kktsolver='chol') (oracle/_ref) on the same problems — same status and iteration
 count per problem, objectives to rtol 1e-8, x / s / z to the tolerances of test_batch_gpu.py."""
 import ctypes as C
@@ -81,8 +81,9 @@ def test_cone_batch_refinement_option(ref, refinement):
 
 
 @pytest.mark.gpu
-def test_l_only_batch_with_refinement_takes_the_cone_path(ref):
-    """refinement on an 'l'-only batch runs the cone path's 'l' rows; the reference is solvers.qp with the option"""
+def test_l_only_batch_with_refinement_stays_fused(ref):
+    """refinement on an 'l'-only batch keeps di² in the SYRK (Gs is not formed); the reference is solvers.qp with
+    the option"""
     import cvxopt_b200
     from cvxopt import matrix, solvers
     from problems import dense_qp

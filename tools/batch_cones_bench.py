@@ -1,9 +1,9 @@
-"""Throughput of the batch solver's cone path (dims with 'q' cones, csrc/batch_ipm.cu kc_* kernels).
+"""Throughput of the batch solver with 'q' cones (csrc/batch_ipm.cu; Gs = W^{-T} G is materialised only with them).
 
 Two workloads, each printed as one JSON line:
   cone4  512 problems, n = 512, {'l': 512, 'q': [16]*32} (cdim 1024, the m of BASELINE config 4), run alternately in
-         the same process with config 4 itself ({'l': 1024}, the fused-scaling 'l' path): the difference is the cost of
-         the cone path at an equal G size.
+         the same process with config 4 itself ({'l': 1024}, di² fused into the SYRK): the difference is the cost of
+         the cones at an equal G size.
   soc    256 problems, n = 256, {'l': 0, 'q': [8]*64}.
 Both use one sub-batch (nsub=1), so solve_ms / lockstep_iterations is the time of one lock-step iteration.  With
 oracle/_ref built, the reference loop over solvers.coneqp runs on the first 16 problems: its wall time and whether
