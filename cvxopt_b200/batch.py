@@ -1,12 +1,13 @@
 """Batch of independent dense QPs solved in lock-step on the device (BASELINE config 4).
 
-    minimize 1/2 x'P x + q'x   subject to   G x + s = h,  s in K      (no A)
+    minimize 1/2 x'P x + q'x   subject to   G x + s = h,  s in K,   A x = b
 
-K is one 'l' cone of m rows by default, or dims = {'l': ml, 'q': [...]} shared by every problem.
+K is one 'l' cone of m rows by default, or dims = {'l': ml, 'q': [...]} shared by every problem, and so is the
+number p of equality rows (none by default).
 The per-problem algorithm is coneprog.coneqp (reference src/python/coneprog.py:1998-2547) with
-kktsolver='chol' and default options — same start, stopping rule, Mehrotra steps and iterative
-refinement — so every problem converges in the same number of iterations as
-`solvers.coneqp(P, q, G, h, dims)` (for dims={'l': m}: `solvers.qp(P, q, G, h)`) does.
+default options — kktsolver='chol', or 'chol2' for 'l'-only problems with A; same start, stopping rule, Mehrotra
+steps and iterative refinement — so every problem converges in the same number of iterations as
+`solvers.coneqp(P, q, G, h, dims, A, b)` (for dims={'l': m}: `solvers.qp(P, q, G, h, A, b)`) does.
 The reference has no batch API; its counterpart is a Python loop over those calls.
 """
 import ctypes as C
@@ -56,15 +57,46 @@ def _stack(P, q, G, h):
     return Pcm, q, Gcm, h, B, n, m
 
 
-class QPBatch:
-    """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}."""
+def _eq_rows(A, b, B, n):
+    """p, the number of equality rows of A (B, p, n) and b (B, p); 0 when both are None.  The shape checks are
+    coneqp's TypeErrors (coneprog.py:1910-1925)."""
+    if A is None and b is None:
+        return 0
+    if A is None or b is None:
+        raise TypeError("'A' and 'b' must be given together")
+    A, b = np.asarray(A), np.asarray(b)
+    if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n:
+        raise TypeError("'A' must have shape (B, p, %d) with B = %d" % (n, B))
+    if b.shape != (B, A.shape[1]):
+        raise TypeError("'b' must have shape (B, %d)" % A.shape[1])
+    return A.shape[1]
 
-    def __init__(self, nprob, n, m, device=0, dims=None):
+
+def _stack_eq(A, b, B, n):
+    """-> contiguous (B,n,p) [= p x n column-major per problem], (B,p), p; (None, None, 0) without A"""
+    p = _eq_rows(A, b, B, n)
+    if A is None:
+        return None, None, 0
+    Acm = np.ascontiguousarray(np.transpose(np.asarray(A, dtype=np.float64), (0, 2, 1)))
+    return Acm, np.ascontiguousarray(np.asarray(b, dtype=np.float64)), p
+
+
+class QPBatch:
+    """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
+    p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
+
+    def __init__(self, nprob, n, m, device=0, dims=None, p=0):
+        if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
+            raise TypeError("p must be an integer")
         d, keep, cdim = _batch_dims(dims, m)
         self._lib = _lib.load()
         self._h = C.c_void_p()
-        self.B, self.n, self.m = int(nprob), int(n), int(cdim)
-        if d is None:
+        self.B, self.n, self.m, self.p = int(nprob), int(n), int(cdim), int(p)
+        if self.p != 0:
+            if d is None:
+                d, keep, _ = _batch_dims({"l": self.m})
+            rc = self._lib.cvxb_batch_create_eq(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
+        elif d is None:
             rc = self._lib.cvxb_batch_create(C.byref(self._h), self.B, self.n, self.m, device)
         else:
             rc = self._lib.cvxb_batch_create_cones(C.byref(self._h), self.B, self.n, C.byref(d), device)
@@ -72,17 +104,27 @@ class QPBatch:
         _lib.check(rc, "batch")
         self._refinement = None
 
-    def load(self, P, q, G, h):
+    def load(self, P, q, G, h, A=None, b=None):
         Pcm, q, Gcm, h, B, n, m = _stack(P, q, G, h)
         if (B, n, m) != (self.B, self.n, self.m):
             raise TypeError("problem shapes do not match the batch")
+        Acm, bv, p = _stack_eq(A, b, B, n)
+        if p != self.p:
+            raise TypeError("A has %d rows; the batch was created with p = %d" % (p, self.p))
         rc = self._lib.cvxb_batch_load(self._h, Pcm.ctypes.data, q.ctypes.data, Gcm.ctypes.data,
                                        h.ctypes.data, _lib.HOST)
         _lib.check(rc, "batch_load")
+        if p:
+            _lib.check(self._lib.cvxb_batch_load_eq(self._h, Acm.ctypes.data, bv.ctypes.data, _lib.HOST),
+                       "batch_load_eq")
 
-    def load_ptr(self, P, q, G, h, space=_lib.DEVICE):
-        """raw addresses of already laid-out buffers (device-resident callers)"""
+    def load_ptr(self, P, q, G, h, space=_lib.DEVICE, A=None, b=None):
+        """raw addresses of already laid-out buffers (device-resident callers); A: p x n column-major per problem"""
         _lib.check(self._lib.cvxb_batch_load(self._h, P, q, G, h, space), "batch_load")
+        if self.p:
+            if A is None or b is None:
+                raise TypeError("the batch has p = %d equality rows: give A and b" % self.p)
+            _lib.check(self._lib.cvxb_batch_load_eq(self._h, A, b, space), "batch_load_eq")
 
     def solve(self, refinement=None, **options):
         """refinement: steps of iterative refinement per Newton solve (coneqp's option); None keeps the default
@@ -110,7 +152,10 @@ class QPBatch:
                                           status.ctypes.data, iters.ctypes.data, pobj.ctypes.data,
                                           dobj.ctypes.data, _lib.HOST)
         _lib.check(rc, "batch_results")
-        return {"x": x, "s": s, "z": z, "status": [STATUS[int(k)] for k in status],
+        y = np.zeros((B, self.p))
+        if self.p:
+            _lib.check(self._lib.cvxb_batch_results_y(self._h, y.ctypes.data, _lib.HOST), "batch_results_y")
+        return {"x": x, "y": y, "s": s, "z": z, "status": [STATUS[int(k)] for k in status],
                 "status_code": status, "iterations": iters, "primal objective": pobj,
                 "dual objective": dobj}
 
@@ -151,7 +196,7 @@ class QPBatchGroup:
     as ITS slowest problem is done.  Interleaved slices (problem i -> sub-batch i mod nsub) spread hard and easy
     problems evenly."""
 
-    def __init__(self, nprob, n, m, device=0, nsub=None, dims=None):
+    def __init__(self, nprob, n, m, device=0, nsub=None, dims=None, p=0):
         if nsub is None:
             # a few sub-batches let the finished problems of one leave the lock-step loop early (counts chosen
             # when the kernels were tuned, not re-measured on H100; CVXB_BATCH_NSUB overrides)
@@ -159,12 +204,13 @@ class QPBatchGroup:
                 2 if nprob >= 256 else (max(1, min(8, nprob // 8)) if nprob >= 16 else 1))
         # one library batch holds at most BATCH_MAX problems (include/cvxopt_b200.h): larger batches take more parts
         self.nsub = max(1, min(int(nsub), nprob), -(-int(nprob) // BATCH_MAX))
-        self.B, self.n, self.m = int(nprob), int(n), int(m)
+        self.B, self.n, self.m, self.p = int(nprob), int(n), int(m), int(p)
         self.idx = [np.arange(r, self.B, self.nsub) for r in range(self.nsub)]
         self.parts = []
+        eq = {"p": self.p} if self.p else {}
         try:
             for ix in self.idx:
-                self.parts.append(QPBatch(len(ix), n, m, device, dims))
+                self.parts.append(QPBatch(len(ix), n, m, device, dims, **eq))
         except BaseException:
             self.close()
             raise
@@ -174,10 +220,14 @@ class QPBatchGroup:
         for r, (ix, b) in enumerate(zip(self.idx, self.parts)):
             loader(r, ix, b)
 
-    def load(self, P, q, G, h):
+    def load(self, P, q, G, h, A=None, b=None):
         P, q, G, h = (np.asarray(a) for a in (P, q, G, h))
-        for ix, b in zip(self.idx, self.parts):
-            b.load(P[ix], q[ix], G[ix], h[ix])
+        if A is not None:
+            A = np.asarray(A)
+        if b is not None:
+            b = np.asarray(b)
+        for ix, part in zip(self.idx, self.parts):
+            part.load(P[ix], q[ix], G[ix], h[ix], None if A is None else A[ix], None if b is None else b[ix])
 
     def solve(self, **options):
         if self.nsub == 1:
@@ -201,7 +251,7 @@ class QPBatchGroup:
 
     def results(self):
         B, n, m = self.B, self.n, self.m
-        out = {"x": np.zeros((B, n)), "s": np.zeros((B, m)), "z": np.zeros((B, m)),
+        out = {"x": np.zeros((B, n)), "y": np.zeros((B, self.p)), "s": np.zeros((B, m)), "z": np.zeros((B, m)),
                "status_code": np.zeros(B, dtype=np.int32), "iterations": np.zeros(B, dtype=np.int32),
                "primal objective": np.zeros(B), "dual objective": np.zeros(B)}
         for ix, b in zip(self.idx, self.parts):
@@ -223,8 +273,9 @@ class QPBatchGroup:
             b.close()
 
 
-def qp_batch(P, q, G, h, device=0, nsub=None, dims=None, **options):
-    """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,cdim,n), h (B,cdim).
+def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, **options):
+    """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,cdim,n), h (B,cdim); optional
+    equality constraints A (B,p,n) x = b (B,p), given together.
     nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches), and never fewer
     than ceil(B / 65535), the most problems one library batch holds.
     dims: cone dimensions shared by every problem ({'l': ml, 'q': [...]}); None is {'l': cdim}.
@@ -234,19 +285,20 @@ def qp_batch(P, q, G, h, device=0, nsub=None, dims=None, **options):
     if P.ndim != 3 or G.ndim != 3:
         raise TypeError("P must have shape (B, n, n) and G (B, cdim, n)")
     _, _, cdim = _batch_dims(dims, G.shape[1])
-    b = QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims)
+    p = _eq_rows(A, b, P.shape[0], P.shape[1])
+    grp = QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims, p)
     try:
-        b.load(P, q, G, h)
+        grp.load(P, q, G, h, A, b)
         import time
         t0 = time.perf_counter()
-        b.solve(**options)
+        grp.solve(**options)
         wall = (time.perf_counter() - t0) * 1e3
-        out = b.results()
-        out.update(b.stats())
+        out = grp.results()
+        out.update(grp.stats())
         out["solve_wall_ms"] = wall
         return out
     finally:
-        b.close()
+        grp.close()
 
 
 # ---------------------------------------------------------------------------------------
@@ -283,11 +335,12 @@ def _p2p(ops):
             w.wait()
 
 
-def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interleaved", timings=None,
+def qp_batch_distributed(P, q, G, h, A=None, b=None, solver=None, group=None, sharding="interleaved", timings=None,
                          nsub=None, dims=None, **options):
     """Rank 0 passes the full batch (other ranks pass None); every rank returns its shard's results and
     rank 0 additionally gets the gathered batch, in the original problem order, under key 'all'.
-    Every rank passes the same `dims` (and options); shards are (k, cdim, n).
+    Every rank passes the same `dims` (and options); shards are (k, cdim, n).  Equality constraints A (B,p,n),
+    b (B,p) travel with the other inputs and y comes back with x; a stand-in `solver` then receives A and b too.
 
     `timings` (dict, optional) receives scatter_ms / solve_ms / gather_ms of this rank, measured with
     device events on the current stream (wall clock on CPU)."""
@@ -323,26 +376,28 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
                 self.t[name] = (time.perf_counter() - e0) * 1e3
     clk = _Clock()
 
-    meta = torch.zeros(3, dtype=torch.int64, device=dev)
+    meta = torch.zeros(4, dtype=torch.int64, device=dev)
     full = None
     if rank == 0:
-        # the batch in the layout QPBatch loads: column-major n x n / m x n per problem
+        # the batch in the layout QPBatch loads: column-major n x n / m x n / p x n per problem
         Pcm, qh, Gcm, hh, Btot, n, m = _stack(P, q, G, h)
         _batch_dims(dims, m)
-        meta = torch.tensor([Btot, n, m], dtype=torch.int64, device=dev)
-        full = [torch.from_numpy(a).to(dev) for a in (Pcm, qh, Gcm, hh)]       # one H2D of the whole batch
+        Acm, bh, p = _stack_eq(A, b, Btot, n)
+        meta = torch.tensor([Btot, n, m, p], dtype=torch.int64, device=dev)
+        arrays = (Pcm, qh, Gcm, hh) + ((Acm, bh) if p else ())
+        full = [torch.from_numpy(a).to(dev) for a in arrays]                     # one H2D of the whole batch
     if world > 1:
         dist.broadcast(meta, 0, group=group)
-    Btot, n, m = (int(v) for v in meta.tolist())
+    Btot, n, m, p = (int(v) for v in meta.tolist())
     owners = shard_indices(Btot, world, sharding)
     mine = owners[rank]
     k = len(mine)
-    tails = [(n, n), (n,), (n, m), (m,)]
+    tails = [(n, n), (n,), (n, m), (m,)] + ([(n, p), (p,)] if p else [])
 
     # ---- setup (not data path): this rank's batch object = its device allocations ----
     local_dev = torch.cuda.current_device() if on_gpu else 0
     clk.start("setup_ms")
-    bobj = QPBatchGroup(k, n, m, local_dev, nsub, dims) if (solver is None and k) else None
+    bobj = QPBatchGroup(k, n, m, local_dev, nsub, dims, p) if (solver is None and k) else None
     clk.stop()
 
     # ---- scatter ----
@@ -372,10 +427,12 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
     clk.start("solve_ms")
     if solver is not None:
         # stand-in (CPU tests): numpy in the public (B, m, n) layout
-        Pn, qn, Gn, hn = (t.cpu().numpy() for t in shard)
-        res = solver(np.transpose(Pn, (0, 2, 1)), qn, np.transpose(Gn, (0, 2, 1)), hn) if k else None
-        xs, ss, zs = ((torch.from_numpy(np.ascontiguousarray(res[key])).to(dev) if k
-                       else torch.empty((0, d), dtype=f64, device=dev)) for key, d in (("x", n), ("s", m), ("z", m)))
+        Pn, qn, Gn, hn = (t.cpu().numpy() for t in shard[:4])
+        eq = [np.transpose(shard[4].cpu().numpy(), (0, 2, 1)), shard[5].cpu().numpy()] if p else []
+        res = solver(np.transpose(Pn, (0, 2, 1)), qn, np.transpose(Gn, (0, 2, 1)), hn, *eq) if k else None
+        xs, ss, zs, ys = ((torch.from_numpy(np.ascontiguousarray(res[key])).to(dev) if k and d
+                           else torch.zeros((k, d), dtype=f64, device=dev))
+                          for key, d in (("x", n), ("s", m), ("z", m), ("y", p)))
         sc = torch.zeros((k, 4), dtype=f64, device=dev)
         if k:
             for j, key in enumerate(("status_code", "iterations", "primal objective", "dual objective")):
@@ -385,6 +442,7 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
         xs = torch.empty((k, n), dtype=f64, device=dev)
         ss = torch.empty((k, m), dtype=f64, device=dev)
         zs = torch.empty((k, m), dtype=f64, device=dev)
+        ys = torch.empty((k, p), dtype=f64, device=dev)
         sc = torch.zeros((k, 4), dtype=f64, device=dev)
         stats = {}
         if k:
@@ -400,7 +458,9 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
                     # the library copies on the sub-batch's own stream: the slices (written on torch's current
                     # stream) must be complete before it reads them
                     torch.cuda.current_stream().synchronize()
-                    part.load_ptr(sl[0].data_ptr(), sl[1].data_ptr(), sl[2].data_ptr(), sl[3].data_ptr(), _lib.DEVICE)
+                    eq = (sl[4].data_ptr(), sl[5].data_ptr()) if p else ()
+                    part.load_ptr(sl[0].data_ptr(), sl[1].data_ptr(), sl[2].data_ptr(), sl[3].data_ptr(), _lib.DEVICE,
+                                  *eq)
                 tw = time.perf_counter()
                 b.load_ptr_sliced(loader)
                 del keepalive
@@ -423,6 +483,10 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
                                                       None, None, _lib.DEVICE), "batch_results")
                     _lib.check(lib.cvxb_batch_results(part._h, None, None, None, status.ctypes.data, iters.ctypes.data,
                                                       pobj.ctypes.data, dobj.ctypes.data, _lib.HOST), "batch_results")
+                    if p:
+                        py = torch.empty((kk, p), dtype=f64, device=dev)
+                        _lib.check(lib.cvxb_batch_results_y(part._h, py.data_ptr(), _lib.DEVICE), "batch_results_y")
+                        ys.index_copy_(0, it, py)
                     xs.index_copy_(0, it, px); ss.index_copy_(0, it, ps); zs.index_copy_(0, it, pz)
                     sc.index_copy_(0, it, torch.from_numpy(np.stack(
                         [status.astype(np.float64), iters.astype(np.float64), pobj, dobj], axis=1)).to(dev))
@@ -437,15 +501,16 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
 
     # ---- gather ----
     clk.start("gather_ms")
-    local = [xs, ss, zs, sc]
+    local = [xs, ss, zs, sc] + ([ys] if p else [])
+    widths = (n, m, m, 4) + ((p,) if p else ())
     gathered = None
     if rank == 0:
-        outs = [torch.empty((Btot, d), dtype=f64, device=dev) for d in (n, m, m, 4)]
+        outs = [torch.empty((Btot, d), dtype=f64, device=dev) for d in widths]
         ops, bufs = [], {}
         for r in range(1, world):
             kr = len(owners[r])
             if kr:
-                bufs[r] = [torch.empty((kr, d), dtype=f64, device=dev) for d in (n, m, m, 4)]
+                bufs[r] = [torch.empty((kr, d), dtype=f64, device=dev) for d in widths]
                 ops += [dist.P2POp(dist.irecv, t, r, group) for t in bufs[r]]
         _p2p(ops)
         bufs[0] = local
@@ -463,14 +528,15 @@ def qp_batch_distributed(P, q, G, h, solver=None, group=None, sharding="interlea
         timings.update(clk.t)
 
     scn = sc.cpu().numpy()
-    res = {"x": xs.cpu().numpy(), "s": ss.cpu().numpy(), "z": zs.cpu().numpy(),
+    res = {"x": xs.cpu().numpy(), "y": ys.cpu().numpy(), "s": ss.cpu().numpy(), "z": zs.cpu().numpy(),
            "status_code": scn[:, 0].astype(np.int32), "iterations": scn[:, 1].astype(np.int32),
            "primal objective": scn[:, 2].copy(), "dual objective": scn[:, 3].copy(), "indices": mine}
     res.update(stats)
     res["status"] = [STATUS[int(c)] for c in res["status_code"]]
     if rank == 0:
         g = gathered
-        res["all"] = {"x": g[0], "s": g[1], "z": g[2], "status_code": g[3][:, 0].astype(np.int64),
+        res["all"] = {"x": g[0], "y": g[4] if p else np.zeros((Btot, 0)), "s": g[1], "z": g[2],
+                      "status_code": g[3][:, 0].astype(np.int64),
                       "iterations": g[3][:, 1].astype(np.int64), "primal objective": g[3][:, 2].copy(),
                       "dual objective": g[3][:, 3].copy(),
                       "status": [STATUS[int(c)] for c in g[3][:, 0]]}

@@ -1,6 +1,6 @@
 // Device-resident primal-dual interior-point method for a BATCH of independent dense QPs
 //
-//      minimize  1/2 x'P x + q'x    subject to  G x + s = h,  s in 'l' x 'q'[0] x ...          (no A)
+//      minimize  1/2 x'P x + q'x    subject to  G x + s = h,  s in 'l' x 'q'[0] x ...,  A x = b
 //
 // run in lock-step, one problem per CTA-group, with per-problem convergence masks
 // (BASELINE config 4; the reference has no batch API — its counterpart is a Python loop over
@@ -10,8 +10,11 @@
 // Newton solve (:2330-2347) and scaling update (misc.py:439-573).  Every KKT solve is the same path as cvxb_kkt_*:
 // SYRK, Cholesky, GEMV/TRSV — here batched over the problems through blockIdx.z / blockIdx.y.  Without 'q' cones
 // di² is fused into the SYRK operand and W^{-T} G is never formed; with them each factorisation writes Gs = W^{-T} G.
+// With p > 0 equality rows the reduced system is solved by kkt_chol2's elimination (misc.py:1352-1560): S = P + Gs'Gs
+// (+ A'A for a problem whose S was singular at the start), S = L L', Asct = L^{-1} A', Kp = Asct'Asct = Lp Lp'.
 // Nothing leaves the device between iterations except one int ("how many are done").
 #include "cone.cuh"
+#include <algorithm>
 #include <cstdlib>
 #include <memory>
 
@@ -22,6 +25,7 @@ namespace {
 struct Scal {                       // per-problem scalars, device resident
     double resx0, resz0, gap, mu, sigma, eta, step, dsdz;
     double xPxq, xq, resx, resz, zrz, pcost, dcost, relgap, pres, dres;
+    double resy0, resy, yry;          // equality rows: max(1, ||b||), ||A x - b||, y'(A x - b)
     int relgap_valid, done, iters, status;   // status: 0 running, 1 optimal, 2 maxiters, 3 singular
 };
 
@@ -29,7 +33,8 @@ struct Scal {                       // per-problem scalars, device resident
 // scaling W_k = beta_k (2 v_k v_k' - J) lives in the per-slot state row (misc.py:290-352).  'l' rows are spread over
 // the threads of the CTA, 'q' cones over its warps: lane i of the warp owns entries i, i+32, ... of the cone in every
 // pass, and the entry-0 values every lane needs are formed from warp sums; a pass that reads an entry another lane
-// wrote follows a __syncwarp().  Kernels templated on CONES compile the cone loops out for batches without cones.
+// wrote follows a __syncwarp().  Kernels templated on CONES compile the cone loops out for batches without cones;
+// those templated on EQ compile the equality rows out for batches without them.
 struct Ptrs {
     int n, m, ml, nq, refinement;
     const double *q, *h;
@@ -40,14 +45,20 @@ struct Ptrs {
     // inside a slot's row: v (sum q, indexed by row - ml) and beta (nq) with cones, the refinement vectors with
     // refinement > 0
     double *v, *beta, *wx, *wx2, *wz, *ws, *wz2, *ws2, *wz3;
+    // equality rows (neq > 0): p-vectors of every slot, Kp's per-slot Cholesky info; wy, wy2 in the state row
+    int neq;
+    const double *beq;
+    double *y, *ry, *dy, *aw, *wy, *wy2;   // aw: the 0/1 weight of A'A in S (1: S was singular at the start)
+    const int *infop;
 };
 #define PB_SETUP                                                                                       \
     const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;                                      \
     const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;                                       \
     const long long on = (long long)b * p.n, om = (long long)b * p.m, oc = (long long)b * p.L;         \
+    const long long oq = (long long)b * p.neq;                                                         \
     __shared__ double sh[32];                                                                          \
     Scal &S = p.sc[b];                                                                                 \
-    (void)lane; (void)warp; (void)nwarp; (void)on; (void)om; (void)oc; (void)sh; (void)S;
+    (void)lane; (void)warp; (void)nwarp; (void)on; (void)om; (void)oc; (void)oq; (void)sh; (void)S;
 #define FOR_CONES(o, len)                                                  \
     for (int k_ = warp; k_ < p.nq; k_ += nwarp)                            \
         if (const int o = p.qoff[k_], len = p.qoff[k_ + 1] - p.qoff[k_]; true)
@@ -113,10 +124,15 @@ __device__ __forceinline__ double q_margin(const double *x, double x0, int len, 
 }
 
 // starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2055-2080): d = di = 1,
-// v = e1 and beta = 1 for each cone
-__global__ void k_init_rhs(Ptrs p) {
+// v = e1 and beta = 1 for each cone.  EQ: y = b (the solve overwrites it, :2078-2081), aw = 0 (no A'A in S yet)
+template <bool EQ> __global__ void k_init_rhs(Ptrs p) {
     PB_SETUP
-    double nq = 0, nh = 0;
+    double nq = 0, nh = 0, nb = 0;
+    if (EQ) for (int i = tid; i < p.neq; i += nt) {
+        const double v = p.beq[oq + i];
+        p.y[oq + i] = v; p.aw[oq + i] = 0.0;
+        nb += v * v;
+    }
     for (int i = tid; i < p.n; i += nt) { double v = p.q[on + i]; p.dx[on + i] = -v; nq += v * v; }
     for (int i = tid; i < p.m; i += nt) {
         double v = p.h[om + i];
@@ -131,9 +147,11 @@ __global__ void k_init_rhs(Ptrs p) {
     }
     nq = block_sum(nq, sh);
     nh = block_sum(nh, sh);
+    if (EQ) nb = block_sum(nb, sh);
     if (tid == 0) {
         S.resx0 = fmax(1.0, sqrt(nq));                  // :1998
         S.resz0 = fmax(1.0, sqrt(nh));                  // :2000 (snrm2 == 2-norm for 'l' and 'q')
+        if (EQ) S.resy0 = fmax(1.0, sqrt(nb));          // :1999
         S.done = 0; S.iters = 0; S.status = 0; S.sigma = 0; S.eta = 0; S.step = 0;
     }
 }
@@ -180,11 +198,12 @@ template <bool CONES> __global__ void k_init_point(Ptrs p) {
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
-// rx = q  (then rx += P x by GEMV)
-__global__ void k_res_begin(Ptrs p) {
+// rx = q  (then rx += P x by GEMV); EQ: ry = b (then ry := A x - ry)
+template <bool EQ> __global__ void k_res_begin(Ptrs p) {
     PB_SETUP
     for (int i = tid; i < p.n; i += nt) p.rx[on + i] = p.q[on + i];
     for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i] - p.h[om + i];      // :2183-2184
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = p.beq[oq + i];         // :2177-2178
 }
 // f0 pieces once rx = P x + q   (:2172)
 __global__ void k_res_dots(Ptrs p) {
@@ -194,27 +213,32 @@ __global__ void k_res_dots(Ptrs p) {
     a = block_sum(a, sh); c = block_sum(c, sh);
     if (tid == 0) { S.xPxq = a; S.xq = c; }
 }
-// statistics + stopping rule (:2175-2234); row-wise, so every cone row is treated alike
-__global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol, double feastol,
-                        int *ndone, int *doneflags) {
+// statistics + stopping rule (:2175-2234); row-wise, so every cone row is treated alike.  EQ with m = 0 is coneqp's
+// cdim == 0 branch (:2002-2040): the starting point is the solution, 'optimal' after 0 iterations, dcost = pcost.
+template <bool EQ> __global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol,
+                                           double feastol, int *ndone, int *doneflags) {
     PB_SETUP
-    double rx2 = 0, rz2 = 0, zrz = 0;
+    double rx2 = 0, rz2 = 0, zrz = 0, ry2 = 0, yry = 0;
     for (int i = tid; i < p.n; i += nt) { double v = p.rx[on + i]; rx2 += v * v; }
     for (int i = tid; i < p.m; i += nt) { double v = p.rz[om + i]; rz2 += v * v; zrz += p.z[om + i] * v; }
+    if (EQ) for (int i = tid; i < p.neq; i += nt) { double v = p.ry[oq + i]; ry2 += v * v; yry += p.y[oq + i] * v; }
     rx2 = block_sum(rx2, sh); rz2 = block_sum(rz2, sh); zrz = block_sum(zrz, sh);
+    if (EQ) { ry2 = block_sum(ry2, sh); yry = block_sum(yry, sh); }
     if (tid == 0) {
         if (!S.done) {
             const double f0 = 0.5 * (S.xPxq + S.xq);
             S.resx = sqrt(rx2); S.resz = sqrt(rz2); S.zrz = zrz;
             S.pcost = f0;
-            S.dcost = f0 + zrz - S.gap;
+            if (EQ) { S.resy = sqrt(ry2); S.yry = yry; }
+            S.dcost = EQ ? f0 + yry + zrz - S.gap : f0 + zrz - S.gap;
+            if (EQ && p.m == 0) S.dcost = f0;
             if (S.pcost < 0.0) { S.relgap = S.gap / -S.pcost; S.relgap_valid = 1; }
             else if (S.dcost > 0.0) { S.relgap = S.gap / S.dcost; S.relgap_valid = 1; }
             else { S.relgap = 0.0; S.relgap_valid = 0; }
-            S.pres = S.resz / S.resz0;
+            S.pres = EQ ? fmax(S.resy / S.resy0, S.resz / S.resz0) : S.resz / S.resz0;
             S.dres = S.resx / S.resx0;
-            const bool opt = S.pres <= feastol && S.dres <= feastol &&
-                             (S.gap <= abstol || (S.relgap_valid && S.relgap <= reltol));
+            const bool opt = (EQ && p.m == 0) || (S.pres <= feastol && S.dres <= feastol &&
+                             (S.gap <= abstol || (S.relgap_valid && S.relgap <= reltol)));
             if (opt || iter == maxiters) {
                 S.done = 1; S.iters = iter; S.status = opt ? 1 : 2;
             }
@@ -229,16 +253,22 @@ __global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double re
 // slot below the new active count trades places with an active slot from the tail: everything a problem owns between
 // iterations (P, G, its 17 vectors, its scalars, its state row; K / inv / info / Gs are rebuilt every iteration) is
 // swapped, so the active problems stay a contiguous prefix and finished ones keep their final iterates in the tail.
-// ~6.3 MB per swap at n=512, m=1024, at most one swap per problem per solve.
+// ~6.3 MB per swap at n=512, m=1024, at most one swap per problem per solve.  With equality rows A and the NPV
+// p-vectors (b y ry dy aw) move too; Asct / Kp / its inverses / infop are rebuilt every factorisation.
+constexpr int NPV = 5;
 struct SwapArgs {
     double *P, *G, *vecs; Scal *sc;
     long long sP, sG;
     int n, me, Btot;
+    double *A, *pvecs;               // neq > 0 only
+    long long sA;
+    int neq;
 };
 __global__ void k_swap_slots(SwapArgs a, const int *pairs) {
     const int i = pairs[2 * blockIdx.y], j = pairs[2 * blockIdx.y + 1];
     const long long eP = a.sP, eG = a.sG, eN = 4LL * a.n, eM = 13LL * a.me, eS = (long long)(sizeof(Scal) / sizeof(double));
-    const long long total = eP + eG + eN + eM + eS;
+    const long long eA = a.neq ? a.sA : 0, eQ = (long long)NPV * a.neq;
+    const long long total = eP + eG + eN + eM + eS + eA + eQ;
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
         double *x, *y;
         long long r = e;
@@ -252,8 +282,14 @@ __global__ void k_swap_slots(SwapArgs a, const int *pairs) {
             const long long arr = r / a.me, k = r % a.me;
             double *base = a.vecs + 4LL * a.Btot * a.n + arr * (long long)a.Btot * a.me;
             x = base + (long long)i * a.me + k; y = base + (long long)j * a.me + k;
+        } else if ((r -= eM) < eA) {
+            x = a.A + i * a.sA + r; y = a.A + j * a.sA + r;
+        } else if ((r -= eA) < eQ) {
+            const long long arr = r / a.neq, k = r % a.neq;
+            double *base = a.pvecs + arr * (long long)a.Btot * a.neq;
+            x = base + (long long)i * a.neq + k; y = base + (long long)j * a.neq + k;
         } else {
-            r -= eM;
+            r -= eQ;
             x = reinterpret_cast<double *>(a.sc + i) + r; y = reinterpret_cast<double *>(a.sc + j) + r;
         }
         const double t = *x; *x = *y; *y = t;
@@ -366,14 +402,19 @@ __device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double
 
 // right-hand side of the i-th Newton system (coneprog.py:2373-2399), a copy of it for the refinement (:2331-2335),
 // then f4_no_ir's steps before the solve.  Cone rows are formed row-wise over the CTA; after a barrier the warp that
-// owns a cone adds sigma mu to its entry 0 and runs the cone part.
-template <bool CONES> __global__ void k_dir_rhs(Ptrs p, int i) {
+// owns a cone adds sigma mu to its entry 0 and runs the cone part.  EQ: dy = c ry (:2395-2397)
+template <bool CONES, bool EQ> __global__ void k_dir_rhs(Ptrs p, int i) {
     PB_SETUP
     const double sm = S.sigma * S.mu, c = -1.0 + S.eta;
     for (int k = tid; k < p.n; k += nt) {
         const double dx = c * p.rx[on + k];
         p.dx[on + k] = dx;
         if (p.refinement) p.wx[oc + k] = dx;
+    }
+    if (EQ) for (int k = tid; k < p.neq; k += nt) {
+        const double dy = c * p.ry[oq + k];
+        p.dy[oq + k] = dy;
+        if (p.refinement) p.wy[oc + k] = dy;
     }
     // row r: z = c rz, s = -ws3 (the Mehrotra correction, i = 1) - lmbda o lmbda (+ sigma mu where e is 1)
     auto rhs = [&](int r, bool e, double &z, double &s) {
@@ -416,7 +457,8 @@ __global__ void k_f4_pre(Ptrs p, double *z, long long sz, double *s, long long s
     FOR_CONES(o, len) f4_pre_cone(p, om, oc, k_, o, len, lane, z, s);
 }
 // f4_no_ir after a solve that refinement follows or that is a refinement step.  acc: the refinement step,
-// (dx, dz, ds) += (x, z, s)
+// (dx, dz, ds) += (x, z, s), and with EQ dy += wy2 (a refinement step's y is always wy2)
+template <bool EQ>
 __global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long sz, double *s, long long ss, int acc) {
     PB_SETUP
     x += b * sx; z += b * sz; s += b * ss;
@@ -427,13 +469,16 @@ __global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long 
         if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
     }
     if (acc) for (int i = tid; i < p.n; i += nt) p.dx[on + i] += x[i];
+    if (EQ && acc) for (int i = tid; i < p.neq; i += nt) p.dy[oq + i] += p.wy2[oc + i];
 }
 // refinement residual, the elementwise part of res() (coneprog.py:1930-1960): wx2 = wx, wz3 = W^{-1} dz,
-// wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds).  The P, G and G' products follow as batched GEMVs.
-__global__ void k_res(Ptrs p) {
+// wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds); EQ: wy2 = wy.  The P, A, A', G and G' products follow as
+// batched GEMVs.
+template <bool EQ> __global__ void k_res(Ptrs p) {
     PB_SETUP
     const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om;
     for (int i = tid; i < p.n; i += nt) p.wx2[oc + i] = p.wx[oc + i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.wy2[oc + i] = p.wy[oc + i];
     double *wz3 = p.wz3 + oc, *wz2 = p.wz2 + oc, *ws2 = p.ws2 + oc;
     for (int i = tid; i < p.ml; i += nt) {
         wz3[i] = p.di[om + i] * dz[i];
@@ -507,16 +552,17 @@ template <bool CONES> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
     }
 }
 // x += step dx; ds, dz := e + step d; scale2 inverse; update_scaling (misc.py:439-573); s = W' lmbda,
-// z = W^{-1} lmbda; gap (coneprog.py:2459-2547)
-template <bool CONES> __global__ void k_update(Ptrs p, const int *info, int iter) {
+// z = W^{-1} lmbda; gap (coneprog.py:2459-2547).  EQ: y += step dy (:2460); a singular Kp stops the problem too
+template <bool CONES, bool EQ> __global__ void k_update(Ptrs p, const int *info, int iter) {
     PB_SETUP
     if (S.done) return;
-    if (info[b] > 0) {      // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
+    if (info[b] > 0 || (EQ && p.infop[b] > 0)) {   // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
         if (tid == 0) { S.done = 1; S.status = 3; S.iters = iter; }
         return;
     }
     const double step = S.step;
     for (int k = tid; k < p.n; k += nt) p.x[on + k] += step * p.dx[on + k];
+    if (EQ) for (int k = tid; k < p.neq; k += nt) p.y[oq + k] += step * p.dy[oq + k];
     double *ds = p.ds + om, *dz = p.dz + om, *l = p.lmbda + om, *s = p.s + om, *z = p.z + om;
     double gap = 0;
     for (int k = tid; k < p.ml; k += nt) {
@@ -582,6 +628,12 @@ template <bool CONES> __global__ void k_update(Ptrs p, const int *info, int iter
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
+// the S + A'A switch of kkt_chol2's first factorisation (misc.py:1421-1447), per problem: a slot whose S = P + Gs'Gs
+// was singular at the start (info > 0) weights A'A by 1 in every later S
+__global__ void k_switch(double *aw, const int *info, int neq) {
+    const double w = info[blockIdx.x] > 0 ? 1.0 : 0.0;
+    for (int k = threadIdx.x; k < neq; k += blockDim.x) aw[(long long)blockIdx.x * neq + k] = w;
+}
 
 }  // namespace
 
@@ -617,6 +669,14 @@ struct cvxb_batch {
     DevBuf<double> Gs;               // W^{-T} G per slot (ld ldg), rebuilt every factorisation; only with 'q' cones
     DevBuf<double> cst;              // per-slot state row (moves with its problem); empty without cones and refinement
     long long L = 0;
+    // equality rows (cvxb_batch_create_eq, neq = p > 0), per problem: A (p x n, ld lda), Asct = L^{-1} A' (n x p,
+    // ld ldas), Kp (p x p, ld ldkp) and its diagonal-block inverses, the NPV p-vectors b y ry dy aw, Kp's info
+    int neq = 0;
+    long long lda = 0, sA = 0, ldas = 0, sAs = 0, ldkp = 0, sKp = 0, sInvp = 0;
+    DevBuf<double> A, Asct, Kp, invp, pvecs;
+    DevBuf<int> d_infop;
+    bool eq_loaded = false;          // cvxb_batch_load_eq since the last cvxb_batch_load
+    bool switched = false;           // some problem of this solve factors S + A'A (its aw is 1)
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -626,17 +686,17 @@ struct cvxb_batch {
 
 namespace {
 
-// The per-slot state row: v (sum q) | beta (nq) with cones, wx wx2 (n) | wz ws wz2 ws2 wz3 (m) with refinement;
-// every piece starts 16-byte aligned.  Reallocated when the layout changes: nothing in it outlives a solve.
+// The per-slot state row: v (sum q) | beta (nq) with cones, wx wx2 (n) | wz ws wz2 ws2 wz3 (m) | wy wy2 (p) with
+// refinement; every piece starts 16-byte aligned.  Reallocated when the layout changes: nothing in it outlives a solve.
 int state_alloc(cvxb_batch *b) {
     Ptrs &p = b->p;
     auto ev = [](long long x) { return (x + 1) & ~1LL; };
-    const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m);
-    const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 : 0;
+    const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m), p2 = ev(b->neq);
+    const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
     if (b->L == cone + ref) return 0;
     b->L = p.L = 0;
     b->cst.reset();
-    p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = nullptr;
+    p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = p.wy = p.wy2 = nullptr;
     if (cone + ref == 0) return 0;
     CVXB_TRY(b->cst.alloc((size_t)b->B * (cone + ref)));
     CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * (cone + ref) * sizeof(double)));
@@ -645,14 +705,42 @@ int state_alloc(cvxb_batch *b) {
     if (cone) { p.v = r; r += ev(sumq); p.beta = r; r += ev(p.nq); }
     if (ref) {
         p.wx = r; r += n2; p.wx2 = r; r += n2;
-        p.wz = r; r += m2; p.ws = r; r += m2; p.wz2 = r; r += m2; p.ws2 = r; r += m2; p.wz3 = r;
+        p.wz = r; r += m2; p.ws = r; r += m2; p.wz2 = r; r += m2; p.ws2 = r; r += m2; p.wz3 = r; r += m2;
+        if (p2) { p.wy = r; r += p2; p.wy2 = r; }
     }
     return 0;
 }
 
-// K = P + Gs' Gs with Gs = W^{-T} G (misc.py:1267-1282), then its Cholesky factor.  With 'q' cones Gs is formed;
-// without, diag(di)² is applied inside the SYRK (w = di2), or by the int8 slicing for a single large problem.
-int batch_factor(cvxb_batch *b) {
+// Asct := L^{-1} A' (blocked forward substitution with S's diagonal-block inverses), Kp := Asct' Asct, Kp = Lp Lp'
+// (misc.py:1464-1472).  Kp's per-slot info goes to d_infop.
+int factor_kp(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int n = b->n, pq = b->neq, B = b->Bact;
+    CVXB_TRY(transpose_copy(b->A.p, b->lda, b->Asct.p, b->ldas, pq, n, st, B, b->sA, b->sAs));
+    CVXB_TRY(trsm_lower_left(n, b->K.p, b->ldk, b->inv.p, b->Asct.p, b->ldas, pq, st, B, b->sK, b->sInv, b->sAs));
+    GemmDesc g;
+    g.M = pq; g.N = pq; g.K = n;
+    g.X = b->Asct.p; g.ldx = (int)b->ldas; g.x_kmajor = true; g.sX = b->sAs;
+    g.Y = g.X; g.ldy = g.ldx; g.y_kmajor = true; g.sY = b->sAs;
+    g.C = b->Kp.p; g.ldc = (int)b->ldkp; g.sC = b->sKp;
+    g.lower_only = true; g.batch = B;
+    if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
+    CVXB_TRY(dmma_gemm(g, st));
+    if (b->B == 1) {
+        CVXB_TRY(potrf_lower(pq, b->Kp.p, (int)b->ldkp, b->invp.p, b->cw, st));
+        CVXB_CUDA(cudaMemcpyAsync(b->d_infop.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
+    } else {
+        CVXB_TRY(potrf_lower_batched(pq, b->Kp.p, (int)b->ldkp, b->sKp, b->invp.p, b->sInvp, B, b->d_infop.p,
+                                     b->panel.p, (pq + 1) & ~1, st));
+    }
+    return 0;
+}
+
+// K = P + Gs' Gs (+ A' diag(aw) A) with Gs = W^{-T} G (misc.py:1267-1282), then its Cholesky factor, then with
+// equality rows (kp) Kp.  With 'q' cones Gs is formed; without, diag(di)² is applied inside the SYRK (w = di2), or
+// by the int8 slicing for a single large problem.  A'A is added only while some problem is switched: aw = 0 adds
+// exact zeros to the others.
+int batch_factor(cvxb_batch *b, bool kp = true) {
     cudaStream_t st = b->st;
     const bool cones = b->p.nq > 0;
     if (cones) {
@@ -677,6 +765,18 @@ int batch_factor(cvxb_batch *b) {
         if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
         CVXB_TRY(dmma_gemm(g, st));
     }
+    if (b->switched) {
+        GemmDesc g;
+        g.M = b->n; g.N = b->n; g.K = b->neq;
+        g.X = b->A.p; g.ldx = (int)b->lda; g.x_kmajor = true; g.sX = b->sA;
+        g.Y = g.X; g.ldy = g.ldx; g.y_kmajor = true; g.sY = b->sA;
+        g.w = b->p.aw; g.sW = b->neq;
+        g.D = b->K.p; g.ldd = (int)b->ldk; g.sD = b->sK; g.beta = 1.0;
+        g.C = b->K.p; g.ldc = (int)b->ldk; g.sC = b->sK;
+        g.lower_only = true; g.batch = b->Bact;
+        if (b->B == 1) g.splitk_ws = b->cw.splitk_ws.p;
+        CVXB_TRY(dmma_gemm(g, st));
+    }
     if (b->B == 1) {
         CVXB_TRY(potrf_lower(b->n, b->K.p, (int)b->ldk, b->inv.p, b->cw, st));
         CVXB_CUDA(cudaMemcpyAsync(b->d_info.p, b->cw.d_info.p, sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -684,21 +784,36 @@ int batch_factor(cvxb_batch *b) {
         CVXB_TRY(potrf_lower_batched(b->n, b->K.p, (int)b->ldk, b->sK, b->inv.p, b->sInv, b->Bact, b->d_info.p,
                                      b->panel.p, (b->n + 1) & ~1, st));
     }
+    if (kp && b->neq > 0) CVXB_TRY(factor_kp(b));
     return 0;
 }
 
-// (x, bzp) := solution of the reduced KKT system; on entry x = bx (slot k at x + k*sx), bzp = W^{-T} bz.
-// Gs is G with the weights di when it is not formed.
-int batch_solve(cvxb_batch *b, double *x, long long sx) {
+// (x, y, bzp) := solution of the reduced KKT system; on entry x = bx (slot k at x + k*sx), y = by (slot k at
+// y + k*sy, equality rows only), bzp = W^{-T} bz.  Gs is G with the weights di when it is not formed.
+int batch_solve(cvxb_batch *b, double *x, long long sx, double *y = nullptr, long long sy = 0) {
     cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact;
+    const int n = b->n, m = b->m, B = b->Bact, pq = b->neq;
     const bool cones = b->p.nq > 0;
     const double *A = cones ? b->Gs.p : b->G.p, *w = cones ? nullptr : b->p.di;
     const long long sw = w ? m : 0;
     // x := x + Gs' bzp
     GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sw = sw; gt.sx = m; gt.sy = sx;
     CVXB_TRY(gemv_t(m, n, A, b->ldg, w, b->p.bzp, 1.0, 1.0, x, st, gt));
-    CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, b->cw, st, B, b->sK, b->sInv, sx));
+    if (pq == 0) {
+        CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, b->cw, st, B, b->sK, b->sInv, sx));
+    } else {
+        // kkt_chol2's elimination of the equality rows (misc.py:1526-1558)
+        GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sw = pq; ga.sx = sy; ga.sy = sx;
+        if (b->switched)     // x += A' by for a switched problem (aw = 1), + 0 for the others
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, b->p.aw, y, 1.0, 1.0, x, st, ga));
+        CVXB_TRY(trsv_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, false, b->cw, st, B, b->sK, b->sInv, sx));
+        GemvBatch gs; gs.batch = B; gs.sA = b->sAs; gs.sx = sx; gs.sy = sy;          // y := Asct' x - y
+        CVXB_TRY(gemv_t(n, pq, b->Asct.p, b->ldas, nullptr, x, 1.0, -1.0, y, st, gs));
+        CVXB_TRY(potrs_lower(pq, b->Kp.p, (int)b->ldkp, b->invp.p, y, b->cw, st, B, b->sKp, b->sInvp, sy));
+        GemvBatch gy; gy.batch = B; gy.sA = b->sAs; gy.sx = sy; gy.sy = sx;          // x -= Asct y
+        CVXB_TRY(gemv_n(n, pq, b->Asct.p, b->ldas, nullptr, y, -1.0, 1.0, x, b->gemv_ws.p, st, gy));
+        CVXB_TRY(trsv_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, true, b->cw, st, B, b->sK, b->sInv, sx));
+    }
     // bzp := Gs x - bzp
     GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sw = sw; gn.sx = sx; gn.sy = m;
     CVXB_TRY(gemv_n(m, n, A, b->ldg, w, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
@@ -707,25 +822,34 @@ int batch_solve(cvxb_batch *b, double *x, long long sx) {
 
 // the i-th Newton direction: f4 (coneprog.py:2288-2347) on the right-hand side, i.e. f4_no_ir and then `refinement`
 // correction steps from the residual, followed by the step length and sigma
-template <bool CONES> int direction(cvxb_batch *b, int i) {
+template <bool CONES, bool EQ> int direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact, T = 256;
+    const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
     const long long L = b->L;
-    k_dir_rhs<CONES><<<B, T, 0, st>>>(p, i); count_launch();
-    CVXB_TRY(batch_solve(b, p.dx, n));
-    if (p.refinement) { k_f4_post<<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
+    k_dir_rhs<CONES, EQ><<<B, T, 0, st>>>(p, i); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
+    if (p.refinement) { k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
     for (int r = 0; r < p.refinement; ++r) {
-        k_res<<<B, T, 0, st>>>(p); count_launch();
+        // res() (coneprog.py:1930-1952): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx, wz2 -= G dx + W' ds
+        k_res<EQ><<<B, T, 0, st>>>(p); count_launch();
         GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
         CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
+        }
         GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
         CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
+        }
         GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
         CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
         k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
-        CVXB_TRY(batch_solve(b, p.wx2, L));
-        k_f4_post<<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1); count_launch();
+        CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
+        k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1); count_launch();
     }
     k_dir_post<CONES><<<B, T, 0, st>>>(p, i, p.refinement == 0); count_launch();
     return 0;
@@ -739,6 +863,7 @@ int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     SwapArgs a;
     a.P = b->P.p; a.G = b->G.p; a.vecs = b->vecs.p; a.sc = b->sc.p; a.sP = b->sP; a.sG = b->sG;
     a.n = b->n; a.me = b->m > 0 ? b->m : 1; a.Btot = b->B;
+    a.A = b->A.p; a.pvecs = b->pvecs.p; a.sA = b->sA; a.neq = b->neq;
     k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs.p);
     count_launch();
     if (b->cst.p) {
@@ -766,33 +891,53 @@ int restore_order(cvxb_batch *b) {
     return 0;
 }
 
-// the lock-step IPM over the active slots; CONES: the batch has 'q' cones
-template <bool CONES> int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+// the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows
+template <bool CONES, bool EQ>
+int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, T = 256;
+    const int n = b->n, m = b->m, T = 256, pq = b->neq;
     int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
     b->Bact = B;
+    b->switched = false;
     const Ptrs &p = b->p;
     GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
     GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
     GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
+    GemvBatch gAt; gAt.batch = B; gAt.sA = b->sA; gAt.sx = pq; gAt.sy = n;
+    GemvBatch gAn; gAn.batch = B; gAn.sA = b->sA; gAn.sx = n; gAn.sy = pq;
     CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I ----
-    k_init_rhs<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_factor(b));
+    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
+    CVXB_TRY(batch_factor(b, false));
+    std::vector<int> info(B), infop(EQ ? B : 0);
+    if (EQ) {
+        // kkt_chol2's first factorisation (misc.py:1421-1447): a problem whose S is singular factors S + A'A from
+        // now on
+        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaStreamSynchronize(st));
+        for (int i = 0; i < B; ++i) b->switched |= info[i] > 0;
+        if (b->switched) {
+            k_switch<<<B, T, 0, st>>>(p.aw, b->d_info.p, pq); count_launch();
+            CVXB_TRY(batch_factor(b, false));
+        }
+        CVXB_TRY(factor_kp(b));
+    }
     k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_solve(b, p.dx, n));
+    CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
     k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
     CVXB_LAUNCH_CHECK();
     {
-        // a singular first factorisation is the reference's "Rank([P; G]) < n" ValueError
-        std::vector<int> info(B);
+        // a singular first factorisation is the reference's "Rank(A) < p or Rank([P; A; G]) < n" ValueError
+        // (coneprog.py:2065-2067); without A it can only be Rank([P; G]) < n
         CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        if (EQ) CVXB_CUDA(cudaMemcpyAsync(infop.data(), b->d_infop.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaStreamSynchronize(st));
         for (int i = 0; i < B; ++i)
-            if (info[i] > 0) {
-                set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
+            if (info[i] > 0 || (EQ && infop[i] > 0)) {
+                if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
+                                  "at the start)", i);
+                else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
                 return CVXB_E_ARG;
             }
     }
@@ -800,15 +945,20 @@ template <bool CONES> int solve_lockstep(cvxb_batch *b, int maxiters, double abs
     int it = 0;
     for (it = 0; it <= maxiters; ++it) {
         // residuals (:2169-2186)
-        k_res_begin<<<B, T, 0, st>>>(p); count_launch();
+        k_res_begin<EQ><<<B, T, 0, st>>>(p); count_launch();
         CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
         k_res_dots<<<B, T, 0, st>>>(p); count_launch();
+        if (EQ) {
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, 1.0, 1.0, p.rx, st, gAt));                  // rx += A'y
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, gAn));   // ry = Ax - b
+        }
         if (m > 0) {
             CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
             CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_stats<<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p); count_launch();
+        k_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        count_launch();
         int ndone = 0;
         CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -830,12 +980,12 @@ template <bool CONES> int solve_lockstep(cvxb_batch *b, int maxiters, double abs
             b->permuted = true;
             B = nb;
             b->Bact = B;
-            gP.batch = gGt.batch = gGn.batch = B;
+            gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
         }
         k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         CVXB_TRY(batch_factor(b));
-        for (int i = 0; i < 2; ++i) CVXB_TRY(direction<CONES>(b, i));
-        k_update<CONES><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
+        for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ>(b, i)));
+        k_update<CONES, EQ><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -845,6 +995,23 @@ template <bool CONES> int solve_lockstep(cvxb_batch *b, int maxiters, double abs
     float t = 0;
     cudaEventElapsedTime(&t, b->e0, b->e1);
     b->solve_ms = t;
+    return 0;
+}
+
+// dst[problem] = src[slot] for a [B x len] per-slot array, through the slot permutation (d_perm, uploaded by the
+// caller) when the last solve compacted
+int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space) {
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    const size_t B = b->B;
+    if (!b->permuted) { CVXB_CUDA(cudaMemcpy(dst, src, B * len * sizeof(double), kind)); return 0; }
+    double *tmp = (space == CVXB_DEVICE) ? dst : nullptr;
+    if (!tmp) CVXB_CUDA(tmp_malloc(&tmp, B * len * sizeof(double)));
+    k_unpermute_rows<<<(unsigned)B, 256, 0, b->st>>>(src, tmp, b->d_perm.p, len);
+    count_launch();
+    cudaError_t e = cudaStreamSynchronize(b->st);
+    if (e == cudaSuccess && tmp != dst) e = cudaMemcpy(dst, tmp, B * len * sizeof(double), kind);
+    if (tmp != dst) tmp_free(tmp);
+    CVXB_CUDA(e);
     return 0;
 }
 
@@ -944,6 +1111,47 @@ int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims 
     return 0;
 }
 
+int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+    if (out) *out = nullptr;
+    if (!out || p < 0) { set_error("batch_create_eq: bad sizes (p must be nonnegative)"); return CVXB_E_ARG; }
+    if (n > 0 && p > n) {                         // coneqp's check before the first factorisation (coneprog.py:1962)
+        set_error("batch_create_eq: Rank(A) < p or Rank([P; A; G]) < n (p = %d > n = %d)", p, n);
+        return CVXB_E_ARG;
+    }
+    cvxb_batch *b = nullptr;
+    CVXB_TRY(cvxb_batch_create_cones(&b, nprob, n, dims, device));    // sizes and dims are checked before the device
+    std::unique_ptr<cvxb_batch> own(b);
+    if (p > 0) {
+        const size_t B = b->B;
+        b->neq = p;
+        b->lda = b->ldkp = ((p + 1) & ~1) > 2 ? ((p + 1) & ~1) : 2;
+        b->ldas = b->ldk;
+        b->sA = b->lda * n; b->sAs = b->ldas * p; b->sKp = b->ldkp * p;
+        b->sInvp = (long long)2 * ((p + NB - 1) / NB) * NB * NB;
+        CVXB_TRY(b->A.alloc(B * b->sA));
+        CVXB_CUDA(cudaMemset(b->A.p, 0, B * b->sA * sizeof(double)));
+        CVXB_TRY(b->Asct.alloc(B * b->sAs));
+        CVXB_TRY(b->Kp.alloc(B * b->sKp));
+        CVXB_TRY(b->invp.alloc(B * b->sInvp));
+        CVXB_TRY(b->pvecs.alloc(B * NPV * p));
+        CVXB_CUDA(cudaMemset(b->pvecs.p, 0, B * NPV * p * sizeof(double)));
+        CVXB_TRY(b->d_infop.alloc(B));
+        CVXB_CUDA(cudaMemset(b->d_infop.p, 0, B * sizeof(int)));
+        // GEMV workspace: A x (p rows), Asct y (n rows) besides the G x of create
+        const size_t me = b->m > 0 ? b->m : 1;
+        const size_t ws = std::max({me * gemv_n_chunks(n), (size_t)p * gemv_n_chunks(n), (size_t)n * gemv_n_chunks(p)});
+        if (B * ws > b->gemv_ws.n) { b->gemv_ws.reset(); CVXB_TRY(b->gemv_ws.alloc(B * ws)); }
+        Ptrs &q = b->p;
+        double *v = b->pvecs.p;
+        q.neq = p;
+        q.beq = v; q.y = v + B * p; q.ry = v + 2 * B * p; q.dy = v + 3 * B * p; q.aw = v + 4 * B * p;
+        q.infop = b->d_infop.p;
+        CVXB_TRY(state_alloc(b));
+    }
+    *out = own.release();
+    return 0;
+}
+
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
@@ -978,42 +1186,64 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->loaded = true;
+    b->eq_loaded = false;
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     b->permuted = false;
     return 0;
 }
 
+int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space) {
+    if (!b) { set_error("batch_load_eq: batch is NULL"); return CVXB_E_ARG; }
+    if (b->neq == 0) return 0;
+    if (!A || !bvec) { set_error("batch_load_eq: NULL argument"); return CVXB_E_ARG; }
+    if (!b->loaded) { set_error("batch_load_eq: call cvxb_batch_load first"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    CVXB_TRY(restore_order(b));                  // A and b are written to the problems' own slots
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const size_t B = b->B, n = b->n, pq = b->neq;
+    CVXB_CUDA(cudaMemcpy2DAsync(b->A.p, b->lda * sizeof(double), A, pq * sizeof(double), pq * sizeof(double),
+                                n * B, kind, b->st));
+    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->p.beq), bvec, B * pq * sizeof(double), kind, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->eq_loaded = true;
+    return 0;
+}
+
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     if (!b || !b->loaded) { set_error("batch_solve: load the problems first"); return CVXB_E_ARG; }
+    if (b->neq > 0 && !b->eq_loaded) {
+        set_error("batch_solve: the batch has p = %d equality rows: load A and b (cvxb_batch_load_eq) after "
+                  "cvxb_batch_load", b->neq);
+        return CVXB_E_ARG;
+    }
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
-    return b->p.nq > 0 ? solve_lockstep<true>(b, maxiters, abstol, reltol, feastol)
-                       : solve_lockstep<false>(b, maxiters, abstol, reltol, feastol);
+    const bool cones = b->p.nq > 0;
+    if (b->neq > 0) return cones ? solve_lockstep<true, true>(b, maxiters, abstol, reltol, feastol)
+                                 : solve_lockstep<false, true>(b, maxiters, abstol, reltol, feastol);
+    return cones ? solve_lockstep<true, false>(b, maxiters, abstol, reltol, feastol)
+                 : solve_lockstep<false, false>(b, maxiters, abstol, reltol, feastol);
+}
+
+int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {
+    if (!b || !y) { set_error("batch_results_y: NULL argument"); return CVXB_E_ARG; }
+    if (b->neq == 0) return 0;
+    CVXB_CUDA(cudaSetDevice(b->device));
+    if (b->permuted)
+        CVXB_CUDA(cudaMemcpy(b->d_perm.p, b->perm.data(), (size_t)b->B * sizeof(int), cudaMemcpyHostToDevice));
+    return give_rows(b, y, b->p.y, b->neq, space);
 }
 
 int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *status, int *iters,
                        double *pobj, double *dobj, int space) {
     if (!b) { set_error("batch is NULL"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
-    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     const size_t B = b->B;
     // slot -> problem (identity unless the solve compacted finished problems away)
     if (b->permuted) CVXB_CUDA(cudaMemcpy(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice));
-    auto give = [&](double *dst, const double *src, int len) -> int {
-        if (!b->permuted) { CVXB_CUDA(cudaMemcpy(dst, src, B * len * sizeof(double), kind)); return 0; }
-        double *tmp = (space == CVXB_DEVICE) ? dst : nullptr;
-        if (!tmp) CVXB_CUDA(tmp_malloc(&tmp, B * len * sizeof(double)));
-        k_unpermute_rows<<<(unsigned)B, 256, 0, b->st>>>(src, tmp, b->d_perm.p, len);
-        count_launch();
-        cudaError_t e = cudaStreamSynchronize(b->st);
-        if (e == cudaSuccess && tmp != dst) e = cudaMemcpy(dst, tmp, B * len * sizeof(double), kind);
-        if (tmp != dst) tmp_free(tmp);
-        CVXB_CUDA(e);
-        return 0;
-    };
-    if (x) CVXB_TRY(give(x, b->p.x, b->n));
-    if (s && b->m) CVXB_TRY(give(s, b->p.s, b->m));
-    if (z && b->m) CVXB_TRY(give(z, b->p.z, b->m));
+    if (x) CVXB_TRY(give_rows(b, x, b->p.x, b->n, space));
+    if (s && b->m) CVXB_TRY(give_rows(b, s, b->p.s, b->m, space));
+    if (z && b->m) CVXB_TRY(give_rows(b, z, b->p.z, b->m, space));
     if (status || iters || pobj || dobj) {
         if (space == CVXB_DEVICE) { set_error("batch_results: scalars are returned to host memory only"); return CVXB_E_ARG; }
         std::vector<Scal> sc(B);

@@ -369,6 +369,11 @@ int trsv_lower(int n, const double *L, int ldl, const double *inv, double *b, bo
                long long sb = 0);
 int potrf_lower_batched(int n, double *A, int lda, long long sA, double *inv, long long sInv,
                         int batch, int *d_info, double *panel, int ldw, cudaStream_t st);
+// B := L^{-1} B for the n x n Cholesky factor L (lower, ld ldl) with its diagonal-block inverses `inv`
+// (potrf_lower's output); B is n x ncols (ld ldb), updated in place by blocked forward substitution (DMMA GEMMs).
+// Batched: problem p uses L + p*sL, inv + p*sInv, B + p*sB.  Defined in kkt_api.cu.
+int trsm_lower_left(int n, const double *L, long long ldl, const double *inv, double *B, long long ldb, int ncols,
+                    cudaStream_t st, int batch = 1, long long sL = 0, long long sInv = 0, long long sB = 0);
 
 // ---- device selection ----------------------------------------------------------
 // CVXB_E_NOGPU unless `device` exists and is sm_90; selects it.

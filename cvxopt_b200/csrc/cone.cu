@@ -315,8 +315,9 @@ __global__ void gemv_n_reduce_kernel(int nrows, int nchunks, const double *ws, c
 
 // dst (cols x rows, ld ldd) = src' where src is rows x cols (ld lds); 32x32 tiles through smem
 __global__ void transpose_kernel(const double *src, long long lds, double *dst, long long ldd,
-                                 int rows, int cols) {
+                                 int rows, int cols, long long ssrc, long long sdst) {
     __shared__ double t[32][33];
+    src += blockIdx.z * ssrc; dst += blockIdx.z * sdst;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     for (int cc = ty; cc < 32; cc += 8) {
@@ -466,10 +467,10 @@ int gemv_n(int nrows, int ncols, const double *A, long long lda, const double *w
 }
 
 int transpose_copy(const double *src, long long lds, double *dst, long long ldd, int rows, int cols,
-                   cudaStream_t st) {
-    if (rows <= 0 || cols <= 0) return 0;
-    dim3 grid((rows + 31) / 32, (cols + 31) / 32);
-    transpose_kernel<<<grid, 256, 0, st>>>(src, lds, dst, ldd, rows, cols);
+                   cudaStream_t st, int batch, long long ssrc, long long sdst) {
+    if (rows <= 0 || cols <= 0 || batch <= 0) return 0;
+    dim3 grid((rows + 31) / 32, (cols + 31) / 32, batch);
+    transpose_kernel<<<grid, 256, 0, st>>>(src, lds, dst, ldd, rows, cols, ssrc, sdst);
     count_launch();
     CVXB_LAUNCH_CHECK();
     return 0;

@@ -84,8 +84,8 @@ int gemv_n(int nrows, int ncols, const double *A, long long lda, const double *w
 int vec_mul(int n, const double *a, const double *b, double *out, cudaStream_t st);  // out = a.*b
 int vec_axpby(int n, double alpha, const double *x, double beta, double *y, cudaStream_t st);
 int symmetrize_lower(int n, double *A, long long lda, int batch, long long stride, cudaStream_t st);
-// dst (cols x rows) = src' for src rows x cols
+// dst (cols x rows) = src' for src rows x cols; batched: problem p uses src + p*ssrc, dst + p*sdst
 int transpose_copy(const double *src, long long lds, double *dst, long long ldd, int rows, int cols,
-                   cudaStream_t st);
+                   cudaStream_t st, int batch = 1, long long ssrc = 0, long long sdst = 0);
 
 }  // namespace cvxb

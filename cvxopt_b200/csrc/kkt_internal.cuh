@@ -98,10 +98,6 @@ int upload_matrix(double *dst, long long ldd, const double *src, long long lds, 
                   cudaStream_t st);
 int xfer_vec(double *dst, const double *src, size_t n, int space, bool to_device, cudaStream_t st);
 inline long long kkt_ldk(const cvxb_kkt *k) { long long l = (k->n + 1) & ~1; return l > 2 ? l : 2; }
-// B := L^{-1} B for the n x n Cholesky factor L (lower, ld ldl) with its diagonal-block inverses `inv`
-// (potrf_lower's output); B is n x ncols (ld ldb), updated in place by blocked forward substitution (DMMA GEMMs).
-int trsm_lower_left(int n, const double *L, long long ldl, const double *inv, double *B, long long ldb, int ncols,
-                    cudaStream_t st);
 int kkt_pack_bz(cvxb_kkt *k, const double *zd);      // k->bzp := pack(W^{-T} bz)
 int kkt_unpack_z(cvxb_kkt *k, double *zd);           // z := unpack(k->bzp)
 // the 'q' and 's' rows of pack(W^{-T} G): dst is where the first 'q' row goes (ld ldd), the packed 's' rows follow

@@ -227,17 +227,34 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device);
 /* batch of  min 1/2 x'Px + q'x  s.t.  G x + s = h,  s in 'l' x 'q' cones  (B x coneqp, coneprog.py:1440).
  * dims->mnl != 0, a cone order q[k] < 1, nprob > CVXB_BATCH_MAX: CVXB_E_ARG; dims->ns > 0: CVXB_E_UNSUP. */
 int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device);
+/* batch of  min 1/2 x'Px + q'x  s.t.  G x + s = h,  s in 'l' x 'q' cones,  A x = b  with p equality rows per
+ * problem (B x coneqp(P, q, G, h, dims, A, b); kktsolver 'chol2' without 'q' cones, 'chol' with them: both
+ * eliminate A through S = P + Gs'Gs, Asct = L^{-1} A', Kp = Asct'Asct, misc.py:1352-1560).  p = 0 is
+ * cvxb_batch_create_cones.  p < 0 and the dims / nprob violations of cvxb_batch_create_cones are CVXB_E_ARG, and so
+ * is p > n ("Rank(A) < p or Rank([P; A; G]) < n"), all checked before the device.  A problem whose S is singular at
+ * the start factors S + A'A for the rest of the solve (misc.py:1421-1447); if that, or Kp, is singular at the start,
+ * cvxb_batch_solve returns CVXB_E_ARG naming the problem.  Device memory per problem on top of the p = 0 batch, in
+ * doubles: lda*n (A, lda = p rounded up to even, at least 2) + ldk*p (Asct, ldk = n rounded up to even) + lda*p (Kp)
+ * + 2*ceil(p/128)*128^2 (Kp's diagonal-block inverses, even for small p) + 5p (b, y, ry, dy, A'A weight) + 2p
+ * rounded up to even with refinement (wy, wy2), plus one int (Kp's info); all of it is counted by cvxb_device_bytes
+ * and freed by cvxb_batch_destroy. */
+int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);
 /* P: nprob x (n x n, ld n); q: nprob x n; G: nprob x (m x n column-major, ld m); h: nprob x m; m = cdim */
 int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
                     const double *h, int space);
+/* A: nprob x (p x n column-major, ld p); bvec: nprob x p.  Call it after every cvxb_batch_load of a batch with
+ * p > 0 equality rows (cvxb_batch_solve refuses such a batch with CVXB_E_ARG until it is); a no-op when p = 0. */
+int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space);
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol);
 /* status: 1 optimal, 2 maximum iterations reached, 3 singular KKT matrix ('unknown' in the
  * reference for 2 and 3).  x/s/z may be device pointers (space), scalars go to host memory. */
 int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *status,
                        int *iters, double *pobj, double *dobj, int space);
+/* y: nprob x p, the multipliers of A x = b in the caller's problem order (as x, s, z); nothing when p = 0 */
+int cvxb_batch_results_y(cvxb_batch *b, double *y, int space);
 /* CUDA-event time of the last cvxb_batch_solve and the number of lock-step iterations run */
 int cvxb_batch_stats(cvxb_batch *b, double *solve_ms, int *iterations);
 /* kernel of the factorisations' SYRK in the last solve: 1 fp64 DMMA, 2 int8 slices (as cvxb_kkt_syrk_path) */
