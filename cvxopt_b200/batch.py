@@ -9,6 +9,10 @@ default options — kktsolver='chol', or 'chol2' for 'l'-only problems with A; s
 steps and iterative refinement — so every problem converges in the same number of iterations as
 `solvers.coneqp(P, q, G, h, dims, A, b)` (for dims={'l': m}: `solvers.qp(P, q, G, h, A, b)`) does.
 The reference has no batch API; its counterpart is a Python loop over those calls.
+
+Cone LPs  minimize c'x  subject to  G x + s = h,  s in K,  A x = b  run coneprog.conelp (coneprog.py:31-1436) in the
+same lock-step machinery (ConeLPBatch, conelp_batch): a Python loop over `solvers.conelp(c, G, h, dims, A, b)`
+(`solvers.lp` for dims={'l': m}), with its infeasibility certificates.
 """
 import ctypes as C
 
@@ -16,7 +20,7 @@ import numpy as np
 
 from . import _lib
 
-STATUS = {0: "running", 1: "optimal", 2: "unknown", 3: "unknown"}
+STATUS = {0: "running", 1: "optimal", 2: "unknown", 3: "unknown", 4: "primal infeasible", 5: "dual infeasible"}
 DEFAULTS = dict(maxiters=100, abstol=1e-7, reltol=1e-6, feastol=1e-7)   # coneprog.py:436-456
 BATCH_MAX = 65535        # CVXB_BATCH_MAX: problems per cvxb_batch handle
 
@@ -196,6 +200,11 @@ class QPBatchGroup:
     as ITS slowest problem is done.  Interleaved slices (problem i -> sub-batch i mod nsub) spread hard and easy
     problems evenly."""
 
+    @staticmethod
+    def _part():
+        """the kind of batch each slice is (ConeLPBatchGroup: ConeLPBatch)"""
+        return QPBatch
+
     def __init__(self, nprob, n, m, device=0, nsub=None, dims=None, p=0):
         if nsub is None:
             # a few sub-batches let the finished problems of one leave the lock-step loop early (counts chosen
@@ -210,7 +219,7 @@ class QPBatchGroup:
         eq = {"p": self.p} if self.p else {}
         try:
             for ix in self.idx:
-                self.parts.append(QPBatch(len(ix), n, m, device, dims, **eq))
+                self.parts.append(self._part()(len(ix), n, m, device, dims, **eq))
         except BaseException:
             self.close()
             raise
@@ -221,13 +230,17 @@ class QPBatchGroup:
             loader(r, ix, b)
 
     def load(self, P, q, G, h, A=None, b=None):
-        P, q, G, h = (np.asarray(a) for a in (P, q, G, h))
+        self._load_sliced((P, q, G, h), A, b)
+
+    def _load_sliced(self, data, A, b):
+        """each part loads its slice of the per-problem arrays `data`, then of A and b"""
+        data = [np.asarray(a) for a in data]
         if A is not None:
             A = np.asarray(A)
         if b is not None:
             b = np.asarray(b)
         for ix, part in zip(self.idx, self.parts):
-            part.load(P[ix], q[ix], G[ix], h[ix], None if A is None else A[ix], None if b is None else b[ix])
+            part.load(*(a[ix] for a in data), None if A is None else A[ix], None if b is None else b[ix])
 
     def solve(self, **options):
         if self.nsub == 1:
@@ -271,6 +284,114 @@ class QPBatchGroup:
     def close(self):
         for b in self.parts:
             b.close()
+
+
+class ConeLPBatch(QPBatch):
+    """B cone LPs  min c'x  s.t.  G x + s = h,  s in K,  A x = b  (B x coneprog.conelp with default options, kktsolver
+    'chol2' for 'l'-only problems, 'chol' with 'q' cones).  dims: 'l' and 'q' only, None is {'l': m}; m = cdim >= 1.
+    p: equality rows per problem.  solve / results / stats / close are QPBatch's; results()["status"] is one of
+    'optimal', 'primal infeasible', 'dual infeasible' or 'unknown', with NaN where conelp returns None."""
+
+    def __init__(self, nprob, n, m, device=0, dims=None, p=0):
+        if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
+            raise TypeError("p must be an integer")
+        d, keep, cdim = _batch_dims(dims, m)
+        if d is None:
+            d, keep, _ = _batch_dims({"l": int(cdim)})
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.B, self.n, self.m, self.p = int(nprob), int(n), int(cdim), int(p)
+        rc = self._lib.cvxb_batch_create_lp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
+        del keep
+        _lib.check(rc, "batch")
+        self._refinement = None
+
+    def load(self, c, G, h, A=None, b=None):
+        c = np.ascontiguousarray(np.asarray(c, dtype=np.float64))
+        h = np.ascontiguousarray(np.asarray(h, dtype=np.float64))
+        G = np.asarray(G, dtype=np.float64)
+        B, n, m = self.B, self.n, self.m
+        if c.shape != (B, n) or G.shape != (B, m, n) or h.shape != (B, m):
+            raise TypeError("problem shapes do not match the batch")
+        Acm, bv, p = _stack_eq(A, b, B, n)
+        if p != self.p:
+            raise TypeError("A has %d rows; the batch was created with p = %d" % (p, self.p))
+        Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
+        _lib.check(self._lib.cvxb_batch_load_lp(self._h, c.ctypes.data, Gcm.ctypes.data, h.ctypes.data, _lib.HOST),
+                   "batch_load_lp")
+        if p:
+            _lib.check(self._lib.cvxb_batch_load_eq(self._h, Acm.ctypes.data, bv.ctypes.data, _lib.HOST),
+                       "batch_load_eq")
+
+    def load_ptr(self, c, G, h, space=_lib.DEVICE, A=None, b=None):
+        """raw addresses of already laid-out buffers: c (B, n), G m x n column-major per problem, h (B, m), A p x n
+        column-major per problem, b (B, p)"""
+        _lib.check(self._lib.cvxb_batch_load_lp(self._h, c, G, h, space), "batch_load_lp")
+        if self.p:
+            if A is None or b is None:
+                raise TypeError("the batch has p = %d equality rows: give A and b" % self.p)
+            _lib.check(self._lib.cvxb_batch_load_eq(self._h, A, b, space), "batch_load_eq")
+
+
+class ConeLPBatchGroup(QPBatchGroup):
+    """QPBatchGroup's interleaved sub-batches, solved concurrently, for cone LPs"""
+
+    @staticmethod
+    def _part():
+        return ConeLPBatch
+
+    def load(self, c, G, h, A=None, b=None):
+        self._load_sliced((c, G, h), A, b)
+
+
+def _lp_shapes(c, G, h, dims, A, b):
+    """conelp's argument checks (coneprog.py:487-562) on the batch: -> B, n, cdim, p"""
+    c, G, h = np.asarray(c), np.asarray(G), np.asarray(h)
+    if c.ndim != 2:
+        raise TypeError("'c' must have shape (B, n): one column per problem")
+    B, n = c.shape
+    if h.ndim != 2 or h.shape[0] != B:
+        raise TypeError("'h' must have shape (B, cdim): one column per problem")
+    cdim = h.shape[1] if dims is None else _batch_dims(dims)[2]
+    if h.shape[1] != cdim:
+        raise TypeError("'h' must be a 'd' matrix of size (%d,1)" % cdim)
+    if G.ndim != 3 or G.shape != (B, cdim, n):
+        raise TypeError("'G' must be a 'd' matrix of size (%d, %d)" % (cdim, n))
+    if (A is None) != (b is None):
+        raise TypeError("'A' and 'b' must be given together")
+    p = 0
+    if A is not None:
+        A, b = np.asarray(A), np.asarray(b)
+        if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n:
+            raise TypeError("'A' must be a 'd' matrix with %d columns " % n)
+        p = A.shape[1]
+        if b.shape != (B, p):
+            raise TypeError("'b' must have length %d" % p)
+    if p > n or p + cdim < n:
+        raise ValueError("Rank(A) < p or Rank([G; A]) < n")          # coneprog.py:572-573
+    return B, n, cdim, p
+
+
+def conelp_batch(c, G, h, dims=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent cone LPs on one GPU, each as solvers.conelp(c, G, h, dims, A, b) does.  c (B,n),
+    G (B,cdim,n), h (B,cdim); optional A (B,p,n), b (B,p), given together.  dims: shared by every problem ('l' and
+    'q' only); None is {'l': cdim}, i.e. solvers.lp.  nsub and the returned dict are qp_batch's; status is 'optimal',
+    'primal infeasible', 'dual infeasible' or 'unknown', and entries the reference returns as None are NaN.
+    options: maxiters, abstol, reltol, feastol, refinement (as conelp's)."""
+    B, n, cdim, p = _lp_shapes(c, G, h, dims, A, b)
+    grp = ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p)
+    try:
+        grp.load(c, G, h, A, b)
+        import time
+        t0 = time.perf_counter()
+        grp.solve(**options)
+        wall = (time.perf_counter() - t0) * 1e3
+        out = grp.results()
+        out.update(grp.stats())
+        out["solve_wall_ms"] = wall
+        return out
+    finally:
+        grp.close()
 
 
 def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, **options):

@@ -13,6 +13,8 @@
 // With p > 0 equality rows the reduced system is solved by kkt_chol2's elimination (misc.py:1352-1560): S = P + Gs'Gs
 // (+ A'A for a problem whose S was singular at the start), S = L L', Asct = L^{-1} A', Kp = Asct'Asct = Lp Lp'.
 // Nothing leaves the device between iterations except one int ("how many are done").
+// A cone LP batch (no P: minimize c'x over the same constraints) runs coneprog.conelp (coneprog.py:31-1436) instead, in
+// solve_conelp: the same factorisations and solves with the self-dual embedding's tau / kappa arithmetic around them.
 #include "cone.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -50,7 +52,20 @@ struct Ptrs {
     const double *beq;
     double *y, *ry, *dy, *aw, *wy, *wy2;   // aw: the 0/1 weight of A'A in S (1: S was singular at the start)
     const int *infop;
+    // cone LP batches (cvxb_batch_create_lp): q holds c; lps is the LPScal at the end of a slot's state row;
+    // x1 (n), y1 (p), z1 and th (m) are rebuilt every iteration
+    double *lps, *x1, *y1, *z1, *th;
 };
+// per-problem scalars of conelp's self-dual embedding (coneprog.py:847, :1031-1047), in the state row so that they
+// move with their slot
+struct LPScal {
+    double tau, kappa, dg, dgi, lg, lgsq;          // lg = lmbda[-1] = sqrt(tau kappa) in the scaled variables
+    double rt, dtau, dkappa, wkappa3, tt, tk, z1sq;
+    double wtau, wkappa, wtau2, wkappa2;           // refinement copies (coneprog.py:1201-1235)
+};
+__device__ __forceinline__ LPScal &lp_scal(const Ptrs &p, long long oc) {
+    return *reinterpret_cast<LPScal *>(p.lps + oc);
+}
 #define PB_SETUP                                                                                       \
     const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;                                      \
     const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;                                       \
@@ -327,12 +342,14 @@ __global__ void k_build_gs(Ptrs p, const double *G, double *Gs, long long ldg, l
     }
 }
 // NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357).
-// di2 = di² is the SYRK's weight when W^{-T} G is not formed
-template <bool CONES> __global__ void k_scaling(Ptrs p, int first) {
+// di2 = di² is the SYRK's weight when W^{-T} G is not formed.  LP: conelp's dg, dgi and lmbdag at iteration 0, its
+// lmbdasq[-1] and mu = ||lmbda||² / (1 + cdim) (coneprog.py:1031-1047, :1248)
+template <bool CONES, bool LP = false> __global__ void k_scaling(Ptrs p, int first) {
     PB_SETUP
     if (S.done) return;
     double *l = p.lmbda + om, *lsq = p.lmbdasq + om;
     const double *s = p.s + om, *z = p.z + om;
+    double ll = 0;
     for (int i = tid; i < p.ml; i += nt) {
         if (first) {
             const double d = sqrt(s[i] / z[i]), di = 1.0 / d;
@@ -341,7 +358,9 @@ template <bool CONES> __global__ void k_scaling(Ptrs p, int first) {
             if (!CONES) p.di2[om + i] = di * di;
             l[i] = sqrt(s[i] * z[i]);
         }
-        lsq[i] = l[i] * l[i];
+        const double li2 = l[i] * l[i];
+        lsq[i] = li2;
+        if (LP) ll += li2;
     }
     double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     if (CONES) FOR_CONES(o, len) {
@@ -372,8 +391,17 @@ template <bool CONES> __global__ void k_scaling(Ptrs p, int first) {
         nl = warp_sum(nl);
         const double l0 = l[o];
         FOR_LANE(i, len) lsq[o + i] = (i == 0) ? nl : 2.0 * l0 * l[o + i];
+        if (LP && lane == 0) ll += nl;
     }
-    if (tid == 0) { S.mu = S.gap / (p.ml + p.nq); S.sigma = 0.0; S.eta = 0.0; }
+    if (LP) {
+        ll = block_sum(ll, sh);
+        if (tid == 0) {
+            LPScal &T = lp_scal(p, oc);
+            if (first) { T.dg = sqrt(T.kappa / T.tau); T.dgi = sqrt(T.tau / T.kappa); T.lg = sqrt(T.tau * T.kappa); }
+            T.lgsq = T.lg * T.lg;
+            S.mu = (ll + T.lgsq) / (1.0 + p.m); S.sigma = 0.0;
+        }
+    } else if (tid == 0) { S.mu = S.gap / (p.ml + p.nq); S.sigma = 0.0; S.eta = 0.0; }
 }
 
 // f4_no_ir before the solve (coneprog.py:2301-2309): s := lmbda o\ s; z := z - W's; bzp := W^{-T} z.
@@ -500,8 +528,9 @@ template <bool EQ> __global__ void k_res(Ptrs p) {
     }
 }
 // after the i-th direction: ds o dz, scale2 of ds and dz, step length, sigma (coneprog.py:2423-2456).
-// f4_post: the solve has just run without refinement, so f4_no_ir's step after it is done here first
-template <bool CONES> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
+// f4_post: the solve has just run without refinement, so f4_no_ir's step after it is done here first.
+// LP: conelp's dkappa dtau product, tt and tk in the step, sigma = (1 - step)^3 (coneprog.py:1302-1333)
+template <bool CONES, bool LP = false> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
     PB_SETUP
     double *ds = p.ds + om, *dz = p.dz + om;
     const double *l = p.lmbda + om;
@@ -539,12 +568,21 @@ template <bool CONES> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
     mins = block_min(mins, sh);
     minz = block_min(minz, sh);
     if (tid == 0) {
-        const double t = fmax(0.0, fmax(-mins, -minz));
+        double t = fmax(0.0, fmax(-mins, -minz));
+        if (LP) {
+            LPScal &T = lp_scal(p, oc);
+            if (i == 0) T.wkappa3 = T.dtau * T.dkappa;
+            T.tt = -T.dtau / T.lg; T.tk = -T.dkappa / T.lg;
+            t = fmax(t, fmax(T.tt, T.tk));
+        }
         double step;
         if (t == 0.0) step = 1.0;
         else step = (i == 0) ? fmin(1.0, 1.0 / t) : fmin(1.0, 0.99 / t);
         S.step = step; S.dsdz = dsdz;
-        if (i == 0) {
+        if (i == 0 && LP) {
+            const double v = 1.0 - step;
+            S.sigma = v * v * v;
+        } else if (i == 0) {
             const double v = fmin(1.0, fmax(0.0, 1.0 - step + dsdz / S.gap * step * step));
             S.sigma = v * v * v;
             S.eta = 0.0;
@@ -552,11 +590,19 @@ template <bool CONES> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
     }
 }
 // x += step dx; ds, dz := e + step d; scale2 inverse; update_scaling (misc.py:439-573); s = W' lmbda,
-// z = W^{-1} lmbda; gap (coneprog.py:2459-2547).  EQ: y += step dy (:2460); a singular Kp stops the problem too
-template <bool CONES, bool EQ> __global__ void k_update(Ptrs p, const int *info, int iter) {
+// z = W^{-1} lmbda; gap (coneprog.py:2459-2547).  EQ: y += step dy (:2460); a singular Kp stops the problem too.
+// LP: conelp's dg, lmbdag, tau, kappa and gap (coneprog.py:1405-1436); a singular factorisation returns the iterate
+// divided by tau (:1078-1109)
+template <bool CONES, bool EQ, bool LP = false> __global__ void k_update(Ptrs p, const int *info, int iter) {
     PB_SETUP
     if (S.done) return;
     if (info[b] > 0 || (EQ && p.infop[b] > 0)) {   // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
+        if (LP) {
+            const double ti = 1.0 / lp_scal(p, oc).tau;
+            for (int k = tid; k < p.n; k += nt) p.x[on + k] *= ti;
+            if (EQ) for (int k = tid; k < p.neq; k += nt) p.y[oq + k] *= ti;
+            for (int k = tid; k < p.m; k += nt) { p.s[om + k] *= ti; p.z[om + k] *= ti; }
+        }
         if (tid == 0) { S.done = 1; S.status = 3; S.iters = iter; }
         return;
     }
@@ -626,13 +672,325 @@ template <bool CONES, bool EQ> __global__ void k_update(Ptrs p, const int *info,
         if (lane == 0) gap += g;
     }
     gap = block_sum(gap, sh);
-    if (tid == 0) S.gap = gap;
+    if (LP) {
+        if (tid == 0) {
+            LPScal &T = lp_scal(p, oc);
+            T.dg *= sqrt(1.0 - step * T.tk) / sqrt(1.0 - step * T.tt);
+            T.dgi = 1.0 / T.dg;
+            T.lg *= sqrt(1.0 - step * T.tt) * sqrt(1.0 - step * T.tk);
+            T.kappa = T.lg / T.dgi; T.tau = T.lg * T.dgi;
+            const double g = sqrt(gap) / T.tau;
+            S.gap = g * g;
+        }
+    } else if (tid == 0) S.gap = gap;
 }
 // the S + A'A switch of kkt_chol2's first factorisation (misc.py:1421-1447), per problem: a slot whose S = P + Gs'Gs
 // was singular at the start (info > 0) weights A'A by 1 in every later S
 __global__ void k_switch(double *aw, const int *info, int neq) {
     const double w = info[blockIdx.x] > 0 ? 1.0 : 0.0;
     for (int k = threadIdx.x; k < neq; k += blockDim.x) aw[(long long)blockIdx.x * neq + k] = w;
+}
+
+// ---- cone LPs: coneprog.conelp (coneprog.py:31-1436) ----
+// The kernels below are the arithmetic in which conelp's homogeneous self-dual embedding differs from coneqp; the
+// scaling, the factorisation, the KKT solves, f4_no_ir's cone steps, the step length and the update are coneqp's.
+// The primal start's solve has left uz in bzp: s = -uz (:698-701).  The dual start's right-hand side (-c, 0, 0):
+// k_init_rhs put -c in dx, here y = 0 and bz = 0 (:724-728)
+template <bool EQ> __global__ void k_lp_start_mid(Ptrs p) {
+    PB_SETUP
+    for (int i = tid; i < p.m; i += nt) { p.s[om + i] = -p.bzp[om + i]; p.bzp[om + i] = 0.0; }
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = 0.0;
+}
+// the starting point (:737-857): z from the dual start's solve, ts / tz, the "already optimal" return at iteration 0
+// (:744-804), the shifts by 1 + ts and 1 + tz, tau = kappa = 1, gap
+template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double abstol, double reltol) {
+    PB_SETUP
+    double *s = p.s + om, *z = p.z + om;
+    const double *zn = p.bzp + om, *h = p.h + om;
+    double ns = 0, nz = 0, sz = 0, cx = 0, by = 0, hz = 0, mins = INFINITY, minz = INFINITY;
+    for (int i = tid; i < p.n; i += nt) cx += p.q[on + i] * p.x[on + i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) by += p.beq[oq + i] * p.y[oq + i];
+    for (int i = tid; i < p.m; i += nt) {
+        const double zv = zn[i], sv = s[i];
+        z[i] = zv;
+        ns += sv * sv; nz += zv * zv; sz += sv * zv; hz += h[i] * zv;
+        if (i < p.ml) { mins = fmin(mins, sv); minz = fmin(minz, zv); }
+    }
+    if (CONES) FOR_CONES(o, len) {
+        mins = fmin(mins, q_margin(s + o, s[o], len, lane));
+        minz = fmin(minz, q_margin(zn + o, zn[o], len, lane));
+    }
+    ns = sqrt(block_sum(ns, sh)); nz = sqrt(block_sum(nz, sh));
+    sz = block_sum(sz, sh); cx = block_sum(cx, sh); hz = block_sum(hz, sh);
+    if (EQ) by = block_sum(by, sh);
+    mins = block_min(mins, sh); minz = block_min(minz, sh);
+    const double ts = -mins, tz = -minz, dcost = -by - hz;
+    const bool relv = cx < 0.0 || dcost > 0.0;
+    const double relgap = cx < 0.0 ? sz / -cx : sz / dcost;
+    if (ts <= 0 && tz <= 0 && (sz <= abstol || (relv && relgap <= reltol))) {
+        if (tid == 0) {
+            S.done = 1; S.status = 1; S.iters = 0; S.gap = sz;
+            S.pcost = cx; S.dcost = -(by + hz);
+        }
+        return;
+    }
+    const double as = (ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
+    const double az = (tz >= -1e-8 * fmax(nz, 1.0)) ? 1.0 + tz : 0.0;
+    for (int i = tid; i < p.ml; i += nt) { s[i] += as; z[i] += az; }
+    if (CONES) for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
+    __syncthreads();
+    double gap = 0;
+    for (int i = tid; i < p.m; i += nt) gap += s[i] * z[i];
+    gap = block_sum(gap, sh);
+    if (tid == 0) {
+        S.gap = gap;
+        LPScal &T = lp_scal(p, oc);
+        T.tau = 1.0; T.kappa = 1.0;
+    }
+}
+// residuals, part 1: rx = 0, rz = s, ry = 0; the GEMVs then make them hrx = -A'y - G'z, hrz = s + G x, hry = A x
+template <bool EQ> __global__ void k_lp_res_begin(Ptrs p) {
+    PB_SETUP
+    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = 0.0;
+    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = 0.0;
+}
+// residuals, part 2, and the stopping rule (:864-1023): rx = hrx - c tau, ry = hry - b tau, rz = hrz - h tau, rt;
+// optimal or maxiters divide the iterate by tau; a primal infeasibility certificate divides y and z by -h'z - b'y
+// and x, s become NaN (the reference's None); a dual infeasibility certificate divides x and s by -c'x and y, z
+// become NaN.  Status 4 primal infeasible, 5 dual infeasible.
+template <bool EQ> __global__ void k_lp_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol,
+                                              double feastol, int *ndone, int *doneflags) {
+    PB_SETUP
+    __shared__ int act;
+    __shared__ double fac;
+    if (!S.done) {
+        LPScal &T = lp_scal(p, oc);
+        const double tau = T.tau;
+        double hx = 0, rx2 = 0, hy = 0, ry2 = 0, hzz = 0, rz2 = 0, cx = 0, by = 0, hz = 0;
+        for (int i = tid; i < p.n; i += nt) {
+            const double v = p.rx[on + i], c = p.q[on + i], r = v + (-tau) * c;
+            p.rx[on + i] = r;
+            hx += v * v; rx2 += r * r; cx += c * p.x[on + i];
+        }
+        if (EQ) for (int i = tid; i < p.neq; i += nt) {
+            const double v = p.ry[oq + i], bb = p.beq[oq + i], r = v + (-tau) * bb;
+            p.ry[oq + i] = r;
+            hy += v * v; ry2 += r * r; by += bb * p.y[oq + i];
+        }
+        for (int i = tid; i < p.m; i += nt) {
+            const double v = p.rz[om + i], hh = p.h[om + i], r = v + (-tau) * hh;
+            p.rz[om + i] = r;
+            hzz += v * v; rz2 += r * r; hz += hh * p.z[om + i];
+        }
+        hx = block_sum(hx, sh); rx2 = block_sum(rx2, sh); cx = block_sum(cx, sh);
+        hzz = block_sum(hzz, sh); rz2 = block_sum(rz2, sh); hz = block_sum(hz, sh);
+        if (EQ) { hy = block_sum(hy, sh); ry2 = block_sum(ry2, sh); by = block_sum(by, sh); }
+        if (tid == 0) {
+            const double resx = sqrt(rx2) / tau, resy = sqrt(ry2) / tau, resz = sqrt(rz2) / tau;
+            T.rt = T.kappa + cx + by + hz;
+            S.resx = resx; S.resz = resz; S.resy = resy;
+            S.pcost = cx / tau; S.dcost = -(by + hz) / tau;
+            if (S.pcost < 0.0) { S.relgap = S.gap / -S.pcost; S.relgap_valid = 1; }
+            else if (S.dcost > 0.0) { S.relgap = S.gap / S.dcost; S.relgap_valid = 1; }
+            else { S.relgap = 0.0; S.relgap_valid = 0; }
+            S.pres = EQ ? fmax(resy / S.resy0, resz / S.resz0) : resz / S.resz0;
+            S.dres = resx / S.resx0;
+            const bool pinf = hz + by < 0.0 && sqrt(hx) / S.resx0 / (-hz - by) <= feastol;
+            const double dinfres = EQ ? fmax(sqrt(hy) / S.resy0, sqrt(hzz) / S.resz0) : sqrt(hzz) / S.resz0;
+            const bool dinf = cx < 0.0 && dinfres / (-cx) <= feastol;
+            const bool opt = S.pres <= feastol && S.dres <= feastol &&
+                             (S.gap <= abstol || (S.relgap_valid && S.relgap <= reltol));
+            act = 0;
+            if (opt || iter == maxiters) { act = 1; fac = 1.0 / tau; S.status = opt ? 1 : 2; }
+            else if (pinf) { act = 2; fac = 1.0 / (-hz - by); S.status = 4; S.pcost = NAN; S.dcost = 1.0; }
+            else if (dinf) { act = 3; fac = 1.0 / (-cx); S.status = 5; S.pcost = -1.0; S.dcost = NAN; }
+            if (act) { S.done = 1; S.iters = iter; }
+        }
+        __syncthreads();
+        if (act) {
+            const double f = fac, nan = NAN;
+            const double fx = act == 2 ? nan : f, fy = act == 3 ? nan : f;
+            for (int i = tid; i < p.n; i += nt) p.x[on + i] = act == 2 ? nan : p.x[on + i] * fx;
+            if (EQ) for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = act == 3 ? nan : p.y[oq + i] * fy;
+            for (int i = tid; i < p.m; i += nt) {
+                p.s[om + i] = act == 2 ? nan : p.s[om + i] * fx;
+                p.z[om + i] = act == 3 ? nan : p.z[om + i] * fy;
+            }
+        }
+    }
+    if (tid == 0) {
+        if (S.done) atomicAdd(ndone, 1);
+        doneflags[b] = S.done;
+    }
+}
+// the extra solve's right-hand side (:1066-1074): x1 = -c, y1 = b, z1 = h, and th = W^{-T} h (:1125-1128), which is
+// also the solve's bzp
+template <bool EQ> __global__ void k_lp_x1_rhs(Ptrs p) {
+    PB_SETUP
+    for (int i = tid; i < p.n; i += nt) p.x1[on + i] = -p.q[on + i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.y1[oq + i] = p.beq[oq + i];
+    const double *h = p.h + om;
+    double *th = p.th + om, *bz = p.bzp + om;
+    for (int i = tid; i < p.ml; i += nt) { const double t = p.di[om + i] * h[i]; th[i] = t; bz[i] = t; }
+    const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
+    FOR_CONES(o, len) {
+        q_scale(v + o, beta[k_], h + o, th + o, len, lane, true);
+        __syncwarp();
+        FOR_LANE(i, len) bz[o + i] = th[o + i];
+    }
+}
+// (x1, y1, z1) *= dgi (:1075-1077); z1'z1 for f6_no_ir
+template <bool EQ> __global__ void k_lp_x1_post(Ptrs p) {
+    PB_SETUP
+    const double dgi = lp_scal(p, oc).dgi;
+    for (int i = tid; i < p.n; i += nt) p.x1[on + i] *= dgi;
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.y1[oq + i] *= dgi;
+    double a = 0;
+    for (int i = tid; i < p.m; i += nt) { const double v = dgi * p.bzp[om + i]; p.z1[om + i] = v; a += v * v; }
+    a = block_sum(a, sh);
+    if (tid == 0) lp_scal(p, oc).z1sq = a;
+}
+// right-hand side of the i-th Newton system (:1268-1298), the refinement's copy of it (:1212-1218), then f6_no_ir's
+// steps before the solve (:1154-1165): y := -y, and f4_no_ir's cone steps on (-bz, -bs) are s := -lmbda o\ bs,
+// z := -(bz + W's) with bzp = W^{-T} z.  Negation is exact, so this is the reference's arithmetic.
+template <bool CONES, bool EQ> __global__ void k_lp_dir_rhs(Ptrs p, int i) {
+    PB_SETUP
+    LPScal &T = lp_scal(p, oc);
+    const double sm = S.sigma * S.mu, c = 1.0 - S.sigma;
+    for (int k = tid; k < p.n; k += nt) {
+        const double dx = c * p.rx[on + k];
+        p.dx[on + k] = dx;
+        if (p.refinement) p.wx[oc + k] = dx;
+    }
+    if (EQ) for (int k = tid; k < p.neq; k += nt) {
+        const double dy = c * p.ry[oq + k];
+        p.dy[oq + k] = -dy;
+        if (p.refinement) p.wy[oc + k] = dy;
+    }
+    // row r: bs = lmbdasq (+ ws3 - sigma mu where e is 1, i = 1), bz = (1 - sigma) rz; returns -bz, -bs
+    auto rhs = [&](int r, bool e, double &z, double &s) {
+        s = p.lmbdasq[om + r];
+        if (i == 1) { s += p.ws3[om + r]; if (e) s -= sm; }
+        z = c * p.rz[om + r];
+        if (p.refinement) { p.wz[oc + r] = z; p.ws[oc + r] = s; }
+        z = -z; s = -s;
+    };
+#pragma unroll 1
+    for (int k = tid; k < p.ml; k += nt) {
+        double z, s;
+        rhs(k, true, z, s);
+        f4_pre_row(p, om + k, z, s);
+        p.dz[om + k] = z; p.ds[om + k] = s;
+    }
+    if (CONES) {
+        for (int k = p.ml + tid; k < p.m; k += nt) {
+            double z, s;
+            rhs(k, false, z, s);
+            p.dz[om + k] = z; p.ds[om + k] = s;
+        }
+        __syncthreads();
+        FOR_CONES(o, len) {
+            if (lane == 0 && i == 1) { p.ds[om + o] += sm; if (p.refinement) p.ws[oc + o] -= sm; }
+            __syncwarp();
+            f4_pre_cone(p, om, oc, k_, o, len, lane, p.dz + om, p.ds + om);
+        }
+    }
+    if (tid == 0) {
+        T.dtau = c * T.rt;
+        T.dkappa = (i == 1) ? T.lgsq + (T.wkappa3 - sm) : T.lgsq;
+        if (p.refinement) { T.wtau = T.dtau; T.wkappa = T.dkappa; }
+    }
+}
+// f6_no_ir after the solve (:1180-1195): with the solve's (x, y) and uz in bzp, kappa := -bkappa / lmbdag,
+// tau := dgi (btau - bkappa / tau + c'x + b'y + th'uz) / (1 + z1'z1), (x, y, z) += tau (x1, y1, z1), s := s - z,
+// kappa -= tau.  acc = 0: the Newton solve, in place on (dx, dy, ds), z to dz, (btau, bkappa) = (dtau, dkappa).
+// acc = 1: a refinement step on (wx2, wy2, ws2) with (wtau2, wkappa2), added to the direction (:1230-1235).
+template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx, double *y, long long sy, double *s,
+                                                long long ss, int acc) {
+    PB_SETUP
+    LPScal &T = lp_scal(p, oc);
+    x += b * sx; s += b * ss;
+    if (EQ) y += b * sy;
+    const double *uz = p.bzp + om, *c = p.q + on, *x1 = p.x1 + on, *z1 = p.z1 + om, *th = p.th + om;
+    const double tin = acc ? T.wtau2 : T.dtau, kin = acc ? T.wkappa2 : T.dkappa;
+    double cx = 0, by = 0, tz = 0;
+    for (int i = tid; i < p.n; i += nt) cx += c[i] * x[i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) by += p.beq[oq + i] * y[i];
+    for (int i = tid; i < p.m; i += nt) tz += th[i] * uz[i];
+    cx = block_sum(cx, sh); tz = block_sum(tz, sh);
+    if (EQ) by = block_sum(by, sh);
+    double kap = -kin / T.lg;
+    double tau = tin + kap / T.dgi;
+    tau = T.dgi * (tau + cx + by + tz) / (1.0 + T.z1sq);
+    for (int i = tid; i < p.n; i += nt) {
+        const double v = x[i] + tau * x1[i];
+        if (acc) p.dx[on + i] += v; else x[i] = v;
+    }
+    if (EQ) for (int i = tid; i < p.neq; i += nt) {
+        const double v = y[i] + tau * p.y1[oq + i];
+        if (acc) p.dy[oq + i] += v; else y[i] = v;
+    }
+    for (int i = tid; i < p.m; i += nt) {
+        const double zv = uz[i] + tau * z1[i], sv = s[i] - zv;
+        if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
+        else { p.dz[om + i] = zv; s[i] = sv; }
+    }
+    kap -= tau;
+    if (tid == 0) {
+        if (acc) { T.dtau += tau; T.dkappa += kap; }
+        else { T.dtau = tau; T.dkappa = kap; }
+    }
+}
+// refinement residual, the elementwise part of conelp's res() (:599-631) on the copies of the right-hand side:
+// wx2 = wx - c dtau/dg, wz3 = W^{-1} dz, wtau2 = wtau + dg dkappa + c'dx + b'dy + h'wz3, wkappa2 = wkappa +
+// lmbdag (dtau + dkappa), and, negated for the following f6_no_ir (y := -y, f4_no_ir on (-bz, -bs)):
+// wy2 = -(wy - b dtau/dg), wz2 = -(wz - h dtau/dg + W'ds), ws2 = -(ws + lmbda o (dz + ds)).  The A, A', G and G'
+// products follow as batched GEMVs.
+template <bool EQ> __global__ void k_lp_res(Ptrs p) {
+    PB_SETUP
+    LPScal &T = lp_scal(p, oc);
+    const double ut = T.dtau / T.dg;
+    const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om, *h = p.h + om;
+    double cx = 0, by = 0, hz = 0;
+    for (int i = tid; i < p.n; i += nt) {
+        const double c = p.q[on + i];
+        p.wx2[oc + i] = p.wx[oc + i] + (-ut) * c;
+        cx += c * p.dx[on + i];
+    }
+    if (EQ) for (int i = tid; i < p.neq; i += nt) {
+        const double bb = p.beq[oq + i];
+        p.wy2[oc + i] = -(p.wy[oc + i] + (-ut) * bb);
+        by += bb * p.dy[oq + i];
+    }
+    double *wz3 = p.wz3 + oc, *wz2 = p.wz2 + oc, *ws2 = p.ws2 + oc;
+    for (int i = tid; i < p.ml; i += nt) {
+        const double w3 = p.di[om + i] * dz[i];
+        wz3[i] = w3;
+        hz += h[i] * w3;
+        wz2[i] = -((p.wz[oc + i] + (-ut) * h[i]) + p.d[om + i] * ds[i]);
+        ws2[i] = -(p.ws[oc + i] + l[i] * (dz[i] + ds[i]));
+    }
+    const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
+    FOR_CONES(o, len) {
+        q_scale(v + o, beta[k_], dz + o, wz3 + o, len, lane, true);
+        q_scale(v + o, beta[k_], ds + o, wz2 + o, len, lane, false);
+        double a = 0;
+        FOR_LANE(i, len) a += l[o + i] * (ds[o + i] + dz[o + i]);
+        a = warp_sum(a);
+        const double u0 = ds[o] + dz[o], l0 = l[o];
+        FOR_LANE(i, len) {
+            hz += h[o + i] * wz3[o + i];
+            wz2[o + i] = -((p.wz[oc + o + i] + (-ut) * h[o + i]) + wz2[o + i]);
+            ws2[o + i] = -(p.ws[oc + o + i] + ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]));
+        }
+    }
+    cx = block_sum(cx, sh); hz = block_sum(hz, sh);
+    if (EQ) by = block_sum(by, sh);
+    if (tid == 0) {
+        T.wtau2 = T.wtau + (T.dg * T.dkappa + cx + by + hz);
+        T.wkappa2 = T.wkappa + T.lg * (T.dtau + T.dkappa);
+    }
 }
 
 }  // namespace
@@ -677,6 +1035,9 @@ struct cvxb_batch {
     DevBuf<int> d_infop;
     bool eq_loaded = false;          // cvxb_batch_load_eq since the last cvxb_batch_load
     bool switched = false;           // some problem of this solve factors S + A'A (its aw is 1)
+    // cone LP batch (cvxb_batch_create_lp): no P; q holds c; lpv holds x1 (n), z1 and th (m), y1 (p) per slot
+    bool lp = false;
+    DevBuf<double> lpv;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -687,27 +1048,29 @@ struct cvxb_batch {
 namespace {
 
 // The per-slot state row: v (sum q) | beta (nq) with cones, wx wx2 (n) | wz ws wz2 ws2 wz3 (m) | wy wy2 (p) with
-// refinement; every piece starts 16-byte aligned.  Reallocated when the layout changes: nothing in it outlives a solve.
+// refinement, LPScal in a cone LP batch; every piece starts 16-byte aligned.  Reallocated when the layout changes: nothing in it outlives a solve.
 int state_alloc(cvxb_batch *b) {
     Ptrs &p = b->p;
     auto ev = [](long long x) { return (x + 1) & ~1LL; };
     const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m), p2 = ev(b->neq);
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
-    if (b->L == cone + ref) return 0;
+    const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
+    if (b->L == cone + ref + lps) return 0;
     b->L = p.L = 0;
     b->cst.reset();
-    p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = p.wy = p.wy2 = nullptr;
-    if (cone + ref == 0) return 0;
-    CVXB_TRY(b->cst.alloc((size_t)b->B * (cone + ref)));
-    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * (cone + ref) * sizeof(double)));
-    b->L = p.L = cone + ref;
+    p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = p.wy = p.wy2 = p.lps = nullptr;
+    if (cone + ref + lps == 0) return 0;
+    CVXB_TRY(b->cst.alloc((size_t)b->B * (cone + ref + lps)));
+    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * (cone + ref + lps) * sizeof(double)));
+    b->L = p.L = cone + ref + lps;
     double *r = b->cst.p;
     if (cone) { p.v = r; r += ev(sumq); p.beta = r; r += ev(p.nq); }
     if (ref) {
         p.wx = r; r += n2; p.wx2 = r; r += n2;
         p.wz = r; r += m2; p.ws = r; r += m2; p.wz2 = r; r += m2; p.ws2 = r; r += m2; p.wz3 = r; r += m2;
-        if (p2) { p.wy = r; r += p2; p.wy2 = r; }
+        if (p2) { p.wy = r; r += p2; p.wy2 = r; r += p2; }
     }
+    if (lps) p.lps = r;
     return 0;
 }
 
@@ -861,7 +1224,7 @@ int swap_slots(cvxb_batch *b, const std::vector<int> &pairs) {
     if (np == 0) return 0;
     CVXB_CUDA(cudaMemcpyAsync(b->d_pairs.p, pairs.data(), pairs.size() * sizeof(int), cudaMemcpyHostToDevice, b->st));
     SwapArgs a;
-    a.P = b->P.p; a.G = b->G.p; a.vecs = b->vecs.p; a.sc = b->sc.p; a.sP = b->sP; a.sG = b->sG;
+    a.P = b->P.p; a.G = b->G.p; a.vecs = b->vecs.p; a.sc = b->sc.p; a.sP = b->P.p ? b->sP : 0; a.sG = b->sG;
     a.n = b->n; a.me = b->m > 0 ? b->m : 1; a.Btot = b->B;
     a.A = b->A.p; a.pvecs = b->pvecs.p; a.sA = b->sA; a.neq = b->neq;
     k_swap_slots<<<dim3(96, np), 256, 0, b->st>>>(a, b->d_pairs.p);
@@ -891,6 +1254,66 @@ int restore_order(cvxb_batch *b) {
     return 0;
 }
 
+// the starting point's factorisation with W = I.  EQ: kkt_chol2's first factorisation (misc.py:1421-1447): a problem
+// whose S is singular factors S + A'A from now on
+template <bool EQ> int start_factor(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int B = b->Bact;
+    CVXB_TRY(batch_factor(b, false));
+    if (EQ) {
+        std::vector<int> info(B);
+        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaStreamSynchronize(st));
+        for (int i = 0; i < B; ++i) b->switched |= info[i] > 0;
+        if (b->switched) {
+            k_switch<<<B, 256, 0, st>>>(b->p.aw, b->d_info.p, b->neq); count_launch();
+            CVXB_TRY(batch_factor(b, false));
+        }
+        CVXB_TRY(factor_kp(b));
+    }
+    return 0;
+}
+
+// a singular first factorisation is the reference's "Rank(A) < p or Rank([P; A; G]) < n" ValueError
+// (coneprog.py:2065-2067), without A Rank([P; G]) < n; conelp's is "Rank(A) < p or Rank([G; A]) < n" (:680-700)
+template <bool EQ> int start_check(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int B = b->Bact;
+    std::vector<int> info(B), infop(EQ ? B : 0);
+    CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (EQ) CVXB_CUDA(cudaMemcpyAsync(infop.data(), b->d_infop.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i < B; ++i)
+        if (info[i] > 0 || (EQ && infop[i] > 0)) {
+            if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
+                                 "the start)", i);
+            else if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
+                                   "at the start)", i);
+            else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
+            return CVXB_E_ARG;
+        }
+    return 0;
+}
+
+// finished slots below the new active count trade places with active slots from the tail; b->Bact becomes the
+// number of active problems
+int compact_slots(cvxb_batch *b, int B, int ndone, const std::vector<int> &flags, std::vector<int> &pairs) {
+    const int nb = B - ndone;
+    pairs.clear();
+    int j = B - 1;
+    for (int i = 0; i < nb; ++i) {
+        if (!flags[i]) continue;
+        while (flags[j]) --j;             // an active slot in [nb, B): there are as many as finished ones below nb
+        pairs.push_back(i); pairs.push_back(j);
+        std::swap(b->perm[i], b->perm[j]);
+        --j;
+    }
+    CVXB_TRY(swap_slots(b, pairs));
+    b->permuted = true;
+    b->Bact = nb;
+    return 0;
+}
+
 // the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows
 template <bool CONES, bool EQ>
 int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
@@ -909,38 +1332,12 @@ int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, do
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I ----
     k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_factor(b, false));
-    std::vector<int> info(B), infop(EQ ? B : 0);
-    if (EQ) {
-        // kkt_chol2's first factorisation (misc.py:1421-1447): a problem whose S is singular factors S + A'A from
-        // now on
-        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        for (int i = 0; i < B; ++i) b->switched |= info[i] > 0;
-        if (b->switched) {
-            k_switch<<<B, T, 0, st>>>(p.aw, b->d_info.p, pq); count_launch();
-            CVXB_TRY(batch_factor(b, false));
-        }
-        CVXB_TRY(factor_kp(b));
-    }
+    CVXB_TRY(start_factor<EQ>(b));
     k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
     CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
     k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
     CVXB_LAUNCH_CHECK();
-    {
-        // a singular first factorisation is the reference's "Rank(A) < p or Rank([P; A; G]) < n" ValueError
-        // (coneprog.py:2065-2067); without A it can only be Rank([P; G]) < n
-        CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        if (EQ) CVXB_CUDA(cudaMemcpyAsync(infop.data(), b->d_infop.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        for (int i = 0; i < B; ++i)
-            if (info[i] > 0 || (EQ && infop[i] > 0)) {
-                if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
-                                  "at the start)", i);
-                else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
-                return CVXB_E_ARG;
-            }
-    }
+    CVXB_TRY(start_check<EQ>(b));
     std::vector<int> flags(B), pairs;
     int it = 0;
     for (it = 0; it <= maxiters; ++it) {
@@ -965,27 +1362,119 @@ int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, do
         CVXB_CUDA(cudaStreamSynchronize(st));
         if (ndone >= B) break;
         if (ndone > 0 && b->compact && b->B > 1) {
-            // finished slots below the new active count trade places with active slots from the tail
-            const int nb = B - ndone;
-            pairs.clear();
-            int j = B - 1;
-            for (int i = 0; i < nb; ++i) {
-                if (!flags[i]) continue;
-                while (flags[j]) --j;             // an active slot in [nb, B): there are as many as finished ones below nb
-                pairs.push_back(i); pairs.push_back(j);
-                std::swap(b->perm[i], b->perm[j]);
-                --j;
-            }
-            CVXB_TRY(swap_slots(b, pairs));
-            b->permuted = true;
-            B = nb;
-            b->Bact = B;
+            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
+            B = b->Bact;
             gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
         }
         k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         CVXB_TRY(batch_factor(b));
         for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ>(b, i)));
         k_update<CONES, EQ><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
+        CVXB_LAUNCH_CHECK();
+    }
+    b->iters_run = it;
+    b->Bact = b->B;
+    CVXB_CUDA(cudaEventRecord(b->e1, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    float t = 0;
+    cudaEventElapsedTime(&t, b->e0, b->e1);
+    b->solve_ms = t;
+    return 0;
+}
+
+// conelp's i-th Newton direction: f6 (coneprog.py:1211-1235), i.e. f6_no_ir and then `refinement` correction steps
+// from res(), followed by the step length and sigma
+template <bool CONES, bool EQ> int direction_lp(cvxb_batch *b, int i) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
+    const Ptrs &p = b->p;
+    const long long L = b->L;
+    k_lp_dir_rhs<CONES, EQ><<<B, T, 0, st>>>(p, i); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
+    k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch();
+    for (int r = 0; r < p.refinement; ++r) {
+        // res() (:599-631): wx2 -= A' dy + G' W^{-1} dz, -wy2 += A dx, -wz2 += G dx
+        k_lp_res<EQ><<<B, T, 0, st>>>(p); count_launch();
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
+        }
+        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
+        }
+        GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
+        k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
+        CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
+        k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1); count_launch();
+    }
+    k_dir_post<CONES, true><<<B, T, 0, st>>>(p, i, 0); count_launch();
+    return 0;
+}
+
+// the lock-step conelp over the active slots (coneprog.py:662-1436): the same factorisations, solves, scaling and
+// compaction as solve_lockstep, on a batch without P, with the self-dual embedding's tau and kappa, one more KKT
+// solve per iteration for (x1, y1, z1), and infeasibility certificates
+template <bool CONES, bool EQ>
+int solve_conelp(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, T = 256, pq = b->neq;
+    int B = b->B;
+    b->Bact = B;
+    b->switched = false;
+    const Ptrs &p = b->p;
+    GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
+    GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
+    GemvBatch gAt; gAt.batch = B; gAt.sA = b->sA; gAt.sx = pq; gAt.sy = n;
+    GemvBatch gAn; gAn.batch = B; gAn.sA = b->sA; gAn.sx = n; gAn.sy = pq;
+    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
+    CVXB_CUDA(cudaEventRecord(b->e0, st));
+    // ---- starting point: W = I (:662-857) ----
+    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();       // dx = -c, y = b, dz = h, resx0 / resy0 / resz0
+    CVXB_TRY(start_factor<EQ>(b));
+    k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
+    CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
+    CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));                // primal start: (0, b, h)
+    k_lp_start_mid<EQ><<<B, T, 0, st>>>(p); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));               // dual start: (-c, 0, 0)
+    k_lp_init_point<CONES, EQ><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
+    CVXB_LAUNCH_CHECK();
+    CVXB_TRY(start_check<EQ>(b));
+    std::vector<int> flags(B), pairs;
+    int it = 0;
+    for (it = 0; it <= maxiters; ++it) {
+        // residuals (:861-896)
+        k_lp_res_begin<EQ><<<B, T, 0, st>>>(p); count_launch();
+        if (EQ) {
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, -1.0, 1.0, p.rx, st, gAt));                // -A'y
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, 1.0, p.ry, b->gemv_ws.p, st, gAn));   // A x
+        }
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, -1.0, 1.0, p.rx, st, gGt));
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_lp_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        count_launch();
+        int ndone = 0;
+        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_CUDA(cudaStreamSynchronize(st));
+        if (ndone >= B) break;
+        if (ndone > 0 && b->compact && b->B > 1) {
+            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
+            B = b->Bact;
+            gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
+        }
+        k_scaling<CONES, true><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
+        CVXB_TRY(batch_factor(b));
+        // (x1, y1, z1) from (-c, b, h) (:1066-1077), th = W^{-T} h
+        k_lp_x1_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
+        CVXB_TRY(batch_solve(b, p.x1, n, p.y1, pq));
+        k_lp_x1_post<EQ><<<B, T, 0, st>>>(p); count_launch();
+        for (int i = 0; i < 2; ++i) CVXB_TRY((direction_lp<CONES, EQ>(b, i)));
+        k_update<CONES, EQ, true><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -1015,11 +1504,8 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
     return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
+// a batch of QPs, or of cone LPs (lp: no P)
+int create_batch(cvxb_batch **out, int nprob, int n, int m, int device, bool lp) {
     if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
     if (nprob > CVXB_BATCH_MAX) {
         set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
@@ -1028,7 +1514,7 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     *out = nullptr;
     CVXB_TRY(check_device(device));
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
-    b->device = device; b->B = nprob; b->n = n; b->m = m;
+    b->device = device; b->B = nprob; b->n = n; b->m = m; b->lp = lp;
     b->i8_mode = ozaki_mode();
     b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
@@ -1039,7 +1525,7 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     CVXB_CUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
     CVXB_CUDA(cudaEventCreate(&b->e0)); CVXB_CUDA(cudaEventCreate(&b->e1));
     CVXB_TRY(chol_work_create(b->cw));
-    CVXB_TRY(b->P.alloc(B * b->sP));
+    if (!lp) CVXB_TRY(b->P.alloc(B * b->sP));
     CVXB_TRY(b->G.alloc(B * b->sG));
     CVXB_TRY(b->K.alloc(B * b->sK));
     CVXB_TRY(b->inv.alloc(B * b->sInv));
@@ -1074,7 +1560,7 @@ int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     return 0;
 }
 
-int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
+int create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device, bool lp) {
     if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
     if (nprob > CVXB_BATCH_MAX) {
         set_error("batch_create_cones: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob,
@@ -1094,7 +1580,7 @@ int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims 
     if (m > (1LL << 30)) { set_error("batch_create_cones: too many cone rows"); return CVXB_E_ARG; }
     if (dims->ns > 0) { set_error("batch_create_cones: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
     cvxb_batch *b = nullptr;
-    CVXB_TRY(cvxb_batch_create(&b, nprob, n, (int)m, device));
+    CVXB_TRY(create_batch(&b, nprob, n, (int)m, device, lp));
     std::unique_ptr<cvxb_batch> own(b);
     if (dims->nq > 0) {
         const int nq = dims->nq;
@@ -1111,7 +1597,7 @@ int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims 
     return 0;
 }
 
-int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+int create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp) {
     if (out) *out = nullptr;
     if (!out || p < 0) { set_error("batch_create_eq: bad sizes (p must be nonnegative)"); return CVXB_E_ARG; }
     if (n > 0 && p > n) {                         // coneqp's check before the first factorisation (coneprog.py:1962)
@@ -1119,7 +1605,7 @@ int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_d
         return CVXB_E_ARG;
     }
     cvxb_batch *b = nullptr;
-    CVXB_TRY(cvxb_batch_create_cones(&b, nprob, n, dims, device));    // sizes and dims are checked before the device
+    CVXB_TRY(create_cones(&b, nprob, n, dims, device, lp));     // sizes and dims are checked before the device
     std::unique_ptr<cvxb_batch> own(b);
     if (p > 0) {
         const size_t B = b->B;
@@ -1152,6 +1638,63 @@ int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_d
     return 0;
 }
 
+}  // namespace
+
+extern "C" {
+
+int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
+    return create_batch(out, nprob, n, m, device, false);
+}
+
+int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
+    return create_cones(out, nprob, n, dims, device, false);
+}
+
+int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+    return create_eq(out, nprob, n, p, dims, device, false);
+}
+
+int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+    if (out) *out = nullptr;
+    if (!out || nprob <= 0 || n <= 0 || p < 0 || !dims) {
+        set_error("batch_create_lp: bad sizes (nprob and n positive, p nonnegative, dims given)");
+        return CVXB_E_ARG;
+    }
+    if (nprob > CVXB_BATCH_MAX) {
+        set_error("batch_create_lp: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("batch_create_lp: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
+        return CVXB_E_ARG;
+    }
+    long long m = dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("batch_create_lp: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
+        m += dims->q[k];
+    }
+    if (dims->ns > 0) { set_error("batch_create_lp: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    if (m == 0) {                                 // deliberate: every problem needs at least one cone row
+        set_error("batch_create_lp: the batch needs at least one 'l' or 'q' row (m = 0)");
+        return CVXB_E_ARG;
+    }
+    if (p > n || p + m < n) {                     // conelp's check before the first factorisation (coneprog.py:572-573)
+        set_error("batch_create_lp: Rank(A) < p or Rank([G; A]) < n (p = %d, n = %d, cdim = %lld)", p, n, m);
+        return CVXB_E_ARG;
+    }
+    cvxb_batch *b = nullptr;
+    CVXB_TRY(create_eq(&b, nprob, n, p, dims, device, true));
+    std::unique_ptr<cvxb_batch> own(b);
+    const size_t B = b->B;
+    CVXB_TRY(b->lpv.alloc(B * ((size_t)n + 2 * (size_t)m + (size_t)p)));
+    CVXB_CUDA(cudaMemset(b->lpv.p, 0, B * ((size_t)n + 2 * (size_t)m + (size_t)p) * sizeof(double)));
+    Ptrs &q = b->p;
+    q.x1 = b->lpv.p; q.z1 = q.x1 + B * n; q.th = q.z1 + B * m; q.y1 = q.th + B * m;
+    CVXB_TRY(state_alloc(b));
+    *out = own.release();
+    return 0;
+}
+
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
@@ -1170,6 +1713,7 @@ void cvxb_batch_destroy(cvxb_batch *b) {
 int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
                     const double *h, int space) {
     if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
+    if (b->lp) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t B = b->B, n = b->n, m = b->m;
@@ -1184,6 +1728,24 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
     // only tril(P) is significant in the reference; make the resident copies symmetric
     CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    b->eq_loaded = false;
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    b->permuted = false;
+    return 0;
+}
+
+int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space) {
+    if (!b || !c || !G || !h) { set_error("batch_load_lp: NULL argument"); return CVXB_E_ARG; }
+    if (!b->lp) { set_error("batch_load_lp: a QP batch is loaded with cvxb_batch_load"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const size_t B = b->B, n = b->n, m = b->m;
+    CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double), m * sizeof(double), n * B,
+                                kind, b->st));
+    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
+    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), c, B * n * sizeof(double), kind, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->loaded = true;
     b->eq_loaded = false;
@@ -1219,6 +1781,12 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
     const bool cones = b->p.nq > 0;
+    if (b->lp) {
+        if (b->neq > 0) return cones ? solve_conelp<true, true>(b, maxiters, abstol, reltol, feastol)
+                                     : solve_conelp<false, true>(b, maxiters, abstol, reltol, feastol);
+        return cones ? solve_conelp<true, false>(b, maxiters, abstol, reltol, feastol)
+                     : solve_conelp<false, false>(b, maxiters, abstol, reltol, feastol);
+    }
     if (b->neq > 0) return cones ? solve_lockstep<true, true>(b, maxiters, abstol, reltol, feastol)
                                  : solve_lockstep<false, true>(b, maxiters, abstol, reltol, feastol);
     return cones ? solve_lockstep<true, false>(b, maxiters, abstol, reltol, feastol)

@@ -239,6 +239,18 @@ int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims 
  * rounded up to even with refinement (wy, wy2), plus one int (Kp's info); all of it is counted by cvxb_device_bytes
  * and freed by cvxb_batch_destroy. */
 int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
+/* batch of cone LPs  min c'x  s.t.  G x + s = h,  s in 'l' x 'q' cones,  A x = b  with p equality rows per problem
+ * (B x conelp(c, G, h, dims, A, b), coneprog.py:31-1436: the self-dual embedding with its infeasibility
+ * certificates; kktsolver 'chol2' without 'q' cones, 'chol' with them; refinement 0 without 'q' cones, 1 with them).
+ * Load it with cvxb_batch_load_lp (and cvxb_batch_load_eq when p > 0); every other cvxb_batch_* call serves both kinds
+ * of batch.  CVXB_E_ARG, checked before the device: dims->mnl != 0, a cone order q[k] < 1, nprob > CVXB_BATCH_MAX,
+ * p < 0, and, as conelp's "Rank(A) < p or Rank([G; A]) < n", p > n or p + cdim < n.  m = cdim = 0 is CVXB_E_ARG too:
+ * a cone LP batch needs at least one cone row.  dims->ns > 0: CVXB_E_UNSUP.  A singular factorisation at the start
+ * (W = I) makes cvxb_batch_solve return CVXB_E_ARG naming the problem.  Device memory per problem, in doubles: that of
+ * the QP batch of the same n, cdim, p and dims without P's ldp*n (ldp = n rounded up to even), plus n + 2*cdim + p
+ * (x1, z1, W^{-T} h, y1) and 18 scalars (tau, kappa and the rest of the embedding) in the per-problem state row; all
+ * of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy. */
+int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);
@@ -248,9 +260,15 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
 /* A: nprob x (p x n column-major, ld p); bvec: nprob x p.  Call it after every cvxb_batch_load of a batch with
  * p > 0 equality rows (cvxb_batch_solve refuses such a batch with CVXB_E_ARG until it is); a no-op when p = 0. */
 int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space);
+/* cone LP batch only (cvxb_batch_load on it, and this call on a QP batch, are CVXB_E_ARG):
+ * c: nprob x n; G: nprob x (m x n column-major, ld m); h: nprob x m; m = cdim */
+int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space);
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol);
 /* status: 1 optimal, 2 maximum iterations reached, 3 singular KKT matrix ('unknown' in the
- * reference for 2 and 3).  x/s/z may be device pointers (space), scalars go to host memory. */
+ * reference for 2 and 3), and for cone LP batches 4 primal infeasible, 5 dual infeasible.  Where conelp returns None
+ * the results hold NaN: x, s and the primal objective of a primal infeasible problem (its dual objective is 1, y and
+ * z the certificate), y, z and the dual objective of a dual infeasible one (its primal objective is -1, x and s the
+ * certificate).  x/s/z may be device pointers (space), scalars go to host memory. */
 int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *status,
                        int *iters, double *pobj, double *dobj, int space);
 /* y: nprob x p, the multipliers of A x = b in the caller's problem order (as x, s, z); nothing when p = 0 */
