@@ -88,6 +88,7 @@ def _stack_eq(A, b, B, n):
 class QPBatch:
     """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
+    _lp = False              # ConeLPBatch: a batch of cone LPs
 
     def __init__(self, nprob, n, m, device=0, dims=None, p=0):
         if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
@@ -96,9 +97,11 @@ class QPBatch:
         self._lib = _lib.load()
         self._h = C.c_void_p()
         self.B, self.n, self.m, self.p = int(nprob), int(n), int(cdim), int(p)
-        if self.p != 0:
-            if d is None:
-                d, keep, _ = _batch_dims({"l": self.m})
+        if d is None and (self._lp or self.p):
+            d, keep, _ = _batch_dims({"l": self.m})
+        if self._lp:
+            rc = self._lib.cvxb_batch_create_lp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
+        elif self.p:
             rc = self._lib.cvxb_batch_create_eq(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
         elif d is None:
             rc = self._lib.cvxb_batch_create(C.byref(self._h), self.B, self.n, self.m, device)
@@ -108,27 +111,38 @@ class QPBatch:
         _lib.check(rc, "batch")
         self._refinement = None
 
+    def _host_eq(self, A, b):
+        """host A (B, p, n) and b (B, p) in the layout cvxb_batch_load_eq takes, checked against the batch's p"""
+        Acm, bv, p = _stack_eq(A, b, self.B, self.n)
+        if p != self.p:
+            raise TypeError("A has %d rows; the batch was created with p = %d" % (p, self.p))
+        return Acm, bv
+
+    def _load_eq(self, A, b, space):
+        """A and b after the problem data, nothing without equality rows: _host_eq's arrays, or raw addresses in
+        `space` of p x n column-major blocks and p-vectors"""
+        if not self.p:
+            return
+        if A is None or b is None:
+            raise TypeError("the batch has p = %d equality rows: give A and b" % self.p)
+        if isinstance(A, np.ndarray):
+            A, b = A.ctypes.data, b.ctypes.data
+        _lib.check(self._lib.cvxb_batch_load_eq(self._h, A, b, space), "batch_load_eq")
+
     def load(self, P, q, G, h, A=None, b=None):
         Pcm, q, Gcm, h, B, n, m = _stack(P, q, G, h)
         if (B, n, m) != (self.B, self.n, self.m):
             raise TypeError("problem shapes do not match the batch")
-        Acm, bv, p = _stack_eq(A, b, B, n)
-        if p != self.p:
-            raise TypeError("A has %d rows; the batch was created with p = %d" % (p, self.p))
+        Acm, bv = self._host_eq(A, b)
         rc = self._lib.cvxb_batch_load(self._h, Pcm.ctypes.data, q.ctypes.data, Gcm.ctypes.data,
                                        h.ctypes.data, _lib.HOST)
         _lib.check(rc, "batch_load")
-        if p:
-            _lib.check(self._lib.cvxb_batch_load_eq(self._h, Acm.ctypes.data, bv.ctypes.data, _lib.HOST),
-                       "batch_load_eq")
+        self._load_eq(Acm, bv, _lib.HOST)
 
     def load_ptr(self, P, q, G, h, space=_lib.DEVICE, A=None, b=None):
         """raw addresses of already laid-out buffers (device-resident callers); A: p x n column-major per problem"""
         _lib.check(self._lib.cvxb_batch_load(self._h, P, q, G, h, space), "batch_load")
-        if self.p:
-            if A is None or b is None:
-                raise TypeError("the batch has p = %d equality rows: give A and b" % self.p)
-            _lib.check(self._lib.cvxb_batch_load_eq(self._h, A, b, space), "batch_load_eq")
+        self._load_eq(A, b, space)
 
     def solve(self, refinement=None, **options):
         """refinement: steps of iterative refinement per Newton solve (coneqp's option); None keeps the default
@@ -289,22 +303,10 @@ class QPBatchGroup:
 class ConeLPBatch(QPBatch):
     """B cone LPs  min c'x  s.t.  G x + s = h,  s in K,  A x = b  (B x coneprog.conelp with default options, kktsolver
     'chol2' for 'l'-only problems, 'chol' with 'q' cones).  dims: 'l' and 'q' only, None is {'l': m}; m = cdim >= 1.
-    p: equality rows per problem.  solve / results / stats / close are QPBatch's; results()["status"] is one of
-    'optimal', 'primal infeasible', 'dual infeasible' or 'unknown', with NaN where conelp returns None."""
-
-    def __init__(self, nprob, n, m, device=0, dims=None, p=0):
-        if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
-            raise TypeError("p must be an integer")
-        d, keep, cdim = _batch_dims(dims, m)
-        if d is None:
-            d, keep, _ = _batch_dims({"l": int(cdim)})
-        self._lib = _lib.load()
-        self._h = C.c_void_p()
-        self.B, self.n, self.m, self.p = int(nprob), int(n), int(cdim), int(p)
-        rc = self._lib.cvxb_batch_create_lp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
-        del keep
-        _lib.check(rc, "batch")
-        self._refinement = None
+    p: equality rows per problem.  The constructor, solve / results / stats / close are QPBatch's;
+    results()["status"] is one of 'optimal', 'primal infeasible', 'dual infeasible' or 'unknown', with NaN where
+    conelp returns None."""
+    _lp = True
 
     def load(self, c, G, h, A=None, b=None):
         c = np.ascontiguousarray(np.asarray(c, dtype=np.float64))
@@ -313,24 +315,17 @@ class ConeLPBatch(QPBatch):
         B, n, m = self.B, self.n, self.m
         if c.shape != (B, n) or G.shape != (B, m, n) or h.shape != (B, m):
             raise TypeError("problem shapes do not match the batch")
-        Acm, bv, p = _stack_eq(A, b, B, n)
-        if p != self.p:
-            raise TypeError("A has %d rows; the batch was created with p = %d" % (p, self.p))
+        Acm, bv = self._host_eq(A, b)
         Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
         _lib.check(self._lib.cvxb_batch_load_lp(self._h, c.ctypes.data, Gcm.ctypes.data, h.ctypes.data, _lib.HOST),
                    "batch_load_lp")
-        if p:
-            _lib.check(self._lib.cvxb_batch_load_eq(self._h, Acm.ctypes.data, bv.ctypes.data, _lib.HOST),
-                       "batch_load_eq")
+        self._load_eq(Acm, bv, _lib.HOST)
 
     def load_ptr(self, c, G, h, space=_lib.DEVICE, A=None, b=None):
         """raw addresses of already laid-out buffers: c (B, n), G m x n column-major per problem, h (B, m), A p x n
         column-major per problem, b (B, p)"""
         _lib.check(self._lib.cvxb_batch_load_lp(self._h, c, G, h, space), "batch_load_lp")
-        if self.p:
-            if A is None or b is None:
-                raise TypeError("the batch has p = %d equality rows: give A and b" % self.p)
-            _lib.check(self._lib.cvxb_batch_load_eq(self._h, A, b, space), "batch_load_eq")
+        self._load_eq(A, b, space)
 
 
 class ConeLPBatchGroup(QPBatchGroup):
@@ -379,9 +374,13 @@ def conelp_batch(c, G, h, dims=None, A=None, b=None, device=0, nsub=None, **opti
     'primal infeasible', 'dual infeasible' or 'unknown', and entries the reference returns as None are NaN.
     options: maxiters, abstol, reltol, feastol, refinement (as conelp's)."""
     B, n, cdim, p = _lp_shapes(c, G, h, dims, A, b)
-    grp = ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p)
+    return _run_group(ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p), (c, G, h, A, b), options)
+
+
+def _run_group(grp, data, options):
+    """load `data` into the batch group, solve it timed, and return its results and stats; the group is closed"""
     try:
-        grp.load(c, G, h, A, b)
+        grp.load(*data)
         import time
         t0 = time.perf_counter()
         grp.solve(**options)
@@ -407,19 +406,7 @@ def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, **optio
         raise TypeError("P must have shape (B, n, n) and G (B, cdim, n)")
     _, _, cdim = _batch_dims(dims, G.shape[1])
     p = _eq_rows(A, b, P.shape[0], P.shape[1])
-    grp = QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims, p)
-    try:
-        grp.load(P, q, G, h, A, b)
-        import time
-        t0 = time.perf_counter()
-        grp.solve(**options)
-        wall = (time.perf_counter() - t0) * 1e3
-        out = grp.results()
-        out.update(grp.stats())
-        out["solve_wall_ms"] = wall
-        return out
-    finally:
-        grp.close()
+    return _run_group(QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims, p), (P, q, G, h, A, b), options)
 
 
 # ---------------------------------------------------------------------------------------

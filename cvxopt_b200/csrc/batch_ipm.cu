@@ -13,8 +13,9 @@
 // With p > 0 equality rows the reduced system is solved by kkt_chol2's elimination (misc.py:1352-1560): S = P + Gs'Gs
 // (+ A'A for a problem whose S was singular at the start), S = L L', Asct = L^{-1} A', Kp = Asct'Asct = Lp Lp'.
 // Nothing leaves the device between iterations except one int ("how many are done").
-// A cone LP batch (no P: minimize c'x over the same constraints) runs coneprog.conelp (coneprog.py:31-1436) instead, in
-// solve_conelp: the same factorisations and solves with the self-dual embedding's tau / kappa arithmetic around them.
+// A cone LP batch (no P: minimize c'x over the same constraints) runs coneprog.conelp (coneprog.py:31-1436) instead,
+// through the same loop, solve<CONES, EQ, LP> with LP = true: the same factorisations, solves and refinement with the
+// self-dual embedding's tau / kappa arithmetic around them.
 #include "cone.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -213,12 +214,13 @@ template <bool CONES> __global__ void k_init_point(Ptrs p) {
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
-// rx = q  (then rx += P x by GEMV); EQ: ry = b (then ry := A x - ry)
-template <bool EQ> __global__ void k_res_begin(Ptrs p) {
+// residuals, part 1: rx = q (then rx += P x by GEMV), rz = s - h; EQ: ry = b (then ry := A x - ry).
+// LP: rx = 0, rz = s, ry = 0; the GEMVs then make them conelp's hrx = -A'y - G'z, hrz = s + G x, hry = A x (:861-896)
+template <bool EQ, bool LP> __global__ void k_res_begin(Ptrs p) {
     PB_SETUP
-    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = p.q[on + i];
-    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i] - p.h[om + i];      // :2183-2184
-    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = p.beq[oq + i];         // :2177-2178
+    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = LP ? 0.0 : p.q[on + i];
+    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = LP ? p.s[om + i] : p.s[om + i] - p.h[om + i];   // :2183-2184
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = LP ? 0.0 : p.beq[oq + i];           // :2177-2178
 }
 // f0 pieces once rx = P x + q   (:2172)
 __global__ void k_res_dots(Ptrs p) {
@@ -430,12 +432,18 @@ __device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double
 
 // right-hand side of the i-th Newton system (coneprog.py:2373-2399), a copy of it for the refinement (:2331-2335),
 // then f4_no_ir's steps before the solve.  Cone rows are formed row-wise over the CTA; after a barrier the warp that
-// owns a cone adds sigma mu to its entry 0 and runs the cone part.  EQ: dy = c ry (:2395-2397)
-template <bool CONES, bool EQ> __global__ void k_dir_rhs(Ptrs p, int i) {
+// owns a cone adds sigma mu to its entry 0 and runs the cone part.  EQ: dy = c ry (:2395-2397).
+// LP: conelp's right-hand side (:1268-1298) and its refinement copy (:1212-1218), as f6_no_ir leaves them for the
+// solve (:1154-1165): y := -y, and f4_no_ir's cone steps on (-bz, -bs).  That is coneqp's right-hand side with
+// c = -1 + sigma and sigma mu in the corrector (i = 1) only; dx = -c rx keeps conelp's sign.  Negation is exact, so this
+// is the reference's arithmetic.  Then dtau = (1 - sigma) rt and dkappa.
+template <bool CONES, bool EQ, bool LP> __global__ void k_dir_rhs(Ptrs p, int i) {
     PB_SETUP
-    const double sm = S.sigma * S.mu, c = -1.0 + S.eta;
+    const double sm = S.sigma * S.mu, c = -1.0 + (LP ? S.sigma : S.eta);
+    const bool add_sm = !LP || i == 1;
+    LPScal &T = lp_scal(p, oc);                          // LP only
     for (int k = tid; k < p.n; k += nt) {
-        const double dx = c * p.rx[on + k];
+        const double dx = (LP ? -c : c) * p.rx[on + k];
         p.dx[on + k] = dx;
         if (p.refinement) p.wx[oc + k] = dx;
     }
@@ -444,11 +452,12 @@ template <bool CONES, bool EQ> __global__ void k_dir_rhs(Ptrs p, int i) {
         p.dy[oq + k] = dy;
         if (p.refinement) p.wy[oc + k] = dy;
     }
-    // row r: z = c rz, s = -ws3 (the Mehrotra correction, i = 1) - lmbda o lmbda (+ sigma mu where e is 1)
+    // row r: z = c rz, s = -ws3 (the Mehrotra correction, i = 1) - lmbda o lmbda (+ sigma mu where e is 1).  LP starts
+    // from -0.0 so that s is conelp's -lmbdasq down to the sign of a zero
     auto rhs = [&](int r, bool e, double &z, double &s) {
-        s = (i == 1) ? -p.ws3[om + r] : 0.0;
+        s = (i == 1) ? -p.ws3[om + r] : (LP ? -0.0 : 0.0);
         s -= p.lmbdasq[om + r];
-        if (e) s += sm;
+        if (e && add_sm) s += sm;
         z = c * p.rz[om + r];
         if (p.refinement) { p.wz[oc + r] = z; p.ws[oc + r] = s; }
     };
@@ -467,10 +476,15 @@ template <bool CONES, bool EQ> __global__ void k_dir_rhs(Ptrs p, int i) {
         }
         __syncthreads();
         FOR_CONES(o, len) {
-            if (lane == 0) { p.ds[om + o] += sm; if (p.refinement) p.ws[oc + o] += sm; }
+            if (lane == 0 && add_sm) { p.ds[om + o] += sm; if (p.refinement) p.ws[oc + o] += sm; }
             __syncwarp();
             f4_pre_cone(p, om, oc, k_, o, len, lane, p.dz + om, p.ds + om);
         }
+    }
+    if (LP && tid == 0) {
+        T.dtau = -c * T.rt;
+        T.dkappa = (i == 1) ? T.lgsq + (T.wkappa3 - sm) : T.lgsq;
+        if (p.refinement) { T.wtau = T.dtau; T.wkappa = T.dkappa; }
     }
 }
 // f4_no_ir before the solve of a refinement step, on slot b's z and s at z + b*sz, s + b*ss
@@ -501,16 +515,34 @@ __global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long 
 }
 // refinement residual, the elementwise part of res() (coneprog.py:1930-1960): wx2 = wx, wz3 = W^{-1} dz,
 // wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds); EQ: wy2 = wy.  The P, A, A', G and G' products follow as
-// batched GEMVs.
-template <bool EQ> __global__ void k_res(Ptrs p) {
+// batched GEMVs.  LP: conelp's res() (:599-631) adds the embedding's column ut (-c, b, h), ut = dtau / dg, to
+// (wx2, wy2, wz2), and forms wtau2 = wtau + dg dkappa + c'dx + b'dy + h'wz3, wkappa2 = wkappa + lmbdag (dtau + dkappa).
+template <bool EQ, bool LP> __global__ void k_res(Ptrs p) {
     PB_SETUP
-    const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om;
-    for (int i = tid; i < p.n; i += nt) p.wx2[oc + i] = p.wx[oc + i];
-    if (EQ) for (int i = tid; i < p.neq; i += nt) p.wy2[oc + i] = p.wy[oc + i];
+    const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om, *h = p.h + om;
+    const double ut = LP ? lp_scal(p, oc).dtau / lp_scal(p, oc).dg : 0.0;
+    double cx = 0, by = 0, hz = 0;
+    for (int i = tid; i < p.n; i += nt) {
+        if (LP) {
+            const double c = p.q[on + i];
+            p.wx2[oc + i] = p.wx[oc + i] + (-ut) * c;
+            cx += c * p.dx[on + i];
+        } else p.wx2[oc + i] = p.wx[oc + i];
+    }
+    if (EQ) for (int i = tid; i < p.neq; i += nt) {
+        if (LP) {
+            const double bb = p.beq[oq + i];
+            p.wy2[oc + i] = p.wy[oc + i] + ut * bb;
+            by += bb * p.dy[oq + i];
+        } else p.wy2[oc + i] = p.wy[oc + i];
+    }
     double *wz3 = p.wz3 + oc, *wz2 = p.wz2 + oc, *ws2 = p.ws2 + oc;
     for (int i = tid; i < p.ml; i += nt) {
-        wz3[i] = p.di[om + i] * dz[i];
-        wz2[i] = p.wz[oc + i] - p.d[om + i] * ds[i];
+        const double w3 = p.di[om + i] * dz[i];
+        wz3[i] = w3;
+        double w = p.wz[oc + i];
+        if (LP) { hz += h[i] * w3; w += ut * h[i]; }
+        wz2[i] = w - p.d[om + i] * ds[i];
         ws2[i] = p.ws[oc + i] - l[i] * (dz[i] + ds[i]);
     }
     const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
@@ -522,8 +554,19 @@ template <bool EQ> __global__ void k_res(Ptrs p) {
         a = warp_sum(a);
         const double u0 = ds[o] + dz[o], l0 = l[o];
         FOR_LANE(i, len) {
-            wz2[o + i] = p.wz[oc + o + i] - wz2[o + i];
+            double w = p.wz[oc + o + i];
+            if (LP) { hz += h[o + i] * wz3[o + i]; w += ut * h[o + i]; }
+            wz2[o + i] = w - wz2[o + i];
             ws2[o + i] = p.ws[oc + o + i] - ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]);
+        }
+    }
+    if (LP) {
+        cx = block_sum(cx, sh); hz = block_sum(hz, sh);
+        if (EQ) by = block_sum(by, sh);
+        if (tid == 0) {
+            LPScal &T = lp_scal(p, oc);
+            T.wtau2 = T.wtau + (T.dg * T.dkappa + cx + by + hz);
+            T.wkappa2 = T.wkappa + T.lg * (T.dtau + T.dkappa);
         }
     }
 }
@@ -693,7 +736,8 @@ __global__ void k_switch(double *aw, const int *info, int neq) {
 
 // ---- cone LPs: coneprog.conelp (coneprog.py:31-1436) ----
 // The kernels below are the arithmetic in which conelp's homogeneous self-dual embedding differs from coneqp; the
-// scaling, the factorisation, the KKT solves, f4_no_ir's cone steps, the step length and the update are coneqp's.
+// scaling, the factorisation, the KKT solves, f4_no_ir's cone steps, the right-hand side, the refinement residual, the
+// step length and the update are coneqp's kernels with LP = true.
 // The primal start's solve has left uz in bzp: s = -uz (:698-701).  The dual start's right-hand side (-c, 0, 0):
 // k_init_rhs put -c in dx, here y = 0 and bz = 0 (:724-728)
 template <bool EQ> __global__ void k_lp_start_mid(Ptrs p) {
@@ -747,13 +791,6 @@ template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double ab
         LPScal &T = lp_scal(p, oc);
         T.tau = 1.0; T.kappa = 1.0;
     }
-}
-// residuals, part 1: rx = 0, rz = s, ry = 0; the GEMVs then make them hrx = -A'y - G'z, hrz = s + G x, hry = A x
-template <bool EQ> __global__ void k_lp_res_begin(Ptrs p) {
-    PB_SETUP
-    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = 0.0;
-    for (int i = tid; i < p.m; i += nt) p.rz[om + i] = p.s[om + i];
-    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = 0.0;
 }
 // residuals, part 2, and the stopping rule (:864-1023): rx = hrx - c tau, ry = hry - b tau, rz = hrz - h tau, rt;
 // optimal or maxiters divide the iterate by tau; a primal infeasibility certificate divides y and z by -h'z - b'y
@@ -851,57 +888,6 @@ template <bool EQ> __global__ void k_lp_x1_post(Ptrs p) {
     a = block_sum(a, sh);
     if (tid == 0) lp_scal(p, oc).z1sq = a;
 }
-// right-hand side of the i-th Newton system (:1268-1298), the refinement's copy of it (:1212-1218), then f6_no_ir's
-// steps before the solve (:1154-1165): y := -y, and f4_no_ir's cone steps on (-bz, -bs) are s := -lmbda o\ bs,
-// z := -(bz + W's) with bzp = W^{-T} z.  Negation is exact, so this is the reference's arithmetic.
-template <bool CONES, bool EQ> __global__ void k_lp_dir_rhs(Ptrs p, int i) {
-    PB_SETUP
-    LPScal &T = lp_scal(p, oc);
-    const double sm = S.sigma * S.mu, c = 1.0 - S.sigma;
-    for (int k = tid; k < p.n; k += nt) {
-        const double dx = c * p.rx[on + k];
-        p.dx[on + k] = dx;
-        if (p.refinement) p.wx[oc + k] = dx;
-    }
-    if (EQ) for (int k = tid; k < p.neq; k += nt) {
-        const double dy = c * p.ry[oq + k];
-        p.dy[oq + k] = -dy;
-        if (p.refinement) p.wy[oc + k] = dy;
-    }
-    // row r: bs = lmbdasq (+ ws3 - sigma mu where e is 1, i = 1), bz = (1 - sigma) rz; returns -bz, -bs
-    auto rhs = [&](int r, bool e, double &z, double &s) {
-        s = p.lmbdasq[om + r];
-        if (i == 1) { s += p.ws3[om + r]; if (e) s -= sm; }
-        z = c * p.rz[om + r];
-        if (p.refinement) { p.wz[oc + r] = z; p.ws[oc + r] = s; }
-        z = -z; s = -s;
-    };
-#pragma unroll 1
-    for (int k = tid; k < p.ml; k += nt) {
-        double z, s;
-        rhs(k, true, z, s);
-        f4_pre_row(p, om + k, z, s);
-        p.dz[om + k] = z; p.ds[om + k] = s;
-    }
-    if (CONES) {
-        for (int k = p.ml + tid; k < p.m; k += nt) {
-            double z, s;
-            rhs(k, false, z, s);
-            p.dz[om + k] = z; p.ds[om + k] = s;
-        }
-        __syncthreads();
-        FOR_CONES(o, len) {
-            if (lane == 0 && i == 1) { p.ds[om + o] += sm; if (p.refinement) p.ws[oc + o] -= sm; }
-            __syncwarp();
-            f4_pre_cone(p, om, oc, k_, o, len, lane, p.dz + om, p.ds + om);
-        }
-    }
-    if (tid == 0) {
-        T.dtau = c * T.rt;
-        T.dkappa = (i == 1) ? T.lgsq + (T.wkappa3 - sm) : T.lgsq;
-        if (p.refinement) { T.wtau = T.dtau; T.wkappa = T.dkappa; }
-    }
-}
 // f6_no_ir after the solve (:1180-1195): with the solve's (x, y) and uz in bzp, kappa := -bkappa / lmbdag,
 // tau := dgi (btau - bkappa / tau + c'x + b'y + th'uz) / (1 + z1'z1), (x, y, z) += tau (x1, y1, z1), s := s - z,
 // kappa -= tau.  acc = 0: the Newton solve, in place on (dx, dy, ds), z to dz, (btau, bkappa) = (dtau, dkappa).
@@ -942,57 +928,6 @@ template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx,
         else { T.dtau = tau; T.dkappa = kap; }
     }
 }
-// refinement residual, the elementwise part of conelp's res() (:599-631) on the copies of the right-hand side:
-// wx2 = wx - c dtau/dg, wz3 = W^{-1} dz, wtau2 = wtau + dg dkappa + c'dx + b'dy + h'wz3, wkappa2 = wkappa +
-// lmbdag (dtau + dkappa), and, negated for the following f6_no_ir (y := -y, f4_no_ir on (-bz, -bs)):
-// wy2 = -(wy - b dtau/dg), wz2 = -(wz - h dtau/dg + W'ds), ws2 = -(ws + lmbda o (dz + ds)).  The A, A', G and G'
-// products follow as batched GEMVs.
-template <bool EQ> __global__ void k_lp_res(Ptrs p) {
-    PB_SETUP
-    LPScal &T = lp_scal(p, oc);
-    const double ut = T.dtau / T.dg;
-    const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om, *h = p.h + om;
-    double cx = 0, by = 0, hz = 0;
-    for (int i = tid; i < p.n; i += nt) {
-        const double c = p.q[on + i];
-        p.wx2[oc + i] = p.wx[oc + i] + (-ut) * c;
-        cx += c * p.dx[on + i];
-    }
-    if (EQ) for (int i = tid; i < p.neq; i += nt) {
-        const double bb = p.beq[oq + i];
-        p.wy2[oc + i] = -(p.wy[oc + i] + (-ut) * bb);
-        by += bb * p.dy[oq + i];
-    }
-    double *wz3 = p.wz3 + oc, *wz2 = p.wz2 + oc, *ws2 = p.ws2 + oc;
-    for (int i = tid; i < p.ml; i += nt) {
-        const double w3 = p.di[om + i] * dz[i];
-        wz3[i] = w3;
-        hz += h[i] * w3;
-        wz2[i] = -((p.wz[oc + i] + (-ut) * h[i]) + p.d[om + i] * ds[i]);
-        ws2[i] = -(p.ws[oc + i] + l[i] * (dz[i] + ds[i]));
-    }
-    const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
-    FOR_CONES(o, len) {
-        q_scale(v + o, beta[k_], dz + o, wz3 + o, len, lane, true);
-        q_scale(v + o, beta[k_], ds + o, wz2 + o, len, lane, false);
-        double a = 0;
-        FOR_LANE(i, len) a += l[o + i] * (ds[o + i] + dz[o + i]);
-        a = warp_sum(a);
-        const double u0 = ds[o] + dz[o], l0 = l[o];
-        FOR_LANE(i, len) {
-            hz += h[o + i] * wz3[o + i];
-            wz2[o + i] = -((p.wz[oc + o + i] + (-ut) * h[o + i]) + wz2[o + i]);
-            ws2[o + i] = -(p.ws[oc + o + i] + ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]));
-        }
-    }
-    cx = block_sum(cx, sh); hz = block_sum(hz, sh);
-    if (EQ) by = block_sum(by, sh);
-    if (tid == 0) {
-        T.wtau2 = T.wtau + (T.dg * T.dkappa + cx + by + hz);
-        T.wkappa2 = T.wkappa + T.lg * (T.dtau + T.dkappa);
-    }
-}
-
 }  // namespace
 
 struct cvxb_batch {
@@ -1183,21 +1118,26 @@ int batch_solve(cvxb_batch *b, double *x, long long sx, double *y = nullptr, lon
     return 0;
 }
 
-// the i-th Newton direction: f4 (coneprog.py:2288-2347) on the right-hand side, i.e. f4_no_ir and then `refinement`
-// correction steps from the residual, followed by the step length and sigma
-template <bool CONES, bool EQ> int direction(cvxb_batch *b, int i) {
+// the i-th Newton direction: coneqp's f4 (coneprog.py:2288-2347) or, LP, conelp's f6 (:1211-1235) on the right-hand
+// side, i.e. the unrefined solve and then `refinement` correction steps from the residual, followed by the step
+// length and sigma
+template <bool CONES, bool EQ, bool LP> int direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
     const long long L = b->L;
-    k_dir_rhs<CONES, EQ><<<B, T, 0, st>>>(p, i); count_launch();
+    k_dir_rhs<CONES, EQ, LP><<<B, T, 0, st>>>(p, i); count_launch();
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
-    if (p.refinement) { k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
+    if (LP) { k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch(); }
+    else if (p.refinement) { k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
     for (int r = 0; r < p.refinement; ++r) {
-        // res() (coneprog.py:1930-1952): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx, wz2 -= G dx + W' ds
-        k_res<EQ><<<B, T, 0, st>>>(p); count_launch();
-        GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
-        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
+        // res() (coneprog.py:1930-1952, :599-631): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx,
+        // wz2 -= G dx + W' ds; an LP has no P
+        k_res<EQ, LP><<<B, T, 0, st>>>(p); count_launch();
+        if (!LP) {
+            GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
+            CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
+        }
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
             CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
@@ -1212,9 +1152,11 @@ template <bool CONES, bool EQ> int direction(cvxb_batch *b, int i) {
         CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
         k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
-        k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1); count_launch();
+        if (LP) k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1);
+        else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
+        count_launch();
     }
-    k_dir_post<CONES><<<B, T, 0, st>>>(p, i, p.refinement == 0); count_launch();
+    k_dir_post<CONES, LP><<<B, T, 0, st>>>(p, i, !LP && p.refinement == 0); count_launch();
     return 0;
 }
 
@@ -1314,9 +1256,11 @@ int compact_slots(cvxb_batch *b, int B, int ndone, const std::vector<int> &flags
     return 0;
 }
 
-// the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows
-template <bool CONES, bool EQ>
-int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+// the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows.  LP: coneprog.conelp
+// (coneprog.py:662-1436) on a batch without P: the self-dual embedding's tau and kappa, one more KKT solve per
+// iteration for (x1, y1, z1), and infeasibility certificates
+template <bool CONES, bool EQ, bool LP>
+int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
     int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
@@ -1330,31 +1274,44 @@ int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, do
     GemvBatch gAn; gAn.batch = B; gAn.sA = b->sA; gAn.sx = n; gAn.sy = pq;
     CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
     CVXB_CUDA(cudaEventRecord(b->e0, st));
-    // ---- starting point: W = I ----
-    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
+    // ---- starting point: W = I (coneqp :2055-2106, conelp :662-857) ----
+    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();       // dx = -q, y = b, dz = h, resx0 / resy0 / resz0
     CVXB_TRY(start_factor<EQ>(b));
     k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
-    k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
+    if (LP) {
+        CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
+        CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));            // primal start: (0, b, h)
+        k_lp_start_mid<EQ><<<B, T, 0, st>>>(p); count_launch();
+        CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));           // dual start: (-c, 0, 0)
+        k_lp_init_point<CONES, EQ><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
+    } else {
+        CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
+        k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
+    }
     CVXB_LAUNCH_CHECK();
     CVXB_TRY(start_check<EQ>(b));
+    // residual GEMV signs: coneqp's rx = P x + q + A'y + G'z, ry = A x - b; conelp's hrx = -A'y - G'z, hry = A x
+    const double sgn = LP ? -1.0 : 1.0;
     std::vector<int> flags(B), pairs;
     int it = 0;
     for (it = 0; it <= maxiters; ++it) {
-        // residuals (:2169-2186)
-        k_res_begin<EQ><<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
-        k_res_dots<<<B, T, 0, st>>>(p); count_launch();
+        // residuals (coneqp :2169-2186, conelp :861-896)
+        k_res_begin<EQ, LP><<<B, T, 0, st>>>(p); count_launch();
+        if (!LP) {
+            CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.x, 1.0, 1.0, p.rx, st, gP));
+            k_res_dots<<<B, T, 0, st>>>(p); count_launch();
+        }
         if (EQ) {
-            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, 1.0, 1.0, p.rx, st, gAt));                  // rx += A'y
-            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, gAn));   // ry = Ax - b
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, sgn, 1.0, p.rx, st, gAt));
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -sgn, p.ry, b->gemv_ws.p, st, gAn));
         }
         if (m > 0) {
-            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, 1.0, 1.0, p.rx, st, gGt));
+            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, sgn, 1.0, p.rx, st, gGt));
             CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        if (LP) k_lp_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        else k_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
         int ndone = 0;
         CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1366,115 +1323,16 @@ int solve_lockstep(cvxb_batch *b, int maxiters, double abstol, double reltol, do
             B = b->Bact;
             gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
         }
-        k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
+        k_scaling<CONES, LP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         CVXB_TRY(batch_factor(b));
-        for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ>(b, i)));
-        k_update<CONES, EQ><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
-        CVXB_LAUNCH_CHECK();
-    }
-    b->iters_run = it;
-    b->Bact = b->B;
-    CVXB_CUDA(cudaEventRecord(b->e1, st));
-    CVXB_CUDA(cudaStreamSynchronize(st));
-    float t = 0;
-    cudaEventElapsedTime(&t, b->e0, b->e1);
-    b->solve_ms = t;
-    return 0;
-}
-
-// conelp's i-th Newton direction: f6 (coneprog.py:1211-1235), i.e. f6_no_ir and then `refinement` correction steps
-// from res(), followed by the step length and sigma
-template <bool CONES, bool EQ> int direction_lp(cvxb_batch *b, int i) {
-    cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
-    const Ptrs &p = b->p;
-    const long long L = b->L;
-    k_lp_dir_rhs<CONES, EQ><<<B, T, 0, st>>>(p, i); count_launch();
-    CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
-    k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch();
-    for (int r = 0; r < p.refinement; ++r) {
-        // res() (:599-631): wx2 -= A' dy + G' W^{-1} dz, -wy2 += A dx, -wz2 += G dx
-        k_lp_res<EQ><<<B, T, 0, st>>>(p); count_launch();
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
-            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
+        if (LP) {
+            // (x1, y1, z1) from (-c, b, h) (:1066-1077), th = W^{-T} h
+            k_lp_x1_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
+            CVXB_TRY(batch_solve(b, p.x1, n, p.y1, pq));
+            k_lp_x1_post<EQ><<<B, T, 0, st>>>(p); count_launch();
         }
-        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
-            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
-        }
-        GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
-        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
-        k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
-        CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
-        k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1); count_launch();
-    }
-    k_dir_post<CONES, true><<<B, T, 0, st>>>(p, i, 0); count_launch();
-    return 0;
-}
-
-// the lock-step conelp over the active slots (coneprog.py:662-1436): the same factorisations, solves, scaling and
-// compaction as solve_lockstep, on a batch without P, with the self-dual embedding's tau and kappa, one more KKT
-// solve per iteration for (x1, y1, z1), and infeasibility certificates
-template <bool CONES, bool EQ>
-int solve_conelp(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
-    cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, T = 256, pq = b->neq;
-    int B = b->B;
-    b->Bact = B;
-    b->switched = false;
-    const Ptrs &p = b->p;
-    GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
-    GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
-    GemvBatch gAt; gAt.batch = B; gAt.sA = b->sA; gAt.sx = pq; gAt.sy = n;
-    GemvBatch gAn; gAn.batch = B; gAn.sA = b->sA; gAn.sx = n; gAn.sy = pq;
-    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
-    CVXB_CUDA(cudaEventRecord(b->e0, st));
-    // ---- starting point: W = I (:662-857) ----
-    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();       // dx = -c, y = b, dz = h, resx0 / resy0 / resz0
-    CVXB_TRY(start_factor<EQ>(b));
-    k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
-    CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
-    CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));                // primal start: (0, b, h)
-    k_lp_start_mid<EQ><<<B, T, 0, st>>>(p); count_launch();
-    CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));               // dual start: (-c, 0, 0)
-    k_lp_init_point<CONES, EQ><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
-    CVXB_LAUNCH_CHECK();
-    CVXB_TRY(start_check<EQ>(b));
-    std::vector<int> flags(B), pairs;
-    int it = 0;
-    for (it = 0; it <= maxiters; ++it) {
-        // residuals (:861-896)
-        k_lp_res_begin<EQ><<<B, T, 0, st>>>(p); count_launch();
-        if (EQ) {
-            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, -1.0, 1.0, p.rx, st, gAt));                // -A'y
-            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, 1.0, p.ry, b->gemv_ws.p, st, gAn));   // A x
-        }
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, -1.0, 1.0, p.rx, st, gGt));
-        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
-        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_lp_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
-        count_launch();
-        int ndone = 0;
-        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
-        if (ndone >= B) break;
-        if (ndone > 0 && b->compact && b->B > 1) {
-            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
-            B = b->Bact;
-            gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
-        }
-        k_scaling<CONES, true><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
-        CVXB_TRY(batch_factor(b));
-        // (x1, y1, z1) from (-c, b, h) (:1066-1077), th = W^{-T} h
-        k_lp_x1_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(batch_solve(b, p.x1, n, p.y1, pq));
-        k_lp_x1_post<EQ><<<B, T, 0, st>>>(p); count_launch();
-        for (int i = 0; i < 2; ++i) CVXB_TRY((direction_lp<CONES, EQ>(b, i)));
-        k_update<CONES, EQ, true><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
+        for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ, LP>(b, i)));
+        k_update<CONES, EQ, LP><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -1504,15 +1362,42 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
     return 0;
 }
 
-// a batch of QPs, or of cone LPs (lp: no P)
-int create_batch(cvxb_batch **out, int nprob, int n, int m, int device, bool lp) {
-    if (!out || nprob <= 0 || n <= 0 || m < 0) { set_error("batch_create: bad sizes"); return CVXB_E_ARG; }
+// a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q') and p equality rows.
+// Every argument is checked before the device is.
+int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp) {
+    if (out) *out = nullptr;
+    if (!out || nprob <= 0 || n <= 0 || !dims) {
+        set_error("batch_create: bad sizes (nprob and n positive, dims given)");
+        return CVXB_E_ARG;
+    }
+    if (p < 0) { set_error("batch_create: bad sizes (p must be nonnegative)"); return CVXB_E_ARG; }
     if (nprob > CVXB_BATCH_MAX) {
         set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
         return CVXB_E_ARG;
     }
-    *out = nullptr;
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("batch_create: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
+        return CVXB_E_ARG;
+    }
+    long long mm = dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("batch_create: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
+        mm += dims->q[k];
+    }
+    if (mm > (1LL << 30)) { set_error("batch_create: too many cone rows"); return CVXB_E_ARG; }
+    if (dims->ns > 0) { set_error("batch_create: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    if (lp && mm == 0) {                          // deliberate: every cone LP needs at least one cone row
+        set_error("batch_create_lp: the batch needs at least one 'l' or 'q' row (m = 0)");
+        return CVXB_E_ARG;
+    }
+    // the checks before the first factorisation: coneqp's (coneprog.py:1962), conelp's (:572-573)
+    if (p > n || (lp && p + mm < n)) {
+        set_error("batch_create: Rank(A) < p or Rank([%s]) < n (p = %d, n = %d, cdim = %lld)", lp ? "G; A" : "P; A; G",
+                  p, n, mm);
+        return CVXB_E_ARG;
+    }
     CVXB_TRY(check_device(device));
+    const int m = (int)mm;
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
     b->device = device; b->B = nprob; b->n = n; b->m = m; b->lp = lp;
     b->i8_mode = ozaki_mode();
@@ -1530,24 +1415,27 @@ int create_batch(cvxb_batch **out, int nprob, int n, int m, int device, bool lp)
     CVXB_TRY(b->K.alloc(B * b->sK));
     CVXB_TRY(b->inv.alloc(B * b->sInv));
     CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
-    CVXB_TRY(b->gemv_ws.alloc(B * (size_t)(m > 0 ? m : 1) * gemv_n_chunks(n)));
+    // GEMV workspace: G x (m rows); with equality rows also A x (p rows) and Asct y (n rows)
+    const size_t me = (size_t)(m > 0 ? m : 1);
+    size_t ws = me * gemv_n_chunks(n);
+    if (p > 0) ws = std::max({ws, (size_t)p * gemv_n_chunks(n), (size_t)n * gemv_n_chunks(p)});
+    CVXB_TRY(b->gemv_ws.alloc(B * ws));
     // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
     const size_t nv = 4, mv = 13;
-    const size_t me = (size_t)(m > 0 ? m : 1);
     CVXB_TRY(b->vecs.alloc(B * (nv * n + mv * me)));
     CVXB_CUDA(cudaMemset(b->vecs.p, 0, B * (nv * n + mv * me) * sizeof(double)));
     double *v = b->vecs.p;
     auto take = [&](size_t len) { double *r = v; v += B * len; return r; };
-    Ptrs &p = b->p;
-    p = Ptrs{};
-    b->q = take(n); p.x = take(n); p.rx = take(n); p.dx = take(n);
-    b->h = take(me); p.s = take(me); p.z = take(me); p.rz = take(me); p.ds = take(me);
-    p.dz = take(me); p.lmbda = take(me); p.lmbdasq = take(me); p.d = take(me);
-    p.di = take(me); p.di2 = take(me); p.ws3 = take(me); p.bzp = take(me);
-    p.q = b->q; p.h = b->h; p.n = n; p.m = m; p.ml = m;
+    Ptrs &q = b->p;
+    q = Ptrs{};
+    b->q = take(n); q.x = take(n); q.rx = take(n); q.dx = take(n);
+    b->h = take(me); q.s = take(me); q.z = take(me); q.rz = take(me); q.ds = take(me);
+    q.dz = take(me); q.lmbda = take(me); q.lmbdasq = take(me); q.d = take(me);
+    q.di = take(me); q.di2 = take(me); q.ws3 = take(me); q.bzp = take(me);
+    q.q = b->q; q.h = b->h; q.n = n; q.m = m; q.ml = dims->ml;
     CVXB_TRY(b->sc.alloc(B));
     CVXB_CUDA(cudaMemset(b->sc.p, 0, B * sizeof(Scal)));
-    p.sc = b->sc.p;
+    q.sc = b->sc.p;
     CVXB_TRY(b->d_info.alloc(B));
     CVXB_TRY(b->d_ndone.alloc(1));
     CVXB_TRY(b->d_done.alloc(B));
@@ -1556,59 +1444,17 @@ int create_batch(cvxb_batch **out, int nprob, int n, int m, int device, bool lp)
     b->perm.resize(B);
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
-    *out = b.release();
-    return 0;
-}
-
-int create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device, bool lp) {
-    if (!out || nprob <= 0 || n <= 0 || !dims) { set_error("batch_create_cones: bad sizes"); return CVXB_E_ARG; }
-    if (nprob > CVXB_BATCH_MAX) {
-        set_error("batch_create_cones: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob,
-                  CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    *out = nullptr;
-    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("batch_create_cones: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
-        return CVXB_E_ARG;
-    }
-    long long m = dims->ml;
-    for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("batch_create_cones: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
-        m += dims->q[k];
-    }
-    if (m > (1LL << 30)) { set_error("batch_create_cones: too many cone rows"); return CVXB_E_ARG; }
-    if (dims->ns > 0) { set_error("batch_create_cones: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
-    cvxb_batch *b = nullptr;
-    CVXB_TRY(create_batch(&b, nprob, n, (int)m, device, lp));
-    std::unique_ptr<cvxb_batch> own(b);
     if (dims->nq > 0) {
         const int nq = dims->nq;
         std::vector<int> off(nq + 1, dims->ml);
         for (int k = 0; k < nq; ++k) off[k + 1] = off[k] + dims->q[k];
         CVXB_TRY(b->qoff.alloc(nq + 1));
         CVXB_CUDA(cudaMemcpy(b->qoff.p, off.data(), (nq + 1) * sizeof(int), cudaMemcpyHostToDevice));
-        CVXB_TRY(b->Gs.alloc((size_t)b->B * b->sG));
-        b->p.ml = dims->ml; b->p.nq = nq; b->p.qoff = b->qoff.p;
-        b->p.refinement = 1;                      // coneqp's default with 'q' cones (coneprog.py:1862-1865)
-        CVXB_TRY(state_alloc(b));
+        CVXB_TRY(b->Gs.alloc(B * b->sG));
+        q.nq = nq; q.qoff = b->qoff.p;
+        q.refinement = 1;                         // the default with 'q' cones (coneprog.py:1862-1865)
     }
-    *out = own.release();
-    return 0;
-}
-
-int create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp) {
-    if (out) *out = nullptr;
-    if (!out || p < 0) { set_error("batch_create_eq: bad sizes (p must be nonnegative)"); return CVXB_E_ARG; }
-    if (n > 0 && p > n) {                         // coneqp's check before the first factorisation (coneprog.py:1962)
-        set_error("batch_create_eq: Rank(A) < p or Rank([P; A; G]) < n (p = %d > n = %d)", p, n);
-        return CVXB_E_ARG;
-    }
-    cvxb_batch *b = nullptr;
-    CVXB_TRY(create_cones(&b, nprob, n, dims, device, lp));     // sizes and dims are checked before the device
-    std::unique_ptr<cvxb_batch> own(b);
     if (p > 0) {
-        const size_t B = b->B;
         b->neq = p;
         b->lda = b->ldkp = ((p + 1) & ~1) > 2 ? ((p + 1) & ~1) : 2;
         b->ldas = b->ldk;
@@ -1623,18 +1469,37 @@ int create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, 
         CVXB_CUDA(cudaMemset(b->pvecs.p, 0, B * NPV * p * sizeof(double)));
         CVXB_TRY(b->d_infop.alloc(B));
         CVXB_CUDA(cudaMemset(b->d_infop.p, 0, B * sizeof(int)));
-        // GEMV workspace: A x (p rows), Asct y (n rows) besides the G x of create
-        const size_t me = b->m > 0 ? b->m : 1;
-        const size_t ws = std::max({me * gemv_n_chunks(n), (size_t)p * gemv_n_chunks(n), (size_t)n * gemv_n_chunks(p)});
-        if (B * ws > b->gemv_ws.n) { b->gemv_ws.reset(); CVXB_TRY(b->gemv_ws.alloc(B * ws)); }
-        Ptrs &q = b->p;
-        double *v = b->pvecs.p;
+        double *w = b->pvecs.p;
         q.neq = p;
-        q.beq = v; q.y = v + B * p; q.ry = v + 2 * B * p; q.dy = v + 3 * B * p; q.aw = v + 4 * B * p;
+        q.beq = w; q.y = w + B * p; q.ry = w + 2 * B * p; q.dy = w + 3 * B * p; q.aw = w + 4 * B * p;
         q.infop = b->d_infop.p;
-        CVXB_TRY(state_alloc(b));
     }
-    *out = own.release();
+    if (lp) {
+        const size_t len = (size_t)n + 2 * (size_t)m + (size_t)p;
+        CVXB_TRY(b->lpv.alloc(B * len));
+        CVXB_CUDA(cudaMemset(b->lpv.p, 0, B * len * sizeof(double)));
+        q.x1 = b->lpv.p; q.z1 = q.x1 + B * n; q.th = q.z1 + B * m; q.y1 = q.th + B * m;
+    }
+    CVXB_TRY(state_alloc(b.get()));
+    *out = b.release();
+    return 0;
+}
+
+// G, h and q (c) of every problem, then a fresh batch: problems in their own slots, A and b still to load
+int load_common(cvxb_batch *b, const double *q, const double *G, const double *h, cudaMemcpyKind kind) {
+    const size_t B = b->B, n = b->n, m = b->m;
+    // one strided 2-D copy per matrix operand: rows of the "matrix of columns" are the matrix columns
+    if (m > 0) {
+        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double),
+                                    m * sizeof(double), n * B, kind, b->st));
+        CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
+    }
+    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    b->eq_loaded = false;
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    b->permuted = false;
     return 0;
 }
 
@@ -1643,56 +1508,21 @@ int create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, 
 extern "C" {
 
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
-    return create_batch(out, nprob, n, m, device, false);
+    cvxb_dims dims{};
+    dims.ml = m;
+    return create(out, nprob, n, 0, &dims, device, false);
 }
 
 int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
-    return create_cones(out, nprob, n, dims, device, false);
+    return create(out, nprob, n, 0, dims, device, false);
 }
 
 int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    return create_eq(out, nprob, n, p, dims, device, false);
+    return create(out, nprob, n, p, dims, device, false);
 }
 
 int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    if (out) *out = nullptr;
-    if (!out || nprob <= 0 || n <= 0 || p < 0 || !dims) {
-        set_error("batch_create_lp: bad sizes (nprob and n positive, p nonnegative, dims given)");
-        return CVXB_E_ARG;
-    }
-    if (nprob > CVXB_BATCH_MAX) {
-        set_error("batch_create_lp: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("batch_create_lp: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
-        return CVXB_E_ARG;
-    }
-    long long m = dims->ml;
-    for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("batch_create_lp: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
-        m += dims->q[k];
-    }
-    if (dims->ns > 0) { set_error("batch_create_lp: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
-    if (m == 0) {                                 // deliberate: every problem needs at least one cone row
-        set_error("batch_create_lp: the batch needs at least one 'l' or 'q' row (m = 0)");
-        return CVXB_E_ARG;
-    }
-    if (p > n || p + m < n) {                     // conelp's check before the first factorisation (coneprog.py:572-573)
-        set_error("batch_create_lp: Rank(A) < p or Rank([G; A]) < n (p = %d, n = %d, cdim = %lld)", p, n, m);
-        return CVXB_E_ARG;
-    }
-    cvxb_batch *b = nullptr;
-    CVXB_TRY(create_eq(&b, nprob, n, p, dims, device, true));
-    std::unique_ptr<cvxb_batch> own(b);
-    const size_t B = b->B;
-    CVXB_TRY(b->lpv.alloc(B * ((size_t)n + 2 * (size_t)m + (size_t)p)));
-    CVXB_CUDA(cudaMemset(b->lpv.p, 0, B * ((size_t)n + 2 * (size_t)m + (size_t)p) * sizeof(double)));
-    Ptrs &q = b->p;
-    q.x1 = b->lpv.p; q.z1 = q.x1 + B * n; q.th = q.z1 + B * m; q.y1 = q.th + B * m;
-    CVXB_TRY(state_alloc(b));
-    *out = own.release();
-    return 0;
+    return create(out, nprob, n, p, dims, device, true);
 }
 
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
@@ -1716,42 +1546,19 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     if (b->lp) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const size_t B = b->B, n = b->n, m = b->m;
-    // one strided 2-D copy per operand: rows of the "matrix of columns" are the matrix columns
+    const size_t n = b->n;
     CVXB_CUDA(cudaMemcpy2DAsync(b->P.p, b->ldp * sizeof(double), P, n * sizeof(double), n * sizeof(double),
-                                n * B, kind, b->st));
-    if (m > 0) {
-        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double),
-                                    m * sizeof(double), n * B, kind, b->st));
-        CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
-    }
-    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
+                                n * b->B, kind, b->st));
     // only tril(P) is significant in the reference; make the resident copies symmetric
     CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->B, b->sP, b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    b->eq_loaded = false;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
-    return 0;
+    return load_common(b, q, G, h, kind);
 }
 
 int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space) {
     if (!b || !c || !G || !h) { set_error("batch_load_lp: NULL argument"); return CVXB_E_ARG; }
     if (!b->lp) { set_error("batch_load_lp: a QP batch is loaded with cvxb_batch_load"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
-    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const size_t B = b->B, n = b->n, m = b->m;
-    CVXB_CUDA(cudaMemcpy2DAsync(b->G.p, b->ldg * sizeof(double), G, m * sizeof(double), m * sizeof(double), n * B,
-                                kind, b->st));
-    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
-    CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), c, B * n * sizeof(double), kind, b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    b->eq_loaded = false;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
-    return 0;
+    return load_common(b, c, G, h, (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
 }
 
 int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space) {
@@ -1780,17 +1587,12 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     }
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
-    const bool cones = b->p.nq > 0;
-    if (b->lp) {
-        if (b->neq > 0) return cones ? solve_conelp<true, true>(b, maxiters, abstol, reltol, feastol)
-                                     : solve_conelp<false, true>(b, maxiters, abstol, reltol, feastol);
-        return cones ? solve_conelp<true, false>(b, maxiters, abstol, reltol, feastol)
-                     : solve_conelp<false, false>(b, maxiters, abstol, reltol, feastol);
-    }
-    if (b->neq > 0) return cones ? solve_lockstep<true, true>(b, maxiters, abstol, reltol, feastol)
-                                 : solve_lockstep<false, true>(b, maxiters, abstol, reltol, feastol);
-    return cones ? solve_lockstep<true, false>(b, maxiters, abstol, reltol, feastol)
-                 : solve_lockstep<false, false>(b, maxiters, abstol, reltol, feastol);
+    using Solve = int (*)(cvxb_batch *, int, double, double, double);
+    static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
+                                     solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,
+                                     solve<false, true, true>,   solve<true, true, true>};
+    const int k = (b->p.nq > 0 ? 1 : 0) + (b->neq > 0 ? 2 : 0) + (b->lp ? 4 : 0);     // CONES, EQ, LP
+    return solvers[k](b, maxiters, abstol, reltol, feastol);
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {

@@ -1,7 +1,7 @@
-"""Cone LP batches (conelp_batch, csrc/batch_ipm.cu's solve_conelp) against a Python loop over the reference's
-solvers.conelp(c, G, h, dims, A, b) (oracle/_ref): default kktsolver ('chol2') for 'l'-only problems, kktsolver='chol'
-with 'q' cones (the reference's default there is 'qr').  Converged solutions, iterates, infeasibility certificates,
-the S + A'A switch, the start, and the batch mechanics."""
+"""Cone LP batches (conelp_batch, csrc/batch_ipm.cu's solve<CONES, EQ, LP> with LP = true) against a Python loop over
+the reference's solvers.conelp(c, G, h, dims, A, b) (oracle/_ref): default kktsolver ('chol2') for 'l'-only problems,
+kktsolver='chol' with 'q' cones (the reference's default there is 'qr').  Converged solutions, iterates, infeasibility
+certificates, the S + A'A switch, the start, and the batch mechanics."""
 import ctypes as C
 
 import numpy as np
