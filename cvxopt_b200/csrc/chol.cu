@@ -7,11 +7,12 @@
 //   step j:  (1) potf2_inv   : one CTA factors the 128x128 diagonal block in shared
 //                              memory and also produces its inverse (kept for the solves)
 //            (2) panel TRSM  : L21 = A21 * inv(L11)'  as a DMMA GEMM (gemm_dmma.cu)
-//            (3) trailing    : A22 -= L21 L21'  (lower tiles) as a DMMA GEMM
-//   Look-ahead: the first tile column of (3) — the next panel — runs on the
-//   high-priority panel stream together with (1),(2); the rest of (3) runs on the
-//   update stream, so the latency-bound panel work of step j+1 hides behind the
-//   throughput-bound update of step j.
+//            (3) trailing    : A22 -= L21 L21'  (lower tiles)
+//   Look-ahead: the next block column of (3) runs on the high-priority panel stream together with (1),(2)
+//   (dmma_gemm_kernel).  The rest of (3) is grouped by four panels: the columns inside the panel's group on a
+//   high-priority stream (dmma_gemm_kernel, K = 128), the next group's columns per panel and everything beyond
+//   as one K = 512 far update per group on the low-priority update stream (syrk_tma_kernel, from a K-major copy
+//   of the group's panels), so the latency-bound panel work hides behind the throughput-bound updates.
 //
 // trsv_lower: blocked substitution that re-uses the diagonal-block inverses; one CTA
 //   per 128-row block, progress published through acquire/release flags so that the
@@ -27,6 +28,7 @@ constexpr int PB = 8;                  // inner block width of the in-CTA factor
 constexpr int SP = 12;                 // row stride (doubles) of the panel buffer: conflict-free frags
 constexpr int LDM = NB + 4;            // column stride (doubles) of the shared-memory block
 constexpr int POTF2_SMEM = (NB * LDM + NB * SP + 4 * 80) * 8;
+constexpr int kGroup = 4;              // panels per far update of potrf_lower (K = 512)
 
 // acc[cf][rf] -= sum_k Lt[c, k] Lt[r, k] over k = 0..127 for the tiles rf >= S_cf of each column
 // fragment cf (Lt in shared memory, column-major with stride LDM; Ma/Mb already offset by lane).
@@ -553,6 +555,21 @@ trsv_kernel(int n, const double *__restrict__ L, long long ldl, const double *__
 
 std::atomic<int> g_trsv_epoch{0};   // flags written by an earlier launch never equal a later epoch
 
+// WT[k + r * ldt] = W[r + k * ldw] for r < rows, k < NB: a column-major panel to the K-major layout the TMA-fed
+// update kernel reads.  32x32 tiles through shared memory, 32x8 threads.
+__global__ void __launch_bounds__(256)
+transpose_panel_kernel(const double *__restrict__ W, long long ldw, int rows, double *__restrict__ WT, long long ldt) {
+    __shared__ double t[32][33];
+    const int r0 = blockIdx.x * 32, k0 = blockIdx.y * 32, tx = threadIdx.x, ty = threadIdx.y;
+#pragma unroll
+    for (int i = ty; i < 32; i += 8)
+        if (r0 + tx < rows) t[i][tx] = W[r0 + tx + (long long)(k0 + i) * ldw];
+    __syncthreads();
+#pragma unroll
+    for (int i = ty; i < 32; i += 8)
+        if (r0 + i < rows) WT[k0 + tx + (long long)(r0 + i) * ldt] = t[tx][i];
+}
+
 }  // namespace
 
 int chol_work_create(CholWork &w) {
@@ -561,7 +578,9 @@ int chol_work_create(CholWork &w) {
     CVXB_CUDA(cudaStreamCreateWithPriority(&w.panel_stream, cudaStreamNonBlocking, greatest));
     CVXB_CUDA(cudaStreamCreateWithPriority(&w.trsm_stream, cudaStreamNonBlocking, greatest));
     CVXB_CUDA(cudaStreamCreateWithPriority(&w.update_stream, cudaStreamNonBlocking, least));
+    CVXB_CUDA(cudaStreamCreateWithPriority(&w.near_stream, cudaStreamNonBlocking, greatest));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_t, cudaEventDisableTiming));
+    CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_n, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_start, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_p, cudaEventDisableTiming));
     CVXB_CUDA(cudaEventCreateWithFlags(&w.ev_end_u, cudaEventDisableTiming));
@@ -580,22 +599,45 @@ int chol_work_create(CholWork &w) {
 }
 
 CholWork::~CholWork() {
-    for (cudaStream_t s : {panel_stream, update_stream, trsm_stream}) if (s) cudaStreamDestroy(s);
+    for (cudaStream_t s : {panel_stream, update_stream, trsm_stream, near_stream}) if (s) cudaStreamDestroy(s);
     for (auto &g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    for (cudaEvent_t e : {ev_end_t, ev_start, ev_end_p, ev_end_u}) if (e) cudaEventDestroy(e);
-    for (auto *v : {&ev_dg, &ev_tr, &ev_c0, &ev_r})
+    for (cudaEvent_t e : {ev_end_t, ev_end_n, ev_start, ev_end_p, ev_end_u}) if (e) cudaEventDestroy(e);
+    for (auto *v : {&ev_dg, &ev_tr, &ev_c0, &ev_na, &ev_nb, &ev_n})
         for (cudaEvent_t e : *v) cudaEventDestroy(e);
 }
 
-// Look-ahead schedule (three streams, per-step events):
-//   D  (diag chain)   Dg(j): potf2_inv of block (j,j); for j>0 its prologue first applies the
-//                     step j-1 update to the block from the RAW tile A(j,j-1) and inv(j-1), so the
-//                     chain Dg(j-1) -> Dg(j) never waits for a full-width kernel.
-//   T  (panel)        Tr(j): Wp = A(j+1:, j) inv(j)'           needs Dg(j), C0(j-1)
-//                     C0(j): block column j+1 below the diagonal block -= Wp Wp'   needs R(j-1)
-//   U  (bulk)         R(j):  all later block columns (lower tiles) -= Wp Wp'        needs Tr(j)
-//   Dg(j) needs C0(j-2) and R(j-2) (they produced the tiles it reads).  L21 is copied from Wp
-//   back into A on D after Dg(j+1) has consumed the raw tile.
+// Panels jb are grouped by q = jb / kGroup; group q's block columns are kGroup q .. kGroup q + kGroup - 1, and
+// gq = kGroup (q + 1) is the first column of the next group.  Panel jb reaches block column c > jb exactly once:
+//   c == jb + 1                       C0(jb)   on T  (K = 128, dmma_gemm_kernel)
+//   jb + 2 <= c < gq                  Na(jb)   on N  near update inside the group (K = 128, dmma_gemm_kernel)
+//   max(gq, jb + 2) <= c < gq + kGroup  Nb(jb)   on U  near update of the next group (K = 128, from the K-major copy)
+//   c >= gq + kGroup                  F(q)     on U  far update, the whole group at once (K = kGroup * 128,
+//                                                  syrk_tma_kernel), issued after the group's last panel
+// (and the diagonal block (jb+1, jb+1) by the prologue of Dg(jb+1)).  F lags one group behind the chain: the
+// columns of group q+1 get group q's panels from the small Nb updates, so the chain reaches F(q)'s first column
+// only after factoring the whole of group q+1, while F(q) runs.
+//
+// Streams, per-step events:
+//   D  (diag chain)   Dg(j): potf2_inv of block (j,j); for j>0 its prologue first applies panel j-1 to the block
+//                     from the RAW tile A(j,j-1) and inv(j-1), so Dg(j-1) -> Dg(j) never waits for a full-width kernel.
+//   T  (panel)        Tr(j): Wp = A(j+1:, j) inv(j)';  C0(j);  L(j:, j-1) copied from Wp back into A (after Dg(j)
+//                     has consumed the raw tile).
+//   N  (near)         Na(j), then the transpose of Wp's rows >= gq into slot j % kGroup of the group buffer.
+//   U  (bulk)         Nb(j), and F(q) after Nb of the group's last panel.
+// Ordering.  A writer of column c with panel p must follow every writer of c with a panel < p (read-modify-write of
+// the same tiles); wait_col(s, c) orders stream s behind all updates of column c by panels <= c - 2, which is what
+// Dg(c) (diagonal block, rows of the raw tile) and C0(c-1) need:
+//   * Na(p) for p in c's group (p >= kGroup (c / kGroup)): N is in order, so ev_na[c-2] covers them;
+//   * Nb(p) for p in the group before c's, and every F(q) with c >= its first column kGroup (q + 2): those F were
+//     issued at steps <= kGroup (c / kGroup) - 5, so U runs them before Nb of the group before c's, and the wait
+//     on ev_nb of the last such panel <= c - 2 covers both.  No wait is on an F that does not touch c, so the chain
+//     never waits for the far update it is overlapping.
+// The other orderings: Tr(j) rewrites panel[j & 1] after N's reads of step j-2 (ev_n[j-2]; the reads of T are in
+// order).  Na(j) of a group's first panel follows Nb(j-1), which wrote the same columns (ev_nb[j-1]); the later
+// Na of the group follow it on N.  Nb(j) follows the transpose (ev_n[j]) and, on U, F(q-1) (the previous panel's
+// writer of its columns).  F(q) follows the group's transposes through Nb(j).  The group buffer of group q is
+// rewritten by group q+2's transposes, each behind Tr -> Dg(c >= kGroup (q + 2)), which waited for an Nb queued
+// after F(q).  Columns the chain leaves (c < j) are only read: the copy-back of L(j:, j-1) follows Dg(j) on T.
 static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cudaStream_t st) {
     if (n <= 0) return 0;
     const int nblk = (n + NB - 1) / NB;
@@ -604,30 +646,50 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         for (auto &g : w.graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
         w.graphs.clear();
         for (DevBuf<double> &pb : w.panel) pb.reset();
+        for (DevBuf<double> &gb : w.group) gb.reset();
         // two panel buffers (rows x NB): the TRSM result of step jb goes to panel[jb & 1], so it can be
-        // written while the bulk update of step jb-1 still reads the other one
+        // written while the near updates of step jb-1 still read the other one; two group buffers
+        // (kGroup NB x rows, K-major), group q's in group[q & 1] while the far update of group q-1 reads the other
         const int rows = (n + 1) & ~1;
         for (DevBuf<double> &pb : w.panel) CVXB_TRY(pb.alloc((size_t)rows * NB));
+        for (DevBuf<double> &gb : w.group) CVXB_TRY(gb.alloc((size_t)rows * kGroup * NB));
         w.panel_rows = rows;
     }
     while ((int)w.ev_dg.size() < nblk) {
-        cudaEvent_t e[4];
-        for (int i = 0; i < 4; ++i) CVXB_CUDA(cudaEventCreateWithFlags(&e[i], cudaEventDisableTiming));
-        w.ev_dg.push_back(e[0]); w.ev_tr.push_back(e[1]); w.ev_c0.push_back(e[2]); w.ev_r.push_back(e[3]);
+        cudaEvent_t e[6];
+        for (int i = 0; i < 6; ++i) CVXB_CUDA(cudaEventCreateWithFlags(&e[i], cudaEventDisableTiming));
+        w.ev_dg.push_back(e[0]); w.ev_tr.push_back(e[1]); w.ev_c0.push_back(e[2]);
+        w.ev_na.push_back(e[3]); w.ev_nb.push_back(e[4]); w.ev_n.push_back(e[5]);
     }
     if (getenv("CVXB_TRACE") && !w.trace.p) CVXB_TRY(w.trace.alloc(8 * 4096));
     unsigned long long *trace = w.trace.p;
     if (trace) CVXB_CUDA(cudaMemsetAsync(trace, 0, 8 * 4096 * sizeof(unsigned long long), st));
     const int ldw = w.panel_rows;
-    const int panel_tiles = NB / dmma_gemm_tile_cols();      // c tiles that make up one block column
-    cudaStream_t D = w.panel_stream, T = w.trsm_stream, U = w.update_stream;
+    const int ldg = kGroup * NB;                             // leading dimension of a group buffer
+    cudaStream_t D = w.panel_stream, T = w.trsm_stream, U = w.update_stream, N = w.near_stream;
     CVXB_CUDA(cudaMemsetAsync(w.d_info.p, 0, sizeof(int), st));
     CVXB_CUDA(cudaEventRecord(w.ev_start, st));
-    CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_start, 0));
-    CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_start, 0));
-    CVXB_CUDA(cudaStreamWaitEvent(U, w.ev_start, 0));
-    int last_r = -1;                       // last step that recorded ev_r
-    int prev_r = -1;                       // the one before
+    for (cudaStream_t s : {D, T, U, N}) CVXB_CUDA(cudaStreamWaitEvent(s, w.ev_start, 0));
+    // A22 -= X X' (lower) on block columns [lo, hi) and every row below, X = rows lo*NB.. of a K-wide panel
+    auto update = [&](int lo, int hi, const double *X, int ldx, bool kmajor, int K, unsigned long long *tr,
+                      cudaStream_t s) -> int {
+        double *Acc = A + (long long)lo * NB * (1 + (long long)lda);
+        GemmDesc u;
+        u.M = n - lo * NB; u.N = (hi * NB < n ? hi * NB : n) - lo * NB; u.K = K;
+        u.X = X; u.ldx = ldx; u.x_kmajor = kmajor;
+        u.Y = X; u.ldy = ldx; u.y_kmajor = kmajor;
+        u.D = Acc; u.ldd = lda; u.C = Acc; u.ldc = lda;
+        u.alpha = -1.0; u.beta = 1.0; u.lower_only = true;
+        u.trace = tr;
+        return dmma_gemm(u, s);
+    };
+    auto wait_col = [&](cudaStream_t s, int c) -> int {
+        const int p = c - 2, g0 = kGroup * (c / kGroup);
+        if (p < 0) return 0;
+        if (p >= g0) CVXB_CUDA(cudaStreamWaitEvent(s, w.ev_na[p], 0));
+        if (g0 > 0) CVXB_CUDA(cudaStreamWaitEvent(s, w.ev_nb[p < g0 - 1 ? p : g0 - 1], 0));
+        return 0;
+    };
     for (int jb = 0; jb < nblk; ++jb) {
         const int j = jb * NB;
         const int wj = (n - j < NB) ? (n - j) : NB;
@@ -637,15 +699,9 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         double *invTj = inv + (long long)(nblk + jb) * NB * NB;
         double *Wp = w.panel[jb & 1].p;
         // ---- D: diagonal block.  Needs A(jb,jb) updated through panel jb-2 and the raw tile A(jb,jb-1)
-        // (block column jb-1 complete through panel jb-2): C0(jb-2) and the last bulk update that touched
-        // block column jb.
-        if (jb >= 2) {
-            CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_c0[jb - 2], 0));
-            // the latest bulk update issued at a step <= jb-2 (a later one belongs to panels the prologue
-            // applies itself, waiting for it would serialise the chain behind the bulk work)
-            const int rd = (last_r <= jb - 2) ? last_r : prev_r;
-            if (rd >= 0) CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_r[rd], 0));
-        }
+        // (block column jb-1 complete through panel jb-2): C0(jb-2) and the updates of column jb.
+        if (jb >= 2) CVXB_CUDA(cudaStreamWaitEvent(D, w.ev_c0[jb - 2], 0));
+        CVXB_TRY(wait_col(D, jb));
         const double *Tprev = jb > 0 ? A + j + (long long)(j - NB) * lda : nullptr;
         const double *invprev = jb > 0 ? inv + (long long)(jb - 1) * NB * NB : nullptr;
         potf2_inv_kernel<<<1, 256, POTF2_SMEM, D>>>(Ajj, lda, wj, invj, invTj, w.d_info.p, j, 0, 0, Tprev,
@@ -672,8 +728,8 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         double *A22 = A21 + (long long)wj * lda;
         // ---- T: panel TRSM as a GEMM with the block inverse (out of place) ----
         CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_dg[jb], 0));
-        // the panel buffer about to be overwritten was read by the bulk update two steps ago
-        if (prev_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[prev_r], 0));
+        // the panel buffer about to be overwritten was read on N two steps ago
+        if (jb >= 2) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_n[jb - 2], 0));
         {
             GemmDesc g;
             g.M = m; g.N = wj; g.K = wj;
@@ -684,8 +740,7 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
             CVXB_TRY(dmma_gemm(g, T));
         }
         CVXB_CUDA(cudaEventRecord(w.ev_tr[jb], T));
-        // every later write of this step into block columns >= jb+1 is ordered behind the last bulk update
-        if (last_r >= 0) CVXB_CUDA(cudaStreamWaitEvent(T, w.ev_r[last_r], 0));
+        CVXB_TRY(wait_col(T, jb + 1));
         const int wn = (m < NB) ? m : NB;          // width of block column jb+1
         // ---- T: next block column, rows below its diagonal block ----
         if (m > wn) {
@@ -701,29 +756,41 @@ static int potrf_enqueue(int n, double *A, int lda, double *inv, CholWork &w, cu
         }
         CVXB_CUDA(cudaEventRecord(w.ev_c0[jb], T));
         CVXB_TRY(copy_back_prev());
-        // ---- U: the rest of the trailing matrix ----
-        if (m > NB) {
-            CVXB_CUDA(cudaStreamWaitEvent(U, w.ev_tr[jb], 0));
-            GemmDesc u;
-            u.M = m; u.N = m; u.K = wj;
-            u.X = Wp; u.ldx = ldw; u.x_kmajor = false;
-            u.Y = Wp; u.ldy = ldw; u.y_kmajor = false;
-            u.D = A22; u.ldd = lda; u.C = A22; u.ldc = lda;
-            u.alpha = -1.0; u.beta = 1.0; u.lower_only = true;
-            u.ct_begin = panel_tiles; u.ct_end = 1 << 30;
-            u.trace = trace ? trace + 8 * jb + 6 : nullptr;
-            CVXB_TRY(dmma_gemm(u, U));
-            CVXB_CUDA(cudaEventRecord(w.ev_r[jb], U));
-            prev_r = last_r;
-            last_r = jb;
+        // ---- N: near update inside the group, then this panel's rows >= gq into the group buffer ----
+        const int q = jb / kGroup, s = jb % kGroup, gq = kGroup * (q + 1);
+        double *Wg = w.group[q & 1].p;
+        unsigned long long *tr_near = trace ? trace + 8 * jb + 6 : nullptr;
+        CVXB_CUDA(cudaStreamWaitEvent(N, w.ev_tr[jb], 0));
+        if (s == 0 && jb > 0) CVXB_CUDA(cudaStreamWaitEvent(N, w.ev_nb[jb - 1], 0));
+        {
+            const int lo = jb + 2, hi = gq < nblk ? gq : nblk;
+            if (lo < hi) CVXB_TRY(update(lo, hi, Wp + (lo - jb - 1) * NB, ldw, false, NB, tr_near, N));
+        }
+        CVXB_CUDA(cudaEventRecord(w.ev_na[jb], N));
+        if (gq < nblk) {
+            const int rows = n - gq * NB;
+            transpose_panel_kernel<<<dim3((rows + 31) / 32, NB / 32), dim3(32, 8), 0, N>>>(
+                Wp + (gq - jb - 1) * NB, ldw, rows, Wg + s * NB, ldg);
+            count_launch();
+            CVXB_LAUNCH_CHECK();
+        }
+        CVXB_CUDA(cudaEventRecord(w.ev_n[jb], N));
+        // ---- U: near update of the next group's columns from the group buffer, and the far update ----
+        if (gq < nblk) {
+            CVXB_CUDA(cudaStreamWaitEvent(U, w.ev_n[jb], 0));
+            const int lo = gq > jb + 2 ? gq : jb + 2, hi = gq + kGroup < nblk ? gq + kGroup : nblk;
+            if (lo < hi) CVXB_TRY(update(lo, hi, Wg + s * NB + (long long)(lo - gq) * NB * ldg, ldg, true, NB, tr_near, U));
+            CVXB_CUDA(cudaEventRecord(w.ev_nb[jb], U));
+            if (s == kGroup - 1 && gq + kGroup < nblk)
+                CVXB_TRY(update(gq + kGroup, nblk, Wg + (long long)kGroup * NB * ldg, ldg, true, kGroup * NB,
+                                trace ? trace + 8 * 2048 + 8 * jb + 5 : nullptr, U));
         }
     }
     CVXB_CUDA(cudaEventRecord(w.ev_end_p, D));
     CVXB_CUDA(cudaEventRecord(w.ev_end_u, U));
     CVXB_CUDA(cudaEventRecord(w.ev_end_t, T));
-    CVXB_CUDA(cudaStreamWaitEvent(st, w.ev_end_p, 0));
-    CVXB_CUDA(cudaStreamWaitEvent(st, w.ev_end_u, 0));
-    CVXB_CUDA(cudaStreamWaitEvent(st, w.ev_end_t, 0));
+    CVXB_CUDA(cudaEventRecord(w.ev_end_n, N));
+    for (cudaEvent_t e : {w.ev_end_p, w.ev_end_u, w.ev_end_t, w.ev_end_n}) CVXB_CUDA(cudaStreamWaitEvent(st, e, 0));
     return 0;
 }
 

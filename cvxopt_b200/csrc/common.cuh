@@ -338,10 +338,13 @@ int ozaki_syrk(int n, int m, const double *A, long long lda, const double *d, co
 struct CholWork {
     cudaStream_t panel_stream = nullptr;   // high-priority: diagonal block, panel, next-panel update
     cudaStream_t trsm_stream = nullptr;    // high-priority: panel TRSM + next block column update
-    cudaStream_t update_stream = nullptr;  // low-priority: bulk trailing update
-    cudaEvent_t ev_end_t = nullptr;
-    std::vector<cudaEvent_t> ev_dg, ev_tr, ev_c0, ev_r;   // one per block step
-    DevBuf<unsigned long long> trace;      // CVXB_TRACE=1: per step {Dg, Tr, C0, R} x {start, end}
+    cudaStream_t update_stream = nullptr;  // low-priority: near updates of the next group, grouped far updates
+    cudaStream_t near_stream = nullptr;    // high-priority: near updates inside the group, panel transposes
+    cudaEvent_t ev_end_t = nullptr, ev_end_n = nullptr;
+    std::vector<cudaEvent_t> ev_dg, ev_tr, ev_c0, ev_na, ev_nb, ev_n;   // one per block step
+    // CVXB_TRACE=1: per step {Dg, Tr, C0, near} x {start, end}; far update of the group ending at step j at
+    // [8 * 2048 + 8 * j + 5], [.. + 6]
+    DevBuf<unsigned long long> trace;
     struct GraphEntry {                    // captured factorisation, keyed by its arguments
         int n = 0, lda = 0, launches = 0;
         const void *A = nullptr, *inv = nullptr;
@@ -354,6 +357,7 @@ struct CholWork {
     DevBuf<int> d_flags;                   // trsv progress flags (batch * ceil(n/NB) ints)
     DevBuf<double> splitk_ws;
     DevBuf<double> panel[2];               // out-of-place TRSM results (double-buffered)
+    DevBuf<double> group[2];               // K-major copies of a group's panels (double-buffered by group)
     int panel_rows = 0;
     ~CholWork();                           // also right after a chol_work_create that failed part-way
 };

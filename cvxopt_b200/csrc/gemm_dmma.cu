@@ -6,7 +6,7 @@
 //   * normal-equations assembly  K = H + G' diag(di^2) G        (X=Y=G, K-major, w=di^2,
 //     lower tiles only; replaces scale(Gs)+blas.syrk+`K += H`,   reference misc.py:1268-1276)
 //   * Cholesky panel TRSM  L21 = A21 * L11^{-T}                  (X=A21, Y=inv(L11), M-major)
-//   * Cholesky trailing update A22 -= L21 L21'                   (X=Y=L21, M-major, lower)
+//   * Cholesky next-column and in-group near updates A22 -= L21 L21'  (X=Y=L21, M-major, lower, K = 128)
 //   * the 's'-cone congruences r' X r                            (batched general GEMMs)
 //
 // wgmma has no fp64 form, so the fp64 tensor path is warp-level mma.sync.  sm_90 runs the
@@ -25,7 +25,8 @@
 //   * per-thread copy descriptors hoisted out of the k loop
 //
 // Single K-major lower-triangle SYRKs with 16-byte aligned operands and even leading dimensions (the KKT
-// normal equations, A'A, Asct'Asct, cvxb_syrk_scaled) run on syrk_tma_kernel instead: 128x128 tiles, one
+// normal equations, A'A, Asct'Asct, cvxb_syrk_scaled, and the Cholesky's updates from its K-major group buffer: the
+// far updates at K = 512 and the near updates of the next group at K = 128) run on syrk_tma_kernel instead: 128x128 tiles, one
 // CTA per SM, operands fed by TMA through an mbarrier ring by a producer warpgroup (see its comment).  It keeps
 // this kernel's warp tiles, fragments and k order, so the two agree bit for bit outside the split-K tail.
 //
