@@ -34,10 +34,9 @@ struct Scal {                       // per-problem scalars, device resident
 
 // The 'l' rows [0, ml) keep d / di / lmbda in the m-vectors; cone k occupies rows [qoff[k], qoff[k+1]) and its NT
 // scaling W_k = beta_k (2 v_k v_k' - J) lives in the per-slot state row (misc.py:290-352).  'l' rows are spread over
-// the threads of the CTA, 'q' cones over its warps: lane i of the warp owns entries i, i+32, ... of the cone in every
-// pass, and the entry-0 values every lane needs are formed from warp sums; a pass that reads an entry another lane
-// wrote follows a __syncwarp().  Kernels templated on CONES compile the cone loops out for batches without cones;
-// those templated on EQ compile the equality rows out for batches without them.
+// the threads of the CTA, 'q' cones over its warps: each warp runs cone.cuh's 'q' functions as a WarpTeam, and a pass
+// that reads an entry another lane wrote follows a __syncwarp().  Kernels templated on CONES compile the cone loops out
+// for batches without cones; those templated on EQ compile the equality rows out for batches without them.
 struct Ptrs {
     int n, m, ml, nq, refinement;
     const double *q, *h;
@@ -74,70 +73,12 @@ __device__ __forceinline__ LPScal &lp_scal(const Ptrs &p, long long oc) {
     const long long oq = (long long)b * p.neq;                                                         \
     __shared__ double sh[32];                                                                          \
     Scal &S = p.sc[b];                                                                                 \
-    (void)lane; (void)warp; (void)nwarp; (void)on; (void)om; (void)oc; (void)oq; (void)sh; (void)S;
+    const WarpTeam wt{lane};                                                                           \
+    (void)lane; (void)warp; (void)nwarp; (void)on; (void)om; (void)oc; (void)oq; (void)sh; (void)S; (void)wt;
 #define FOR_CONES(o, len)                                                  \
     for (int k_ = warp; k_ < p.nq; k_ += nwarp)                            \
         if (const int o = p.qoff[k_], len = p.qoff[k_ + 1] - p.qoff[k_]; true)
 #define FOR_LANE(i, len) for (int i = lane; i < len; i += 32)
-
-// y := W_k x (inverse = 0) or W_k^{-1} x (inverse = 1) for one cone, x and y of this lane's entries (misc_solvers.c:144-183)
-__device__ __forceinline__ void q_scale(const double *v, double beta, const double *x, double *y, int len, int lane,
-                                        bool inverse) {
-    double a = 0;
-    FOR_LANE(i, len) a += (inverse && i > 0 ? -v[i] : v[i]) * x[i];
-    a = warp_sum(a);                                      // v'x, or v'Jx for the inverse
-    const double bb = inverse ? 1.0 / beta : beta;
-    __syncwarp();
-    FOR_LANE(i, len) {
-        const double xi = x[i];
-        double r;
-        if (!inverse) r = (i == 0) ? 2.0 * v[i] * a - xi : 2.0 * v[i] * a + xi;
-        else          r = (i == 0) ? 2.0 * v[i] * a - xi : xi - 2.0 * v[i] * a;
-        y[i] = bb * r;
-    }
-}
-// x := lmbda o\ x for one cone (misc_solvers.c:813-836)
-__device__ __forceinline__ void q_sinv(const double *l, double *x, int len, int lane) {
-    const double x0 = x[0], l0 = l[0];
-    double nl = 0, d = 0;
-    FOR_LANE(i, len) if (i > 0) { nl += l[i] * l[i]; d += x[i] * l[i]; }
-    nl = sqrt(warp_sum(nl)); d = warp_sum(d);
-    const double a = (l0 + nl) * (l0 - nl), ai = 1.0 / a;
-    const double al1 = a / l0, al2 = d / l0 - x0;
-    __syncwarp();
-    FOR_LANE(i, len) x[i] = (i == 0) ? (x0 * l0 - d) * ai : (al1 * x[i] + al2 * l[i]) * ai;
-}
-// x := H(lmbda^{1/2}) x (inverse = 0) or H(lmbda^{-1/2}) x (inverse = 1) for one cone (misc_solvers.c:315-342);
-// returns the new x[0]
-__device__ __forceinline__ double q_scale2(const double *l, double *x, int len, int lane, bool inverse) {
-    const double x0 = x[0], l0 = l[0];
-    double nl = 0, lx = 0;
-    FOR_LANE(i, len) {
-        if (i > 0) nl += l[i] * l[i];
-        lx += (i > 0 && !inverse) ? -l[i] * x[i] : l[i] * x[i];
-    }
-    nl = sqrt(warp_sum(nl)); lx = warp_sum(lx);
-    double a = sqrt(l0 + nl) * sqrt(l0 - nl);
-    lx /= a;
-    double bb = (x0 + lx) / (l0 / a + 1.0) / a;
-    if (!inverse) { bb = -bb; a = 1.0 / a; }
-    __syncwarp();
-    FOR_LANE(i, len) x[i] = (i == 0) ? lx * a : (x[i] + bb * l[i]) * a;
-    return lx * a;
-}
-// sqrt(x' J x) of this lane's entries, x0 given
-__device__ __forceinline__ double q_jnrm2(const double *x, double x0, int len, int lane) {
-    double a = 0;
-    FOR_LANE(i, len) if (i > 0) a += x[i] * x[i];
-    a = sqrt(warp_sum(a));
-    return sqrt(x0 - a) * sqrt(x0 + a);
-}
-// min over the cone of the 'l'-style margin: x0 - ||x1|| (max_step is its negative, misc_solvers.c:1073-1085)
-__device__ __forceinline__ double q_margin(const double *x, double x0, int len, int lane) {
-    double a = 0;
-    FOR_LANE(i, len) if (i > 0) a += x[i] * x[i];
-    return x0 - sqrt(warp_sum(a));
-}
 
 // starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2055-2080): d = di = 1,
 // v = e1 and beta = 1 for each cone.  EQ: y = b (the solve overwrites it, :2078-2081), aw = 0 (no A'A in S yet)
@@ -178,7 +119,7 @@ __global__ void k_scale_bz(Ptrs p) {
     double *dst = p.bzp + om;
     for (int i = tid; i < p.ml; i += nt) dst[i] = p.di[om + i] * src[i];
     const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
-    FOR_CONES(o, len) q_scale(v + o, beta[k_], src + o, dst + o, len, lane, true);
+    FOR_CONES(o, len) q_scale(wt, v + o, beta[k_], src + o, dst + o, len, true);
 }
 // starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both, gap
 template <bool CONES> __global__ void k_init_point(Ptrs p) {
@@ -194,7 +135,7 @@ template <bool CONES> __global__ void k_init_point(Ptrs p) {
         if (i < p.ml) { mins = fmin(mins, -zv); minz = fmin(minz, zv); }
     }
     if (CONES) FOR_CONES(o, len) {                      // s = -z: ||s1|| = ||z1||, s0 = -z0
-        const double z0 = zn[o], mz = q_margin(zn + o, z0, len, lane);
+        const double z0 = zn[o], mz = -q_max_step(wt, zn + o, len);
         mins = fmin(mins, -z0 - (z0 - mz));
         minz = fmin(minz, mz);
     }
@@ -340,7 +281,7 @@ __global__ void k_build_gs(Ptrs p, const double *G, double *Gs, long long ldg, l
     const double *v = p.v + (long long)b * p.L - p.ml, *beta = p.beta + (long long)b * p.L;
     for (int k = 0; k < p.nq; ++k) {
         const int r = p.qoff[k], len = p.qoff[k + 1] - r;
-        q_scale(v + r, beta[k], g + r, o + r, len, lane, true);
+        q_scale(WarpTeam{lane}, v + r, beta[k], g + r, o + r, len, true);
     }
 }
 // NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357).
@@ -367,25 +308,7 @@ template <bool CONES, bool LP = false> __global__ void k_scaling(Ptrs p, int fir
     double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     if (CONES) FOR_CONES(o, len) {
         if (first) {
-            const double s0 = s[o], z0 = z[o];
-            const double aa = q_jnrm2(s + o, s0, len, lane), bb = q_jnrm2(z + o, z0, len, lane);
-            double sz = 0;
-            FOR_LANE(i, len) sz += s[o + i] * z[o + i];
-            sz = warp_sum(sz);
-            const double cc = sqrt((sz / aa / bb + 1.0) / 2.0);
-            // v = (s/a + J z/b) / (2c), then v := (v + e) / sqrt(2 (v0 + 1))
-            const double v0 = (z0 / bb + s0 / aa) * (1.0 / 2.0 / cc) + 1.0;
-            const double sc = 1.0 / sqrt(2.0 * v0);
-            const double dd = 2 * cc + s0 / aa + z0 / bb;
-            const double cs = (cc + z0 / bb) / dd / aa, cz = (cc + s0 / aa) / dd / bb, r = sqrt(aa * bb);
-            FOR_LANE(i, len) {
-                if (i == 0) { v[o] = v0 * sc; l[o] = cc * r; }
-                else {
-                    v[o + i] = (-z[o + i] / bb + s[o + i] / aa) * (1.0 / 2.0 / cc) * sc;
-                    l[o + i] = (s[o + i] * cs + z[o + i] * cz) * r;
-                }
-            }
-            if (lane == 0) beta[k_] = sqrt(aa / bb);
+            q_nt_compute(wt, s + o, z + o, v + o, l + o, beta + k_, len);
             __syncwarp();
         }
         double nl = 0;
@@ -416,12 +339,14 @@ __device__ __forceinline__ void f4_pre_row(const Ptrs &p, long long r, double &z
 // cone k at rows [o, o + len) of slot b's z and s, one warp; bzp holds W's until it receives W^{-T} z
 __device__ __forceinline__ void f4_pre_cone(const Ptrs &p, long long om, long long oc, int k, int o, int len,
                                             int lane, double *z, double *s) {
+    const WarpTeam wt{lane};
     const double *v = p.v + oc - p.ml;
     double *t = p.bzp + om;
-    q_sinv(p.lmbda + om + o, s + o, len, lane);
-    q_scale(v + o, p.beta[oc + k], s + o, t + o, len, lane, false);
+    q_sinv(wt, p.lmbda + om + o, s + o, len);
+    __syncwarp();
+    q_scale(wt, v + o, p.beta[oc + k], s + o, t + o, len, false);
     FOR_LANE(i, len) z[o + i] -= t[o + i];
-    q_scale(v + o, p.beta[oc + k], z + o, t + o, len, lane, true);
+    q_scale(wt, v + o, p.beta[oc + k], z + o, t + o, len, true);
 }
 // f4_no_ir after the solve (coneprog.py:2316), row r: z := W uz (the solve leaves it in bzp), s := s - z; returns z
 __device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double &s) {
@@ -547,17 +472,17 @@ template <bool EQ, bool LP> __global__ void k_res(Ptrs p) {
     }
     const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) {
-        q_scale(v + o, beta[k_], dz + o, wz3 + o, len, lane, true);
-        q_scale(v + o, beta[k_], ds + o, wz2 + o, len, lane, false);
-        double a = 0;
-        FOR_LANE(i, len) a += l[o + i] * (ds[o + i] + dz[o + i]);
-        a = warp_sum(a);
-        const double u0 = ds[o] + dz[o], l0 = l[o];
+        q_scale(wt, v + o, beta[k_], dz + o, wz3 + o, len, true);
+        q_scale(wt, v + o, beta[k_], ds + o, wz2 + o, len, false);
+        FOR_LANE(i, len) ws2[o + i] = ds[o + i] + dz[o + i];
+        __syncwarp();
+        q_sprod(wt, l + o, ws2 + o, ws2 + o, len);
+        __syncwarp();
         FOR_LANE(i, len) {
             double w = p.wz[oc + o + i];
             if (LP) { hz += h[o + i] * wz3[o + i]; w += ut * h[o + i]; }
             wz2[o + i] = w - wz2[o + i];
-            ws2[o + i] = p.ws[oc + o + i] - ((i == 0) ? a : l0 * (ds[o + i] + dz[o + i]) + u0 * l[o + i]);
+            ws2[o + i] = p.ws[oc + o + i] - ws2[o + i];
         }
     }
     if (LP) {
@@ -593,19 +518,14 @@ template <bool CONES, bool LP = false> __global__ void k_dir_post(Ptrs p, int i,
         __syncthreads();
     }
     if (CONES) FOR_CONES(o, len) {
-        double a = 0;
-        FOR_LANE(k, len) a += ds[o + k] * dz[o + k];
-        a = warp_sum(a);
+        const double a = q_sprod(wt, dz + o, ds + o, i == 0 ? p.ws3 + om + o : nullptr, len);
         if (lane == 0) dsdz += a;
-        if (i == 0) {
-            const double s0 = ds[o], z0 = dz[o];
-            FOR_LANE(k, len) p.ws3[om + o + k] = (k == 0) ? a : z0 * ds[o + k] + s0 * dz[o + k];
-        }
         __syncwarp();
-        const double s0 = q_scale2(l + o, ds + o, len, lane, false);
-        const double z0 = q_scale2(l + o, dz + o, len, lane, false);
-        mins = fmin(mins, q_margin(ds + o, s0, len, lane));
-        minz = fmin(minz, q_margin(dz + o, z0, len, lane));
+        q_scale2(wt, l + o, ds + o, len, false);
+        q_scale2(wt, l + o, dz + o, len, false);
+        __syncwarp();
+        mins = fmin(mins, -q_max_step(wt, ds + o, len));
+        minz = fmin(minz, -q_max_step(wt, dz + o, len));
     }
     dsdz = block_sum(dsdz, sh);
     mins = block_min(mins, sh);
@@ -673,42 +593,15 @@ template <bool CONES, bool EQ, bool LP = false> __global__ void k_update(Ptrs p,
             dz[o + k] = step * dz[o + k] + (k == 0 ? 1.0 : 0.0);
         }
         __syncwarp();
-        const double s0r = q_scale2(l + o, ds + o, len, lane, true);
-        const double z0r = q_scale2(l + o, dz + o, len, lane, true);
-        // update_scaling: st = ds / a, zt = dz / b
-        const double aa = q_jnrm2(ds + o, s0r, len, lane), bb = q_jnrm2(dz + o, z0r, len, lane);
-        const double s0 = s0r / aa, z0 = z0r / bb, v0 = v[o];
-        double sz = 0, vs = 0, vz = 0;
-        FOR_LANE(k, len) {
-            const double sk = ds[o + k] / aa, zk = dz[o + k] / bb;
-            ds[o + k] = sk; dz[o + k] = zk;
-            sz += sk * zk;
-            vs += v[o + k] * sk;
-            vz += (k == 0) ? v[o + k] * zk : -v[o + k] * zk;
-        }
-        sz = warp_sum(sz); vs = warp_sum(vs); vz = warp_sum(vz);
-        const double cc = sqrt((1.0 + sz) / 2.0);
-        const double vq = (vs + vz) / 2.0 / cc, vu = vs - vz;
-        const double wk0 = 2 * v0 * vq - (s0 + z0) / 2.0 / cc;
-        const double dd = (v0 * vu - s0 / 2.0 + z0 / 2.0) / (wk0 + 1.0);
-        const double r = sqrt(aa * bb);
-        const double nv0 = 2.0 * vq * v0 - s0 / 2.0 / cc - 0.5 / cc * z0 + 1.0, sc = 1.0 / sqrt(2.0 * nv0);
-        __syncwarp();                                     // every lane has read v[o] and l[o]
-        FOR_LANE(k, len) {
-            const double sk = ds[o + k], zk = dz[o + k], vk = v[o + k];
-            if (k == 0) { l[o] = cc * r; v[o] = nv0 * sc; }
-            else {
-                l[o + k] = (vk * (2.0 * (-dd * vq + 0.5 * vu)) + sk * (0.5 * (1.0 - dd / cc)) +
-                            zk * (0.5 * (1.0 + dd / cc))) * r;
-                v[o + k] = (2.0 * vq * vk + 0.5 / cc * sk - 0.5 / cc * zk) * sc;
-            }
-        }
-        const double bk = beta[k_] * sqrt(aa / bb);
+        q_scale2(wt, l + o, ds + o, len, true);
+        q_scale2(wt, l + o, dz + o, len, true);
         __syncwarp();
-        if (lane == 0) beta[k_] = bk;
+        q_nt_update(wt, ds + o, dz + o, v + o, l + o, beta + k_, len);
+        __syncwarp();
         // unscale with the new W and lambda
-        q_scale(v + o, bk, l + o, s + o, len, lane, false);
-        q_scale(v + o, bk, l + o, z + o, len, lane, true);
+        const double bk = beta[k_];
+        q_scale(wt, v + o, bk, l + o, s + o, len, false);
+        q_scale(wt, v + o, bk, l + o, z + o, len, true);
         double g = 0;
         FOR_LANE(k, len) g += l[o + k] * l[o + k];
         g = warp_sum(g);
@@ -761,8 +654,8 @@ template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double ab
         if (i < p.ml) { mins = fmin(mins, sv); minz = fmin(minz, zv); }
     }
     if (CONES) FOR_CONES(o, len) {
-        mins = fmin(mins, q_margin(s + o, s[o], len, lane));
-        minz = fmin(minz, q_margin(zn + o, zn[o], len, lane));
+        mins = fmin(mins, -q_max_step(wt, s + o, len));
+        minz = fmin(minz, -q_max_step(wt, zn + o, len));
     }
     ns = sqrt(block_sum(ns, sh)); nz = sqrt(block_sum(nz, sh));
     sz = block_sum(sz, sh); cx = block_sum(cx, sh); hz = block_sum(hz, sh);
@@ -872,7 +765,7 @@ template <bool EQ> __global__ void k_lp_x1_rhs(Ptrs p) {
     for (int i = tid; i < p.ml; i += nt) { const double t = p.di[om + i] * h[i]; th[i] = t; bz[i] = t; }
     const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) {
-        q_scale(v + o, beta[k_], h + o, th + o, len, lane, true);
+        q_scale(wt, v + o, beta[k_], h + o, th + o, len, true);
         __syncwarp();
         FOR_LANE(i, len) bz[o + i] = th[o + i];
     }

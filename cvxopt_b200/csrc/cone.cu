@@ -115,29 +115,8 @@ scale_q_kernel(const double *src, long long lds, double *dst, long long ldd, int
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long j = (long long)blockIdx.x * 4 + warp;
     if (j >= xc) return;
-    const int m = q[k];
-    const double *x = src + qoff[k] + j * lds;
-    double *y = dst + qoff[k] + j * ldd;
-    const double *v = vall + voff[k];
-    // w = v' * x   (with x0 negated first when applying the inverse; misc_solvers.c:166-170)
-    double w = 0.0;
-    for (int i = lane; i < m; i += 32) {
-        double xi = x[i];
-        if (inverse && i == 0) xi = -xi;
-        w += v[i] * xi;
-    }
-    w = warp_sum(w);
-    const double tw = 2.0 * w;
-    double b = betaall[k];
-    if (inverse) b = 1.0 / b;
-    for (int i = lane; i < m; i += 32) {
-        double xi = x[i];
-        // forward: x0 := -x0 before the rank-one update (:171); inverse: x0 was flipped twice
-        if (!inverse && i == 0) xi = -xi;
-        double yi = xi + v[i] * tw;           // dger (:172)
-        if (inverse && i == 0) yi = -yi;      // (:174-175)
-        y[i] = yi * b;                        // (:180-181)
-    }
+    q_scale(WarpTeam{lane}, vall + voff[k], betaall[k], src + qoff[k] + j * lds, dst + qoff[k] + j * ldd, q[k],
+            inverse);
 }
 
 __global__ void pack_s_kernel(const double *src, long long lds, double *dst, long long ldd,

@@ -88,4 +88,180 @@ int symmetrize_lower(int n, double *A, long long lda, int batch, long long strid
 int transpose_copy(const double *src, long long lds, double *dst, long long ldd, int rows, int cols,
                    cudaStream_t st, int batch = 1, long long ssrc = 0, long long sdst = 0);
 
+#ifdef __CUDACC__
+// ---- 'q' cone algebra, one cone at a time ------------------------------------------------
+// The single-problem kernels and the batch IPM share these.  Each function runs on the team of threads that owns one
+// cone: a warp (the batch kernels, scale_q) or the whole CTA (the misc_solvers mirror and the NT scaling kernels).
+// A pass gives thread `rank` the entries rank, rank + size, ..., or 1 + rank, 1 + rank + size, ... when entry 0 is
+// handled apart, and rank 0 writes entry 0.  Entry-0 values every thread needs are read after the team's sums, and a
+// function syncs before it overwrites what other threads read.  The two orders give an entry to different threads,
+// so a caller syncs between two calls when the second reads what the first wrote.
+struct WarpTeam {
+    int rank;                                   // lane
+    static constexpr int size = 32;
+    __device__ __forceinline__ double sum(double v) const { return warp_sum(v); }
+    __device__ __forceinline__ void sync() const { __syncwarp(); }
+};
+struct CtaTeam {
+    int rank, size;                             // threadIdx.x, blockDim.x
+    double *sh;                                 // block_sum's 32 doubles of shared memory
+    __device__ __forceinline__ double sum(double v) const { return block_sum(v, sh); }
+    __device__ __forceinline__ void sync() const { __syncthreads(); }
+};
+// Not unrolled: a cone seldom gives a thread more than one entry, and unrolled passes cost the batch kernels registers.
+#define TEAM_FOR(i, t, i0, m) _Pragma("unroll 1") for (int i = (i0) + (t).rank; i < (m); i += (t).size)
+
+// y := W x (inverse = false) or W^{-1} x, W = beta (2 v v' - J) (misc_solvers.c:144-183).  y may be x.
+template <class Team>
+__device__ __forceinline__ void q_scale(const Team &t, const double *v, double beta, const double *x, double *y, int m,
+                                        bool inverse) {
+    // w = v' x, with x0 negated first when applying the inverse (:166-170)
+    double w = 0.0;
+    TEAM_FOR(i, t, 0, m) {
+        double xi = x[i];
+        if (inverse && i == 0) xi = -xi;
+        w += v[i] * xi;
+    }
+    const double tw = 2.0 * t.sum(w);
+    const double b = inverse ? 1.0 / beta : beta;
+    TEAM_FOR(i, t, 0, m) {
+        double xi = x[i];
+        // forward: x0 := -x0 before the rank-one update (:171); inverse: x0 was flipped twice
+        if (!inverse && i == 0) xi = -xi;
+        double yi = xi + v[i] * tw;           // dger (:172)
+        if (inverse && i == 0) yi = -yi;      // (:174-175)
+        y[i] = yi * b;                        // (:180-181)
+    }
+}
+
+// x := H(lmbda^{1/2}) x (inverse = false) or H(lmbda^{-1/2}) x (misc_solvers.c:315-342)
+template <class Team>
+__device__ __forceinline__ void q_scale2(const Team &t, const double *l, double *x, int m, bool inverse) {
+    double n2 = 0, dot = 0;
+    TEAM_FOR(i, t, 1, m) { n2 += l[i] * l[i]; dot += l[i] * x[i]; }
+    n2 = t.sum(n2); dot = t.sum(dot);
+    const double nrm = sqrt(n2), l0 = l[0], x0 = x[0];
+    const double a = sqrt(l0 + nrm) * sqrt(l0 - nrm);
+    const double lx = inverse ? (l0 * x0 + dot) / a : (l0 * x0 - dot) / a;
+    double b = (x0 + lx) / (l0 / a + 1.0) / a;
+    if (!inverse) b = -b;
+    const double sc = inverse ? a : 1.0 / a;
+    t.sync();
+    TEAM_FOR(i, t, 1, m) x[i] = (x[i] + b * l[i]) * sc;
+    if (t.rank == 0) x[0] = lx * sc;
+}
+
+// out := y o x (misc_solvers.c:634-767); out may be x.  Returns y'x, the product's entry 0; with out == nullptr
+// that is all it computes.
+template <class Team>
+__device__ __forceinline__ double q_sprod(const Team &t, const double *y, const double *x, double *out, int m) {
+    double d = 0;
+    TEAM_FOR(i, t, 0, m) d += y[i] * x[i];
+    d = t.sum(d);
+    if (!out) return d;
+    const double y0 = y[0], x0 = x[0];
+    t.sync();
+    TEAM_FOR(i, t, 1, m) out[i] = y0 * x[i] + x0 * y[i];
+    if (t.rank == 0) out[0] = d;
+    return d;
+}
+
+// x := lmbda o\ x (misc_solvers.c:813-836)
+template <class Team>
+__device__ __forceinline__ void q_sinv(const Team &t, const double *l, double *x, int m) {
+    double n2 = 0, d = 0;
+    TEAM_FOR(i, t, 1, m) { n2 += l[i] * l[i]; d += x[i] * l[i]; }
+    n2 = t.sum(n2); d = t.sum(d);
+    const double nrm = sqrt(n2), l0 = l[0], x0 = x[0];
+    const double a = (l0 + nrm) * (l0 - nrm);
+    const double al1 = a / l0, al2 = d / l0 - x0, ia = 1.0 / a;
+    t.sync();
+    TEAM_FOR(i, t, 1, m) x[i] = (x[i] * al1 + al2 * l[i]) * ia;
+    if (t.rank == 0) x[0] = (x0 * l0 - d) * ia;
+}
+
+// sqrt(x' J x) the way misc.jnrm2 evaluates it (misc.py:848-856): a = |x[1:]|, sqrt(x0 - a) * sqrt(x0 + a)
+template <class Team>
+__device__ __forceinline__ double q_jnrm2(const Team &t, const double *x, int m) {
+    double n2 = 0.0;
+    TEAM_FOR(i, t, 1, m) n2 += x[i] * x[i];
+    const double a = sqrt(t.sum(n2));
+    return sqrt(x[0] - a) * sqrt(x[0] + a);
+}
+
+// the cone's term of max_step, |x[1:]| - x0 (misc_solvers.c:1073-1085)
+template <class Team>
+__device__ __forceinline__ double q_max_step(const Team &t, const double *x, int m) {
+    double n2 = 0;
+    TEAM_FOR(i, t, 1, m) n2 += x[i] * x[i];
+    return sqrt(t.sum(n2)) - x[0];
+}
+
+// NT scaling of the cone from s and z (misc.py:311-354): v, lmbda, and *beta = sqrt(a / b)
+template <class Team>
+__device__ __forceinline__ void q_nt_compute(const Team &t, const double *s, const double *z, double *v, double *lm,
+                                             double *beta, int m) {
+    const double aa = q_jnrm2(t, s, m), bb = q_jnrm2(t, z, m);
+    double sz = 0.0;
+    TEAM_FOR(i, t, 0, m) sz += s[i] * z[i];
+    const double dot = t.sum(sz);
+    const double cc = sqrt((dot / aa / bb + 1.0) / 2.0);
+    // vk = 1/(2c) ( s/a + J z/b ),  then  v = (vk + e) / sqrt(2 (vk0 + 1))
+    const double v0 = ((s[0] / aa) + (z[0] / bb)) / 2.0 / cc + 1.0;
+    const double sc = 1.0 / sqrt(2.0 * v0);
+    const double dd = 2.0 * cc + s[0] / aa + z[0] / bb;
+    const double c1 = (cc + z[0] / bb) / dd / aa, c2 = (cc + s[0] / aa) / dd / bb, sab = sqrt(aa * bb);
+    TEAM_FOR(i, t, 0, m) {
+        if (i == 0) {
+            v[0] = v0 * sc;
+            lm[0] = cc * sab;
+        } else {
+            v[i] = ((s[i] / aa - z[i] / bb) / 2.0 / cc) * sc;
+            lm[i] = (c1 * s[i] + c2 * z[i]) * sab;
+        }
+    }
+    if (t.rank == 0) *beta = sqrt(aa / bb);
+}
+
+// NT scaling update of the cone (misc.py:504-573): s, z hold the new iterates in the current scaling and are
+// normalised in place; v and lmbda are overwritten, *beta *= sqrt(a / b)
+template <class Team>
+__device__ __forceinline__ void q_nt_update(const Team &t, double *s, double *z, double *v, double *lm, double *beta,
+                                            int m) {
+    const double aa = q_jnrm2(t, s, m), bb = q_jnrm2(t, z, m);
+    t.sync();                                   // every thread has read s[0] and z[0]
+    double t1 = 0.0, t2 = 0.0, t3 = 0.0;
+    TEAM_FOR(i, t, 0, m) {
+        const double si = s[i] * (1.0 / aa), zi = z[i] * (1.0 / bb);
+        s[i] = si; z[i] = zi;
+        t1 += si * zi;
+        t2 += v[i] * si;
+        t3 += (i == 0 ? v[i] * zi : -v[i] * zi);     // jdot: v' J z
+    }
+    const double dot = t.sum(t1), vs = t.sum(t2), vz = t.sum(t3);
+    t.sync();                                   // s[0] and z[0] are written
+    const double cc = sqrt((1.0 + dot) / 2.0);
+    const double vq = (vs + vz) / 2.0 / cc, vu = vs - vz;
+    const double s0 = s[0], z0 = z[0], vk0 = v[0];
+    const double wk0 = 2.0 * vk0 * vq - (s0 + z0) / 2.0 / cc;
+    const double dd = (vk0 * vu - s0 / 2.0 + z0 / 2.0) / (wk0 + 1.0);
+    const double sab = sqrt(aa * bb);
+    // new v before its square root:  v := 2 (v'q) v - (J st/a + zt/b) / (2c)
+    const double vn0 = 2.0 * vq * vk0 - s0 / 2.0 / cc - 0.5 / cc * z0 + 1.0;
+    const double sc = 1.0 / sqrt(2.0 * vn0);
+    t.sync();
+    TEAM_FOR(i, t, 0, m) {
+        const double vi = v[i], si = s[i], zi = z[i];
+        if (i == 0) {
+            lm[0] = cc * sab;
+            v[0] = vn0 * sc;
+        } else {
+            lm[i] = (vi * (2.0 * (-dd * vq + 0.5 * vu)) + 0.5 * (1.0 - dd / cc) * si + 0.5 * (1.0 + dd / cc) * zi) * sab;
+            v[i] = (2.0 * vq * vi + 0.5 / cc * si - 0.5 / cc * zi) * sc;
+        }
+    }
+    if (t.rank == 0) *beta *= sqrt(aa / bb);
+}
+#endif
+
 }  // namespace cvxb

@@ -29,20 +29,8 @@ __global__ void scale2_kernel(const double *lm, double *x, Cones c, int inverse)
     for (int i = tid; i < c.nl; i += nt) x[i] = inverse ? x[i] * lm[i] : x[i] / lm[i];
     int m = c.nl;
     for (int k = 0; k < c.nq; ++k) {
-        const int mk = c.q[k];
-        double n2 = 0, dot = 0;
-        for (int i = 1 + tid; i < mk; i += nt) { n2 += lm[m + i] * lm[m + i]; dot += lm[m + i] * x[m + i]; }
-        n2 = block_sum(n2, sh); dot = block_sum(dot, sh);
-        const double nrm = sqrt(n2), l0 = lm[m], x0 = x[m];
-        double a = sqrt(l0 + nrm) * sqrt(l0 - nrm);
-        const double lx = inverse ? (l0 * x0 + dot) / a : (l0 * x0 - dot) / a;
-        double b = (x0 + lx) / (l0 / a + 1.0) / a;
-        if (!inverse) b = -b;
-        const double sc = inverse ? a : 1.0 / a;
-        __syncthreads();
-        for (int i = 1 + tid; i < mk; i += nt) x[m + i] = (x[m + i] + b * lm[m + i]) * sc;
-        if (tid == 0) x[m] = lx * sc;
-        m += mk;
+        q_scale2(CtaTeam{tid, nt, sh}, lm + m, x + m, c.q[k], inverse);
+        m += c.q[k];
         __syncthreads();
     }
     int ind2 = m;
@@ -64,15 +52,8 @@ __global__ void sprod_kernel(double *x, const double *y, Cones c, int diag_d) {
     for (int i = tid; i < c.nl; i += nt) x[i] *= y[i];
     int m = c.nl;
     for (int k = 0; k < c.nq; ++k) {
-        const int mk = c.q[k];
-        double d = 0;
-        for (int i = tid; i < mk; i += nt) d += y[m + i] * x[m + i];
-        d = block_sum(d, sh);
-        const double y0 = y[m], x0 = x[m];
-        __syncthreads();
-        for (int i = 1 + tid; i < mk; i += nt) x[m + i] = y0 * x[m + i] + x0 * y[m + i];
-        if (tid == 0) x[m] = d;
-        m += mk;
+        q_sprod(CtaTeam{tid, nt, sh}, y + m, x + m, x + m, c.q[k]);
+        m += c.q[k];
         __syncthreads();
     }
     if (!diag_d) return;
@@ -100,17 +81,8 @@ __global__ void sinv_kernel(double *x, const double *y, Cones c) {
     for (int i = tid; i < c.nl; i += nt) x[i] /= y[i];
     int m = c.nl;
     for (int k = 0; k < c.nq; ++k) {
-        const int mk = c.q[k];
-        double n2 = 0, d = 0;
-        for (int i = 1 + tid; i < mk; i += nt) { n2 += y[m + i] * y[m + i]; d += x[m + i] * y[m + i]; }
-        n2 = block_sum(n2, sh); d = block_sum(d, sh);
-        const double nrm = sqrt(n2), y0 = y[m], cx = x[m];
-        const double a = (y0 + nrm) * (y0 - nrm);
-        const double al1 = a / y0, al2 = d / y0 - cx, ia = 1.0 / a;
-        __syncthreads();
-        for (int i = 1 + tid; i < mk; i += nt) x[m + i] = (x[m + i] * al1 + al2 * y[m + i]) * ia;
-        if (tid == 0) x[m] = (cx * y0 - d) * ia;
-        m += mk;
+        q_sinv(CtaTeam{tid, nt, sh}, y + m, x + m, c.q[k]);
+        m += c.q[k];
         __syncthreads();
     }
     int ind2 = m;
@@ -172,12 +144,8 @@ __global__ void max_step_kernel(const double *x, Cones c, double *out) {
     __syncthreads();
     int m = c.nl;
     for (int k = 0; k < c.nq; ++k) {
-        const int mk = c.q[k];
-        double n2 = 0;
-        for (int i = 1 + tid; i < mk; i += nt) n2 += x[m + i] * x[m + i];
-        n2 = block_sum(n2, sh);
-        t = fmax(t, sqrt(n2) - x[m]);
-        m += mk;
+        t = fmax(t, q_max_step(CtaTeam{tid, nt, sh}, x + m, c.q[k]));
+        m += c.q[k];
         __syncthreads();
     }
     if (tid == 0) *out = (m > 0) ? t : 0.0;

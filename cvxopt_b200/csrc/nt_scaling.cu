@@ -44,84 +44,22 @@ __global__ void nt_l_update_kernel(int m, double *s, double *z, double *d, doubl
 }
 
 // ---------------------------------------------------------------- 'q' cones
-// sqrt(x' J x) the way misc.jnrm2 evaluates it (misc.py:848-856): a = |x[1:]|, sqrt(x0 - a) * sqrt(x0 + a)
-__device__ __forceinline__ double jnrm2_dev(const double *x, int m, double *sh) {
-    double t = 0.0;
-    for (int i = 1 + threadIdx.x; i < m; i += blockDim.x) t += x[i] * x[i];
-    const double a = sqrt(block_sum(t, sh));
-    return sqrt(x[0] - a) * sqrt(x[0] + a);
-}
-
 // one CTA per cone                                                               (misc.py:311-354)
 __global__ void nt_q_compute_kernel(const int *q, const int *qoff, const int *voff, int lam_base, const double *s,
                                     const double *z, double *vall, double *beta, double *lm) {
     __shared__ double sh[32];
-    const int k = blockIdx.x, m = q[k];
-    const double *sk = s + qoff[k], *zk = z + qoff[k];
-    double *v = vall + voff[k], *lk = lm + lam_base + voff[k];
-    const double aa = jnrm2_dev(sk, m, sh), bb = jnrm2_dev(zk, m, sh);
-    double t = 0.0;
-    for (int i = threadIdx.x; i < m; i += blockDim.x) t += sk[i] * zk[i];
-    const double dot = block_sum(t, sh);
-    const double cc = sqrt((dot / aa / bb + 1.0) / 2.0);
-    // vk = 1/(2c) ( sk/a + J zk/b ),  then  v = (vk + e) / sqrt(2 (vk0 + 1))
-    const double v0 = ((sk[0] / aa) + (zk[0] / bb)) / 2.0 / cc + 1.0;
-    const double sc = 1.0 / sqrt(2.0 * v0);
-    const double dd = 2.0 * cc + sk[0] / aa + zk[0] / bb;
-    const double c1 = (cc + zk[0] / bb) / dd / aa, c2 = (cc + sk[0] / aa) / dd / bb, sab = sqrt(aa * bb);
-    for (int i = threadIdx.x; i < m; i += blockDim.x) {
-        if (i == 0) {
-            v[0] = v0 * sc;
-            lk[0] = cc * sab;
-        } else {
-            v[i] = ((sk[i] / aa - zk[i] / bb) / 2.0 / cc) * sc;
-            lk[i] = (c1 * sk[i] + c2 * zk[i]) * sab;
-        }
-    }
-    if (threadIdx.x == 0) beta[k] = sqrt(aa / bb);
+    const int k = blockIdx.x;
+    q_nt_compute(CtaTeam{(int)threadIdx.x, (int)blockDim.x, sh}, s + qoff[k], z + qoff[k], vall + voff[k],
+                 lm + lam_base + voff[k], beta + k, q[k]);
 }
 
 // one CTA per cone; s, z hold the new iterates in the current scaling and are normalised in place   (misc.py:504-573)
 __global__ void nt_q_update_kernel(const int *q, const int *qoff, const int *voff, int lam_base, double *s, double *z,
                                    double *vall, double *beta, double *lm) {
     __shared__ double sh[32];
-    const int k = blockIdx.x, m = q[k];
-    double *sk = s + qoff[k], *zk = z + qoff[k];
-    double *v = vall + voff[k], *lk = lm + lam_base + voff[k];
-    const double aa = jnrm2_dev(sk, m, sh);
-    for (int i = threadIdx.x; i < m; i += blockDim.x) sk[i] *= 1.0 / aa;
-    __syncthreads();
-    const double bb = jnrm2_dev(zk, m, sh);
-    for (int i = threadIdx.x; i < m; i += blockDim.x) zk[i] *= 1.0 / bb;
-    __syncthreads();
-    double t1 = 0.0, t2 = 0.0, t3 = 0.0;
-    for (int i = threadIdx.x; i < m; i += blockDim.x) {
-        t1 += sk[i] * zk[i];
-        t2 += v[i] * sk[i];
-        t3 += (i == 0 ? v[i] * zk[i] : -v[i] * zk[i]);     // jdot: v' J z
-    }
-    const double dot = block_sum(t1, sh), vs = block_sum(t2, sh), vz = block_sum(t3, sh);
-    const double cc = sqrt((1.0 + dot) / 2.0);
-    const double vq = (vs + vz) / 2.0 / cc, vu = vs - vz;
-    const double s0 = sk[0], z0 = zk[0], vk0 = v[0];
-    const double wk0 = 2.0 * vk0 * vq - (s0 + z0) / 2.0 / cc;
-    const double dd = (vk0 * vu - s0 / 2.0 + z0 / 2.0) / (wk0 + 1.0);
-    const double sab = sqrt(aa * bb);
-    // new v before its square root:  v := 2 (v'q) v - (J st/a + zt/b) / (2c)
-    const double vn0 = 2.0 * vq * vk0 - s0 / 2.0 / cc - 0.5 / cc * z0 + 1.0;
-    const double sc = 1.0 / sqrt(2.0 * vn0);
-    __syncthreads();
-    for (int i = threadIdx.x; i < m; i += blockDim.x) {
-        const double vi = v[i], si = sk[i], zi = zk[i];
-        if (i == 0) {
-            lk[0] = cc * sab;
-            v[0] = vn0 * sc;
-        } else {
-            lk[i] = (vi * (2.0 * (-dd * vq + 0.5 * vu)) + 0.5 * (1.0 - dd / cc) * si + 0.5 * (1.0 + dd / cc) * zi) * sab;
-            v[i] = (2.0 * vq * vi + 0.5 / cc * si - 0.5 / cc * zi) * sc;
-        }
-    }
-    if (threadIdx.x == 0) beta[k] *= sqrt(aa / bb);
+    const int k = blockIdx.x;
+    q_nt_update(CtaTeam{(int)threadIdx.x, (int)blockDim.x, sh}, s + qoff[k], z + qoff[k], vall + voff[k],
+                lm + lam_base + voff[k], beta + k, q[k]);
 }
 
 // ---------------------------------------------------------------- 's' cones: helpers
