@@ -88,6 +88,18 @@ _SIGS = {
     "cvxb_potrs": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_gemm": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_void_p,
                             C.c_int, C.c_void_p, C.c_int, C.c_double, C.c_void_p, C.c_int, C.c_int]),
+    "cvxb_potrf_batched": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong,
+                                     C.c_int, C.c_void_p, C.c_int]),
+    "cvxb_trsv_batched": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong,
+                                    C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int]),
+    "cvxb_trsm_batched": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong,
+                                    C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_int, C.c_int]),
+    "cvxb_syrk_batched": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_longlong,
+                                    C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_int, C.c_longlong,
+                                    C.c_int, C.c_int]),
+    "cvxb_gemv_batched": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p,
+                                    C.c_longlong, C.c_void_p, C.c_longlong, C.c_double, C.c_double, C.c_void_p,
+                                    C.c_longlong, C.c_int, C.c_int]),
     "cvxb_batch_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]),
     "cvxb_batch_create_cones": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(Dims), C.c_int]),
     "cvxb_batch_create_eq": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Dims),

@@ -115,6 +115,119 @@ int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const d
     return 0;
 }
 
+// ---------------------------------------------------------------- batched building blocks of the batch solver
+// Problem b of every operand is at base + b * stride.  The arguments are checked before the device, as the batch
+// constructors do.
+static int batch_args(const char *what, int batch, int size0, int size1) {
+    if (batch < 1 || batch > CVXB_BATCH_MAX) {
+        set_error("%s: batch = %d outside 1..%d", what, batch, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (size0 < 0 || size1 < 0) {
+        set_error("%s: negative size", what);
+        return CVXB_E_ARG;
+    }
+    return 0;
+}
+static int ld_arg(const char *what, const char *name, long long ld, int rows) {
+    if (ld < (rows > 1 ? rows : 1)) {
+        set_error("%s: %s = %lld < max(1, %d)", what, name, ld, rows);
+        return CVXB_E_ARG;
+    }
+    return 0;
+}
+
+int cvxb_potrf_batched(int n, double *A, int lda, long long sA, double *work_inv, long long sInv, int batch,
+                       int *info, int device) {
+    CVXB_TRY(batch_args("potrf_batched", batch, n, 0));
+    CVXB_TRY(ld_arg("potrf_batched", "lda", lda, n));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    Scratch<int> d_info;
+    Scratch<double> panel;
+    const int ldw = (n + 1) & ~1;
+    CVXB_TRY(d_info.alloc(batch));
+    CVXB_TRY(panel.alloc((size_t)batch * ldw * NB));
+    int rc = potrf_lower_batched(n, A, lda, sA, work_inv, sInv, batch, d_info.p, panel.p, ldw, ctx.st);
+    if (rc == 0 && n > 0) {
+        const cudaError_t e = cudaMemcpyAsync(info, d_info.p, (size_t)batch * sizeof(int), cudaMemcpyDeviceToHost,
+                                              ctx.st);
+        if (e != cudaSuccess) { set_error("potrf_batched: %s", cudaGetErrorString(e)); rc = CVXB_E_CUDA; }
+    } else if (rc == 0) {
+        for (int b = 0; b < batch; ++b) info[b] = 0;
+    }
+    const cudaError_t e = cudaStreamSynchronize(ctx.st);        // before the scratch goes back to the cache
+    if (rc) return rc;
+    if (e != cudaSuccess) { set_error("potrf_batched: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
+    return 0;
+}
+
+int cvxb_trsv_batched(int n, const double *L, int ldl, long long sL, const double *inv, long long sInv, double *b,
+                      long long sb, int trans, int batch, int device) {
+    CVXB_TRY(batch_args("trsv_batched", batch, n, 0));
+    CVXB_TRY(ld_arg("trsv_batched", "ldl", ldl, n));
+    if (trans != 'N' && trans != 'T') { set_error("trsv_batched: trans must be 'N' or 'T'"); return CVXB_E_ARG; }
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    CVXB_TRY(trsv_lower(n, L, ldl, inv, b, trans == 'T', *ctx.cw, ctx.st, batch, sL, sInv, sb));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
+    return 0;
+}
+
+int cvxb_trsm_batched(int n, const double *L, int ldl, long long sL, const double *inv, long long sInv, double *B,
+                      int ldb, long long sB, int ncols, int batch, int device) {
+    CVXB_TRY(batch_args("trsm_batched", batch, n, ncols));
+    CVXB_TRY(ld_arg("trsm_batched", "ldl", ldl, n));
+    CVXB_TRY(ld_arg("trsm_batched", "ldb", ldb, n));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    CVXB_TRY(trsm_lower_left(n, L, ldl, inv, B, ldb, ncols, ctx.st, batch, sL, sInv, sB));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
+    return 0;
+}
+
+int cvxb_syrk_batched(int n, int k, const double *A, int lda, long long sA, const double *w, long long sw,
+                      const double *D, int ldd, long long sD, double *C, int ldc, long long sC, int batch,
+                      int device) {
+    CVXB_TRY(batch_args("syrk_batched", batch, n, k));
+    CVXB_TRY(ld_arg("syrk_batched", "lda", lda, k));
+    CVXB_TRY(ld_arg("syrk_batched", "ldc", ldc, n));
+    if (D) CVXB_TRY(ld_arg("syrk_batched", "ldd", ldd, n));
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    GemmDesc g;
+    g.M = n; g.N = n; g.K = k;
+    g.X = A; g.ldx = lda; g.x_kmajor = true; g.sX = sA;
+    g.Y = A; g.ldy = lda; g.y_kmajor = true; g.sY = sA;
+    g.w = w; g.sW = w ? sw : 0;
+    g.D = D; g.ldd = D ? ldd : 0; g.sD = D ? sD : 0; g.beta = D ? 1.0 : 0.0;
+    g.C = C; g.ldc = ldc; g.sC = sC;
+    g.lower_only = true; g.batch = batch;
+    // no split-K workspace: the result depends on the problem and the layout only
+    CVXB_TRY(dmma_gemm(g, ctx.st));
+    CVXB_CUDA(cudaStreamSynchronize(ctx.st));
+    return 0;
+}
+
+int cvxb_gemv_batched(int trans, int nrows, int ncols, const double *A, int lda, long long sA, const double *w,
+                      long long sw, const double *x, long long sx, double alpha, double beta, double *y,
+                      long long sy, int batch, int device) {
+    CVXB_TRY(batch_args("gemv_batched", batch, nrows, ncols));
+    CVXB_TRY(ld_arg("gemv_batched", "lda", lda, nrows));
+    if (trans != 'N' && trans != 'T') { set_error("gemv_batched: trans must be 'N' or 'T'"); return CVXB_E_ARG; }
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    GemvBatch bs;
+    bs.batch = batch; bs.sA = sA; bs.sw = w ? sw : 0; bs.sx = sx; bs.sy = sy;
+    if (trans == 'T') {
+        CVXB_TRY(gemv_t(nrows, ncols, A, lda, w, x, alpha, beta, y, ctx.st, bs));
+        CVXB_CUDA(cudaStreamSynchronize(ctx.st));
+        return 0;
+    }
+    Scratch<double> ws;
+    CVXB_TRY(ws.alloc((size_t)batch * nrows * gemv_n_chunks(ncols)));
+    const int rc = gemv_n(nrows, ncols, A, lda, w, x, alpha, beta, y, ws.p, ctx.st, bs);
+    const cudaError_t e = cudaStreamSynchronize(ctx.st);        // before the workspace goes back to the cache
+    if (rc) return rc;
+    if (e != cudaSuccess) { set_error("gemv_batched: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
+    return 0;
+}
+
 // ---------------------------------------------------------------- misc_solvers mirror
 int cvxb_scale(double *x, int xr, int xc, const cvxb_dims *dims, const cvxb_scaling *W, int trans,
                int inverse, int space) {

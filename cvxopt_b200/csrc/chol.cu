@@ -864,7 +864,8 @@ int trsv_lower(int n, const double *L, int ldl, const double *inv, double *b, bo
     if (nflags > w.d_flags.n) {
         w.d_flags.reset();
         CVXB_TRY(w.d_flags.alloc(nflags));
-        CVXB_CUDA(cudaMemset(w.d_flags.p, 0, nflags * sizeof(int)));
+        // on st: a plain cudaMemset runs on the legacy stream, which the non-blocking st does not wait for
+        CVXB_CUDA(cudaMemsetAsync(w.d_flags.p, 0, nflags * sizeof(int), st));
     }
     const int epoch = g_trsv_epoch.fetch_add(1) + 1;
     const double *invT = inv + (long long)nblk * NB * NB;

@@ -211,6 +211,33 @@ int cvxb_potrs(int n, const double *L, int ldl, const double *inv, double *b, in
 int cvxb_gemm(int transa, int transb, int m, int n, int k, double alpha, const double *A,
               int lda, const double *B, int ldb, double beta, double *C, int ldc, int device);
 
+/* ---- batched dense building blocks: the factorisation, solves and products the batch solver below runs on all of
+ * its problems at once, exposed for tests and for callers that batch their own factorisations.  Device pointers,
+ * column-major; problem b of an operand is at base + b * stride (strides in doubles).  batch outside
+ * 1..CVXB_BATCH_MAX, a negative size, a leading dimension below max(1, rows) or an unknown trans is CVXB_E_ARG,
+ * checked before the device.  Nothing is split or reduced across problems: a problem's result depends on its own
+ * data and the layout only. */
+/* n x n Cholesky (lower) of every problem in place; work_inv as for cvxb_potrf, per problem (stride sInv >=
+ * 2 * ceil(n/128) * 128*128).  info (host, batch ints) receives LAPACK's info per problem; returns 0 or CVXB_E_*. */
+int cvxb_potrf_batched(int n, double *A, int lda, long long sA, double *work_inv, long long sInv,
+                       int batch, int *info, int device);
+/* in place on b with cvxb_potrf_batched's factors: trans 'N' solves L x = b, 'T' solves L' x = b ('N' then 'T' is
+ * potrs) */
+int cvxb_trsv_batched(int n, const double *L, int ldl, long long sL, const double *inv, long long sInv,
+                      double *b, long long sb, int trans, int batch, int device);
+/* B := L^{-1} B in place, B n x ncols */
+int cvxb_trsm_batched(int n, const double *L, int ldl, long long sL, const double *inv, long long sInv,
+                      double *B, int ldb, long long sB, int ncols, int batch, int device);
+/* lower triangle of C = A' diag(w) A + D, A k x n; w and D may be NULL, D may equal C */
+int cvxb_syrk_batched(int n, int k, const double *A, int lda, long long sA, const double *w, long long sw,
+                      const double *D, int ldd, long long sD, double *C, int ldc, long long sC,
+                      int batch, int device);
+/* A nrows x ncols.  trans 'T': y = alpha A' (w .* x) + beta y;  'N': y = alpha w .* (A x) + beta y.  w may be NULL;
+ * beta = 0 does not read y */
+int cvxb_gemv_batched(int trans, int nrows, int ncols, const double *A, int lda, long long sA,
+                      const double *w, long long sw, const double *x, long long sx, double alpha,
+                      double beta, double *y, long long sy, int batch, int device);
+
 /* ---- batch of independent dense QPs (BASELINE config 4): one problem per
  * CTA-group, lock-step primal-dual IPM fully on device (oracle: a Python loop
  * over coneqp).  Problems are  min 1/2 x'P x + q'x  s.t.  G x + s = h, s in the

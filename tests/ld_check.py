@@ -120,9 +120,79 @@ def backward_error(A, x, b):
 
 
 def check_potrs(A, x, b, kappa, c=1.0):
-    """normwise backward error of a solve with A = L L' <= c n u max(1, kappa); returns (error / bound, error)"""
+    """normwise backward error of a solve with A = L L' <= c (n + 2) u max(1, kappa); returns (error / bound, error).
+    The residual is taken against A, so it includes the factorisation's own residual, whose bound check_potrf states
+    as (n + 2) u max(1, kappa) |L| |L'|.  An earlier n u was below that and wrong for the smallest n: a 1 x 1 solve
+    rounds the square root, the reciprocal and two products, and showed a backward error of 1.3 u."""
     n = A.shape[0]
     eta = backward_error(A, x, b)
-    bound = c * n * EPS * max(1.0, kappa)
+    bound = c * (n + 2) * EPS * max(1.0, kappa)
     assert eta <= bound, (eta, bound)
     return eta / bound, eta
+
+
+def check_trsv(L, x, b, trans, kappa, c=1.0):
+    """triangular solve op(L) x = b (op(L) = L for 'N', L' for 'T'; only L's lower triangle is read): normwise
+    backward error ||b - op(L) x||_inf / (||op(L)||_inf ||x||_inf + ||b||_inf) <= c n u max(1, kappa), kappa =
+    diag_block_kappa(L).  The blocked solves form each block of x as inv(L_ii) t, so the residual carries kappa(L_ii)
+    as in check_potrs.  Returns error / bound."""
+    n = L.shape[0]
+    Lt = np.tril(L)
+    eta = backward_error(Lt.T if trans == "T" else Lt, x, b)
+    bound = c * n * EPS * max(1.0, kappa)
+    assert eta <= bound, (trans, eta, bound)
+    return eta / bound
+
+
+def check_trsm(L, X, B, kappa, c=1.0):
+    """X = L^{-1} B column by column, each within check_trsv's bound; returns the largest error / bound"""
+    return max((check_trsv(L, X[:, j], B[:, j], "N", kappa, c) for j in range(B.shape[1])), default=0.0)
+
+
+def check_gemv(trans, A, w, x, alpha, beta, y0, y):
+    """'T': y = alpha A' (w .* x) + beta y0 with fl(w .* x) formed in fp64 first, like the kernel: a sum of nrows
+    products (nterms = nrows).  'N': y = alpha w .* (A x) + beta y0 with the weight applied after the sum of ncols
+    products, one more rounding (nterms = ncols + 1).  Entrywise (nterms + 2) u (|alpha| |op(A)| |w x| + |beta| |y0|)
+    (check_sums).  beta == 0 ignores y0 (it may be NaN).  Returns error / bound."""
+    nrows, ncols = A.shape
+    AL = A.astype(LD)
+    if trans == "T":
+        xw = x * w if w is not None else x                     # fp64 product, as the kernel forms it
+        ref = LD(alpha) * (AL.T @ xw.astype(LD))
+        mag = abs(LD(alpha)) * (np.abs(AL.T) @ np.abs(xw).astype(LD))
+        nterms = nrows
+    else:
+        wl = w.astype(LD) if w is not None else LD(1)
+        ref = LD(alpha) * wl * (AL @ x.astype(LD))
+        mag = abs(LD(alpha)) * np.abs(wl) * (np.abs(AL) @ np.abs(x).astype(LD))
+        nterms = ncols + 1
+    if beta != 0.0:
+        ref = ref + LD(beta) * y0.astype(LD)
+        mag = mag + abs(LD(beta)) * np.abs(y0).astype(LD)
+    return check_sums(y, ref, mag, nterms)
+
+
+def check_qscale(v, beta, x, y, inverse):
+    """y = W x (inverse False) or W^{-1} x for one second-order cone of order m, W = beta (2 v v' - J), J = diag(1, -1,
+    .., -1), so W x = beta (2 v (v'x) - J x) and W^{-1} x = (1/beta) (2 J v (v' J x) - J x).  x may have several
+    columns (m x xc).
+
+    Bound, per entry i, to first order in u: the kernel forms s = v' (+-x) with an error of at most m u |v|'|x|, t = 2s
+    exactly, fl(v_i t) (one rounding), fl(+-x_i + v_i t) (one), and the product with b = beta or fl(1/beta) (one, and
+    one for fl(1/beta)).  With b the exact beta^{+-1} and M_i = |x_i| + 2 |v_i| |v|'|x|,
+        |y_i - exact_i| <= (m + 4) u b M_i.
+    Returns error / bound."""
+    m = v.shape[0]
+    X = x.reshape(m, -1).astype(LD)
+    vl = v.astype(LD)
+    J = -np.ones(m, dtype=LD)
+    J[0] = 1
+    Jx = X * J[:, None]
+    b = LD(1) / LD(beta) if inverse else LD(beta)
+    if inverse:
+        ref = b * (2 * (J * vl)[:, None] * (vl @ Jx)[None, :] - Jx)
+    else:
+        ref = b * (2 * vl[:, None] * (vl @ X)[None, :] - Jx)
+    mag = np.abs(X) + 2 * np.abs(vl)[:, None] * (np.abs(vl) @ np.abs(X))[None, :]
+    err = np.abs(y.reshape(m, -1).astype(LD) - ref)
+    return check_bound(err, (m + 4) * EPS * abs(b) * mag)

@@ -78,3 +78,39 @@ def test_dims_validation():
         make_dims({"l": 1, "q": [0], "s": []})
     d, keep, cdim, cp = make_dims({"l": 2, "q": [3], "s": [2, 3]})
     assert (cdim, cp) == (2 + 3 + 4 + 9, 2 + 3 + 3 + 6)
+
+
+def test_batched_blocks_check_arguments_before_the_device():
+    """the batched building blocks refuse a batch outside 1..CVXB_BATCH_MAX and an unknown trans with CVXB_E_ARG
+    before they look for a device, and without a GPU fail with CVXB_E_NOGPU, never fall back"""
+    import numpy as np
+    import cvxopt_b200
+    from cvxopt_b200 import _lib
+    lib = _lib.load()
+    a, inv = np.eye(2, order="F"), np.zeros(2 * 128 * 128)
+    x, y = np.ones(2), np.zeros(2)
+    info = np.zeros(1, dtype=np.intc)
+    A, I, X, Y, P = a.ctypes.data, inv.ctypes.data, x.ctypes.data, y.ctypes.data, info.ctypes.data
+    calls = {
+        "potrf": lambda batch, tr: lib.cvxb_potrf_batched(2, A, 2, 4, I, 0, batch, P, 0),
+        "trsv": lambda batch, tr: lib.cvxb_trsv_batched(2, A, 2, 4, I, 0, X, 2, tr, batch, 0),
+        "trsm": lambda batch, tr: lib.cvxb_trsm_batched(2, A, 2, 4, I, 0, A, 2, 4, 2, batch, 0),
+        "syrk": lambda batch, tr: lib.cvxb_syrk_batched(2, 2, A, 2, 4, None, 0, None, 0, 0, A, 2, 4, batch, 0),
+        "gemv": lambda batch, tr: lib.cvxb_gemv_batched(tr, 2, 2, A, 2, 4, None, 0, X, 2, 1.0, 0.0, Y, 2, batch, 0),
+    }
+    for name, call in calls.items():
+        for batch in (0, -1, 65535 + 1):
+            assert call(batch, ord("N")) == _lib.E_ARG, (name, batch)
+            assert "batch" in _lib.last_error(), name
+        if name in ("trsv", "gemv"):
+            assert call(1, ord("X")) == _lib.E_ARG, name
+            assert "trans" in _lib.last_error(), name
+    assert lib.cvxb_potrf_batched(-1, A, 2, 4, I, 0, 1, P, 0) == _lib.E_ARG
+    assert lib.cvxb_gemv_batched(ord("T"), 2, -3, A, 2, 4, None, 0, X, 2, 1.0, 0.0, Y, 2, 1, 0) == _lib.E_ARG
+    assert lib.cvxb_syrk_batched(2, 3, A, 2, 4, None, 0, None, 0, 0, A, 2, 4, 1, 0) == _lib.E_ARG   # lda < k
+    if cvxopt_b200.device_count() > 0:
+        pytest.skip("a GPU is visible")
+    for name, call in calls.items():
+        for batch in (1, 65535):
+            assert call(batch, ord("T")) == _lib.E_NOGPU, (name, batch)
+            assert "no CUDA device available" in _lib.last_error(), name

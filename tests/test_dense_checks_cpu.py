@@ -6,8 +6,8 @@ import pytest
 import scipy.linalg.blas as blas
 import scipy.linalg.lapack as lapack
 
-from ld_check import (backward_error, block_edge_cols, check_gemm, check_lower_only_written, check_potrf,
-                      check_potrs, diag_block_kappa)
+from ld_check import (backward_error, block_edge_cols, check_gemm, check_gemv, check_lower_only_written, check_potrf,
+                      check_potrs, check_qscale, check_trsm, check_trsv, diag_block_kappa)
 
 
 def _spd(n, seed):
@@ -86,3 +86,105 @@ def test_gemm_checker_passes_blas_and_fails_a_perturbed_entry(k):
     Cz[3, 3] = np.nan
     with pytest.raises(AssertionError):
         check_gemm(A, B, 1.0, 0.0, None, Cz)
+
+
+@pytest.mark.parametrize("trans", ["N", "T"])
+def test_trsv_checker_passes_blas_and_fails_a_wrong_solution(trans):
+    n = 300
+    A = _spd(n, 5)
+    L, _ = lapack.dpotrf(A, lower=1, clean=1)
+    kap = diag_block_kappa(L)
+    b = np.random.Generator(np.random.PCG64(6)).standard_normal(n)
+    x = blas.dtrsv(L, b, lower=1, trans=int(trans == "T"))
+    assert check_trsv(L, x, b, trans, kap) < 0.1
+    # the strict upper triangle is not read: garbage there changes nothing
+    assert check_trsv(L + np.triu(np.full((n, n), 1e3), 1), x, b, trans, kap) < 0.1
+    for i in (0, 37, 128, n - 1):
+        xp = x.copy()
+        xp[i] *= 1 + 1e-9
+        with pytest.raises(AssertionError):
+            check_trsv(L, xp, b, trans, kap)
+    # solving with the other triangle is caught
+    with pytest.raises(AssertionError):
+        check_trsv(L, blas.dtrsv(L, b, lower=1, trans=int(trans != "T")), b, trans, kap)
+
+
+def test_trsm_checker_passes_blas_and_fails_a_perturbed_column():
+    n, ncols = 257, 65
+    A = _spd(n, 7)
+    L, _ = lapack.dpotrf(A, lower=1, clean=1)
+    kap = diag_block_kappa(L)
+    B = np.random.Generator(np.random.PCG64(8)).standard_normal((n, ncols))
+    X = blas.dtrsm(1.0, L, B, lower=1)
+    assert check_trsm(L, X, B, kap) < 0.1
+    for i, j in ((0, 0), (130, 31), (n - 1, ncols - 1)):
+        Xp = X.copy()
+        Xp[i, j] *= 1 + 1e-9
+        with pytest.raises(AssertionError):
+            check_trsm(L, Xp, B, kap)
+
+
+def _gemv_ld(trans, A, w, x, alpha, beta, y0):
+    """the exact result rounded once to fp64 (the weighted forms, which BLAS has no call for)"""
+    LD = np.longdouble
+    if trans == "T":
+        xw = x * w if w is not None else x
+        r = LD(alpha) * (A.astype(LD).T @ xw.astype(LD))
+    else:
+        r = LD(alpha) * (w.astype(LD) if w is not None else LD(1)) * (A.astype(LD) @ x.astype(LD))
+    if beta != 0.0:
+        r = r + LD(beta) * y0.astype(LD)
+    return r.astype(np.float64)
+
+
+@pytest.mark.parametrize("weighted", [False, True])
+@pytest.mark.parametrize("trans", ["N", "T"])
+def test_gemv_checker_passes_blas_and_fails_a_perturbed_entry(trans, weighted):
+    rng = np.random.Generator(np.random.PCG64(9 + weighted))
+    nrows, ncols = 129, 65
+    A = rng.standard_normal((nrows, ncols))
+    w = 10.0 ** rng.uniform(-4, 4, nrows) if weighted else None
+    x = rng.standard_normal(nrows if trans == "T" else ncols)
+    y0 = rng.standard_normal(ncols if trans == "T" else nrows)
+    if weighted:
+        y = _gemv_ld(trans, A, w, x, 0.7, -0.3, y0)
+    else:
+        y = blas.dgemv(0.7, A, x, -0.3, y0.copy(), trans=int(trans == "T"))
+    assert check_gemv(trans, A, w, x, 0.7, -0.3, y0, y) < 0.5
+    for i in np.argsort(-np.abs(y))[:3]:                # the largest entries: no cancellation to hide behind
+        yp = y.copy()
+        yp[i] *= 1 + 1e-12
+        with pytest.raises(AssertionError):
+            check_gemv(trans, A, w, x, 0.7, -0.3, y0, yp)
+    # beta = 0: y0 is not read, NaN in it is fine; NaN in the result is not
+    y1 = _gemv_ld(trans, A, w, x, -1.0, 0.0, None)
+    check_gemv(trans, A, w, x, -1.0, 0.0, np.full(y0.size, np.nan), y1)
+    y1[3] = np.nan
+    with pytest.raises(AssertionError):
+        check_gemv(trans, A, w, x, -1.0, 0.0, None, y1)
+
+
+@pytest.mark.parametrize("inverse", [False, True])
+def test_qscale_checker_passes_long_double_and_fails_a_perturbed_entry(inverse):
+    rng = np.random.Generator(np.random.PCG64(11 + inverse))
+    m, xc = 65, 4
+    u = rng.standard_normal(m - 1)
+    v = np.r_[np.sqrt(1.0 + u @ u), u]            # on the hyperboloid v' J v = 1
+    beta = 7.3
+    x = rng.standard_normal((m, xc))
+    LD = np.longdouble
+    J = np.r_[1.0, -np.ones(m - 1)].astype(LD)
+    vl, X = v.astype(LD), x.astype(LD)
+    if inverse:
+        y = ((2 * (J * vl)[:, None] * (vl @ (X * J[:, None]))[None, :] - X * J[:, None]) / LD(beta)).astype(np.float64)
+    else:
+        y = (LD(beta) * (2 * vl[:, None] * (vl @ X)[None, :] - X * J[:, None])).astype(np.float64)
+    assert check_qscale(v, beta, x, y, inverse) < 0.1
+    # W and W^{-1} are inverses: the forward result is not the inverse one
+    with pytest.raises(AssertionError):
+        check_qscale(v, beta, x, y, not inverse)
+    for i, j in ((0, 0), (1, 1), (m - 1, xc - 1)):
+        yp = y.copy()
+        yp[i, j] *= 1 + 1e-12
+        with pytest.raises(AssertionError):
+            check_qscale(v, beta, x, yp, inverse)
