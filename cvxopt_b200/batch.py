@@ -85,21 +85,34 @@ def _stack_eq(A, b, B, n):
     return Acm, np.ascontiguousarray(np.asarray(b, dtype=np.float64)), p
 
 
+def _sdp_dims(dims, m=None):
+    """_batch_dims for SDPBatch: dims may hold 's' blocks"""
+    from . import kkt
+    dims = {"l": dims.get("l", 0), "q": list(dims.get("q", [])), "s": list(dims.get("s", []))}
+    d, keep, cdim, _ = kkt.make_dims(dims)
+    if m is not None and int(m) != cdim:
+        raise TypeError("m = %d does not match the cone dimension %d of dims" % (int(m), cdim))
+    return d, keep, cdim
+
+
 class QPBatch:
     """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
     _lp = False              # ConeLPBatch: a batch of cone LPs
+    _sdp = False             # SDPBatch: cone LPs whose dims may hold 's' blocks
 
     def __init__(self, nprob, n, m, device=0, dims=None, p=0):
         if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
             raise TypeError("p must be an integer")
-        d, keep, cdim = _batch_dims(dims, m)
+        d, keep, cdim = (_sdp_dims if self._sdp else _batch_dims)(dims, m)
         self._lib = _lib.load()
         self._h = C.c_void_p()
         self.B, self.n, self.m, self.p = int(nprob), int(n), int(cdim), int(p)
         if d is None and (self._lp or self.p):
             d, keep, _ = _batch_dims({"l": self.m})
-        if self._lp:
+        if self._sdp:
+            rc = self._lib.cvxb_batch_create_sdp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
+        elif self._lp:
             rc = self._lib.cvxb_batch_create_lp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
         elif self.p:
             rc = self._lib.cvxb_batch_create_eq(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
@@ -375,6 +388,95 @@ def conelp_batch(c, G, h, dims=None, A=None, b=None, device=0, nsub=None, **opti
     options: maxiters, abstol, reltol, feastol, refinement (as conelp's)."""
     B, n, cdim, p = _lp_shapes(c, G, h, dims, A, b)
     return _run_group(ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p), (c, G, h, A, b), options)
+
+
+class SDPBatch(ConeLPBatch):
+    """ConeLPBatch whose dims may hold 's' blocks of order <= 32 (cvxb_batch_create_sdp): B x conelp(c, G, h, dims, A,
+    b) with kktsolver 'chol'.  load() takes conelp's stacked c (B, n), G (B, cdim, n), h (B, cdim), with each 's'
+    block's rows unpacked column-major; only the lower triangle of an 's' block of G and h is read, and results()
+    returns s and z with symmetric 's' blocks."""
+    _sdp = True
+
+    def __init__(self, nprob, n, dims, p=0, device=0):
+        super().__init__(nprob, n, None, device, dims, p)
+
+
+class SDPBatchGroup(ConeLPBatchGroup):
+    """ConeLPBatchGroup of SDPBatch parts"""
+
+    def __init__(self, nprob, n, dims, p=0, device=0, nsub=None):
+        super().__init__(nprob, n, _sdp_dims(dims)[2], device, nsub, dims, p)
+
+    @staticmethod
+    def _part():
+        return lambda nprob, n, m, device, dims, p=0: SDPBatch(nprob, n, dims, p, device)
+
+
+def _sdp_args(c, Gl, hl, Gs, hs, A, b):
+    """sdp's argument checks (coneprog.py:3846-3888) on the batch -> c, G, h, dims, A, b, ms as conelp takes them"""
+    c = np.asarray(c, dtype=np.float64) if c is not None else None
+    if c is None or c.ndim != 2:
+        raise TypeError("'c' must be a dense column matrix")
+    B, n = c.shape
+    if n < 1:
+        raise ValueError("number of variables must be at least 1")
+    Gl = np.zeros((B, 0, n)) if Gl is None else np.asarray(Gl, dtype=np.float64)
+    if Gl.ndim != 3 or Gl.shape[0] != B or Gl.shape[2] != n:
+        raise TypeError("'Gl' must be a dense or sparse 'd' matrix with %d columns" % n)
+    ml = Gl.shape[1]
+    hl = np.zeros((B, 0)) if hl is None else np.asarray(hl, dtype=np.float64)
+    if hl.shape != (B, ml):
+        raise TypeError("'hl' must be a 'd' matrix of size (%d,1)" % ml)
+    Gs = [] if Gs is None else Gs
+    if not isinstance(Gs, list) or [G for G in Gs if np.ndim(G) != 3 or np.shape(G)[0] != B or np.shape(G)[2] != n]:
+        raise TypeError("'Gs' must be a list of sparse or dense 'd' matrices with %d columns" % n)
+    ms = [int(np.sqrt(np.shape(G)[1])) for G in Gs]
+    a = [k for k in range(len(ms)) if ms[k] ** 2 != np.shape(Gs[k])[1]]
+    if a:
+        raise TypeError("the squareroot of the number of rows in 'Gs[%d]' is not an integer" % a[-1])
+    hs = [] if hs is None else hs
+    if not isinstance(hs, list) or len(hs) != len(ms) or [h for h in hs if np.ndim(h) != 3 or np.shape(h)[0] != B]:
+        raise TypeError("'hs' must be a list of %d dense or sparse 'd' matrices" % len(ms))
+    a = [k for k in range(len(ms)) if np.shape(hs[k])[1:] != (ms[k], ms[k])]
+    if a:
+        k = a[0]
+        raise TypeError("hs[%d] has size (%d,%d).  Expected size is (%d,%d)."
+                        % (k, np.shape(hs[k])[1], np.shape(hs[k])[2], ms[k], ms[k]))
+    A = np.zeros((B, 0, n)) if A is None else np.asarray(A, dtype=np.float64)
+    if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n:
+        raise TypeError("'A' must be a dense or sparse 'd' matrix with %d columns" % n)
+    p = A.shape[1]
+    b = np.zeros((B, 0)) if b is None else np.asarray(b, dtype=np.float64)
+    if b.shape != (B, p):
+        raise TypeError("'b' must be a dense matrix of size (%d,1)" % p)
+    G = np.concatenate([Gl] + [np.asarray(G, dtype=np.float64) for G in Gs], axis=1)
+    h = np.concatenate([hl] + [np.asarray(h, dtype=np.float64).transpose(0, 2, 1).reshape(B, -1) for h in hs], axis=1)
+    if p > n or p + ml + sum(k * (k + 1) // 2 for k in ms) < n:
+        raise ValueError("Rank(A) < p or Rank([G; A]) < n")          # conelp, coneprog.py:572-573
+    return c, G, h, {"l": ml, "q": [], "s": ms}, A, b, ms
+
+
+def sdp_batch(c, Gl=None, hl=None, Gs=None, hs=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent SDPs on one GPU, each as solvers.sdp(c, Gl, hl, Gs, hs, A, b, kktsolver='chol') does.
+    c (B, n), Gl (B, ml, n), hl (B, ml), Gs a list of (B, ms², n), hs a list of (B, ms, ms), A (B, p, n), b (B, p);
+    every 's' order at most 32.  Returns sdp's keys x, sl, ss (list of (B, ms, ms)), y, zl, zs, status, status_code,
+    iterations, primal objective, dual objective, with conelp_batch's stats; NaN where sdp returns None.
+    options: maxiters, abstol, reltol, feastol, refinement (as sdp's)."""
+    c, G, h, dims, A, b, ms = _sdp_args(c, Gl, hl, Gs, hs, A, b)
+    B, n = c.shape
+    p = A.shape[1]
+    out = _run_group(SDPBatchGroup(B, n, dims, p, device, nsub), (c, G, h, A if p else None, b if p else None),
+                     options)
+    ml = dims["l"]
+    for key in ("s", "z"):
+        v = out.pop(key)
+        out[key + "l"] = v[:, :ml]
+        blocks, o = [], ml
+        for k in ms:
+            blocks.append(v[:, o:o + k * k].reshape(B, k, k).transpose(0, 2, 1).copy())
+            o += k * k
+        out[key + "s"] = blocks
+    return out
 
 
 def _run_group(grp, data, options):

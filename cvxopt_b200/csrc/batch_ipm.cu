@@ -55,6 +55,15 @@ struct Ptrs {
     // cone LP batches (cvxb_batch_create_lp): q holds c; lps is the LPScal at the end of a slot's state row;
     // x1 (n), y1 (p), z1 and th (m) are rebuilt every iteration
     double *lps, *x1, *y1, *z1, *th;
+    // 's' blocks (cvxb_batch_create_sdp; cone LP batches only).  Rows [mlq, m) of the m-vectors are the blocks,
+    // unpacked (ms² rows each, column-major); bzp, th, z1 and Gs hold them packed in rows [mlq, mpk).  rw: the sdot
+    // weight of each m-row (1 'l' / 'q' rows and diagonals, 2 strict lower, 0 strict upper); u2p: for each 's' row,
+    // its packed row minus mlq.  sinfo: per block ms, unpacked row, packed row, offset in r / rti, offset in sigs.
+    // r, rti, sigs and sigz are in the state row; spart holds 4 per-(slot, block) partial results of the block kernels
+    int ns, mlq, mpk, mdg;
+    const int *sinfo, *u2p;
+    const double *rw;
+    double *sr, *srti, *sigs, *sigz, *spart;
 };
 // per-problem scalars of conelp's self-dual embedding (coneprog.py:847, :1031-1047), in the state row so that they
 // move with their slot
@@ -82,9 +91,19 @@ __device__ __forceinline__ LPScal &lp_scal(const Ptrs &p, long long oc) {
 
 // starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2055-2080): d = di = 1,
 // v = e1 and beta = 1 for each cone.  EQ: y = b (the solve overwrites it, :2078-2081), aw = 0 (no A'A in S yet)
-template <bool EQ> __global__ void k_init_rhs(Ptrs p) {
+template <bool EQ, bool SDP = false> __global__ void k_init_rhs(Ptrs p) {
     PB_SETUP
     double nq = 0, nh = 0, nb = 0;
+    if (SDP) {                                           // W = I: r = rti = I; snrm2(h) weighs the 's' rows
+        for (int i = tid; i < p.m; i += nt) { const double v = p.h[om + i]; nh += p.rw[i] * v * v; }
+        for (int k = 0; k < p.ns; ++k) {
+            const int ms = p.sinfo[5 * k], ro = p.sinfo[5 * k + 3];
+            for (int e = tid; e < ms * ms; e += nt) {
+                const double v = (e % ms == e / ms) ? 1.0 : 0.0;
+                p.sr[oc + ro + e] = v; p.srti[oc + ro + e] = v;
+            }
+        }
+    }
     if (EQ) for (int i = tid; i < p.neq; i += nt) {
         const double v = p.beq[oq + i];
         p.y[oq + i] = v; p.aw[oq + i] = 0.0;
@@ -95,7 +114,7 @@ template <bool EQ> __global__ void k_init_rhs(Ptrs p) {
         double v = p.h[om + i];
         p.dz[om + i] = v;
         p.d[om + i] = 1.0; p.di[om + i] = 1.0; p.di2[om + i] = 1.0;
-        nh += v * v;
+        if (!SDP) nh += v * v;
     }
     double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) {
@@ -287,7 +306,7 @@ __global__ void k_build_gs(Ptrs p, const double *G, double *Gs, long long ldg, l
 // NT scaling at iteration 0 (misc.py:284-352), lambda o lambda (misc.py:945-959), mu (coneprog.py:2357).
 // di2 = di² is the SYRK's weight when W^{-T} G is not formed.  LP: conelp's dg, dgi and lmbdag at iteration 0, its
 // lmbdasq[-1] and mu = ||lmbda||² / (1 + cdim) (coneprog.py:1031-1047, :1248)
-template <bool CONES, bool LP = false> __global__ void k_scaling(Ptrs p, int first) {
+template <bool CONES, bool LP = false, bool SDP = false> __global__ void k_scaling(Ptrs p, int first) {
     PB_SETUP
     if (S.done) return;
     double *l = p.lmbda + om, *lsq = p.lmbdasq + om;
@@ -318,13 +337,16 @@ template <bool CONES, bool LP = false> __global__ void k_scaling(Ptrs p, int fir
         FOR_LANE(i, len) lsq[o + i] = (i == 0) ? nl : 2.0 * l0 * l[o + i];
         if (LP && lane == 0) ll += nl;
     }
+    // 's' blocks: lambda (k_s_nt_compute / k_s_update) on the diagonal rows, lmbdasq = lambda² there, 0 elsewhere
+    if (SDP) for (int i = p.mlq + tid; i < p.m; i += nt)
+        if (p.rw[i] == 1.0) { const double li2 = l[i] * l[i]; lsq[i] = li2; ll += li2; }
     if (LP) {
         ll = block_sum(ll, sh);
         if (tid == 0) {
             LPScal &T = lp_scal(p, oc);
             if (first) { T.dg = sqrt(T.kappa / T.tau); T.dgi = sqrt(T.tau / T.kappa); T.lg = sqrt(T.tau * T.kappa); }
             T.lgsq = T.lg * T.lg;
-            S.mu = (ll + T.lgsq) / (1.0 + p.m); S.sigma = 0.0;
+            S.mu = (ll + T.lgsq) / (1.0 + (SDP ? p.mdg : p.m)); S.sigma = 0.0;
         }
     } else if (tid == 0) { S.mu = S.gap / (p.ml + p.nq); S.sigma = 0.0; S.eta = 0.0; }
 }
@@ -362,7 +384,7 @@ __device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double
 // solve (:1154-1165): y := -y, and f4_no_ir's cone steps on (-bz, -bs).  That is coneqp's right-hand side with
 // c = -1 + sigma and sigma mu in the corrector (i = 1) only; dx = -c rx keeps conelp's sign.  Negation is exact, so this
 // is the reference's arithmetic.  Then dtau = (1 - sigma) rt and dkappa.
-template <bool CONES, bool EQ, bool LP> __global__ void k_dir_rhs(Ptrs p, int i) {
+template <bool CONES, bool EQ, bool LP, bool SDP = false> __global__ void k_dir_rhs(Ptrs p, int i) {
     PB_SETUP
     const double sm = S.sigma * S.mu, c = -1.0 + (LP ? S.sigma : S.eta);
     const bool add_sm = !LP || i == 1;
@@ -393,8 +415,13 @@ template <bool CONES, bool EQ, bool LP> __global__ void k_dir_rhs(Ptrs p, int i)
         f4_pre_row(p, om + k, z, s);
         p.dz[om + k] = z; p.ds[om + k] = s;
     }
+    if (SDP) for (int k = p.mlq + tid; k < p.m; k += nt) {   // e is the identity: sigma mu on the diagonal rows
+        double z, s;
+        rhs(k, p.rw[k] == 1.0, z, s);
+        p.dz[om + k] = z; p.ds[om + k] = s;
+    }
     if (CONES) {
-        for (int k = p.ml + tid; k < p.m; k += nt) {
+        for (int k = p.ml + tid; k < (SDP ? p.mlq : p.m); k += nt) {
             double z, s;
             rhs(k, false, z, s);
             p.dz[om + k] = z; p.ds[om + k] = s;
@@ -442,7 +469,7 @@ __global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long 
 // wz2 = wz - W' ds, ws2 = ws - lmbda o (dz + ds); EQ: wy2 = wy.  The P, A, A', G and G' products follow as
 // batched GEMVs.  LP: conelp's res() (:599-631) adds the embedding's column ut (-c, b, h), ut = dtau / dg, to
 // (wx2, wy2, wz2), and forms wtau2 = wtau + dg dkappa + c'dx + b'dy + h'wz3, wkappa2 = wkappa + lmbdag (dtau + dkappa).
-template <bool EQ, bool LP> __global__ void k_res(Ptrs p) {
+template <bool EQ, bool LP, bool SDP = false> __global__ void k_res(Ptrs p) {
     PB_SETUP
     const double *l = p.lmbda + om, *dz = p.dz + om, *ds = p.ds + om, *h = p.h + om;
     const double ut = LP ? lp_scal(p, oc).dtau / lp_scal(p, oc).dg : 0.0;
@@ -490,6 +517,7 @@ template <bool EQ, bool LP> __global__ void k_res(Ptrs p) {
         if (EQ) by = block_sum(by, sh);
         if (tid == 0) {
             LPScal &T = lp_scal(p, oc);
+            if (SDP) for (int k = 0; k < p.ns; ++k) hz += p.spart[((long long)b * p.ns + k) * 4];   // k_s_res's h'wz3
             T.wtau2 = T.wtau + (T.dg * T.dkappa + cx + by + hz);
             T.wkappa2 = T.wkappa + T.lg * (T.dtau + T.dkappa);
         }
@@ -498,7 +526,7 @@ template <bool EQ, bool LP> __global__ void k_res(Ptrs p) {
 // after the i-th direction: ds o dz, scale2 of ds and dz, step length, sigma (coneprog.py:2423-2456).
 // f4_post: the solve has just run without refinement, so f4_no_ir's step after it is done here first.
 // LP: conelp's dkappa dtau product, tt and tk in the step, sigma = (1 - step)^3 (coneprog.py:1302-1333)
-template <bool CONES, bool LP = false> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
+template <bool CONES, bool LP = false, bool SDP = false> __global__ void k_dir_post(Ptrs p, int i, int f4_post) {
     PB_SETUP
     double *ds = p.ds + om, *dz = p.dz + om;
     const double *l = p.lmbda + om;
@@ -531,6 +559,10 @@ template <bool CONES, bool LP = false> __global__ void k_dir_post(Ptrs p, int i,
     mins = block_min(mins, sh);
     minz = block_min(minz, sh);
     if (tid == 0) {
+        if (SDP) for (int k = 0; k < p.ns; ++k) {        // k_s_dir_post: sdot(ds, dz) and the smallest eigenvalues
+            const double *q = p.spart + ((long long)b * p.ns + k) * 4;
+            dsdz += q[0]; mins = fmin(mins, q[1]); minz = fmin(minz, q[2]);
+        }
         double t = fmax(0.0, fmax(-mins, -minz));
         if (LP) {
             LPScal &T = lp_scal(p, oc);
@@ -556,10 +588,13 @@ template <bool CONES, bool LP = false> __global__ void k_dir_post(Ptrs p, int i,
 // z = W^{-1} lmbda; gap (coneprog.py:2459-2547).  EQ: y += step dy (:2460); a singular Kp stops the problem too.
 // LP: conelp's dg, lmbdag, tau, kappa and gap (coneprog.py:1405-1436); a singular factorisation returns the iterate
 // divided by tau (:1078-1109)
-template <bool CONES, bool EQ, bool LP = false> __global__ void k_update(Ptrs p, const int *info, int iter) {
+template <bool CONES, bool EQ, bool LP = false, bool SDP = false>
+__global__ void k_update(Ptrs p, const int *info, int iter) {
     PB_SETUP
     if (S.done) return;
-    if (info[b] > 0 || (EQ && p.infop[b] > 0)) {   // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
+    bool fail = false;                               // SDP: a block's Jacobi SVD did not converge (k_s_update)
+    if (SDP) for (int k = 0; k < p.ns; ++k) fail |= p.spart[((long long)b * p.ns + k) * 4 + 3] != 0.0;
+    if (fail || info[b] > 0 || (EQ && p.infop[b] > 0)) {   // non-positive pivot: "Terminated (singular KKT matrix)" (:2257-2275)
         if (LP) {
             const double ti = 1.0 / lp_scal(p, oc).tau;
             for (int k = tid; k < p.n; k += nt) p.x[on + k] *= ti;
@@ -607,6 +642,18 @@ template <bool CONES, bool EQ, bool LP = false> __global__ void k_update(Ptrs p,
         g = warp_sum(g);
         if (lane == 0) gap += g;
     }
+    if (SDP) {                                       // commit what k_s_update staged (every block succeeded)
+        for (int k = p.mlq + tid; k < p.m; k += nt) {
+            s[k] = ds[k]; z[k] = dz[k];
+            if (p.rw[k] == 1.0) { const double lk = p.lmbdasq[om + k]; l[k] = lk; gap += lk * lk; }
+        }
+        for (int k = 0; k < p.ns; ++k) {
+            const int ms = p.sinfo[5 * k], so = p.sinfo[5 * k + 1], ro = p.sinfo[5 * k + 3];
+            for (int e = tid; e < ms * ms; e += nt) {
+                p.sr[oc + ro + e] = p.d[om + so + e]; p.srti[oc + ro + e] = p.di[om + so + e];
+            }
+        }
+    }
     gap = block_sum(gap, sh);
     if (LP) {
         if (tid == 0) {
@@ -633,20 +680,43 @@ __global__ void k_switch(double *aw, const int *info, int neq) {
 // step length and the update are coneqp's kernels with LP = true.
 // The primal start's solve has left uz in bzp: s = -uz (:698-701).  The dual start's right-hand side (-c, 0, 0):
 // k_init_rhs put -c in dx, here y = 0 and bz = 0 (:724-728)
-template <bool EQ> __global__ void k_lp_start_mid(Ptrs p) {
+// value of m-row i (an 's' row when i >= mlq) of a vector whose 's' blocks are packed (bzp, z1)
+__device__ __forceinline__ double unpacked(const Ptrs &p, const double *x, int i) {
+    return i < p.mlq ? x[i] : x[p.mlq + p.u2p[i - p.mlq]] * (p.rw[i] == 1.0 ? 1.0 : M_SQRT1_2);
+}
+template <bool EQ, bool SDP = false> __global__ void k_lp_start_mid(Ptrs p) {
     PB_SETUP
+    if (SDP) {
+        for (int i = tid; i < p.m; i += nt) p.s[om + i] = -unpacked(p, p.bzp + om, i);
+        __syncthreads();
+        for (int i = tid; i < p.mpk; i += nt) p.bzp[om + i] = 0.0;
+    } else
     for (int i = tid; i < p.m; i += nt) { p.s[om + i] = -p.bzp[om + i]; p.bzp[om + i] = 0.0; }
     if (EQ) for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = 0.0;
 }
 // the starting point (:737-857): z from the dual start's solve, ts / tz, the "already optimal" return at iteration 0
 // (:744-804), the shifts by 1 + ts and 1 + tz, tau = kappa = 1, gap
-template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double abstol, double reltol) {
+template <bool CONES, bool EQ, bool SDP = false> __global__ void k_lp_init_point(Ptrs p, double abstol, double reltol) {
     PB_SETUP
     double *s = p.s + om, *z = p.z + om;
     const double *zn = p.bzp + om, *h = p.h + om;
     double ns = 0, nz = 0, sz = 0, cx = 0, by = 0, hz = 0, mins = INFINITY, minz = INFINITY;
     for (int i = tid; i < p.n; i += nt) cx += p.q[on + i] * p.x[on + i];
     if (EQ) for (int i = tid; i < p.neq; i += nt) by += p.beq[oq + i] * p.y[oq + i];
+    if (SDP) {
+        // z unpacked from the solve's bzp; snrm2 / sdot weigh the 's' rows; the blocks' smallest eigenvalues come
+        // from k_s_eig_start
+        for (int i = tid; i < p.m; i += nt) {
+            const double zv = unpacked(p, zn, i), sv = s[i], w = p.rw[i];
+            z[i] = zv;
+            ns += w * sv * sv; nz += w * zv * zv; sz += w * sv * zv; hz += w * h[i] * zv;
+            if (i < p.ml) { mins = fmin(mins, sv); minz = fmin(minz, zv); }
+        }
+        if (tid == 0) for (int k = 0; k < p.ns; ++k) {
+            const double *q = p.spart + ((long long)b * p.ns + k) * 4;
+            mins = fmin(mins, q[1]); minz = fmin(minz, q[2]);
+        }
+    } else
     for (int i = tid; i < p.m; i += nt) {
         const double zv = zn[i], sv = s[i];
         z[i] = zv;
@@ -675,9 +745,10 @@ template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double ab
     const double az = (tz >= -1e-8 * fmax(nz, 1.0)) ? 1.0 + tz : 0.0;
     for (int i = tid; i < p.ml; i += nt) { s[i] += as; z[i] += az; }
     if (CONES) for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
+    if (SDP) for (int i = p.mlq + tid; i < p.m; i += nt) if (p.rw[i] == 1.0) { s[i] += as; z[i] += az; }
     __syncthreads();
     double gap = 0;
-    for (int i = tid; i < p.m; i += nt) gap += s[i] * z[i];
+    for (int i = tid; i < p.m; i += nt) gap += (SDP ? p.rw[i] : 1.0) * s[i] * z[i];
     gap = block_sum(gap, sh);
     if (tid == 0) {
         S.gap = gap;
@@ -689,8 +760,9 @@ template <bool CONES, bool EQ> __global__ void k_lp_init_point(Ptrs p, double ab
 // optimal or maxiters divide the iterate by tau; a primal infeasibility certificate divides y and z by -h'z - b'y
 // and x, s become NaN (the reference's None); a dual infeasibility certificate divides x and s by -c'x and y, z
 // become NaN.  Status 4 primal infeasible, 5 dual infeasible.
-template <bool EQ> __global__ void k_lp_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol,
-                                              double feastol, int *ndone, int *doneflags) {
+template <bool EQ, bool SDP = false>
+__global__ void k_lp_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol, double feastol, int *ndone,
+                           int *doneflags) {
     PB_SETUP
     __shared__ int act;
     __shared__ double fac;
@@ -711,7 +783,8 @@ template <bool EQ> __global__ void k_lp_stats(Ptrs p, int iter, int maxiters, do
         for (int i = tid; i < p.m; i += nt) {
             const double v = p.rz[om + i], hh = p.h[om + i], r = v + (-tau) * hh;
             p.rz[om + i] = r;
-            hzz += v * v; rz2 += r * r; hz += hh * p.z[om + i];
+            if (SDP) { const double w = p.rw[i]; hzz += w * v * v; rz2 += w * r * r; hz += w * hh * p.z[om + i]; }
+            else { hzz += v * v; rz2 += r * r; hz += hh * p.z[om + i]; }
         }
         hx = block_sum(hx, sh); rx2 = block_sum(rx2, sh); cx = block_sum(cx, sh);
         hzz = block_sum(hzz, sh); rz2 = block_sum(rz2, sh); hz = block_sum(hz, sh);
@@ -771,13 +844,14 @@ template <bool EQ> __global__ void k_lp_x1_rhs(Ptrs p) {
     }
 }
 // (x1, y1, z1) *= dgi (:1075-1077); z1'z1 for f6_no_ir
-template <bool EQ> __global__ void k_lp_x1_post(Ptrs p) {
+template <bool EQ, bool SDP = false> __global__ void k_lp_x1_post(Ptrs p) {
     PB_SETUP
     const double dgi = lp_scal(p, oc).dgi;
     for (int i = tid; i < p.n; i += nt) p.x1[on + i] *= dgi;
     if (EQ) for (int i = tid; i < p.neq; i += nt) p.y1[oq + i] *= dgi;
     double a = 0;
-    for (int i = tid; i < p.m; i += nt) { const double v = dgi * p.bzp[om + i]; p.z1[om + i] = v; a += v * v; }
+    // SDP: z1 stays packed, so z1'z1 is its sdot
+    for (int i = tid; i < (SDP ? p.mpk : p.m); i += nt) { const double v = dgi * p.bzp[om + i]; p.z1[om + i] = v; a += v * v; }
     a = block_sum(a, sh);
     if (tid == 0) lp_scal(p, oc).z1sq = a;
 }
@@ -785,8 +859,8 @@ template <bool EQ> __global__ void k_lp_x1_post(Ptrs p) {
 // tau := dgi (btau - bkappa / tau + c'x + b'y + th'uz) / (1 + z1'z1), (x, y, z) += tau (x1, y1, z1), s := s - z,
 // kappa -= tau.  acc = 0: the Newton solve, in place on (dx, dy, ds), z to dz, (btau, bkappa) = (dtau, dkappa).
 // acc = 1: a refinement step on (wx2, wy2, ws2) with (wtau2, wkappa2), added to the direction (:1230-1235).
-template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx, double *y, long long sy, double *s,
-                                                long long ss, int acc) {
+template <bool EQ, bool SDP = false>
+__global__ void k_lp_f6_post(Ptrs p, double *x, long long sx, double *y, long long sy, double *s, long long ss, int acc) {
     PB_SETUP
     LPScal &T = lp_scal(p, oc);
     x += b * sx; s += b * ss;
@@ -796,7 +870,7 @@ template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx,
     double cx = 0, by = 0, tz = 0;
     for (int i = tid; i < p.n; i += nt) cx += c[i] * x[i];
     if (EQ) for (int i = tid; i < p.neq; i += nt) by += p.beq[oq + i] * y[i];
-    for (int i = tid; i < p.m; i += nt) tz += th[i] * uz[i];
+    for (int i = tid; i < (SDP ? p.mpk : p.m); i += nt) tz += th[i] * uz[i];   // SDP: packed, sdot(th, uz)
     cx = block_sum(cx, sh); tz = block_sum(tz, sh);
     if (EQ) by = block_sum(by, sh);
     double kap = -kin / T.lg;
@@ -811,7 +885,7 @@ template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx,
         if (acc) p.dy[oq + i] += v; else y[i] = v;
     }
     for (int i = tid; i < p.m; i += nt) {
-        const double zv = uz[i] + tau * z1[i], sv = s[i] - zv;
+        const double zv = SDP ? unpacked(p, uz, i) + tau * unpacked(p, z1, i) : uz[i] + tau * z1[i], sv = s[i] - zv;
         if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
         else { p.dz[om + i] = zv; s[i] = sv; }
     }
@@ -820,6 +894,322 @@ template <bool EQ> __global__ void k_lp_f6_post(Ptrs p, double *x, long long sx,
         if (acc) { T.dtau += tau; T.dkappa += kap; }
         else { T.dtau = tau; T.dkappa = kap; }
     }
+}
+
+// ---- 's' blocks: one CTA of SB_T threads per (block, slot), grid (ns, Bact) ----
+// A block of order ms <= CVXB_BATCH_SMAX is an ms x ms column-major matrix in shared memory.  The kernels read only
+// the lower triangle of what they are given (the reference reads no more, misc_solvers.c scale / sdot), and write
+// s, z, ds, dz and the refinement vectors with both triangles.  Per-block partial sums go to spart; the per-problem
+// kernels add them up in block order.
+constexpr int SB_T = 256, SMX = CVXB_BATCH_SMAX * CVXB_BATCH_SMAX, JAC_SWEEPS = 30;
+#define SB_SETUP                                                                                       \
+    const int k = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;                                       \
+    const int ms = p.sinfo[5 * k], so = p.sinfo[5 * k + 1], sp = p.sinfo[5 * k + 2];                   \
+    const int sro = p.sinfo[5 * k + 3], sgo = p.sinfo[5 * k + 4];                                      \
+    const long long om = (long long)b * p.m, oc = (long long)b * p.L;                                  \
+    Scal &S = p.sc[b];                                                                                 \
+    (void)tid; (void)sp; (void)sro; (void)sgo; (void)om; (void)oc; (void)S;
+#define SB_PART double *part = p.spart + ((long long)b * p.ns + k) * 4
+#define SB_FOR(e, ms) for (int e = threadIdx.x; e < (ms) * (ms); e += SB_T)
+
+// X := sym(lower triangle of the column-major block x)
+__device__ void s_load(double *X, const double *x, int ms) {
+    SB_FOR(e, ms) { const int i = e % ms, j = e / ms; X[e] = i >= j ? x[e] : x[j + i * ms]; }
+    __syncthreads();
+}
+// X := the block unpacked from packed storage with sqrt(2) off-diagonals (misc.unpack)
+__device__ void s_load_packed(double *X, const double *x, int ms) {
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms, c = min(i, j), r = max(i, j);
+        const double v = x[c * ms - c * (c - 1) / 2 + r - c];
+        X[e] = i == j ? v : v * M_SQRT1_2;
+    }
+    __syncthreads();
+}
+// packed storage of X's lower triangle, off-diagonals times sqrt(2) (misc.pack / pack2)
+__device__ void s_store_packed(double *x, const double *X, int ms) {
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms;
+        if (i >= j) x[j * ms - j * (j - 1) / 2 + i - j] = i == j ? X[e] : M_SQRT2 * X[e];
+    }
+}
+// C := op(A) op(B).  The lanes of a warp take consecutive rows i.  With ta they would read A' at a stride of ms
+// doubles, all in one bank when ms = 32, so each lane starts its sum at l = i (mod ms); it is never called with ta and
+// tb both set, where that would move the conflict onto B.
+__device__ void s_mm(double *C, const double *A, bool ta, const double *B, bool tb, int ms) {
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms;
+        double a = 0.0;
+        int l = ta ? i : 0;
+        for (int c = 0; c < ms; ++c, l = (l + 1 == ms) ? 0 : l + 1)
+            a += (ta ? A[l + i * ms] : A[i + l * ms]) * (tb ? B[j + l * ms] : B[l + j * ms]);
+        C[e] = a;
+    }
+    __syncthreads();
+}
+// C := A' X A (tr = true) or A X A' for symmetric X; T is scratch
+__device__ void s_congr(double *C, const double *A, const double *X, double *T, bool tr, int ms) {
+    s_mm(T, X, false, A, !tr, ms);
+    s_mm(C, A, tr, T, false, ms);
+}
+// sdot's share of one block: diagonal once, strict lower triangle twice
+__device__ double s_dot(const double *X, const double *Y, int ms, double *sh) {
+    double a = 0.0;
+    SB_FOR(e, ms) { const int i = e % ms, j = e / ms; if (i >= j) a += (i == j ? 1.0 : 2.0) * X[e] * Y[e]; }
+    return block_sum(a, sh);
+}
+// in-CTA Cholesky X = L L' (lower, upper triangle zeroed); false for a non-positive pivot
+__device__ bool s_chol(double *X, int ms) {
+    __shared__ int ok;
+    __syncthreads();                                  // every thread has read the previous call's ok
+    if (threadIdx.x == 0) ok = 1;
+    for (int j = 0; j < ms; ++j) {
+        __syncthreads();
+        if (threadIdx.x == 0) { const double d = X[j + j * ms]; if (!(d > 0.0)) ok = 0; X[j + j * ms] = sqrt(d); }
+        __syncthreads();
+        for (int i = j + 1 + threadIdx.x; i < ms; i += SB_T) X[i + j * ms] /= X[j + j * ms];
+        __syncthreads();
+        for (int e = threadIdx.x; e < ms * ms; e += SB_T) {
+            const int i = e % ms, c = e / ms;
+            if (c > j && i >= c) X[e] -= X[i + j * ms] * X[c + j * ms];
+        }
+    }
+    __syncthreads();
+    SB_FOR(e, ms) if (e % ms < e / ms) X[e] = 0.0;
+    __syncthreads();
+    return ok;
+}
+// SVD A = U diag(sig) V' of the block in A by cone.cuh's one-sided Jacobi (A := U, one warp per column pair, a column
+// one element per lane); false when the sweeps ran out or a singular value is not positive
+__device__ bool s_svd(double *A, double *V, double *sig, int ms) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    SB_FOR(e, ms) V[e] = (e % ms == e / ms) ? 1.0 : 0.0;
+    __syncthreads();
+    __shared__ int rot;
+    const bool conv = jacobi_svd_cta(ms, A, V, JAC_SWEEPS, rot);
+    __shared__ int ok;
+    if (threadIdx.x == 0) ok = conv;
+    __syncthreads();
+    for (int j = warp; j < ms; j += SB_T / 32) {
+        const double x = lane < ms ? A[j * ms + lane] : 0.0, nrm = sqrt(warp_sum(x * x));
+        if (lane < ms) A[j * ms + lane] = x / nrm;
+        if (lane == 0) { sig[j] = nrm; if (!(nrm > 0.0)) ok = 0; }
+    }
+    __syncthreads();
+    return ok;
+}
+// eigendecomposition of the symmetric block in A = V diag(ev) V' by cone.cuh's two-sided Jacobi (jac_eig_cta, with
+// jac_small_kernel's convergence rule); W is its second buffer, A and W are overwritten; false when the sweeps ran out
+__device__ bool s_eig(double *A, double *W, double *V, double *ev, int ms, double *sh) {
+    SB_FOR(e, ms) V[e] = (e % ms == e / ms) ? 1.0 : 0.0;
+    __syncthreads();
+    double *w0 = A, *w1 = W;
+    const bool ok = jac_eig_cta<true>(w0, w1, V, ms, JAC_SWEEPS, sh, threadIdx.x, SB_T);
+    for (int i = threadIdx.x; i < ms; i += SB_T) ev[i] = w0[i + i * ms];
+    __syncthreads();
+    return ok;
+}
+__device__ double s_min(const double *ev, int ms) {
+    double t = INFINITY;
+    for (int i = 0; i < ms; ++i) t = fmin(t, ev[i]);
+    return t;
+}
+// write X (both triangles) to x
+__device__ void s_store(double *x, const double *X, int ms) { SB_FOR(e, ms) x[e] = X[e]; }
+__device__ __forceinline__ double s_lam(const Ptrs &p, long long om, int so, int ms, int i) {
+    return p.lmbda[om + so + i * (ms + 1)];
+}
+
+// bzp := pack(W^{-T} z) = pack(rti' z rti) (mode 0; mode 1 also th := bzp, the x1 solve's W^{-T} h), or f4_no_ir's
+// steps before the solve (mode 2): s := lmbda o\ s, z := z - W' s = z - r s r', bzp := pack(rti' z rti) (misc.py
+// :1305-1307, coneprog.py :1154-1165).  z and s of slot b at z + b*sz, s + b*ss.
+__global__ void __launch_bounds__(SB_T) k_s_wtz(Ptrs p, const double *z, long long sz, double *s, long long ss,
+                                                int mode) {
+    SB_SETUP
+    __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX];
+    s_load(X, z + b * sz + so, ms);
+    if (mode == 2) {
+        double *sb = s + b * ss + so;
+        s_load(Y, sb, ms);
+        SB_FOR(e, ms) Y[e] /= 0.5 * (s_lam(p, om, so, ms, e % ms) + s_lam(p, om, so, ms, e / ms));
+        __syncthreads();
+        s_store(sb, Y, ms);
+        SB_FOR(e, ms) R[e] = p.sr[oc + sro + e];
+        __syncthreads();
+        s_mm(T, Y, false, R, true, ms);
+        s_mm(Y, R, false, T, false, ms);              // Y := r s r'
+        SB_FOR(e, ms) X[e] -= Y[e];
+        __syncthreads();
+    }
+    SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+    __syncthreads();
+    s_congr(Y, R, X, T, true, ms);
+    s_store_packed(p.bzp + om + sp, Y, ms);
+    if (mode == 1) s_store_packed(p.th + om + sp, Y, ms);
+}
+// Gs = pack(W^{-T} G) for the 's' rows (misc.py:1267-1272): column j of Gs is pack(rti' mat(g_j) rti); grid.z
+// splits the columns
+__global__ void __launch_bounds__(SB_T) k_s_build_gs(Ptrs p, const double *G, double *Gs, long long ldg, long long sG) {
+    SB_SETUP
+    __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX];
+    SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+    __syncthreads();
+    const int per = (p.n + gridDim.z - 1) / gridDim.z, j0 = blockIdx.z * per, j1 = min(p.n, j0 + per);
+    for (int j = j0; j < j1; ++j) {
+        const long long off = (long long)b * sG + (long long)j * ldg;
+        s_load(X, G + off + so, ms);
+        s_congr(Y, R, X, T, true, ms);
+        s_store_packed(Gs + off + sp, Y, ms);
+        __syncthreads();
+    }
+}
+// NT scaling at iteration 0 (misc.py:374-417): s = Ls Ls', z = Lz Lz', Lz' Ls = U diag(lambda) V',
+// r = Lz^{-T} U diag(lambda)^{1/2}, rti = Lz U diag(lambda)^{-1/2}.  part[3] = 1 when a factorisation failed.
+__global__ void __launch_bounds__(SB_T) k_s_nt_compute(Ptrs p) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double Ls[SMX], Lz[SMX], U[SMX], V[SMX], lam[CVXB_BATCH_SMAX];
+    if (S.done) return;
+    s_load(Ls, p.s + om + so, ms);
+    s_load(Lz, p.z + om + so, ms);
+    bool ok = s_chol(Ls, ms);
+    ok = s_chol(Lz, ms) && ok;
+    s_mm(U, Lz, true, Ls, false, ms);
+    ok = s_svd(U, V, lam, ms) && ok;
+    // V := Lz^{-T} U (one column per thread), Ls := Lz U
+    for (int c = threadIdx.x; c < ms; c += SB_T)
+        for (int i = ms - 1; i >= 0; --i) {
+            double a = U[i + c * ms];
+            for (int l = i + 1; l < ms; ++l) a -= Lz[l + i * ms] * V[l + c * ms];
+            V[i + c * ms] = a / Lz[i + i * ms];
+        }
+    __syncthreads();
+    s_mm(Ls, Lz, false, U, false, ms);
+    SB_FOR(e, ms) {
+        const double a = sqrt(lam[e / ms]);
+        p.sr[oc + sro + e] = V[e] * a;
+        p.srti[oc + sro + e] = Ls[e] * (1.0 / a);
+    }
+    for (int i = threadIdx.x; i < ms; i += SB_T) p.lmbda[om + so + i * (ms + 1)] = ok ? lam[i] : NAN;
+    if (tid == 0) part[3] = ok ? 0.0 : 1.0;        // a failed Cholesky or SVD stops the problem (k_update)
+}
+// the starting point's smallest eigenvalues (misc.max_step, coneprog.py:707, :737): s (unpacked), z (bzp, packed)
+__global__ void __launch_bounds__(SB_T) k_s_eig_start(Ptrs p) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double A[SMX], W[SMX], V[SMX], ev[CVXB_BATCH_SMAX], sh[32];
+    s_load(A, p.s + om + so, ms);
+    const bool ok1 = s_eig(A, W, V, ev, ms, sh);
+    const double m1 = s_min(ev, ms);
+    s_load_packed(A, p.bzp + om + sp, ms);
+    const bool ok2 = s_eig(A, W, V, ev, ms, sh);
+    if (tid == 0) { part[1] = ok1 ? m1 : NAN; part[2] = ok2 ? s_min(ev, ms) : NAN; }
+}
+// the 's' rows of the refinement residual res() (coneprog.py:599-631): wz3 = W^{-1} dz = rti dz rti',
+// wz2 = wz + ut h - W' ds = wz + ut h - r ds r', ws2 = ws - lmbda o (dz + ds); part[0] = sdot(h, wz3)
+__global__ void __launch_bounds__(SB_T) k_s_res(Ptrs p) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX], H[SMX], sh[32];
+    const double ut = lp_scal(p, oc).dtau / lp_scal(p, oc).dg;
+    s_load(X, p.dz + om + so, ms);
+    s_load(H, p.h + om + so, ms);
+    SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+    __syncthreads();
+    s_congr(Y, R, X, T, false, ms);
+    s_store(p.wz3 + oc + so, Y, ms);
+    const double hz = s_dot(H, Y, ms, sh);
+    s_load(Y, p.ds + om + so, ms);
+    SB_FOR(e, ms) { R[e] = p.sr[oc + sro + e]; X[e] += Y[e]; }      // X := dz + ds
+    __syncthreads();
+    s_mm(T, Y, false, R, true, ms);
+    s_mm(Y, R, false, T, false, ms);                                 // Y := W' ds = r ds r'
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms, lo = i >= j ? e : j + i * ms;
+        p.wz2[oc + so + e] = (p.wz[oc + so + lo] + ut * H[e]) - Y[e];
+        p.ws2[oc + so + e] = p.ws[oc + so + lo] - 0.5 * (s_lam(p, om, so, ms, i) + s_lam(p, om, so, ms, j)) * X[e];
+    }
+    if (tid == 0) part[0] = hz;
+}
+// after the i-th direction (coneprog.py:1302-1321): part[0] = sdot(ds, dz); i = 0: ws3 = ds o dz; ds and dz scaled
+// by lambda^{-1/2} on both sides (scale2); part[1], part[2] their smallest eigenvalues; i = 1 also leaves the
+// eigenvectors in ds and dz and the eigenvalues in sigs and sigz
+__global__ void __launch_bounds__(SB_T) k_s_dir_post(Ptrs p, int i) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double Ds[SMX], Dz[SMX], V[SMX], T[SMX], ev[CVXB_BATCH_SMAX], sh[32];
+    double *ds = p.ds + om + so, *dz = p.dz + om + so;
+    s_load(Ds, ds, ms);
+    s_load(Dz, dz, ms);
+    const double dsdz = s_dot(Ds, Dz, ms, sh);
+    if (i == 0) {
+        s_mm(T, Ds, false, Dz, false, ms);
+        SB_FOR(e, ms) p.ws3[om + so + e] = 0.5 * (T[e] + T[e / ms + (e % ms) * ms]);
+    }
+    SB_FOR(e, ms) {
+        const double c = sqrt(s_lam(p, om, so, ms, e % ms)) * sqrt(s_lam(p, om, so, ms, e / ms));
+        Ds[e] /= c; Dz[e] /= c;
+    }
+    __syncthreads();
+    bool ok = s_eig(Ds, T, V, ev, ms, sh);
+    const double m1 = s_min(ev, ms);
+    if (i == 1) {
+        s_store(ds, V, ms);
+        for (int j = tid; j < ms; j += SB_T) p.sigs[oc + sgo + j] = ev[j];
+    }
+    __syncthreads();
+    ok = s_eig(Dz, T, V, ev, ms, sh) && ok;
+    if (i == 1) {
+        s_store(dz, V, ms);
+        for (int j = tid; j < ms; j += SB_T) p.sigz[oc + sgo + j] = ev[j];
+    }
+    if (tid == 0) { part[0] = dsdz; part[1] = ok ? m1 : NAN; part[2] = ok ? s_min(ev, ms) : NAN; }
+}
+// the update (coneprog.py:1365-1433, misc.py:592-634): Ls = diag(l)^{1/2} Qs diag(l)^{1/2} diag((1 + step sigs) / l)^{1/2},
+// likewise Lz; r := r Ls V diag(lambda+)^{-1/2}, rti := rti Lz U diag(lambda+)^{-1/2} with Lz' Ls = U diag(lambda+) V';
+// s = r diag(lambda+) r', z = rti diag(lambda+) rti'.  The results are staged in the block's rows of d (r), di (rti),
+// ds (s), dz (z) and the diagonal rows of lmbdasq (lambda), which the 's' rows do not otherwise use at this point;
+// k_update commits them only when every block of the problem succeeded, so a problem that stops keeps one
+// iterate.  part[3] = 1 when the SVD failed (first: also when k_s_nt_compute failed, which skips the update).
+template <bool EQ> __global__ void __launch_bounds__(SB_T) k_s_update(Ptrs p, const int *info, int first) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double M0[SMX], M1[SMX], M2[SMX], M3[SMX], M4[SMX], lam[CVXB_BATCH_SMAX];
+    if (S.done || info[b] > 0 || (EQ && p.infop[b] > 0) || (first && part[3] != 0.0)) return;
+    const double step = S.step;
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms;
+        const double li = s_lam(p, om, so, ms, i), lj = s_lam(p, om, so, ms, j), c = sqrt(li) * sqrt(lj);
+        const double gs = (step * p.sigs[oc + sgo + j] + 1.0) / lj, gz = (step * p.sigz[oc + sgo + j] + 1.0) / lj;
+        M2[e] = p.ds[om + so + e] * c * sqrt(gs);
+        M3[e] = p.dz[om + so + e] * c * sqrt(gz);
+        M0[e] = p.sr[oc + sro + e];
+        M1[e] = p.srti[oc + sro + e];
+    }
+    __syncthreads();
+    s_mm(M4, M0, false, M2, false, ms);           // r Ls
+    s_mm(M0, M1, false, M3, false, ms);           // rti Lz
+    s_mm(M1, M3, true, M2, false, ms);            // Lz' Ls = U diag(lambda+) V'
+    const bool ok = s_svd(M1, M2, lam, ms);
+    s_mm(M3, M4, false, M2, false, ms);           // r Ls V
+    s_mm(M4, M0, false, M1, false, ms);           // rti Lz U
+    if (tid == 0) part[3] = ok ? 0.0 : 1.0;
+    if (!ok) return;
+    SB_FOR(e, ms) {
+        const double a = 1.0 / sqrt(lam[e / ms]);
+        M3[e] *= a; M4[e] *= a;
+        p.d[om + so + e] = M3[e]; p.di[om + so + e] = M4[e];
+    }
+    __syncthreads();
+    SB_FOR(e, ms) {                               // lower triangle, mirrored: s and z are returned exactly symmetric
+        const int i = e % ms, j = e / ms;
+        if (i < j) continue;
+        double a = 0.0, c = 0.0;
+        for (int l = 0; l < ms; ++l) { a += M3[i + l * ms] * lam[l] * M3[j + l * ms]; c += M4[i + l * ms] * lam[l] * M4[j + l * ms]; }
+        p.ds[om + so + e] = a; p.dz[om + so + e] = c;
+        p.ds[om + so + j + i * ms] = a; p.dz[om + so + j + i * ms] = c;
+    }
+    for (int i = tid; i < ms; i += SB_T) p.lmbdasq[om + so + i * (ms + 1)] = lam[i];
 }
 }  // namespace
 
@@ -866,6 +1256,11 @@ struct cvxb_batch {
     // cone LP batch (cvxb_batch_create_lp): no P; q holds c; lpv holds x1 (n), z1 and th (m), y1 (p) per slot
     bool lp = false;
     DevBuf<double> lpv;
+    // 's' blocks (cvxb_batch_create_sdp): p.ns blocks of positive order; Gs has mpk = cdim_pckd rows
+    int mpk = 0;
+    long long sums = 0, sums2 = 0;   // sum of the orders, of their squares
+    DevBuf<int> sinfo, u2p;
+    DevBuf<double> rw, spart;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -883,16 +1278,23 @@ int state_alloc(cvxb_batch *b) {
     const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m), p2 = ev(b->neq);
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
     const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
-    if (b->L == cone + ref + lps) return 0;
+    const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
+    const long long L = cone + sb + ref + lps;
+    if (b->L == L) return 0;
     b->L = p.L = 0;
     b->cst.reset();
     p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = p.wy = p.wy2 = p.lps = nullptr;
-    if (cone + ref + lps == 0) return 0;
-    CVXB_TRY(b->cst.alloc((size_t)b->B * (cone + ref + lps)));
-    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * (cone + ref + lps) * sizeof(double)));
-    b->L = p.L = cone + ref + lps;
+    p.sr = p.srti = p.sigs = p.sigz = nullptr;
+    if (L == 0) return 0;
+    CVXB_TRY(b->cst.alloc((size_t)b->B * L));
+    CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * L * sizeof(double)));
+    b->L = p.L = L;
     double *r = b->cst.p;
     if (cone) { p.v = r; r += ev(sumq); p.beta = r; r += ev(p.nq); }
+    if (sb) {
+        p.sr = r; r += ev(b->sums2); p.srti = r; r += ev(b->sums2);
+        p.sigs = r; r += ev(b->sums); p.sigz = r; r += ev(b->sums);
+    }
     if (ref) {
         p.wx = r; r += n2; p.wx2 = r; r += n2;
         p.wz = r; r += m2; p.ws = r; r += m2; p.wz2 = r; r += m2; p.ws2 = r; r += m2; p.wz3 = r; r += m2;
@@ -933,9 +1335,13 @@ int factor_kp(cvxb_batch *b) {
 // exact zeros to the others.
 int batch_factor(cvxb_batch *b, bool kp = true) {
     cudaStream_t st = b->st;
-    const bool cones = b->p.nq > 0;
-    if (cones) {
+    const bool cones = b->p.nq > 0 || b->p.ns > 0;     // Gs = W^{-T} G is formed, mpk rows
+    if (b->p.nq > 0 || (b->p.ns > 0 && b->p.mlq > 0)) {
         k_build_gs<<<dim3((b->n + 7) / 8, b->Bact), 256, 0, st>>>(b->p, b->G.p, b->Gs.p, b->ldg, b->sG);
+        count_launch();
+    }
+    if (b->p.ns > 0) {
+        k_s_build_gs<<<dim3(b->p.ns, b->Bact, (b->n + 15) / 16), SB_T, 0, st>>>(b->p, b->G.p, b->Gs.p, b->ldg, b->sG);
         count_launch();
     }
     // K = P + G' diag(di)^2 G from nine int8 slices per entry (fp64-accurate, ~1.8x the DMMA SYRK)
@@ -946,7 +1352,7 @@ int batch_factor(cvxb_batch *b, bool kp = true) {
                             b->oz_work.p, st));
     } else {
         GemmDesc g;
-        g.M = b->n; g.N = b->n; g.K = b->m;
+        g.M = b->n; g.N = b->n; g.K = b->mpk;
         g.X = cones ? b->Gs.p : b->G.p; g.ldx = (int)b->ldg; g.x_kmajor = true; g.sX = b->sG;
         g.Y = g.X; g.ldy = (int)b->ldg; g.y_kmajor = true; g.sY = b->sG;
         if (!cones) { g.w = b->p.di2; g.sW = b->m; }
@@ -983,13 +1389,13 @@ int batch_factor(cvxb_batch *b, bool kp = true) {
 // y + k*sy, equality rows only), bzp = W^{-T} bz.  Gs is G with the weights di when it is not formed.
 int batch_solve(cvxb_batch *b, double *x, long long sx, double *y = nullptr, long long sy = 0) {
     cudaStream_t st = b->st;
-    const int n = b->n, m = b->m, B = b->Bact, pq = b->neq;
-    const bool cones = b->p.nq > 0;
+    const int n = b->n, m = b->m, B = b->Bact, pq = b->neq, mpk = b->mpk;
+    const bool cones = b->p.nq > 0 || b->p.ns > 0;
     const double *A = cones ? b->Gs.p : b->G.p, *w = cones ? nullptr : b->p.di;
     const long long sw = w ? m : 0;
     // x := x + Gs' bzp
     GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sw = sw; gt.sx = m; gt.sy = sx;
-    CVXB_TRY(gemv_t(m, n, A, b->ldg, w, b->p.bzp, 1.0, 1.0, x, st, gt));
+    CVXB_TRY(gemv_t(mpk, n, A, b->ldg, w, b->p.bzp, 1.0, 1.0, x, st, gt));
     if (pq == 0) {
         CVXB_TRY(potrs_lower(n, b->K.p, (int)b->ldk, b->inv.p, x, b->cw, st, B, b->sK, b->sInv, sx));
     } else {
@@ -1007,26 +1413,29 @@ int batch_solve(cvxb_batch *b, double *x, long long sx, double *y = nullptr, lon
     }
     // bzp := Gs x - bzp
     GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sw = sw; gn.sx = sx; gn.sy = m;
-    CVXB_TRY(gemv_n(m, n, A, b->ldg, w, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
+    CVXB_TRY(gemv_n(mpk, n, A, b->ldg, w, x, 1.0, -1.0, b->p.bzp, b->gemv_ws.p, st, gn));
     return 0;
 }
 
 // the i-th Newton direction: coneqp's f4 (coneprog.py:2288-2347) or, LP, conelp's f6 (:1211-1235) on the right-hand
 // side, i.e. the unrefined solve and then `refinement` correction steps from the residual, followed by the step
 // length and sigma
-template <bool CONES, bool EQ, bool LP> int direction(cvxb_batch *b, int i) {
+template <bool CONES, bool EQ, bool LP, bool SDP = false> int direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
     const long long L = b->L;
-    k_dir_rhs<CONES, EQ, LP><<<B, T, 0, st>>>(p, i); count_launch();
+    const dim3 sg(p.ns, B);                          // SDP: one CTA per ('s' block, slot)
+    k_dir_rhs<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, i); count_launch();
+    if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.dz, m, p.ds, m, 2); count_launch(); }
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
-    if (LP) { k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch(); }
+    if (LP) { k_lp_f6_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch(); }
     else if (p.refinement) { k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
     for (int r = 0; r < p.refinement; ++r) {
         // res() (coneprog.py:1930-1952, :599-631): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx,
         // wz2 -= G dx + W' ds; an LP has no P
-        k_res<EQ, LP><<<B, T, 0, st>>>(p); count_launch();
+        if (SDP) { k_s_res<<<sg, SB_T, 0, st>>>(p); count_launch(); }
+        k_res<EQ, LP, SDP><<<B, T, 0, st>>>(p); count_launch();
         if (!LP) {
             GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
             CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
@@ -1035,8 +1444,8 @@ template <bool CONES, bool EQ, bool LP> int direction(cvxb_batch *b, int i) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
             CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
         }
-        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;      // SDP: G' trisc(wz3) (misc.sgemv)
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
             CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
@@ -1044,12 +1453,14 @@ template <bool CONES, bool EQ, bool LP> int direction(cvxb_batch *b, int i) {
         GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
         CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
         k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
+        if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.wz2, L, p.ws2, L, 2); count_launch(); }
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
-        if (LP) k_lp_f6_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1);
+        if (LP) k_lp_f6_post<EQ, SDP><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1);
         else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
         count_launch();
     }
-    k_dir_post<CONES, LP><<<B, T, 0, st>>>(p, i, !LP && p.refinement == 0); count_launch();
+    if (SDP) { k_s_dir_post<<<sg, SB_T, 0, st>>>(p, i); count_launch(); }
+    k_dir_post<CONES, LP, SDP><<<B, T, 0, st>>>(p, i, !LP && p.refinement == 0); count_launch();
     return 0;
 }
 
@@ -1152,7 +1563,7 @@ int compact_slots(cvxb_batch *b, int B, int ndone, const std::vector<int> &flags
 // the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows.  LP: coneprog.conelp
 // (coneprog.py:662-1436) on a batch without P: the self-dual embedding's tau and kappa, one more KKT solve per
 // iteration for (x1, y1, z1), and infeasibility certificates
-template <bool CONES, bool EQ, bool LP>
+template <bool CONES, bool EQ, bool LP, bool SDP = false>
 int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
@@ -1168,15 +1579,17 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
     CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I (coneqp :2055-2106, conelp :662-857) ----
-    k_init_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();       // dx = -q, y = b, dz = h, resx0 / resy0 / resz0
+    k_init_rhs<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();  // dx = -q, y = b, dz = h, resx0 / resy0 / resz0
     CVXB_TRY(start_factor<EQ>(b));
     k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
+    if (SDP) { k_s_wtz<<<dim3(p.ns, B), SB_T, 0, st>>>(p, p.dz, m, nullptr, 0, 0); count_launch(); }
     if (LP) {
         CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
         CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));            // primal start: (0, b, h)
-        k_lp_start_mid<EQ><<<B, T, 0, st>>>(p); count_launch();
+        k_lp_start_mid<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();
         CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));           // dual start: (-c, 0, 0)
-        k_lp_init_point<CONES, EQ><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
+        if (SDP) { k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
+        k_lp_init_point<CONES, EQ, SDP><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
     } else {
         CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
         k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
@@ -1198,12 +1611,12 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
             CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.y, sgn, 1.0, p.rx, st, gAt));
             CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -sgn, p.ry, b->gemv_ws.p, st, gAn));
         }
-        if (m > 0) {
-            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.z, sgn, 1.0, p.rx, st, gGt));
+        if (m > 0) {                                              // SDP: G' trisc(z) (misc.sgemv)
+            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.z, sgn, 1.0, p.rx, st, gGt));
             CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.x, 1.0, 1.0, p.rz, b->gemv_ws.p, st, gGn));
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        if (LP) k_lp_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        if (LP) k_lp_stats<EQ, SDP><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         else k_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
         int ndone = 0;
@@ -1216,16 +1629,19 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
             B = b->Bact;
             gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
         }
-        k_scaling<CONES, LP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
+        if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
+        k_scaling<CONES, LP, SDP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         CVXB_TRY(batch_factor(b));
         if (LP) {
             // (x1, y1, z1) from (-c, b, h) (:1066-1077), th = W^{-T} h
             k_lp_x1_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
+            if (SDP) { k_s_wtz<<<dim3(p.ns, B), SB_T, 0, st>>>(p, p.h, m, nullptr, 0, 1); count_launch(); }
             CVXB_TRY(batch_solve(b, p.x1, n, p.y1, pq));
-            k_lp_x1_post<EQ><<<B, T, 0, st>>>(p); count_launch();
+            k_lp_x1_post<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();
         }
-        for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ, LP>(b, i)));
-        k_update<CONES, EQ, LP><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
+        for (int i = 0; i < 2; ++i) CVXB_TRY((direction<CONES, EQ, LP, SDP>(b, i)));
+        if (SDP) { k_s_update<EQ><<<dim3(p.ns, B), SB_T, 0, st>>>(p, b->d_info.p, it == 0); count_launch(); }
+        k_update<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -1257,7 +1673,7 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
 
 // a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q') and p equality rows.
 // Every argument is checked before the device is.
-int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp) {
+int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp, bool sdp = false) {
     if (out) *out = nullptr;
     if (!out || nprob <= 0 || n <= 0 || !dims) {
         set_error("batch_create: bad sizes (nprob and n positive, dims given)");
@@ -1278,15 +1694,31 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
         mm += dims->q[k];
     }
     if (mm > (1LL << 30)) { set_error("batch_create: too many cone rows"); return CVXB_E_ARG; }
-    if (dims->ns > 0) { set_error("batch_create: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    if (dims->ns > 0 && !sdp) { set_error("batch_create: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
+    const long long mlq = mm;
+    long long mpk = mm;                           // cdim_pckd
+    if (sdp && dims->ns > 0) {
+        if (!dims->s) { set_error("batch_create_sdp: dims has ns > 0 and no 's' orders"); return CVXB_E_ARG; }
+        for (int k = 0; k < dims->ns; ++k) {
+            const int s = dims->s[k];
+            if (s < 0) { set_error("batch_create_sdp: dims['s'][%d] = %d < 0", k, s); return CVXB_E_ARG; }
+            if (s > CVXB_BATCH_SMAX) {
+                set_error("batch_create_sdp: dims['s'][%d] = %d > %d, the largest 's' order of the batch", k, s,
+                          CVXB_BATCH_SMAX);
+                return CVXB_E_UNSUP;
+            }
+            mm += (long long)s * s; mpk += (long long)s * (s + 1) / 2;
+        }
+    }
+    if (mm > (1LL << 30)) { set_error("batch_create: too many cone rows"); return CVXB_E_ARG; }
     if (lp && mm == 0) {                          // deliberate: every cone LP needs at least one cone row
         set_error("batch_create_lp: the batch needs at least one 'l' or 'q' row (m = 0)");
         return CVXB_E_ARG;
     }
-    // the checks before the first factorisation: coneqp's (coneprog.py:1962), conelp's (:572-573)
-    if (p > n || (lp && p + mm < n)) {
+    // the checks before the first factorisation: coneqp's (coneprog.py:1962), conelp's (:572-573, with cdim_pckd)
+    if (p > n || (lp && p + mpk < n)) {
         set_error("batch_create: Rank(A) < p or Rank([%s]) < n (p = %d, n = %d, cdim = %lld)", lp ? "G; A" : "P; A; G",
-                  p, n, mm);
+                  p, n, mpk);
         return CVXB_E_ARG;
     }
     CVXB_TRY(check_device(device));
@@ -1346,6 +1778,40 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
         CVXB_TRY(b->Gs.alloc(B * b->sG));
         q.nq = nq; q.qoff = b->qoff.p;
         q.refinement = 1;                         // the default with 'q' cones (coneprog.py:1862-1865)
+    }
+    b->mpk = (int)mpk;
+    q.mlq = (int)mlq; q.mpk = (int)mpk; q.mdg = (int)mlq;
+    if (sdp && mm > mlq) {                        // 's' blocks of positive order; order 0 adds no rows (:497-499)
+        std::vector<int> info;
+        std::vector<int> u2p(mm - mlq);
+        std::vector<double> rw(m, 1.0);
+        long long so = mlq, sp = 0, sro = 0, sgo = 0;
+        for (int k = 0; k < dims->ns; ++k) {
+            const int s = dims->s[k];
+            if (s == 0) continue;
+            info.insert(info.end(), {s, (int)so, (int)(mlq + sp), (int)sro, (int)sgo});
+            for (int j = 0; j < s; ++j)
+                for (int i = 0; i < s; ++i) {
+                    const int r = std::max(i, j), c = std::min(i, j);
+                    u2p[so - mlq + i + j * s] = (int)(sp + c * s - c * (c - 1) / 2 + r - c);
+                    rw[so + i + j * s] = i == j ? 1.0 : (i > j ? 2.0 : 0.0);
+                }
+            so += (long long)s * s; sp += (long long)s * (s + 1) / 2; sro += (long long)s * s; sgo += s;
+        }
+        const int ns = (int)info.size() / 5;
+        b->sums = sgo; b->sums2 = sro;
+        CVXB_TRY(b->sinfo.alloc(info.size()));
+        CVXB_CUDA(cudaMemcpy(b->sinfo.p, info.data(), info.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CVXB_TRY(b->u2p.alloc(u2p.size()));
+        CVXB_CUDA(cudaMemcpy(b->u2p.p, u2p.data(), u2p.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CVXB_TRY(b->rw.alloc(rw.size()));
+        CVXB_CUDA(cudaMemcpy(b->rw.p, rw.data(), rw.size() * sizeof(double), cudaMemcpyHostToDevice));
+        CVXB_TRY(b->spart.alloc(B * ns * 4));
+        CVXB_CUDA(cudaMemset(b->spart.p, 0, B * ns * 4 * sizeof(double)));
+        if (!b->Gs.p) CVXB_TRY(b->Gs.alloc(B * b->sG));
+        q.ns = ns; q.mdg = (int)(mlq + sgo);
+        q.sinfo = b->sinfo.p; q.u2p = b->u2p.p; q.rw = b->rw.p; q.spart = b->spart.p;
+        q.refinement = 1;                         // the default with 's' cones (coneprog.py:502-507)
     }
     if (p > 0) {
         b->neq = p;
@@ -1418,6 +1884,10 @@ int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_d
     return create(out, nprob, n, p, dims, device, true);
 }
 
+int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+    return create(out, nprob, n, p, dims, device, true, true);
+}
+
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
@@ -1484,7 +1954,10 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
                                      solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,
                                      solve<false, true, true>,   solve<true, true, true>};
+    static const Solve sdp_solvers[4] = {solve<false, false, true, true>, solve<true, false, true, true>,
+                                         solve<false, true, true, true>, solve<true, true, true, true>};
     const int k = (b->p.nq > 0 ? 1 : 0) + (b->neq > 0 ? 2 : 0) + (b->lp ? 4 : 0);     // CONES, EQ, LP
+    if (b->p.ns > 0) return sdp_solvers[k & 3](b, maxiters, abstol, reltol, feastol);  // SDP batches are cone LPs
     return solvers[k](b, maxiters, abstol, reltol, feastol);
 }
 

@@ -262,6 +262,155 @@ __device__ __forceinline__ void q_nt_update(const Team &t, double *s, double *z,
     }
     if (t.rank == 0) *beta *= sqrt(aa / bb);
 }
+
+// ---- in-CTA Jacobi solvers for small blocks ---------------------------------------------------------------
+// The single-problem kernels (cone_vec.cu jac_small_kernel, nt_scaling.cu jacobi_small_kernel) and the batch
+// IPM's 's'-block kernels call the same bodies.
+// Round-robin pairing of m2 (even) players: round r, slot t -> columns (p, q); an index >= m is a bye.
+__device__ __forceinline__ void svd_pair(int m2, int r, int t, int &p, int &q) {
+    const int n1 = m2 - 1;
+    if (t == 0) { p = n1; q = r % n1; }
+    else { p = (r + t) % n1; q = (r - t + n1) % n1; }
+    if (p > q) { const int w = p; p = q; q = w; }
+}
+// Round r of the round-robin ("chess tournament") ordering on N (even) indices: N/2 disjoint pairs.
+__device__ __forceinline__ void rr_pair(int N, int r, int k, int &p, int &q) {
+    int a, b;
+    if (k == 0) { a = N - 1; b = r; }
+    else { a = (r + k) % (N - 1); b = (r - k + (N - 1)) % (N - 1); }
+    p = min(a, b); q = max(a, b);
+}
+
+// rotation J = [c s; -s c] annihilating a_pq in J'[app apq; apq aqq]J;  t = tan of the angle
+__device__ __forceinline__ void jac_rot(double app, double aqq, double apq, double &c, double &s, double &t) {
+    if (apq == 0.0) { c = 1.0; s = 0.0; t = 0.0; return; }
+    const double tau = (aqq - app) / (2.0 * apq);
+    t = copysign(1.0, tau) / (fabs(tau) + sqrt(1.0 + tau * tau));     // tau*tau = inf -> t = 0
+    c = 1.0 / sqrt(1.0 + t * t);
+    s = t * c;
+}
+
+// One thread's share of a round: the 2x2 block (rows of pair I, columns of pair J) of
+// dst = J'.src.J, and the same block of V := V.J.  Indices >= mk belong to the padding.
+template <bool WITH_V>
+__device__ __forceinline__ void jac_block(const double *src, double *dst, double *V, int mk, int N,
+                                          int r, int I, int J) {
+    int pi, qi, pj, qj;
+    rr_pair(N, r, I, pi, qi);
+    rr_pair(N, r, J, pj, qj);
+    if (pi >= mk || pj >= mk) return;
+    const bool vi = qi < mk, vj = qj < mk;
+    double ci = 1, si = 0, ti = 0, cj = 1, sj = 0, tj = 0;
+    if (vi) jac_rot(src[pi + (size_t)pi * mk], src[qi + (size_t)qi * mk], src[qi + (size_t)pi * mk], ci, si, ti);
+    if (I == J) { cj = ci; sj = si; tj = ti; }
+    else if (vj) jac_rot(src[pj + (size_t)pj * mk], src[qj + (size_t)qj * mk], src[qj + (size_t)pj * mk], cj, sj, tj);
+    const double b00 = src[pi + (size_t)pj * mk];
+    const double b01 = vj ? src[pi + (size_t)qj * mk] : 0.0;
+    const double b10 = vi ? src[qi + (size_t)pj * mk] : 0.0;
+    const double b11 = (vi && vj) ? src[qi + (size_t)qj * mk] : 0.0;
+    double d00, d01, d10, d11;
+    if (I == J) {
+        d00 = b00 - ti * b10; d11 = b11 + ti * b10; d01 = 0.0; d10 = 0.0;
+    } else {
+        const double r00 = ci * b00 - si * b10, r01 = ci * b01 - si * b11;
+        const double r10 = si * b00 + ci * b10, r11 = si * b01 + ci * b11;
+        d00 = cj * r00 - sj * r01; d01 = sj * r00 + cj * r01;
+        d10 = cj * r10 - sj * r11; d11 = sj * r10 + cj * r11;
+    }
+    dst[pi + (size_t)pj * mk] = d00;
+    if (vj) dst[pi + (size_t)qj * mk] = d01;
+    if (vi) dst[qi + (size_t)pj * mk] = d10;
+    if (vi && vj) dst[qi + (size_t)qj * mk] = d11;
+    if (WITH_V) {
+        const double v00 = V[pi + (size_t)pj * mk];
+        const double v01 = vj ? V[pi + (size_t)qj * mk] : 0.0;
+        V[pi + (size_t)pj * mk] = cj * v00 - sj * v01;
+        if (vj) V[pi + (size_t)qj * mk] = sj * v00 + cj * v01;
+        if (vi) {
+            const double v10 = V[qi + (size_t)pj * mk];
+            const double v11 = vj ? V[qi + (size_t)qj * mk] : 0.0;
+            V[qi + (size_t)pj * mk] = cj * v10 - sj * v11;
+            if (vj) V[qi + (size_t)qj * mk] = sj * v10 + cj * v11;
+        }
+    }
+}
+// convergence of one block from its (off^2, total^2): at rounding level, or stagnating just above it
+__host__ __device__ inline bool jac_done(double off2, double tot2, double prev_off2, int mk) {
+    const double eps = 2.220446049250313e-16;
+    if (!(off2 > eps * eps * (double)mk * tot2)) return off2 == off2;       // NaN never converges
+    return off2 <= 1e-26 * tot2 && off2 >= 0.25 * prev_off2;
+}
+
+// Two-sided Jacobi sweeps on the symmetric mk x mk block in w0 (both triangles), ping-ponging with w1; V := V J when
+// WITH_V; tid, nt: threadIdx.x, blockDim.x.  Needs blockDim.x >= (N/2)^2 with N = mk rounded up to even.  On return w0 points at the rotated block
+// (eigenvalues on its diagonal, eigenvectors in the columns of V); false when max_sweeps ran out (jac_done).
+template <bool WITH_V>
+__device__ __forceinline__ bool jac_eig_cta(double *&w0, double *&w1, double *V, int mk, int max_sweeps, double *sh,
+                                            int tid, int nt) {
+    const int N = max(2, mk + (mk & 1)), h = N / 2;
+    const int I = tid % h, J = tid / h;          // I fastest: rows of the column-major block
+    double prev = 1e300;
+    int sweep = 0;
+    bool ok = false;
+    for (;; ++sweep) {
+        double off = 0, tot = 0;
+        for (int e = tid; e < mk * mk; e += nt) {
+            const double v = w0[e] * w0[e];
+            tot += v;
+            if (e % mk != e / mk) off += v;
+        }
+        off = block_sum(off, sh); tot = block_sum(tot, sh);
+        if (jac_done(off, tot, prev, mk)) { ok = true; break; }
+        if (sweep == max_sweeps) break;
+        prev = off;
+        for (int r = 0; r < N - 1; ++r) {
+            if (J < h) jac_block<WITH_V>(w0, w1, V, mk, N, r, I, J);
+            __syncthreads();
+            double *t = w0; w0 = w1; w1 = t;
+        }
+    }
+    return ok;
+}
+
+// One-sided Jacobi on the columns of the m x m block B (column-major, ld m), V := V J: one warp per column pair,
+// until a sweep rotates nothing or maxsweeps have run (true: the former).  B and V are shared memory; the caller
+// initialises V; rot is a shared int of the caller's.
+__device__ __forceinline__ bool jacobi_svd_cta(int m, double *B, double *V, int maxsweeps, int &rot) {
+    const int m2 = (m + 1) & ~1, npairs = m2 / 2;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
+    for (int sweep = 0; sweep < maxsweeps; ++sweep) {
+        if (threadIdx.x == 0) rot = 0;
+        __syncthreads();
+        for (int r = 0; r < m2 - 1; ++r) {
+            for (int t = warp; t < npairs; t += nwarp) {        // one warp per pair
+                int p, q;
+                svd_pair(m2, r, t, p, q);
+                if (q >= m) continue;
+                double *bp = B + p * m, *bq = B + q * m;
+                double a = 0.0, b = 0.0, g = 0.0;
+                for (int i = lane; i < m; i += 32) { const double x = bp[i], y = bq[i]; a += x * x; b += y * y; g += x * y; }
+                a = warp_sum(a); b = warp_sum(b); g = warp_sum(g);
+                if (!(fabs(g) > (2.0 * 2.220446049250313e-16 * sqrt((double)m)) * sqrt(a * b)) || g == 0.0) continue;
+                const double zeta = (b - a) / (2.0 * g);
+                const double tt = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+                const double c = 1.0 / sqrt(1.0 + tt * tt), sn = c * tt;
+                double *vp = V + p * m, *vq = V + q * m;
+                for (int i = lane; i < m; i += 32) {
+                    const double x = bp[i], y = bq[i];
+                    bp[i] = c * x - sn * y; bq[i] = sn * x + c * y;
+                    const double u = vp[i], w = vq[i];
+                    vp[i] = c * u - sn * w; vq[i] = sn * u + c * w;
+                }
+                if (lane == 0) atomicAdd(&rot, 1);
+            }
+            __syncthreads();
+        }
+        const int done = (rot == 0);
+        __syncthreads();
+        if (done) break;
+    }
+    return rot == 0;
+}
 #endif
 
 }  // namespace cvxb

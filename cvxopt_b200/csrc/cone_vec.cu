@@ -152,68 +152,7 @@ __global__ void max_step_kernel(const double *x, Cones c, double *out) {
 }
 
 
-// ---- symmetric eigensolver for the 's' blocks (parallel-order cyclic Jacobi) ----------------
-// Round r of the round-robin ("chess tournament") ordering on N (even) indices: N/2 disjoint pairs.
-__device__ __forceinline__ void rr_pair(int N, int r, int k, int &p, int &q) {
-    int a, b;
-    if (k == 0) { a = N - 1; b = r; }
-    else { a = (r + k) % (N - 1); b = (r - k + (N - 1)) % (N - 1); }
-    p = min(a, b); q = max(a, b);
-}
-
-// rotation J = [c s; -s c] annihilating a_pq in J'[app apq; apq aqq]J;  t = tan of the angle
-__device__ __forceinline__ void jac_rot(double app, double aqq, double apq, double &c, double &s, double &t) {
-    if (apq == 0.0) { c = 1.0; s = 0.0; t = 0.0; return; }
-    const double tau = (aqq - app) / (2.0 * apq);
-    t = copysign(1.0, tau) / (fabs(tau) + sqrt(1.0 + tau * tau));     // tau*tau = inf -> t = 0
-    c = 1.0 / sqrt(1.0 + t * t);
-    s = t * c;
-}
-
-// One thread's share of a round: the 2x2 block (rows of pair I, columns of pair J) of
-// dst = J'.src.J, and the same block of V := V.J.  Indices >= mk belong to the padding.
-template <bool WITH_V>
-__device__ __forceinline__ void jac_block(const double *src, double *dst, double *V, int mk, int N,
-                                          int r, int I, int J) {
-    int pi, qi, pj, qj;
-    rr_pair(N, r, I, pi, qi);
-    rr_pair(N, r, J, pj, qj);
-    if (pi >= mk || pj >= mk) return;
-    const bool vi = qi < mk, vj = qj < mk;
-    double ci = 1, si = 0, ti = 0, cj = 1, sj = 0, tj = 0;
-    if (vi) jac_rot(src[pi + (size_t)pi * mk], src[qi + (size_t)qi * mk], src[qi + (size_t)pi * mk], ci, si, ti);
-    if (I == J) { cj = ci; sj = si; tj = ti; }
-    else if (vj) jac_rot(src[pj + (size_t)pj * mk], src[qj + (size_t)qj * mk], src[qj + (size_t)pj * mk], cj, sj, tj);
-    const double b00 = src[pi + (size_t)pj * mk];
-    const double b01 = vj ? src[pi + (size_t)qj * mk] : 0.0;
-    const double b10 = vi ? src[qi + (size_t)pj * mk] : 0.0;
-    const double b11 = (vi && vj) ? src[qi + (size_t)qj * mk] : 0.0;
-    double d00, d01, d10, d11;
-    if (I == J) {
-        d00 = b00 - ti * b10; d11 = b11 + ti * b10; d01 = 0.0; d10 = 0.0;
-    } else {
-        const double r00 = ci * b00 - si * b10, r01 = ci * b01 - si * b11;
-        const double r10 = si * b00 + ci * b10, r11 = si * b01 + ci * b11;
-        d00 = cj * r00 - sj * r01; d01 = sj * r00 + cj * r01;
-        d10 = cj * r10 - sj * r11; d11 = sj * r10 + cj * r11;
-    }
-    dst[pi + (size_t)pj * mk] = d00;
-    if (vj) dst[pi + (size_t)qj * mk] = d01;
-    if (vi) dst[qi + (size_t)pj * mk] = d10;
-    if (vi && vj) dst[qi + (size_t)qj * mk] = d11;
-    if (WITH_V) {
-        const double v00 = V[pi + (size_t)pj * mk];
-        const double v01 = vj ? V[pi + (size_t)qj * mk] : 0.0;
-        V[pi + (size_t)pj * mk] = cj * v00 - sj * v01;
-        if (vj) V[pi + (size_t)qj * mk] = sj * v00 + cj * v01;
-        if (vi) {
-            const double v10 = V[qi + (size_t)pj * mk];
-            const double v11 = vj ? V[qi + (size_t)qj * mk] : 0.0;
-            V[qi + (size_t)pj * mk] = cj * v10 - sj * v11;
-            if (vj) V[qi + (size_t)qj * mk] = sj * v10 + cj * v11;
-        }
-    }
-}
+// The symmetric eigensolver for the 's' blocks (parallel-order cyclic Jacobi) is cone.cuh's jac_block / jac_eig_cta.
 
 struct JacArgs {
     const double *x;        // first 's' row of the cone vector (lower triangles significant)
@@ -303,12 +242,6 @@ __global__ void jac_vec_kernel(JacArgs a) {
     }
 }
 
-// convergence of one block from its (off^2, total^2): at rounding level, or stagnating just above it
-__host__ __device__ inline bool jac_done(double off2, double tot2, double prev_off2, int mk) {
-    const double eps = 2.220446049250313e-16;
-    if (!(off2 > eps * eps * (double)mk * tot2)) return off2 == off2;       // NaN never converges
-    return off2 <= 1e-26 * tot2 && off2 >= 0.25 * prev_off2;
-}
 
 // All blocks of order <= 64: one CTA per block runs every sweep itself (block-level barriers only).
 template <bool WITH_V>
@@ -325,28 +258,7 @@ __global__ void __launch_bounds__(1024) jac_small_kernel(JacArgs a, int max_swee
         if (WITH_V) V[e] = (i == j) ? 1.0 : 0.0;
     }
     __syncthreads();
-    const int N = max(2, mk + (mk & 1)), h = N / 2;
-    const int I = tid % h, J = tid / h;          // I fastest: rows of the column-major block
-    double prev = 1e300;
-    int sweep = 0;
-    bool ok = false;
-    for (;; ++sweep) {
-        double off = 0, tot = 0;
-        for (int e = tid; e < mk * mk; e += nt) {
-            const double v = w0[e] * w0[e];
-            tot += v;
-            if (e % mk != e / mk) off += v;
-        }
-        off = block_sum(off, sh); tot = block_sum(tot, sh);
-        if (jac_done(off, tot, prev, mk)) { ok = true; break; }
-        if (sweep == max_sweeps) break;
-        prev = off;
-        for (int r = 0; r < N - 1; ++r) {
-            if (J < h) jac_block<WITH_V>(w0, w1, V, mk, N, r, I, J);
-            __syncthreads();
-            double *t = w0; w0 = w1; w1 = t;
-        }
-    }
+    const bool ok = jac_eig_cta<WITH_V>(w0, w1, V, mk, max_sweeps, sh, tid, nt);
     if (!ok && tid == 0) atomicExch(fail, 1);
     for (int i = tid; i < mk; i += nt) {
         const double di = w0[i + (size_t)i * mk];

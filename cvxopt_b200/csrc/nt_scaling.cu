@@ -76,19 +76,12 @@ __global__ void set_identity_kernel(int m, double *V) {
     V[e] = (e % m == e / m) ? 1.0 : 0.0;
 }
 
-// Round-robin pairing of m2 (even) players: round r, slot t -> columns (p, q); an index >= m is a bye.
-__device__ __forceinline__ void rr_pair(int m2, int r, int t, int &p, int &q) {
-    const int n1 = m2 - 1;
-    if (t == 0) { p = n1; q = r % n1; }
-    else { p = (r + t) % n1; q = (r - t + n1) % n1; }
-    if (p > q) { const int w = p; p = q; q = w; }
-}
 
 // One round of one-sided Jacobi: CTA t orthogonalises columns (p, q) of B and applies the same rotation to V.
 __global__ void __launch_bounds__(128) jacobi_round_kernel(int m, int m2, int r, double *B, double *V, int *nrot) {
     __shared__ double sh[32];
     int p, q;
-    rr_pair(m2, r, blockIdx.x, p, q);
+    svd_pair(m2, r, blockIdx.x, p, q);
     if (q >= m) return;                        // bye
     double *bp = B + (size_t)p * m, *bq = B + (size_t)q * m;
     double a = 0.0, b = 0.0, g = 0.0;
@@ -123,7 +116,7 @@ __global__ void __launch_bounds__(128) jacobi_sweep_kernel(int m, int m2, double
     int rotated = 0;
     for (int r = 0; r < m2 - 1; ++r) {
         int p, q;
-        rr_pair(m2, r, blockIdx.x, p, q);
+        svd_pair(m2, r, blockIdx.x, p, q);
         if (q < m) {
             double *bp = B + (size_t)p * m, *bq = B + (size_t)q * m;
             double a = 0.0, b = 0.0, g = 0.0;
@@ -165,39 +158,7 @@ __global__ void __launch_bounds__(256) jacobi_small_kernel(int m, double *Bg, do
     __shared__ int rot;
     for (int e = threadIdx.x; e < m * m; e += blockDim.x) { B[e] = Bg[e]; V[e] = (e % m == e / m) ? 1.0 : 0.0; }
     __syncthreads();
-    const int m2 = (m + 1) & ~1, npairs = m2 / 2;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarp = blockDim.x >> 5;
-    for (int sweep = 0; sweep < maxsweeps; ++sweep) {
-        if (threadIdx.x == 0) rot = 0;
-        __syncthreads();
-        for (int r = 0; r < m2 - 1; ++r) {
-            for (int t = warp; t < npairs; t += nwarp) {        // one warp per pair
-                int p, q;
-                rr_pair(m2, r, t, p, q);
-                if (q >= m) continue;
-                double *bp = B + p * m, *bq = B + q * m;
-                double a = 0.0, b = 0.0, g = 0.0;
-                for (int i = lane; i < m; i += 32) { const double x = bp[i], y = bq[i]; a += x * x; b += y * y; g += x * y; }
-                a = warp_sum(a); b = warp_sum(b); g = warp_sum(g);
-                if (!(fabs(g) > (2.0 * 2.220446049250313e-16 * sqrt((double)m)) * sqrt(a * b)) || g == 0.0) continue;
-                const double zeta = (b - a) / (2.0 * g);
-                const double tt = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-                const double c = 1.0 / sqrt(1.0 + tt * tt), sn = c * tt;
-                double *vp = V + p * m, *vq = V + q * m;
-                for (int i = lane; i < m; i += 32) {
-                    const double x = bp[i], y = bq[i];
-                    bp[i] = c * x - sn * y; bq[i] = sn * x + c * y;
-                    const double u = vp[i], w = vq[i];
-                    vp[i] = c * u - sn * w; vq[i] = sn * u + c * w;
-                }
-                if (lane == 0) atomicAdd(&rot, 1);
-            }
-            __syncthreads();
-        }
-        const int done = (rot == 0);
-        __syncthreads();
-        if (done) break;
-    }
+    jacobi_svd_cta(m, B, V, maxsweeps, rot);
     for (int e = threadIdx.x; e < m * m; e += blockDim.x) { Bg[e] = B[e]; Vg[e] = V[e]; }
 }
 

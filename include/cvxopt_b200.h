@@ -278,6 +278,21 @@ int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_d
  * (x1, z1, W^{-T} h, y1) and 18 scalars (tau, kappa and the rest of the embedding) in the per-problem state row; all
  * of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy. */
 int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
+/* the largest 's' order of a batch: one CTA holds a block's working matrices in shared memory */
+#define CVXB_BATCH_SMAX 32
+/* batch of cone LPs whose dims may hold 's' blocks as well as 'l' and 'q' cones: B x conelp(c, G, h, dims, A, b) with
+ * kktsolver 'chol', the reference's solvers.sdp when dims is {'l': ml, 's': [...]}.  It refuses what
+ * cvxb_batch_create_lp refuses, and, before the device: an order s[k] < 0 (CVXB_E_ARG), s[k] > CVXB_BATCH_SMAX
+ * (CVXB_E_UNSUP), and conelp's rank check with the packed dimension, p > n or p + cdim_pckd < n (CVXB_E_ARG).  An
+ * order-0 block adds no rows.  Every other cvxb_batch_* call serves it: G is cdim x n column-major with each 's'
+ * block's rows unpacked (s[k]^2 rows, the block column-major), as the reference's G; only the lower triangle of each
+ * 's' block of G and h is read.  cvxb_batch_results returns s and z with 's' blocks symmetric.  Refinement defaults
+ * to 1.  Device memory per problem, in doubles: that of the cone LP batch of the same n, cdim and p, plus ldg*n for
+ * Gs if dims has no 'q' cone, 2*sum(s^2) + 2*sum(s) (r, rti, and the eigenvalues sigs, sigz) each rounded up to even
+ * in the state row, and 4 per block of partial sums; and, shared by the batch, cdim doubles of row weights and
+ * cdim - ml - sum(q) + 5 ns ints of layout; all of it is counted by cvxb_device_bytes and freed by
+ * cvxb_batch_destroy. */
+int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);
