@@ -10,9 +10,11 @@ from .conelp import conelp  # noqa: F401
 from .batch import QPBatch, QPBatchGroup, qp_batch, qp_batch_distributed, shard_bounds, shard_indices  # noqa: F401
 from .batch import ConeLPBatch, ConeLPBatchGroup, conelp_batch  # noqa: F401
 from .batch import SDPBatch, SDPBatchGroup, sdp_batch  # noqa: F401
+from .batch import SDPQPBatch, SDPQPBatchGroup, coneqp_batch  # noqa: F401
 
 __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolver", "cpl_kktsolver", "QPBatch", "qp_batch", "conelp", "qp_batch_distributed", "load",
            "ConeLPBatch", "conelp_batch", "SDPBatch", "SDPBatchGroup", "sdp_batch",
+           "SDPQPBatch", "SDPQPBatchGroup", "coneqp_batch",
            "device_count", "launch_count"]
 
 

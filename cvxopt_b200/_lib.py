@@ -108,6 +108,8 @@ _SIGS = {
                                        C.c_int]),
     "cvxb_batch_create_sdp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Dims),
                                         C.c_int]),
+    "cvxb_batch_create_sdp_qp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Dims),
+                                           C.c_int]),
     "cvxb_batch_load_eq": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_load_lp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_results_y": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),

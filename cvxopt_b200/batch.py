@@ -13,6 +13,8 @@ The reference has no batch API; its counterpart is a Python loop over those call
 Cone LPs  minimize c'x  subject to  G x + s = h,  s in K,  A x = b  run coneprog.conelp (coneprog.py:31-1436) in the
 same lock-step machinery (ConeLPBatch, conelp_batch): a Python loop over `solvers.conelp(c, G, h, dims, A, b)`
 (`solvers.lp` for dims={'l': m}), with its infeasibility certificates.
+
+Dims with 's' blocks (orders <= 32) run through SDPBatch / sdp_batch (conelp) and SDPQPBatch / coneqp_batch (coneqp).
 """
 import ctypes as C
 
@@ -99,7 +101,7 @@ class QPBatch:
     """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
     _lp = False              # ConeLPBatch: a batch of cone LPs
-    _sdp = False             # SDPBatch: cone LPs whose dims may hold 's' blocks
+    _sdp = False             # SDPBatch, SDPQPBatch: dims may hold 's' blocks
 
     def __init__(self, nprob, n, m, device=0, dims=None, p=0):
         if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
@@ -111,7 +113,8 @@ class QPBatch:
         if d is None and (self._lp or self.p):
             d, keep, _ = _batch_dims({"l": self.m})
         if self._sdp:
-            rc = self._lib.cvxb_batch_create_sdp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
+            create = self._lib.cvxb_batch_create_sdp if self._lp else self._lib.cvxb_batch_create_sdp_qp
+            rc = create(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
         elif self._lp:
             rc = self._lib.cvxb_batch_create_lp(C.byref(self._h), self.B, self.n, self.p, C.byref(d), device)
         elif self.p:
@@ -477,6 +480,42 @@ def sdp_batch(c, Gl=None, hl=None, Gs=None, hs=None, A=None, b=None, device=0, n
             o += k * k
         out[key + "s"] = blocks
     return out
+
+
+class SDPQPBatch(QPBatch):
+    """QPBatch whose dims may hold 's' blocks of order <= 32 (cvxb_batch_create_sdp_qp): B x coneqp(P, q, G, h, dims,
+    A, b).  load() takes QPBatch's P (B, n, n), q (B, n), G (B, cdim, n), h (B, cdim), with each 's' block's rows
+    unpacked column-major; only the lower triangle of an 's' block of G and h is read, and results() returns s and z
+    with symmetric 's' blocks."""
+    _sdp = True
+
+    def __init__(self, nprob, n, dims, p=0, device=0):
+        super().__init__(nprob, n, None, device, dims, p)
+
+
+class SDPQPBatchGroup(QPBatchGroup):
+    """QPBatchGroup of SDPQPBatch parts"""
+
+    def __init__(self, nprob, n, dims, p=0, device=0, nsub=None):
+        super().__init__(nprob, n, _sdp_dims(dims)[2], device, nsub, dims, p)
+
+    @staticmethod
+    def _part():
+        return lambda nprob, n, m, device, dims, p=0: SDPQPBatch(nprob, n, dims, p, device)
+
+
+def coneqp_batch(P, q, G, h, dims, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent cone QPs on one GPU, each as solvers.coneqp(P, q, G, h, dims, A, b) does.  P (B,n,n),
+    q (B,n), G (B,cdim,n), h (B,cdim); optional A (B,p,n), b (B,p), given together.  dims: shared by every problem,
+    with 'l', 'q' and 's' (orders at most 32); each 's' block's rows of G and h are unpacked column-major, as the
+    reference's G, and only their lower triangles are read.  nsub and the returned dict are qp_batch's; its s and z
+    have symmetric 's' blocks.  options: maxiters, abstol, reltol, feastol, refinement (as coneqp's)."""
+    _, _, _, _, B, n, m = _stack(P, q, G, h)
+    _sdp_dims(dims, m)
+    p = _eq_rows(A, b, B, n)
+    if p > n:
+        raise ValueError("Rank(A) < p or Rank([P; G; A]) < n")        # coneprog.py:1970-1971
+    return _run_group(SDPQPBatchGroup(B, n, dims, p, device, nsub), (P, q, G, h, A, b), options)
 
 
 def _run_group(grp, data, options):

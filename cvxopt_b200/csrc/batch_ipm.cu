@@ -15,7 +15,8 @@
 // Nothing leaves the device between iterations except one int ("how many are done").
 // A cone LP batch (no P: minimize c'x over the same constraints) runs coneprog.conelp (coneprog.py:31-1436) instead,
 // through the same loop, solve<CONES, EQ, LP> with LP = true: the same factorisations, solves and refinement with the
-// self-dual embedding's tau / kappa arithmetic around them.
+// self-dual embedding's tau / kappa arithmetic around them.  Batches with 's' blocks (SDP = true) run either
+// algorithm: cvxb_batch_create_sdp builds cone LPs, cvxb_batch_create_sdp_qp QPs.
 #include "cone.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -55,7 +56,7 @@ struct Ptrs {
     // cone LP batches (cvxb_batch_create_lp): q holds c; lps is the LPScal at the end of a slot's state row;
     // x1 (n), y1 (p), z1 and th (m) are rebuilt every iteration
     double *lps, *x1, *y1, *z1, *th;
-    // 's' blocks (cvxb_batch_create_sdp; cone LP batches only).  Rows [mlq, m) of the m-vectors are the blocks,
+    // 's' blocks (cvxb_batch_create_sdp, cvxb_batch_create_sdp_qp).  Rows [mlq, m) of the m-vectors are the blocks,
     // unpacked (ms² rows each, column-major); bzp, th, z1 and Gs hold them packed in rows [mlq, mpk).  rw: the sdot
     // weight of each m-row (1 'l' / 'q' rows and diagonals, 2 strict lower, 0 strict upper); u2p: for each 's' row,
     // its packed row minus mlq.  sinfo: per block ms, unpacked row, packed row, offset in r / rti, offset in sigs.
@@ -88,6 +89,11 @@ __device__ __forceinline__ LPScal &lp_scal(const Ptrs &p, long long oc) {
     for (int k_ = warp; k_ < p.nq; k_ += nwarp)                            \
         if (const int o = p.qoff[k_], len = p.qoff[k_ + 1] - p.qoff[k_]; true)
 #define FOR_LANE(i, len) for (int i = lane; i < len; i += 32)
+
+// value of m-row i (an 's' row when i >= mlq) of a vector whose 's' blocks are packed (bzp, z1)
+__device__ __forceinline__ double unpacked(const Ptrs &p, const double *x, int i) {
+    return i < p.mlq ? x[i] : x[p.mlq + p.u2p[i - p.mlq]] * (p.rw[i] == 1.0 ? 1.0 : M_SQRT1_2);
+}
 
 // starting point, part 1: rhs of [P G'; G -I][x; z] = [-q; h] with W = I   (coneprog.py:2055-2080): d = di = 1,
 // v = e1 and beta = 1 for each cone.  EQ: y = b (the solve overwrites it, :2078-2081), aw = 0 (no A'A in S yet)
@@ -140,23 +146,39 @@ __global__ void k_scale_bz(Ptrs p) {
     const double *v = p.v + oc - p.ml, *beta = p.beta + oc;
     FOR_CONES(o, len) q_scale(wt, v + o, beta[k_], src + o, dst + o, len, true);
 }
-// starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both, gap
-template <bool CONES> __global__ void k_init_point(Ptrs p) {
+// starting point with 's' blocks, the part before k_s_eig_start reads s (coneprog.py:2083-2086): x = dx, z = the
+// solve's bzp unpacked, s = -z
+__global__ void k_init_sz(Ptrs p) {
+    PB_SETUP
+    for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
+    for (int i = tid; i < p.m; i += nt) {
+        const double zv = unpacked(p, p.bzp + om, i);
+        p.z[om + i] = zv; p.s[om + i] = -zv;
+    }
+}
+// starting point, part 2 (coneprog.py:2083-2106, :2165): x = dx, z = bzp, s = -z, then e shifts on both, gap.
+// SDP: k_init_sz has set x, z and s, and k_s_eig_start has left each block's smallest eigenvalues of s and z in
+// spart; snrm2 and sdot weigh the 's' rows, and the shifts go to the blocks' diagonal rows
+template <bool CONES, bool SDP = false> __global__ void k_init_point(Ptrs p) {
     PB_SETUP
     double *s = p.s + om, *z = p.z + om;
     const double *zn = p.bzp + om;                      // the solve leaves W uz in bzp
     double ns = 0, mins = INFINITY, minz = INFINITY;
-    for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
+    if (!SDP) for (int i = tid; i < p.n; i += nt) p.x[on + i] = p.dx[on + i];
     for (int i = tid; i < p.m; i += nt) {
-        const double zv = zn[i];
-        z[i] = zv; s[i] = -zv;
-        ns += zv * zv;
+        const double zv = SDP ? z[i] : zn[i];
+        if (SDP) ns += p.rw[i] * zv * zv;
+        else { z[i] = zv; s[i] = -zv; ns += zv * zv; }
         if (i < p.ml) { mins = fmin(mins, -zv); minz = fmin(minz, zv); }
     }
     if (CONES) FOR_CONES(o, len) {                      // s = -z: ||s1|| = ||z1||, s0 = -z0
         const double z0 = zn[o], mz = -q_max_step(wt, zn + o, len);
         mins = fmin(mins, -z0 - (z0 - mz));
         minz = fmin(minz, mz);
+    }
+    if (SDP && tid == 0) for (int k = 0; k < p.ns; ++k) {
+        const double *q = p.spart + ((long long)b * p.ns + k) * 4;
+        mins = fmin(mins, q[1]); minz = fmin(minz, q[2]);
     }
     ns = sqrt(block_sum(ns, sh));
     mins = block_min(mins, sh);
@@ -165,12 +187,14 @@ template <bool CONES> __global__ void k_init_point(Ptrs p) {
     const double as = (ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
     const double az = (tz >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + tz : 0.0;   // nrmz == nrms here
     for (int i = tid; i < p.ml; i += nt) { s[i] += as; z[i] += az; }
-    if (CONES) {
-        for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
-        __syncthreads();
-    }
+    if (CONES) for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
+    if (SDP) for (int i = p.mlq + tid; i < p.m; i += nt) if (p.rw[i] == 1.0) { s[i] += as; z[i] += az; }
+    if (CONES || SDP) __syncthreads();
     double gap = 0;
-    for (int i = tid; i < p.m; i += nt) gap += s[i] * z[i];
+    for (int i = tid; i < p.m; i += nt) {
+        if (SDP) gap += p.rw[i] * s[i] * z[i];
+        else gap += s[i] * z[i];
+    }
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
@@ -192,12 +216,17 @@ __global__ void k_res_dots(Ptrs p) {
 }
 // statistics + stopping rule (:2175-2234); row-wise, so every cone row is treated alike.  EQ with m = 0 is coneqp's
 // cdim == 0 branch (:2002-2040): the starting point is the solution, 'optimal' after 0 iterations, dcost = pcost.
-template <bool EQ> __global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol, double reltol,
-                                           double feastol, int *ndone, int *doneflags) {
+// SDP: snrm2(rz) and sdot(z, rz) weigh the 's' rows (rw), so only their lower triangles count
+template <bool EQ, bool SDP = false> __global__ void k_stats(Ptrs p, int iter, int maxiters, double abstol,
+                                                             double reltol, double feastol, int *ndone, int *doneflags) {
     PB_SETUP
     double rx2 = 0, rz2 = 0, zrz = 0, ry2 = 0, yry = 0;
     for (int i = tid; i < p.n; i += nt) { double v = p.rx[on + i]; rx2 += v * v; }
-    for (int i = tid; i < p.m; i += nt) { double v = p.rz[om + i]; rz2 += v * v; zrz += p.z[om + i] * v; }
+    for (int i = tid; i < p.m; i += nt) {
+        const double v = p.rz[om + i];
+        if (SDP) { const double w = p.rw[i]; rz2 += w * v * v; zrz += w * p.z[om + i] * v; }
+        else { rz2 += v * v; zrz += p.z[om + i] * v; }
+    }
     if (EQ) for (int i = tid; i < p.neq; i += nt) { double v = p.ry[oq + i]; ry2 += v * v; yry += p.y[oq + i] * v; }
     rx2 = block_sum(rx2, sh); rz2 = block_sum(rz2, sh); zrz = block_sum(zrz, sh);
     if (EQ) { ry2 = block_sum(ry2, sh); yry = block_sum(yry, sh); }
@@ -348,7 +377,10 @@ template <bool CONES, bool LP = false, bool SDP = false> __global__ void k_scali
             T.lgsq = T.lg * T.lg;
             S.mu = (ll + T.lgsq) / (1.0 + (SDP ? p.mdg : p.m)); S.sigma = 0.0;
         }
-    } else if (tid == 0) { S.mu = S.gap / (p.ml + p.nq); S.sigma = 0.0; S.eta = 0.0; }
+    } else if (tid == 0) {                           // SDP: the degree counts each block's order (:2357)
+        S.mu = SDP ? S.gap / (p.ml + p.nq + (p.mdg - p.mlq)) : S.gap / (p.ml + p.nq);
+        S.sigma = 0.0; S.eta = 0.0;
+    }
 }
 
 // f4_no_ir before the solve (coneprog.py:2301-2309): s := lmbda o\ s; z := z - W's; bzp := W^{-T} z.
@@ -370,7 +402,8 @@ __device__ __forceinline__ void f4_pre_cone(const Ptrs &p, long long om, long lo
     FOR_LANE(i, len) z[o + i] -= t[o + i];
     q_scale(wt, v + o, p.beta[oc + k], z + o, t + o, len, true);
 }
-// f4_no_ir after the solve (coneprog.py:2316), row r: z := W uz (the solve leaves it in bzp), s := s - z; returns z
+// f4_no_ir after the solve (coneprog.py:2316), row r: z := W uz (the solve leaves it in bzp), s := s - z; returns z.
+// Not for the rows of 's' blocks, which bzp holds packed (k_f4_post<EQ, true> unpacks them)
 __device__ __forceinline__ double f4_post_row(const Ptrs &p, long long r, double &s) {
     const double z = p.bzp[r];
     s -= z;
@@ -451,14 +484,16 @@ __global__ void k_f4_pre(Ptrs p, double *z, long long sz, double *s, long long s
     FOR_CONES(o, len) f4_pre_cone(p, om, oc, k_, o, len, lane, z, s);
 }
 // f4_no_ir after a solve that refinement follows or that is a refinement step.  acc: the refinement step,
-// (dx, dz, ds) += (x, z, s), and with EQ dy += wy2 (a refinement step's y is always wy2)
-template <bool EQ>
+// (dx, dz, ds) += (x, z, s), and with EQ dy += wy2 (a refinement step's y is always wy2).  SDP: z is unpacked from
+// bzp; a QP batch with 's' blocks also runs it after an unrefined solve, where k_s_dir_post reads its result
+template <bool EQ, bool SDP = false>
 __global__ void k_f4_post(Ptrs p, double *x, long long sx, double *z, long long sz, double *s, long long ss, int acc) {
     PB_SETUP
     x += b * sx; z += b * sz; s += b * ss;
     for (int i = tid; i < p.m; i += nt) {
-        double sv = s[i];
-        const double zv = f4_post_row(p, om + i, sv);
+        double sv = s[i], zv;
+        if (SDP) { zv = unpacked(p, p.bzp + om, i); sv -= zv; }
+        else zv = f4_post_row(p, om + i, sv);
         z[i] = zv; s[i] = sv;
         if (acc) { p.dz[om + i] += zv; p.ds[om + i] += sv; }
     }
@@ -680,10 +715,6 @@ __global__ void k_switch(double *aw, const int *info, int neq) {
 // step length and the update are coneqp's kernels with LP = true.
 // The primal start's solve has left uz in bzp: s = -uz (:698-701).  The dual start's right-hand side (-c, 0, 0):
 // k_init_rhs put -c in dx, here y = 0 and bz = 0 (:724-728)
-// value of m-row i (an 's' row when i >= mlq) of a vector whose 's' blocks are packed (bzp, z1)
-__device__ __forceinline__ double unpacked(const Ptrs &p, const double *x, int i) {
-    return i < p.mlq ? x[i] : x[p.mlq + p.u2p[i - p.mlq]] * (p.rw[i] == 1.0 ? 1.0 : M_SQRT1_2);
-}
 template <bool EQ, bool SDP = false> __global__ void k_lp_start_mid(Ptrs p) {
     PB_SETUP
     if (SDP) {
@@ -1106,19 +1137,20 @@ __global__ void __launch_bounds__(SB_T) k_s_eig_start(Ptrs p) {
     if (tid == 0) { part[1] = ok1 ? m1 : NAN; part[2] = ok2 ? s_min(ev, ms) : NAN; }
 }
 // the 's' rows of the refinement residual res() (coneprog.py:599-631): wz3 = W^{-1} dz = rti dz rti',
-// wz2 = wz + ut h - W' ds = wz + ut h - r ds r', ws2 = ws - lmbda o (dz + ds); part[0] = sdot(h, wz3)
-__global__ void __launch_bounds__(SB_T) k_s_res(Ptrs p) {
+// wz2 = wz + ut h - W' ds = wz + ut h - r ds r', ws2 = ws - lmbda o (dz + ds); part[0] = sdot(h, wz3).
+// A QP batch (LP = false) has no embedding: coneqp's res() (coneprog.py:1930-1960) is the same without ut and h'wz3
+template <bool LP> __global__ void __launch_bounds__(SB_T) k_s_res(Ptrs p) {
     SB_SETUP
     SB_PART;
     __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX], H[SMX], sh[32];
-    const double ut = lp_scal(p, oc).dtau / lp_scal(p, oc).dg;
+    const double ut = LP ? lp_scal(p, oc).dtau / lp_scal(p, oc).dg : 0.0;
     s_load(X, p.dz + om + so, ms);
-    s_load(H, p.h + om + so, ms);
+    if (LP) s_load(H, p.h + om + so, ms);
     SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
     __syncthreads();
     s_congr(Y, R, X, T, false, ms);
     s_store(p.wz3 + oc + so, Y, ms);
-    const double hz = s_dot(H, Y, ms, sh);
+    const double hz = LP ? s_dot(H, Y, ms, sh) : 0.0;
     s_load(Y, p.ds + om + so, ms);
     SB_FOR(e, ms) { R[e] = p.sr[oc + sro + e]; X[e] += Y[e]; }      // X := dz + ds
     __syncthreads();
@@ -1126,10 +1158,10 @@ __global__ void __launch_bounds__(SB_T) k_s_res(Ptrs p) {
     s_mm(Y, R, false, T, false, ms);                                 // Y := W' ds = r ds r'
     SB_FOR(e, ms) {
         const int i = e % ms, j = e / ms, lo = i >= j ? e : j + i * ms;
-        p.wz2[oc + so + e] = (p.wz[oc + so + lo] + ut * H[e]) - Y[e];
+        p.wz2[oc + so + e] = (LP ? p.wz[oc + so + lo] + ut * H[e] : p.wz[oc + so + lo]) - Y[e];
         p.ws2[oc + so + e] = p.ws[oc + so + lo] - 0.5 * (s_lam(p, om, so, ms, i) + s_lam(p, om, so, ms, j)) * X[e];
     }
-    if (tid == 0) part[0] = hz;
+    if (LP && tid == 0) part[0] = hz;
 }
 // after the i-th direction (coneprog.py:1302-1321): part[0] = sdot(ds, dz); i = 0: ws3 = ds o dz; ds and dz scaled
 // by lambda^{-1/2} on both sides (scale2); part[1], part[2] their smallest eigenvalues; i = 1 also leaves the
@@ -1429,12 +1461,14 @@ template <bool CONES, bool EQ, bool LP, bool SDP = false> int direction(cvxb_bat
     k_dir_rhs<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, i); count_launch();
     if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.dz, m, p.ds, m, 2); count_launch(); }
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
+    // f4_no_ir's step after the solve: k_dir_post folds it in for an unrefined QP solve, except with 's' blocks, whose
+    // rows k_s_dir_post reads before k_dir_post runs
     if (LP) { k_lp_f6_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch(); }
-    else if (p.refinement) { k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
+    else if (p.refinement || SDP) { k_f4_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
     for (int r = 0; r < p.refinement; ++r) {
         // res() (coneprog.py:1930-1952, :599-631): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx,
         // wz2 -= G dx + W' ds; an LP has no P
-        if (SDP) { k_s_res<<<sg, SB_T, 0, st>>>(p); count_launch(); }
+        if (SDP) { k_s_res<LP><<<sg, SB_T, 0, st>>>(p); count_launch(); }
         k_res<EQ, LP, SDP><<<B, T, 0, st>>>(p); count_launch();
         if (!LP) {
             GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
@@ -1456,11 +1490,11 @@ template <bool CONES, bool EQ, bool LP, bool SDP = false> int direction(cvxb_bat
         if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.wz2, L, p.ws2, L, 2); count_launch(); }
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
         if (LP) k_lp_f6_post<EQ, SDP><<<B, T, 0, st>>>(p, p.wx2, L, p.wy2, L, p.ws2, L, 1);
-        else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
+        else k_f4_post<EQ, SDP><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
         count_launch();
     }
     if (SDP) { k_s_dir_post<<<sg, SB_T, 0, st>>>(p, i); count_launch(); }
-    k_dir_post<CONES, LP, SDP><<<B, T, 0, st>>>(p, i, !LP && p.refinement == 0); count_launch();
+    k_dir_post<CONES, LP, SDP><<<B, T, 0, st>>>(p, i, !LP && !SDP && p.refinement == 0); count_launch();
     return 0;
 }
 
@@ -1592,7 +1626,11 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
         k_lp_init_point<CONES, EQ, SDP><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
     } else {
         CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
-        k_init_point<CONES><<<B, T, 0, st>>>(p); count_launch();
+        if (SDP) {
+            k_init_sz<<<B, T, 0, st>>>(p); count_launch();
+            k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch();
+        }
+        k_init_point<CONES, SDP><<<B, T, 0, st>>>(p); count_launch();
     }
     CVXB_LAUNCH_CHECK();
     CVXB_TRY(start_check<EQ>(b));
@@ -1617,7 +1655,7 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
         if (LP) k_lp_stats<EQ, SDP><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
-        else k_stats<EQ><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        else k_stats<EQ, SDP><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
         int ndone = 0;
         CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1671,8 +1709,8 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
     return 0;
 }
 
-// a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q') and p equality rows.
-// Every argument is checked before the device is.
+// a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q', and with sdp 's' blocks)
+// and p equality rows.  Every argument is checked before the device is.
 int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp, bool sdp = false) {
     if (out) *out = nullptr;
     if (!out || nprob <= 0 || n <= 0 || !dims) {
@@ -1888,6 +1926,10 @@ int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_
     return create(out, nprob, n, p, dims, device, true, true);
 }
 
+int cvxb_batch_create_sdp_qp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
+    return create(out, nprob, n, p, dims, device, false, true);
+}
+
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
@@ -1954,10 +1996,12 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
                                      solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,
                                      solve<false, true, true>,   solve<true, true, true>};
-    static const Solve sdp_solvers[4] = {solve<false, false, true, true>, solve<true, false, true, true>,
-                                         solve<false, true, true, true>, solve<true, true, true, true>};
+    static const Solve sdp_solvers[8] = {solve<false, false, false, true>, solve<true, false, false, true>,
+                                         solve<false, true, false, true>,  solve<true, true, false, true>,
+                                         solve<false, false, true, true>,  solve<true, false, true, true>,
+                                         solve<false, true, true, true>,   solve<true, true, true, true>};
     const int k = (b->p.nq > 0 ? 1 : 0) + (b->neq > 0 ? 2 : 0) + (b->lp ? 4 : 0);     // CONES, EQ, LP
-    if (b->p.ns > 0) return sdp_solvers[k & 3](b, maxiters, abstol, reltol, feastol);  // SDP batches are cone LPs
+    if (b->p.ns > 0) return sdp_solvers[k](b, maxiters, abstol, reltol, feastol);     // 's' blocks of positive order
     return solvers[k](b, maxiters, abstol, reltol, feastol);
 }
 

@@ -293,6 +293,21 @@ int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_d
  * cdim - ml - sum(q) + 5 ns ints of layout; all of it is counted by cvxb_device_bytes and freed by
  * cvxb_batch_destroy. */
 int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
+/* batch of QPs  min 1/2 x'Px + q'x  s.t.  G x + s = h,  s in 'l' x 'q' x 's' cones,  A x = b  with p equality rows per
+ * problem: B x coneqp(P, q, G, h, dims, A, b) with its default kktsolver ('chol' with 's' cones), each 's' order at
+ * most CVXB_BATCH_SMAX.  It refuses, before the device, what cvxb_batch_create_eq refuses (CVXB_E_ARG: dims->mnl != 0,
+ * a cone order q[k] < 1, nprob > CVXB_BATCH_MAX, p < 0, and coneqp's only rank check, p > n) and an order s[k] < 0
+ * (CVXB_E_ARG) or s[k] > CVXB_BATCH_SMAX (CVXB_E_UNSUP); p + cdim_pckd < n is accepted, since P may have full rank.
+ * Load it with cvxb_batch_load (and cvxb_batch_load_eq when p > 0), G and h laid out as for cvxb_batch_create_sdp;
+ * results come back through cvxb_batch_results (s and z with symmetric 's' blocks) and cvxb_batch_results_y.  A
+ * singular factorisation at the start makes cvxb_batch_solve return CVXB_E_ARG naming the problem.  Refinement
+ * defaults to 1.  Device memory per problem, in doubles: that of the cvxb_batch_create_eq batch of the same n, cdim
+ * (with the 's' blocks unpacked) and p, plus ldg*n for Gs if dims has no 'q' cone, 2*sum(s^2) + 2*sum(s) (r, rti,
+ * sigs, sigz) each rounded up to even in the state row, and 4 per block of partial sums; and, shared by the batch,
+ * cdim doubles of row weights and cdim - ml - sum(q) + 5 ns ints of layout; all of it is counted by
+ * cvxb_device_bytes and freed by cvxb_batch_destroy.  Dims without an 's' block of positive order run exactly what
+ * cvxb_batch_create_eq's batch runs. */
+int cvxb_batch_create_sdp_qp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);
