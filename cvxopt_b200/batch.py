@@ -87,6 +87,74 @@ def _stack_eq(A, b, B, n):
     return Acm, np.ascontiguousarray(np.asarray(b, dtype=np.float64)), p
 
 
+def _start_arrays(start, B, n, p, m, what="initvals"):
+    """a start dict with keys among x, s, y, z -> {key: contiguous float64 (B, len)}: x (B, n), y (B, p), s and z
+    (B, cdim) laid out as h.  An unknown key or a wrong shape is a TypeError"""
+    if not isinstance(start, dict):
+        raise TypeError("'%s' must be a dictionary" % what)
+    lens = {"x": n, "s": m, "y": p, "z": m}
+    out = {}
+    for key, v in start.items():
+        if key not in lens:
+            raise TypeError("'%s' has an unknown key %r" % (what, key))
+        a = np.ascontiguousarray(np.asarray(v, dtype=np.float64))
+        if a.shape != (B, lens[key]):
+            raise TypeError("%s['%s'] must have shape (%d, %d)" % (what, key, B, lens[key]))
+        out[key] = a
+    return out
+
+
+def _lp_start(primalstart, dualstart, B, n, p, m):
+    """conelp's primalstart {'x', 's'} and dualstart {'z'[, 'y']} -> one _start_arrays dict, or None without either"""
+    start = {}
+    if primalstart is not None:
+        if not isinstance(primalstart, dict) or set(primalstart) != {"x", "s"}:
+            raise TypeError("'primalstart' must be a dictionary with keys 'x' and 's'")
+        start.update(_start_arrays(primalstart, B, n, p, m, "primalstart"))
+    if dualstart is not None:
+        if not isinstance(dualstart, dict) or "z" not in dualstart or not set(dualstart) <= {"y", "z"}:
+            raise TypeError("'dualstart' must be a dictionary with key 'z' and optionally 'y'")
+        start.update(_start_arrays(dualstart, B, n, p, m, "dualstart"))
+    return start or None
+
+
+def _sdp_start(primalstart, dualstart, B, n, p, ml, ms):
+    """sdp's primalstart {'x', 'sl', 'ss'} and dualstart {'zl', 'zs'[, 'y']} -> conelp's, 'ss' / 'zs' lists of
+    (B, ms, ms) unpacked column-major after the 'l' rows as _sdp_args assembles hs"""
+    def stack(d, lk, sk, what):
+        if ml and lk not in d or ms and sk not in d:
+            raise TypeError("'%s' must have the keys %s" % (what, ", ".join(repr(k) for k in
+                                                                           ([lk] if ml else []) + ([sk] if ms else []))))
+        parts = []
+        if ml:
+            v = np.asarray(d[lk], dtype=np.float64)
+            if v.shape != (B, ml):
+                raise TypeError("%s['%s'] must have shape (%d, %d)" % (what, lk, B, ml))
+            parts.append(v)
+        if ms:
+            blocks = d[sk]
+            if not isinstance(blocks, list) or len(blocks) != len(ms):
+                raise TypeError("%s['%s'] must be a list of %d arrays" % (what, sk, len(ms)))
+            for k, (v, o) in enumerate(zip(blocks, ms)):
+                v = np.asarray(v, dtype=np.float64)
+                if v.shape != (B, o, o):
+                    raise TypeError("%s['%s'][%d] must have shape (%d, %d, %d)" % (what, sk, k, B, o, o))
+                parts.append(v.transpose(0, 2, 1).reshape(B, -1))
+        return np.concatenate(parts, axis=1) if parts else np.zeros((B, 0))
+    ps = ds = None
+    if primalstart is not None:
+        if not isinstance(primalstart, dict) or "x" not in primalstart or not set(primalstart) <= {"x", "sl", "ss"}:
+            raise TypeError("'primalstart' must be a dictionary with keys 'x', 'sl' and 'ss'")
+        ps = {"x": primalstart["x"], "s": stack(primalstart, "sl", "ss", "primalstart")}
+    if dualstart is not None:
+        if not isinstance(dualstart, dict) or not set(dualstart) <= {"y", "zl", "zs"}:
+            raise TypeError("'dualstart' must be a dictionary with keys 'zl', 'zs' and optionally 'y'")
+        ds = {"z": stack(dualstart, "zl", "zs", "dualstart")}
+        if "y" in dualstart:
+            ds["y"] = dualstart["y"]
+    return _lp_start(ps, ds, B, n, p, ml + sum(k * k for k in ms))
+
+
 def _sdp_dims(dims, m=None):
     """_batch_dims for SDPBatch: dims may hold 's' blocks"""
     from . import kkt
@@ -160,6 +228,23 @@ class QPBatch:
         _lib.check(self._lib.cvxb_batch_load(self._h, P, q, G, h, space), "batch_load")
         self._load_eq(A, b, space)
 
+    def load_start(self, x=None, s=None, y=None, z=None):
+        """the starting point of the next solves, kept until load_start or clear_start: coneqp's initvals on a QP batch
+        (absent keys: x = y = 0, s = z = e), conelp's primalstart (x and s) and / or dualstart (z, optionally y) on a
+        cone LP batch.  x (B, n), y (B, p), s and z (B, cdim) laid out as h; only the lower triangle of an 's' block is
+        read"""
+        given = {k: v for k, v in (("x", x), ("s", s), ("y", y), ("z", z)) if v is not None}
+        a = _start_arrays(given, self.B, self.n, self.p, self.m)
+        self.load_start_ptr(*(a[k].ctypes.data if k in a else None for k in "xsyz"), space=_lib.HOST)
+
+    def load_start_ptr(self, x=None, s=None, y=None, z=None, space=_lib.DEVICE):
+        """load_start from raw addresses in `space` of (B, n), (B, cdim), (B, p) and (B, cdim) arrays; None: absent"""
+        _lib.check(self._lib.cvxb_batch_load_start(self._h, x, s, y, z, space), "batch_load_start")
+
+    def clear_start(self):
+        """back to the cold start"""
+        _lib.check(self._lib.cvxb_batch_clear_start(self._h), "batch_clear_start")
+
     def solve(self, refinement=None, **options):
         """refinement: steps of iterative refinement per Newton solve (coneqp's option); None keeps the default
         (1 with 'q' cones, else 0)"""
@@ -172,8 +257,8 @@ class QPBatch:
             self._refinement = refinement
         rc = self._lib.cvxb_batch_solve(self._h, int(o["maxiters"]), float(o["abstol"]),
                                         float(o["reltol"]), float(o["feastol"]))
-        if rc == _lib.E_ARG and "Rank(" in _lib.last_error():
-            raise ValueError(_lib.last_error())       # coneprog.py:2065-2067
+        if rc == _lib.E_ARG and ("Rank(" in _lib.last_error() or "is not positive" in _lib.last_error()):
+            raise ValueError(_lib.last_error())       # coneprog.py:2065-2067, :2130, :2144
         _lib.check(rc, "batch_solve")
 
     def results(self):
@@ -271,6 +356,17 @@ class QPBatchGroup:
             b = np.asarray(b)
         for ix, part in zip(self.idx, self.parts):
             part.load(*(a[ix] for a in data), None if A is None else A[ix], None if b is None else b[ix])
+
+    def load_start(self, x=None, s=None, y=None, z=None):
+        """QPBatch.load_start on every part with its slice of the arrays"""
+        given = {k: v for k, v in (("x", x), ("s", s), ("y", y), ("z", z)) if v is not None}
+        a = _start_arrays(given, self.B, self.n, self.p, self.m)
+        for ix, part in zip(self.idx, self.parts):
+            part.load_start(**{k: v[ix] for k, v in a.items()})
+
+    def clear_start(self):
+        for part in self.parts:
+            part.clear_start()
 
     def solve(self, **options):
         if self.nsub == 1:
@@ -383,14 +479,17 @@ def _lp_shapes(c, G, h, dims, A, b):
     return B, n, cdim, p
 
 
-def conelp_batch(c, G, h, dims=None, A=None, b=None, device=0, nsub=None, **options):
+def conelp_batch(c, G, h, dims=None, A=None, b=None, device=0, nsub=None, primalstart=None, dualstart=None,
+                 **options):
     """Solve B independent cone LPs on one GPU, each as solvers.conelp(c, G, h, dims, A, b) does.  c (B,n),
     G (B,cdim,n), h (B,cdim); optional A (B,p,n), b (B,p), given together.  dims: shared by every problem ('l' and
     'q' only); None is {'l': cdim}, i.e. solvers.lp.  nsub and the returned dict are qp_batch's; status is 'optimal',
     'primal infeasible', 'dual infeasible' or 'unknown', and entries the reference returns as None are NaN.
+    primalstart {'x': (B,n), 's': (B,cdim)} and dualstart {'z': (B,cdim), 'y': (B,p) optional} are conelp's.
     options: maxiters, abstol, reltol, feastol, refinement (as conelp's)."""
     B, n, cdim, p = _lp_shapes(c, G, h, dims, A, b)
-    return _run_group(ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p), (c, G, h, A, b), options)
+    start = _lp_start(primalstart, dualstart, B, n, p, cdim)
+    return _run_group(ConeLPBatchGroup(B, n, cdim, device, nsub, dims, p), (c, G, h, A, b), options, start)
 
 
 class SDPBatch(ConeLPBatch):
@@ -459,17 +558,21 @@ def _sdp_args(c, Gl, hl, Gs, hs, A, b):
     return c, G, h, {"l": ml, "q": [], "s": ms}, A, b, ms
 
 
-def sdp_batch(c, Gl=None, hl=None, Gs=None, hs=None, A=None, b=None, device=0, nsub=None, **options):
+def sdp_batch(c, Gl=None, hl=None, Gs=None, hs=None, A=None, b=None, device=0, nsub=None, primalstart=None,
+              dualstart=None, **options):
     """Solve B independent SDPs on one GPU, each as solvers.sdp(c, Gl, hl, Gs, hs, A, b, kktsolver='chol') does.
     c (B, n), Gl (B, ml, n), hl (B, ml), Gs a list of (B, ms², n), hs a list of (B, ms, ms), A (B, p, n), b (B, p);
     every 's' order at most 32.  Returns sdp's keys x, sl, ss (list of (B, ms, ms)), y, zl, zs, status, status_code,
     iterations, primal objective, dual objective, with conelp_batch's stats; NaN where sdp returns None.
+    primalstart {'x', 'sl', 'ss'} and dualstart {'zl', 'zs', 'y'} are sdp's, in the shapes of x, hl, hs and b; 'sl' /
+    'zl' are needed when ml > 0, 'ss' / 'zs' when there are 's' blocks, and 'y' is optional (0 without it).
     options: maxiters, abstol, reltol, feastol, refinement (as sdp's)."""
     c, G, h, dims, A, b, ms = _sdp_args(c, Gl, hl, Gs, hs, A, b)
     B, n = c.shape
     p = A.shape[1]
+    start = _sdp_start(primalstart, dualstart, B, n, p, dims["l"], ms)
     out = _run_group(SDPBatchGroup(B, n, dims, p, device, nsub), (c, G, h, A if p else None, b if p else None),
-                     options)
+                     options, start)
     ml = dims["l"]
     for key in ("s", "z"):
         v = out.pop(key)
@@ -504,24 +607,29 @@ class SDPQPBatchGroup(QPBatchGroup):
         return lambda nprob, n, m, device, dims, p=0: SDPQPBatch(nprob, n, dims, p, device)
 
 
-def coneqp_batch(P, q, G, h, dims, A=None, b=None, device=0, nsub=None, **options):
+def coneqp_batch(P, q, G, h, dims, A=None, b=None, device=0, nsub=None, initvals=None, **options):
     """Solve B independent cone QPs on one GPU, each as solvers.coneqp(P, q, G, h, dims, A, b) does.  P (B,n,n),
     q (B,n), G (B,cdim,n), h (B,cdim); optional A (B,p,n), b (B,p), given together.  dims: shared by every problem,
     with 'l', 'q' and 's' (orders at most 32); each 's' block's rows of G and h are unpacked column-major, as the
     reference's G, and only their lower triangles are read.  nsub and the returned dict are qp_batch's; its s and z
-    have symmetric 's' blocks.  options: maxiters, abstol, reltol, feastol, refinement (as coneqp's)."""
+    have symmetric 's' blocks.  initvals: qp_batch's.  options: maxiters, abstol, reltol, feastol, refinement (as
+    coneqp's)."""
     _, _, _, _, B, n, m = _stack(P, q, G, h)
     _sdp_dims(dims, m)
     p = _eq_rows(A, b, B, n)
     if p > n:
         raise ValueError("Rank(A) < p or Rank([P; G; A]) < n")        # coneprog.py:1970-1971
-    return _run_group(SDPQPBatchGroup(B, n, dims, p, device, nsub), (P, q, G, h, A, b), options)
+    start = None if initvals is None else _start_arrays(initvals, B, n, p, m)
+    return _run_group(SDPQPBatchGroup(B, n, dims, p, device, nsub), (P, q, G, h, A, b), options, start)
 
 
-def _run_group(grp, data, options):
-    """load `data` into the batch group, solve it timed, and return its results and stats; the group is closed"""
+def _run_group(grp, data, options, start=None):
+    """load `data` (and a start dict of load_start's keys) into the batch group, solve it timed, and return its results
+    and stats; the group is closed"""
     try:
         grp.load(*data)
+        if start is not None:
+            grp.load_start(**start)
         import time
         t0 = time.perf_counter()
         grp.solve(**options)
@@ -534,12 +642,14 @@ def _run_group(grp, data, options):
         grp.close()
 
 
-def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, **options):
+def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, initvals=None, **options):
     """Solve B independent dense QPs on one GPU.  P (B,n,n), q (B,n), G (B,cdim,n), h (B,cdim); optional
     equality constraints A (B,p,n) x = b (B,p), given together.
     nsub: number of concurrently solved sub-batches (QPBatchGroup); default 4 (1 for tiny batches), and never fewer
     than ceil(B / 65535), the most problems one library batch holds.
     dims: cone dimensions shared by every problem ({'l': ml, 'q': [...]}); None is {'l': cdim}.
+    initvals: coneqp's starting point {'x': (B,n), 's': (B,cdim), 'y': (B,p), 'z': (B,cdim)}, every key optional
+    (x = y = 0 and s = z = e without it; {} is the e start); None is the default start.
     options: maxiters, abstol, reltol, feastol, refinement (as coneqp's)."""
     P = np.asarray(P)
     G = np.asarray(G)
@@ -547,7 +657,9 @@ def qp_batch(P, q, G, h, A=None, b=None, device=0, nsub=None, dims=None, **optio
         raise TypeError("P must have shape (B, n, n) and G (B, cdim, n)")
     _, _, cdim = _batch_dims(dims, G.shape[1])
     p = _eq_rows(A, b, P.shape[0], P.shape[1])
-    return _run_group(QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims, p), (P, q, G, h, A, b), options)
+    start = None if initvals is None else _start_arrays(initvals, P.shape[0], P.shape[1], p, cdim)
+    return _run_group(QPBatchGroup(P.shape[0], P.shape[1], cdim, device, nsub, dims, p), (P, q, G, h, A, b), options,
+                      start)
 
 
 # ---------------------------------------------------------------------------------------
@@ -590,9 +702,12 @@ def qp_batch_distributed(P, q, G, h, A=None, b=None, solver=None, group=None, sh
     rank 0 additionally gets the gathered batch, in the original problem order, under key 'all'.
     Every rank passes the same `dims` (and options); shards are (k, cdim, n).  Equality constraints A (B,p,n),
     b (B,p) travel with the other inputs and y comes back with x; a stand-in `solver` then receives A and b too.
+    It takes no starting point: every shard starts cold (qp_batch's initvals is not forwarded).
 
     `timings` (dict, optional) receives scatter_ms / solve_ms / gather_ms of this rank, measured with
     device events on the current stream (wall clock on CPU)."""
+    if "initvals" in options:
+        raise TypeError("qp_batch_distributed takes no starting point (initvals)")
     import time
     import torch
     import torch.distributed as dist

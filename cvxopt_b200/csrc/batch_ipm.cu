@@ -76,6 +76,10 @@ struct LPScal {
 __device__ __forceinline__ LPScal &lp_scal(const Ptrs &p, long long oc) {
     return *reinterpret_cast<LPScal *>(p.lps + oc);
 }
+// a loaded start (cvxb_batch_load_start) in problem order, laid out as x, y, s and z; nullptr: the key is absent
+struct Warm {
+    const double *x, *y, *s, *z;
+};
 #define PB_SETUP                                                                                       \
     const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;                                      \
     const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;                                       \
@@ -197,6 +201,71 @@ template <bool CONES, bool SDP = false> __global__ void k_init_point(Ptrs p) {
     }
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
+}
+// a loaded start, part 1: x, y, s and z.  QP (coneqp's initvals, coneprog.py:2109-2149): the given keys, else x = y = 0
+// and s = z = e.  LP (conelp's primalstart / dualstart, :689-740): x and s given or, without them, the W = I solve's x
+// and s = -uz; z given (y given or 0) or, without it, the W = I solve's y and z = uz.  A given 's' block is read from
+// its lower triangle and stored symmetric
+template <bool CONES, bool EQ, bool LP, bool SDP = false> __global__ void k_warm_copy(Ptrs p, Warm w) {
+    PB_SETUP
+    const double *bz = p.bzp + om;                      // the W = I solve's uz (SDP: packed)
+    if (w.x) for (int i = tid; i < p.n; i += nt) p.x[on + i] = w.x[on + i];
+    else if (!LP) for (int i = tid; i < p.n; i += nt) p.x[on + i] = 0.0;
+    if (EQ && (!LP || w.z)) for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = w.y ? w.y[oq + i] : 0.0;
+    auto fill = [&](double *v, const double *g, double sg) {
+        for (int i = tid; i < p.ml; i += nt) v[i] = g ? g[om + i] : LP ? sg * bz[i] : 1.0;
+        if (CONES) FOR_CONES(o, len) FOR_LANE(i, len)
+            v[o + i] = g ? g[om + o + i] : LP ? sg * bz[o + i] : (i == 0 ? 1.0 : 0.0);
+        if (SDP) for (int k = 0; k < p.ns; ++k) {
+            const int ms = p.sinfo[5 * k], so = p.sinfo[5 * k + 1];
+            for (int e = tid; e < ms * ms; e += nt) {
+                const int r = e % ms, c = e / ms, lo = so + (r >= c ? e : c + r * ms);
+                v[so + e] = g ? g[om + lo] : LP ? sg * unpacked(p, bz, so + e) : (r == c ? 1.0 : 0.0);
+            }
+        }
+    };
+    fill(p.s + om, w.s, -1.0);
+    fill(p.z + om, w.z, 1.0);
+}
+// a loaded start, part 2 (coneprog.py:704-740, :842-857, :2128-2165): ts and tz (SDP: the blocks' smallest
+// eigenvalues from k_s_eig_warm), bad[b] = 1 (2) when the given s (z) is not strictly inside the cone; a one-sided
+// cone LP start shifts the other half by 1 + ts or 1 + tz; tau = kappa = 1, gap = sdot(s, z)
+template <bool CONES, bool EQ, bool LP, bool SDP = false> __global__ void k_warm_point(Ptrs p, Warm w, int *bad) {
+    PB_SETUP
+    double *s = p.s + om, *z = p.z + om;
+    double ns = 0, nz = 0, mins = INFINITY, minz = INFINITY;
+    for (int i = tid; i < p.m; i += nt) {
+        const double sv = s[i], zv = z[i], wr = SDP ? p.rw[i] : 1.0;
+        ns += wr * sv * sv; nz += wr * zv * zv;
+        if (i < p.ml) { mins = fmin(mins, sv); minz = fmin(minz, zv); }
+    }
+    if (CONES) FOR_CONES(o, len) {
+        mins = fmin(mins, -q_max_step(wt, s + o, len));
+        minz = fmin(minz, -q_max_step(wt, z + o, len));
+    }
+    if (SDP && tid == 0) for (int k = 0; k < p.ns; ++k) {
+        const double *q = p.spart + ((long long)b * p.ns + k) * 4;
+        mins = fmin(mins, q[1]); minz = fmin(minz, q[2]);
+    }
+    ns = sqrt(block_sum(ns, sh)); nz = sqrt(block_sum(nz, sh));
+    mins = block_min(mins, sh); minz = block_min(minz, sh);
+    const double ts = -mins, tz = -minz;
+    if (tid == 0) bad[b] = (w.s && ts >= 0.0) ? 1 : (w.z && tz >= 0.0) ? 2 : 0;
+    if (LP) {
+        const double as = (!w.s && ts >= -1e-8 * fmax(ns, 1.0)) ? 1.0 + ts : 0.0;
+        const double az = (!w.z && tz >= -1e-8 * fmax(nz, 1.0)) ? 1.0 + tz : 0.0;
+        for (int i = tid; i < p.ml; i += nt) { s[i] += as; z[i] += az; }
+        if (CONES) for (int k = tid; k < p.nq; k += nt) { s[p.qoff[k]] += as; z[p.qoff[k]] += az; }
+        if (SDP) for (int i = p.mlq + tid; i < p.m; i += nt) if (p.rw[i] == 1.0) { s[i] += as; z[i] += az; }
+        __syncthreads();
+    }
+    double gap = 0;
+    for (int i = tid; i < p.m; i += nt) gap += (SDP ? p.rw[i] : 1.0) * s[i] * z[i];
+    gap = block_sum(gap, sh);
+    if (tid == 0) {
+        S.gap = gap;
+        if (LP) { LPScal &T = lp_scal(p, oc); T.tau = 1.0; T.kappa = 1.0; }
+    }
 }
 // residuals, part 1: rx = q (then rx += P x by GEMV), rz = s - h; EQ: ry = b (then ry := A x - ry).
 // LP: rx = 0, rz = s, ry = 0; the GEMVs then make them conelp's hrx = -A'y - G'z, hrz = s + G x, hry = A x (:861-896)
@@ -1136,6 +1205,18 @@ __global__ void __launch_bounds__(SB_T) k_s_eig_start(Ptrs p) {
     const bool ok2 = s_eig(A, W, V, ev, ms, sh);
     if (tid == 0) { part[1] = ok1 ? m1 : NAN; part[2] = ok2 ? s_min(ev, ms) : NAN; }
 }
+// k_s_eig_start for a loaded start, whose s and z are both unpacked (k_warm_copy)
+__global__ void __launch_bounds__(SB_T) k_s_eig_warm(Ptrs p) {
+    SB_SETUP
+    SB_PART;
+    __shared__ double A[SMX], W[SMX], V[SMX], ev[CVXB_BATCH_SMAX], sh[32];
+    s_load(A, p.s + om + so, ms);
+    const bool ok1 = s_eig(A, W, V, ev, ms, sh);
+    const double m1 = s_min(ev, ms);
+    s_load(A, p.z + om + so, ms);
+    const bool ok2 = s_eig(A, W, V, ev, ms, sh);
+    if (tid == 0) { part[1] = ok1 ? m1 : NAN; part[2] = ok2 ? s_min(ev, ms) : NAN; }
+}
 // the 's' rows of the refinement residual res() (coneprog.py:599-631): wz3 = W^{-1} dz = rti dz rti',
 // wz2 = wz + ut h - W' ds = wz + ut h - r ds r', ws2 = ws - lmbda o (dz + ds); part[0] = sdot(h, wz3).
 // A QP batch (LP = false) has no embedding: coneqp's res() (coneprog.py:1930-1960) is the same without ut and h'wz3
@@ -1293,6 +1374,11 @@ struct cvxb_batch {
     long long sums = 0, sums2 = 0;   // sum of the orders, of their squares
     DevBuf<int> sinfo, u2p;
     DevBuf<double> rw, spart;
+    // the start (cvxb_batch_load_start): B * (n + p + 2 cdim) doubles in problem order, allocated on the first load;
+    // warm_set until cvxb_batch_clear_start, warm's pointers into it for the given keys
+    DevBuf<double> start;
+    Warm warm{};
+    bool warm_set = false;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -1534,12 +1620,11 @@ int restore_order(cvxb_batch *b) {
     return 0;
 }
 
-// the starting point's factorisation with W = I.  EQ: kkt_chol2's first factorisation (misc.py:1421-1447): a problem
-// whose S is singular factors S + A'A from now on
-template <bool EQ> int start_factor(cvxb_batch *b) {
+// kkt_chol2's first factorisation (misc.py:1421-1447) once batch_factor(b, false) has factored S: a problem whose S is
+// singular factors S + A'A from now on; then Kp.  Nothing to do without equality rows
+template <bool EQ> int first_switch(cvxb_batch *b) {
     cudaStream_t st = b->st;
     const int B = b->Bact;
-    CVXB_TRY(batch_factor(b, false));
     if (EQ) {
         std::vector<int> info(B);
         CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1553,9 +1638,15 @@ template <bool EQ> int start_factor(cvxb_batch *b) {
     }
     return 0;
 }
+// the starting point's factorisation with W = I, kkt_chol2's first
+template <bool EQ> int start_factor(cvxb_batch *b) {
+    CVXB_TRY(batch_factor(b, false));
+    return first_switch<EQ>(b);
+}
 
 // a singular first factorisation is the reference's "Rank(A) < p or Rank([P; A; G]) < n" ValueError
-// (coneprog.py:2065-2067), without A Rank([P; G]) < n; conelp's is "Rank(A) < p or Rank([G; A]) < n" (:680-700)
+// (coneprog.py:2065-2067), without A Rank([P; G]) < n; conelp's is "Rank(A) < p or Rank([G; A]) < n" (:680-700).
+// After a loaded start the first factorisation is iteration 0's (:2256-2259, :1078-1080), over the active slots
 template <bool EQ> int start_check(cvxb_batch *b) {
     cudaStream_t st = b->st;
     const int B = b->Bact;
@@ -1565,11 +1656,50 @@ template <bool EQ> int start_check(cvxb_batch *b) {
     CVXB_CUDA(cudaStreamSynchronize(st));
     for (int i = 0; i < B; ++i)
         if (info[i] > 0 || (EQ && infop[i] > 0)) {
+            const int k = b->perm[i];
             if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
-                                 "the start)", i);
+                                 "the start)", k);
             else if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
-                                   "at the start)", i);
-            else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", i);
+                                   "at the start)", k);
+            else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", k);
+            return CVXB_E_ARG;
+        }
+    return 0;
+}
+
+// the starting point from a loaded start (coneqp :2109-2149, conelp :662-857).  A cone LP with one of primalstart and
+// dualstart factors W = I and solves for the other half; coneqp and a cone LP with both skip the factorisation, so
+// that iteration 0's is the first.  A given s or z not strictly inside the cone is CVXB_E_ARG naming the problem
+template <bool CONES, bool EQ, bool LP, bool SDP> int warm_start(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
+    const Ptrs &p = b->p;
+    const Warm w = b->warm;
+    if (LP && !(w.s && w.z)) {
+        CVXB_TRY(start_factor<EQ>(b));
+        if (!w.s) {                                                // primal start (0, b, h): s = -uz
+            k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
+            if (SDP) { k_s_wtz<<<dim3(p.ns, B), SB_T, 0, st>>>(p, p.dz, m, nullptr, 0, 0); count_launch(); }
+            CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
+            CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));
+        } else {                                                   // dual start (-c, 0, 0): z = uz
+            CVXB_CUDA(cudaMemsetAsync(p.bzp, 0, (size_t)B * m * sizeof(double), st));
+            if (EQ) CVXB_CUDA(cudaMemsetAsync(p.y, 0, (size_t)B * pq * sizeof(double), st));
+            CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
+        }
+        CVXB_LAUNCH_CHECK();
+        CVXB_TRY(start_check<EQ>(b));
+    }
+    k_warm_copy<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, w); count_launch();
+    if (SDP) { k_s_eig_warm<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
+    k_warm_point<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, w, b->d_info.p); count_launch();
+    CVXB_LAUNCH_CHECK();
+    std::vector<int> bad(B);
+    CVXB_CUDA(cudaMemcpyAsync(bad.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i < B; ++i)
+        if (bad[i]) {
+            set_error("batch_solve: problem %d: initial %c is not positive", i, bad[i] == 1 ? 's' : 'z');
             return CVXB_E_ARG;
         }
     return 0;
@@ -1614,26 +1744,31 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
     CVXB_CUDA(cudaEventRecord(b->e0, st));
     // ---- starting point: W = I (coneqp :2055-2106, conelp :662-857) ----
     k_init_rhs<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();  // dx = -q, y = b, dz = h, resx0 / resy0 / resz0
-    CVXB_TRY(start_factor<EQ>(b));
-    k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
-    if (SDP) { k_s_wtz<<<dim3(p.ns, B), SB_T, 0, st>>>(p, p.dz, m, nullptr, 0, 0); count_launch(); }
-    if (LP) {
-        CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
-        CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));            // primal start: (0, b, h)
-        k_lp_start_mid<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();
-        CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));           // dual start: (-c, 0, 0)
-        if (SDP) { k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
-        k_lp_init_point<CONES, EQ, SDP><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
-    } else {
-        CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
-        if (SDP) {
-            k_init_sz<<<B, T, 0, st>>>(p); count_launch();
-            k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch();
+    // a loaded start (coneqp's cdim == 0 branch, :2002, ignores it); firstcall: iteration 0's factorisation is the first
+    const bool warm = b->warm_set && m > 0, firstcall = warm && (!LP || (b->warm.s && b->warm.z));
+    if (warm) CVXB_TRY((warm_start<CONES, EQ, LP, SDP>(b)));
+    else {
+        CVXB_TRY(start_factor<EQ>(b));
+        k_scale_bz<<<B, T, 0, st>>>(p); count_launch();
+        if (SDP) { k_s_wtz<<<dim3(p.ns, B), SB_T, 0, st>>>(p, p.dz, m, nullptr, 0, 0); count_launch(); }
+        if (LP) {
+            CVXB_CUDA(cudaMemsetAsync(p.x, 0, (size_t)B * n * sizeof(double), st));
+            CVXB_TRY(batch_solve(b, p.x, n, p.y, pq));            // primal start: (0, b, h)
+            k_lp_start_mid<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();
+            CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));           // dual start: (-c, 0, 0)
+            if (SDP) { k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
+            k_lp_init_point<CONES, EQ, SDP><<<B, T, 0, st>>>(p, abstol, reltol); count_launch();
+        } else {
+            CVXB_TRY(batch_solve(b, p.dx, n, p.y, pq));
+            if (SDP) {
+                k_init_sz<<<B, T, 0, st>>>(p); count_launch();
+                k_s_eig_start<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch();
+            }
+            k_init_point<CONES, SDP><<<B, T, 0, st>>>(p); count_launch();
         }
-        k_init_point<CONES, SDP><<<B, T, 0, st>>>(p); count_launch();
+        CVXB_LAUNCH_CHECK();
+        CVXB_TRY(start_check<EQ>(b));
     }
-    CVXB_LAUNCH_CHECK();
-    CVXB_TRY(start_check<EQ>(b));
     // residual GEMV signs: coneqp's rx = P x + q + A'y + G'z, ry = A x - b; conelp's hrx = -A'y - G'z, hry = A x
     const double sgn = LP ? -1.0 : 1.0;
     std::vector<int> flags(B), pairs;
@@ -1669,7 +1804,11 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
         }
         if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
         k_scaling<CONES, LP, SDP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
-        CVXB_TRY(batch_factor(b));
+        if (firstcall && it == 0) {              // kkt_chol2's first call; still singular: the Rank ValueError
+            CVXB_TRY(batch_factor(b, false));
+            CVXB_TRY(first_switch<EQ>(b));
+            CVXB_TRY(start_check<EQ>(b));
+        } else CVXB_TRY(batch_factor(b));
         if (LP) {
             // (x1, y1, z1) from (-c, b, h) (:1066-1077), th = W^{-T} h
             k_lp_x1_rhs<EQ><<<B, T, 0, st>>>(p); count_launch();
@@ -1980,6 +2119,37 @@ int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int s
     CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->p.beq), bvec, B * pq * sizeof(double), kind, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->eq_loaded = true;
+    return 0;
+}
+
+int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const double *y, const double *z,
+                          int space) {
+    if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
+    if (b->lp && ((!x) != (!s) || (y && !z) || (!x && !z))) {
+        set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
+                  "both");
+        return CVXB_E_ARG;
+    }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq;
+    if (!b->start.p) CVXB_TRY(b->start.alloc(B * (n + pq + 2 * m)));
+    double *x0 = b->start.p, *y0 = x0 + B * n, *s0 = y0 + B * pq, *z0 = s0 + B * m;
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    b->warm_set = false;                          // a failed copy leaves no start
+    if (x) CVXB_CUDA(cudaMemcpyAsync(x0, x, B * n * sizeof(double), kind, b->st));
+    if (y && pq) CVXB_CUDA(cudaMemcpyAsync(y0, y, B * pq * sizeof(double), kind, b->st));
+    if (s && m) CVXB_CUDA(cudaMemcpyAsync(s0, s, B * m * sizeof(double), kind, b->st));
+    if (z && m) CVXB_CUDA(cudaMemcpyAsync(z0, z, B * m * sizeof(double), kind, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->warm = Warm{x ? x0 : nullptr, (y && pq) ? y0 : nullptr, (s && m) ? s0 : nullptr, (z && m) ? z0 : nullptr};
+    b->warm_set = true;
+    return 0;
+}
+
+int cvxb_batch_clear_start(cvxb_batch *b) {
+    if (!b) { set_error("batch_clear_start: batch is NULL"); return CVXB_E_ARG; }
+    b->warm = Warm{};
+    b->warm_set = false;
     return 0;
 }
 

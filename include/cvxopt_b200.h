@@ -320,6 +320,25 @@ int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int s
 /* cone LP batch only (cvxb_batch_load on it, and this call on a QP batch, are CVXB_E_ARG):
  * c: nprob x n; G: nprob x (m x n column-major, ld m); h: nprob x m; m = cdim */
 int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space);
+/* the starting point of the next solves (warm start): x nprob x n, y nprob x p, s and z nprob x cdim laid out as h
+ * (an 's' block unpacked column-major, only its lower triangle read).  NULL: the key is absent.
+ * QP batch: coneqp(..., initvals) with the given keys (coneprog.py:2109-2149); an absent x or y is 0, an absent s or
+ * z is e (1 on the 'l' rows, on each 'q' cone's first row and on each 's' block's diagonal), so all NULL is the e
+ * start.  Nothing is shifted, the W = I factorisation is skipped and iteration 0's factorisation is the first one:
+ * kkt_chol2's S + A'A switch is decided there, and a KKT matrix still singular there makes cvxb_batch_solve return
+ * CVXB_E_ARG naming the problem (Rank(A) < p or ...).  A batch without constraint rows (cdim = 0) ignores the start.
+ * Cone LP batch: conelp(..., primalstart, dualstart) (coneprog.py:662-857): x and s together are primalstart, z with
+ * an optional y is dualstart; x without s, s without x, y without z, or neither start is CVXB_E_ARG.  With one of the
+ * two the W = I factorisation solves for the other half, which is shifted as conelp shifts it; with both, iteration 0's
+ * factorisation is the first, as for a QP.
+ * A given s or z that is not strictly inside the cone makes cvxb_batch_solve return CVXB_E_ARG with "problem %d:
+ * initial s (z) is not positive".  The start is kept in the caller's problem order across solves and across
+ * cvxb_batch_load*, until the next cvxb_batch_load_start or cvxb_batch_clear_start.  The first call allocates
+ * nprob * (n + p + 2 cdim) doubles of device memory, counted by cvxb_device_bytes and freed by cvxb_batch_destroy. */
+int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const double *y, const double *z,
+                          int space);
+/* back to the cold start (the W = I start of coneqp and conelp); the start's memory stays with the handle */
+int cvxb_batch_clear_start(cvxb_batch *b);
 int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol);
 /* status: 1 optimal, 2 maximum iterations reached, 3 singular KKT matrix ('unknown' in the
  * reference for 2 and 3), and for cone LP batches 4 primal infeasible, 5 dual infeasible.  Where conelp returns None
