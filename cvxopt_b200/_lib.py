@@ -27,6 +27,18 @@ class Scaling(C.Structure):
                 ("dnl", "dnli", "d", "di", "v", "beta", "r", "rti")]
 
 
+class SblockArgs(C.Structure):
+    """cvxb_sblock_args"""
+    _fields_ = ([("nblk", C.c_int), ("orders", C.c_void_p), ("m", C.c_longlong), ("L", C.c_longlong),
+                 ("n", C.c_int), ("ldg", C.c_longlong), ("sG", C.c_longlong), ("step", C.c_double),
+                 ("ut", C.c_double), ("done", C.c_void_p), ("info", C.c_void_p), ("spart", C.c_void_p)]
+                + [(name, C.c_void_p) for name in
+                   ("s", "z", "ds", "dz", "h", "lmbda", "lmbdasq", "d", "di", "bzp", "th", "ws3",
+                    "r", "rti", "sigs", "sigz", "wz", "ws", "wz2", "ws2", "wz3", "G", "Gs")])
+
+
+SK_NT_COMPUTE, SK_UPDATE, SK_DIR_POST, SK_EIG_START, SK_EIG_WARM, SK_BUILD_GS, SK_WTZ, SK_RES = range(8)
+
 _SIGS = {
     # name: (restype, argtypes)
     "cvxb_last_error": (C.c_char_p, []),
@@ -100,6 +112,7 @@ _SIGS = {
     "cvxb_gemv_batched": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p,
                                     C.c_longlong, C.c_void_p, C.c_longlong, C.c_double, C.c_double, C.c_void_p,
                                     C.c_longlong, C.c_int, C.c_int]),
+    "cvxb_sblock_batched": (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(SblockArgs), C.c_int]),
     "cvxb_batch_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int]),
     "cvxb_batch_create_cones": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(Dims), C.c_int]),
     "cvxb_batch_create_eq": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Dims),

@@ -19,7 +19,9 @@
 // algorithm: cvxb_batch_create_sdp builds cone LPs, cvxb_batch_create_sdp_qp QPs.
 #include "cone.cuh"
 #include <algorithm>
+#include <climits>
 #include <cstdlib>
+#include <vector>
 #include <memory>
 
 using namespace cvxb;
@@ -2206,6 +2208,145 @@ int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *stat
             if (dobj) dobj[i] = sc[slot].dcost;
         }
     }
+    return 0;
+}
+
+// ---------------------------------------------------------------- the 's' block kernels on caller data
+// A Ptrs with only what the kernels read: the block layout of cvxb_batch_create_sdp without 'l' and 'q' rows (mlq = 0),
+// one Scal per problem (done, step), zero info and the caller's spart.  The launches are the solver's.
+int cvxb_sblock_batched(int kernel, int mode, int batch, const cvxb_sblock_args *a, int device) {
+    if (batch < 1 || batch > CVXB_BATCH_MAX) {
+        set_error("sblock_batched: batch = %d outside 1..%d", batch, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (!a || a->nblk < 1 || !a->orders || !a->spart) {
+        set_error("sblock_batched: missing arguments, block orders or spart");
+        return CVXB_E_ARG;
+    }
+    std::vector<int> info;
+    long long so = 0, sp = 0, sgo = 0;
+    for (int k = 0; k < a->nblk; ++k) {
+        const int s = a->orders[k];
+        if (s < 1 || s > CVXB_BATCH_SMAX) {
+            set_error("sblock_batched: order %d of block %d outside 1..%d", s, k, CVXB_BATCH_SMAX);
+            return CVXB_E_ARG;
+        }
+        info.insert(info.end(), {s, (int)so, (int)sp, (int)so, (int)sgo});
+        so += (long long)s * s; sp += (long long)s * (s + 1) / 2; sgo += s;
+    }
+    if (a->m < so || a->L < so) {
+        set_error("sblock_batched: m = %lld or L = %lld below the %lld rows of the blocks", a->m, a->L, so);
+        return CVXB_E_ARG;
+    }
+    if (a->m > INT_MAX) {
+        set_error("sblock_batched: m = %lld above %d (the solver keeps m in an int)", a->m, INT_MAX);
+        return CVXB_E_ARG;
+    }
+    const bool lp = kernel == CVXB_SK_RES && mode == 1;
+    const long long nlps = sizeof(LPScal) / sizeof(double);
+    if (lp && a->L < nlps) {
+        set_error("sblock_batched: L = %lld below the %lld doubles of the embedding's scalars", a->L, nlps);
+        return CVXB_E_ARG;
+    }
+    int maxmode = 0;
+    std::vector<const void *> need;
+    switch (kernel) {
+    case CVXB_SK_NT_COMPUTE: need = {a->s, a->z, a->r, a->rti, a->lmbda}; break;
+    case CVXB_SK_UPDATE:
+        maxmode = 1;
+        need = {a->lmbda, a->sigs, a->sigz, a->ds, a->dz, a->r, a->rti, a->d, a->di, a->lmbdasq};
+        break;
+    case CVXB_SK_DIR_POST:
+        maxmode = 1;
+        need = {a->ds, a->dz, a->lmbda, mode == 0 ? a->ws3 : a->sigs, mode == 0 ? a->ws3 : a->sigz};
+        break;
+    case CVXB_SK_EIG_START: need = {a->s, a->bzp}; break;
+    case CVXB_SK_EIG_WARM: need = {a->s, a->z}; break;
+    case CVXB_SK_BUILD_GS:
+        need = {a->rti, a->G, a->Gs};
+        if (a->n < 1 || a->ldg < so || a->sG < a->ldg * a->n) {
+            set_error("sblock_batched: build_gs needs n >= 1, ldg >= %lld, sG >= ldg * n", so);
+            return CVXB_E_ARG;
+        }
+        break;
+    case CVXB_SK_WTZ:
+        maxmode = 2;
+        need = {a->z, a->rti, a->bzp};
+        if (mode == 1) need.push_back(a->th);
+        if (mode == 2) need.insert(need.end(), {a->s, a->lmbda, a->r});
+        break;
+    case CVXB_SK_RES:
+        maxmode = 1;
+        need = {a->dz, a->ds, a->rti, a->r, a->wz, a->ws, a->lmbda, a->wz3, a->wz2, a->ws2};
+        if (lp) need.push_back(a->h);
+        break;
+    default: set_error("sblock_batched: unknown kernel %d", kernel); return CVXB_E_ARG;
+    }
+    if (mode < 0 || mode > maxmode) {
+        set_error("sblock_batched: mode %d outside 0..%d for kernel %d", mode, maxmode, kernel);
+        return CVXB_E_ARG;
+    }
+    for (const void *q : need)
+        if (!q) { set_error("sblock_batched: kernel %d mode %d is missing an operand", kernel, mode); return CVXB_E_ARG; }
+
+    CallCtx ctx; CVXB_TRY(ctx.acquire(device));
+    cudaStream_t st = ctx.st;
+    const int ns = a->nblk;
+    std::vector<Scal> sc(batch);                  // value-initialised: all zero
+    for (int b = 0; b < batch; ++b) { sc[b].done = a->done ? a->done[b] : 0; sc[b].step = a->step; }
+    std::vector<int> hinfo(batch, 0);
+    if (a->info) std::copy(a->info, a->info + batch, hinfo.begin());
+    Scratch<int> d_sinfo, d_info;
+    Scratch<Scal> d_sc;
+    Scratch<double> d_spart, d_lps;
+    CVXB_TRY(d_sinfo.alloc(info.size()));
+    CVXB_TRY(d_info.alloc(batch));
+    CVXB_TRY(d_sc.alloc(batch));
+    CVXB_TRY(d_spart.alloc((size_t)batch * ns * 4));
+    CVXB_CUDA(cudaMemcpyAsync(d_sinfo.p, info.data(), info.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(d_info.p, hinfo.data(), batch * sizeof(int), cudaMemcpyHostToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(d_sc.p, sc.data(), batch * sizeof(Scal), cudaMemcpyHostToDevice, st));
+    CVXB_CUDA(cudaMemcpyAsync(d_spart.p, a->spart, (size_t)batch * ns * 4 * sizeof(double), cudaMemcpyHostToDevice,
+                              st));
+    std::vector<double> lps;
+    if (lp) {                                     // dtau / dg = ut for every problem
+        lps.assign((size_t)batch * a->L, 0.0);
+        for (int b = 0; b < batch; ++b) {
+            LPScal *T = reinterpret_cast<LPScal *>(lps.data() + (size_t)b * a->L);
+            T->dtau = a->ut; T->dg = 1.0;
+        }
+        CVXB_TRY(d_lps.alloc(lps.size()));
+        CVXB_CUDA(cudaMemcpyAsync(d_lps.p, lps.data(), lps.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    Ptrs p{};
+    p.n = a->n; p.m = (int)a->m; p.L = a->L; p.mlq = 0; p.mpk = (int)sp; p.mdg = (int)sgo; p.ns = ns;
+    p.sinfo = d_sinfo.p; p.sc = d_sc.p; p.spart = d_spart.p; p.lps = d_lps.p;
+    p.s = a->s; p.z = a->z; p.ds = a->ds; p.dz = a->dz; p.h = a->h; p.lmbda = a->lmbda; p.lmbdasq = a->lmbdasq;
+    p.d = a->d; p.di = a->di; p.bzp = a->bzp; p.th = a->th; p.ws3 = a->ws3;
+    p.sr = a->r; p.srti = a->rti; p.sigs = a->sigs; p.sigz = a->sigz;
+    p.wz = a->wz; p.ws = a->ws; p.wz2 = a->wz2; p.ws2 = a->ws2; p.wz3 = a->wz3;
+    const dim3 sg(ns, batch);
+    switch (kernel) {
+    case CVXB_SK_NT_COMPUTE: k_s_nt_compute<<<sg, SB_T, 0, st>>>(p); break;
+    case CVXB_SK_UPDATE: k_s_update<false><<<sg, SB_T, 0, st>>>(p, d_info.p, mode); break;
+    case CVXB_SK_DIR_POST: k_s_dir_post<<<sg, SB_T, 0, st>>>(p, mode); break;
+    case CVXB_SK_EIG_START: k_s_eig_start<<<sg, SB_T, 0, st>>>(p); break;
+    case CVXB_SK_EIG_WARM: k_s_eig_warm<<<sg, SB_T, 0, st>>>(p); break;
+    case CVXB_SK_BUILD_GS:
+        k_s_build_gs<<<dim3(ns, batch, (a->n + 15) / 16), SB_T, 0, st>>>(p, a->G, a->Gs, a->ldg, a->sG);
+        break;
+    case CVXB_SK_WTZ: k_s_wtz<<<sg, SB_T, 0, st>>>(p, a->z, a->m, a->s, a->m, mode); break;
+    default:
+        if (lp) k_s_res<true><<<sg, SB_T, 0, st>>>(p);
+        else k_s_res<false><<<sg, SB_T, 0, st>>>(p);
+    }
+    count_launch();
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(a->spart, d_spart.p, (size_t)batch * ns * 4 * sizeof(double), cudaMemcpyDeviceToHost, st);
+    const cudaError_t e2 = cudaStreamSynchronize(st);        // before the scratch goes back to the cache
+    if (e == cudaSuccess) e = e2;
+    if (e != cudaSuccess) { set_error("sblock_batched: %s", cudaGetErrorString(e)); return CVXB_E_CUDA; }
     return 0;
 }
 

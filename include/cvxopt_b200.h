@@ -308,6 +308,44 @@ int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_
  * cvxb_device_bytes and freed by cvxb_batch_destroy.  Dims without an 's' block of positive order run exactly what
  * cvxb_batch_create_eq's batch runs. */
 int cvxb_batch_create_sdp_qp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device);
+/* ---- the batch solver's 's' block kernels on caller data, for tests: one launch of the kernel the solver runs, one
+ * CTA per (block, problem), on blocks of the given orders laid out as in the solver without 'l' and 'q' rows.  Device
+ * pointers; problem b of an m-vector operand is at base + b * m, of a state-row operand at base + b * L.  m-vectors
+ * (s, z, ds, dz, h, lmbda, lmbdasq, d, di, ws3): the blocks one after another, each ms x ms column-major, lambda on a
+ * block's diagonal rows; bzp and th hold the blocks packed (lower triangle by columns, off-diagonals times sqrt 2).
+ * State rows: r, rti, wz, ws, wz2, ws2, wz3 at the blocks' unpacked offsets, sigs and sigz at sum of the earlier
+ * orders.  G and Gs: column j of problem b at base + b * sG + j * ldg, rows as an m-vector (Gs packed).  Outputs the
+ * solver stages come back staged: k_s_update's r in d, rti in di, s in ds, z in dz, lambda+ in lmbdasq's diagonal rows.
+ * spart (host, batch * nblk * 4, problem-major) is uploaded before the launch and returned after it: per (problem,
+ * block) sdot, the two smallest eigenvalues and the failure flag as the kernel leaves them.  done (host, batch ints)
+ * and info (host, batch ints, k_s_update) may be NULL for all zero.  mode: k_s_update's `first`, k_s_dir_post's i,
+ * k_s_wtz's mode (0, 1, 2), k_s_res's LP flag (1: ut = dtau / dg for every problem, needs L >= 17); 0 otherwise.
+ * CVXB_E_ARG, before the device: batch outside 1..CVXB_BATCH_MAX, nblk < 1, an order outside 1..CVXB_BATCH_SMAX,
+ * m or L below the blocks' rows, an unknown kernel or mode, or an operand the kernel reads or writes missing. */
+#define CVXB_SK_NT_COMPUTE 0
+#define CVXB_SK_UPDATE 1
+#define CVXB_SK_DIR_POST 2
+#define CVXB_SK_EIG_START 3
+#define CVXB_SK_EIG_WARM 4
+#define CVXB_SK_BUILD_GS 5
+#define CVXB_SK_WTZ 6
+#define CVXB_SK_RES 7
+typedef struct {
+    int nblk;
+    const int *orders;                /* host, nblk */
+    long long m, L;                   /* per-problem strides of the m-vector and the state-row operands */
+    int n;                            /* columns of G (k_s_build_gs) */
+    long long ldg, sG;
+    double step;                      /* Scal.step of every problem (k_s_update) */
+    double ut;                        /* k_s_res<true> */
+    const int *done, *info;
+    double *spart;
+    double *s, *z, *ds, *dz, *h, *lmbda, *lmbdasq, *d, *di, *bzp, *th, *ws3;
+    double *r, *rti, *sigs, *sigz, *wz, *ws, *wz2, *ws2, *wz3;
+    const double *G;
+    double *Gs;
+} cvxb_sblock_args;
+int cvxb_sblock_batched(int kernel, int mode, int batch, const cvxb_sblock_args *args, int device);
 /* steps of iterative refinement per Newton solve; default 1 if dims has 'q' cones, else 0 (coneprog.py:1862-1865) */
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement);
 void cvxb_batch_destroy(cvxb_batch *b);

@@ -114,3 +114,66 @@ def test_batched_blocks_check_arguments_before_the_device():
         for batch in (1, 65535):
             assert call(batch, ord("T")) == _lib.E_NOGPU, (name, batch)
             assert "no CUDA device available" in _lib.last_error(), name
+
+
+def test_sblock_kernels_check_arguments_before_the_device():
+    """cvxb_sblock_batched refuses, with CVXB_E_ARG and before it looks for a device, a batch outside
+    1..CVXB_BATCH_MAX, an order outside 1..CVXB_BATCH_SMAX, strides below the blocks' rows, an unknown kernel or mode
+    and a missing operand; every kernel id with all its operands fails with CVXB_E_NOGPU without a GPU"""
+    import ctypes
+    import numpy as np
+    import cvxopt_b200
+    from cvxopt_b200 import _lib
+    lib = _lib.load()
+    buf = np.zeros(64)
+    orders = np.array([2, 3], dtype=np.intc)
+    spart = np.zeros(4 * 2 * 65535)
+
+    def args(**kw):
+        a = _lib.SblockArgs(nblk=2, orders=orders.ctypes.data, m=13, L=17, n=1, ldg=13, sG=13,
+                            spart=spart.ctypes.data)
+        for name in ("s", "z", "ds", "dz", "h", "lmbda", "lmbdasq", "d", "di", "bzp", "th", "ws3", "r", "rti",
+                     "sigs", "sigz", "wz", "ws", "wz2", "ws2", "wz3", "G", "Gs"):
+            setattr(a, name, buf.ctypes.data)
+        for k, v in kw.items():
+            setattr(a, k, v)
+        return a
+
+    def call(kernel=_lib.SK_NT_COMPUTE, mode=0, batch=1, **kw):
+        return lib.cvxb_sblock_batched(kernel, mode, batch, ctypes.byref(args(**kw)), 0)
+
+    for batch in (0, -1, 65536):
+        assert call(batch=batch) == _lib.E_ARG and "batch" in _lib.last_error(), batch
+    for bad in ([0, 3], [2, 33], [-1, 2]):
+        o = np.array(bad, dtype=np.intc)
+        assert call(orders=o.ctypes.data) == _lib.E_ARG and "order" in _lib.last_error(), bad
+    assert call(nblk=0) == _lib.E_ARG
+    assert call(orders=None) == _lib.E_ARG
+    assert call(spart=None) == _lib.E_ARG
+    assert lib.cvxb_sblock_batched(0, 0, 1, None, 0) == _lib.E_ARG
+    assert call(m=12) == _lib.E_ARG and call(L=12) == _lib.E_ARG          # 4 + 9 rows
+    assert call(m=2 ** 31) == _lib.E_ARG and "int" in _lib.last_error()
+    assert call(kernel=_lib.SK_RES, mode=1, L=16) == _lib.E_ARG            # the embedding's scalars need 17
+    assert call(kernel=8) == _lib.E_ARG and "kernel" in _lib.last_error()
+    assert call(kernel=-1) == _lib.E_ARG
+    modes = {_lib.SK_NT_COMPUTE: 0, _lib.SK_UPDATE: 1, _lib.SK_DIR_POST: 1, _lib.SK_EIG_START: 0,
+             _lib.SK_EIG_WARM: 0, _lib.SK_BUILD_GS: 0, _lib.SK_WTZ: 2, _lib.SK_RES: 1}
+    for kernel, top in modes.items():
+        assert call(kernel=kernel, mode=top + 1) == _lib.E_ARG and "mode" in _lib.last_error(), kernel
+        assert call(kernel=kernel, mode=-1) == _lib.E_ARG, kernel
+    missing = [(_lib.SK_NT_COMPUTE, 0, "lmbda"), (_lib.SK_UPDATE, 0, "sigz"), (_lib.SK_DIR_POST, 0, "ws3"),
+               (_lib.SK_DIR_POST, 1, "sigs"), (_lib.SK_EIG_START, 0, "bzp"), (_lib.SK_EIG_WARM, 0, "z"),
+               (_lib.SK_BUILD_GS, 0, "Gs"), (_lib.SK_WTZ, 1, "th"), (_lib.SK_WTZ, 2, "r"), (_lib.SK_RES, 0, "wz3"),
+               (_lib.SK_RES, 1, "h")]
+    for kernel, mode, name in missing:
+        assert call(kernel=kernel, mode=mode, **{name: None}) == _lib.E_ARG, (kernel, mode, name)
+        assert "missing" in _lib.last_error()
+    assert call(kernel=_lib.SK_BUILD_GS, n=0) == _lib.E_ARG
+    assert call(kernel=_lib.SK_BUILD_GS, ldg=12) == _lib.E_ARG
+    if cvxopt_b200.device_count() > 0:
+        pytest.skip("a GPU is visible")
+    for kernel, top in modes.items():
+        for mode in range(top + 1):
+            for batch in (1, 65535):
+                assert call(kernel=kernel, mode=mode, batch=batch) == _lib.E_NOGPU, (kernel, mode, batch)
+                assert "no CUDA device available" in _lib.last_error()
