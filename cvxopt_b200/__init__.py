@@ -11,10 +11,11 @@ from .batch import QPBatch, QPBatchGroup, qp_batch, qp_batch_distributed, shard_
 from .batch import ConeLPBatch, ConeLPBatchGroup, conelp_batch  # noqa: F401
 from .batch import SDPBatch, SDPBatchGroup, sdp_batch  # noqa: F401
 from .batch import SDPQPBatch, SDPQPBatchGroup, coneqp_batch  # noqa: F401
+from .batch import GPBatch, GPBatchGroup, gp_batch  # noqa: F401
 
 __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolver", "cpl_kktsolver", "QPBatch", "qp_batch", "conelp", "qp_batch_distributed", "load",
            "ConeLPBatch", "conelp_batch", "SDPBatch", "SDPBatchGroup", "sdp_batch",
-           "SDPQPBatch", "SDPQPBatchGroup", "coneqp_batch",
+           "SDPQPBatch", "SDPQPBatchGroup", "coneqp_batch", "GPBatch", "GPBatchGroup", "gp_batch",
            "device_count", "launch_count"]
 
 

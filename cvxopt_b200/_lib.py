@@ -135,6 +135,10 @@ _SIGS = {
     "cvxb_batch_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_double]),
     "cvxb_batch_stats": (C.c_int, [C.c_void_p, c_double_p, c_int_p]),
     "cvxb_batch_syrk_path": (C.c_int, [C.c_void_p]),
+    "cvxb_batch_create_gp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                       C.c_int, C.c_int, C.c_int]),
+    "cvxb_batch_load_gp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "cvxb_batch_ls_rounds": (C.c_int, [C.c_void_p]),
     "cvxb_batch_results": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
 }

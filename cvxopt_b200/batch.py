@@ -623,6 +623,113 @@ def coneqp_batch(P, q, G, h, dims, A=None, b=None, device=0, nsub=None, initvals
     return _run_group(SDPQPBatchGroup(B, n, dims, p, device, nsub), (P, q, G, h, A, b), options, start)
 
 
+class GPBatch(QPBatch):
+    """B geometric programs (cvxb_batch_create_gp): B x solvers.gp(K, F, g, G, h, A, b), cpl's lock-step iteration on
+    gp's epigraph problem.  K (block sizes of F, mnl = len(K) - 1), ml rows of G and p rows of A are shared by the
+    batch.  load() takes F (B, sum K, n), g (B, sum K), G (B, ml, n), h (B, ml) and, with p > 0, A (B, p, n), b (B, p).
+    results()' s and z are [snl; sl] and [znl; zl] (mnl + ml columns); its primal objective is gp's t."""
+
+    def __init__(self, nprob, n, K, ml, p=0, device=0):
+        K = [int(k) for k in K]
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.B, self.n, self.K, self.p = int(nprob), int(n), K, int(p)
+        self.mnl, self.ml = len(K) - 1, int(ml)
+        self.m = self.mnl + self.ml
+        karr = (C.c_int * max(1, len(K)))(*K)
+        rc = self._lib.cvxb_batch_create_gp(C.byref(self._h), self.B, self.n, len(K), karr, self.ml, self.p, device)
+        _lib.check(rc, "batch")
+        self._refinement = None
+
+    def load(self, F, g, G, h, A=None, b=None):
+        B, n, S = self.B, self.n, sum(self.K)
+        F = np.asarray(F, dtype=np.float64)
+        g = np.ascontiguousarray(np.asarray(g, dtype=np.float64))
+        G = np.zeros((B, 0, n)) if G is None else np.asarray(G, dtype=np.float64)
+        h = np.zeros((B, 0)) if h is None else np.ascontiguousarray(np.asarray(h, dtype=np.float64))
+        if F.shape != (B, S, n) or g.shape != (B, S) or G.shape != (B, self.ml, n) or h.shape != (B, self.ml):
+            raise TypeError("problem shapes do not match the batch")
+        Acm, bv = self._host_eq(A, b)
+        Fcm = np.ascontiguousarray(np.transpose(F, (0, 2, 1)))
+        Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
+        _lib.check(self._lib.cvxb_batch_load_gp(self._h, Fcm.ctypes.data, g.ctypes.data,
+                                                Gcm.ctypes.data if self.ml else None,
+                                                h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_gp")
+        self._load_eq(Acm, bv, _lib.HOST)
+
+    def stats(self):
+        out = super().stats()
+        out["line_search_rounds"] = self._lib.cvxb_batch_ls_rounds(self._h)
+        return out
+
+
+class GPBatchGroup(QPBatchGroup):
+    """QPBatchGroup's interleaved sub-batches, solved concurrently, for geometric programs"""
+
+    def __init__(self, nprob, n, K, ml, p=0, device=0, nsub=None):
+        self._K, self._ml = list(K), int(ml)
+        super().__init__(nprob, n, len(K) - 1 + int(ml), device, nsub, None, p)
+
+    def _part(self):
+        return lambda nprob, n, m, device, dims, p=0: GPBatch(nprob, n, self._K, self._ml, p, device)
+
+    def load(self, F, g, G, h, A=None, b=None):
+        self._load_sliced((F, g, G, h), A, b)
+
+    def stats(self):
+        out = super().stats()
+        out["line_search_rounds"] = max(b._lib.cvxb_batch_ls_rounds(b._h) for b in self.parts)
+        return out
+
+
+def _gp_args(K, F, g, G, h, A, b):
+    """gp's argument checks (cvxprog.py:2056-2092) on the batch -> F, g, G, h, A, b with the defaults filled in"""
+    if type(K) is not list or [k for k in K if type(k) is not int or k <= 0]:
+        raise TypeError("'K' must be a list of positive integers")
+    S = sum(K)
+    F = np.asarray(F) if F is not None else None
+    if F is None or F.ndim != 3 or F.shape[1] != S or F.dtype.kind != "f":
+        raise TypeError("'F' must be a dense or sparse 'd' matrix with %d rows" % S)
+    B, n = F.shape[0], F.shape[2]
+    g = np.asarray(g) if g is not None else None
+    if g is None or g.shape != (B, S) or g.dtype.kind != "f":
+        raise TypeError("'g' must be a dene 'd' matrix of size (%d,1)" % S)
+    G = np.zeros((B, 0, n)) if G is None else np.asarray(G)
+    if G.ndim != 3 or G.shape[0] != B or G.shape[2] != n or G.dtype.kind != "f":
+        raise TypeError("'G' must be a dense or sparse 'd' matrix with %d columns" % n)
+    ml = G.shape[1]
+    h = np.zeros((B, 0)) if h is None else np.asarray(h)
+    if h.shape != (B, ml) or h.dtype.kind != "f":
+        raise TypeError("'h' must be a dense 'd' matrix of size (%d,1)" % ml)
+    A = np.zeros((B, 0, n)) if A is None else np.asarray(A)
+    if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n or A.dtype.kind != "f":
+        raise TypeError("'A' must be a dense or sparse 'd' matrix with %d columns" % n)
+    p = A.shape[1]
+    b = np.zeros((B, 0)) if b is None else np.asarray(b)
+    if b.shape != (B, p) or b.dtype.kind != "f":
+        raise TypeError("'b' must be a dense 'd' matrix of size (%d,1)" % p)
+    if p > n:
+        raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
+    return F, g, G, h, A, b
+
+
+def gp_batch(K, F, g, G=None, h=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent geometric programs on one GPU, each as solvers.gp(K, F, g, G, h, A, b) does:
+    minimize log sum exp(F0 x + g0) s.t. log sum exp(Fi x + gi) <= 0, G x <= h, A x = b.  K (list of block sizes) is
+    shared by the batch; F (B, sum K, n), g (B, sum K), G (B, ml, n), h (B, ml), A (B, p, n), b (B, p), the last four
+    optional.  Returns gp's x, snl, sl, znl, zl, y, status ('optimal' or 'unknown'), iterations, primal objective and
+    dual objective, with the batch's stats (solve_ms, lock-step iterations, line-search rounds).  nsub is qp_batch's.
+    options: maxiters, abstol, reltol, feastol, refinement (as gp's)."""
+    F, g, G, h, A, b = _gp_args(K, F, g, G, h, A, b)
+    B, n, p, mnl = F.shape[0], F.shape[2], A.shape[1], len(K) - 1
+    out = _run_group(GPBatchGroup(B, n, K, G.shape[1], p, device, nsub), (F, g, G, h, A if p else None,
+                                                                           b if p else None), options)
+    for key in ("s", "z"):
+        v = out.pop(key)
+        out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]
+    return out
+
+
 def _run_group(grp, data, options, start=None):
     """load `data` (and a start dict of load_start's keys) into the batch group, solve it timed, and return its results
     and stats; the group is closed"""

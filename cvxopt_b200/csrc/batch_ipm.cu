@@ -1326,6 +1326,468 @@ template <bool EQ> __global__ void __launch_bounds__(SB_T) k_s_update(Ptrs p, co
     }
     for (int i = tid; i < ms; i += SB_T) p.lmbdasq[om + so + i * (ms + 1)] = lam[i];
 }
+
+// ---- geometric programs: cvxprog.gp -> cp -> cpl (cvxprog.py:1967-2155, :1746-1964, :556-1356) ----
+// gp solves the epigraph problem of cp with cpl: the variable is (x, t), the objective t, the nonlinear rows are
+// f0(x) - t, f1(x), ..., fmnl(x) with fi = log sum exp(Fi x + gi), and the 'l' rows G x <= h.  Every row is diagonally
+// scaled.  The m-vectors hold rows [f1..fmnl; 'l'] (m = mnl + ml); the epigraph row f0 - t and t itself are scalars
+// of GPScal.  The batch's G holds [Df[1:]; G] in rows [0, m) (the KKT operand kkt_chol2 scales by [dnli; di]) and F in
+// rows [m, m + sum K); P holds H = sum_i z_i Fi'(diag(yi) - yi yi')Fi.  kktsolver_e (:1890-1943) eliminates t around
+// one batch_solve.  Per-slot scalars and the relaxed line search's saved state live in the state row.
+struct GPScal {
+    double t, dt, s0, z0, ds0, dz0, ds20, dz20, l0, lsq0, d0, di0, rxt, rz0, a;   // epigraph row and t
+    double wxt, wx2t, wz0, ws0, wz20, ws20, wz30;                                  // refinement copies
+    double resznl, resx0, resznl0, pres0, th1, th2, th3, phi, dphi, relaxed, searching;
+    double nt, ns0, nz0;                                                           // line-search trial
+    // the saved state of a series of relaxed line searches (:1190-1215)
+    double phi0, dphi0, gap0, step0, dsdz0, sigma0, eta0;
+    double t0, dt0, s00, z00, ds00, dz00, ds200, dz200, l00, d00, di00, rxt0, rz00;
+};
+struct GPPtrs {
+    int nK, sumK, mnl;
+    long long ldg, sG, ldh, sH;
+    const int *koff;                 // nK + 1 row offsets of the blocks Fi in F
+    double *G;                       // per slot [Df[1:]; G; F], ld ldg
+    // per slot, rebuilt every iteration: H's scaled rows (sum K x n, ld ldh) and their weights z_i, y = F x + g and
+    // then the softmax, w = z_i y, f, grad f0, the unscaled steps ds2 / dz2 and the line search's trial point
+    double *Hr, *hw, *yv, *wv, *fv, *gf0, *ds2, *dz2, *nx, *ny, *nz, *ns, *nrx;
+    // in the state row: g (sum K), GPScal, and the saved vectors
+    double *g, *gs, *x0, *dx0, *rx0, *y0, *dy0, *ry0, *s0, *z0, *ds0, *dz0, *ds20, *dz20, *l0, *d0, *di0, *rz0;
+};
+constexpr int GP_MAX_RELAXED = 8;
+constexpr double GP_ALPHA = 0.01, GP_BETA = 0.5, GP_STEP = 0.99;
+__device__ __forceinline__ GPScal &gp_scal(const GPPtrs &g, long long oc) {
+    return *reinterpret_cast<GPScal *>(g.gs + oc);
+}
+#define GP_SETUP                                                                                       \
+    PB_SETUP                                                                                           \
+    GPScal &T = gp_scal(g, oc);                                                                        \
+    const long long ok = (long long)b * g.sumK;                                                        \
+    (void)T; (void)ok;
+
+// the starting point (:556-570): x = 0, t = 0, y = 0, s = z = e, relaxed_iters = 0
+__global__ void k_gp_init(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    for (int i = tid; i < p.n; i += nt) p.x[on + i] = 0.0;
+    for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = 0.0;
+    for (int i = tid; i < p.m; i += nt) { p.s[om + i] = 1.0; p.z[om + i] = 1.0; }
+    if (tid == 0) {
+        T = GPScal{};
+        T.s0 = 1.0; T.z0 = 1.0;
+    }
+}
+// F(x) of gp (:2102-2153) for block i of slot b, grid (nK, Bact): yv holds F x on entry; y := softmax(F x + g),
+// f_i = max + log sum exp, w = z_i y (z_i from z, or from the trial point's nz).  FULL: also Df_i = Fi' y (grad f0 or
+// row i - 1 of G), H's rows sqrt(y_k)(F_k - Df_i) and their weights z_i.  trial: only slots still searching
+template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) {
+    const int i = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, nt = blockDim.x;
+    const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
+    __shared__ double sh[32];
+    const GPScal &T = gp_scal(g, (long long)b * p.L);
+    if (p.sc[b].done || (trial && T.searching == 0.0)) return;
+    const int k0 = g.koff[i], K = g.koff[i + 1] - k0;
+    const long long ok = (long long)b * g.sumK + k0;
+    const double *F = g.G + (long long)b * g.sG + p.m + k0, *gv = g.g + (long long)b * p.L + k0;
+    double *y = g.yv + ok;
+    double mx = -INFINITY;
+    for (int k = tid; k < K; k += nt) { const double v = y[k] + gv[k]; y[k] = v; mx = fmax(mx, v); }
+    mx = -block_min(-mx, sh);
+    double sum = 0.0;
+    for (int k = tid; k < K; k += nt) { const double e = exp(y[k] - mx); y[k] = e; sum += e; }
+    sum = block_sum(sum, sh);
+    const double r = 1.0 / sum;
+    const double *zs = trial ? g.nz : p.z;
+    const double zi = i == 0 ? (trial ? T.nz0 : T.z0) : zs[(long long)b * p.m + i - 1];
+    for (int k = tid; k < K; k += nt) {
+        const double v = y[k] * r;
+        y[k] = v; g.wv[ok + k] = zi * v;
+        if (FULL) g.hw[ok + k] = zi;
+    }
+    if (tid == 0) g.fv[(long long)b * g.nK + i] = mx + log(sum);
+    if (!FULL) return;
+    __syncthreads();
+    double *hr = g.Hr + (long long)b * g.sH + k0;
+    for (int j = warp; j < p.n; j += nwarp) {           // one warp per column of Fi, its lanes down the rows
+        const double *Fj = F + (long long)j * g.ldg;
+        double a = 0.0;
+        for (int k = lane; k < K; k += 32) a += Fj[k] * y[k];
+        a = warp_sum(a);
+        if (lane == 0) {
+            if (i == 0) g.gf0[(long long)b * p.n + j] = a;
+            else g.G[(long long)b * g.sG + (i - 1) + (long long)j * g.ldg] = a;
+        }
+        for (int k = lane; k < K; k += 32) hr[k + (long long)j * g.ldh] = sqrt(y[k]) * (Fj[k] - a);
+    }
+}
+// residuals, part 1 (:668-691): rx = 0 (the GEMVs add Df'znl + G'zl + A'y), rxt = 1 - z0; rz = s + f on the
+// nonlinear rows, s - h on the 'l' rows (G x follows); rznl's epigraph row s0 + f0 - t; EQ: ry = b (A x - ry follows)
+template <bool EQ> __global__ void k_gp_res_begin(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    const double *f = g.fv + (long long)b * g.nK;
+    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = 0.0;
+    for (int i = tid; i < p.m; i += nt)
+        p.rz[om + i] = i < g.mnl ? p.s[om + i] + f[i + 1] : p.s[om + i] - p.h[om + i];
+    if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = p.beq[oq + i];
+    if (tid == 0) { T.rxt = -T.z0 + 1.0; T.rz0 = T.s0 + (f[0] - T.t); }
+}
+// statistics and stopping rule (:693-755); iteration 0 fixes resx0, resznl0, pres0, dres0 and the merit weights
+template <bool EQ> __global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int maxiters, double abstol, double reltol,
+                                              double feastol, int *ndone, int *doneflags) {
+    GP_SETUP
+    if (!S.done) {
+        double rx2 = 0, ry2 = 0, yry = 0, rn2 = 0, rl2 = 0, zrn = 0, zrl = 0, gap = 0;
+        for (int i = tid; i < p.n; i += nt) { const double v = p.rx[on + i]; rx2 += v * v; }
+        if (EQ) for (int i = tid; i < p.neq; i += nt) { const double v = p.ry[oq + i]; ry2 += v * v; yry += p.y[oq + i] * v; }
+        for (int i = tid; i < p.m; i += nt) {
+            const double v = p.rz[om + i], zv = p.z[om + i];
+            if (i < g.mnl) { rn2 += v * v; zrn += zv * v; } else { rl2 += v * v; zrl += zv * v; }
+            gap += p.s[om + i] * zv;
+        }
+        rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh); rl2 = block_sum(rl2, sh);
+        zrn = block_sum(zrn, sh); zrl = block_sum(zrl, sh); gap = block_sum(gap, sh);
+        if (EQ) { ry2 = block_sum(ry2, sh); yry = block_sum(yry, sh); }
+        if (tid == 0) {
+            gap += T.s0 * T.z0;
+            const double resx = sqrt(rx2 + T.rxt * T.rxt), resy = sqrt(ry2);
+            const double resznl = sqrt(rn2 + T.rz0 * T.rz0), reszl = sqrt(rl2);
+            const double pcost = T.t;                    // c'(x, t) with c = (0, 1)
+            const double dcost = pcost + yry + (zrn + T.z0 * T.rz0) + zrl - gap;
+            S.pcost = pcost; S.dcost = dcost; S.gap = gap; S.resx = resx; S.resy = resy; S.resz = reszl;
+            T.resznl = resznl;
+            if (pcost < 0.0) { S.relgap = gap / -pcost; S.relgap_valid = 1; }
+            else if (dcost > 0.0) { S.relgap = gap / dcost; S.relgap_valid = 1; }
+            else { S.relgap = 0.0; S.relgap_valid = 0; }
+            const double pres = sqrt(resy * resy + resznl * resznl + reszl * reszl);
+            if (iter == 0) {
+                T.resx0 = fmax(1.0, resx); T.resznl0 = fmax(1.0, resznl);
+                T.pres0 = fmax(1.0, pres); S.resx0 = fmax(1.0, resx);          // dres0
+                T.th1 = 1.0 / gap; T.th2 = 1.0 / T.resx0; T.th3 = 1.0 / T.resznl0;
+            }
+            S.pres = pres / T.pres0; S.dres = resx / S.resx0;
+            const bool opt = S.pres <= feastol && S.dres <= feastol &&
+                             (gap <= abstol || (S.relgap_valid && S.relgap <= reltol));
+            if (opt || iter == maxiters) { S.done = 1; S.iters = iter; S.status = opt ? 1 : 2; }
+        }
+    }
+    if (tid == 0) {
+        if (S.done) atomicAdd(ndone, 1);
+        doneflags[b] = S.done;
+    }
+}
+// the scaling at iteration 0 (misc.py:compute_scaling, dnl and d alike) and lambda o lambda every iteration;
+// di2 = di² is the SYRK's weight of [Df[1:]; G]
+__global__ void k_gp_scaling(Ptrs p, GPPtrs g, int first) {
+    GP_SETUP
+    if (S.done) return;
+    for (int i = tid; i <= p.m; i += nt) {
+        const bool e = i == p.m;                         // the epigraph row
+        double &l = e ? T.l0 : p.lmbda[om + i];
+        if (first) {
+            const double s = e ? T.s0 : p.s[om + i], z = e ? T.z0 : p.z[om + i];
+            const double d = sqrt(s / z), di = 1.0 / d;
+            if (e) { T.d0 = d; T.di0 = di; }
+            else { p.d[om + i] = d; p.di[om + i] = di; p.di2[om + i] = di * di; }
+            l = sqrt(s * z);
+        }
+        if (e) T.lsq0 = l * l; else p.lmbdasq[om + i] = l * l;
+    }
+    if (tid == 0) { S.sigma = 0.0; S.eta = 0.0; }       // :966
+}
+// the i-th Newton right-hand side (:978-1002), its refinement copy (:940-944) and f4_no_ir's steps before the solve
+// (:868-876): s := lmbda o\ s, z := z - W's.  Then kktsolver_e's (:1933-1937): a = z[0], ux = bx + bt grad f0 (in dx),
+// bzp = W^{-T} z[1:]
+__global__ void k_gp_dir_rhs(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    const double mu = S.gap / (p.m + 1), sm = S.sigma * mu, c = -1.0 + S.eta;
+    const double dt = c * T.rxt;
+    const bool ref = p.refinement > 0;
+    for (int k = tid; k < p.n; k += nt) {
+        const double v = c * p.rx[on + k];
+        if (ref) p.wx[oc + k] = v;
+        p.dx[on + k] = v + dt * g.gf0[on + k];
+    }
+    for (int k = tid; k < p.neq; k += nt) {
+        const double v = c * p.ry[oq + k];
+        p.dy[oq + k] = v;
+        if (ref) p.wy[oc + k] = v;
+    }
+    for (int k = tid; k <= p.m; k += nt) {
+        const bool e = k == p.m;
+        double s = -(e ? T.lsq0 : p.lmbdasq[om + k]) + sm, z = c * (e ? T.rz0 : p.rz[om + k]);
+        if (e) {
+            if (ref) { T.ws0 = s; T.wz0 = z; T.wxt = dt; }
+            s = s / T.l0; z = z - T.d0 * s;
+            T.ds0 = s; T.a = z; T.dt = dt;
+        } else {
+            if (ref) { p.ws[oc + k] = s; p.wz[oc + k] = z; }
+            s = s / p.lmbda[om + k]; z = z - p.d[om + k] * s;
+            p.ds[om + k] = s; p.bzp[om + k] = p.di[om + k] * z;
+        }
+    }
+}
+// f4_no_ir's steps before a refinement solve, on (wx2, wx2t, wz2, ws2): as k_gp_dir_rhs's
+__global__ void k_gp_f4_pre(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    const double bt = T.wx2t;
+    for (int k = tid; k < p.n; k += nt) p.wx2[oc + k] += bt * g.gf0[on + k];
+    for (int k = tid; k <= p.m; k += nt) {
+        if (k == p.m) {
+            const double s = T.ws20 / T.l0;
+            T.ws20 = s; T.a = T.wz20 - T.d0 * s;
+        } else {
+            const double s = p.ws2[oc + k] / p.lmbda[om + k], z = p.wz2[oc + k] - p.d[om + k] * s;
+            p.ws2[oc + k] = s; p.bzp[om + k] = p.di[om + k] * z;
+        }
+    }
+}
+// after batch_solve (kktsolver_e :1938-1941, f4_no_ir :883): z[0] = -bt dnl[0], z[1:] = W uz, t = grad f0'ux +
+// dnl[0]² bt - a, s := s - z.  acc = 0: the direction, in (dx, dt, dz, ds).  acc = 1: a refinement step on
+// (wx2, wx2t, wz2, ws2), added to the direction (:953-956)
+__global__ void k_gp_f4_post(Ptrs p, GPPtrs g, int acc) {
+    GP_SETUP
+    if (S.done) return;
+    const double *ux = acc ? p.wx2 + oc : p.dx + on;
+    double a = 0.0;
+    for (int k = tid; k < p.n; k += nt) a += g.gf0[on + k] * ux[k];
+    a = block_sum(a, sh);
+    for (int k = tid; k < p.m; k += nt) {
+        const double z = p.bzp[om + k];
+        if (acc) {
+            const double s = p.ws2[oc + k] - z;
+            p.wz2[oc + k] = z; p.ws2[oc + k] = s;
+            p.dz[om + k] += z; p.ds[om + k] += s;
+        } else {
+            p.dz[om + k] = z; p.ds[om + k] -= z;
+        }
+    }
+    if (acc) {
+        for (int k = tid; k < p.n; k += nt) p.dx[on + k] += ux[k];
+        for (int k = tid; k < p.neq; k += nt) p.dy[oq + k] += p.wy2[oc + k];
+    }
+    if (tid == 0) {
+        const double bt = acc ? T.wx2t : T.dt, d0 = T.d0;
+        const double z0 = -bt * d0, t = a + d0 * d0 * bt - T.a;
+        if (acc) {
+            const double s0 = T.ws20 - z0;
+            T.wz20 = z0; T.ws20 = s0; T.wx2t = t;
+            T.dz0 += z0; T.ds0 += s0; T.dt += t;
+        } else {
+            T.dz0 = z0; T.ds0 -= z0; T.dt = t;
+        }
+    }
+}
+// refinement residual, the elementwise part of res() (:889-923): wx2 = wx - grad f0 wz3[0], wx2t = 2 wxt + wz3[0]
+// (cp's H_e doubles v[1], :1812), wz3 = W^{-1} dz, wz2 = wz - W' ds (and the epigraph row's - (grad f0'dx - dt)),
+// ws2 = ws - lmbda o (dz + ds); EQ: wy2 = wy.  The H, A, A', [Df[1:]; G] and its transpose products follow as GEMVs
+__global__ void k_gp_res(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    double a = 0.0;
+    for (int k = tid; k < p.n; k += nt) a += g.gf0[on + k] * p.dx[on + k];
+    a = block_sum(a, sh);
+    const double w30 = T.di0 * T.dz0;
+    for (int k = tid; k < p.n; k += nt) p.wx2[oc + k] = p.wx[oc + k] - g.gf0[on + k] * w30;
+    for (int k = tid; k < p.neq; k += nt) p.wy2[oc + k] = p.wy[oc + k];
+    for (int k = tid; k < p.m; k += nt) {
+        const double dz = p.dz[om + k], ds = p.ds[om + k];
+        p.wz3[oc + k] = p.di[om + k] * dz;
+        p.wz2[oc + k] = p.wz[oc + k] - p.d[om + k] * ds;
+        p.ws2[oc + k] = p.ws[oc + k] - p.lmbda[om + k] * (ds + dz);
+    }
+    if (tid == 0) {
+        T.wz30 = w30;
+        T.wx2t = w30 + (T.wxt + T.wxt);
+        T.wz20 = (T.wz0 - (a - T.dt)) - T.d0 * T.ds0;
+        T.ws20 = T.ws0 - T.l0 * (T.ds0 + T.dz0);
+    }
+}
+// after the i-th direction (:1030-1078): dsdz, the unscaled steps dz2 = W^{-1} dz and ds2 = W' ds, scale2 of ds and
+// dz, the step to the boundary, phi and its directional derivative; the problem starts its line search
+__global__ void k_gp_dir_post(Ptrs p, GPPtrs g, int i) {
+    GP_SETUP
+    if (S.done) return;
+    double dsdz = 0, mins = INFINITY, minz = INFINITY;
+    for (int k = tid; k < p.m; k += nt) {
+        const double ds = p.ds[om + k], dz = p.dz[om + k], l = p.lmbda[om + k];
+        dsdz += ds * dz;
+        g.dz2[om + k] = p.di[om + k] * dz; g.ds2[om + k] = p.d[om + k] * ds;
+        const double ss = ds / l, zs = dz / l;
+        p.ds[om + k] = ss; p.dz[om + k] = zs;
+        mins = fmin(mins, ss); minz = fmin(minz, zs);
+    }
+    dsdz = block_sum(dsdz, sh);
+    mins = block_min(mins, sh);
+    minz = block_min(minz, sh);
+    if (tid == 0) {
+        dsdz += T.ds0 * T.dz0;
+        T.dz20 = T.di0 * T.dz0; T.ds20 = T.d0 * T.ds0;
+        T.ds0 /= T.l0; T.dz0 /= T.l0;
+        mins = fmin(mins, T.ds0); minz = fmin(minz, T.dz0);
+        const double t = fmax(0.0, fmax(-mins, -minz));
+        S.step = t == 0.0 ? 1.0 : fmin(1.0, GP_STEP / t);
+        S.dsdz = dsdz;
+        T.phi = T.th1 * S.gap + T.th2 * S.resx + T.th3 * T.resznl;
+        T.dphi = i == 0 ? -T.phi
+                        : -T.th1 * (1 - S.sigma) * S.gap - T.th2 * (1 - S.eta) * S.resx - T.th3 * (1 - S.eta) * T.resznl;
+        T.searching = 1.0;
+    }
+}
+// the line search's trial point (:1127-1130): (x, t, y, z, s) + step (dx, dt, dy, dz2, ds2); nrx = 0 (the GEMVs add
+// newDf'newznl + G'newzl + A'newy)
+__global__ void k_gp_trial(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done || T.searching == 0.0) return;
+    const double st = S.step;
+    for (int k = tid; k < p.n; k += nt) { g.nx[on + k] = p.x[on + k] + st * p.dx[on + k]; g.nrx[on + k] = 0.0; }
+    for (int k = tid; k < p.neq; k += nt) g.ny[oq + k] = p.y[oq + k] + st * p.dy[oq + k];
+    for (int k = tid; k < p.m; k += nt) {
+        g.nz[om + k] = p.z[om + k] + st * g.dz2[om + k];
+        g.ns[om + k] = p.s[om + k] + st * g.ds2[om + k];
+    }
+    if (tid == 0) { T.nt = T.t + st * T.dt; T.nz0 = T.z0 + st * T.dz20; T.ns0 = T.s0 + st * T.ds20; }
+}
+// copies of the state a relaxed line search saves (:1190-1214) and a resumed one restores (:1239-1260); `dir`: the
+// step vectors too (not on the restore after a singular KKT matrix, :790-813, which restores the residuals instead)
+__device__ void gp_save(const Ptrs &p, const GPPtrs &g, int b, bool save, bool dir, bool res) {
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const long long on = (long long)b * p.n, om = (long long)b * p.m, oc = (long long)b * p.L, oq = (long long)b * p.neq;
+    auto cp = [save](double *live, double *kept) { if (save) *kept = *live; else *live = *kept; };
+    for (int k = tid; k < p.n; k += nt) {
+        cp(p.x + on + k, g.x0 + oc + k);
+        if (dir) cp(p.dx + on + k, g.dx0 + oc + k);
+        if (res) cp(p.rx + on + k, g.rx0 + oc + k);
+    }
+    for (int k = tid; k < p.neq; k += nt) {
+        cp(p.y + oq + k, g.y0 + oc + k);
+        if (dir) cp(p.dy + oq + k, g.dy0 + oc + k);
+        if (res) cp(p.ry + oq + k, g.ry0 + oc + k);
+    }
+    for (int k = tid; k < p.m; k += nt) {
+        cp(p.s + om + k, g.s0 + oc + k); cp(p.z + om + k, g.z0 + oc + k);
+        cp(p.lmbda + om + k, g.l0 + oc + k);
+        cp(p.d + om + k, g.d0 + oc + k); cp(p.di + om + k, g.di0 + oc + k);
+        if (!save) p.di2[om + k] = p.di[om + k] * p.di[om + k];
+        if (dir) {
+            cp(p.ds + om + k, g.ds0 + oc + k); cp(p.dz + om + k, g.dz0 + oc + k);
+            cp(g.ds2 + om + k, g.ds20 + oc + k); cp(g.dz2 + om + k, g.dz20 + oc + k);
+        }
+        if (res) cp(p.rz + om + k, g.rz0 + oc + k);
+    }
+    if (tid == 0) {
+        GPScal &T = gp_scal(g, oc);
+        cp(&T.t, &T.t0); cp(&T.s0, &T.s00); cp(&T.z0, &T.z00); cp(&T.l0, &T.l00); cp(&T.d0, &T.d00);
+        cp(&T.di0, &T.di00);
+        if (dir) { cp(&T.dt, &T.dt0); cp(&T.ds0, &T.ds00); cp(&T.dz0, &T.dz00); cp(&T.ds20, &T.ds200); cp(&T.dz20, &T.dz200); }
+        if (res) { cp(&T.rxt, &T.rxt0); cp(&T.rz0, &T.rz00); }
+    }
+}
+// the line search's decision for slot b (:1131-1261) once the GEMVs have formed newrx: newgap, newphi and cpl's
+// relaxed-line-search state machine.  A problem still searching halves its step (or resumes the saved search) and
+// counts itself in nsearch; a step that underflows to 0 ends the problem 'unknown' (status 3) on its iterate
+template <bool EQ> __global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, int *nsearch) {
+    GP_SETUP
+    __shared__ int act;                                  // 1: save the state, 2: restore it
+    if (S.done || T.searching == 0.0) return;
+    const double *f = g.fv + (long long)b * g.nK;
+    double rx2 = 0, rn2 = 0;
+    for (int k = tid; k < p.n; k += nt) { const double v = g.nrx[on + k]; rx2 += v * v; }
+    for (int k = tid; k < g.mnl; k += nt) { const double v = g.ns[om + k] + f[k + 1]; rn2 += v * v; }
+    rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh);
+    if (tid == 0) {
+        const double rxt = -T.nz0 + 1.0, r0 = T.ns0 + (f[0] - T.nt);
+        const double nresx = sqrt(rx2 + rxt * rxt), nresznl = sqrt(rn2 + r0 * r0);
+        const double step = S.step, gap = S.gap;
+        const double ngap = (1.0 - (1.0 - S.sigma) * step) * gap + step * step * S.dsdz;
+        const double nphi = T.th1 * ngap + T.th2 * nresx + T.th3 * nresznl;
+        const int rel = (int)T.relaxed;
+        bool back = true;
+        act = 0;
+        if (i == 0) {
+            if (ngap <= (1.0 - GP_ALPHA * step) * gap &&
+                ((0 <= rel && rel < GP_MAX_RELAXED) || nphi <= T.phi + GP_ALPHA * step * T.dphi)) {
+                back = false;
+                S.sigma = fmin(ngap / gap, pow(ngap / gap, 3.0));
+                S.eta = 0.0;
+            }
+        } else if (rel == -1) {                          // standard; relaxed_iters stays -1 (:1178 compares)
+            if (nphi <= T.phi + GP_ALPHA * step * T.dphi) back = false;
+        } else if (rel == 0) {
+            if (!(nphi <= T.phi + GP_ALPHA * step * T.dphi)) {
+                T.phi0 = T.phi; T.dphi0 = T.dphi; T.gap0 = gap; T.step0 = step; T.dsdz0 = S.dsdz;
+                T.sigma0 = S.sigma; T.eta0 = S.eta;
+                T.relaxed = 1; act = 1;
+            }
+            back = false;
+        } else if (rel < GP_MAX_RELAXED) {
+            T.relaxed = nphi <= T.phi0 + GP_ALPHA * T.step0 * T.dphi0 ? 0 : rel + 1;
+            back = false;
+        } else if (nphi <= T.phi0 + GP_ALPHA * T.step0 * T.dphi0) {
+            back = false; T.relaxed = 0;
+        } else {                                         // resume the saved line search as a standard one
+            T.phi = T.phi0; T.dphi = T.dphi0; S.gap = T.gap0; S.step = T.step0; S.dsdz = T.dsdz0;
+            S.sigma = T.sigma0; S.eta = T.eta0;
+            T.relaxed = -1; act = 2;
+        }
+        if (back && act == 0) S.step = step * GP_BETA;
+        if (!back) T.searching = 0.0;
+        else if (S.step == 0.0) { T.searching = 0.0; S.done = 1; S.status = 3; S.iters = iter; }
+        else atomicAdd(nsearch, 1);
+    }
+    __syncthreads();
+    if (act) gp_save(p, g, b, act == 1, true, act == 1);
+}
+// a singular KKT matrix after iteration 0 (:778-840): with 0 < relaxed_iters < 8 the problem restores the saved state
+// (W, x, y, s, z, lmbda, the residuals, phi and gap) and is factored again (counted in nre); otherwise, or when the
+// second factorisation fails too (second = 1), it ends 'unknown' (status 3) on its current iterate
+template <bool EQ> __global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *info, int iter, int second, int *nre) {
+    GP_SETUP
+    __shared__ int act;
+    if (S.done || (info[b] <= 0 && !(EQ && p.infop[b] > 0))) return;
+    if (tid == 0) {
+        act = !second && T.relaxed > 0 && T.relaxed < GP_MAX_RELAXED;
+        if (act) {
+            T.phi = T.phi0; S.gap = T.gap0; T.relaxed = -1;
+            atomicAdd(nre, 1);
+        } else { S.done = 1; S.status = 3; S.iters = iter; }
+    }
+    __syncthreads();
+    if (!act) return;
+    gp_save(p, g, b, false, false, true);
+    __syncthreads();
+    double rx2 = 0, rn2 = 0;
+    for (int k = tid; k < p.n; k += nt) { const double v = p.rx[on + k]; rx2 += v * v; }
+    for (int k = tid; k < g.mnl; k += nt) { const double v = p.rz[om + k]; rn2 += v * v; }
+    rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh);
+    if (tid == 0) { S.resx = sqrt(rx2 + T.rxt * T.rxt); T.resznl = sqrt(rn2 + T.rz0 * T.rz0); }
+}
+// the update (:1264-1355): x, t, y += step d; ds, dz := e + step d; scale2 inverse; update_scaling with dnl and d
+// alike; s = W' lmbda, z = W^{-1} lmbda; gap = lmbda'lmbda
+__global__ void k_gp_update(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    const double step = S.step;
+    for (int k = tid; k < p.n; k += nt) p.x[on + k] += step * p.dx[on + k];
+    for (int k = tid; k < p.neq; k += nt) p.y[oq + k] += step * p.dy[oq + k];
+    double gap = 0.0;
+    for (int k = tid; k <= p.m; k += nt) {
+        const bool e = k == p.m;
+        const double lk = e ? T.l0 : p.lmbda[om + k];
+        const double ss = sqrt((1.0 + step * (e ? T.ds0 : p.ds[om + k])) * lk);
+        const double sz = sqrt((1.0 + step * (e ? T.dz0 : p.dz[om + k])) * lk);
+        const double d = (e ? T.d0 : p.d[om + k]) * ss / sz, di = 1.0 / d, ln = ss * sz;
+        if (e) { T.d0 = d; T.di0 = di; T.l0 = ln; T.s0 = d * ln; T.z0 = di * ln; T.t += step * T.dt; }
+        else {
+            p.d[om + k] = d; p.di[om + k] = di; p.di2[om + k] = di * di; p.lmbda[om + k] = ln;
+            p.s[om + k] = d * ln; p.z[om + k] = di * ln;
+        }
+        gap += ln * ln;
+    }
+    gap = block_sum(gap, sh);
+    if (tid == 0) S.gap = gap;
+}
 }  // namespace
 
 struct cvxb_batch {
@@ -1349,6 +1811,7 @@ struct cvxb_batch {
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     bool loaded = false;
     int iters_run = 0;
+    int ls_rounds = 0;               // gp: line-search rounds of the last solve
     double solve_ms = 0;
     // single large problem: SYRK on the int8 tensor path (ozaki_syrk.cu), same rule as cvxb_kkt_factor
     // (ozaki_use) when B == 1 and there are no 'q' cones; ozaki_mode() at create
@@ -1381,6 +1844,13 @@ struct cvxb_batch {
     DevBuf<double> start;
     Warm warm{};
     bool warm_set = false;
+    // geometric programs (cvxb_batch_create_gp): m = mnl + ml rows, G holds [Df[1:]; G; F] (ld ldg = m + sum K rounded
+    // up to even), P holds H; gq's per-slot vectors live in gpv, H's scaled rows in gph, the block offsets in koff and
+    // g, in problem order, in gpg (copied into the state row by each solve)
+    bool gp = false;
+    GPPtrs gq{};
+    DevBuf<double> gpv, gph, gpg;
+    DevBuf<int> koff;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -1399,7 +1869,9 @@ int state_alloc(cvxb_batch *b) {
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
     const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
-    const long long L = cone + sb + ref + lps;
+    // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m)
+    const long long gpl = b->gp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
+    const long long L = cone + sb + ref + lps + gpl;
     if (b->L == L) return 0;
     b->L = p.L = 0;
     b->cst.reset();
@@ -1421,6 +1893,13 @@ int state_alloc(cvxb_batch *b) {
         if (p2) { p.wy = r; r += p2; p.wy2 = r; r += p2; }
     }
     if (lps) p.lps = r;
+    if (gpl) {
+        GPPtrs &g = b->gq;
+        g.g = r; r += ev(g.sumK); g.gs = r; r += ev(sizeof(GPScal) / sizeof(double));
+        for (double **v : {&g.x0, &g.dx0, &g.rx0}) { *v = r; r += n2; }
+        for (double **v : {&g.y0, &g.dy0, &g.ry0}) { *v = r; r += p2; }
+        for (double **v : {&g.s0, &g.z0, &g.ds0, &g.dz0, &g.ds20, &g.dz20, &g.l0, &g.d0, &g.di0, &g.rz0}) { *v = r; r += m2; }
+    }
     return 0;
 }
 
@@ -1659,7 +2138,9 @@ template <bool EQ> int start_check(cvxb_batch *b) {
     for (int i = 0; i < B; ++i)
         if (info[i] > 0 || (EQ && infop[i] > 0)) {
             const int k = b->perm[i];
-            if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
+            if (b->gp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (singular KKT "
+                                 "matrix at the start)", k);
+            else if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
                                  "the start)", k);
             else if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
                                    "at the start)", k);
@@ -1833,6 +2314,194 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
     return 0;
 }
 
+// ---- geometric programs: the lock-step cpl (cvxprog.py:622-1356) of gp's epigraph problem ----
+// F(x) over the active slots at x (slot k at x + k*sx): yv = F x, then k_gp_eval (full: with Df, H's rows and weights)
+int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) {
+    const GPPtrs &g = b->gq;
+    const int B = b->Bact;
+    GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = sx; gf.sy = g.sumK;
+    CVXB_TRY(gemv_n(g.sumK, b->n, g.G + b->m, g.ldg, nullptr, x, 1.0, 0.0, g.yv, b->gemv_ws.p, b->st, gf));
+    if (full) k_gp_eval<true><<<dim3(g.nK, B), 256, 0, b->st>>>(b->p, g, trial);
+    else k_gp_eval<false><<<dim3(g.nK, B), 256, 0, b->st>>>(b->p, g, trial);
+    count_launch();
+    return 0;
+}
+// r += F' w + G' zl (+ A' y): Df' znl + G' zl + A' y with Df' znl = F'(z_i y) (slot k's z at z + k*m)
+template <bool EQ> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r) {
+    const GPPtrs &g = b->gq;
+    const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
+    GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
+    CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
+    if (ml > 0) {
+        GemvBatch gl; gl.batch = B; gl.sA = g.sG; gl.sx = m; gl.sy = n;
+        CVXB_TRY(gemv_t(ml, n, g.G + g.mnl, g.ldg, nullptr, z + g.mnl, 1.0, 1.0, r, b->st, gl));
+    }
+    if (EQ) {
+        GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = b->neq; ga.sy = n;
+        CVXB_TRY(gemv_t(b->neq, n, b->A.p, b->lda, nullptr, y, 1.0, 1.0, r, b->st, ga));
+    }
+    return 0;
+}
+// H = sum_i z_i Fi'(diag(yi) - yi yi')Fi from k_gp_eval's rows (the reference's syrk with alpha = z[i], :2141-2150),
+// lower triangle; mirrored when the refinement's residual multiplies by it
+int gp_hessian(cvxb_batch *b) {
+    const GPPtrs &g = b->gq;
+    GemmDesc h;
+    h.M = b->n; h.N = b->n; h.K = g.sumK;
+    h.X = g.Hr; h.ldx = (int)g.ldh; h.x_kmajor = true; h.sX = g.sH;
+    h.Y = g.Hr; h.ldy = (int)g.ldh; h.y_kmajor = true; h.sY = g.sH;
+    h.w = g.hw; h.sW = g.sumK;
+    h.C = b->P.p; h.ldc = (int)b->ldp; h.sC = b->sP;
+    h.lower_only = true; h.batch = b->Bact;
+    if (b->B == 1) h.splitk_ws = b->cw.splitk_ws.p;
+    CVXB_TRY(dmma_gemm(h, b->st));
+    if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, b->st));
+    return 0;
+}
+// one int of the device counter d_ndone, after the stream has drained
+int read_count(cvxb_batch *b, int &v) {
+    CVXB_CUDA(cudaMemcpyAsync(&v, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    return 0;
+}
+// the i-th Newton direction of cpl (:966-1045): right-hand side, kktsolver_e's solve and `refinement` steps from
+// res() (:889-956), then the step to the boundary and the merit function's slope
+template <bool EQ> int gp_direction(cvxb_batch *b, int i) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
+    const Ptrs &p = b->p;
+    const GPPtrs &g = b->gq;
+    const long long L = b->L;
+    k_gp_dir_rhs<<<B, T, 0, st>>>(p, g); count_launch();
+    CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
+    k_gp_f4_post<<<B, T, 0, st>>>(p, g, 0); count_launch();
+    for (int r = 0; r < p.refinement; ++r) {
+        k_gp_res<<<B, T, 0, st>>>(p, g); count_launch();
+        GemvBatch gH; gH.batch = B; gH.sA = b->sP; gH.sx = n; gH.sy = L;                 // wx2 -= H dx
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gH));
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
+            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
+        }
+        if (m > 0) {                                     // wx2 -= [Df[1:]; G]' wz3[1:]
+            GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
+            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+        }
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
+        }
+        if (m > 0) {                                     // wz2[1:] -= [Df[1:]; G] dx
+            GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
+            CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
+        }
+        k_gp_f4_pre<<<B, T, 0, st>>>(p, g); count_launch();
+        CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
+        k_gp_f4_post<<<B, T, 0, st>>>(p, g, 1); count_launch();
+    }
+    k_gp_dir_post<<<B, T, 0, st>>>(p, g, i); count_launch();
+    return 0;
+}
+// the lock-step line search after the i-th direction (:1125-1261): each round evaluates F and newrx at every
+// searching problem's trial point and takes its decision; one readback of the count still searching per round
+template <bool EQ> int gp_line_search(cvxb_batch *b, int i, int it) {
+    cudaStream_t st = b->st;
+    const int n = b->n, B = b->Bact, T = 256;
+    const Ptrs &p = b->p;
+    const GPPtrs &g = b->gq;
+    for (int left = 1; left > 0; b->ls_rounds++) {
+        k_gp_trial<<<B, T, 0, st>>>(p, g); count_launch();
+        CVXB_TRY(gp_eval(b, g.nx, n, false, 1));
+        CVXB_TRY(gp_rx<EQ>(b, g.nz, g.ny, g.nrx));
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_gp_ls<EQ><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p); count_launch();
+        CVXB_LAUNCH_CHECK();
+        CVXB_TRY(read_count(b, left));
+    }
+    return 0;
+}
+// H into P and K = H + [Df[1:]; G]' diag(di²) [Df[1:]; G] (+ A'A) factored, from F(x) at the slots' iterates
+int gp_factor(cvxb_batch *b, bool first) {
+    CVXB_TRY(gp_hessian(b));
+    return batch_factor(b, !first);
+}
+template <bool EQ> int solve_gp(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, T = 256, pq = b->neq;
+    const Ptrs &p = b->p;
+    const GPPtrs &g = b->gq;
+    const int ml = m - g.mnl;
+    int B = b->B;
+    b->Bact = B;
+    b->switched = false;
+    b->ls_rounds = 0;
+    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
+    CVXB_CUDA(cudaEventRecord(b->e0, st));
+    // every problem in its own slot (restore_order ran): g into the state row
+    CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
+                                g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
+    k_gp_init<<<B, T, 0, st>>>(p, g); count_launch();
+    std::vector<int> flags(B), pairs;
+    int it = 0;
+    for (it = 0; it <= maxiters; ++it) {
+        // F(x, z[:mnl]) and the residuals (:627-691)
+        CVXB_TRY(gp_eval(b, p.x, n, true, 0));
+        k_gp_res_begin<EQ><<<B, T, 0, st>>>(p, g); count_launch();
+        CVXB_TRY(gp_rx<EQ>(b, p.z, p.y, p.rx));
+        if (EQ) {
+            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = pq;
+            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, ga));
+        }
+        if (ml > 0) {
+            GemvBatch gl; gl.batch = B; gl.sA = g.sG; gl.sx = n; gl.sy = m;
+            CVXB_TRY(gemv_n(ml, n, g.G + g.mnl, g.ldg, nullptr, p.x, 1.0, 1.0, p.rz + g.mnl, b->gemv_ws.p, st, gl));
+        }
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_gp_stats<EQ><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        count_launch();
+        int ndone = 0;
+        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CVXB_TRY(read_count(b, ndone));
+        if (ndone >= B) break;
+        if (ndone > 0 && b->compact && b->B > 1) {
+            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
+            B = b->Bact;
+            if (!pairs.empty()) CVXB_TRY(gp_eval(b, p.x, n, true, 0));    // F(x)'s per-slot results stay put
+        }
+        k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0); count_launch();
+        if (it == 0) {                   // kkt_chol2's first call; still singular: the Rank ValueError (:778-783)
+            CVXB_TRY(gp_factor(b, true));
+            CVXB_TRY(first_switch<EQ>(b));
+            CVXB_TRY(start_check<EQ>(b));
+        } else {
+            CVXB_TRY(gp_factor(b, false));
+            CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+            k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p); count_launch();
+            int nre = 0;
+            CVXB_TRY(read_count(b, nre));
+            if (nre > 0) {               // restored problems are factored again at their saved iterates
+                CVXB_TRY(gp_eval(b, p.x, n, true, 0));
+                CVXB_TRY(gp_factor(b, false));
+                k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p); count_launch();
+            }
+        }
+        for (int i = 0; i < 2; ++i) {
+            CVXB_TRY(gp_direction<EQ>(b, i));
+            CVXB_TRY(gp_line_search<EQ>(b, i, it));
+        }
+        k_gp_update<<<B, T, 0, st>>>(p, g); count_launch();
+        CVXB_LAUNCH_CHECK();
+    }
+    b->iters_run = it;
+    b->Bact = b->B;
+    CVXB_CUDA(cudaEventRecord(b->e1, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    float t = 0;
+    cudaEventElapsedTime(&t, b->e0, b->e1);
+    b->solve_ms = t;
+    return 0;
+}
+
 // dst[problem] = src[slot] for a [B x len] per-slot array, through the slot permutation (d_perm, uploaded by the
 // caller) when the last solve compacted
 int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space) {
@@ -1852,7 +2521,9 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
 
 // a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q', and with sdp 's' blocks)
 // and p equality rows.  Every argument is checked before the device is.
-int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp, bool sdp = false) {
+// xrows > 0 (a GP batch): G gets xrows more rows below the m cone rows, for F
+int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp, bool sdp = false,
+           int xrows = 0) {
     if (out) *out = nullptr;
     if (!out || nprob <= 0 || n <= 0 || !dims) {
         set_error("batch_create: bad sizes (nprob and n positive, dims given)");
@@ -1905,7 +2576,7 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
     b->device = device; b->B = nprob; b->n = n; b->m = m; b->lp = lp;
     b->i8_mode = ozaki_mode();
-    b->ldg = ((m + 1) & ~1) > 2 ? ((m + 1) & ~1) : 2;
+    b->ldg = ((m + xrows + 1) & ~1) > 2 ? ((m + xrows + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
     b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;
     b->nblk = (n + NB - 1) / NB;
@@ -1921,7 +2592,7 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
     // GEMV workspace: G x (m rows); with equality rows also A x (p rows) and Asct y (n rows)
     const size_t me = (size_t)(m > 0 ? m : 1);
-    size_t ws = me * gemv_n_chunks(n);
+    size_t ws = std::max(me, (size_t)xrows) * gemv_n_chunks(n);
     if (p > 0) ws = std::max({ws, (size_t)p * gemv_n_chunks(n), (size_t)n * gemv_n_chunks(p)});
     CVXB_TRY(b->gemv_ws.alloc(B * ws));
     // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
@@ -2071,6 +2742,54 @@ int cvxb_batch_create_sdp_qp(cvxb_batch **out, int nprob, int n, int p, const cv
     return create(out, nprob, n, p, dims, device, false, true);
 }
 
+int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *K, int ml, int p, int device) {
+    if (out) *out = nullptr;
+    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || nK < 1 || !K || ml < 0 || p < 0) {
+        set_error("batch_create_gp: bad sizes (nprob in 1..%d, n >= 1, nK >= 1 with K given, ml and p nonnegative)",
+                  CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    long long sumK = 0;
+    for (int i = 0; i < nK; ++i) {
+        if (K[i] < 1) { set_error("batch_create_gp: K[%d] = %d < 1", i, K[i]); return CVXB_E_ARG; }
+        sumK += K[i];
+    }
+    if (sumK + nK + ml > (1LL << 30)) { set_error("batch_create_gp: too many rows"); return CVXB_E_ARG; }
+    const int mnl = nK - 1;
+    cvxb_dims d{};
+    d.ml = mnl + ml;
+    cvxb_batch *raw = nullptr;
+    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, false, (int)sumK));
+    std::unique_ptr<cvxb_batch> b(raw);
+    const size_t B = nprob, m = b->m;
+    GPPtrs &g = b->gq;
+    g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
+    g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
+    g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
+    std::vector<int> off(nK + 1, 0);
+    for (int i = 0; i < nK; ++i) off[i + 1] = off[i] + K[i];
+    CVXB_TRY(b->koff.alloc(nK + 1));
+    CVXB_CUDA(cudaMemcpy(b->koff.p, off.data(), (nK + 1) * sizeof(int), cudaMemcpyHostToDevice));
+    g.koff = b->koff.p;
+    CVXB_TRY(b->gph.alloc(B * g.sH));
+    CVXB_TRY(b->gpg.alloc(B * sumK));
+    // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
+    const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * m;
+    CVXB_TRY(b->gpv.alloc(B * len));
+    CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
+    double *v = b->gpv.p;
+    auto take = [&](size_t l) { double *r = v; v += B * l; return r; };
+    g.Hr = b->gph.p;
+    g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
+    g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
+    g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
+    b->gp = true;
+    b->p.refinement = m > 0 ? 1 : 0;                  // cpl's default (cvxprog.py:422)
+    CVXB_TRY(state_alloc(b.get()));
+    *out = b.release();
+    return 0;
+}
+
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
@@ -2090,6 +2809,7 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
                     const double *h, int space) {
     if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
     if (b->lp) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
+    if (b->gp) { set_error("batch_load: a GP batch is loaded with cvxb_batch_load_gp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t n = b->n;
@@ -2102,10 +2822,38 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
 
 int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space) {
     if (!b || !c || !G || !h) { set_error("batch_load_lp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->lp) { set_error("batch_load_lp: a QP batch is loaded with cvxb_batch_load"); return CVXB_E_ARG; }
+    if (!b->lp) { set_error("batch_load_lp: a QP or GP batch is not a cone LP batch"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     return load_common(b, c, G, h, (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
 }
+
+int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const double *G, const double *h, int space) {
+    if (!b || !F || !g || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_gp: NULL argument"); return CVXB_E_ARG; }
+    if (!b->gp) { set_error("batch_load_gp: not a GP batch (cvxb_batch_create_gp)"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const size_t B = b->B, n = b->n, m = b->m, mnl = b->gq.mnl, ml = m - mnl, sK = b->gq.sumK;
+    // F below the m rows of [Df[1:]; G], G below the mnl rows of Df[1:], h in the 'l' rows; q (c's x part) is 0
+    CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + m, b->ldg * sizeof(double), F, sK * sizeof(double), sK * sizeof(double),
+                                n * B, kind, b->st));
+    CVXB_CUDA(cudaMemcpyAsync(b->gpg.p, g, B * sK * sizeof(double), kind, b->st));
+    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->h), 0, B * (m ? m : 1) * sizeof(double), b->st));
+    if (ml > 0) {
+        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + mnl, b->ldg * sizeof(double), G, ml * sizeof(double),
+                                    ml * sizeof(double), n * B, kind, b->st));
+        CVXB_CUDA(cudaMemcpy2DAsync(const_cast<double *>(b->h) + mnl, m * sizeof(double), h, ml * sizeof(double),
+                                    ml * sizeof(double), B, kind, b->st));
+    }
+    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    b->eq_loaded = false;
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    b->permuted = false;
+    return 0;
+}
+
+int cvxb_batch_ls_rounds(cvxb_batch *b) { return b ? b->ls_rounds : CVXB_E_ARG; }
 
 int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space) {
     if (!b) { set_error("batch_load_eq: batch is NULL"); return CVXB_E_ARG; }
@@ -2127,6 +2875,7 @@ int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int s
 int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const double *y, const double *z,
                           int space) {
     if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
+    if (b->gp) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
     if (b->lp && ((!x) != (!s) || (y && !z) || (!x && !z))) {
         set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
                   "both");
@@ -2164,6 +2913,8 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     }
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
+    if (b->gp) return b->neq > 0 ? solve_gp<true>(b, maxiters, abstol, reltol, feastol)
+                                 : solve_gp<false>(b, maxiters, abstol, reltol, feastol);
     using Solve = int (*)(cvxb_batch *, int, double, double, double);
     static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
                                      solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,

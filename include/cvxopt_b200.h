@@ -391,6 +391,30 @@ int cvxb_batch_results_y(cvxb_batch *b, double *y, int space);
 int cvxb_batch_stats(cvxb_batch *b, double *solve_ms, int *iterations);
 /* kernel of the factorisations' SYRK in the last solve: 1 fp64 DMMA, 2 int8 slices (as cvxb_kkt_syrk_path) */
 int cvxb_batch_syrk_path(cvxb_batch *b);
+/* batch of geometric programs (B x solvers.gp, cvxprog.py:1967-2155, with its default kktsolver 'chol2'):
+ *     minimize  log sum exp(F0 x + g0)  s.t.  log sum exp(Fi x + gi) <= 0 (i = 1..mnl),  G x <= h,  A x = b
+ * with the block sizes K[0..nK-1] (mnl = nK - 1) shared by the batch, ml rows of G and p rows of A.  It runs cpl on
+ * gp's epigraph problem (cp, :1746-1964) in lock-step, line search included.  CVXB_E_ARG, checked before the device:
+ * nprob outside 1..CVXB_BATCH_MAX, n < 1, nK < 1, some K[i] < 1, ml < 0, p < 0, and gp's "Rank(A) < p" for p > n.
+ * Load it with cvxb_batch_load_gp (and cvxb_batch_load_eq when p > 0); cvxb_batch_load, cvxb_batch_load_lp and
+ * cvxb_batch_load_start on it are CVXB_E_ARG (gp takes no starting point).  Solve, set_refinement (default 1, as cpl),
+ * results, results_y, stats and destroy are the other batches' calls: s and z have the mnl + ml rows [snl; sl] and
+ * [znl; zl] (the epigraph row is dropped), the primal objective is t and the dual objective cpl's.  Status 1 optimal,
+ * 2 maximum iterations, 3 singular KKT matrix or a line-search step that underflowed to 0 ('unknown' for 2 and 3).
+ * A singular factorisation at iteration 0 makes cvxb_batch_solve return CVXB_E_ARG with "problem %d: Rank(A) < p or
+ * Rank([H(x); A; Df(x); G]) < n".  Device memory per problem, with m = mnl + ml, S = sum K, ev() rounding up to even:
+ * what cvxb_batch_create_eq's batch of the same n, p and dims {'l': m} holds with refinement 1, except that G is
+ * ev(m + S) x n and the GEMV workspace holds max(m, S) rows, plus ev(S)*n (H's scaled rows), 4S + nK + 3n + p + 4m
+ * (softmax, weights, f, grad f0, g, the unscaled steps and the line search's trial point) and ev(S) + 56 + 3 ev(n) +
+ * 3 ev(p) + 10 ev(m) in the state row (g, the scalars and the line search's saved state); and, shared by the batch,
+ * nK + 1 ints; all of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy. */
+int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *K, int ml, int p, int device);
+/* GP batch only: F nprob x (S x n column-major, ld S), g nprob x S, G nprob x (ml x n column-major, ld ml), h
+ * nprob x ml; G and h may be NULL when ml = 0.  A and b come through cvxb_batch_load_eq. */
+int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const double *G, const double *h, int space);
+/* line-search rounds of the last solve of a GP batch (every round evaluates F at every searching problem's trial
+ * point); 0 for the other batches */
+int cvxb_batch_ls_rounds(cvxb_batch *b);
 
 #ifdef __cplusplus
 }
