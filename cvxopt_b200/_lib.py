@@ -39,6 +39,10 @@ class SblockArgs(C.Structure):
 
 SK_NT_COMPUTE, SK_UPDATE, SK_DIR_POST, SK_EIG_START, SK_EIG_WARM, SK_BUILD_GS, SK_WTZ, SK_RES = range(8)
 
+# cvxb_cp_eval_fn(ctx, k, full, x, z, problem, f, Df, H, stream)
+CP_EVAL_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                         C.c_void_p, C.c_void_p, C.c_void_p)
+
 _SIGS = {
     # name: (restype, argtypes)
     "cvxb_last_error": (C.c_char_p, []),
@@ -139,6 +143,9 @@ _SIGS = {
                                        C.c_int, C.c_int, C.c_int]),
     "cvxb_batch_load_gp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_ls_rounds": (C.c_int, [C.c_void_p]),
+    "cvxb_batch_create_cp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "cvxb_batch_load_cp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "cvxb_batch_set_cp_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "cvxb_batch_results": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
 }

@@ -730,6 +730,213 @@ def gp_batch(K, F, g, G=None, h=None, A=None, b=None, device=0, nsub=None, **opt
     return out
 
 
+class _DevArray:
+    """a device buffer of the batch handle, for torch.as_tensor (__cuda_array_interface__, no copy)"""
+
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = {"data": (ptr, False), "shape": shape, "typestr": typestr, "version": 2}
+
+
+class CPBatch(QPBatch):
+    """B smooth convex programs (cvxb_batch_create_cp): B x solvers.cp(F, G, h, dims={'l': ml}, A, b), the GP batch's
+    lock-step cpl on cp's epigraph problem with F evaluated by the caller's batched F on the device.  mnl, ml rows of
+    G and p rows of A are shared by the batch.  load() takes x0 (B, n), G (B, ml, n), h (B, ml) and, with p > 0,
+    A (B, p, n), b (B, p); set_F() takes cp_batch's F.  `index` is each problem's index in the caller's order, passed to
+    F as idx.  results()' s and z are [snl; sl] and [znl; zl]; its primal objective is cp's t."""
+
+    def __init__(self, nprob, n, mnl, ml, p=0, device=0, index=None):
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.B, self.n, self.p, self.device = int(nprob), int(n), int(p), int(device)
+        self.mnl, self.ml = int(mnl), int(ml)
+        self.m = self.mnl + self.ml
+        rc = self._lib.cvxb_batch_create_cp(C.byref(self._h), self.B, self.n, self.mnl, self.ml, self.p, self.device)
+        _lib.check(rc, "batch")
+        self._refinement = None
+        self.index = np.arange(self.B) if index is None else np.asarray(index)
+        self._cb = None
+        self._err = None
+
+    def load(self, x0, G, h, A=None, b=None):
+        B, n = self.B, self.n
+        x0 = np.ascontiguousarray(np.asarray(x0, dtype=np.float64))
+        G = np.zeros((B, 0, n)) if G is None else np.asarray(G, dtype=np.float64)
+        h = np.zeros((B, 0)) if h is None else np.ascontiguousarray(np.asarray(h, dtype=np.float64))
+        if x0.shape != (B, n) or G.shape != (B, self.ml, n) or h.shape != (B, self.ml):
+            raise TypeError("problem shapes do not match the batch")
+        Acm, bv = self._host_eq(A, b)
+        Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
+        _lib.check(self._lib.cvxb_batch_load_cp(self._h, x0.ctypes.data, Gcm.ctypes.data if self.ml else None,
+                                                h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_cp")
+        self._load_eq(Acm, bv, _lib.HOST)
+
+    def set_F(self, F):
+        """F(x, idx=idx) -> (f, Df) and F(x, z, idx=idx) -> (f, Df, H), as cp_batch takes it.  The callback runs F on
+        the batch's stream and copies what it returns into the handle's buffers; an exception in F is kept and
+        re-raised by solve()"""
+        import torch
+        dev = torch.device("cuda", self.device)
+        B, n, nf = self.B, self.n, self.mnl + 1
+        gidx = torch.as_tensor(self.index, dtype=torch.int64, device=dev)
+        views, streams = {}, {}
+
+        def view(ptr, shape, typestr="<f8"):
+            t = views.get(ptr)
+            if t is None:
+                t = views[ptr] = torch.as_tensor(_DevArray(ptr, (B,) + shape, typestr), device=dev)
+            return t
+
+        def check(v, shape, which, rows, cols):
+            if not isinstance(v, torch.Tensor) or v.dtype != torch.float64 or tuple(v.shape) != shape or \
+                    v.device != dev:
+                raise TypeError("%s output argument of F() must be a 'd' matrix of size (%d,%d): a float64 tensor "
+                                "of shape %s on %s" % (which, rows, cols, shape, dev))
+            return v
+
+        def cb(ctx, k, full, x, z, problem, f, Df, H, stream):
+            try:
+                st = streams.get(stream)
+                if st is None:
+                    st = streams[stream] = torch.cuda.ExternalStream(stream, device=dev)
+                with torch.cuda.device(dev), torch.cuda.stream(st):
+                    idx = gidx[view(problem, (), "<i4")[:k].long()]
+                    X = view(x, (n,))[:k]
+                    out = F(X, view(z, (nf,))[:k], idx=idx) if full else F(X, idx=idx)
+                    if not isinstance(out, (tuple, list)) or len(out) != (3 if full else 2):
+                        raise TypeError("F(x, z) must return (f, Df, H)" if full else "F(x) must return (f, Df)")
+                    view(f, (nf,))[:k].copy_(check(out[0], (k, nf), "first", nf, 1))
+                    view(Df, (nf, n))[:k].copy_(check(out[1], (k, nf, n), "second", nf, n))
+                    if full:
+                        view(H, (n, n))[:k].copy_(check(out[2], (k, n, n), "third", n, n))
+                return 0
+            except BaseException as e:      # noqa: BLE001  re-raised by solve()
+                self._err = e
+                return 1
+        self._cb = _lib.CP_EVAL_FN(cb)
+        _lib.check(self._lib.cvxb_batch_set_cp_eval(self._h, C.cast(self._cb, C.c_void_p), None), "batch_set_cp_eval")
+
+    def solve(self, refinement=None, **options):
+        """QPBatch.solve; an exception raised in F comes out unchanged, and a problem named in an error is named by its
+        index in the caller's order"""
+        import re
+        self._err = None
+        try:
+            super().solve(refinement, **options)
+        except ValueError as e:
+            err, self._err = self._err, None
+            if err is not None:
+                raise err
+            k = re.search(r"problem (\d+):", str(e))
+            if k is None:
+                raise
+            raise ValueError(str(e).replace(k.group(0), "problem %d:" % self.index[int(k.group(1))], 1)) from None
+
+    def stats(self):
+        out = super().stats()
+        out["line_search_rounds"] = self._lib.cvxb_batch_ls_rounds(self._h)
+        return out
+
+    def close(self):
+        super().close()
+        self._cb = None
+
+
+class CPBatchGroup(QPBatchGroup):
+    """QPBatchGroup's interleaved sub-batches, solved concurrently, for convex programs.  Each sub-batch calls F from
+    its own host thread; F holds the GIL, so evaluations of different sub-batches run one at a time while their CUDA
+    work overlaps"""
+
+    def __init__(self, nprob, n, mnl, ml, p=0, device=0, nsub=None):
+        self._mnl, self._ml = int(mnl), int(ml)
+        super().__init__(nprob, n, self._mnl + self._ml, device, nsub, None, p)
+        for ix, part in zip(self.idx, self.parts):
+            part.index = ix
+
+    def _part(self):
+        return lambda nprob, n, m, device, dims, p=0: CPBatch(nprob, n, self._mnl, self._ml, p, device)
+
+    def set_F(self, F):
+        for part in self.parts:
+            part.set_F(F)
+
+    def load(self, x0, G, h, A=None, b=None):
+        self._load_sliced((x0, G, h), A, b)
+
+    def stats(self):
+        out = super().stats()
+        out["line_search_rounds"] = max(b._lib.cvxb_batch_ls_rounds(b._h) for b in self.parts)
+        return out
+
+
+def _cp_args(F, G, h, dims, A, b):
+    """cp's argument checks (cvxprog.py:1653-1728) on the batch -> mnl, x0, G, h, A, b with the defaults filled in"""
+    try:
+        mnl, x0 = F()
+    except Exception:
+        raise ValueError("function call 'F()' failed") from None
+    if type(mnl) is not int or mnl < 0:
+        raise TypeError("the first output of F() must be a nonnegative integer")
+    if hasattr(x0, "detach"):
+        x0 = x0.detach().cpu().numpy()
+    x0 = np.asarray(x0)
+    if x0.ndim != 2 or x0.dtype != np.float64:
+        raise TypeError("'x0' must be a 'd' matrix with one column: a float64 array of shape (B, n)")
+    B, n = x0.shape
+    if dims is not None and (dims.get("q") or dims.get("s")):
+        raise NotImplementedError("the CP batch takes 'l' inequalities only (dims without 'q' and 's' cones)")
+    h = np.zeros((B, 0)) if h is None else np.asarray(h)
+    if h.ndim != 2 or h.shape[0] != B or h.dtype.kind != "f":
+        raise TypeError("'h' must be a 'd' matrix with one column")
+    ml = h.shape[1] if not dims else int(dims.get("l", 0))
+    if h.shape[1] != ml:
+        raise TypeError("'h' must be a 'd' matrix of size (%d,1)" % ml)
+    G = np.zeros((B, 0, n)) if G is None else np.asarray(G)
+    if G.shape != (B, ml, n) or G.dtype.kind != "f":
+        raise TypeError("'G' must be a 'd' matrix with size (%d, %d)" % (ml, n))
+    A = np.zeros((B, 0, n)) if A is None else np.asarray(A)
+    if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n or A.dtype.kind != "f":
+        raise TypeError("'A' must be a 'd' matrix with %d columns" % n)
+    p = A.shape[1]
+    b = np.zeros((B, 0)) if b is None else np.asarray(b)
+    if b.ndim != 2 or b.shape[0] != B or b.dtype.kind != "f":
+        raise TypeError("'b' must be a 'd' matrix with one column")
+    if b.shape[1] != p:
+        raise TypeError("'b' must have length %d" % p)
+    if p > n:
+        raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
+    return mnl, x0, G, h, A, b
+
+
+def cp_batch(F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent smooth convex programs on one GPU, each as solvers.cp(F, G, h, dims, A, b) does:
+    minimize f0(x) s.t. fk(x) <= 0 (k = 1..mnl), G x <= h, A x = b.  F is batched, with float64 torch tensors on the
+    device:
+      F() -> (mnl, x0): mnl shared by the batch, x0 (B, n) strictly inside dom f (numpy array or tensor), called once;
+      F(x, idx=idx) -> (f, Df): x (k, n) the points of k problems, idx (k,) int64 their indices in x0's order,
+          f (k, mnl + 1), Df (k, mnl + 1, n).  A row of f with a NaN or an infinite entry means x is not in dom f;
+          F must accept such points without raising;
+      F(x, z, idx=idx) -> (f, Df, H): z (k, mnl + 1), H (k, n, n) = sum_i z_i grad² f_i(x), only its lower triangle
+          read.
+    F runs on the batch's CUDA stream and must return the same values for the same point.  G (B, ml, n), h (B, ml),
+    A (B, p, n), b (B, p) are optional; dims, if given, is {'l': ml}.  Returns cp's x, snl, sl, znl, zl, y, status
+    ('optimal' or 'unknown'), iterations, primal objective and dual objective, with the batch's stats (solve_ms,
+    lock-step iterations, line-search rounds, nsub, solve_wall_ms).  nsub is qp_batch's.
+    options: maxiters, abstol, reltol, feastol, refinement (as cp's)."""
+    mnl, x0, G, h, A, b = _cp_args(F, G, h, dims, A, b)
+    B, n, p = x0.shape[0], x0.shape[1], A.shape[1]
+    grp = CPBatchGroup(B, n, mnl, G.shape[1], p, device, nsub)
+    try:
+        grp.set_F(F)
+    except BaseException:
+        grp.close()
+        raise
+    out = _run_group(grp, (x0, G, h, A if p else None, b if p else None), options)
+    for key in ("s", "z"):
+        v = out.pop(key)
+        out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]
+    return out
+
+
 def _run_group(grp, data, options, start=None):
     """load `data` (and a start dict of load_start's keys) into the batch group, solve it timed, and return its results
     and stats; the group is closed"""

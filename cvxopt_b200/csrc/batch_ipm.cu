@@ -1788,6 +1788,96 @@ __global__ void k_gp_update(Ptrs p, GPPtrs g) {
     gap = block_sum(gap, sh);
     if (tid == 0) S.gap = gap;
 }
+
+// ---- convex programs: cvxprog.cp (:1359-1964) with the caller's F ----
+// A CP batch is a GP batch without F (sum K = 0, nK = mnl + 1): the same epigraph problem, GPScal, state row and
+// kernels, with f, Df and H written by the caller's callback (cvxb_cp_eval_fn) into per-slot buffers that the kernels
+// below take into fv, gf0, G's rows [0, mnl) and P, where k_gp_eval writes them for a GP
+struct CPPtrs {
+    double *f, *Df, *H, *z;          // the callback's buffers, row-major per slot: nK, nK x n, n x n, nK
+    const int *idx;                  // slot -> load index (the callback's `problem`)
+    int *bad;                        // the smallest load index whose f at its iterate was not finite
+    double *P;                       // the batch's P, ld ldp
+    long long ldp, sP;
+};
+// Df'[z0; z[:mnl]] at column j of the slot's Df (nK x n, row-major)
+__device__ __forceinline__ double cp_dfz(const double *Df, int n, int nK, double z0, const double *z, int j) {
+    double a = z0 * Df[j];
+    for (int i = 1; i < nK; ++i) a += z[i - 1] * Df[(long long)i * n + j];
+    return a;
+}
+// the z of a full evaluation, [z0; z[:mnl]], for every active slot
+__global__ void k_cp_zpack(Ptrs p, GPPtrs g, CPPtrs c) {
+    GP_SETUP
+    double *zc = c.z + (long long)b * g.nK;
+    for (int i = tid; i < g.nK; i += nt) zc[i] = i == 0 ? T.z0 : p.z[om + i - 1];
+}
+// the callback's F at slot b's iterate (FULL) or trial point: f into fv.  FULL: a non-finite f recorded in bad,
+// Df[0] into gf0, Df[1:] into G's rows [0, mnl) and H's lower triangle into P's, by 32 x 32 tiles through shared
+// memory (H row-major, P column-major).  Trial, only the problems still searching: newrx's nonlinear part
+// Df'[nz0; nz[:mnl]] into nrx (the GEMVs add G'newzl + A'newy).  256 threads
+template <bool FULL> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GPPtrs g, CPPtrs c) {
+    GP_SETUP
+    if (S.done || (!FULL && T.searching == 0.0)) return;
+    const int n = p.n, nK = g.nK;
+    const double *f = c.f + (long long)b * nK, *Df = c.Df + (long long)b * nK * n;
+    for (int i = tid; i < nK; i += nt) g.fv[(long long)b * nK + i] = f[i];
+    if (!FULL) {
+        for (int j = tid; j < n; j += nt) g.nrx[on + j] = cp_dfz(Df, n, nK, T.nz0, g.nz + om, j);
+        return;
+    }
+    if (tid == 0) {
+        bool fin = true;
+        for (int i = 0; i < nK; ++i) fin = fin && isfinite(f[i]);
+        if (!fin) atomicMin(c.bad, c.idx[b]);
+    }
+    for (int j = tid; j < n; j += nt) g.gf0[on + j] = Df[j];
+    double *G = g.G + (long long)b * g.sG;
+    for (long long e = tid; e < (long long)g.mnl * n; e += nt) {
+        const long long i = e % g.mnl, j = e / g.mnl;
+        G[i + j * g.ldg] = Df[(i + 1) * n + j];
+    }
+    __shared__ double tile[32][33];
+    const double *H = c.H + (long long)b * n * n;
+    double *P = c.P + (long long)b * c.sP;
+    const int tx = tid & 31, ty = tid >> 5, nb = (n + 31) / 32;
+    for (int bj = 0; bj < nb; ++bj)
+        for (int bi = bj; bi < nb; ++bi) {
+            __syncthreads();
+            for (int r = ty; r < 32; r += 8) {                 // rows of H, coalesced along them
+                const int i = bi * 32 + r, j = bj * 32 + tx;
+                if (i < n && j < n) tile[r][tx] = H[(long long)i * n + j];
+            }
+            __syncthreads();
+            for (int q = ty; q < 32; q += 8) {                 // columns of P, coalesced down them
+                const int i = bi * 32 + tx, j = bj * 32 + q;
+                if (i < n && i >= j) P[i + (long long)j * c.ldp] = tile[tx][q];
+            }
+        }
+}
+// rx += Df'[z0; z[:mnl]] at the iterates, from the callback's Df (after k_gp_res_begin; the GEMVs add G'zl + A'y)
+__global__ void k_cp_rx(Ptrs p, GPPtrs g, CPPtrs c) {
+    GP_SETUP
+    if (S.done) return;
+    const double *Df = c.Df + (long long)b * g.nK * p.n;
+    for (int j = tid; j < p.n; j += nt) p.rx[on + j] += cp_dfz(Df, p.n, g.nK, T.z0, p.z + om, j);
+}
+// a domain round's decision (:1052-1062) once the callback has evaluated F at the trial points x + step dx: a problem
+// still searching whose f has a non-finite entry halves its step and counts itself in nsearch; a step that underflows
+// to 0 ends the problem 'unknown' (status 3) on its iterate, as in k_gp_ls.  32 threads
+__global__ void k_cp_dom(Ptrs p, GPPtrs g, CPPtrs c, int iter, int *nsearch) {
+    GP_SETUP
+    if (S.done || T.searching == 0.0) return;
+    const double *f = c.f + (long long)b * g.nK;
+    bool fin = true;
+    for (int i = tid; i < g.nK; i += nt) fin = fin && isfinite(f[i]);
+    fin = __all_sync(0xffffffffu, fin);
+    if (tid == 0 && !fin) {
+        S.step *= GP_BETA;
+        if (S.step == 0.0) { T.searching = 0.0; S.done = 1; S.status = 3; S.iters = iter; }
+        else atomicAdd(nsearch, 1);
+    }
+}
 }  // namespace
 
 struct cvxb_batch {
@@ -1851,6 +1941,14 @@ struct cvxb_batch {
     GPPtrs gq{};
     DevBuf<double> gpv, gph, gpg;
     DevBuf<int> koff;
+    // convex programs (cvxb_batch_create_cp): gq of a GP batch without F (sum K = 0, nK = mnl + 1); the callback's
+    // buffers in cpv, x0 in problem order in cpx0, slot -> load index and the non-finite flag in cpi
+    bool cp = false;
+    CPPtrs cq{};
+    DevBuf<double> cpv, cpx0;
+    DevBuf<int> cpi;
+    cvxb_cp_eval_fn cfn = nullptr;
+    void *cctx = nullptr;
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -1870,7 +1968,7 @@ int state_alloc(cvxb_batch *b) {
     const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
     // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m)
-    const long long gpl = b->gp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
+    const long long gpl = b->gp || b->cp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
     const long long L = cone + sb + ref + lps + gpl;
     if (b->L == L) return 0;
     b->L = p.L = 0;
@@ -2138,8 +2236,8 @@ template <bool EQ> int start_check(cvxb_batch *b) {
     for (int i = 0; i < B; ++i)
         if (info[i] > 0 || (EQ && infop[i] > 0)) {
             const int k = b->perm[i];
-            if (b->gp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (singular KKT "
-                                 "matrix at the start)", k);
+            if (b->gp || b->cp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n "
+                                          "(singular KKT matrix at the start)", k);
             else if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
                                  "the start)", k);
             else if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
@@ -2326,12 +2424,17 @@ int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) 
     count_launch();
     return 0;
 }
-// r += F' w + G' zl (+ A' y): Df' znl + G' zl + A' y with Df' znl = F'(z_i y) (slot k's z at z + k*m)
-template <bool EQ> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r) {
+// r += Df'[z0; znl] + G' zl (+ A' y) (slot k's z at z + k*m).  GP: Df'[z0; znl] = F'(z_i y) from k_gp_eval's
+// weights.  CP: at the iterates (full) k_cp_rx adds it; at trial points k_cp_take<false> has written it into r
+template <bool EQ> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
-    GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
-    CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
+    if (!b->cp) {
+        GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
+        CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
+    } else if (full) {
+        k_cp_rx<<<B, 256, 0, b->st>>>(b->p, g, b->cq); count_launch();
+    }
     if (ml > 0) {
         GemvBatch gl; gl.batch = B; gl.sA = g.sG; gl.sx = m; gl.sy = n;
         CVXB_TRY(gemv_t(ml, n, g.G + g.mnl, g.ldg, nullptr, z + g.mnl, 1.0, 1.0, r, b->st, gl));
@@ -2362,6 +2465,54 @@ int gp_hessian(cvxb_batch *b) {
 int read_count(cvxb_batch *b, int &v) {
     CVXB_CUDA(cudaMemcpyAsync(&v, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
+    return 0;
+}
+// the caller's F over the active slots at x (slot k at x + k*n); full: at the iterates, with z = [z0; z[:mnl]] and H
+int cp_call(cvxb_batch *b, const double *x, bool full) {
+    const CPPtrs &c = b->cq;
+    const int rc = b->cfn(b->cctx, b->Bact, full ? 1 : 0, x, full ? c.z : nullptr, c.idx, c.f, c.Df,
+                          full ? c.H : nullptr, (void *)b->st);
+    if (rc != 0) { set_error("batch_solve: the evaluation callback returned %d", rc); return CVXB_E_ARG; }
+    return 0;
+}
+// F(x, z[:mnl]) at the iterates: f into fv, grad f0 into gf0, Df[1:] into G's rows [0, mnl); CP also H into P
+// (GP forms H in gp_hessian)
+int cpl_eval_full(cvxb_batch *b) {
+    if (!b->cp) return gp_eval(b, b->p.x, b->n, true, 0);
+    const int B = b->Bact;
+    k_cp_zpack<<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    CVXB_TRY(cp_call(b, b->p.x, true));
+    k_cp_take<true><<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, B, b->sP, b->st));
+    return 0;
+}
+// F at the line search's trial points g.nx, for the problems still searching: f into fv; CP also newrx's nonlinear
+// part into nrx
+int cpl_eval_trial(cvxb_batch *b) {
+    if (!b->cp) return gp_eval(b, b->gq.nx, b->n, false, 1);
+    CVXB_TRY(cp_call(b, b->gq.nx, false));
+    k_cp_take<false><<<b->Bact, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    return 0;
+}
+// slot -> load index for the callback, after a solve's start or a compaction
+int cp_upload_idx(cvxb_batch *b) {
+    CVXB_CUDA(cudaMemcpyAsync(b->cpi.p, b->perm.data(), (size_t)b->Bact * sizeof(int), cudaMemcpyHostToDevice, b->st));
+    return 0;
+}
+// cp's backtracking into dom f after the i-th direction (:1052-1060): each round evaluates F at every searching
+// problem's x + step dx (k_gp_trial) and halves the step of those whose f is not finite; one readback per round.
+// dom f is convex, so the merit line search's shorter steps stay inside it
+int cp_domain(cvxb_batch *b, int it) {
+    cudaStream_t st = b->st;
+    const int B = b->Bact;
+    for (int left = 1; left > 0; b->ls_rounds++) {
+        k_gp_trial<<<B, 256, 0, st>>>(b->p, b->gq); count_launch();
+        CVXB_TRY(cp_call(b, b->gq.nx, false));
+        CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
+        k_cp_dom<<<B, 32, 0, st>>>(b->p, b->gq, b->cq, it, b->d_ndone.p); count_launch();
+        CVXB_LAUNCH_CHECK();
+        CVXB_TRY(read_count(b, left));
+    }
     return 0;
 }
 // the i-th Newton direction of cpl (:966-1045): right-hand side, kktsolver_e's solve and `refinement` steps from
@@ -2406,13 +2557,13 @@ template <bool EQ> int gp_direction(cvxb_batch *b, int i) {
 // searching problem's trial point and takes its decision; one readback of the count still searching per round
 template <bool EQ> int gp_line_search(cvxb_batch *b, int i, int it) {
     cudaStream_t st = b->st;
-    const int n = b->n, B = b->Bact, T = 256;
+    const int B = b->Bact, T = 256;
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     for (int left = 1; left > 0; b->ls_rounds++) {
         k_gp_trial<<<B, T, 0, st>>>(p, g); count_launch();
-        CVXB_TRY(gp_eval(b, g.nx, n, false, 1));
-        CVXB_TRY(gp_rx<EQ>(b, g.nz, g.ny, g.nrx));
+        CVXB_TRY(cpl_eval_trial(b));
+        CVXB_TRY(gp_rx<EQ>(b, g.nz, g.ny, g.nrx, false));
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
         k_gp_ls<EQ><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p); count_launch();
         CVXB_LAUNCH_CHECK();
@@ -2420,12 +2571,15 @@ template <bool EQ> int gp_line_search(cvxb_batch *b, int i, int it) {
     }
     return 0;
 }
-// H into P and K = H + [Df[1:]; G]' diag(di²) [Df[1:]; G] (+ A'A) factored, from F(x) at the slots' iterates
-int gp_factor(cvxb_batch *b, bool first) {
-    CVXB_TRY(gp_hessian(b));
+// K = H + [Df[1:]; G]' diag(di²) [Df[1:]; G] (+ A'A) factored from F(x) at the slots' iterates (a GP's H formed
+// into P first; a CP's is there from cpl_eval_full)
+int cpl_factor(cvxb_batch *b, bool first) {
+    if (!b->cp) CVXB_TRY(gp_hessian(b));
     return batch_factor(b, !first);
 }
-template <bool EQ> int solve_gp(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+// the lock-step cpl of a GP or CP batch's epigraph problem.  A CP batch starts from its x0 and backtracks each step
+// into dom f before the line search; it calls back to the host, so the loop is never captured into a graph
+template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
@@ -2437,17 +2591,23 @@ template <bool EQ> int solve_gp(cvxb_batch *b, int maxiters, double abstol, doub
     b->ls_rounds = 0;
     CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
     CVXB_CUDA(cudaEventRecord(b->e0, st));
-    // every problem in its own slot (restore_order ran): g into the state row
-    CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
-                                g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
+    // every problem in its own slot (restore_order ran): g into the state row, or x0 into x
+    if (!b->cp)
+        CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
+                                    g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
     k_gp_init<<<B, T, 0, st>>>(p, g); count_launch();
+    if (b->cp) {
+        CVXB_CUDA(cudaMemcpyAsync(p.x, b->cpx0.p, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        CVXB_TRY(cp_upload_idx(b));
+        CVXB_CUDA(cudaMemsetAsync(b->cq.bad, 0x7f, sizeof(int), st));
+    }
     std::vector<int> flags(B), pairs;
     int it = 0;
     for (it = 0; it <= maxiters; ++it) {
         // F(x, z[:mnl]) and the residuals (:627-691)
-        CVXB_TRY(gp_eval(b, p.x, n, true, 0));
+        CVXB_TRY(cpl_eval_full(b));
         k_gp_res_begin<EQ><<<B, T, 0, st>>>(p, g); count_launch();
-        CVXB_TRY(gp_rx<EQ>(b, p.z, p.y, p.rx));
+        CVXB_TRY(gp_rx<EQ>(b, p.z, p.y, p.rx, true));
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = pq;
             CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, ga));
@@ -2459,34 +2619,44 @@ template <bool EQ> int solve_gp(cvxb_batch *b, int maxiters, double abstol, doub
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
         k_gp_stats<EQ><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
-        int ndone = 0;
+        int ndone = 0, bad = 0;
         CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
+        if (b->cp) CVXB_CUDA(cudaMemcpyAsync(&bad, b->cq.bad, sizeof(int), cudaMemcpyDeviceToHost, st));
         CVXB_TRY(read_count(b, ndone));
+        if (b->cp && bad < b->B) {       // the reference keeps its iterates inside dom f
+            if (it == 0) set_error("batch_solve: problem %d: x0 not in the domain of f", bad);
+            else set_error("batch_solve: problem %d: f is not finite at the iterate of iteration %d", bad, it);
+            return CVXB_E_ARG;
+        }
         if (ndone >= B) break;
         if (ndone > 0 && b->compact && b->B > 1) {
             CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
             B = b->Bact;
-            if (!pairs.empty()) CVXB_TRY(gp_eval(b, p.x, n, true, 0));    // F(x)'s per-slot results stay put
+            if (!pairs.empty()) {        // F(x)'s per-slot results stay put
+                if (b->cp) CVXB_TRY(cp_upload_idx(b));
+                CVXB_TRY(cpl_eval_full(b));
+            }
         }
         k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0); count_launch();
         if (it == 0) {                   // kkt_chol2's first call; still singular: the Rank ValueError (:778-783)
-            CVXB_TRY(gp_factor(b, true));
+            CVXB_TRY(cpl_factor(b, true));
             CVXB_TRY(first_switch<EQ>(b));
             CVXB_TRY(start_check<EQ>(b));
         } else {
-            CVXB_TRY(gp_factor(b, false));
+            CVXB_TRY(cpl_factor(b, false));
             CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
             k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p); count_launch();
             int nre = 0;
             CVXB_TRY(read_count(b, nre));
             if (nre > 0) {               // restored problems are factored again at their saved iterates
-                CVXB_TRY(gp_eval(b, p.x, n, true, 0));
-                CVXB_TRY(gp_factor(b, false));
+                CVXB_TRY(cpl_eval_full(b));
+                CVXB_TRY(cpl_factor(b, false));
                 k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p); count_launch();
             }
         }
         for (int i = 0; i < 2; ++i) {
             CVXB_TRY(gp_direction<EQ>(b, i));
+            if (b->cp) CVXB_TRY(cp_domain(b, it));
             CVXB_TRY(gp_line_search<EQ>(b, i, it));
         }
         k_gp_update<<<B, T, 0, st>>>(p, g); count_launch();
@@ -2712,6 +2882,51 @@ int load_common(cvxb_batch *b, const double *q, const double *G, const double *h
     return 0;
 }
 
+// the common part of a GP and a CP batch (cpl on cp's epigraph problem): a QP batch with m = mnl + ml 'l' rows, nK =
+// mnl + 1 nonlinear rows with sumK rows of F below the m rows of G, and gq's per-slot vectors
+int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int nK, long long sumK, int ml, int p, int device) {
+    const int mnl = nK - 1;
+    cvxb_dims d{};
+    d.ml = mnl + ml;
+    cvxb_batch *raw = nullptr;
+    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, false, (int)sumK));
+    b.reset(raw);
+    const size_t B = nprob, m = b->m;
+    GPPtrs &g = b->gq;
+    g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
+    g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
+    // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
+    const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * m;
+    CVXB_TRY(b->gpv.alloc(B * len));
+    CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
+    double *v = b->gpv.p;
+    auto take = [&](size_t l) { double *r = v; v += B * l; return r; };
+    g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
+    g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
+    g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
+    return 0;
+}
+
+// the rows of a GP or CP batch after its own data: G below the mnl rows of Df[1:], h in the 'l' rows (0 on the
+// nonlinear ones), q (c's x part) 0; then a fresh batch
+int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyKind kind) {
+    const size_t B = b->B, n = b->n, m = b->m, mnl = b->gq.mnl, ml = m - mnl;
+    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->h), 0, B * (m ? m : 1) * sizeof(double), b->st));
+    if (ml > 0) {
+        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + mnl, b->ldg * sizeof(double), G, ml * sizeof(double),
+                                    ml * sizeof(double), n * B, kind, b->st));
+        CVXB_CUDA(cudaMemcpy2DAsync(const_cast<double *>(b->h) + mnl, m * sizeof(double), h, ml * sizeof(double),
+                                    ml * sizeof(double), B, kind, b->st));
+    }
+    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    b->eq_loaded = false;
+    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
+    b->permuted = false;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2755,16 +2970,10 @@ int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *
         sumK += K[i];
     }
     if (sumK + nK + ml > (1LL << 30)) { set_error("batch_create_gp: too many rows"); return CVXB_E_ARG; }
-    const int mnl = nK - 1;
-    cvxb_dims d{};
-    d.ml = mnl + ml;
-    cvxb_batch *raw = nullptr;
-    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, false, (int)sumK));
-    std::unique_ptr<cvxb_batch> b(raw);
-    const size_t B = nprob, m = b->m;
+    std::unique_ptr<cvxb_batch> b;
+    CVXB_TRY(create_cpl(b, nprob, n, nK, sumK, ml, p, device));
+    const size_t B = nprob;
     GPPtrs &g = b->gq;
-    g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
-    g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
     g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
     std::vector<int> off(nK + 1, 0);
     for (int i = 0; i < nK; ++i) off[i + 1] = off[i] + K[i];
@@ -2773,27 +2982,58 @@ int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *
     g.koff = b->koff.p;
     CVXB_TRY(b->gph.alloc(B * g.sH));
     CVXB_TRY(b->gpg.alloc(B * sumK));
-    // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
-    const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * m;
-    CVXB_TRY(b->gpv.alloc(B * len));
-    CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
-    double *v = b->gpv.p;
-    auto take = [&](size_t l) { double *r = v; v += B * l; return r; };
     g.Hr = b->gph.p;
-    g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
-    g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
-    g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
     b->gp = true;
-    b->p.refinement = m > 0 ? 1 : 0;                  // cpl's default (cvxprog.py:422)
+    b->p.refinement = b->m > 0 ? 1 : 0;               // cpl's default (cvxprog.py:422)
     CVXB_TRY(state_alloc(b.get()));
     *out = b.release();
+    return 0;
+}
+
+int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, int p, int device) {
+    if (out) *out = nullptr;
+    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || ml < 0 || p < 0) {
+        set_error("batch_create_cp: bad sizes (nprob in 1..%d, n >= 1, mnl, ml and p nonnegative)", CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (p > n) {                                      // cp's check before the first factorisation
+        set_error("batch_create_cp: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", p, n);
+        return CVXB_E_ARG;
+    }
+    if ((long long)mnl + ml + 1 > (1LL << 30)) { set_error("batch_create_cp: too many rows"); return CVXB_E_ARG; }
+    std::unique_ptr<cvxb_batch> b;
+    CVXB_TRY(create_cpl(b, nprob, n, mnl + 1, 0, ml, p, device));
+    const size_t B = nprob, nK = mnl + 1, nn = n;
+    // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
+    const size_t len = 2 * nK + nK * nn + nn * nn;
+    CVXB_TRY(b->cpv.alloc(B * len));
+    CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
+    CVXB_TRY(b->cpx0.alloc(B * nn));
+    CVXB_TRY(b->cpi.alloc(B + 1));
+    CPPtrs &c = b->cq;
+    c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
+    c.idx = b->cpi.p; c.bad = b->cpi.p + B;
+    c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
+    b->cp = true;
+    b->p.refinement = 1;                              // cpl's default (cvxprog.py:422); the epigraph row is always there
+    CVXB_TRY(state_alloc(b.get()));
+    *out = b.release();
+    return 0;
+}
+
+int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx) {
+    if (!b) { set_error("batch_set_cp_eval: batch is NULL"); return CVXB_E_ARG; }
+    if (!b->cp) { set_error("batch_set_cp_eval: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
+    b->cfn = fn;
+    b->cctx = ctx;
     return 0;
 }
 
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
-    b->p.refinement = b->m > 0 ? refinement : 0;     // a batch without constraint rows takes unrefined steps
+    // a batch without constraint rows takes unrefined steps; a CP batch always has cp's epigraph row
+    b->p.refinement = b->m > 0 || b->cp ? refinement : 0;
     CVXB_TRY(state_alloc(b));
     return 0;
 }
@@ -2810,6 +3050,7 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
     if (b->lp) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
     if (b->gp) { set_error("batch_load: a GP batch is loaded with cvxb_batch_load_gp"); return CVXB_E_ARG; }
+    if (b->cp) { set_error("batch_load: a CP batch is loaded with cvxb_batch_load_cp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t n = b->n;
@@ -2822,7 +3063,7 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
 
 int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space) {
     if (!b || !c || !G || !h) { set_error("batch_load_lp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->lp) { set_error("batch_load_lp: a QP or GP batch is not a cone LP batch"); return CVXB_E_ARG; }
+    if (!b->lp) { set_error("batch_load_lp: a QP, GP or CP batch is not a cone LP batch"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     return load_common(b, c, G, h, (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
 }
@@ -2832,25 +3073,21 @@ int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const do
     if (!b->gp) { set_error("batch_load_gp: not a GP batch (cvxb_batch_create_gp)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const size_t B = b->B, n = b->n, m = b->m, mnl = b->gq.mnl, ml = m - mnl, sK = b->gq.sumK;
-    // F below the m rows of [Df[1:]; G], G below the mnl rows of Df[1:], h in the 'l' rows; q (c's x part) is 0
+    const size_t B = b->B, n = b->n, m = b->m, sK = b->gq.sumK;
+    // F below the m rows of [Df[1:]; G]
     CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + m, b->ldg * sizeof(double), F, sK * sizeof(double), sK * sizeof(double),
                                 n * B, kind, b->st));
     CVXB_CUDA(cudaMemcpyAsync(b->gpg.p, g, B * sK * sizeof(double), kind, b->st));
-    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->h), 0, B * (m ? m : 1) * sizeof(double), b->st));
-    if (ml > 0) {
-        CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + mnl, b->ldg * sizeof(double), G, ml * sizeof(double),
-                                    ml * sizeof(double), n * B, kind, b->st));
-        CVXB_CUDA(cudaMemcpy2DAsync(const_cast<double *>(b->h) + mnl, m * sizeof(double), h, ml * sizeof(double),
-                                    ml * sizeof(double), B, kind, b->st));
-    }
-    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    b->eq_loaded = false;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
-    return 0;
+    return load_cpl_common(b, G, h, kind);
+}
+
+int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const double *h, int space) {
+    if (!b || !x0 || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_cp: NULL argument"); return CVXB_E_ARG; }
+    if (!b->cp) { set_error("batch_load_cp: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, (size_t)b->B * b->n * sizeof(double), kind, b->st));
+    return load_cpl_common(b, G, h, kind);
 }
 
 int cvxb_batch_ls_rounds(cvxb_batch *b) { return b ? b->ls_rounds : CVXB_E_ARG; }
@@ -2876,6 +3113,7 @@ int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const
                           int space) {
     if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
     if (b->gp) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
+    if (b->cp) { set_error("batch_load_start: cp starts from the x0 of cvxb_batch_load_cp"); return CVXB_E_ARG; }
     if (b->lp && ((!x) != (!s) || (y && !z) || (!x && !z))) {
         set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
                   "both");
@@ -2913,8 +3151,9 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     }
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
-    if (b->gp) return b->neq > 0 ? solve_gp<true>(b, maxiters, abstol, reltol, feastol)
-                                 : solve_gp<false>(b, maxiters, abstol, reltol, feastol);
+    if (b->cp && !b->cfn) { set_error("batch_solve: a CP batch needs its F (cvxb_batch_set_cp_eval)"); return CVXB_E_ARG; }
+    if (b->gp || b->cp) return b->neq > 0 ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
+                                          : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
     using Solve = int (*)(cvxb_batch *, int, double, double, double);
     static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
                                      solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,

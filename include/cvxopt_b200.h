@@ -412,9 +412,48 @@ int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *
 /* GP batch only: F nprob x (S x n column-major, ld S), g nprob x S, G nprob x (ml x n column-major, ld ml), h
  * nprob x ml; G and h may be NULL when ml = 0.  A and b come through cvxb_batch_load_eq. */
 int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const double *G, const double *h, int space);
-/* line-search rounds of the last solve of a GP batch (every round evaluates F at every searching problem's trial
- * point); 0 for the other batches */
+/* line-search rounds of the last solve of a GP or CP batch (every round evaluates F at every searching problem's trial
+ * point; a CP batch's domain rounds count too); 0 for the other batches */
 int cvxb_batch_ls_rounds(cvxb_batch *b);
+/* batch of smooth convex programs (B x solvers.cp(F, G, h, dims={'l': ml}, A, b), cvxprog.py:1359-1964, with its
+ * default kktsolver 'chol2'):
+ *     minimize  f0(x)  s.t.  fk(x) <= 0 (k = 1..mnl),  G x <= h,  A x = b
+ * with F evaluated by the caller (cvxb_batch_set_cp_eval).  It runs the GP batch's lock-step cpl on cp's epigraph
+ * problem, starting from the loaded x0 with t = 0, y = 0 and s = z = e, and backtracks each direction's step into
+ * dom f before the line search (:1052-1060).  CVXB_E_ARG, checked before the device: nprob outside
+ * 1..CVXB_BATCH_MAX, n < 1, mnl < 0, ml < 0, p < 0, and cp's "Rank(A) < p" for p > n.  Load it with
+ * cvxb_batch_load_cp (and cvxb_batch_load_eq when p > 0); cvxb_batch_load, load_lp, load_gp and load_start on it are
+ * CVXB_E_ARG.  Solve, set_refinement (default 1, as cpl, also when mnl + ml = 0), results, results_y, stats,
+ * ls_rounds and destroy are the GP batch's calls with its semantics: s and z are [snl; sl] and [znl; zl], the primal
+ * objective is t, status 3 is a singular KKT matrix or a step that underflowed to 0 in the domain or merit line
+ * search.  Solving without an evaluator is CVXB_E_ARG, as is a callback that returns non-zero ("the evaluation
+ * callback returned %d"), a singular KKT matrix at iteration 0 ("problem %d: Rank(A) < p or Rank([H(x); A; Df(x);
+ * G]) < n") and an f that is not finite at an iterate ("problem %d: x0 not in the domain of f" at iteration 0).
+ * The solve calls back to the host, so it must not be captured into a CUDA graph.  Device memory per problem, with
+ * m = mnl + ml, nf = mnl + 1 and ev() rounding up to even: what cvxb_batch_create_eq's batch of the same n, p and
+ * dims {'l': m} holds with refinement 1, plus nf(n + 2) + n² (the callback's f, Df, z and H), nf + 3n + p + 4m (f,
+ * grad f0, the unscaled steps and the line search's trial point), n (x0), 56 + 3 ev(n) + 3 ev(p) + 10 ev(m) in the
+ * state row (the scalars and the line search's saved state) and one int (slot -> problem); and one int shared by the
+ * batch; all of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy. */
+int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, int p, int device);
+/* CP batch only: x0 nprob x n (strictly inside dom f), G nprob x (ml x n column-major, ld ml), h nprob x ml; G and h
+ * may be NULL when ml = 0.  A and b come through cvxb_batch_load_eq. */
+int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const double *h, int space);
+/* F of a CP batch, called on the solving thread with k = the active problems (every evaluation covers all of them;
+ * rows of problems that are not searching are evaluated and ignored).  Device buffers owned by the handle, row-major
+ * per problem and problem-contiguous, nf = mnl + 1:
+ *     x        k x n            in: the points (read only)
+ *     z        k x nf           in, full evaluations only: [z0; znl] (read only)
+ *     problem  k ints           in: the load index of each row (read only)
+ *     f        k x nf           out: f(x); a row with a NaN or an infinite entry means x is not in dom f
+ *     Df       k x nf x n       out: the rows of Df(x)
+ *     H        k x n x n        out, full evaluations only: sum_i z_i grad² f_i(x), only its lower triangle is read
+ * full = 1 at the iterates, where f must be finite; full = 0 (z and H NULL) at trial points.  stream is the batch's
+ * cudaStream_t: the callback enqueues its work there and does not synchronise.  It must return 0, and the same
+ * values for the same point.  fn = NULL clears the evaluator. */
+typedef int (*cvxb_cp_eval_fn)(void *ctx, int k, int full, const double *x, const double *z, const int *problem,
+                               double *f, double *Df, double *H, void *stream);
+int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx);
 
 #ifdef __cplusplus
 }
