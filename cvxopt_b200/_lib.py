@@ -146,6 +146,9 @@ _SIGS = {
     "cvxb_batch_create_cp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "cvxb_batch_load_cp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_set_cp_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cvxb_batch_create_cpl": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                        C.c_int]),
+    "cvxb_batch_load_cpl": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_results": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
 }

@@ -743,6 +743,7 @@ class CPBatch(QPBatch):
     G and p rows of A are shared by the batch.  load() takes x0 (B, n), G (B, ml, n), h (B, ml) and, with p > 0,
     A (B, p, n), b (B, p); set_F() takes cp_batch's F.  `index` is each problem's index in the caller's order, passed to
     F as idx.  results()' s and z are [snl; sl] and [znl; zl]; its primal objective is cp's t."""
+    _epi = 1                 # rows of F's f and Df before the mnl: cp's objective (CPLBatch: none)
 
     def __init__(self, nprob, n, mnl, ml, p=0, device=0, index=None):
         self._lib = _lib.load()
@@ -750,12 +751,15 @@ class CPBatch(QPBatch):
         self.B, self.n, self.p, self.device = int(nprob), int(n), int(p), int(device)
         self.mnl, self.ml = int(mnl), int(ml)
         self.m = self.mnl + self.ml
-        rc = self._lib.cvxb_batch_create_cp(C.byref(self._h), self.B, self.n, self.mnl, self.ml, self.p, self.device)
-        _lib.check(rc, "batch")
+        self._nf = self.mnl + self._epi
+        _lib.check(self._create(), "batch")
         self._refinement = None
         self.index = np.arange(self.B) if index is None else np.asarray(index)
         self._cb = None
         self._err = None
+
+    def _create(self):
+        return self._lib.cvxb_batch_create_cp(C.byref(self._h), self.B, self.n, self.mnl, self.ml, self.p, self.device)
 
     def load(self, x0, G, h, A=None, b=None):
         B, n = self.B, self.n
@@ -776,14 +780,14 @@ class CPBatch(QPBatch):
         re-raised by solve()"""
         import torch
         dev = torch.device("cuda", self.device)
-        B, n, nf = self.B, self.n, self.mnl + 1
+        B, n, nf = self.B, self.n, self._nf
         gidx = torch.as_tensor(self.index, dtype=torch.int64, device=dev)
         views, streams = {}, {}
 
         def view(ptr, shape, typestr="<f8"):
-            t = views.get(ptr)
+            t = views.get((ptr, shape))
             if t is None:
-                t = views[ptr] = torch.as_tensor(_DevArray(ptr, (B,) + shape, typestr), device=dev)
+                t = views[ptr, shape] = torch.as_tensor(_DevArray(ptr, (B,) + shape, typestr), device=dev)
             return t
 
         def check(v, shape, which, rows, cols):
@@ -801,11 +805,15 @@ class CPBatch(QPBatch):
                 with torch.cuda.device(dev), torch.cuda.stream(st):
                     idx = gidx[view(problem, (), "<i4")[:k].long()]
                     X = view(x, (n,))[:k]
-                    out = F(X, view(z, (nf,))[:k], idx=idx) if full else F(X, idx=idx)
+                    Z = (view(z, (nf,))[:k] if nf else X.new_zeros((k, 0))) if full else None
+                    out = F(X, Z, idx=idx) if full else F(X, idx=idx)
                     if not isinstance(out, (tuple, list)) or len(out) != (3 if full else 2):
                         raise TypeError("F(x, z) must return (f, Df, H)" if full else "F(x) must return (f, Df)")
-                    view(f, (nf,))[:k].copy_(check(out[0], (k, nf), "first", nf, 1))
-                    view(Df, (nf, n))[:k].copy_(check(out[1], (k, nf, n), "second", nf, n))
+                    fv = check(out[0], (k, nf), "first", nf, 1)
+                    Dfv = check(out[1], (k, nf, n), "second", nf, n)
+                    if nf:
+                        view(f, (nf,))[:k].copy_(fv)
+                        view(Df, (nf, n))[:k].copy_(Dfv)
                     if full:
                         view(H, (n, n))[:k].copy_(check(out[2], (k, n, n), "third", n, n))
                 return 0
@@ -931,6 +939,143 @@ def cp_batch(F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, 
         grp.close()
         raise
     out = _run_group(grp, (x0, G, h, A if p else None, b if p else None), options)
+    for key in ("s", "z"):
+        v = out.pop(key)
+        out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]
+    return out
+
+
+class CPLBatch(CPBatch):
+    """B cpl problems (cvxb_batch_create_cpl): B x solvers.cpl(c, F, G, h, dims, A, b) with 'l' and 'q' cones, the CP
+    batch's lock-step cpl without the epigraph row.  mnl, dims and p are shared by the batch.  load() takes c (B, n),
+    x0 (B, n), G (B, cdim, n), h (B, cdim) and, with p > 0, A (B, p, n), b (B, p); set_F() takes cpl_batch's F.
+    results()' s and z are [snl; sl] and [znl; zl], the 'q' rows in sl and zl; its primal objective is c'x."""
+
+    _epi = 0
+
+    def __init__(self, nprob, n, mnl, dims, p=0, device=0, index=None):
+        self._dims = _batch_dims(dims or {"l": 0})      # (ctypes dims, keep-alive, cdim)
+        super().__init__(nprob, n, mnl, self._dims[2], p, device, index)      # ml: the rows of G and h
+
+    def _create(self):
+        return self._lib.cvxb_batch_create_cpl(C.byref(self._h), self.B, self.n, self.mnl, C.byref(self._dims[0]),
+                                               self.p, self.device)
+
+    def load(self, c, x0, G, h, A=None, b=None):
+        B, n, cd = self.B, self.n, self.ml
+        c = np.ascontiguousarray(np.asarray(c, dtype=np.float64))
+        x0 = np.ascontiguousarray(np.asarray(x0, dtype=np.float64))
+        G = np.zeros((B, 0, n)) if G is None else np.asarray(G, dtype=np.float64)
+        h = np.zeros((B, 0)) if h is None else np.ascontiguousarray(np.asarray(h, dtype=np.float64))
+        if c.shape != (B, n) or x0.shape != (B, n) or G.shape != (B, cd, n) or h.shape != (B, cd):
+            raise TypeError("problem shapes do not match the batch")
+        Acm, bv = self._host_eq(A, b)
+        Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
+        _lib.check(self._lib.cvxb_batch_load_cpl(self._h, c.ctypes.data, x0.ctypes.data,
+                                                 Gcm.ctypes.data if cd else None, h.ctypes.data if cd else None,
+                                                 _lib.HOST), "batch_load_cpl")
+        self._load_eq(Acm, bv, _lib.HOST)
+
+
+class CPLBatchGroup(CPBatchGroup):
+    """CPBatchGroup for cpl problems: interleaved CPLBatch sub-batches solved concurrently, F called with each
+    sub-batch's idx"""
+
+    def __init__(self, nprob, n, mnl, dims, p=0, device=0, nsub=None):
+        self._dims = dims
+        cdim = _batch_dims(dims or {"l": 0})[2]
+        super().__init__(nprob, n, mnl, cdim, p, device, nsub)
+
+    def _part(self):
+        return lambda nprob, n, m, device, dims, p=0: CPLBatch(nprob, n, self._mnl, self._dims, p, device)
+
+    def load(self, c, x0, G, h, A=None, b=None):
+        self._load_sliced((c, x0, G, h), A, b)
+
+
+def _cpl_args(c, F, G, h, dims, A, b):
+    """cpl's argument checks (cvxprog.py:426-530) on the batch -> mnl, c, x0, G, h, dims, A, b with the defaults
+    filled in; 's' cones raise NotImplementedError and p > n the Rank ValueError, before anything is created.  cpl reads
+    dims['q'] and dims['s'] (a missing key is its KeyError, :427, :472) and does not check their entries, which the
+    batch needs: those are checked with coneprog's TypeErrors (coneprog.py:493-500)"""
+    for key in ("q", "s"):
+        if dims and key not in dims:
+            raise KeyError(key)
+    try:
+        mnl, x0 = F()
+    except Exception:
+        raise ValueError("function call 'F()' failed") from None
+    if type(mnl) is not int or mnl < 0:
+        raise TypeError("the first output of F() must be a nonnegative integer")
+    if hasattr(x0, "detach"):
+        x0 = x0.detach().cpu().numpy()
+    x0 = np.asarray(x0)
+    if x0.ndim != 2 or x0.dtype != np.float64:
+        raise TypeError("'x0' must be a 'd' matrix with one column: a float64 array of shape (B, n)")
+    B, n = x0.shape
+    if hasattr(c, "detach"):
+        c = c.detach().cpu().numpy()
+    c = np.asarray(c)
+    if c.shape != (B, n) or c.dtype != np.float64:
+        raise TypeError("'c' must be a 'd' matrix of size (%d,1)" % n)
+    h = np.zeros((B, 0)) if h is None else np.asarray(h)
+    if h.ndim != 2 or h.shape[0] != B or h.dtype.kind != "f":
+        raise TypeError("'h' must be a 'd' matrix with 1 column")
+    if not dims:
+        dims = {"l": h.shape[1], "q": [], "s": []}
+    if not isinstance(dims["l"], (int, np.integer)) or dims["l"] < 0:
+        raise TypeError("'dims['l']' must be a nonnegative integer")
+    if [k for k in dims["q"] if not isinstance(k, (int, np.integer)) or k < 1]:
+        raise TypeError("'dims['q']' must be a list of positive integers")
+    if [k for k in dims["s"] if not isinstance(k, (int, np.integer)) or k < 0]:
+        raise TypeError("'dims['s']' must be a list of nonnegative integers")
+    cdim = dims["l"] + sum(dims["q"]) + sum(k * k for k in dims["s"])
+    if h.shape[1] != cdim:
+        raise TypeError("'h' must be a 'd' matrix of size (%d,1)" % cdim)
+    G = np.zeros((B, 0, n)) if G is None else np.asarray(G)
+    if G.shape != (B, cdim, n) or G.dtype.kind != "f":
+        raise TypeError("'G' must be a 'd' matrix with size (%d, %d)" % (cdim, n))
+    A = np.zeros((B, 0, n)) if A is None else np.asarray(A)
+    if A.ndim != 3 or A.shape[0] != B or A.shape[2] != n or A.dtype.kind != "f":
+        raise TypeError("'A' must be a 'd' matrix with %d columns" % n)
+    p = A.shape[1]
+    b = np.zeros((B, 0)) if b is None else np.asarray(b)
+    if b.ndim != 2 or b.shape[0] != B or b.dtype.kind != "f":
+        raise TypeError("'b' must be a 'd' matrix with one column")
+    if b.shape[1] != p:
+        raise TypeError("'b' must have length %d" % p)
+    if dims["s"]:
+        raise NotImplementedError("the cpl batch takes 'l' and 'q' cones only (dims without 's')")
+    if p > n:
+        raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
+    if mnl + cdim == 0:
+        raise ValueError("cpl needs at least one constraint row (mnl + cdim = 0): its merit weight 1 / gap is undefined")
+    return mnl, c, x0, G, h, dims, A, b
+
+
+def cpl_batch(c, F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent convex problems with a linear objective on one GPU, each as solvers.cpl(c, F, G, h, dims,
+    A, b) does with its default kktsolver: minimize c'x s.t. fk(x) <= 0 (k = 1..mnl), G x + s = h with s in the 'l' and
+    'q' cones of dims, A x = b.  F is cp_batch's without the objective row:
+      F() -> (mnl, x0): mnl shared by the batch (0 allowed), x0 (B, n) strictly inside dom f, called once;
+      F(x, idx=idx) -> (f, Df): f (k, mnl), Df (k, mnl, n); a row of f with a NaN or an infinite entry means x is not
+          in dom f (with mnl = 0, F is still called and dom f is everything);
+      F(x, z, idx=idx) -> (f, Df, H): z (k, mnl), H (k, n, n) = sum_i z_i grad² f_i(x), only its lower triangle read
+          (zero when mnl = 0).
+    c (B, n), G (B, cdim, n), h (B, cdim), A (B, p, n), b (B, p); dims as cpl's, without 's' cones.  A nonlinear
+    objective f0 goes in as its epigraph: add a variable t, minimise t, and make f0(x) - t the first row of f.
+    Returns cpl's x, snl, sl, znl, zl, y, status, iterations, primal and dual objective, with the batch's stats
+    (solve_ms, lock-step iterations, line-search rounds, nsub, solve_wall_ms).  nsub is qp_batch's.
+    options: maxiters, abstol, reltol, feastol, refinement (as cpl's; refinement 1 by default)."""
+    mnl, c, x0, G, h, dims, A, b = _cpl_args(c, F, G, h, dims, A, b)
+    B, n, p = x0.shape[0], x0.shape[1], A.shape[1]
+    grp = CPLBatchGroup(B, n, mnl, dims, p, device, nsub)
+    try:
+        grp.set_F(F)
+    except BaseException:
+        grp.close()
+        raise
+    out = _run_group(grp, (c, x0, G, h, A if p else None, b if p else None), options)
     for key in ("s", "z"):
         v = out.pop(key)
         out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]

@@ -1354,6 +1354,12 @@ struct GPPtrs {
     // in the state row: g (sum K), GPScal, and the saved vectors
     double *g, *gs, *x0, *dx0, *rx0, *y0, *dy0, *ry0, *s0, *z0, *ds0, *dz0, *ds20, *dz20, *l0, *d0, *di0, *rz0;
 };
+// the 'q' part of W that a cpl batch's relaxed line search saves with the rest (cvxprog.py:1196-1198): v (sum q) and
+// beta (nq) in the state row.  A kernel's last argument, so that the GP and CP kernels' other arguments stay where
+// they are
+struct QSave {
+    double *v0, *beta0;
+};
 constexpr int GP_MAX_RELAXED = 8;
 constexpr double GP_ALPHA = 0.01, GP_BETA = 0.5, GP_STEP = 0.99;
 __device__ __forceinline__ GPScal &gp_scal(const GPPtrs &g, long long oc) {
@@ -1365,12 +1371,20 @@ __device__ __forceinline__ GPScal &gp_scal(const GPPtrs &g, long long oc) {
     const long long ok = (long long)b * g.sumK;                                                        \
     (void)T; (void)ok;
 
-// the starting point (:556-570): x = 0, t = 0, y = 0, s = z = e, relaxed_iters = 0
-__global__ void k_gp_init(Ptrs p, GPPtrs g) {
+// the starting point (:556-570): x = 0, t = 0, y = 0, s = z = e, relaxed_iters = 0.  CONES: e is 1 at each cone's
+// first row and 0 in the rest of it
+template <bool CONES> __global__ void k_gp_init(Ptrs p, GPPtrs g) {
     GP_SETUP
     for (int i = tid; i < p.n; i += nt) p.x[on + i] = 0.0;
     for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = 0.0;
-    for (int i = tid; i < p.m; i += nt) { p.s[om + i] = 1.0; p.z[om + i] = 1.0; }
+    for (int i = tid; i < p.m; i += nt) {
+        const double e = !CONES || i < p.ml ? 1.0 : 0.0;
+        p.s[om + i] = e; p.z[om + i] = e;
+    }
+    if (CONES) {
+        __syncthreads();
+        for (int k = tid; k < p.nq; k += nt) { p.s[om + p.qoff[k]] = 1.0; p.z[om + p.qoff[k]] = 1.0; }
+    }
     if (tid == 0) {
         T = GPScal{};
         T.s0 = 1.0; T.z0 = 1.0;
@@ -1420,24 +1434,31 @@ template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) {
     }
 }
 // residuals, part 1 (:668-691): rx = 0 (the GEMVs add Df'znl + G'zl + A'y), rxt = 1 - z0; rz = s + f on the
-// nonlinear rows, s - h on the 'l' rows (G x follows); rznl's epigraph row s0 + f0 - t; EQ: ry = b (A x - ry follows)
-template <bool EQ> __global__ void k_gp_res_begin(Ptrs p, GPPtrs g) {
+// nonlinear rows, s - h on the 'l' rows (G x follows); rznl's epigraph row s0 + f0 - t; EQ: ry = b (A x - ry follows).
+// Without the epigraph row (EPI false, a cpl batch): rx = c, and f has no objective entry
+template <bool EQ, bool EPI = true> __global__ void k_gp_res_begin(Ptrs p, GPPtrs g) {
     GP_SETUP
     if (S.done) return;
     const double *f = g.fv + (long long)b * g.nK;
-    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = 0.0;
+    for (int i = tid; i < p.n; i += nt) p.rx[on + i] = EPI ? 0.0 : p.q[on + i];
     for (int i = tid; i < p.m; i += nt)
-        p.rz[om + i] = i < g.mnl ? p.s[om + i] + f[i + 1] : p.s[om + i] - p.h[om + i];
+        p.rz[om + i] = i < g.mnl ? p.s[om + i] + f[i + (EPI ? 1 : 0)] : p.s[om + i] - p.h[om + i];
     if (EQ) for (int i = tid; i < p.neq; i += nt) p.ry[oq + i] = p.beq[oq + i];
-    if (tid == 0) { T.rxt = -T.z0 + 1.0; T.rz0 = T.s0 + (f[0] - T.t); }
+    if (EPI && tid == 0) { T.rxt = -T.z0 + 1.0; T.rz0 = T.s0 + (f[0] - T.t); }
 }
-// statistics and stopping rule (:693-755); iteration 0 fixes resx0, resznl0, pres0, dres0 and the merit weights
-template <bool EQ> __global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int maxiters, double abstol, double reltol,
-                                              double feastol, int *ndone, int *doneflags) {
+// statistics and stopping rule (:693-755); iteration 0 fixes resx0, resznl0, pres0, dres0 and the merit weights.
+// EPI false: pcost = c'x, and no epigraph row in gap, resx, resznl and dcost.  'q' rows are 'l' rows here: snrm2 and
+// sdot are the 2-norm and the dot product on them
+template <bool EQ, bool EPI = true>
+__global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int maxiters, double abstol, double reltol, double feastol,
+                           int *ndone, int *doneflags) {
     GP_SETUP
     if (!S.done) {
-        double rx2 = 0, ry2 = 0, yry = 0, rn2 = 0, rl2 = 0, zrn = 0, zrl = 0, gap = 0;
-        for (int i = tid; i < p.n; i += nt) { const double v = p.rx[on + i]; rx2 += v * v; }
+        double rx2 = 0, ry2 = 0, yry = 0, rn2 = 0, rl2 = 0, zrn = 0, zrl = 0, gap = 0, cx = 0;
+        for (int i = tid; i < p.n; i += nt) {
+            const double v = p.rx[on + i]; rx2 += v * v;
+            if (!EPI) cx += p.q[on + i] * p.x[on + i];
+        }
         if (EQ) for (int i = tid; i < p.neq; i += nt) { const double v = p.ry[oq + i]; ry2 += v * v; yry += p.y[oq + i] * v; }
         for (int i = tid; i < p.m; i += nt) {
             const double v = p.rz[om + i], zv = p.z[om + i];
@@ -1447,12 +1468,13 @@ template <bool EQ> __global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int ma
         rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh); rl2 = block_sum(rl2, sh);
         zrn = block_sum(zrn, sh); zrl = block_sum(zrl, sh); gap = block_sum(gap, sh);
         if (EQ) { ry2 = block_sum(ry2, sh); yry = block_sum(yry, sh); }
+        if (!EPI) cx = block_sum(cx, sh);
         if (tid == 0) {
-            gap += T.s0 * T.z0;
-            const double resx = sqrt(rx2 + T.rxt * T.rxt), resy = sqrt(ry2);
-            const double resznl = sqrt(rn2 + T.rz0 * T.rz0), reszl = sqrt(rl2);
-            const double pcost = T.t;                    // c'(x, t) with c = (0, 1)
-            const double dcost = pcost + yry + (zrn + T.z0 * T.rz0) + zrl - gap;
+            if (EPI) gap += T.s0 * T.z0;
+            const double resx = EPI ? sqrt(rx2 + T.rxt * T.rxt) : sqrt(rx2), resy = sqrt(ry2);
+            const double resznl = EPI ? sqrt(rn2 + T.rz0 * T.rz0) : sqrt(rn2), reszl = sqrt(rl2);
+            const double pcost = EPI ? T.t : cx;         // EPI: c'(x, t) with c = (0, 1)
+            const double dcost = EPI ? pcost + yry + (zrn + T.z0 * T.rz0) + zrl - gap : pcost + yry + zrn + zrl - gap;
             S.pcost = pcost; S.dcost = dcost; S.gap = gap; S.resx = resx; S.resy = resy; S.resz = reszl;
             T.resznl = resznl;
             if (pcost < 0.0) { S.relgap = gap / -pcost; S.relgap_valid = 1; }
@@ -1605,27 +1627,46 @@ __global__ void k_gp_res(Ptrs p, GPPtrs g) {
     }
 }
 // after the i-th direction (:1030-1078): dsdz, the unscaled steps dz2 = W^{-1} dz and ds2 = W' ds, scale2 of ds and
-// dz, the step to the boundary, phi and its directional derivative; the problem starts its line search
-__global__ void k_gp_dir_post(Ptrs p, GPPtrs g, int i) {
+// dz, the step to the boundary, phi and its directional derivative; the problem starts its line search.  CONES: sdot
+// is the dot product on the 'q' rows too; each cone's warp forms its dz2 = W^{-1} dz, ds2 = W' ds, scale2 and max_step
+template <bool EPI = true, bool CONES = false> __global__ void k_gp_dir_post(Ptrs p, GPPtrs g, int i) {
     GP_SETUP
     if (S.done) return;
     double dsdz = 0, mins = INFINITY, minz = INFINITY;
     for (int k = tid; k < p.m; k += nt) {
         const double ds = p.ds[om + k], dz = p.dz[om + k], l = p.lmbda[om + k];
         dsdz += ds * dz;
+        if (CONES && k >= p.ml) continue;
         g.dz2[om + k] = p.di[om + k] * dz; g.ds2[om + k] = p.d[om + k] * ds;
         const double ss = ds / l, zs = dz / l;
         p.ds[om + k] = ss; p.dz[om + k] = zs;
         mins = fmin(mins, ss); minz = fmin(minz, zs);
     }
+    if (CONES) {
+        __syncthreads();                                 // every row's ds dz is in dsdz before the cones scale them
+        const double *v = p.v + oc - p.ml, *beta = p.beta + oc, *l = p.lmbda + om;
+        double *ds = p.ds + om, *dz = p.dz + om;
+        FOR_CONES(o, len) {
+            q_scale(wt, v + o, beta[k_], dz + o, g.dz2 + om + o, len, true);
+            q_scale(wt, v + o, beta[k_], ds + o, g.ds2 + om + o, len, false);
+            __syncwarp();
+            q_scale2(wt, l + o, ds + o, len, false);
+            q_scale2(wt, l + o, dz + o, len, false);
+            __syncwarp();
+            mins = fmin(mins, -q_max_step(wt, ds + o, len));
+            minz = fmin(minz, -q_max_step(wt, dz + o, len));
+        }
+    }
     dsdz = block_sum(dsdz, sh);
     mins = block_min(mins, sh);
     minz = block_min(minz, sh);
     if (tid == 0) {
-        dsdz += T.ds0 * T.dz0;
-        T.dz20 = T.di0 * T.dz0; T.ds20 = T.d0 * T.ds0;
-        T.ds0 /= T.l0; T.dz0 /= T.l0;
-        mins = fmin(mins, T.ds0); minz = fmin(minz, T.dz0);
+        if (EPI) {
+            dsdz += T.ds0 * T.dz0;
+            T.dz20 = T.di0 * T.dz0; T.ds20 = T.d0 * T.ds0;
+            T.ds0 /= T.l0; T.dz0 /= T.l0;
+            mins = fmin(mins, T.ds0); minz = fmin(minz, T.dz0);
+        }
         const double t = fmax(0.0, fmax(-mins, -minz));
         S.step = t == 0.0 ? 1.0 : fmin(1.0, GP_STEP / t);
         S.dsdz = dsdz;
@@ -1650,8 +1691,10 @@ __global__ void k_gp_trial(Ptrs p, GPPtrs g) {
     if (tid == 0) { T.nt = T.t + st * T.dt; T.nz0 = T.z0 + st * T.dz20; T.ns0 = T.s0 + st * T.ds20; }
 }
 // copies of the state a relaxed line search saves (:1190-1214) and a resumed one restores (:1239-1260); `dir`: the
-// step vectors too (not on the restore after a singular KKT matrix, :790-813, which restores the residuals instead)
-__device__ void gp_save(const Ptrs &p, const GPPtrs &g, int b, bool save, bool dir, bool res) {
+// step vectors too (not on the restore after a singular KKT matrix, :790-813, which restores the residuals instead).
+// CONES: W's v and beta too (:1196-1198); EPI: the epigraph row's scalars
+template <bool EPI = true, bool CONES = false>
+__device__ void gp_save(const Ptrs &p, const GPPtrs &g, const QSave &qs, int b, bool save, bool dir, bool res) {
     const int tid = threadIdx.x, nt = blockDim.x;
     const long long on = (long long)b * p.n, om = (long long)b * p.m, oc = (long long)b * p.L, oq = (long long)b * p.neq;
     auto cp = [save](double *live, double *kept) { if (save) *kept = *live; else *live = *kept; };
@@ -1676,7 +1719,11 @@ __device__ void gp_save(const Ptrs &p, const GPPtrs &g, int b, bool save, bool d
         }
         if (res) cp(p.rz + om + k, g.rz0 + oc + k);
     }
-    if (tid == 0) {
+    if (CONES) {
+        for (int k = tid; k < p.m - p.ml; k += nt) cp(p.v + oc + k, qs.v0 + oc + k);
+        for (int k = tid; k < p.nq; k += nt) cp(p.beta + oc + k, qs.beta0 + oc + k);
+    }
+    if (EPI && tid == 0) {
         GPScal &T = gp_scal(g, oc);
         cp(&T.t, &T.t0); cp(&T.s0, &T.s00); cp(&T.z0, &T.z00); cp(&T.l0, &T.l00); cp(&T.d0, &T.d00);
         cp(&T.di0, &T.di00);
@@ -1687,18 +1734,22 @@ __device__ void gp_save(const Ptrs &p, const GPPtrs &g, int b, bool save, bool d
 // the line search's decision for slot b (:1131-1261) once the GEMVs have formed newrx: newgap, newphi and cpl's
 // relaxed-line-search state machine.  A problem still searching halves its step (or resumes the saved search) and
 // counts itself in nsearch; a step that underflows to 0 ends the problem 'unknown' (status 3) on its iterate
-template <bool EQ> __global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, int *nsearch) {
+template <bool EQ, bool EPI = true, bool CONES = false>
+__global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, int *nsearch, QSave qs) {
     GP_SETUP
     __shared__ int act;                                  // 1: save the state, 2: restore it
     if (S.done || T.searching == 0.0) return;
     const double *f = g.fv + (long long)b * g.nK;
     double rx2 = 0, rn2 = 0;
     for (int k = tid; k < p.n; k += nt) { const double v = g.nrx[on + k]; rx2 += v * v; }
-    for (int k = tid; k < g.mnl; k += nt) { const double v = g.ns[om + k] + f[k + 1]; rn2 += v * v; }
+    for (int k = tid; k < g.mnl; k += nt) { const double v = g.ns[om + k] + f[k + (EPI ? 1 : 0)]; rn2 += v * v; }
     rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh);
     if (tid == 0) {
-        const double rxt = -T.nz0 + 1.0, r0 = T.ns0 + (f[0] - T.nt);
-        const double nresx = sqrt(rx2 + rxt * rxt), nresznl = sqrt(rn2 + r0 * r0);
+        double nresx = sqrt(rx2), nresznl = sqrt(rn2);
+        if (EPI) {
+            const double rxt = -T.nz0 + 1.0, r0 = T.ns0 + (f[0] - T.nt);
+            nresx = sqrt(rx2 + rxt * rxt); nresznl = sqrt(rn2 + r0 * r0);
+        }
         const double step = S.step, gap = S.gap;
         const double ngap = (1.0 - (1.0 - S.sigma) * step) * gap + step * step * S.dsdz;
         const double nphi = T.th1 * ngap + T.th2 * nresx + T.th3 * nresznl;
@@ -1737,12 +1788,14 @@ template <bool EQ> __global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, in
         else atomicAdd(nsearch, 1);
     }
     __syncthreads();
-    if (act) gp_save(p, g, b, act == 1, true, act == 1);
+    if (act) gp_save<EPI, CONES>(p, g, qs, b, act == 1, true, act == 1);
 }
 // a singular KKT matrix after iteration 0 (:778-840): with 0 < relaxed_iters < 8 the problem restores the saved state
 // (W, x, y, s, z, lmbda, the residuals, phi and gap) and is factored again (counted in nre); otherwise, or when the
-// second factorisation fails too (second = 1), it ends 'unknown' (status 3) on its current iterate
-template <bool EQ> __global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *info, int iter, int second, int *nre) {
+// second factorisation fails too (second = 1), it ends 'unknown' (status 3) on its current iterate.  EPI false: mu
+// follows the restored gap (:791), for k_dir_rhs
+template <bool EQ, bool EPI = true, bool CONES = false>
+__global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *info, int iter, int second, int *nre, QSave qs) {
     GP_SETUP
     __shared__ int act;
     if (S.done || (info[b] <= 0 && !(EQ && p.infop[b] > 0))) return;
@@ -1750,18 +1803,22 @@ template <bool EQ> __global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *in
         act = !second && T.relaxed > 0 && T.relaxed < GP_MAX_RELAXED;
         if (act) {
             T.phi = T.phi0; S.gap = T.gap0; T.relaxed = -1;
+            if (!EPI) S.mu = S.gap / (p.ml + p.nq);
             atomicAdd(nre, 1);
         } else { S.done = 1; S.status = 3; S.iters = iter; }
     }
     __syncthreads();
     if (!act) return;
-    gp_save(p, g, b, false, false, true);
+    gp_save<EPI, CONES>(p, g, qs, b, false, false, true);
     __syncthreads();
     double rx2 = 0, rn2 = 0;
     for (int k = tid; k < p.n; k += nt) { const double v = p.rx[on + k]; rx2 += v * v; }
     for (int k = tid; k < g.mnl; k += nt) { const double v = p.rz[om + k]; rn2 += v * v; }
     rx2 = block_sum(rx2, sh); rn2 = block_sum(rn2, sh);
-    if (tid == 0) { S.resx = sqrt(rx2 + T.rxt * T.rxt); T.resznl = sqrt(rn2 + T.rz0 * T.rz0); }
+    if (tid == 0) {
+        if (EPI) { S.resx = sqrt(rx2 + T.rxt * T.rxt); T.resznl = sqrt(rn2 + T.rz0 * T.rz0); }
+        else { S.resx = sqrt(rx2); T.resznl = sqrt(rn2); }
+    }
 }
 // the update (:1264-1355): x, t, y += step d; ds, dz := e + step d; scale2 inverse; update_scaling with dnl and d
 // alike; s = W' lmbda, z = W^{-1} lmbda; gap = lmbda'lmbda
@@ -1806,24 +1863,32 @@ __device__ __forceinline__ double cp_dfz(const double *Df, int n, int nK, double
     for (int i = 1; i < nK; ++i) a += z[i - 1] * Df[(long long)i * n + j];
     return a;
 }
-// the z of a full evaluation, [z0; z[:mnl]], for every active slot
-__global__ void k_cp_zpack(Ptrs p, GPPtrs g, CPPtrs c) {
+// a + Df'z[:nK] at column j of a cpl batch's Df (nK x n, row-major; no objective row)
+__device__ __forceinline__ double cpl_dfz(const double *Df, int n, int nK, double a, const double *z, int j) {
+    for (int i = 0; i < nK; ++i) a += z[i] * Df[(long long)i * n + j];
+    return a;
+}
+// the z of a full evaluation, [z0; z[:mnl]] (EPI false: z[:mnl]), for every active slot
+template <bool EPI = true> __global__ void k_cp_zpack(Ptrs p, GPPtrs g, CPPtrs c) {
     GP_SETUP
     double *zc = c.z + (long long)b * g.nK;
-    for (int i = tid; i < g.nK; i += nt) zc[i] = i == 0 ? T.z0 : p.z[om + i - 1];
+    if (EPI) for (int i = tid; i < g.nK; i += nt) zc[i] = i == 0 ? T.z0 : p.z[om + i - 1];
+    else for (int i = tid; i < g.nK; i += nt) zc[i] = p.z[om + i];
 }
 // the callback's F at slot b's iterate (FULL) or trial point: f into fv.  FULL: a non-finite f recorded in bad,
 // Df[0] into gf0, Df[1:] into G's rows [0, mnl) and H's lower triangle into P's, by 32 x 32 tiles through shared
 // memory (H row-major, P column-major).  Trial, only the problems still searching: newrx's nonlinear part
-// Df'[nz0; nz[:mnl]] into nrx (the GEMVs add G'newzl + A'newy).  256 threads
-template <bool FULL> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GPPtrs g, CPPtrs c) {
+// Df'[nz0; nz[:mnl]] into nrx (the GEMVs add G'newzl + A'newy).  EPI false (a cpl batch): Df is Df[:mnl], all of it
+// goes into G, and newrx starts from c.  256 threads
+template <bool FULL, bool EPI = true> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GPPtrs g, CPPtrs c) {
     GP_SETUP
     if (S.done || (!FULL && T.searching == 0.0)) return;
     const int n = p.n, nK = g.nK;
     const double *f = c.f + (long long)b * nK, *Df = c.Df + (long long)b * nK * n;
     for (int i = tid; i < nK; i += nt) g.fv[(long long)b * nK + i] = f[i];
     if (!FULL) {
-        for (int j = tid; j < n; j += nt) g.nrx[on + j] = cp_dfz(Df, n, nK, T.nz0, g.nz + om, j);
+        for (int j = tid; j < n; j += nt)
+            g.nrx[on + j] = EPI ? cp_dfz(Df, n, nK, T.nz0, g.nz + om, j) : cpl_dfz(Df, n, nK, p.q[on + j], g.nz + om, j);
         return;
     }
     if (tid == 0) {
@@ -1831,11 +1896,11 @@ template <bool FULL> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GP
         for (int i = 0; i < nK; ++i) fin = fin && isfinite(f[i]);
         if (!fin) atomicMin(c.bad, c.idx[b]);
     }
-    for (int j = tid; j < n; j += nt) g.gf0[on + j] = Df[j];
+    if (EPI) for (int j = tid; j < n; j += nt) g.gf0[on + j] = Df[j];
     double *G = g.G + (long long)b * g.sG;
     for (long long e = tid; e < (long long)g.mnl * n; e += nt) {
         const long long i = e % g.mnl, j = e / g.mnl;
-        G[i + j * g.ldg] = Df[(i + 1) * n + j];
+        G[i + j * g.ldg] = Df[(i + (EPI ? 1 : 0)) * n + j];
     }
     __shared__ double tile[32][33];
     const double *H = c.H + (long long)b * n * n;
@@ -1855,12 +1920,14 @@ template <bool FULL> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GP
             }
         }
 }
-// rx += Df'[z0; z[:mnl]] at the iterates, from the callback's Df (after k_gp_res_begin; the GEMVs add G'zl + A'y)
-__global__ void k_cp_rx(Ptrs p, GPPtrs g, CPPtrs c) {
+// rx += Df'[z0; z[:mnl]] (EPI false: Df'z[:mnl]) at the iterates, from the callback's Df (after k_gp_res_begin; the
+// GEMVs add G'zl + A'y)
+template <bool EPI = true> __global__ void k_cp_rx(Ptrs p, GPPtrs g, CPPtrs c) {
     GP_SETUP
     if (S.done) return;
     const double *Df = c.Df + (long long)b * g.nK * p.n;
-    for (int j = tid; j < p.n; j += nt) p.rx[on + j] += cp_dfz(Df, p.n, g.nK, T.z0, p.z + om, j);
+    for (int j = tid; j < p.n; j += nt)
+        p.rx[on + j] += EPI ? cp_dfz(Df, p.n, g.nK, T.z0, p.z + om, j) : cpl_dfz(Df, p.n, g.nK, 0.0, p.z + om, j);
 }
 // a domain round's decision (:1052-1062) once the callback has evaluated F at the trial points x + step dx: a problem
 // still searching whose f has a non-finite entry halves its step and counts itself in nsearch; a step that underflows
@@ -1949,6 +2016,10 @@ struct cvxb_batch {
     DevBuf<int> cpi;
     cvxb_cp_eval_fn cfn = nullptr;
     void *cctx = nullptr;
+    // cpl batches (cvxb_batch_create_cpl): a CP batch (cp is set) of cpl's own problem, without the epigraph row: nK =
+    // mnl, c in q, 'q' cones after the 'l' rows; qs: the relaxed line search's saved v and beta with cones
+    bool cpl = false;
+    QSave qs{};
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
         for (cudaEvent_t e : {e0, e1}) if (e) cudaEventDestroy(e);
@@ -1967,14 +2038,17 @@ int state_alloc(cvxb_batch *b) {
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
     const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
-    // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m)
+    // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m), and with
+    // cones v0 (sum q) | beta0 (nq)
     const long long gpl = b->gp || b->cp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
-    const long long L = cone + sb + ref + lps + gpl;
+    const long long qsv = gpl ? cone : 0;
+    const long long L = cone + sb + ref + lps + gpl + qsv;
     if (b->L == L) return 0;
     b->L = p.L = 0;
     b->cst.reset();
     p.v = p.beta = p.wx = p.wx2 = p.wz = p.ws = p.wz2 = p.ws2 = p.wz3 = p.wy = p.wy2 = p.lps = nullptr;
     p.sr = p.srti = p.sigs = p.sigz = nullptr;
+    b->qs = QSave{};
     if (L == 0) return 0;
     CVXB_TRY(b->cst.alloc((size_t)b->B * L));
     CVXB_CUDA(cudaMemset(b->cst.p, 0, (size_t)b->B * L * sizeof(double)));
@@ -1998,6 +2072,7 @@ int state_alloc(cvxb_batch *b) {
         for (double **v : {&g.y0, &g.dy0, &g.ry0}) { *v = r; r += p2; }
         for (double **v : {&g.s0, &g.z0, &g.ds0, &g.dz0, &g.ds20, &g.dz20, &g.l0, &g.d0, &g.di0, &g.rz0}) { *v = r; r += m2; }
     }
+    if (qsv) { b->qs.v0 = r; r += ev(sumq); b->qs.beta0 = r; }
     return 0;
 }
 
@@ -2426,14 +2501,14 @@ int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) 
 }
 // r += Df'[z0; znl] + G' zl (+ A' y) (slot k's z at z + k*m).  GP: Df'[z0; znl] = F'(z_i y) from k_gp_eval's
 // weights.  CP: at the iterates (full) k_cp_rx adds it; at trial points k_cp_take<false> has written it into r
-template <bool EQ> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
+template <bool EQ, bool EPI = true> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
     if (!b->cp) {
         GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
         CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
     } else if (full) {
-        k_cp_rx<<<B, 256, 0, b->st>>>(b->p, g, b->cq); count_launch();
+        k_cp_rx<EPI><<<B, 256, 0, b->st>>>(b->p, g, b->cq); count_launch();
     }
     if (ml > 0) {
         GemvBatch gl; gl.batch = B; gl.sA = g.sG; gl.sx = m; gl.sy = n;
@@ -2476,22 +2551,22 @@ int cp_call(cvxb_batch *b, const double *x, bool full) {
     return 0;
 }
 // F(x, z[:mnl]) at the iterates: f into fv, grad f0 into gf0, Df[1:] into G's rows [0, mnl); CP also H into P
-// (GP forms H in gp_hessian)
-int cpl_eval_full(cvxb_batch *b) {
+// (GP forms H in gp_hessian).  EPI false (a cpl batch): Df[:mnl] into G's rows [0, mnl)
+template <bool EPI = true> int cpl_eval_full(cvxb_batch *b) {
     if (!b->cp) return gp_eval(b, b->p.x, b->n, true, 0);
     const int B = b->Bact;
-    k_cp_zpack<<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    k_cp_zpack<EPI><<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
     CVXB_TRY(cp_call(b, b->p.x, true));
-    k_cp_take<true><<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    k_cp_take<true, EPI><<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
     if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, B, b->sP, b->st));
     return 0;
 }
 // F at the line search's trial points g.nx, for the problems still searching: f into fv; CP also newrx's nonlinear
-// part into nrx
-int cpl_eval_trial(cvxb_batch *b) {
+// part into nrx (EPI false: c + Df'newznl)
+template <bool EPI = true> int cpl_eval_trial(cvxb_batch *b) {
     if (!b->cp) return gp_eval(b, b->gq.nx, b->n, false, 1);
     CVXB_TRY(cp_call(b, b->gq.nx, false));
-    k_cp_take<false><<<b->Bact, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
+    k_cp_take<false, EPI><<<b->Bact, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
     return 0;
 }
 // slot -> load index for the callback, after a solve's start or a compaction
@@ -2516,18 +2591,26 @@ int cp_domain(cvxb_batch *b, int it) {
     return 0;
 }
 // the i-th Newton direction of cpl (:966-1045): right-hand side, kktsolver_e's solve and `refinement` steps from
-// res() (:889-956), then the step to the boundary and the merit function's slope
-template <bool EQ> int gp_direction(cvxb_batch *b, int i) {
+// res() (:889-956), then the step to the boundary and the merit function's slope.  Without the epigraph row (EPI
+// false) there is no t to eliminate, and cpl's f4 is coneqp's: the right-hand side is k_dir_rhs's without the
+// Mehrotra term (its i = 0), then f4_no_ir around batch_solve and coneqp's refinement residual, 'q' cones included
+template <bool EQ, bool EPI = true, bool CONES = false> int gp_direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     const long long L = b->L;
-    k_gp_dir_rhs<<<B, T, 0, st>>>(p, g); count_launch();
+    if (EPI) k_gp_dir_rhs<<<B, T, 0, st>>>(p, g);
+    else k_dir_rhs<CONES, EQ, false><<<B, T, 0, st>>>(p, 0);
+    count_launch();
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
-    k_gp_f4_post<<<B, T, 0, st>>>(p, g, 0); count_launch();
+    if (EPI) k_gp_f4_post<<<B, T, 0, st>>>(p, g, 0);
+    else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0);
+    count_launch();
     for (int r = 0; r < p.refinement; ++r) {
-        k_gp_res<<<B, T, 0, st>>>(p, g); count_launch();
+        if (EPI) k_gp_res<<<B, T, 0, st>>>(p, g);
+        else k_res<EQ, false><<<B, T, 0, st>>>(p);
+        count_launch();
         GemvBatch gH; gH.batch = B; gH.sA = b->sP; gH.sx = n; gH.sy = L;                 // wx2 -= H dx
         CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gH));
         if (EQ) {
@@ -2546,26 +2629,30 @@ template <bool EQ> int gp_direction(cvxb_batch *b, int i) {
             GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
             CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
         }
-        k_gp_f4_pre<<<B, T, 0, st>>>(p, g); count_launch();
+        if (EPI) k_gp_f4_pre<<<B, T, 0, st>>>(p, g);
+        else k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L);
+        count_launch();
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
-        k_gp_f4_post<<<B, T, 0, st>>>(p, g, 1); count_launch();
+        if (EPI) k_gp_f4_post<<<B, T, 0, st>>>(p, g, 1);
+        else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
+        count_launch();
     }
-    k_gp_dir_post<<<B, T, 0, st>>>(p, g, i); count_launch();
+    k_gp_dir_post<EPI, CONES><<<B, T, 0, st>>>(p, g, i); count_launch();
     return 0;
 }
 // the lock-step line search after the i-th direction (:1125-1261): each round evaluates F and newrx at every
 // searching problem's trial point and takes its decision; one readback of the count still searching per round
-template <bool EQ> int gp_line_search(cvxb_batch *b, int i, int it) {
+template <bool EQ, bool EPI = true, bool CONES = false> int gp_line_search(cvxb_batch *b, int i, int it) {
     cudaStream_t st = b->st;
     const int B = b->Bact, T = 256;
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     for (int left = 1; left > 0; b->ls_rounds++) {
         k_gp_trial<<<B, T, 0, st>>>(p, g); count_launch();
-        CVXB_TRY(cpl_eval_trial(b));
-        CVXB_TRY(gp_rx<EQ>(b, g.nz, g.ny, g.nrx, false));
+        CVXB_TRY(cpl_eval_trial<EPI>(b));
+        CVXB_TRY((gp_rx<EQ, EPI>(b, g.nz, g.ny, g.nrx, false)));
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_gp_ls<EQ><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p); count_launch();
+        k_gp_ls<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p, b->qs); count_launch();
         CVXB_LAUNCH_CHECK();
         CVXB_TRY(read_count(b, left));
     }
@@ -2577,9 +2664,13 @@ int cpl_factor(cvxb_batch *b, bool first) {
     if (!b->cp) CVXB_TRY(gp_hessian(b));
     return batch_factor(b, !first);
 }
-// the lock-step cpl of a GP or CP batch's epigraph problem.  A CP batch starts from its x0 and backtracks each step
-// into dom f before the line search; it calls back to the host, so the loop is never captured into a graph
-template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
+// the lock-step cpl of a GP or CP batch's epigraph problem (EPI) or of a cpl batch's own problem (EPI false, with 'q'
+// cones when CONES).  A CP or cpl batch starts from its x0 and backtracks each step into dom f before the line search;
+// it calls back to the host, so the loop is never captured into a graph.  Without the epigraph row the scaling and
+// the update are coneqp's (k_scaling, k_update: cpl's compute_scaling, ssqr, update_scaling and unscaling are
+// coneqp's, and so is mu = gap / (mnl + ml + len(q)), :978)
+template <bool EQ, bool EPI = true, bool CONES = false>
+int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
@@ -2595,7 +2686,7 @@ template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, dou
     if (!b->cp)
         CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
                                     g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
-    k_gp_init<<<B, T, 0, st>>>(p, g); count_launch();
+    k_gp_init<CONES><<<B, T, 0, st>>>(p, g); count_launch();
     if (b->cp) {
         CVXB_CUDA(cudaMemcpyAsync(p.x, b->cpx0.p, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, st));
         CVXB_TRY(cp_upload_idx(b));
@@ -2605,9 +2696,9 @@ template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, dou
     int it = 0;
     for (it = 0; it <= maxiters; ++it) {
         // F(x, z[:mnl]) and the residuals (:627-691)
-        CVXB_TRY(cpl_eval_full(b));
-        k_gp_res_begin<EQ><<<B, T, 0, st>>>(p, g); count_launch();
-        CVXB_TRY(gp_rx<EQ>(b, p.z, p.y, p.rx, true));
+        CVXB_TRY(cpl_eval_full<EPI>(b));
+        k_gp_res_begin<EQ, EPI><<<B, T, 0, st>>>(p, g); count_launch();
+        CVXB_TRY((gp_rx<EQ, EPI>(b, p.z, p.y, p.rx, true)));
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = pq;
             CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, ga));
@@ -2617,7 +2708,7 @@ template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, dou
             CVXB_TRY(gemv_n(ml, n, g.G + g.mnl, g.ldg, nullptr, p.x, 1.0, 1.0, p.rz + g.mnl, b->gemv_ws.p, st, gl));
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_gp_stats<EQ><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        k_gp_stats<EQ, EPI><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
         int ndone = 0, bad = 0;
         CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2634,10 +2725,12 @@ template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, dou
             B = b->Bact;
             if (!pairs.empty()) {        // F(x)'s per-slot results stay put
                 if (b->cp) CVXB_TRY(cp_upload_idx(b));
-                CVXB_TRY(cpl_eval_full(b));
+                CVXB_TRY(cpl_eval_full<EPI>(b));
             }
         }
-        k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0); count_launch();
+        if (EPI) k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0);
+        else k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0);
+        count_launch();
         if (it == 0) {                   // kkt_chol2's first call; still singular: the Rank ValueError (:778-783)
             CVXB_TRY(cpl_factor(b, true));
             CVXB_TRY(first_switch<EQ>(b));
@@ -2645,21 +2738,24 @@ template <bool EQ> int solve_cpl(cvxb_batch *b, int maxiters, double abstol, dou
         } else {
             CVXB_TRY(cpl_factor(b, false));
             CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-            k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p); count_launch();
+            k_gp_singular<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p, b->qs); count_launch();
             int nre = 0;
             CVXB_TRY(read_count(b, nre));
             if (nre > 0) {               // restored problems are factored again at their saved iterates
-                CVXB_TRY(cpl_eval_full(b));
+                CVXB_TRY(cpl_eval_full<EPI>(b));
                 CVXB_TRY(cpl_factor(b, false));
-                k_gp_singular<EQ><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p); count_launch();
+                k_gp_singular<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p, b->qs);
+                count_launch();
             }
         }
         for (int i = 0; i < 2; ++i) {
-            CVXB_TRY(gp_direction<EQ>(b, i));
+            CVXB_TRY((gp_direction<EQ, EPI, CONES>(b, i)));
             if (b->cp) CVXB_TRY(cp_domain(b, it));
-            CVXB_TRY(gp_line_search<EQ>(b, i, it));
+            CVXB_TRY((gp_line_search<EQ, EPI, CONES>(b, i, it)));
         }
-        k_gp_update<<<B, T, 0, st>>>(p, g); count_launch();
+        if (EPI) k_gp_update<<<B, T, 0, st>>>(p, g);
+        else k_update<CONES, EQ><<<B, T, 0, st>>>(p, b->d_info.p, it);
+        count_launch();
         CVXB_LAUNCH_CHECK();
     }
     b->iters_run = it;
@@ -2882,12 +2978,11 @@ int load_common(cvxb_batch *b, const double *q, const double *G, const double *h
     return 0;
 }
 
-// the common part of a GP and a CP batch (cpl on cp's epigraph problem): a QP batch with m = mnl + ml 'l' rows, nK =
-// mnl + 1 nonlinear rows with sumK rows of F below the m rows of G, and gq's per-slot vectors
-int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int nK, long long sumK, int ml, int p, int device) {
-    const int mnl = nK - 1;
-    cvxb_dims d{};
-    d.ml = mnl + ml;
+// the common part of a GP, a CP and a cpl batch: a QP batch whose 'l' rows begin with the mnl nonlinear rows (d.ml
+// counts them), nK = mnl + 1 nonlinear rows of f (a cpl batch's nK = mnl) with sumK rows of F below the m rows of G,
+// and gq's per-slot vectors
+int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, long long sumK, const cvxb_dims &d,
+               int p, int device) {
     cvxb_batch *raw = nullptr;
     CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, false, (int)sumK));
     b.reset(raw);
@@ -2907,9 +3002,9 @@ int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int nK, long lo
     return 0;
 }
 
-// the rows of a GP or CP batch after its own data: G below the mnl rows of Df[1:], h in the 'l' rows (0 on the
-// nonlinear ones), q (c's x part) 0; then a fresh batch
-int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyKind kind) {
+// the rows of a GP, CP or cpl batch after its own data: G below the mnl rows of Df, h in the 'l' and 'q' rows (0 on
+// the nonlinear ones), q: c (a cpl batch), else 0 (c's x part in the epigraph problem); then a fresh batch
+int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyKind kind, const double *c = nullptr) {
     const size_t B = b->B, n = b->n, m = b->m, mnl = b->gq.mnl, ml = m - mnl;
     CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->h), 0, B * (m ? m : 1) * sizeof(double), b->st));
     if (ml > 0) {
@@ -2918,13 +3013,35 @@ int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyK
         CVXB_CUDA(cudaMemcpy2DAsync(const_cast<double *>(b->h) + mnl, m * sizeof(double), h, ml * sizeof(double),
                                     ml * sizeof(double), B, kind, b->st));
     }
-    CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
+    if (c) CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), c, B * n * sizeof(double), kind, b->st));
+    else CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->loaded = true;
     b->eq_loaded = false;
     for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
     b->permuted = false;
     return 0;
+}
+
+// a batch with the caller's F: CP (the epigraph problem, nK = mnl + 1) or cpl (nK = mnl, 'q' cones in d): the
+// callback's buffers, x0 and the slot -> problem map; refinement 1, cpl's default (cvxprog.py:422)
+int create_cp_common(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, const cvxb_dims &d, int p,
+                     int device) {
+    CVXB_TRY(create_cpl(b, nprob, n, mnl, nK, 0, d, p, device));
+    const size_t B = nprob, nn = n;
+    // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
+    const size_t len = 2 * nK + nK * nn + nn * nn;
+    CVXB_TRY(b->cpv.alloc(B * len));
+    CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
+    CVXB_TRY(b->cpx0.alloc(B * nn));
+    CVXB_TRY(b->cpi.alloc(B + 1));
+    CPPtrs &c = b->cq;
+    c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
+    c.idx = b->cpi.p; c.bad = b->cpi.p + B;
+    c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
+    b->cp = true;
+    b->p.refinement = 1;
+    return state_alloc(b.get());
 }
 
 }  // namespace
@@ -2971,7 +3088,9 @@ int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *
     }
     if (sumK + nK + ml > (1LL << 30)) { set_error("batch_create_gp: too many rows"); return CVXB_E_ARG; }
     std::unique_ptr<cvxb_batch> b;
-    CVXB_TRY(create_cpl(b, nprob, n, nK, sumK, ml, p, device));
+    cvxb_dims d{};
+    d.ml = nK - 1 + ml;
+    CVXB_TRY(create_cpl(b, nprob, n, nK - 1, nK, sumK, d, p, device));
     const size_t B = nprob;
     GPPtrs &g = b->gq;
     g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
@@ -3002,21 +3121,44 @@ int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, in
     }
     if ((long long)mnl + ml + 1 > (1LL << 30)) { set_error("batch_create_cp: too many rows"); return CVXB_E_ARG; }
     std::unique_ptr<cvxb_batch> b;
-    CVXB_TRY(create_cpl(b, nprob, n, mnl + 1, 0, ml, p, device));
-    const size_t B = nprob, nK = mnl + 1, nn = n;
-    // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
-    const size_t len = 2 * nK + nK * nn + nn * nn;
-    CVXB_TRY(b->cpv.alloc(B * len));
-    CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
-    CVXB_TRY(b->cpx0.alloc(B * nn));
-    CVXB_TRY(b->cpi.alloc(B + 1));
-    CPPtrs &c = b->cq;
-    c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
-    c.idx = b->cpi.p; c.bad = b->cpi.p + B;
-    c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
-    b->cp = true;
-    b->p.refinement = 1;                              // cpl's default (cvxprog.py:422); the epigraph row is always there
-    CVXB_TRY(state_alloc(b.get()));
+    cvxb_dims d{};
+    d.ml = mnl + ml;
+    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl + 1, d, p, device));
+    *out = b.release();
+    return 0;
+}
+
+int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
+    if (out) *out = nullptr;
+    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || p < 0 || !dims) {
+        set_error("batch_create_cpl: bad sizes (nprob in 1..%d, n >= 1, mnl and p nonnegative, dims given)",
+                  CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("batch_create_cpl: bad dims (its mnl must be 0; ml and the cone counts nonnegative)");
+        return CVXB_E_ARG;
+    }
+    if (dims->ns > 0) { set_error("batch_create_cpl: 's' cones are not supported by the cpl batch"); return CVXB_E_UNSUP; }
+    long long m = (long long)mnl + dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("batch_create_cpl: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
+        m += dims->q[k];
+    }
+    if (m == 0) {                                     // cpl's theta1 = 1 / gap0 (cvxprog.py:717) needs a row
+        set_error("batch_create_cpl: no constraint rows (mnl + cdim = 0)");
+        return CVXB_E_ARG;
+    }
+    if (m > (1LL << 30)) { set_error("batch_create_cpl: too many rows"); return CVXB_E_ARG; }
+    if (p > n) {                                      // cpl's check before the first factorisation
+        set_error("batch_create_cpl: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", p, n);
+        return CVXB_E_ARG;
+    }
+    std::unique_ptr<cvxb_batch> b;
+    cvxb_dims d = *dims;
+    d.ml += mnl;
+    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl, d, p, device));
+    b->cpl = true;
     *out = b.release();
     return 0;
 }
@@ -3083,11 +3225,20 @@ int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const do
 
 int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const double *h, int space) {
     if (!b || !x0 || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_cp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->cp) { set_error("batch_load_cp: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
+    if (!b->cp || b->cpl) { set_error("batch_load_cp: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, (size_t)b->B * b->n * sizeof(double), kind, b->st));
     return load_cpl_common(b, G, h, kind);
+}
+
+int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const double *G, const double *h, int space) {
+    if (!b || !c || !x0 || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_cpl: NULL argument"); return CVXB_E_ARG; }
+    if (!b->cpl) { set_error("batch_load_cpl: not a cpl batch (cvxb_batch_create_cpl)"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, (size_t)b->B * b->n * sizeof(double), kind, b->st));
+    return load_cpl_common(b, G, h, kind, c);
 }
 
 int cvxb_batch_ls_rounds(cvxb_batch *b) { return b ? b->ls_rounds : CVXB_E_ARG; }
@@ -3113,7 +3264,7 @@ int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const
                           int space) {
     if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
     if (b->gp) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
-    if (b->cp) { set_error("batch_load_start: cp starts from the x0 of cvxb_batch_load_cp"); return CVXB_E_ARG; }
+    if (b->cp) { set_error("batch_load_start: cp and cpl start from the x0 of their load"); return CVXB_E_ARG; }
     if (b->lp && ((!x) != (!s) || (y && !z) || (!x && !z))) {
         set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
                   "both");
@@ -3152,6 +3303,12 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
     if (b->cp && !b->cfn) { set_error("batch_solve: a CP batch needs its F (cvxb_batch_set_cp_eval)"); return CVXB_E_ARG; }
+    if (b->cpl) {
+        using Solve = int (*)(cvxb_batch *, int, double, double, double);
+        static const Solve cpl_solvers[4] = {solve_cpl<false, false, false>, solve_cpl<true, false, false>,
+                                             solve_cpl<false, false, true>, solve_cpl<true, false, true>};
+        return cpl_solvers[(b->neq > 0 ? 1 : 0) + (b->p.nq > 0 ? 2 : 0)](b, maxiters, abstol, reltol, feastol);
+    }
     if (b->gp || b->cp) return b->neq > 0 ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
                                           : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
     using Solve = int (*)(cvxb_batch *, int, double, double, double);

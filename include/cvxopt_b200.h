@@ -454,6 +454,29 @@ int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const d
 typedef int (*cvxb_cp_eval_fn)(void *ctx, int k, int full, const double *x, const double *z, const int *problem,
                                double *f, double *Df, double *H, void *stream);
 int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx);
+/* batch of cpl problems (B x solvers.cpl(c, F, G, h, dims, A, b), cvxprog.py:35-1356, with its default kktsolver):
+ *     minimize  c'x  s.t.  fk(x) <= 0 (k = 1..mnl),  G x + s = h,  s in 'l' x 'q'[0] x ...,  A x = b
+ * with F evaluated by the caller (cvxb_batch_set_cp_eval, nK = mnl: f, Df and z have no objective row).  It runs the
+ * CP batch's lock-step cpl without the epigraph row, the 'q' rows after the 'l' rows, from the loaded x0 with y = 0
+ * and s = z = e.  With 'q' cones the reference's default kktsolver is 'chol' (a QR of A' and a Cholesky of order
+ * n - p); the batch keeps its 'chol2' elimination (S = H + Gs'Gs with Gs = W^{-T} [Df; G], S + A'A for a problem
+ * whose S is singular at the start, then Kp), as the QP batch does with 'q' cones: both solve the same KKT system.
+ * Refused before the device: CVXB_E_ARG for nprob outside 1..CVXB_BATCH_MAX, n < 1, mnl < 0, p < 0, dims NULL,
+ * dims->mnl != 0, a negative count, a q[k] < 1, no constraint rows (mnl + cdim = 0) and cpl's "Rank(A) < p" for
+ * p > n; CVXB_E_UNSUP for dims->ns > 0.  Load it with cvxb_batch_load_cpl (and cvxb_batch_load_eq when p > 0);
+ * cvxb_batch_load, load_lp, load_gp, load_cp and load_start on it are CVXB_E_ARG.  Solve, set_refinement (default 1,
+ * as cpl), results, results_y, stats, ls_rounds and destroy are the CP batch's calls with its semantics, except that
+ * s and z are [snl; sl] and [znl; zl] with the 'q' rows in sl and zl, and the primal objective is c'x.  Device memory
+ * per problem, with m = mnl + cdim and ev() rounding up to even: what cvxb_batch_create_eq's batch of the same n, p
+ * and dims {'l': mnl + ml, 'q': q} holds with refinement 1, plus mnl(n + 2) + n² (the callback's f, Df, z and H),
+ * mnl + 3n + p + 4m (f, the unscaled steps and the line search's trial point), n (x0), 56 + 3 ev(n) + 3 ev(p) +
+ * 10 ev(m) in the state row (the scalars and the line search's saved state), ev(sum q) + ev(nq) more there with 'q'
+ * cones (the saved v and beta), and one int (slot -> problem); and one int shared by the batch. */
+int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device);
+/* cpl batch only: c nprob x n, x0 nprob x n (strictly inside dom f), G nprob x (cdim x n column-major, ld cdim), h
+ * nprob x cdim ('l' rows, then each 'q' cone); G and h may be NULL when cdim = 0.  A and b come through
+ * cvxb_batch_load_eq. */
+int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const double *G, const double *h, int space);
 
 #ifdef __cplusplus
 }
