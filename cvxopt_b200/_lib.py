@@ -149,6 +149,8 @@ _SIGS = {
     "cvxb_batch_create_cpl": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                         C.c_int]),
     "cvxb_batch_load_cpl": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "cvxb_batch_create_sdp_cpl": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                            C.c_int]),
     "cvxb_batch_results": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
 }

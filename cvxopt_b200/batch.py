@@ -15,6 +15,7 @@ same lock-step machinery (ConeLPBatch, conelp_batch): a Python loop over `solver
 (`solvers.lp` for dims={'l': m}), with its infeasibility certificates.
 
 Dims with 's' blocks (orders <= 32) run through SDPBatch / sdp_batch (conelp) and SDPQPBatch / coneqp_batch (coneqp).
+cpl problems with 's' blocks (nonlinear constraints next to an LMI) run through SDPCPLBatch / sdp_cpl_batch.
 """
 import ctypes as C
 
@@ -954,12 +955,12 @@ class CPLBatch(CPBatch):
     _epi = 0
 
     def __init__(self, nprob, n, mnl, dims, p=0, device=0, index=None):
-        self._dims = _batch_dims(dims or {"l": 0})      # (ctypes dims, keep-alive, cdim)
+        self._dims = (_sdp_dims if self._sdp else _batch_dims)(dims or {"l": 0})   # (ctypes dims, keep-alive, cdim)
         super().__init__(nprob, n, mnl, self._dims[2], p, device, index)      # ml: the rows of G and h
 
     def _create(self):
-        return self._lib.cvxb_batch_create_cpl(C.byref(self._h), self.B, self.n, self.mnl, C.byref(self._dims[0]),
-                                               self.p, self.device)
+        create = self._lib.cvxb_batch_create_sdp_cpl if self._sdp else self._lib.cvxb_batch_create_cpl
+        return create(C.byref(self._h), self.B, self.n, self.mnl, C.byref(self._dims[0]), self.p, self.device)
 
     def load(self, c, x0, G, h, A=None, b=None):
         B, n, cd = self.B, self.n, self.ml
@@ -981,23 +982,25 @@ class CPLBatchGroup(CPBatchGroup):
     """CPBatchGroup for cpl problems: interleaved CPLBatch sub-batches solved concurrently, F called with each
     sub-batch's idx"""
 
+    _batch = CPLBatch        # the class of the sub-batches
+
     def __init__(self, nprob, n, mnl, dims, p=0, device=0, nsub=None):
         self._dims = dims
-        cdim = _batch_dims(dims or {"l": 0})[2]
+        cdim = (_sdp_dims if self._batch._sdp else _batch_dims)(dims or {"l": 0})[2]
         super().__init__(nprob, n, mnl, cdim, p, device, nsub)
 
     def _part(self):
-        return lambda nprob, n, m, device, dims, p=0: CPLBatch(nprob, n, self._mnl, self._dims, p, device)
+        return lambda nprob, n, m, device, dims, p=0: self._batch(nprob, n, self._mnl, self._dims, p, device)
 
     def load(self, c, x0, G, h, A=None, b=None):
         self._load_sliced((c, x0, G, h), A, b)
 
 
-def _cpl_args(c, F, G, h, dims, A, b):
+def _cpl_args(c, F, G, h, dims, A, b, sdp=False):
     """cpl's argument checks (cvxprog.py:426-530) on the batch -> mnl, c, x0, G, h, dims, A, b with the defaults
-    filled in; 's' cones raise NotImplementedError and p > n the Rank ValueError, before anything is created.  cpl reads
-    dims['q'] and dims['s'] (a missing key is its KeyError, :427, :472) and does not check their entries, which the
-    batch needs: those are checked with coneprog's TypeErrors (coneprog.py:493-500)"""
+    filled in; 's' cones raise NotImplementedError (unless sdp) and p > n the Rank ValueError, before anything is
+    created.  cpl reads dims['q'] and dims['s'] (a missing key is its KeyError, :427, :472) and does not check their
+    entries, which the batch needs: those are checked with coneprog's TypeErrors (coneprog.py:493-500)"""
     for key in ("q", "s"):
         if dims and key not in dims:
             raise KeyError(key)
@@ -1044,7 +1047,7 @@ def _cpl_args(c, F, G, h, dims, A, b):
         raise TypeError("'b' must be a 'd' matrix with one column")
     if b.shape[1] != p:
         raise TypeError("'b' must have length %d" % p)
-    if dims["s"]:
+    if dims["s"] and not sdp:
         raise NotImplementedError("the cpl batch takes 'l' and 'q' cones only (dims without 's')")
     if p > n:
         raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
@@ -1067,9 +1070,37 @@ def cpl_batch(c, F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=No
     Returns cpl's x, snl, sl, znl, zl, y, status, iterations, primal and dual objective, with the batch's stats
     (solve_ms, lock-step iterations, line-search rounds, nsub, solve_wall_ms).  nsub is qp_batch's.
     options: maxiters, abstol, reltol, feastol, refinement (as cpl's; refinement 1 by default)."""
-    mnl, c, x0, G, h, dims, A, b = _cpl_args(c, F, G, h, dims, A, b)
+    return _cpl_solve(c, F, G, h, dims, A, b, device, nsub, options, sdp=False)
+
+
+class SDPCPLBatch(CPLBatch):
+    """CPLBatch whose dims may hold 's' blocks of order <= 32 (cvxb_batch_create_sdp_cpl): B x solvers.cpl(c, F, G, h,
+    dims, A, b).  load() takes CPLBatch's arguments, with each 's' block's rows of G and h unpacked column-major after
+    the 'q' rows; only the lower triangle of an 's' block of G and h is read, and results() returns sl and zl with
+    symmetric 's' blocks."""
+    _sdp = True
+
+
+class SDPCPLBatchGroup(CPLBatchGroup):
+    """CPLBatchGroup of SDPCPLBatch parts"""
+    _batch = SDPCPLBatch
+
+
+def sdp_cpl_batch(c, F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, **options):
+    """Solve B independent cpl problems with semidefinite cones on one GPU, each as solvers.cpl(c, F, G, h, dims, A, b)
+    does: cpl_batch's arguments, F, options and returned dict, with dims that may hold 's' blocks (orders at most 32).
+    Each 's' block's rows of G and h follow the 'q' rows, unpacked column-major as the reference's G, and only their
+    lower triangles are read; the returned sl and zl have symmetric 's' blocks, as cpl returns them.  A nonlinear
+    objective f0 goes in as its epigraph (a variable t, minimise t, f0(x) - t the first row of f): that is how a
+    solvers.cp problem with an LMI is solved here."""
+    return _cpl_solve(c, F, G, h, dims, A, b, device, nsub, options, sdp=True)
+
+
+def _cpl_solve(c, F, G, h, dims, A, b, device, nsub, options, sdp):
+    """cpl_batch (sdp false) and sdp_cpl_batch: the checks, the group, F, the solve and the returned dict"""
+    mnl, c, x0, G, h, dims, A, b = _cpl_args(c, F, G, h, dims, A, b, sdp)
     B, n, p = x0.shape[0], x0.shape[1], A.shape[1]
-    grp = CPLBatchGroup(B, n, mnl, dims, p, device, nsub)
+    grp = (SDPCPLBatchGroup if sdp else CPLBatchGroup)(B, n, mnl, dims, p, device, nsub)
     try:
         grp.set_F(F)
     except BaseException:

@@ -1280,6 +1280,52 @@ __global__ void __launch_bounds__(SB_T) k_s_dir_post(Ptrs p, int i) {
     }
     if (tid == 0) { part[0] = dsdz; part[1] = ok ? m1 : NAN; part[2] = ok ? s_min(ev, ms) : NAN; }
 }
+// a cpl batch's unscaled steps of the 's' blocks (cvxprog.py:1031-1034): dz2 = W^{-1} dz = rti dz rti' and
+// ds2 = W' ds = r ds r' (m-vectors, slot b at + b*m), from the scaled ds and dz before k_s_dir_post replaces them
+__global__ void __launch_bounds__(SB_T) k_s_steps(Ptrs p, double *ds2, double *dz2) {
+    SB_SETUP
+    __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX];
+    if (S.done) return;
+    s_load(X, p.dz + om + so, ms);
+    SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+    __syncthreads();
+    s_congr(Y, R, X, T, false, ms);
+    s_store(dz2 + om + so, Y, ms);
+    s_load(X, p.ds + om + so, ms);
+    SB_FOR(e, ms) R[e] = p.sr[oc + sro + e];
+    __syncthreads();
+    s_congr(Y, R, X, T, false, ms);
+    s_store(ds2 + om + so, Y, ms);
+}
+// after k_s_dir_post in a cpl batch: each block's eigenpairs of ds (sigs) and of dz (sigz) in ascending order, as
+// max_step's syevd leaves them (misc.py:1046).  The update pairs sigs[i] with the i-th eigenvector, and after a resumed
+// line search those come from different directions (cvxprog.py:1238-1261), so the order is part of the result.  NaN
+// sorts last, so that the ranks are a permutation whatever the values
+__global__ void __launch_bounds__(SB_T) k_s_sort(Ptrs p) {
+    SB_SETUP
+    __shared__ double V[SMX], ev[CVXB_BATCH_SMAX];
+    __shared__ int rk[CVXB_BATCH_SMAX];
+    if (S.done) return;
+    for (int w = 0; w < 2; ++w) {
+        double *x = (w ? p.dz : p.ds) + om + so, *sg = (w ? p.sigz : p.sigs) + oc + sgo;
+        SB_FOR(e, ms) V[e] = x[e];
+        for (int j = tid; j < ms; j += SB_T) ev[j] = sg[j];
+        __syncthreads();
+        for (int j = tid; j < ms; j += SB_T) {
+            int r = 0;
+            for (int i = 0; i < ms; ++i) {
+                const double a = ev[i], c = ev[j];
+                const bool na = isnan(a), nc = isnan(c);
+                r += na != nc ? nc : (na || a == c) ? i < j : a < c;
+            }
+            rk[j] = r;
+        }
+        __syncthreads();
+        SB_FOR(e, ms) x[e % ms + rk[e / ms] * ms] = V[e];
+        for (int j = tid; j < ms; j += SB_T) sg[rk[j]] = ev[j];
+        __syncthreads();
+    }
+}
 // the update (coneprog.py:1365-1433, misc.py:592-634): Ls = diag(l)^{1/2} Qs diag(l)^{1/2} diag((1 + step sigs) / l)^{1/2},
 // likewise Lz; r := r Ls V diag(lambda+)^{-1/2}, rti := rti Lz U diag(lambda+)^{-1/2} with Lz' Ls = U diag(lambda+) V';
 // s = r diag(lambda+) r', z = rti diag(lambda+) rti'.  The results are staged in the block's rows of d (r), di (rti),
@@ -1355,10 +1401,10 @@ struct GPPtrs {
     double *g, *gs, *x0, *dx0, *rx0, *y0, *dy0, *ry0, *s0, *z0, *ds0, *dz0, *ds20, *dz20, *l0, *d0, *di0, *rz0;
 };
 // the 'q' part of W that a cpl batch's relaxed line search saves with the rest (cvxprog.py:1196-1198): v (sum q) and
-// beta (nq) in the state row.  A kernel's last argument, so that the GP and CP kernels' other arguments stay where
-// they are
+// beta (nq) in the state row, and with 's' blocks r and rti (sum s² each, :1199-1201).  A kernel's last argument, so
+// that the GP and CP kernels' other arguments stay where they are
 struct QSave {
-    double *v0, *beta0;
+    double *v0, *beta0, *r0, *rti0;
 };
 constexpr int GP_MAX_RELAXED = 8;
 constexpr double GP_ALPHA = 0.01, GP_BETA = 0.5, GP_STEP = 0.99;
@@ -1372,13 +1418,14 @@ __device__ __forceinline__ GPScal &gp_scal(const GPPtrs &g, long long oc) {
     (void)T; (void)ok;
 
 // the starting point (:556-570): x = 0, t = 0, y = 0, s = z = e, relaxed_iters = 0.  CONES: e is 1 at each cone's
-// first row and 0 in the rest of it
-template <bool CONES> __global__ void k_gp_init(Ptrs p, GPPtrs g) {
+// first row and 0 in the rest of it.  SDP: the identity in each 's' block (its diagonal rows)
+template <bool CONES, bool SDP = false> __global__ void k_gp_init(Ptrs p, GPPtrs g) {
     GP_SETUP
     for (int i = tid; i < p.n; i += nt) p.x[on + i] = 0.0;
     for (int i = tid; i < p.neq; i += nt) p.y[oq + i] = 0.0;
     for (int i = tid; i < p.m; i += nt) {
-        const double e = !CONES || i < p.ml ? 1.0 : 0.0;
+        double e = !CONES || i < p.ml ? 1.0 : 0.0;
+        if (SDP) e = i < p.ml || (i >= p.mlq && p.rw[i] == 1.0) ? 1.0 : 0.0;
         p.s[om + i] = e; p.z[om + i] = e;
     }
     if (CONES) {
@@ -1448,8 +1495,8 @@ template <bool EQ, bool EPI = true> __global__ void k_gp_res_begin(Ptrs p, GPPtr
 }
 // statistics and stopping rule (:693-755); iteration 0 fixes resx0, resznl0, pres0, dres0 and the merit weights.
 // EPI false: pcost = c'x, and no epigraph row in gap, resx, resznl and dcost.  'q' rows are 'l' rows here: snrm2 and
-// sdot are the 2-norm and the dot product on them
-template <bool EQ, bool EPI = true>
+// sdot are the 2-norm and the dot product on them.  SDP: they weigh the 's' rows (rw), so only the lower triangles count
+template <bool EQ, bool EPI = true, bool SDP = false>
 __global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int maxiters, double abstol, double reltol, double feastol,
                            int *ndone, int *doneflags) {
     GP_SETUP
@@ -1462,6 +1509,12 @@ __global__ void k_gp_stats(Ptrs p, GPPtrs g, int iter, int maxiters, double abst
         if (EQ) for (int i = tid; i < p.neq; i += nt) { const double v = p.ry[oq + i]; ry2 += v * v; yry += p.y[oq + i] * v; }
         for (int i = tid; i < p.m; i += nt) {
             const double v = p.rz[om + i], zv = p.z[om + i];
+            if (SDP) {
+                const double w = p.rw[i];
+                if (i < g.mnl) { rn2 += v * v; zrn += zv * v; } else { rl2 += w * v * v; zrl += w * zv * v; }
+                gap += w * p.s[om + i] * zv;
+                continue;
+            }
             if (i < g.mnl) { rn2 += v * v; zrn += zv * v; } else { rl2 += v * v; zrl += zv * v; }
             gap += p.s[om + i] * zv;
         }
@@ -1628,12 +1681,14 @@ __global__ void k_gp_res(Ptrs p, GPPtrs g) {
 }
 // after the i-th direction (:1030-1078): dsdz, the unscaled steps dz2 = W^{-1} dz and ds2 = W' ds, scale2 of ds and
 // dz, the step to the boundary, phi and its directional derivative; the problem starts its line search.  CONES: sdot
-// is the dot product on the 'q' rows too; each cone's warp forms its dz2 = W^{-1} dz, ds2 = W' ds, scale2 and max_step
-template <bool EPI = true, bool CONES = false> __global__ void k_gp_dir_post(Ptrs p, GPPtrs g, int i) {
+// is the dot product on the 'q' rows too; each cone's warp forms its dz2 = W^{-1} dz, ds2 = W' ds, scale2 and max_step.
+// SDP: k_s_steps and k_s_dir_post have done the 's' rows, whose ds and dz now hold eigenvectors; their sdot and
+// smallest eigenvalues come from spart
+template <bool EPI = true, bool CONES = false, bool SDP = false> __global__ void k_gp_dir_post(Ptrs p, GPPtrs g, int i) {
     GP_SETUP
     if (S.done) return;
     double dsdz = 0, mins = INFINITY, minz = INFINITY;
-    for (int k = tid; k < p.m; k += nt) {
+    for (int k = tid; k < (SDP ? p.mlq : p.m); k += nt) {
         const double ds = p.ds[om + k], dz = p.dz[om + k], l = p.lmbda[om + k];
         dsdz += ds * dz;
         if (CONES && k >= p.ml) continue;
@@ -1661,6 +1716,10 @@ template <bool EPI = true, bool CONES = false> __global__ void k_gp_dir_post(Ptr
     mins = block_min(mins, sh);
     minz = block_min(minz, sh);
     if (tid == 0) {
+        if (SDP) for (int k = 0; k < p.ns; ++k) {
+            const double *q = p.spart + ((long long)b * p.ns + k) * 4;
+            dsdz += q[0]; mins = fmin(mins, q[1]); minz = fmin(minz, q[2]);
+        }
         if (EPI) {
             dsdz += T.ds0 * T.dz0;
             T.dz20 = T.di0 * T.dz0; T.ds20 = T.d0 * T.ds0;
@@ -1692,8 +1751,9 @@ __global__ void k_gp_trial(Ptrs p, GPPtrs g) {
 }
 // copies of the state a relaxed line search saves (:1190-1214) and a resumed one restores (:1239-1260); `dir`: the
 // step vectors too (not on the restore after a singular KKT matrix, :790-813, which restores the residuals instead).
-// CONES: W's v and beta too (:1196-1198); EPI: the epigraph row's scalars
-template <bool EPI = true, bool CONES = false>
+// CONES: W's v and beta too (:1196-1198); SDP: W's r and rti (:1199-1201); EPI: the epigraph row's scalars.  The 's'
+// rows of the vectors come with the rest; sigs and sigz are not saved, as in the reference
+template <bool EPI = true, bool CONES = false, bool SDP = false>
 __device__ void gp_save(const Ptrs &p, const GPPtrs &g, const QSave &qs, int b, bool save, bool dir, bool res) {
     const int tid = threadIdx.x, nt = blockDim.x;
     const long long on = (long long)b * p.n, om = (long long)b * p.m, oc = (long long)b * p.L, oq = (long long)b * p.neq;
@@ -1723,6 +1783,12 @@ __device__ void gp_save(const Ptrs &p, const GPPtrs &g, const QSave &qs, int b, 
         for (int k = tid; k < p.m - p.ml; k += nt) cp(p.v + oc + k, qs.v0 + oc + k);
         for (int k = tid; k < p.nq; k += nt) cp(p.beta + oc + k, qs.beta0 + oc + k);
     }
+    if (SDP) for (int k = 0; k < p.ns; ++k) {
+        const int ms = p.sinfo[5 * k], ro = p.sinfo[5 * k + 3];
+        for (int e = tid; e < ms * ms; e += nt) {
+            cp(p.sr + oc + ro + e, qs.r0 + oc + ro + e); cp(p.srti + oc + ro + e, qs.rti0 + oc + ro + e);
+        }
+    }
     if (EPI && tid == 0) {
         GPScal &T = gp_scal(g, oc);
         cp(&T.t, &T.t0); cp(&T.s0, &T.s00); cp(&T.z0, &T.z00); cp(&T.l0, &T.l00); cp(&T.d0, &T.d00);
@@ -1734,7 +1800,7 @@ __device__ void gp_save(const Ptrs &p, const GPPtrs &g, const QSave &qs, int b, 
 // the line search's decision for slot b (:1131-1261) once the GEMVs have formed newrx: newgap, newphi and cpl's
 // relaxed-line-search state machine.  A problem still searching halves its step (or resumes the saved search) and
 // counts itself in nsearch; a step that underflows to 0 ends the problem 'unknown' (status 3) on its iterate
-template <bool EQ, bool EPI = true, bool CONES = false>
+template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false>
 __global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, int *nsearch, QSave qs) {
     GP_SETUP
     __shared__ int act;                                  // 1: save the state, 2: restore it
@@ -1788,13 +1854,13 @@ __global__ void k_gp_ls(Ptrs p, GPPtrs g, int i, int iter, int *nsearch, QSave q
         else atomicAdd(nsearch, 1);
     }
     __syncthreads();
-    if (act) gp_save<EPI, CONES>(p, g, qs, b, act == 1, true, act == 1);
+    if (act) gp_save<EPI, CONES, SDP>(p, g, qs, b, act == 1, true, act == 1);
 }
 // a singular KKT matrix after iteration 0 (:778-840): with 0 < relaxed_iters < 8 the problem restores the saved state
 // (W, x, y, s, z, lmbda, the residuals, phi and gap) and is factored again (counted in nre); otherwise, or when the
 // second factorisation fails too (second = 1), it ends 'unknown' (status 3) on its current iterate.  EPI false: mu
-// follows the restored gap (:791), for k_dir_rhs
-template <bool EQ, bool EPI = true, bool CONES = false>
+// follows the restored gap (:791), for k_dir_rhs; SDP: its degree counts each block's order
+template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false>
 __global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *info, int iter, int second, int *nre, QSave qs) {
     GP_SETUP
     __shared__ int act;
@@ -1803,13 +1869,13 @@ __global__ void k_gp_singular(Ptrs p, GPPtrs g, const int *info, int iter, int s
         act = !second && T.relaxed > 0 && T.relaxed < GP_MAX_RELAXED;
         if (act) {
             T.phi = T.phi0; S.gap = T.gap0; T.relaxed = -1;
-            if (!EPI) S.mu = S.gap / (p.ml + p.nq);
+            if (!EPI) S.mu = SDP ? S.gap / (p.ml + p.nq + (p.mdg - p.mlq)) : S.gap / (p.ml + p.nq);
             atomicAdd(nre, 1);
         } else { S.done = 1; S.status = 3; S.iters = iter; }
     }
     __syncthreads();
     if (!act) return;
-    gp_save<EPI, CONES>(p, g, qs, b, false, false, true);
+    gp_save<EPI, CONES, SDP>(p, g, qs, b, false, false, true);
     __syncthreads();
     double rx2 = 0, rn2 = 0;
     for (int k = tid; k < p.n; k += nt) { const double v = p.rx[on + k]; rx2 += v * v; }
@@ -2039,10 +2105,10 @@ int state_alloc(cvxb_batch *b) {
     const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
     // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m), and with
-    // cones v0 (sum q) | beta0 (nq)
+    // cones v0 (sum q) | beta0 (nq), with 's' blocks r0 rti0 (sum s²)
     const long long gpl = b->gp || b->cp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
-    const long long qsv = gpl ? cone : 0;
-    const long long L = cone + sb + ref + lps + gpl + qsv;
+    const long long qsv = gpl ? cone : 0, ssv = gpl && p.ns ? 2 * ev(b->sums2) : 0;
+    const long long L = cone + sb + ref + lps + gpl + qsv + ssv;
     if (b->L == L) return 0;
     b->L = p.L = 0;
     b->cst.reset();
@@ -2072,7 +2138,8 @@ int state_alloc(cvxb_batch *b) {
         for (double **v : {&g.y0, &g.dy0, &g.ry0}) { *v = r; r += p2; }
         for (double **v : {&g.s0, &g.z0, &g.ds0, &g.dz0, &g.ds20, &g.dz20, &g.l0, &g.d0, &g.di0, &g.rz0}) { *v = r; r += m2; }
     }
-    if (qsv) { b->qs.v0 = r; r += ev(sumq); b->qs.beta0 = r; }
+    if (qsv) { b->qs.v0 = r; r += ev(sumq); b->qs.beta0 = r; r += ev(p.nq); }
+    if (ssv) { b->qs.r0 = r; r += ev(b->sums2); b->qs.rti0 = r; }
     return 0;
 }
 
@@ -2500,8 +2567,10 @@ int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) 
     return 0;
 }
 // r += Df'[z0; znl] + G' zl (+ A' y) (slot k's z at z + k*m).  GP: Df'[z0; znl] = F'(z_i y) from k_gp_eval's
-// weights.  CP: at the iterates (full) k_cp_rx adds it; at trial points k_cp_take<false> has written it into r
-template <bool EQ, bool EPI = true> int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
+// weights.  CP: at the iterates (full) k_cp_rx adds it; at trial points k_cp_take<false> has written it into r.
+// SDP: G' trisc(zl) (misc.sgemv), the row weights rw on the 's' rows
+template <bool EQ, bool EPI = true, bool SDP = false>
+int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
     if (!b->cp) {
@@ -2512,7 +2581,7 @@ template <bool EQ, bool EPI = true> int gp_rx(cvxb_batch *b, const double *z, co
     }
     if (ml > 0) {
         GemvBatch gl; gl.batch = B; gl.sA = g.sG; gl.sx = m; gl.sy = n;
-        CVXB_TRY(gemv_t(ml, n, g.G + g.mnl, g.ldg, nullptr, z + g.mnl, 1.0, 1.0, r, b->st, gl));
+        CVXB_TRY(gemv_t(ml, n, g.G + g.mnl, g.ldg, SDP ? b->p.rw + g.mnl : nullptr, z + g.mnl, 1.0, 1.0, r, b->st, gl));
     }
     if (EQ) {
         GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = b->neq; ga.sy = n;
@@ -2593,23 +2662,29 @@ int cp_domain(cvxb_batch *b, int it) {
 // the i-th Newton direction of cpl (:966-1045): right-hand side, kktsolver_e's solve and `refinement` steps from
 // res() (:889-956), then the step to the boundary and the merit function's slope.  Without the epigraph row (EPI
 // false) there is no t to eliminate, and cpl's f4 is coneqp's: the right-hand side is k_dir_rhs's without the
-// Mehrotra term (its i = 0), then f4_no_ir around batch_solve and coneqp's refinement residual, 'q' cones included
-template <bool EQ, bool EPI = true, bool CONES = false> int gp_direction(cvxb_batch *b, int i) {
+// Mehrotra term (its i = 0), then f4_no_ir around batch_solve and coneqp's refinement residual, 'q' cones included.
+// SDP: the 's' blocks' parts of those are direction<..., SDP>'s (k_s_wtz, k_s_res, G' trisc(wz3)); then k_s_steps
+// forms their dz2 and ds2, and k_s_dir_post their scale2 and max_step, which in cpl keeps the eigenvectors and
+// eigenvalues after either direction (sigs is passed both times, :1042-1045), in syevd's order (k_s_sort)
+template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false> int gp_direction(cvxb_batch *b, int i) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, B = b->Bact, T = 256, pq = b->neq;
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     const long long L = b->L;
+    const dim3 sg(p.ns, B);
     if (EPI) k_gp_dir_rhs<<<B, T, 0, st>>>(p, g);
-    else k_dir_rhs<CONES, EQ, false><<<B, T, 0, st>>>(p, 0);
+    else k_dir_rhs<CONES, EQ, false, SDP><<<B, T, 0, st>>>(p, 0);
     count_launch();
+    if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.dz, m, p.ds, m, 2); count_launch(); }
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
     if (EPI) k_gp_f4_post<<<B, T, 0, st>>>(p, g, 0);
-    else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0);
+    else k_f4_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0);
     count_launch();
     for (int r = 0; r < p.refinement; ++r) {
+        if (SDP) { k_s_res<false><<<sg, SB_T, 0, st>>>(p); count_launch(); }
         if (EPI) k_gp_res<<<B, T, 0, st>>>(p, g);
-        else k_res<EQ, false><<<B, T, 0, st>>>(p);
+        else k_res<EQ, false, SDP><<<B, T, 0, st>>>(p);
         count_launch();
         GemvBatch gH; gH.batch = B; gH.sA = b->sP; gH.sx = n; gH.sy = L;                 // wx2 -= H dx
         CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gH));
@@ -2617,9 +2692,9 @@ template <bool EQ, bool EPI = true, bool CONES = false> int gp_direction(cvxb_ba
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
             CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
         }
-        if (m > 0) {                                     // wx2 -= [Df[1:]; G]' wz3[1:]
+        if (m > 0) {                                     // wx2 -= [Df[1:]; G]' wz3[1:]  (SDP: G' trisc(wz3))
             GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
-            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
         }
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
@@ -2632,17 +2707,24 @@ template <bool EQ, bool EPI = true, bool CONES = false> int gp_direction(cvxb_ba
         if (EPI) k_gp_f4_pre<<<B, T, 0, st>>>(p, g);
         else k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L);
         count_launch();
+        if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.wz2, L, p.ws2, L, 2); count_launch(); }
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
         if (EPI) k_gp_f4_post<<<B, T, 0, st>>>(p, g, 1);
-        else k_f4_post<EQ><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
+        else k_f4_post<EQ, SDP><<<B, T, 0, st>>>(p, p.wx2, L, p.wz2, L, p.ws2, L, 1);
         count_launch();
     }
-    k_gp_dir_post<EPI, CONES><<<B, T, 0, st>>>(p, g, i); count_launch();
+    if (SDP) {
+        k_s_steps<<<sg, SB_T, 0, st>>>(p, g.ds2, g.dz2); count_launch();
+        k_s_dir_post<<<sg, SB_T, 0, st>>>(p, 1); count_launch();
+        k_s_sort<<<sg, SB_T, 0, st>>>(p); count_launch();
+    }
+    k_gp_dir_post<EPI, CONES, SDP><<<B, T, 0, st>>>(p, g, i); count_launch();
     return 0;
 }
 // the lock-step line search after the i-th direction (:1125-1261): each round evaluates F and newrx at every
 // searching problem's trial point and takes its decision; one readback of the count still searching per round
-template <bool EQ, bool EPI = true, bool CONES = false> int gp_line_search(cvxb_batch *b, int i, int it) {
+template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false>
+int gp_line_search(cvxb_batch *b, int i, int it) {
     cudaStream_t st = b->st;
     const int B = b->Bact, T = 256;
     const Ptrs &p = b->p;
@@ -2650,9 +2732,9 @@ template <bool EQ, bool EPI = true, bool CONES = false> int gp_line_search(cvxb_
     for (int left = 1; left > 0; b->ls_rounds++) {
         k_gp_trial<<<B, T, 0, st>>>(p, g); count_launch();
         CVXB_TRY(cpl_eval_trial<EPI>(b));
-        CVXB_TRY((gp_rx<EQ, EPI>(b, g.nz, g.ny, g.nrx, false)));
+        CVXB_TRY((gp_rx<EQ, EPI, SDP>(b, g.nz, g.ny, g.nrx, false)));
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_gp_ls<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p, b->qs); count_launch();
+        k_gp_ls<EQ, EPI, CONES, SDP><<<B, T, 0, st>>>(p, g, i, it, b->d_ndone.p, b->qs); count_launch();
         CVXB_LAUNCH_CHECK();
         CVXB_TRY(read_count(b, left));
     }
@@ -2668,8 +2750,11 @@ int cpl_factor(cvxb_batch *b, bool first) {
 // cones when CONES).  A CP or cpl batch starts from its x0 and backtracks each step into dom f before the line search;
 // it calls back to the host, so the loop is never captured into a graph.  Without the epigraph row the scaling and
 // the update are coneqp's (k_scaling, k_update: cpl's compute_scaling, ssqr, update_scaling and unscaling are
-// coneqp's, and so is mu = gap / (mnl + ml + len(q)), :978)
-template <bool EQ, bool EPI = true, bool CONES = false>
+// coneqp's, and so is mu = gap / (mnl + ml + len(q)), :978).  SDP (a cpl batch with 's' blocks, which follow the 'q'
+// rows): the 's' parts of those are the SDP QP batch's, with k_s_nt_compute before iteration 0's scaling, sdot /
+// snrm2 / G' trisc(z) in the residuals and stopping rule, k_s_update before the update, and r, rti in the line
+// search's saved state; mu's degree counts each block's order
+template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false>
 int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double feastol) {
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
@@ -2686,7 +2771,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
     if (!b->cp)
         CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
                                     g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
-    k_gp_init<CONES><<<B, T, 0, st>>>(p, g); count_launch();
+    k_gp_init<CONES, SDP><<<B, T, 0, st>>>(p, g); count_launch();
     if (b->cp) {
         CVXB_CUDA(cudaMemcpyAsync(p.x, b->cpx0.p, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, st));
         CVXB_TRY(cp_upload_idx(b));
@@ -2698,7 +2783,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         // F(x, z[:mnl]) and the residuals (:627-691)
         CVXB_TRY(cpl_eval_full<EPI>(b));
         k_gp_res_begin<EQ, EPI><<<B, T, 0, st>>>(p, g); count_launch();
-        CVXB_TRY((gp_rx<EQ, EPI>(b, p.z, p.y, p.rx, true)));
+        CVXB_TRY((gp_rx<EQ, EPI, SDP>(b, p.z, p.y, p.rx, true)));
         if (EQ) {
             GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = pq;
             CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.x, 1.0, -1.0, p.ry, b->gemv_ws.p, st, ga));
@@ -2708,7 +2793,8 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
             CVXB_TRY(gemv_n(ml, n, g.G + g.mnl, g.ldg, nullptr, p.x, 1.0, 1.0, p.rz + g.mnl, b->gemv_ws.p, st, gl));
         }
         CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-        k_gp_stats<EQ, EPI><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
+        k_gp_stats<EQ, EPI, SDP><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p,
+                                                  b->d_done.p);
         count_launch();
         int ndone = 0, bad = 0;
         CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2728,8 +2814,9 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
                 CVXB_TRY(cpl_eval_full<EPI>(b));
             }
         }
+        if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
         if (EPI) k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0);
-        else k_scaling<CONES><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0);
+        else k_scaling<CONES, false, SDP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0);
         count_launch();
         if (it == 0) {                   // kkt_chol2's first call; still singular: the Rank ValueError (:778-783)
             CVXB_TRY(cpl_factor(b, true));
@@ -2738,23 +2825,26 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         } else {
             CVXB_TRY(cpl_factor(b, false));
             CVXB_CUDA(cudaMemsetAsync(b->d_ndone.p, 0, sizeof(int), st));
-            k_gp_singular<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p, b->qs); count_launch();
+            k_gp_singular<EQ, EPI, CONES, SDP><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 0, b->d_ndone.p, b->qs);
+            count_launch();
             int nre = 0;
             CVXB_TRY(read_count(b, nre));
-            if (nre > 0) {               // restored problems are factored again at their saved iterates
+            if (nre > 0) {               // restored problems are factored again at their saved iterates (and W)
                 CVXB_TRY(cpl_eval_full<EPI>(b));
                 CVXB_TRY(cpl_factor(b, false));
-                k_gp_singular<EQ, EPI, CONES><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p, b->qs);
+                k_gp_singular<EQ, EPI, CONES, SDP><<<B, T, 0, st>>>(p, g, b->d_info.p, it, 1, b->d_ndone.p, b->qs);
                 count_launch();
             }
         }
         for (int i = 0; i < 2; ++i) {
-            CVXB_TRY((gp_direction<EQ, EPI, CONES>(b, i)));
+            CVXB_TRY((gp_direction<EQ, EPI, CONES, SDP>(b, i)));
             if (b->cp) CVXB_TRY(cp_domain(b, it));
-            CVXB_TRY((gp_line_search<EQ, EPI, CONES>(b, i, it)));
+            CVXB_TRY((gp_line_search<EQ, EPI, CONES, SDP>(b, i, it)));
         }
+        // SDP: the step the line search left, with sigs and sigz of the last direction (not restored on a resume)
+        if (SDP) { k_s_update<EQ><<<dim3(p.ns, B), SB_T, 0, st>>>(p, b->d_info.p, it == 0); count_launch(); }
         if (EPI) k_gp_update<<<B, T, 0, st>>>(p, g);
-        else k_update<CONES, EQ><<<B, T, 0, st>>>(p, b->d_info.p, it);
+        else k_update<CONES, EQ, false, SDP><<<B, T, 0, st>>>(p, b->d_info.p, it);
         count_launch();
         CVXB_LAUNCH_CHECK();
     }
@@ -2980,11 +3070,11 @@ int load_common(cvxb_batch *b, const double *q, const double *G, const double *h
 
 // the common part of a GP, a CP and a cpl batch: a QP batch whose 'l' rows begin with the mnl nonlinear rows (d.ml
 // counts them), nK = mnl + 1 nonlinear rows of f (a cpl batch's nK = mnl) with sumK rows of F below the m rows of G,
-// and gq's per-slot vectors
+// and gq's per-slot vectors.  sdp: d may hold 's' blocks, after the 'q' rows
 int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, long long sumK, const cvxb_dims &d,
-               int p, int device) {
+               int p, int device, bool sdp = false) {
     cvxb_batch *raw = nullptr;
-    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, false, (int)sumK));
+    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, sdp, (int)sumK));
     b.reset(raw);
     const size_t B = nprob, m = b->m;
     GPPtrs &g = b->gq;
@@ -3026,8 +3116,8 @@ int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyK
 // a batch with the caller's F: CP (the epigraph problem, nK = mnl + 1) or cpl (nK = mnl, 'q' cones in d): the
 // callback's buffers, x0 and the slot -> problem map; refinement 1, cpl's default (cvxprog.py:422)
 int create_cp_common(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, const cvxb_dims &d, int p,
-                     int device) {
-    CVXB_TRY(create_cpl(b, nprob, n, mnl, nK, 0, d, p, device));
+                     int device, bool sdp = false) {
+    CVXB_TRY(create_cpl(b, nprob, n, mnl, nK, 0, d, p, device, sdp));
     const size_t B = nprob, nn = n;
     // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
     const size_t len = 2 * nK + nK * nn + nn * nn;
@@ -3042,6 +3132,56 @@ int create_cp_common(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, 
     b->cp = true;
     b->p.refinement = 1;
     return state_alloc(b.get());
+}
+
+// cvxb_batch_create_cpl (sdp false: 's' cones are CVXB_E_UNSUP) and cvxb_batch_create_sdp_cpl (sdp: 's' blocks of
+// order at most CVXB_BATCH_SMAX after the 'q' rows); every refusal comes before the device
+int create_cpl_batch(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device, bool sdp) {
+    const char *fn = sdp ? "batch_create_sdp_cpl" : "batch_create_cpl";
+    if (out) *out = nullptr;
+    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || p < 0 || !dims) {
+        set_error("%s: bad sizes (nprob in 1..%d, n >= 1, mnl and p nonnegative, dims given)", fn, CVXB_BATCH_MAX);
+        return CVXB_E_ARG;
+    }
+    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
+        set_error("%s: bad dims (its mnl must be 0; ml and the cone counts nonnegative)", fn);
+        return CVXB_E_ARG;
+    }
+    if (dims->ns > 0 && !sdp) {
+        set_error("batch_create_cpl: 's' cones are not supported by the cpl batch");
+        return CVXB_E_UNSUP;
+    }
+    long long m = (long long)mnl + dims->ml;
+    for (int k = 0; k < dims->nq; ++k) {
+        if (dims->q[k] < 1) { set_error("%s: dims['q'][%d] = %d < 1", fn, k, dims->q[k]); return CVXB_E_ARG; }
+        m += dims->q[k];
+    }
+    if (dims->ns > 0 && !dims->s) { set_error("%s: dims has ns > 0 and no 's' orders", fn); return CVXB_E_ARG; }
+    for (int k = 0; k < dims->ns; ++k) {
+        const int s = dims->s[k];
+        if (s < 0) { set_error("%s: dims['s'][%d] = %d < 0", fn, k, s); return CVXB_E_ARG; }
+        if (s > CVXB_BATCH_SMAX) {
+            set_error("%s: dims['s'][%d] = %d > %d, the largest 's' order of the batch", fn, k, s, CVXB_BATCH_SMAX);
+            return CVXB_E_UNSUP;
+        }
+        m += (long long)s * s;
+    }
+    if (m == 0) {                                     // cpl's theta1 = 1 / gap0 (cvxprog.py:717) needs a row
+        set_error("%s: no constraint rows (mnl + cdim = 0)", fn);
+        return CVXB_E_ARG;
+    }
+    if (m > (1LL << 30)) { set_error("%s: too many rows", fn); return CVXB_E_ARG; }
+    if (p > n) {                                      // cpl's check before the first factorisation
+        set_error("%s: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", fn, p, n);
+        return CVXB_E_ARG;
+    }
+    std::unique_ptr<cvxb_batch> b;
+    cvxb_dims d = *dims;
+    d.ml += mnl;
+    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl, d, p, device, sdp));
+    b->cpl = true;
+    *out = b.release();
+    return 0;
 }
 
 }  // namespace
@@ -3129,38 +3269,11 @@ int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, in
 }
 
 int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
-    if (out) *out = nullptr;
-    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || p < 0 || !dims) {
-        set_error("batch_create_cpl: bad sizes (nprob in 1..%d, n >= 1, mnl and p nonnegative, dims given)",
-                  CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("batch_create_cpl: bad dims (its mnl must be 0; ml and the cone counts nonnegative)");
-        return CVXB_E_ARG;
-    }
-    if (dims->ns > 0) { set_error("batch_create_cpl: 's' cones are not supported by the cpl batch"); return CVXB_E_UNSUP; }
-    long long m = (long long)mnl + dims->ml;
-    for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("batch_create_cpl: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
-        m += dims->q[k];
-    }
-    if (m == 0) {                                     // cpl's theta1 = 1 / gap0 (cvxprog.py:717) needs a row
-        set_error("batch_create_cpl: no constraint rows (mnl + cdim = 0)");
-        return CVXB_E_ARG;
-    }
-    if (m > (1LL << 30)) { set_error("batch_create_cpl: too many rows"); return CVXB_E_ARG; }
-    if (p > n) {                                      // cpl's check before the first factorisation
-        set_error("batch_create_cpl: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", p, n);
-        return CVXB_E_ARG;
-    }
-    std::unique_ptr<cvxb_batch> b;
-    cvxb_dims d = *dims;
-    d.ml += mnl;
-    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl, d, p, device));
-    b->cpl = true;
-    *out = b.release();
-    return 0;
+    return create_cpl_batch(out, nprob, n, mnl, dims, p, device, false);
+}
+
+int cvxb_batch_create_sdp_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
+    return create_cpl_batch(out, nprob, n, mnl, dims, p, device, true);
 }
 
 int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx) {
@@ -3307,7 +3420,11 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
         using Solve = int (*)(cvxb_batch *, int, double, double, double);
         static const Solve cpl_solvers[4] = {solve_cpl<false, false, false>, solve_cpl<true, false, false>,
                                              solve_cpl<false, false, true>, solve_cpl<true, false, true>};
-        return cpl_solvers[(b->neq > 0 ? 1 : 0) + (b->p.nq > 0 ? 2 : 0)](b, maxiters, abstol, reltol, feastol);
+        static const Solve sdp_cpl_solvers[4] = {solve_cpl<false, false, false, true>, solve_cpl<true, false, false, true>,
+                                                 solve_cpl<false, false, true, true>, solve_cpl<true, false, true, true>};
+        const int k = (b->neq > 0 ? 1 : 0) + (b->p.nq > 0 ? 2 : 0);
+        if (b->p.ns > 0) return sdp_cpl_solvers[k](b, maxiters, abstol, reltol, feastol);   // 's' blocks of positive order
+        return cpl_solvers[k](b, maxiters, abstol, reltol, feastol);
     }
     if (b->gp || b->cp) return b->neq > 0 ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
                                           : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);

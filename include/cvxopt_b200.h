@@ -477,6 +477,23 @@ int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvx
  * nprob x cdim ('l' rows, then each 'q' cone); G and h may be NULL when cdim = 0.  A and b come through
  * cvxb_batch_load_eq. */
 int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const double *G, const double *h, int space);
+/* batch of cpl problems whose dims may hold 's' blocks (B x solvers.cpl(c, F, G, h, dims, A, b) with an LMI), each
+ * 's' order at most CVXB_BATCH_SMAX:
+ *     minimize  c'x  s.t.  fk(x) <= 0 (k = 1..mnl),  G x + s = h,  s in 'l' x 'q' x 's' cones,  A x = b
+ * It refuses, before the device, what cvxb_batch_create_cpl refuses except dims->ns > 0, and an order s[k] < 0
+ * (CVXB_E_ARG) or s[k] > CVXB_BATCH_SMAX (CVXB_E_UNSUP); the 's' rows count as constraint rows.  An order-0 block adds
+ * no rows.  It is the cpl batch in every call: cvxb_batch_load_cpl (G and h rows: 'l', each 'q' cone, then each 's'
+ * block unpacked, s[k]^2 rows column-major as the reference's G; only the lower triangle of an 's' block of G and h is
+ * read), cvxb_batch_load_eq, set_cp_eval, solve, results (s and z with symmetric 's' blocks), results_y, stats,
+ * ls_rounds and destroy.  It starts from s = z = e (the identity in each 's' block).  Device memory per problem, in
+ * doubles, with S = sum(s^2) over the blocks and ev() rounding up to even: that of the cvxb_batch_create_cpl batch of
+ * the same n, mnl and p with dims {'l': ml + S, 'q': q} (the same m = mnl + cdim rows), plus ldg*n for Gs if dims has
+ * no 'q' cone, 2 ev(S) + 2 ev(sum s) (r, rti, sigs, sigz) and 2 ev(S) (the line search's saved r and rti) in the state
+ * row, with 'q' cones 2 (ev(sum q + S) - ev(sum q)) more there (v and the saved v span the blocks' rows), and 4 per
+ * block of partial sums; and, shared by the batch, m doubles of row weights and S + 5 nb ints of layout, nb the number
+ * of blocks of positive order; all of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy.  Dims
+ * without an 's' block of positive order run exactly what cvxb_batch_create_cpl's batch runs. */
+int cvxb_batch_create_sdp_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device);
 
 #ifdef __cplusplus
 }
