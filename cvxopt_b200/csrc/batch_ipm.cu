@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <vector>
 #include <memory>
+#include <type_traits>
 
 using namespace cvxb;
 
@@ -2011,9 +2012,17 @@ __global__ void k_cp_dom(Ptrs p, GPPtrs g, CPPtrs c, int iter, int *nsearch) {
         else atomicAdd(nsearch, 1);
     }
 }
+
+// the problem family of a batch: coneqp, conelp, gp, cp or cpl
+enum class Kind { QP, LP, GP, CP, CPL };
 }  // namespace
 
 struct cvxb_batch {
+    Kind kind = Kind::QP;
+    // GP, CP and cpl batches run the lock-step cpl (solve_cpl) with gq's per-slot state
+    bool cpl_loop() const { return kind == Kind::GP || kind == Kind::CP || kind == Kind::CPL; }
+    // CP and cpl batches evaluate the caller's F through cfn, which calls back to the host
+    bool calls_back() const { return kind == Kind::CP || kind == Kind::CPL; }
     int device = 0, B = 0, n = 0, m = 0;
     long long ldg = 0, ldp = 0, ldk = 0;
     long long sG = 0, sP = 0, sK = 0, sInv = 0;
@@ -2055,7 +2064,6 @@ struct cvxb_batch {
     bool eq_loaded = false;          // cvxb_batch_load_eq since the last cvxb_batch_load
     bool switched = false;           // some problem of this solve factors S + A'A (its aw is 1)
     // cone LP batch (cvxb_batch_create_lp): no P; q holds c; lpv holds x1 (n), z1 and th (m), y1 (p) per slot
-    bool lp = false;
     DevBuf<double> lpv;
     // 's' blocks (cvxb_batch_create_sdp): p.ns blocks of positive order; Gs has mpk = cdim_pckd rows
     int mpk = 0;
@@ -2070,21 +2078,18 @@ struct cvxb_batch {
     // geometric programs (cvxb_batch_create_gp): m = mnl + ml rows, G holds [Df[1:]; G; F] (ld ldg = m + sum K rounded
     // up to even), P holds H; gq's per-slot vectors live in gpv, H's scaled rows in gph, the block offsets in koff and
     // g, in problem order, in gpg (copied into the state row by each solve)
-    bool gp = false;
     GPPtrs gq{};
     DevBuf<double> gpv, gph, gpg;
     DevBuf<int> koff;
     // convex programs (cvxb_batch_create_cp): gq of a GP batch without F (sum K = 0, nK = mnl + 1); the callback's
     // buffers in cpv, x0 in problem order in cpx0, slot -> load index and the non-finite flag in cpi
-    bool cp = false;
     CPPtrs cq{};
     DevBuf<double> cpv, cpx0;
     DevBuf<int> cpi;
     cvxb_cp_eval_fn cfn = nullptr;
     void *cctx = nullptr;
-    // cpl batches (cvxb_batch_create_cpl): a CP batch (cp is set) of cpl's own problem, without the epigraph row: nK =
-    // mnl, c in q, 'q' cones after the 'l' rows; qs: the relaxed line search's saved v and beta with cones
-    bool cpl = false;
+    // cpl batches (cvxb_batch_create_cpl): a CP batch of cpl's own problem, without the epigraph row: nK = mnl, c in
+    // q, 'q' cones after the 'l' rows; qs: the relaxed line search's saved v and beta with cones
     QSave qs{};
     ~cvxb_batch() {                  // synchronises the stream, then releases it and the events
         if (st) cudaStreamSynchronize(st);
@@ -2102,11 +2107,11 @@ int state_alloc(cvxb_batch *b) {
     auto ev = [](long long x) { return (x + 1) & ~1LL; };
     const long long sumq = b->m - p.ml, n2 = ev(b->n), m2 = ev(b->m), p2 = ev(b->neq);
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
-    const long long lps = b->lp ? ev(sizeof(LPScal) / sizeof(double)) : 0;
+    const long long lps = b->kind == Kind::LP ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
     // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m), and with
     // cones v0 (sum q) | beta0 (nq), with 's' blocks r0 rti0 (sum s²)
-    const long long gpl = b->gp || b->cp ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
+    const long long gpl = b->cpl_loop() ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
     const long long qsv = gpl ? cone : 0, ssv = gpl && p.ns ? 2 * ev(b->sums2) : 0;
     const long long L = cone + sb + ref + lps + gpl + qsv + ssv;
     if (b->L == L) return 0;
@@ -2256,6 +2261,37 @@ int batch_solve(cvxb_batch *b, double *x, long long sx, double *y = nullptr, lon
     return 0;
 }
 
+// the GEMVs of a refinement step's residual, res() (coneprog.py:1930-1952, :599-631; cvxprog.py:889-956):
+// wx2 -= P dx + A' dy + G' wz3, wy2 -= A dx, wz2 -= G dx.  SDP: G' trisc(wz3) (misc.sgemv).  An LP has no P; in a GP,
+// CP or cpl batch P holds H and G holds [Df; G]
+template <bool EQ, bool LP, bool SDP> int refinement_gemvs(cvxb_batch *b) {
+    cudaStream_t st = b->st;
+    const int n = b->n, m = b->m, B = b->Bact, pq = b->neq;
+    const Ptrs &p = b->p;
+    const long long L = b->L;
+    if (!LP) {
+        GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
+        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
+    }
+    if (EQ) {
+        GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
+        CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
+    }
+    if (m > 0) {
+        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
+        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
+    }
+    if (EQ) {
+        GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
+        CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
+    }
+    if (m > 0) {
+        GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
+        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
+    }
+    return 0;
+}
+
 // the i-th Newton direction: coneqp's f4 (coneprog.py:2288-2347) or, LP, conelp's f6 (:1211-1235) on the right-hand
 // side, i.e. the unrefined solve and then `refinement` correction steps from the residual, followed by the step
 // length and sigma
@@ -2273,26 +2309,10 @@ template <bool CONES, bool EQ, bool LP, bool SDP = false> int direction(cvxb_bat
     if (LP) { k_lp_f6_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dy, pq, p.ds, m, 0); count_launch(); }
     else if (p.refinement || SDP) { k_f4_post<EQ, SDP><<<B, T, 0, st>>>(p, p.dx, n, p.dz, m, p.ds, m, 0); count_launch(); }
     for (int r = 0; r < p.refinement; ++r) {
-        // res() (coneprog.py:1930-1952, :599-631): wx2 -= P dx + A' dy + G' W^{-1} dz, wy2 -= A dx,
-        // wz2 -= G dx + W' ds; an LP has no P
+        // res(): its elementwise part, then the GEMVs
         if (SDP) { k_s_res<LP><<<sg, SB_T, 0, st>>>(p); count_launch(); }
         k_res<EQ, LP, SDP><<<B, T, 0, st>>>(p); count_launch();
-        if (!LP) {
-            GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = L;
-            CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gP));
-        }
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
-            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
-        }
-        GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;      // SDP: G' trisc(wz3) (misc.sgemv)
-        CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
-            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
-        }
-        GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
-        CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
+        CVXB_TRY((refinement_gemvs<EQ, LP, SDP>(b)));
         k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L); count_launch();
         if (SDP) { k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.wz2, L, p.ws2, L, 2); count_launch(); }
         CVXB_TRY(batch_solve(b, p.wx2, L, p.wy2, L));
@@ -2365,9 +2385,18 @@ template <bool EQ> int start_factor(cvxb_batch *b) {
     return first_switch<EQ>(b);
 }
 
-// a singular first factorisation is the reference's "Rank(A) < p or Rank([P; A; G]) < n" ValueError
-// (coneprog.py:2065-2067), without A Rank([P; G]) < n; conelp's is "Rank(A) < p or Rank([G; A]) < n" (:680-700).
-// After a loaded start the first factorisation is iteration 0's (:2256-2259, :1078-1080), over the active slots
+// the rank condition of the reference's ValueError for a singular KKT matrix: coneqp's "Rank(A) < p or Rank([P; A;
+// G]) < n" (coneprog.py:2065-2067), without A "Rank([P; G]) < n"; conelp's (:680-700); cp's and cpl's (cvxprog.py)
+const char *rank_text(Kind kind, bool eq) {
+    switch (kind) {
+    case Kind::QP: return eq ? "Rank(A) < p or Rank([P; A; G]) < n" : "Rank([P; G]) < n";
+    case Kind::LP: return "Rank(A) < p or Rank([G; A]) < n";
+    default: return "Rank(A) < p or Rank([H(x); A; Df(x); G]) < n";
+    }
+}
+
+// a singular first factorisation is the reference's rank ValueError.  After a loaded start the first factorisation
+// is iteration 0's (coneprog.py:2256-2259, :1078-1080), over the active slots
 template <bool EQ> int start_check(cvxb_batch *b) {
     cudaStream_t st = b->st;
     const int B = b->Bact;
@@ -2377,14 +2406,8 @@ template <bool EQ> int start_check(cvxb_batch *b) {
     CVXB_CUDA(cudaStreamSynchronize(st));
     for (int i = 0; i < B; ++i)
         if (info[i] > 0 || (EQ && infop[i] > 0)) {
-            const int k = b->perm[i];
-            if (b->gp || b->cp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n "
-                                          "(singular KKT matrix at the start)", k);
-            else if (b->lp) set_error("batch_solve: problem %d: Rank(A) < p or Rank([G; A]) < n (singular KKT matrix at "
-                                 "the start)", k);
-            else if (EQ) set_error("batch_solve: problem %d: Rank(A) < p or Rank([P; A; G]) < n (singular KKT matrix "
-                                   "at the start)", k);
-            else set_error("batch_solve: problem %d: Rank([P; G]) < n (singular KKT matrix at the start)", k);
+            set_error("batch_solve: problem %d: %s (singular KKT matrix at the start)", b->perm[i],
+                      rank_text(b->kind, EQ));
             return CVXB_E_ARG;
         }
     return 0;
@@ -2447,6 +2470,51 @@ int compact_slots(cvxb_batch *b, int B, int ndone, const std::vector<int> &flags
     return 0;
 }
 
+// one int of the device counter d_ndone, after the stream has drained
+int read_count(cvxb_batch *b, int &v) {
+    CVXB_CUDA(cudaMemcpyAsync(&v, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    return 0;
+}
+
+// the lock-step loops' scaffold.  solve_begin: every slot active, no problem switched, zero per-slot scalars, and the
+// timing starts
+int solve_begin(cvxb_batch *b) {
+    b->Bact = b->B;
+    b->switched = false;
+    b->ls_rounds = 0;
+    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)b->B * sizeof(Scal), b->st));
+    CVXB_CUDA(cudaEventRecord(b->e0, b->st));
+    return 0;
+}
+// the done-poll once the stopping rule has counted the finished slots in d_ndone and flagged them in d_done: one sync
+// reads both, and with bad also cq.bad (the first problem whose f is not finite; b->B for none).  Unless every active
+// slot is done or bad names a problem, finished slots then leave the active range (compact_slots, b->Bact); moved
+// says whether any slots traded places
+int poll_done(cvxb_batch *b, std::vector<int> &flags, std::vector<int> &pairs, int &ndone, bool &moved,
+              int *bad = nullptr) {
+    const int B = b->Bact;
+    moved = false;
+    CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, b->st));
+    if (bad) CVXB_CUDA(cudaMemcpyAsync(bad, b->cq.bad, sizeof(int), cudaMemcpyDeviceToHost, b->st));
+    CVXB_TRY(read_count(b, ndone));
+    if (ndone >= B || ndone == 0 || (bad && *bad < b->B) || !b->compact || b->B == 1) return 0;
+    CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
+    moved = !pairs.empty();
+    return 0;
+}
+// solve_end after `it` iterations: the results cover every slot again, and the solve's time
+int solve_end(cvxb_batch *b, int it) {
+    b->iters_run = it;
+    b->Bact = b->B;
+    CVXB_CUDA(cudaEventRecord(b->e1, b->st));
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    float t = 0;
+    cudaEventElapsedTime(&t, b->e0, b->e1);
+    b->solve_ms = t;
+    return 0;
+}
+
 // the lock-step IPM over the active slots; CONES: the batch has 'q' cones, EQ: equality rows.  LP: coneprog.conelp
 // (coneprog.py:662-1436) on a batch without P: the self-dual embedding's tau and kappa, one more KKT solve per
 // iteration for (x1, y1, z1), and infeasibility certificates
@@ -2455,16 +2523,13 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
     cudaStream_t st = b->st;
     const int n = b->n, m = b->m, T = 256, pq = b->neq;
     int B = b->B;                                 // active slots: shrinks as problems finish (compaction)
-    b->Bact = B;
-    b->switched = false;
     const Ptrs &p = b->p;
     GemvBatch gP; gP.batch = B; gP.sA = b->sP; gP.sx = n; gP.sy = n;
     GemvBatch gGt; gGt.batch = B; gGt.sA = b->sG; gGt.sx = m; gGt.sy = n;
     GemvBatch gGn; gGn.batch = B; gGn.sA = b->sG; gGn.sx = n; gGn.sy = m;
     GemvBatch gAt; gAt.batch = B; gAt.sA = b->sA; gAt.sx = pq; gAt.sy = n;
     GemvBatch gAn; gAn.batch = B; gAn.sA = b->sA; gAn.sx = n; gAn.sy = pq;
-    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
-    CVXB_CUDA(cudaEventRecord(b->e0, st));
+    CVXB_TRY(solve_begin(b));
     // ---- starting point: W = I (coneqp :2055-2106, conelp :662-857) ----
     k_init_rhs<EQ, SDP><<<B, T, 0, st>>>(p); count_launch();  // dx = -q, y = b, dz = h, resx0 / resy0 / resz0
     // a loaded start (coneqp's cdim == 0 branch, :2002, ignores it); firstcall: iteration 0's factorisation is the first
@@ -2516,20 +2581,15 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
         else k_stats<EQ, SDP><<<B, T, 0, st>>>(p, it, maxiters, abstol, reltol, feastol, b->d_ndone.p, b->d_done.p);
         count_launch();
         int ndone = 0;
-        CVXB_CUDA(cudaMemcpyAsync(&ndone, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_CUDA(cudaStreamSynchronize(st));
+        bool moved = false;
+        CVXB_TRY(poll_done(b, flags, pairs, ndone, moved));
         if (ndone >= B) break;
-        if (ndone > 0 && b->compact && b->B > 1) {
-            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
-            B = b->Bact;
-            gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
-        }
+        B = b->Bact;
+        gP.batch = gGt.batch = gGn.batch = gAt.batch = gAn.batch = B;
         if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
         k_scaling<CONES, LP, SDP><<<B, T, 0, st>>>(p, it == 0 ? 1 : 0); count_launch();
         if (firstcall && it == 0) {              // kkt_chol2's first call; still singular: the Rank ValueError
-            CVXB_TRY(batch_factor(b, false));
-            CVXB_TRY(first_switch<EQ>(b));
+            CVXB_TRY(start_factor<EQ>(b));
             CVXB_TRY(start_check<EQ>(b));
         } else CVXB_TRY(batch_factor(b));
         if (LP) {
@@ -2544,14 +2604,7 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
         k_update<CONES, EQ, LP, SDP><<<B, T, 0, st>>>(p, b->d_info.p, it); count_launch();
         CVXB_LAUNCH_CHECK();
     }
-    b->iters_run = it;
-    b->Bact = b->B;
-    CVXB_CUDA(cudaEventRecord(b->e1, st));
-    CVXB_CUDA(cudaStreamSynchronize(st));
-    float t = 0;
-    cudaEventElapsedTime(&t, b->e0, b->e1);
-    b->solve_ms = t;
-    return 0;
+    return solve_end(b, it);
 }
 
 // ---- geometric programs: the lock-step cpl (cvxprog.py:622-1356) of gp's epigraph problem ----
@@ -2573,7 +2626,7 @@ template <bool EQ, bool EPI = true, bool SDP = false>
 int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
-    if (!b->cp) {
+    if (!b->calls_back()) {
         GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
         CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
     } else if (full) {
@@ -2605,12 +2658,6 @@ int gp_hessian(cvxb_batch *b) {
     if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, b->st));
     return 0;
 }
-// one int of the device counter d_ndone, after the stream has drained
-int read_count(cvxb_batch *b, int &v) {
-    CVXB_CUDA(cudaMemcpyAsync(&v, b->d_ndone.p, sizeof(int), cudaMemcpyDeviceToHost, b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    return 0;
-}
 // the caller's F over the active slots at x (slot k at x + k*n); full: at the iterates, with z = [z0; z[:mnl]] and H
 int cp_call(cvxb_batch *b, const double *x, bool full) {
     const CPPtrs &c = b->cq;
@@ -2622,7 +2669,7 @@ int cp_call(cvxb_batch *b, const double *x, bool full) {
 // F(x, z[:mnl]) at the iterates: f into fv, grad f0 into gf0, Df[1:] into G's rows [0, mnl); CP also H into P
 // (GP forms H in gp_hessian).  EPI false (a cpl batch): Df[:mnl] into G's rows [0, mnl)
 template <bool EPI = true> int cpl_eval_full(cvxb_batch *b) {
-    if (!b->cp) return gp_eval(b, b->p.x, b->n, true, 0);
+    if (!b->calls_back()) return gp_eval(b, b->p.x, b->n, true, 0);
     const int B = b->Bact;
     k_cp_zpack<EPI><<<B, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
     CVXB_TRY(cp_call(b, b->p.x, true));
@@ -2633,7 +2680,7 @@ template <bool EPI = true> int cpl_eval_full(cvxb_batch *b) {
 // F at the line search's trial points g.nx, for the problems still searching: f into fv; CP also newrx's nonlinear
 // part into nrx (EPI false: c + Df'newznl)
 template <bool EPI = true> int cpl_eval_trial(cvxb_batch *b) {
-    if (!b->cp) return gp_eval(b, b->gq.nx, b->n, false, 1);
+    if (!b->calls_back()) return gp_eval(b, b->gq.nx, b->n, false, 1);
     CVXB_TRY(cp_call(b, b->gq.nx, false));
     k_cp_take<false, EPI><<<b->Bact, 256, 0, b->st>>>(b->p, b->gq, b->cq); count_launch();
     return 0;
@@ -2686,24 +2733,7 @@ template <bool EQ, bool EPI = true, bool CONES = false, bool SDP = false> int gp
         if (EPI) k_gp_res<<<B, T, 0, st>>>(p, g);
         else k_res<EQ, false, SDP><<<B, T, 0, st>>>(p);
         count_launch();
-        GemvBatch gH; gH.batch = B; gH.sA = b->sP; gH.sx = n; gH.sy = L;                 // wx2 -= H dx
-        CVXB_TRY(gemv_t(n, n, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.wx2, st, gH));
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = pq; ga.sy = L;
-            CVXB_TRY(gemv_t(pq, n, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.wx2, st, ga));
-        }
-        if (m > 0) {                                     // wx2 -= [Df[1:]; G]' wz3[1:]  (SDP: G' trisc(wz3))
-            GemvBatch gt; gt.batch = B; gt.sA = b->sG; gt.sx = L; gt.sy = L;
-            CVXB_TRY(gemv_t(m, n, b->G.p, b->ldg, SDP ? p.rw : nullptr, p.wz3, -1.0, 1.0, p.wx2, st, gt));
-        }
-        if (EQ) {
-            GemvBatch ga; ga.batch = B; ga.sA = b->sA; ga.sx = n; ga.sy = L;
-            CVXB_TRY(gemv_n(pq, n, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.wy2, b->gemv_ws.p, st, ga));
-        }
-        if (m > 0) {                                     // wz2[1:] -= [Df[1:]; G] dx
-            GemvBatch gn; gn.batch = B; gn.sA = b->sG; gn.sx = n; gn.sy = L;
-            CVXB_TRY(gemv_n(m, n, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.wz2, b->gemv_ws.p, st, gn));
-        }
+        CVXB_TRY((refinement_gemvs<EQ, false, SDP>(b)));     // with the epigraph row: G's rows are [Df[1:]; G]
         if (EPI) k_gp_f4_pre<<<B, T, 0, st>>>(p, g);
         else k_f4_pre<<<B, T, 0, st>>>(p, p.wz2, L, p.ws2, L);
         count_launch();
@@ -2743,7 +2773,7 @@ int gp_line_search(cvxb_batch *b, int i, int it) {
 // K = H + [Df[1:]; G]' diag(di²) [Df[1:]; G] (+ A'A) factored from F(x) at the slots' iterates (a GP's H formed
 // into P first; a CP's is there from cpl_eval_full)
 int cpl_factor(cvxb_batch *b, bool first) {
-    if (!b->cp) CVXB_TRY(gp_hessian(b));
+    if (!b->calls_back()) CVXB_TRY(gp_hessian(b));
     return batch_factor(b, !first);
 }
 // the lock-step cpl of a GP or CP batch's epigraph problem (EPI) or of a cpl batch's own problem (EPI false, with 'q'
@@ -2761,18 +2791,15 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     const int ml = m - g.mnl;
+    const bool cb = b->calls_back();
     int B = b->B;
-    b->Bact = B;
-    b->switched = false;
-    b->ls_rounds = 0;
-    CVXB_CUDA(cudaMemsetAsync(b->sc.p, 0, (size_t)B * sizeof(Scal), st));
-    CVXB_CUDA(cudaEventRecord(b->e0, st));
+    CVXB_TRY(solve_begin(b));
     // every problem in its own slot (restore_order ran): g into the state row, or x0 into x
-    if (!b->cp)
+    if (!cb)
         CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
                                     g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
     k_gp_init<CONES, SDP><<<B, T, 0, st>>>(p, g); count_launch();
-    if (b->cp) {
+    if (cb) {
         CVXB_CUDA(cudaMemcpyAsync(p.x, b->cpx0.p, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, st));
         CVXB_TRY(cp_upload_idx(b));
         CVXB_CUDA(cudaMemsetAsync(b->cq.bad, 0x7f, sizeof(int), st));
@@ -2796,23 +2823,19 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         k_gp_stats<EQ, EPI, SDP><<<B, T, 0, st>>>(p, g, it, maxiters, abstol, reltol, feastol, b->d_ndone.p,
                                                   b->d_done.p);
         count_launch();
-        int ndone = 0, bad = 0;
-        CVXB_CUDA(cudaMemcpyAsync(flags.data(), b->d_done.p, (size_t)B * sizeof(int), cudaMemcpyDeviceToHost, st));
-        if (b->cp) CVXB_CUDA(cudaMemcpyAsync(&bad, b->cq.bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CVXB_TRY(read_count(b, ndone));
-        if (b->cp && bad < b->B) {       // the reference keeps its iterates inside dom f
+        int ndone = 0, bad = b->B;
+        bool moved = false;
+        CVXB_TRY(poll_done(b, flags, pairs, ndone, moved, cb ? &bad : nullptr));
+        if (bad < b->B) {                // the reference keeps its iterates inside dom f
             if (it == 0) set_error("batch_solve: problem %d: x0 not in the domain of f", bad);
             else set_error("batch_solve: problem %d: f is not finite at the iterate of iteration %d", bad, it);
             return CVXB_E_ARG;
         }
         if (ndone >= B) break;
-        if (ndone > 0 && b->compact && b->B > 1) {
-            CVXB_TRY(compact_slots(b, B, ndone, flags, pairs));
-            B = b->Bact;
-            if (!pairs.empty()) {        // F(x)'s per-slot results stay put
-                if (b->cp) CVXB_TRY(cp_upload_idx(b));
-                CVXB_TRY(cpl_eval_full<EPI>(b));
-            }
+        B = b->Bact;
+        if (moved) {                     // F(x)'s per-slot results stay put
+            if (cb) CVXB_TRY(cp_upload_idx(b));
+            CVXB_TRY(cpl_eval_full<EPI>(b));
         }
         if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
         if (EPI) k_gp_scaling<<<B, T, 0, st>>>(p, g, it == 0 ? 1 : 0);
@@ -2838,7 +2861,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         }
         for (int i = 0; i < 2; ++i) {
             CVXB_TRY((gp_direction<EQ, EPI, CONES, SDP>(b, i)));
-            if (b->cp) CVXB_TRY(cp_domain(b, it));
+            if (cb) CVXB_TRY(cp_domain(b, it));
             CVXB_TRY((gp_line_search<EQ, EPI, CONES, SDP>(b, i, it)));
         }
         // SDP: the step the line search left, with sigs and sigz of the last direction (not restored on a resume)
@@ -2848,14 +2871,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         count_launch();
         CVXB_LAUNCH_CHECK();
     }
-    b->iters_run = it;
-    b->Bact = b->B;
-    CVXB_CUDA(cudaEventRecord(b->e1, st));
-    CVXB_CUDA(cudaStreamSynchronize(st));
-    float t = 0;
-    cudaEventElapsedTime(&t, b->e0, b->e1);
-    b->solve_ms = t;
-    return 0;
+    return solve_end(b, it);
 }
 
 // dst[problem] = src[slot] for a [B x len] per-slot array, through the slot permutation (d_perm, uploaded by the
@@ -2875,64 +2891,73 @@ int give_rows(cvxb_batch *b, double *dst, const double *src, int len, int space)
     return 0;
 }
 
-// a batch of QPs, or of cone LPs (lp: no P; q holds c), with the cones of dims ('l' and 'q', and with sdp 's' blocks)
-// and p equality rows.  Every argument is checked before the device is.
-// xrows > 0 (a GP batch): G gets xrows more rows below the m cone rows, for F
-int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device, bool lp, bool sdp = false,
-           int xrows = 0) {
+// every refusal of a creator's arguments, all before the device (fn names the creator): the sizes, the dims of the
+// cone rows, which the mnl rows of f precede, and the rank checks before the first factorisation: coneqp's
+// (coneprog.py:1962), conelp's (:572-573, with cdim_pckd), cp's and cpl's.  Counts G's rows: mlq 'l' and 'q' rows
+// (mnl included), m = mlq + the 's' blocks' s², and mpk = mlq + their s (s + 1) / 2 (cdim_pckd)
+int check_args(const char *fn, Kind kind, cvxb_batch **out, int nprob, int n, int p, int mnl, const cvxb_dims *dims,
+               bool sdp, long long &mlq, long long &m, long long &mpk) {
     if (out) *out = nullptr;
-    if (!out || nprob <= 0 || n <= 0 || !dims) {
-        set_error("batch_create: bad sizes (nprob and n positive, dims given)");
+    if (!out || nprob < 1 || n < 1 || mnl < 0 || !dims) {
+        set_error("%s: bad sizes (nprob and n positive, mnl nonnegative, dims given)", fn);
         return CVXB_E_ARG;
     }
-    if (p < 0) { set_error("batch_create: bad sizes (p must be nonnegative)"); return CVXB_E_ARG; }
+    if (p < 0) { set_error("%s: bad sizes (p must be nonnegative)", fn); return CVXB_E_ARG; }
     if (nprob > CVXB_BATCH_MAX) {
-        set_error("batch_create: nprob = %d > %d (the problem index is a grid y/z coordinate)", nprob, CVXB_BATCH_MAX);
+        set_error("%s: nprob = %d > %d (the problem index is a grid y/z coordinate)", fn, nprob, CVXB_BATCH_MAX);
         return CVXB_E_ARG;
     }
     if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("batch_create: bad dims (mnl must be 0, ml and the cone counts nonnegative)");
+        set_error("%s: bad dims (mnl must be 0, ml and the cone counts nonnegative)", fn);
         return CVXB_E_ARG;
     }
-    long long mm = dims->ml;
+    mlq = (long long)mnl + dims->ml;
     for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("batch_create: dims['q'][%d] = %d < 1", k, dims->q[k]); return CVXB_E_ARG; }
-        mm += dims->q[k];
+        if (dims->q[k] < 1) { set_error("%s: dims['q'][%d] = %d < 1", fn, k, dims->q[k]); return CVXB_E_ARG; }
+        mlq += dims->q[k];
     }
-    if (mm > (1LL << 30)) { set_error("batch_create: too many cone rows"); return CVXB_E_ARG; }
-    if (dims->ns > 0 && !sdp) { set_error("batch_create: 's' cones are not supported by the batch"); return CVXB_E_UNSUP; }
-    const long long mlq = mm;
-    long long mpk = mm;                           // cdim_pckd
-    if (sdp && dims->ns > 0) {
-        if (!dims->s) { set_error("batch_create_sdp: dims has ns > 0 and no 's' orders"); return CVXB_E_ARG; }
-        for (int k = 0; k < dims->ns; ++k) {
-            const int s = dims->s[k];
-            if (s < 0) { set_error("batch_create_sdp: dims['s'][%d] = %d < 0", k, s); return CVXB_E_ARG; }
-            if (s > CVXB_BATCH_SMAX) {
-                set_error("batch_create_sdp: dims['s'][%d] = %d > %d, the largest 's' order of the batch", k, s,
-                          CVXB_BATCH_SMAX);
-                return CVXB_E_UNSUP;
-            }
-            mm += (long long)s * s; mpk += (long long)s * (s + 1) / 2;
+    if (dims->ns > 0 && !sdp) { set_error("%s: 's' cones are not supported by the batch", fn); return CVXB_E_UNSUP; }
+    if (dims->ns > 0 && !dims->s) { set_error("%s: dims has ns > 0 and no 's' orders", fn); return CVXB_E_ARG; }
+    m = mpk = mlq;
+    for (int k = 0; k < dims->ns; ++k) {
+        const int s = dims->s[k];
+        if (s < 0) { set_error("%s: dims['s'][%d] = %d < 0", fn, k, s); return CVXB_E_ARG; }
+        if (s > CVXB_BATCH_SMAX) {
+            set_error("%s: dims['s'][%d] = %d > %d, the largest 's' order of the batch", fn, k, s, CVXB_BATCH_SMAX);
+            return CVXB_E_UNSUP;
         }
+        m += (long long)s * s; mpk += (long long)s * (s + 1) / 2;
     }
-    if (mm > (1LL << 30)) { set_error("batch_create: too many cone rows"); return CVXB_E_ARG; }
-    if (lp && mm == 0) {                          // deliberate: every cone LP needs at least one cone row
-        set_error("batch_create_lp: the batch needs at least one 'l' or 'q' row (m = 0)");
+    if (m > (1LL << 30)) { set_error("%s: too many rows", fn); return CVXB_E_ARG; }
+    // deliberate for a cone LP; cpl's theta1 = 1 / gap0 (cvxprog.py:717) needs a row
+    if (m == 0 && (kind == Kind::LP || kind == Kind::CPL)) {
+        set_error("%s: no constraint rows (mnl + cdim = 0)", fn);
         return CVXB_E_ARG;
     }
-    // the checks before the first factorisation: coneqp's (coneprog.py:1962), conelp's (:572-573, with cdim_pckd)
-    if (p > n || (lp && p + mpk < n)) {
-        set_error("batch_create: Rank(A) < p or Rank([%s]) < n (p = %d, n = %d, cdim = %lld)", lp ? "G; A" : "P; A; G",
-                  p, n, mpk);
+    if (p > n || (kind == Kind::LP && p + mpk < n)) {
+        set_error("%s: %s (p = %d, n = %d, cdim = %lld)", fn, rank_text(kind, true), p, n, mpk);
         return CVXB_E_ARG;
     }
+    return 0;
+}
+
+// a batch of the given kind, once check_args has passed its arguments: QPs, or cone LPs (no P; q holds c), with the
+// cones of dims ('l', 'q' and with sdp 's' blocks) and p equality rows; or a GP, CP or cpl batch, whose G begins with
+// the mnl rows of Df (counted among the 'l' rows), f having nK = mnl + 1 rows with gp's and cp's epigraph row or nK =
+// mnl (cpl).  K: a GP's term counts; the sum K rows of its F go below G's m rows.  Every buffer of the kind, then the
+// state row
+int create(cvxb_batch **out, const char *fn, Kind kind, int nprob, int n, int p, int mnl, const cvxb_dims *dims,
+           bool sdp, int device, const int *K = nullptr) {
+    long long mlq = 0, mm = 0, mpk = 0;
+    CVXB_TRY(check_args(fn, kind, out, nprob, n, p, mnl, dims, sdp, mlq, mm, mpk));
     CVXB_TRY(check_device(device));
-    const int m = (int)mm;
+    const int m = (int)mm, ml = mnl + dims->ml, nK = kind == Kind::CPL ? mnl : mnl + 1;
+    long long sumK = 0;
+    for (int i = 0; K && i < nK; ++i) sumK += K[i];
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
-    b->device = device; b->B = nprob; b->n = n; b->m = m; b->lp = lp;
+    b->kind = kind; b->device = device; b->B = nprob; b->n = n; b->m = m;
     b->i8_mode = ozaki_mode();
-    b->ldg = ((m + xrows + 1) & ~1) > 2 ? ((m + xrows + 1) & ~1) : 2;
+    b->ldg = ((m + sumK + 1) & ~1) > 2 ? ((m + sumK + 1) & ~1) : 2;
     b->ldp = b->ldk = (n + 1) & ~1;
     b->sG = b->ldg * n; b->sP = b->ldp * n; b->sK = b->ldk * n;
     b->nblk = (n + NB - 1) / NB;
@@ -2941,14 +2966,14 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     CVXB_CUDA(cudaStreamCreateWithFlags(&b->st, cudaStreamNonBlocking));
     CVXB_CUDA(cudaEventCreate(&b->e0)); CVXB_CUDA(cudaEventCreate(&b->e1));
     CVXB_TRY(chol_work_create(b->cw));
-    if (!lp) CVXB_TRY(b->P.alloc(B * b->sP));
+    if (kind != Kind::LP) CVXB_TRY(b->P.alloc(B * b->sP));
     CVXB_TRY(b->G.alloc(B * b->sG));
     CVXB_TRY(b->K.alloc(B * b->sK));
     CVXB_TRY(b->inv.alloc(B * b->sInv));
     CVXB_TRY(b->panel.alloc(B * (size_t)((n + 1) & ~1) * NB));
-    // GEMV workspace: G x (m rows); with equality rows also A x (p rows) and Asct y (n rows)
+    // GEMV workspace: G x (m rows), F x (sum K rows); with equality rows also A x (p rows) and Asct y (n rows)
     const size_t me = (size_t)(m > 0 ? m : 1);
-    size_t ws = std::max(me, (size_t)xrows) * gemv_n_chunks(n);
+    size_t ws = std::max(me, (size_t)sumK) * gemv_n_chunks(n);
     if (p > 0) ws = std::max({ws, (size_t)p * gemv_n_chunks(n), (size_t)n * gemv_n_chunks(p)});
     CVXB_TRY(b->gemv_ws.alloc(B * ws));
     // vectors: n-sized: q x rx dx ; m-sized: h s z rz ds dz lmbda lmbdasq d di di2 ws3 bzp
@@ -2963,7 +2988,7 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     b->h = take(me); q.s = take(me); q.z = take(me); q.rz = take(me); q.ds = take(me);
     q.dz = take(me); q.lmbda = take(me); q.lmbdasq = take(me); q.d = take(me);
     q.di = take(me); q.di2 = take(me); q.ws3 = take(me); q.bzp = take(me);
-    q.q = b->q; q.h = b->h; q.n = n; q.m = m; q.ml = dims->ml;
+    q.q = b->q; q.h = b->h; q.n = n; q.m = m; q.ml = ml;
     CVXB_TRY(b->sc.alloc(B));
     CVXB_CUDA(cudaMemset(b->sc.p, 0, B * sizeof(Scal)));
     q.sc = b->sc.p;
@@ -2977,7 +3002,7 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     if (const char *e = getenv("CVXB_BATCH_COMPACT")) b->compact = (e[0] == '0') ? 0 : 1;
     if (dims->nq > 0) {
         const int nq = dims->nq;
-        std::vector<int> off(nq + 1, dims->ml);
+        std::vector<int> off(nq + 1, ml);
         for (int k = 0; k < nq; ++k) off[k + 1] = off[k] + dims->q[k];
         CVXB_TRY(b->qoff.alloc(nq + 1));
         CVXB_CUDA(cudaMemcpy(b->qoff.p, off.data(), (nq + 1) * sizeof(int), cudaMemcpyHostToDevice));
@@ -2987,7 +3012,7 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
     }
     b->mpk = (int)mpk;
     q.mlq = (int)mlq; q.mpk = (int)mpk; q.mdg = (int)mlq;
-    if (sdp && mm > mlq) {                        // 's' blocks of positive order; order 0 adds no rows (:497-499)
+    if (mm > mlq) {                               // 's' blocks of positive order; order 0 adds no rows (:497-499)
         std::vector<int> info;
         std::vector<int> u2p(mm - mlq);
         std::vector<double> rw(m, 1.0);
@@ -3039,18 +3064,66 @@ int create(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int
         q.beq = w; q.y = w + B * p; q.ry = w + 2 * B * p; q.dy = w + 3 * B * p; q.aw = w + 4 * B * p;
         q.infop = b->d_infop.p;
     }
-    if (lp) {
+    if (kind == Kind::LP) {
         const size_t len = (size_t)n + 2 * (size_t)m + (size_t)p;
         CVXB_TRY(b->lpv.alloc(B * len));
         CVXB_CUDA(cudaMemset(b->lpv.p, 0, B * len * sizeof(double)));
         q.x1 = b->lpv.p; q.z1 = q.x1 + B * n; q.th = q.z1 + B * m; q.y1 = q.th + B * m;
+    }
+    GPPtrs &g = b->gq;
+    if (b->cpl_loop()) {
+        g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
+        g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
+        // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
+        const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * (size_t)m;
+        CVXB_TRY(b->gpv.alloc(B * len));
+        CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
+        v = b->gpv.p;
+        g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
+        g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
+        g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
+        q.refinement = m > 0 || b->calls_back() ? 1 : 0;     // cpl's default (cvxprog.py:422)
+    }
+    if (kind == Kind::GP) {
+        g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
+        std::vector<int> off(nK + 1, 0);
+        for (int i = 0; i < nK; ++i) off[i + 1] = off[i] + K[i];
+        CVXB_TRY(b->koff.alloc(nK + 1));
+        CVXB_CUDA(cudaMemcpy(b->koff.p, off.data(), (nK + 1) * sizeof(int), cudaMemcpyHostToDevice));
+        g.koff = b->koff.p;
+        CVXB_TRY(b->gph.alloc(B * g.sH));
+        CVXB_TRY(b->gpg.alloc(B * sumK));
+        g.Hr = b->gph.p;
+    }
+    if (b->calls_back()) {                        // the callback's buffers, x0 and the slot -> problem map
+        const size_t nn = n;
+        // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
+        const size_t len = 2 * nK + nK * nn + nn * nn;
+        CVXB_TRY(b->cpv.alloc(B * len));
+        CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
+        CVXB_TRY(b->cpx0.alloc(B * nn));
+        CVXB_TRY(b->cpi.alloc(B + 1));
+        CPPtrs &c = b->cq;
+        c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
+        c.idx = b->cpi.p; c.bad = b->cpi.p + B;
+        c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
     }
     CVXB_TRY(state_alloc(b.get()));
     *out = b.release();
     return 0;
 }
 
-// G, h and q (c) of every problem, then a fresh batch: problems in their own slots, A and b still to load
+// a fresh batch once its data is on the device: every problem in its own slot, A and b still to load
+int load_done(cvxb_batch *b) {
+    CVXB_CUDA(cudaStreamSynchronize(b->st));
+    b->loaded = true;
+    b->eq_loaded = false;
+    for (int i = 0; i < b->B; ++i) b->perm[i] = i;
+    b->permuted = false;
+    return 0;
+}
+
+// G, h and q (c) of every problem
 int load_common(cvxb_batch *b, const double *q, const double *G, const double *h, cudaMemcpyKind kind) {
     const size_t B = b->B, n = b->n, m = b->m;
     // one strided 2-D copy per matrix operand: rows of the "matrix of columns" are the matrix columns
@@ -3060,40 +3133,11 @@ int load_common(cvxb_batch *b, const double *q, const double *G, const double *h
         CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->h), h, B * m * sizeof(double), kind, b->st));
     }
     CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), q, B * n * sizeof(double), kind, b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    b->eq_loaded = false;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
-    return 0;
-}
-
-// the common part of a GP, a CP and a cpl batch: a QP batch whose 'l' rows begin with the mnl nonlinear rows (d.ml
-// counts them), nK = mnl + 1 nonlinear rows of f (a cpl batch's nK = mnl) with sumK rows of F below the m rows of G,
-// and gq's per-slot vectors.  sdp: d may hold 's' blocks, after the 'q' rows
-int create_cpl(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, long long sumK, const cvxb_dims &d,
-               int p, int device, bool sdp = false) {
-    cvxb_batch *raw = nullptr;
-    CVXB_TRY(create(&raw, nprob, n, p, &d, device, false, sdp, (int)sumK));
-    b.reset(raw);
-    const size_t B = nprob, m = b->m;
-    GPPtrs &g = b->gq;
-    g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
-    g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
-    // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
-    const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * m;
-    CVXB_TRY(b->gpv.alloc(B * len));
-    CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
-    double *v = b->gpv.p;
-    auto take = [&](size_t l) { double *r = v; v += B * l; return r; };
-    g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
-    g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
-    g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
-    return 0;
+    return load_done(b);
 }
 
 // the rows of a GP, CP or cpl batch after its own data: G below the mnl rows of Df, h in the 'l' and 'q' rows (0 on
-// the nonlinear ones), q: c (a cpl batch), else 0 (c's x part in the epigraph problem); then a fresh batch
+// the nonlinear ones), q: c (a cpl batch), else 0 (c's x part in the epigraph problem)
 int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyKind kind, const double *c = nullptr) {
     const size_t B = b->B, n = b->n, m = b->m, mnl = b->gq.mnl, ml = m - mnl;
     CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->h), 0, B * (m ? m : 1) * sizeof(double), b->st));
@@ -3105,83 +3149,16 @@ int load_cpl_common(cvxb_batch *b, const double *G, const double *h, cudaMemcpyK
     }
     if (c) CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->q), c, B * n * sizeof(double), kind, b->st));
     else CVXB_CUDA(cudaMemsetAsync(const_cast<double *>(b->q), 0, B * n * sizeof(double), b->st));
-    CVXB_CUDA(cudaStreamSynchronize(b->st));
-    b->loaded = true;
-    b->eq_loaded = false;
-    for (size_t i = 0; i < B; ++i) b->perm[i] = (int)i;
-    b->permuted = false;
-    return 0;
+    return load_done(b);
 }
 
-// a batch with the caller's F: CP (the epigraph problem, nK = mnl + 1) or cpl (nK = mnl, 'q' cones in d): the
-// callback's buffers, x0 and the slot -> problem map; refinement 1, cpl's default (cvxprog.py:422)
-int create_cp_common(std::unique_ptr<cvxb_batch> &b, int nprob, int n, int mnl, int nK, const cvxb_dims &d, int p,
-                     int device, bool sdp = false) {
-    CVXB_TRY(create_cpl(b, nprob, n, mnl, nK, 0, d, p, device, sdp));
-    const size_t B = nprob, nn = n;
-    // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
-    const size_t len = 2 * nK + nK * nn + nn * nn;
-    CVXB_TRY(b->cpv.alloc(B * len));
-    CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
-    CVXB_TRY(b->cpx0.alloc(B * nn));
-    CVXB_TRY(b->cpi.alloc(B + 1));
-    CPPtrs &c = b->cq;
-    c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
-    c.idx = b->cpi.p; c.bad = b->cpi.p + B;
-    c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
-    b->cp = true;
-    b->p.refinement = 1;
-    return state_alloc(b.get());
-}
-
-// cvxb_batch_create_cpl (sdp false: 's' cones are CVXB_E_UNSUP) and cvxb_batch_create_sdp_cpl (sdp: 's' blocks of
-// order at most CVXB_BATCH_SMAX after the 'q' rows); every refusal comes before the device
-int create_cpl_batch(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device, bool sdp) {
-    const char *fn = sdp ? "batch_create_sdp_cpl" : "batch_create_cpl";
-    if (out) *out = nullptr;
-    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || p < 0 || !dims) {
-        set_error("%s: bad sizes (nprob in 1..%d, n >= 1, mnl and p nonnegative, dims given)", fn, CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    if (dims->mnl != 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 || (dims->nq > 0 && !dims->q)) {
-        set_error("%s: bad dims (its mnl must be 0; ml and the cone counts nonnegative)", fn);
-        return CVXB_E_ARG;
-    }
-    if (dims->ns > 0 && !sdp) {
-        set_error("batch_create_cpl: 's' cones are not supported by the cpl batch");
-        return CVXB_E_UNSUP;
-    }
-    long long m = (long long)mnl + dims->ml;
-    for (int k = 0; k < dims->nq; ++k) {
-        if (dims->q[k] < 1) { set_error("%s: dims['q'][%d] = %d < 1", fn, k, dims->q[k]); return CVXB_E_ARG; }
-        m += dims->q[k];
-    }
-    if (dims->ns > 0 && !dims->s) { set_error("%s: dims has ns > 0 and no 's' orders", fn); return CVXB_E_ARG; }
-    for (int k = 0; k < dims->ns; ++k) {
-        const int s = dims->s[k];
-        if (s < 0) { set_error("%s: dims['s'][%d] = %d < 0", fn, k, s); return CVXB_E_ARG; }
-        if (s > CVXB_BATCH_SMAX) {
-            set_error("%s: dims['s'][%d] = %d > %d, the largest 's' order of the batch", fn, k, s, CVXB_BATCH_SMAX);
-            return CVXB_E_UNSUP;
-        }
-        m += (long long)s * s;
-    }
-    if (m == 0) {                                     // cpl's theta1 = 1 / gap0 (cvxprog.py:717) needs a row
-        set_error("%s: no constraint rows (mnl + cdim = 0)", fn);
-        return CVXB_E_ARG;
-    }
-    if (m > (1LL << 30)) { set_error("%s: too many rows", fn); return CVXB_E_ARG; }
-    if (p > n) {                                      // cpl's check before the first factorisation
-        set_error("%s: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", fn, p, n);
-        return CVXB_E_ARG;
-    }
-    std::unique_ptr<cvxb_batch> b;
-    cvxb_dims d = *dims;
-    d.ml += mnl;
-    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl, d, p, device, sdp));
-    b->cpl = true;
-    *out = b.release();
-    return 0;
+// fn(std::bool_constant<f>...) for the runtime flags f: each combination of the flags instantiates fn once, false
+// before true with the last flag varying fastest (the order of the kernels in the object file follows it)
+template <class Fn> int with_flags(Fn &&fn) { return fn(); }
+template <class Fn, class... Rest> int with_flags(Fn &&fn, bool f, Rest... rest) {
+    auto bind = [&](auto c) { return with_flags([&](auto... cs) { return fn(c, cs...); }, rest...); };
+    if (!f) return bind(std::false_type{});
+    return bind(std::true_type{});
 }
 
 }  // namespace
@@ -3191,94 +3168,62 @@ extern "C" {
 int cvxb_batch_create(cvxb_batch **out, int nprob, int n, int m, int device) {
     cvxb_dims dims{};
     dims.ml = m;
-    return create(out, nprob, n, 0, &dims, device, false);
+    return create(out, "batch_create", Kind::QP, nprob, n, 0, 0, &dims, false, device);
 }
 
 int cvxb_batch_create_cones(cvxb_batch **out, int nprob, int n, const cvxb_dims *dims, int device) {
-    return create(out, nprob, n, 0, dims, device, false);
+    return create(out, "batch_create_cones", Kind::QP, nprob, n, 0, 0, dims, false, device);
 }
 
 int cvxb_batch_create_eq(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    return create(out, nprob, n, p, dims, device, false);
+    return create(out, "batch_create_eq", Kind::QP, nprob, n, p, 0, dims, false, device);
 }
 
 int cvxb_batch_create_lp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    return create(out, nprob, n, p, dims, device, true);
+    return create(out, "batch_create_lp", Kind::LP, nprob, n, p, 0, dims, false, device);
 }
 
 int cvxb_batch_create_sdp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    return create(out, nprob, n, p, dims, device, true, true);
+    return create(out, "batch_create_sdp", Kind::LP, nprob, n, p, 0, dims, true, device);
 }
 
 int cvxb_batch_create_sdp_qp(cvxb_batch **out, int nprob, int n, int p, const cvxb_dims *dims, int device) {
-    return create(out, nprob, n, p, dims, device, false, true);
+    return create(out, "batch_create_sdp_qp", Kind::QP, nprob, n, p, 0, dims, true, device);
 }
 
 int cvxb_batch_create_gp(cvxb_batch **out, int nprob, int n, int nK, const int *K, int ml, int p, int device) {
     if (out) *out = nullptr;
-    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || nK < 1 || !K || ml < 0 || p < 0) {
-        set_error("batch_create_gp: bad sizes (nprob in 1..%d, n >= 1, nK >= 1 with K given, ml and p nonnegative)",
-                  CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
+    if (nK < 1 || !K) { set_error("batch_create_gp: bad sizes (nK >= 1 with K given)"); return CVXB_E_ARG; }
     long long sumK = 0;
     for (int i = 0; i < nK; ++i) {
         if (K[i] < 1) { set_error("batch_create_gp: K[%d] = %d < 1", i, K[i]); return CVXB_E_ARG; }
         sumK += K[i];
     }
     if (sumK + nK + ml > (1LL << 30)) { set_error("batch_create_gp: too many rows"); return CVXB_E_ARG; }
-    std::unique_ptr<cvxb_batch> b;
     cvxb_dims d{};
-    d.ml = nK - 1 + ml;
-    CVXB_TRY(create_cpl(b, nprob, n, nK - 1, nK, sumK, d, p, device));
-    const size_t B = nprob;
-    GPPtrs &g = b->gq;
-    g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
-    std::vector<int> off(nK + 1, 0);
-    for (int i = 0; i < nK; ++i) off[i + 1] = off[i] + K[i];
-    CVXB_TRY(b->koff.alloc(nK + 1));
-    CVXB_CUDA(cudaMemcpy(b->koff.p, off.data(), (nK + 1) * sizeof(int), cudaMemcpyHostToDevice));
-    g.koff = b->koff.p;
-    CVXB_TRY(b->gph.alloc(B * g.sH));
-    CVXB_TRY(b->gpg.alloc(B * sumK));
-    g.Hr = b->gph.p;
-    b->gp = true;
-    b->p.refinement = b->m > 0 ? 1 : 0;               // cpl's default (cvxprog.py:422)
-    CVXB_TRY(state_alloc(b.get()));
-    *out = b.release();
-    return 0;
+    d.ml = ml;
+    return create(out, "batch_create_gp", Kind::GP, nprob, n, p, nK - 1, &d, false, device, K);
 }
 
 int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, int p, int device) {
     if (out) *out = nullptr;
-    if (!out || nprob < 1 || nprob > CVXB_BATCH_MAX || n < 1 || mnl < 0 || ml < 0 || p < 0) {
-        set_error("batch_create_cp: bad sizes (nprob in 1..%d, n >= 1, mnl, ml and p nonnegative)", CVXB_BATCH_MAX);
-        return CVXB_E_ARG;
-    }
-    if (p > n) {                                      // cp's check before the first factorisation
-        set_error("batch_create_cp: Rank(A) < p or Rank([H(x); A; Df(x); G]) < n (p = %d, n = %d)", p, n);
-        return CVXB_E_ARG;
-    }
     if ((long long)mnl + ml + 1 > (1LL << 30)) { set_error("batch_create_cp: too many rows"); return CVXB_E_ARG; }
-    std::unique_ptr<cvxb_batch> b;
     cvxb_dims d{};
-    d.ml = mnl + ml;
-    CVXB_TRY(create_cp_common(b, nprob, n, mnl, mnl + 1, d, p, device));
-    *out = b.release();
-    return 0;
+    d.ml = ml;
+    return create(out, "batch_create_cp", Kind::CP, nprob, n, p, mnl, &d, false, device);
 }
 
 int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
-    return create_cpl_batch(out, nprob, n, mnl, dims, p, device, false);
+    return create(out, "batch_create_cpl", Kind::CPL, nprob, n, p, mnl, dims, false, device);
 }
 
 int cvxb_batch_create_sdp_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
-    return create_cpl_batch(out, nprob, n, mnl, dims, p, device, true);
+    return create(out, "batch_create_sdp_cpl", Kind::CPL, nprob, n, p, mnl, dims, true, device);
 }
 
 int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx) {
     if (!b) { set_error("batch_set_cp_eval: batch is NULL"); return CVXB_E_ARG; }
-    if (!b->cp) { set_error("batch_set_cp_eval: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
+    if (!b->calls_back()) { set_error("batch_set_cp_eval: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
     b->cfn = fn;
     b->cctx = ctx;
     return 0;
@@ -3288,7 +3233,7 @@ int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     // a batch without constraint rows takes unrefined steps; a CP batch always has cp's epigraph row
-    b->p.refinement = b->m > 0 || b->cp ? refinement : 0;
+    b->p.refinement = b->m > 0 || b->calls_back() ? refinement : 0;
     CVXB_TRY(state_alloc(b));
     return 0;
 }
@@ -3303,9 +3248,9 @@ void cvxb_batch_destroy(cvxb_batch *b) {
 int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const double *G,
                     const double *h, int space) {
     if (!b || !P || !q || (b->m > 0 && (!G || !h))) { set_error("batch_load: NULL argument"); return CVXB_E_ARG; }
-    if (b->lp) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
-    if (b->gp) { set_error("batch_load: a GP batch is loaded with cvxb_batch_load_gp"); return CVXB_E_ARG; }
-    if (b->cp) { set_error("batch_load: a CP batch is loaded with cvxb_batch_load_cp"); return CVXB_E_ARG; }
+    if (b->kind == Kind::LP) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
+    if (b->kind == Kind::GP) { set_error("batch_load: a GP batch is loaded with cvxb_batch_load_gp"); return CVXB_E_ARG; }
+    if (b->calls_back()) { set_error("batch_load: a CP batch is loaded with cvxb_batch_load_cp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t n = b->n;
@@ -3318,14 +3263,14 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
 
 int cvxb_batch_load_lp(cvxb_batch *b, const double *c, const double *G, const double *h, int space) {
     if (!b || !c || !G || !h) { set_error("batch_load_lp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->lp) { set_error("batch_load_lp: a QP, GP or CP batch is not a cone LP batch"); return CVXB_E_ARG; }
+    if (b->kind != Kind::LP) { set_error("batch_load_lp: a QP, GP or CP batch is not a cone LP batch"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     return load_common(b, c, G, h, (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice);
 }
 
 int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const double *G, const double *h, int space) {
     if (!b || !F || !g || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_gp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->gp) { set_error("batch_load_gp: not a GP batch (cvxb_batch_create_gp)"); return CVXB_E_ARG; }
+    if (b->kind != Kind::GP) { set_error("batch_load_gp: not a GP batch (cvxb_batch_create_gp)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t B = b->B, n = b->n, m = b->m, sK = b->gq.sumK;
@@ -3338,7 +3283,7 @@ int cvxb_batch_load_gp(cvxb_batch *b, const double *F, const double *g, const do
 
 int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const double *h, int space) {
     if (!b || !x0 || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_cp: NULL argument"); return CVXB_E_ARG; }
-    if (!b->cp || b->cpl) { set_error("batch_load_cp: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
+    if (b->kind != Kind::CP) { set_error("batch_load_cp: not a CP batch (cvxb_batch_create_cp)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, (size_t)b->B * b->n * sizeof(double), kind, b->st));
@@ -3347,7 +3292,7 @@ int cvxb_batch_load_cp(cvxb_batch *b, const double *x0, const double *G, const d
 
 int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const double *G, const double *h, int space) {
     if (!b || !c || !x0 || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_cpl: NULL argument"); return CVXB_E_ARG; }
-    if (!b->cpl) { set_error("batch_load_cpl: not a cpl batch (cvxb_batch_create_cpl)"); return CVXB_E_ARG; }
+    if (b->kind != Kind::CPL) { set_error("batch_load_cpl: not a cpl batch (cvxb_batch_create_cpl)"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, (size_t)b->B * b->n * sizeof(double), kind, b->st));
@@ -3376,9 +3321,9 @@ int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int s
 int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const double *y, const double *z,
                           int space) {
     if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
-    if (b->gp) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
-    if (b->cp) { set_error("batch_load_start: cp and cpl start from the x0 of their load"); return CVXB_E_ARG; }
-    if (b->lp && ((!x) != (!s) || (y && !z) || (!x && !z))) {
+    if (b->kind == Kind::GP) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
+    if (b->calls_back()) { set_error("batch_load_start: cp and cpl start from the x0 of their load"); return CVXB_E_ARG; }
+    if (b->kind == Kind::LP && ((!x) != (!s) || (y && !z) || (!x && !z))) {
         set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
                   "both");
         return CVXB_E_ARG;
@@ -3415,30 +3360,19 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     }
     CVXB_CUDA(cudaSetDevice(b->device));
     CVXB_TRY(restore_order(b));
-    if (b->cp && !b->cfn) { set_error("batch_solve: a CP batch needs its F (cvxb_batch_set_cp_eval)"); return CVXB_E_ARG; }
-    if (b->cpl) {
-        using Solve = int (*)(cvxb_batch *, int, double, double, double);
-        static const Solve cpl_solvers[4] = {solve_cpl<false, false, false>, solve_cpl<true, false, false>,
-                                             solve_cpl<false, false, true>, solve_cpl<true, false, true>};
-        static const Solve sdp_cpl_solvers[4] = {solve_cpl<false, false, false, true>, solve_cpl<true, false, false, true>,
-                                                 solve_cpl<false, false, true, true>, solve_cpl<true, false, true, true>};
-        const int k = (b->neq > 0 ? 1 : 0) + (b->p.nq > 0 ? 2 : 0);
-        if (b->p.ns > 0) return sdp_cpl_solvers[k](b, maxiters, abstol, reltol, feastol);   // 's' blocks of positive order
-        return cpl_solvers[k](b, maxiters, abstol, reltol, feastol);
-    }
-    if (b->gp || b->cp) return b->neq > 0 ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
-                                          : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
-    using Solve = int (*)(cvxb_batch *, int, double, double, double);
-    static const Solve solvers[8] = {solve<false, false, false>, solve<true, false, false>, solve<false, true, false>,
-                                     solve<true, true, false>,   solve<false, false, true>,  solve<true, false, true>,
-                                     solve<false, true, true>,   solve<true, true, true>};
-    static const Solve sdp_solvers[8] = {solve<false, false, false, true>, solve<true, false, false, true>,
-                                         solve<false, true, false, true>,  solve<true, true, false, true>,
-                                         solve<false, false, true, true>,  solve<true, false, true, true>,
-                                         solve<false, true, true, true>,   solve<true, true, true, true>};
-    const int k = (b->p.nq > 0 ? 1 : 0) + (b->neq > 0 ? 2 : 0) + (b->lp ? 4 : 0);     // CONES, EQ, LP
-    if (b->p.ns > 0) return sdp_solvers[k](b, maxiters, abstol, reltol, feastol);     // 's' blocks of positive order
-    return solvers[k](b, maxiters, abstol, reltol, feastol);
+    if (b->calls_back() && !b->cfn) { set_error("batch_solve: a CP batch needs its F (cvxb_batch_set_cp_eval)"); return CVXB_E_ARG; }
+    // SDP: 's' blocks of positive order
+    const bool sdp = b->p.ns > 0, lp = b->kind == Kind::LP, eq = b->neq > 0, cones = b->p.nq > 0;
+    if (b->kind == Kind::CPL)
+        return with_flags([&](auto SDP, auto CONES, auto EQ) {
+            return solve_cpl<EQ, false, CONES, SDP>(b, maxiters, abstol, reltol, feastol);
+        }, sdp, cones, eq);
+    if (b->cpl_loop())                            // GP, CP: the epigraph problem, 'l' rows only
+        return eq ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
+                  : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
+    return with_flags([&](auto SDP, auto LP, auto EQ, auto CONES) {
+        return solve<CONES, EQ, LP, SDP>(b, maxiters, abstol, reltol, feastol);
+    }, sdp, lp, eq, cones);
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {
