@@ -15,6 +15,7 @@ from .batch import GPBatch, GPBatchGroup, gp_batch  # noqa: F401
 from .batch import CPBatch, CPBatchGroup, cp_batch  # noqa: F401
 from .batch import CPLBatch, CPLBatchGroup, cpl_batch  # noqa: F401
 from .batch import SDPCPLBatch, SDPCPLBatchGroup, sdp_cpl_batch  # noqa: F401
+from .batch import QCQPBatch, QCQPBatchGroup, qcqp_batch  # noqa: F401
 
 __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolver", "cpl_kktsolver", "QPBatch", "qp_batch", "conelp", "qp_batch_distributed", "load",
            "ConeLPBatch", "conelp_batch", "SDPBatch", "SDPBatchGroup", "sdp_batch",
@@ -22,6 +23,7 @@ __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolv
            "CPBatch", "CPBatchGroup", "cp_batch",
            "CPLBatch", "CPLBatchGroup", "cpl_batch",
            "SDPCPLBatch", "SDPCPLBatchGroup", "sdp_cpl_batch",
+           "QCQPBatch", "QCQPBatchGroup", "qcqp_batch",
            "device_count", "launch_count"]
 
 

@@ -145,6 +145,10 @@ _SIGS = {
     "cvxb_batch_ls_rounds": (C.c_int, [C.c_void_p]),
     "cvxb_batch_create_cp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
     "cvxb_batch_load_cp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "cvxb_batch_create_qcqp": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                         C.c_int]),
+    "cvxb_batch_load_qcqp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_int]),
     "cvxb_batch_set_cp_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "cvxb_batch_create_cpl": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                         C.c_int]),

@@ -891,6 +891,13 @@ def _cp_args(F, G, h, dims, A, b):
     if x0.ndim != 2 or x0.dtype != np.float64:
         raise TypeError("'x0' must be a 'd' matrix with one column: a float64 array of shape (B, n)")
     B, n = x0.shape
+    G, h, A, b = _cp_rows(B, n, G, h, dims, A, b)
+    return mnl, x0, G, h, A, b
+
+
+def _cp_rows(B, n, G, h, dims, A, b):
+    """cp's checks of G, h, dims, A and b (cvxprog.py:1653-1728) for B problems with n variables -> G, h, A, b with the
+    defaults filled in; 'q' and 's' cones raise NotImplementedError and p > n the Rank ValueError"""
     if dims is not None and (dims.get("q") or dims.get("s")):
         raise NotImplementedError("the CP batch takes 'l' inequalities only (dims without 'q' and 's' cones)")
     h = np.zeros((B, 0)) if h is None else np.asarray(h)
@@ -913,7 +920,7 @@ def _cp_args(F, G, h, dims, A, b):
         raise TypeError("'b' must have length %d" % p)
     if p > n:
         raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
-    return mnl, x0, G, h, A, b
+    return G, h, A, b
 
 
 def cp_batch(F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, **options):
@@ -940,6 +947,91 @@ def cp_batch(F, G=None, h=None, dims=None, A=None, b=None, device=0, nsub=None, 
         grp.close()
         raise
     out = _run_group(grp, (x0, G, h, A if p else None, b if p else None), options)
+    for key in ("s", "z"):
+        v = out.pop(key)
+        out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]
+    return out
+
+
+class QCQPBatch(CPBatch):
+    """B convex QCQPs (cvxb_batch_create_qcqp): B x solvers.cp(F, G, h, dims={'l': ml}, A, b) with f_i(x) = x'P_i x / 2
+    + q_i'x + r_i (i = 0..mnl), the CP batch with F evaluated by the library's kernels (no set_F, no host callback).
+    mnl, ml rows of G and p rows of A are shared by the batch.  load() takes P (B, mnl + 1, n, n), of which only each
+    P_i's lower triangle is read, q (B, mnl + 1, n), r (B, mnl + 1), x0 (B, n) or None for 0, G (B, ml, n), h (B, ml)
+    and, with p > 0, A (B, p, n), b (B, p).  results() are CPBatch's."""
+
+    def _create(self):
+        return self._lib.cvxb_batch_create_qcqp(C.byref(self._h), self.B, self.n, self.mnl, self.ml, self.p,
+                                                self.device)
+
+    def load(self, P, q, r, x0, G, h, A=None, b=None):
+        B, n, nK = self.B, self.n, self.mnl + 1
+        P = np.asarray(P, dtype=np.float64)
+        q = np.ascontiguousarray(np.asarray(q, dtype=np.float64))
+        r = np.ascontiguousarray(np.asarray(r, dtype=np.float64))
+        x0 = np.zeros((B, n)) if x0 is None else np.ascontiguousarray(np.asarray(x0, dtype=np.float64))
+        G = np.zeros((B, 0, n)) if G is None else np.asarray(G, dtype=np.float64)
+        h = np.zeros((B, 0)) if h is None else np.ascontiguousarray(np.asarray(h, dtype=np.float64))
+        if P.shape != (B, nK, n, n) or q.shape != (B, nK, n) or r.shape != (B, nK) or x0.shape != (B, n) or \
+                G.shape != (B, self.ml, n) or h.shape != (B, self.ml):
+            raise TypeError("problem shapes do not match the batch")
+        Acm, bv = self._host_eq(A, b)
+        # per problem the (nK n) x n column-major stack [P_0; ...; P_mnl]: column j holds P_0[:, j], P_1[:, j], ...
+        Pcm = np.ascontiguousarray(np.transpose(P, (0, 3, 1, 2)))
+        Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
+        _lib.check(self._lib.cvxb_batch_load_qcqp(self._h, Pcm.ctypes.data, q.ctypes.data, r.ctypes.data,
+                                                  x0.ctypes.data, Gcm.ctypes.data if self.ml else None,
+                                                  h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_qcqp")
+        self._load_eq(Acm, bv, _lib.HOST)
+
+
+class QCQPBatchGroup(CPBatchGroup):
+    """QPBatchGroup's interleaved sub-batches, solved concurrently on their own streams, for convex QCQPs; nothing
+    calls back to the host, so the sub-batches never wait on each other"""
+
+    def _part(self):
+        return lambda nprob, n, m, device, dims, p=0: QCQPBatch(nprob, n, self._mnl, self._ml, p, device)
+
+    def load(self, P, q, r, x0, G, h, A=None, b=None):
+        self._load_sliced((P, q, r, x0, G, h), A, b)
+
+
+def _qcqp_args(P, q, r, G, h, dims, A, b, x0):
+    """qcqp_batch's checks: P, q, r and x0 with cp's wording, then _cp_rows' -> P, q, r, x0, G, h, A, b as float64
+    arrays with the defaults filled in"""
+    P = np.asarray(P)
+    if P.ndim != 4 or P.shape[1] < 1 or P.shape[2] != P.shape[3] or P.shape[2] < 1 or P.dtype.kind != "f":
+        raise TypeError("'P' must be a 'd' array of shape (B, mnl + 1, n, n)")
+    B, nK, n = P.shape[:3]
+    q = np.asarray(q)
+    if q.shape != (B, nK, n) or q.dtype.kind != "f":
+        raise TypeError("'q' must be a 'd' array of shape (%d, %d, %d)" % (B, nK, n))
+    r = np.asarray(r)
+    if r.shape != (B, nK) or r.dtype.kind != "f":
+        raise TypeError("'r' must be a 'd' array of shape (%d, %d)" % (B, nK))
+    x0 = np.zeros((B, n)) if x0 is None else np.asarray(x0)
+    if x0.shape != (B, n) or x0.dtype.kind != "f":
+        raise TypeError("'x0' must be a 'd' matrix with one column: a float64 array of shape (%d, %d)" % (B, n))
+    G, h, A, b = _cp_rows(B, n, G, h, dims, A, b)
+    f64 = [np.asarray(a, dtype=np.float64) for a in (P, q, r, x0, G, h, A, b)]
+    return tuple(f64)
+
+
+def qcqp_batch(P, q, r, G=None, h=None, dims=None, A=None, b=None, x0=None, device=0, nsub=None, **options):
+    """Solve B independent convex QCQPs on one GPU, each as solvers.cp(F, G, h, dims, A, b) does with the quadratic F
+    f_i(x) = x'P_i x / 2 + q_i'x + r_i, Df_i = (P_i x + q_i)', H = sum_i z_i P_i:
+        minimize f_0(x) s.t. f_i(x) <= 0 (i = 1..mnl), G x <= h, A x = b.
+    P (B, mnl + 1, n, n), only each P_i's lower triangle read (P_0 = 0 is a linear objective; every P_i positive
+    semidefinite is the caller's promise), q (B, mnl + 1, n), r (B, mnl + 1); mnl = 0 is allowed.  G (B, ml, n),
+    h (B, ml), A (B, p, n), b (B, p) and x0 (B, n, default 0; dom f is R^n) are optional; dims, if given, is
+    {'l': ml}.  F is evaluated on the device by the library: nothing calls back to Python.  Returns cp_batch's dict:
+    x, snl, sl, znl, zl, y, status ('optimal' or 'unknown'), iterations, primal objective and dual objective, with the
+    batch's stats (solve_ms, lock-step iterations, line-search rounds, nsub, solve_wall_ms).  nsub is qp_batch's.
+    options: maxiters, abstol, reltol, feastol, refinement (as cp's)."""
+    P, q, r, x0, G, h, A, b = _qcqp_args(P, q, r, G, h, dims, A, b, x0)
+    B, mnl, n, p = P.shape[0], P.shape[1] - 1, P.shape[2], A.shape[1]
+    out = _run_group(QCQPBatchGroup(B, n, mnl, G.shape[1], p, device, nsub),
+                     (P, q, r, x0, G, h, A if p else None, b if p else None), options)
     for key in ("s", "z"):
         v = out.pop(key)
         out[key + "nl"], out[key + "l"] = v[:, :mnl], v[:, mnl:]

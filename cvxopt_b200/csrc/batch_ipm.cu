@@ -2013,16 +2013,105 @@ __global__ void k_cp_dom(Ptrs p, GPPtrs g, CPPtrs c, int iter, int *nsearch) {
     }
 }
 
-// the problem family of a batch: coneqp, conelp, gp, cp or cpl
-enum class Kind { QP, LP, GP, CP, CPL };
+// ---- convex QCQPs: cp with f_i = x'P_i x / 2 + q_i'x + r_i (i = 0..mnl), evaluated by the library ----
+// A QC batch is a CP batch whose F the library knows.  Per slot, G holds the stacked [P_0; ...; P_mnl] (symmetric,
+// nK blocks of n rows) below the m rows of [Df[1:]; G], where a GP's F lies, so compaction moves them with the rest;
+// gp_eval's GEMV forms u = [P_0 x; ...; P_mnl x] in yv.  q (nK x n) and then r (nK) sit in the state row where a GP's
+// g does.  dom f is all of R^n: no domain rounds.
+// f_i = x'(u_i / 2 + q_i) + r_i into fv at slot b's iterate (FULL) or trial point, one warp per i.  FULL: a non-finite
+// f recorded in bad, Df_0 = u_0 + q_0 into gf0, Df_i = u_i + q_i into G's rows [0, mnl).  Trial, only the problems
+// still searching: newrx's nonlinear part Df'[nz0; nz[:mnl]] into nrx (the GEMVs add G'newzl + A'newy).  256 threads
+template <bool FULL> __global__ void __launch_bounds__(256) k_qc_eval(Ptrs p, GPPtrs g, CPPtrs c) {
+    GP_SETUP
+    if (S.done || (!FULL && T.searching == 0.0)) return;
+    const int n = p.n, nK = g.nK;
+    const double *u = g.yv + (long long)b * g.sumK, *qv = g.g + oc, *r = qv + g.sumK;
+    const double *x = (FULL ? p.x : g.nx) + on;
+    double *f = g.fv + (long long)b * nK;
+    for (int i = warp; i < nK; i += nwarp) {
+        const double *ui = u + (long long)i * n, *qi = qv + (long long)i * n;
+        double a = 0.0;
+        for (int k = lane; k < n; k += 32) a += x[k] * (0.5 * ui[k] + qi[k]);
+        a = warp_sum(a);
+        if (lane == 0) f[i] = a + r[i];
+    }
+    if (!FULL) {
+        for (int j = tid; j < n; j += nt) {
+            double a = T.nz0 * (u[j] + qv[j]);
+            for (int i = 1; i < nK; ++i) a += g.nz[om + i - 1] * (u[(long long)i * n + j] + qv[(long long)i * n + j]);
+            g.nrx[on + j] = a;
+        }
+    } else {
+        for (int j = tid; j < n; j += nt) g.gf0[on + j] = u[j] + qv[j];
+        double *G = g.G + (long long)b * g.sG;
+        for (long long e = tid; e < (long long)g.mnl * n; e += nt) {
+            const long long i = e % g.mnl, j = e / g.mnl;
+            G[i + j * g.ldg] = u[(i + 1) * n + j] + qv[(i + 1) * n + j];
+        }
+        __syncthreads();
+        if (tid == 0) {
+            bool fin = true;
+            for (int i = 0; i < nK; ++i) fin = fin && isfinite(f[i]);
+            if (!fin) atomicMin(c.bad, c.idx[b]);
+        }
+    }
+}
+// rx += Df'[z0; z[:mnl]] at the iterates, from grad f0 and G's rows [0, mnl) as k_qc_eval<true> left them (after
+// k_gp_res_begin; the GEMVs add G'zl + A'y)
+__global__ void k_qc_rx(Ptrs p, GPPtrs g) {
+    GP_SETUP
+    if (S.done) return;
+    const double *G = g.G + (long long)b * g.sG;
+    for (int j = tid; j < p.n; j += nt) {
+        double a = T.z0 * g.gf0[on + j];
+        for (int i = 0; i < g.mnl; ++i) a += p.z[om + i] * G[i + (long long)j * g.ldg];
+        p.rx[on + j] += a;
+    }
+}
+// H = z0 P_0 + sum_i z_i P_i at the iterates into P's lower triangle, one 32 x 32 tile (bi >= bj) per CTA, grid
+// (nb (nb + 1) / 2, Bact), 256 threads; each entry sums its nK terms in order.  MIRROR (refinement > 0, whose residual
+// multiplies by all of H): the tile's transpose into the upper triangle too, through shared memory
+template <bool MIRROR> __global__ void __launch_bounds__(256) k_qc_hessian(Ptrs p, GPPtrs g, CPPtrs c) {
+    const int b = blockIdx.y, tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
+    const int n = p.n, nb = (n + 31) / 32;
+    int t = blockIdx.x, bj = 0;
+    while (t >= nb - bj) { t -= nb - bj; ++bj; }
+    const int bi = bj + t;
+    const double z0 = gp_scal(g, (long long)b * p.L).z0, *z = p.z + (long long)b * p.m;
+    const double *Ps = g.G + (long long)b * g.sG + p.m;
+    double *P = c.P + (long long)b * c.sP;
+    __shared__ double tile[32][33];
+    const int i = bi * 32 + tx;
+    for (int q = ty; q < 32; q += 8) {                   // columns of H, coalesced down them
+        const int j = bj * 32 + q;
+        if (i < n && j <= i) {
+            const double *e = Ps + i + (long long)j * g.ldg;
+            double a = z0 * e[0];
+            for (int k = 1; k < g.nK; ++k) a += z[k - 1] * e[(long long)k * n];
+            P[i + (long long)j * c.ldp] = a;
+            if (MIRROR) tile[tx][q] = a;
+        }
+    }
+    if (!MIRROR) return;
+    __syncthreads();
+    for (int q = ty; q < 32; q += 8) {                   // H(j, i) = H(i, j) for i > j, coalesced along j
+        const int ii = bi * 32 + q, j = bj * 32 + tx;
+        if (ii < n && j < ii) P[j + (long long)ii * c.ldp] = tile[q][tx];
+    }
+}
+
+// the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
+enum class Kind { QP, LP, GP, CP, CPL, QC };
 }  // namespace
 
 struct cvxb_batch {
     Kind kind = Kind::QP;
-    // GP, CP and cpl batches run the lock-step cpl (solve_cpl) with gq's per-slot state
-    bool cpl_loop() const { return kind == Kind::GP || kind == Kind::CP || kind == Kind::CPL; }
+    // GP, CP, cpl and QC batches run the lock-step cpl (solve_cpl) with gq's per-slot state
+    bool cpl_loop() const { return kind == Kind::GP || kind == Kind::CP || kind == Kind::CPL || kind == Kind::QC; }
     // CP and cpl batches evaluate the caller's F through cfn, which calls back to the host
     bool calls_back() const { return kind == Kind::CP || kind == Kind::CPL; }
+    // CP, cpl and QC batches start from a loaded x0 and check that f is finite at the iterates
+    bool from_x0() const { return calls_back() || kind == Kind::QC; }
     int device = 0, B = 0, n = 0, m = 0;
     long long ldg = 0, ldp = 0, ldk = 0;
     long long sG = 0, sP = 0, sK = 0, sInv = 0;
@@ -2081,8 +2170,10 @@ struct cvxb_batch {
     GPPtrs gq{};
     DevBuf<double> gpv, gph, gpg;
     DevBuf<int> koff;
+    long long glen = 0;              // gpg's doubles per problem: a GP's sum K, a QC batch's nK n + nK (q and r)
     // convex programs (cvxb_batch_create_cp): gq of a GP batch without F (sum K = 0, nK = mnl + 1); the callback's
-    // buffers in cpv, x0 in problem order in cpx0, slot -> load index and the non-finite flag in cpi
+    // buffers in cpv, x0 in problem order in cpx0, slot -> load index and the non-finite flag in cpi.  A QC batch
+    // (cvxb_batch_create_qcqp) has cpx0 and cpi, and the GP batch's F rows and gpg for its P_i, q_i and r_i
     CPPtrs cq{};
     DevBuf<double> cpv, cpx0;
     DevBuf<int> cpi;
@@ -2109,9 +2200,9 @@ int state_alloc(cvxb_batch *b) {
     const long long cone = p.nq ? ev(sumq) + ev(p.nq) : 0, ref = p.refinement ? 2 * n2 + 5 * m2 + 2 * p2 : 0;
     const long long lps = b->kind == Kind::LP ? ev(sizeof(LPScal) / sizeof(double)) : 0;
     const long long sb = p.ns ? 2 * ev(b->sums2) + 2 * ev(b->sums) : 0;     // r rti (sum ms²) | sigs sigz (sum ms)
-    // gp: g (sum K) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20 dz20 l0 d0 di0 rz0 (m), and with
-    // cones v0 (sum q) | beta0 (nq), with 's' blocks r0 rti0 (sum s²)
-    const long long gpl = b->cpl_loop() ? ev(b->gq.sumK) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
+    // gp: g (glen: a GP's sum K, a QC batch's q and r) | GPScal | x0 dx0 rx0 (n) | y0 dy0 ry0 (p) | s0 z0 ds0 dz0 ds20
+    // dz20 l0 d0 di0 rz0 (m), and with cones v0 (sum q) | beta0 (nq), with 's' blocks r0 rti0 (sum s²)
+    const long long gpl = b->cpl_loop() ? ev(b->glen) + ev(sizeof(GPScal) / sizeof(double)) + 3 * n2 + 3 * p2 + 10 * m2 : 0;
     const long long qsv = gpl ? cone : 0, ssv = gpl && p.ns ? 2 * ev(b->sums2) : 0;
     const long long L = cone + sb + ref + lps + gpl + qsv + ssv;
     if (b->L == L) return 0;
@@ -2138,7 +2229,7 @@ int state_alloc(cvxb_batch *b) {
     if (lps) p.lps = r;
     if (gpl) {
         GPPtrs &g = b->gq;
-        g.g = r; r += ev(g.sumK); g.gs = r; r += ev(sizeof(GPScal) / sizeof(double));
+        g.g = r; r += ev(b->glen); g.gs = r; r += ev(sizeof(GPScal) / sizeof(double));
         for (double **v : {&g.x0, &g.dx0, &g.rx0}) { *v = r; r += n2; }
         for (double **v : {&g.y0, &g.dy0, &g.ry0}) { *v = r; r += p2; }
         for (double **v : {&g.s0, &g.z0, &g.ds0, &g.dz0, &g.ds20, &g.dz20, &g.l0, &g.d0, &g.di0, &g.rz0}) { *v = r; r += m2; }
@@ -2608,27 +2699,33 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
 }
 
 // ---- geometric programs: the lock-step cpl (cvxprog.py:622-1356) of gp's epigraph problem ----
-// F(x) over the active slots at x (slot k at x + k*sx): yv = F x, then k_gp_eval (full: with Df, H's rows and weights)
+// F(x) over the active slots at x (slot k at x + k*sx): yv = F x, then k_gp_eval (full: with Df, H's rows and weights).
+// QC: yv = [P_0 x; ...; P_mnl x], then k_qc_eval (full: with Df; trial: with newrx's nonlinear part)
 int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact;
     GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = sx; gf.sy = g.sumK;
     CVXB_TRY(gemv_n(g.sumK, b->n, g.G + b->m, g.ldg, nullptr, x, 1.0, 0.0, g.yv, b->gemv_ws.p, b->st, gf));
-    if (full) k_gp_eval<true><<<dim3(g.nK, B), 256, 0, b->st>>>(b->p, g, trial);
+    if (b->kind == Kind::QC) {
+        if (full) k_qc_eval<true><<<B, 256, 0, b->st>>>(b->p, g, b->cq);
+        else k_qc_eval<false><<<B, 256, 0, b->st>>>(b->p, g, b->cq);
+    } else if (full) k_gp_eval<true><<<dim3(g.nK, B), 256, 0, b->st>>>(b->p, g, trial);
     else k_gp_eval<false><<<dim3(g.nK, B), 256, 0, b->st>>>(b->p, g, trial);
     count_launch();
     return 0;
 }
 // r += Df'[z0; znl] + G' zl (+ A' y) (slot k's z at z + k*m).  GP: Df'[z0; znl] = F'(z_i y) from k_gp_eval's
 // weights.  CP: at the iterates (full) k_cp_rx adds it; at trial points k_cp_take<false> has written it into r.
-// SDP: G' trisc(zl) (misc.sgemv), the row weights rw on the 's' rows
+// QC: likewise k_qc_rx and k_qc_eval<false>.  SDP: G' trisc(zl) (misc.sgemv), the row weights rw on the 's' rows
 template <bool EQ, bool EPI = true, bool SDP = false>
 int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact, n = b->n, m = b->m, ml = m - g.mnl;
-    if (!b->calls_back()) {
+    if (b->kind == Kind::GP) {
         GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = g.sumK; gf.sy = n;
         CVXB_TRY(gemv_t(g.sumK, n, g.G + m, g.ldg, nullptr, g.wv, 1.0, 1.0, r, b->st, gf));
+    } else if (full && b->kind == Kind::QC) {
+        k_qc_rx<<<B, 256, 0, b->st>>>(b->p, g); count_launch();
     } else if (full) {
         k_cp_rx<EPI><<<B, 256, 0, b->st>>>(b->p, g, b->cq); count_launch();
     }
@@ -2656,6 +2753,15 @@ int gp_hessian(cvxb_batch *b) {
     if (b->B == 1) h.splitk_ws = b->cw.splitk_ws.p;
     CVXB_TRY(dmma_gemm(h, b->st));
     if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, b->st));
+    return 0;
+}
+// a QC batch's H = z0 P_0 + sum_i z_i P_i at the iterates, mirrored when the refinement's residual multiplies by it
+int qc_hessian(cvxb_batch *b) {
+    const int nb = (b->n + 31) / 32;
+    const dim3 grid(nb * (nb + 1) / 2, b->Bact);
+    if (b->p.refinement) k_qc_hessian<true><<<grid, 256, 0, b->st>>>(b->p, b->gq, b->cq);
+    else k_qc_hessian<false><<<grid, 256, 0, b->st>>>(b->p, b->gq, b->cq);
+    count_launch();
     return 0;
 }
 // the caller's F over the active slots at x (slot k at x + k*n); full: at the iterates, with z = [z0; z[:mnl]] and H
@@ -2771,14 +2877,16 @@ int gp_line_search(cvxb_batch *b, int i, int it) {
     return 0;
 }
 // K = H + [Df[1:]; G]' diag(di²) [Df[1:]; G] (+ A'A) factored from F(x) at the slots' iterates (a GP's H formed
-// into P first; a CP's is there from cpl_eval_full)
+// into P first, a QC batch's too; a CP's is there from cpl_eval_full)
 int cpl_factor(cvxb_batch *b, bool first) {
-    if (!b->calls_back()) CVXB_TRY(gp_hessian(b));
+    if (b->kind == Kind::GP) CVXB_TRY(gp_hessian(b));
+    else if (b->kind == Kind::QC) CVXB_TRY(qc_hessian(b));
     return batch_factor(b, !first);
 }
 // the lock-step cpl of a GP or CP batch's epigraph problem (EPI) or of a cpl batch's own problem (EPI false, with 'q'
 // cones when CONES).  A CP or cpl batch starts from its x0 and backtracks each step into dom f before the line search;
-// it calls back to the host, so the loop is never captured into a graph.  Without the epigraph row the scaling and
+// it calls back to the host, so the loop is never captured into a graph.  A QC batch starts from its x0 too, and
+// takes no domain rounds: its dom f is R^n, and the reference discards the values of its domain evaluation.  Without the epigraph row the scaling and
 // the update are coneqp's (k_scaling, k_update: cpl's compute_scaling, ssqr, update_scaling and unscaling are
 // coneqp's, and so is mu = gap / (mnl + ml + len(q)), :978).  SDP (a cpl batch with 's' blocks, which follow the 'q'
 // rows): the 's' parts of those are the SDP QP batch's, with k_s_nt_compute before iteration 0's scaling, sdot /
@@ -2791,15 +2899,15 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     const int ml = m - g.mnl;
-    const bool cb = b->calls_back();
+    const bool cb = b->calls_back(), x0 = b->from_x0();
     int B = b->B;
     CVXB_TRY(solve_begin(b));
-    // every problem in its own slot (restore_order ran): g into the state row, or x0 into x
-    if (!cb)
-        CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, g.sumK * sizeof(double),
-                                    g.sumK * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
+    // every problem in its own slot (restore_order ran): g (a QC batch's q and r) into the state row, x0 into x
+    if (b->glen)
+        CVXB_CUDA(cudaMemcpy2DAsync(g.g, b->L * sizeof(double), b->gpg.p, b->glen * sizeof(double),
+                                    b->glen * sizeof(double), B, cudaMemcpyDeviceToDevice, st));
     k_gp_init<CONES, SDP><<<B, T, 0, st>>>(p, g); count_launch();
-    if (cb) {
+    if (x0) {
         CVXB_CUDA(cudaMemcpyAsync(p.x, b->cpx0.p, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, st));
         CVXB_TRY(cp_upload_idx(b));
         CVXB_CUDA(cudaMemsetAsync(b->cq.bad, 0x7f, sizeof(int), st));
@@ -2825,7 +2933,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         count_launch();
         int ndone = 0, bad = b->B;
         bool moved = false;
-        CVXB_TRY(poll_done(b, flags, pairs, ndone, moved, cb ? &bad : nullptr));
+        CVXB_TRY(poll_done(b, flags, pairs, ndone, moved, x0 ? &bad : nullptr));
         if (bad < b->B) {                // the reference keeps its iterates inside dom f
             if (it == 0) set_error("batch_solve: problem %d: x0 not in the domain of f", bad);
             else set_error("batch_solve: problem %d: f is not finite at the iterate of iteration %d", bad, it);
@@ -2834,7 +2942,7 @@ int solve_cpl(cvxb_batch *b, int maxiters, double abstol, double reltol, double 
         if (ndone >= B) break;
         B = b->Bact;
         if (moved) {                     // F(x)'s per-slot results stay put
-            if (cb) CVXB_TRY(cp_upload_idx(b));
+            if (x0) CVXB_TRY(cp_upload_idx(b));
             CVXB_TRY(cpl_eval_full<EPI>(b));
         }
         if (SDP && it == 0) { k_s_nt_compute<<<dim3(p.ns, B), SB_T, 0, st>>>(p); count_launch(); }
@@ -2944,15 +3052,15 @@ int check_args(const char *fn, Kind kind, cvxb_batch **out, int nprob, int n, in
 // a batch of the given kind, once check_args has passed its arguments: QPs, or cone LPs (no P; q holds c), with the
 // cones of dims ('l', 'q' and with sdp 's' blocks) and p equality rows; or a GP, CP or cpl batch, whose G begins with
 // the mnl rows of Df (counted among the 'l' rows), f having nK = mnl + 1 rows with gp's and cp's epigraph row or nK =
-// mnl (cpl).  K: a GP's term counts; the sum K rows of its F go below G's m rows.  Every buffer of the kind, then the
-// state row
+// mnl (cpl).  K: a GP's term counts; the sum K rows of its F go below G's m rows, where a QC batch keeps its nK n
+// rows of P_i.  Every buffer of the kind, then the state row
 int create(cvxb_batch **out, const char *fn, Kind kind, int nprob, int n, int p, int mnl, const cvxb_dims *dims,
            bool sdp, int device, const int *K = nullptr) {
     long long mlq = 0, mm = 0, mpk = 0;
     CVXB_TRY(check_args(fn, kind, out, nprob, n, p, mnl, dims, sdp, mlq, mm, mpk));
     CVXB_TRY(check_device(device));
     const int m = (int)mm, ml = mnl + dims->ml, nK = kind == Kind::CPL ? mnl : mnl + 1;
-    long long sumK = 0;
+    long long sumK = kind == Kind::QC ? (long long)nK * n : 0;        // QC: nK blocks P_i of n rows
     for (int i = 0; K && i < nK; ++i) sumK += K[i];
     std::unique_ptr<cvxb_batch> b(new cvxb_batch());
     b->kind = kind; b->device = device; b->B = nprob; b->n = n; b->m = m;
@@ -3074,15 +3182,20 @@ int create(cvxb_batch **out, const char *fn, Kind kind, int nprob, int n, int p,
     if (b->cpl_loop()) {
         g.nK = nK; g.sumK = (int)sumK; g.mnl = mnl;
         g.ldg = b->ldg; g.sG = b->sG; g.G = b->G.p;
-        // per slot: yv wv hw (sum K) | fv (nK) | gf0 nx nrx (n) | ny (p) | ds2 dz2 nz ns (m)
-        const size_t len = 3 * sumK + nK + 3 * (size_t)n + p + 4 * (size_t)m;
+        // per slot: yv wv hw (sum K; a QC batch has no softmax weights: wv and hw empty) | fv (nK) | gf0 nx nrx (n) |
+        // ny (p) | ds2 dz2 nz ns (m)
+        const size_t sw = kind == Kind::GP ? sumK : 0;
+        const size_t len = sumK + 2 * sw + nK + 3 * (size_t)n + p + 4 * (size_t)m;
         CVXB_TRY(b->gpv.alloc(B * len));
         CVXB_CUDA(cudaMemset(b->gpv.p, 0, B * len * sizeof(double)));
         v = b->gpv.p;
-        g.yv = take(sumK); g.wv = take(sumK); g.hw = take(sumK); g.fv = take(nK);
+        g.yv = take(sumK); g.wv = take(sw); g.hw = take(sw); g.fv = take(nK);
         g.gf0 = take(n); g.nx = take(n); g.nrx = take(n); g.ny = take(p);
         g.ds2 = take(m); g.dz2 = take(m); g.nz = take(m); g.ns = take(m);
-        q.refinement = m > 0 || b->calls_back() ? 1 : 0;     // cpl's default (cvxprog.py:422)
+        q.refinement = m > 0 || b->from_x0() ? 1 : 0;     // cpl's default (cvxprog.py:422)
+        // per problem, in problem order: a GP's g; a QC batch's q (nK x n), then r (nK)
+        b->glen = kind == Kind::GP ? sumK : kind == Kind::QC ? sumK + nK : 0;
+        if (b->glen) CVXB_TRY(b->gpg.alloc(B * b->glen));
     }
     if (kind == Kind::GP) {
         g.ldh = (sumK + 1) & ~1LL; g.sH = g.ldh * n;
@@ -3092,21 +3205,22 @@ int create(cvxb_batch **out, const char *fn, Kind kind, int nprob, int n, int p,
         CVXB_CUDA(cudaMemcpy(b->koff.p, off.data(), (nK + 1) * sizeof(int), cudaMemcpyHostToDevice));
         g.koff = b->koff.p;
         CVXB_TRY(b->gph.alloc(B * g.sH));
-        CVXB_TRY(b->gpg.alloc(B * sumK));
         g.Hr = b->gph.p;
     }
-    if (b->calls_back()) {                        // the callback's buffers, x0 and the slot -> problem map
+    CPPtrs &c = b->cq;
+    if (b->from_x0()) {                           // x0, the slot -> problem map and the non-finite flag
+        CVXB_TRY(b->cpx0.alloc(B * (size_t)n));
+        CVXB_TRY(b->cpi.alloc(B + 1));
+        c.idx = b->cpi.p; c.bad = b->cpi.p + B;
+        c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
+    }
+    if (b->calls_back()) {                        // the callback's buffers
         const size_t nn = n;
         // per slot: the callback's f, z (nK), Df (nK x n) and H (n x n)
         const size_t len = 2 * nK + nK * nn + nn * nn;
         CVXB_TRY(b->cpv.alloc(B * len));
         CVXB_CUDA(cudaMemset(b->cpv.p, 0, B * len * sizeof(double)));
-        CVXB_TRY(b->cpx0.alloc(B * nn));
-        CVXB_TRY(b->cpi.alloc(B + 1));
-        CPPtrs &c = b->cq;
         c.f = b->cpv.p; c.z = c.f + B * nK; c.Df = c.z + B * nK; c.H = c.Df + B * nK * nn;
-        c.idx = b->cpi.p; c.bad = b->cpi.p + B;
-        c.P = b->P.p; c.ldp = b->ldp; c.sP = b->sP;
     }
     CVXB_TRY(state_alloc(b.get()));
     *out = b.release();
@@ -3213,6 +3327,19 @@ int cvxb_batch_create_cp(cvxb_batch **out, int nprob, int n, int mnl, int ml, in
     return create(out, "batch_create_cp", Kind::CP, nprob, n, p, mnl, &d, false, device);
 }
 
+int cvxb_batch_create_qcqp(cvxb_batch **out, int nprob, int n, int mnl, int ml, int p, int device) {
+    if (out) *out = nullptr;
+    // G's rows: [Df[1:]; G] and below them the nK = mnl + 1 blocks P_i of n rows, a GP's F with K = (n, ..., n);
+    // create counts them
+    if ((long long)mnl + ml + 1 + ((long long)mnl + 1) * (n > 0 ? n : 0) > (1LL << 30)) {
+        set_error("batch_create_qcqp: too many rows");
+        return CVXB_E_ARG;
+    }
+    cvxb_dims d{};
+    d.ml = ml;
+    return create(out, "batch_create_qcqp", Kind::QC, nprob, n, p, mnl, &d, false, device);
+}
+
 int cvxb_batch_create_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device) {
     return create(out, "batch_create_cpl", Kind::CPL, nprob, n, p, mnl, dims, false, device);
 }
@@ -3232,8 +3359,8 @@ int cvxb_batch_set_cp_eval(cvxb_batch *b, cvxb_cp_eval_fn fn, void *ctx) {
 int cvxb_batch_set_refinement(cvxb_batch *b, int refinement) {
     if (!b || refinement < 0) { set_error("batch_set_refinement: refinement must be a nonnegative integer"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
-    // a batch without constraint rows takes unrefined steps; a CP batch always has cp's epigraph row
-    b->p.refinement = b->m > 0 || b->calls_back() ? refinement : 0;
+    // a batch without constraint rows takes unrefined steps; a CP or QC batch always has cp's epigraph row
+    b->p.refinement = b->m > 0 || b->from_x0() ? refinement : 0;
     CVXB_TRY(state_alloc(b));
     return 0;
 }
@@ -3251,6 +3378,7 @@ int cvxb_batch_load(cvxb_batch *b, const double *P, const double *q, const doubl
     if (b->kind == Kind::LP) { set_error("batch_load: a cone LP batch is loaded with cvxb_batch_load_lp"); return CVXB_E_ARG; }
     if (b->kind == Kind::GP) { set_error("batch_load: a GP batch is loaded with cvxb_batch_load_gp"); return CVXB_E_ARG; }
     if (b->calls_back()) { set_error("batch_load: a CP batch is loaded with cvxb_batch_load_cp"); return CVXB_E_ARG; }
+    if (b->kind == Kind::QC) { set_error("batch_load: a QCQP batch is loaded with cvxb_batch_load_qcqp"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(b->device));
     const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     const size_t n = b->n;
@@ -3299,6 +3427,27 @@ int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const 
     return load_cpl_common(b, G, h, kind, c);
 }
 
+int cvxb_batch_load_qcqp(cvxb_batch *b, const double *P, const double *q, const double *r, const double *x0,
+                         const double *G, const double *h, int space) {
+    if (!b || !P || !q || !r || (b->m > b->gq.mnl && (!G || !h))) { set_error("batch_load_qcqp: NULL argument"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QC) { set_error("batch_load_qcqp: not a QCQP batch (cvxb_batch_create_qcqp)"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    const cudaMemcpyKind kind = (space == CVXB_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const size_t B = b->B, n = b->n, m = b->m, nK = b->gq.nK, S = b->gq.sumK, gl = b->glen;
+    // [P_0; ...; P_mnl] below the m rows of [Df[1:]; G], each block mirrored from its lower triangle
+    CVXB_CUDA(cudaMemcpy2DAsync(b->G.p + m, b->ldg * sizeof(double), P, S * sizeof(double), S * sizeof(double),
+                                n * B, kind, b->st));
+    for (size_t i = 0; i < nK; ++i) CVXB_TRY(symmetrize_lower(b->n, b->G.p + m + i * n, b->ldg, b->B, b->sG, b->st));
+    // q and r in problem order, copied into the state row by each solve
+    CVXB_CUDA(cudaMemcpy2DAsync(b->gpg.p, gl * sizeof(double), q, S * sizeof(double), S * sizeof(double), B, kind,
+                                b->st));
+    CVXB_CUDA(cudaMemcpy2DAsync(b->gpg.p + S, gl * sizeof(double), r, nK * sizeof(double), nK * sizeof(double), B,
+                                kind, b->st));
+    if (x0) CVXB_CUDA(cudaMemcpyAsync(b->cpx0.p, x0, B * n * sizeof(double), kind, b->st));
+    else CVXB_CUDA(cudaMemsetAsync(b->cpx0.p, 0, B * n * sizeof(double), b->st));
+    return load_cpl_common(b, G, h, kind);
+}
+
 int cvxb_batch_ls_rounds(cvxb_batch *b) { return b ? b->ls_rounds : CVXB_E_ARG; }
 
 int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int space) {
@@ -3323,6 +3472,7 @@ int cvxb_batch_load_start(cvxb_batch *b, const double *x, const double *s, const
     if (!b) { set_error("batch_load_start: batch is NULL"); return CVXB_E_ARG; }
     if (b->kind == Kind::GP) { set_error("batch_load_start: gp takes no starting point"); return CVXB_E_ARG; }
     if (b->calls_back()) { set_error("batch_load_start: cp and cpl start from the x0 of their load"); return CVXB_E_ARG; }
+    if (b->kind == Kind::QC) { set_error("batch_load_start: qcqp starts from the x0 of its load"); return CVXB_E_ARG; }
     if (b->kind == Kind::LP && ((!x) != (!s) || (y && !z) || (!x && !z))) {
         set_error("batch_load_start: a cone LP start is x and s (primalstart), z with an optional y (dualstart), or "
                   "both");
@@ -3367,7 +3517,7 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
         return with_flags([&](auto SDP, auto CONES, auto EQ) {
             return solve_cpl<EQ, false, CONES, SDP>(b, maxiters, abstol, reltol, feastol);
         }, sdp, cones, eq);
-    if (b->cpl_loop())                            // GP, CP: the epigraph problem, 'l' rows only
+    if (b->cpl_loop())                            // GP, CP, QC: the epigraph problem, 'l' rows only
         return eq ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
                   : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
     return with_flags([&](auto SDP, auto LP, auto EQ, auto CONES) {

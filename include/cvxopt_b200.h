@@ -494,6 +494,31 @@ int cvxb_batch_load_cpl(cvxb_batch *b, const double *c, const double *x0, const 
  * of blocks of positive order; all of it is counted by cvxb_device_bytes and freed by cvxb_batch_destroy.  Dims
  * without an 's' block of positive order run exactly what cvxb_batch_create_cpl's batch runs. */
 int cvxb_batch_create_sdp_cpl(cvxb_batch **out, int nprob, int n, int mnl, const cvxb_dims *dims, int p, int device);
+/* batch of convex QCQPs (B x solvers.cp(F, G, h, dims={'l': ml}, A, b) with its default kktsolver, F's functions
+ * quadratic):
+ *     minimize  f0(x)  s.t.  fi(x) <= 0 (i = 1..mnl),  G x <= h,  A x = b,   fi(x) = x'Pi x / 2 + qi'x + ri
+ * with mnl, ml and p shared by the batch.  It is the CP batch with F evaluated by the library's own kernels: no
+ * evaluator, no host callback, and no domain rounds (dom f is R^n).  Every Pi is the caller's promise to be positive
+ * semidefinite; it is not checked.  mnl = 0 and P0 = 0 are allowed.  Refused before the device with CVXB_E_ARG: what
+ * cvxb_batch_create_cp refuses, and (mnl + 1) n + mnl + ml + 1 > 2^30 ("too many rows").  Load it with
+ * cvxb_batch_load_qcqp (and cvxb_batch_load_eq when p > 0); cvxb_batch_load, load_lp, load_gp, load_cp, load_cpl,
+ * load_start and set_cp_eval on it are CVXB_E_ARG.  Solve, set_refinement (default 1), results, results_y, stats,
+ * ls_rounds and destroy are the CP batch's calls with its semantics (status, s and z as [snl; sl] and [znl; zl], the
+ * primal objective t, the rank error at iteration 0, "problem %d: x0 not in the domain of f" for a non-finite f at
+ * x0).  Device memory per problem, in doubles, with m = mnl + ml, nK = mnl + 1, S = nK n and ev() rounding up to
+ * even: what cvxb_batch_create_eq's batch of the same n, p and dims {'l': m} holds with refinement 1, except that G
+ * is ev(m + S) x n (the stacked P0..Pmnl below [Df[1:]; G]) and the GEMV workspace holds max(m, S) rows, plus
+ * S + nK + 3n + p + 4m (P x, f, grad f0, the unscaled steps and the line search's trial point), S + nK (q and r), n
+ * (x0), ev(S + nK) + 56 + 3 ev(n) + 3 ev(p) + 10 ev(m) in the state row (q and r, the scalars and the line search's
+ * saved state) and one int (slot -> problem); and one int shared by the batch; all of it is counted by
+ * cvxb_device_bytes and freed by cvxb_batch_destroy. */
+int cvxb_batch_create_qcqp(cvxb_batch **out, int nprob, int n, int mnl, int ml, int p, int device);
+/* QCQP batch only: P nprob x ((mnl + 1) n x n column-major, ld (mnl + 1) n), the blocks P0..Pmnl stacked by rows,
+ * only each block's lower triangle read; q nprob x (mnl + 1) x n (q0 first); r nprob x (mnl + 1); x0 nprob x n, or
+ * NULL for 0; G nprob x (ml x n column-major, ld ml), h nprob x ml, NULL when ml = 0.  A and b come through
+ * cvxb_batch_load_eq. */
+int cvxb_batch_load_qcqp(cvxb_batch *b, const double *P, const double *q, const double *r, const double *x0,
+                         const double *G, const double *h, int space);
 
 #ifdef __cplusplus
 }
