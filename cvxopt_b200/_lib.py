@@ -130,6 +130,7 @@ _SIGS = {
     "cvxb_batch_load_eq": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_load_lp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_results_y": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "cvxb_batch_adjoint": (C.c_int, [C.c_void_p] + [C.c_void_p] * 9 + [C.c_int]),
     "cvxb_batch_load_start": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "cvxb_batch_clear_start": (C.c_int, [C.c_void_p]),
     "cvxb_batch_set_refinement": (C.c_int, [C.c_void_p, C.c_int]),

@@ -166,6 +166,26 @@ def _sdp_dims(dims, m=None):
     return d, keep, cdim
 
 
+ADJOINT_KEYS = ("P", "q", "G", "h", "A", "b")
+
+
+def _adjoint_args(gx, gy, gz, want, B, n, p, m):
+    """the gradients gx (B, n), gy (B, p), gz (B, m) as contiguous float64 arrays (None stays None) and `want` as a
+    tuple of ADJOINT_KEYS; a wrong shape or an unknown key is a TypeError"""
+    want = tuple(want)
+    unknown = [k for k in want if k not in ADJOINT_KEYS]
+    if unknown:
+        raise TypeError("want: unknown keys %s; the keys are %s" % (unknown, ADJOINT_KEYS))
+    gs = []
+    for name, a, k in (("gx", gx, n), ("gy", gy, p), ("gz", gz, m)):
+        if a is not None:
+            a = np.ascontiguousarray(np.asarray(a, dtype=np.float64))
+            if a.shape != (B, k):
+                raise TypeError("%s must have shape (%d, %d)" % (name, B, k))
+        gs.append(a)
+    return gs, want
+
+
 class QPBatch:
     """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
@@ -278,6 +298,30 @@ class QPBatch:
         return {"x": x, "y": y, "s": s, "z": z, "status": [STATUS[int(k)] for k in status],
                 "status_code": status, "iterations": iters, "primal objective": pobj,
                 "dual objective": dobj}
+
+    def adjoint(self, gx, gy=None, gz=None, want=ADJOINT_KEYS):
+        """derivatives of the last solve's results for a loss L with gradients gx = dL/dx (B, n), gy = dL/dy (B, p)
+        and gz = dL/dz (B, m), None meaning zero (cvxb_batch_adjoint).  Returns host arrays for the keys in `want`:
+        P (B, n, n, symmetric), q (B, n), G (B, m, n), h (B, m), A (B, p, n) and b (B, p), each dL/d(that input).
+        A problem whose status is not 'optimal' gets NaN.  QP batches whose rows are all 'l' only: any other batch
+        raises NotImplementedError, and a batch not solved since its last load raises ValueError."""
+        B, n, m, p = self.B, self.n, self.m, self.p
+        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m)
+        # C's outputs ux, uy, uz, dP, dG, dA; the matrices column-major per problem
+        shapes = {"q": (B, n), "b": (B, p), "h": (B, m), "P": (B, n, n), "G": (B, n, m), "A": (B, n, p)}
+        bufs = {k: np.empty(shapes[k]) for k in want}
+        ptrs = [None if a is None else a.ctypes.data for a in gs]
+        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("q", "b", "h", "P", "G", "A")]
+        self.adjoint_ptr(*ptrs, space=_lib.HOST)
+        out = {}
+        for k, v in bufs.items():
+            out[k] = -v if k == "q" else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
+        return out
+
+    def adjoint_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dG=None, dA=None,
+                    space=_lib.DEVICE):
+        """cvxb_batch_adjoint on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_adjoint(self._h, gx, gy, gz, ux, uy, uz, dP, dG, dA, space), "batch_adjoint")
 
     def stats(self):
         ms, it = C.c_double(), C.c_int()
@@ -399,6 +443,16 @@ class QPBatchGroup:
             for key in out:
                 out[key][ix] = r[key]
         out["status"] = [STATUS[int(k)] for k in out["status_code"]]
+        return out
+
+    def adjoint(self, gx, gy=None, gz=None, want=ADJOINT_KEYS):
+        """QPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
+        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m)
+        out = {}
+        for ix, part in zip(self.idx, self.parts):
+            r = part.adjoint(*(None if a is None else a[ix] for a in gs), want=want)
+            for k, v in r.items():
+                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
         return out
 
     def stats(self):

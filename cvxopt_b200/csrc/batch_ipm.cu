@@ -2100,6 +2100,93 @@ template <bool MIRROR> __global__ void __launch_bounds__(256) k_qc_hessian(Ptrs 
     }
 }
 
+// ---- the adjoint of an 'l'-only QP batch's solution (cvxb_batch_adjoint) ----
+// Differentiating P x + q + A'y + G'z = 0, A x = b, G x + s = h and s o z = 0 at the returned iterate gives the KKT
+// matrix M = [P A' G'; A 0 0; G 0 -W'W], W'W = diag(s / z).  For a loss's gradients (gx, gy, gz) one reduced solve
+// gives M [ux; uy; uz] = [gx; gy; gz], and then dL/dq = -ux, dL/db = uy, dL/dh = uz, dL/dP = -(ux x' + x ux') / 2,
+// dL/dG = -(z ux' + uz x'), dL/dA = -(y ux' + uy x').  A problem whose results are not optimal, or whose adjoint
+// factorisation failed, gets NaN in every output.
+__device__ __forceinline__ bool adj_bad(const Ptrs &p, const int *info, int b) {
+    return p.sc[b].status != 1 || info[b] > 0 || (p.neq > 0 && p.infop[b] > 0);
+}
+// slot b's right-hand side from problem perm[b]'s gradients (nullptr: zero): dx := gx, dy := gy, bzp := W^{-T} gz, with
+// the scaling of the returned s and z: d = sqrt(s / z), di = 1 / d, di2 = z / s; and g in (rx, ry, rz) for the residual
+__global__ void k_adj_rhs(Ptrs p, const double *gx, const double *gy, const double *gz, const int *perm) {
+    const int b = blockIdx.x;
+    const long long on = (long long)b * p.n, om = (long long)b * p.m, oq = (long long)b * p.neq, k = perm[b];
+    for (int i = threadIdx.x; i < p.n; i += blockDim.x) p.dx[on + i] = p.rx[on + i] = gx ? gx[k * p.n + i] : 0.0;
+    for (int i = threadIdx.x; i < p.neq; i += blockDim.x) p.dy[oq + i] = p.ry[oq + i] = gy ? gy[k * p.neq + i] : 0.0;
+    for (int i = threadIdx.x; i < p.m; i += blockDim.x) {
+        const double s = p.s[om + i], z = p.z[om + i], d = sqrt(s / z), di = 1.0 / d, g = gz ? gz[k * p.m + i] : 0.0;
+        p.d[om + i] = d; p.di[om + i] = di; p.di2[om + i] = z / s;
+        p.bzp[om + i] = di * g; p.rz[om + i] = g;
+    }
+}
+// after the first solve: dz := uz = di o bzp (batch_solve leaves W uz in bzp)
+__global__ void k_adj_uz(Ptrs p) {
+    const long long om = (long long)blockIdx.x * p.m;
+    for (int i = threadIdx.x; i < p.m; i += blockDim.x) p.dz[om + i] = p.di[om + i] * p.bzp[om + i];
+}
+// once the GEMVs have left rz = gz - G ux: rz += W'W uz, the residual's last block, and bzp := W^{-T} rz for the
+// refinement solve
+__global__ void k_adj_res(Ptrs p) {
+    const long long om = (long long)blockIdx.x * p.m;
+    for (int i = threadIdx.x; i < p.m; i += blockDim.x) {
+        const double r = p.rz[om + i] + p.d[om + i] * p.d[om + i] * p.dz[om + i];
+        p.bzp[om + i] = p.di[om + i] * r;
+    }
+}
+// after the refinement solve (the correction in rx, ry and W duz in bzp): ux := dx + rx, uy := dy + ry and uz := dz +
+// di o bzp, uz kept in bzp for k_adj_grad; ux, uy and uz into problem perm[b]'s rows of the outputs that are given
+__global__ void k_adj_vecs(Ptrs p, double *ux, double *uy, double *uz, const int *perm, const int *info) {
+    const int b = blockIdx.x;
+    const long long on = (long long)b * p.n, om = (long long)b * p.m, oq = (long long)b * p.neq, k = perm[b];
+    const bool bad = adj_bad(p, info, b);
+    for (int i = threadIdx.x; i < p.n; i += blockDim.x) p.dx[on + i] += p.rx[on + i];
+    for (int i = threadIdx.x; i < p.neq; i += blockDim.x) p.dy[oq + i] += p.ry[oq + i];
+    for (int i = threadIdx.x; i < p.m; i += blockDim.x) {
+        const double u = p.dz[om + i] + p.di[om + i] * p.bzp[om + i];
+        p.bzp[om + i] = u;
+        if (uz) uz[k * p.m + i] = bad ? NAN : u;
+    }
+    if (ux) for (int i = threadIdx.x; i < p.n; i += blockDim.x) ux[k * p.n + i] = bad ? NAN : p.dx[on + i];
+    if (uy) for (int i = threadIdx.x; i < p.neq; i += blockDim.x) uy[k * p.neq + i] = bad ? NAN : p.dy[oq + i];
+}
+// o[c * rows + i] = f(i, c) for the nj columns c of a rows x nj column-major block, contiguous in memory: flat over the
+// CTA, so that short columns keep every thread busy; (c, i) step by the CTA's stride without a division per entry
+template <class F> __device__ __forceinline__ void adj_store(double *o, int rows, int nj, bool bad, F f) {
+    const int qs = blockDim.x / rows, rs = blockDim.x % rows;
+    int c = threadIdx.x / rows, i = threadIdx.x % rows;
+    while (c < nj) {
+        o[(long long)c * rows + i] = bad ? NAN : f(i, c);
+        i += rs; c += qs;
+        if (i >= rows) { i -= rows; ++c; }
+    }
+}
+// dP, dG and dA (nullptr: not written) of problem perm[b] in one pass over columns [j0, j0 + ADJ_TJ), grid
+// (ceil(n / ADJ_TJ), B): the tile's x_j and ux_j in shared memory, the row vectors read down the columns, and each
+// matrix's tile stored as one contiguous run of its column-major layout
+constexpr int ADJ_TJ = 32;
+__global__ void __launch_bounds__(256) k_adj_grad(Ptrs p, double *dP, double *dG, double *dA, const int *perm,
+                                                  const int *info) {
+    const int b = blockIdx.y, j0 = blockIdx.x * ADJ_TJ, nj = min(ADJ_TJ, p.n - j0), n = p.n, m = p.m, pq = p.neq;
+    const long long on = (long long)b * n, om = (long long)b * m, oq = (long long)b * pq, k = perm[b];
+    const double *__restrict__ x = p.x + on, *__restrict__ ux = p.dx + on;
+    const double *__restrict__ z = p.z + om, *__restrict__ uz = p.bzp + om;
+    const double *__restrict__ y = p.y + oq, *__restrict__ uy = p.dy + oq;
+    __shared__ double xs[ADJ_TJ], uxs[ADJ_TJ];
+    if (threadIdx.x < nj) { xs[threadIdx.x] = x[j0 + threadIdx.x]; uxs[threadIdx.x] = ux[j0 + threadIdx.x]; }
+    __syncthreads();
+    const bool bad = adj_bad(p, info, b);
+    // rounded products, no FMA: dP(i, j) and dP(j, i) are the same sum, so both triangles are bitwise symmetric
+    if (dP) adj_store(dP + (k * n + j0) * n, n, nj, bad,
+                      [&](int i, int c) { return -0.5 * __dadd_rn(__dmul_rn(ux[i], xs[c]), __dmul_rn(x[i], uxs[c])); });
+    if (dG && m) adj_store(dG + (k * n + j0) * m, m, nj, bad,
+                           [&](int i, int c) { return -(z[i] * uxs[c] + uz[i] * xs[c]); });
+    if (dA && pq) adj_store(dA + (k * n + j0) * pq, pq, nj, bad,
+                            [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
+}
+
 // the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
 enum class Kind { QP, LP, GP, CP, CPL, QC };
 }  // namespace
@@ -2131,6 +2218,7 @@ struct cvxb_batch {
     cudaStream_t st = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     bool loaded = false;
+    bool solved = false;             // a cvxb_batch_solve completed since the last load (cvxb_batch_adjoint reads it)
     int iters_run = 0;
     int ls_rounds = 0;               // gp: line-search rounds of the last solve
     double solve_ms = 0;
@@ -3232,6 +3320,7 @@ int load_done(cvxb_batch *b) {
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->loaded = true;
     b->eq_loaded = false;
+    b->solved = false;
     for (int i = 0; i < b->B; ++i) b->perm[i] = i;
     b->permuted = false;
     return 0;
@@ -3464,6 +3553,7 @@ int cvxb_batch_load_eq(cvxb_batch *b, const double *A, const double *bvec, int s
     CVXB_CUDA(cudaMemcpyAsync(const_cast<double *>(b->p.beq), bvec, B * pq * sizeof(double), kind, b->st));
     CVXB_CUDA(cudaStreamSynchronize(b->st));
     b->eq_loaded = true;
+    b->solved = false;
     return 0;
 }
 
@@ -3509,20 +3599,85 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
         return CVXB_E_ARG;
     }
     CVXB_CUDA(cudaSetDevice(b->device));
+    b->solved = false;
     CVXB_TRY(restore_order(b));
     if (b->calls_back() && !b->cfn) { set_error("batch_solve: a CP batch needs its F (cvxb_batch_set_cp_eval)"); return CVXB_E_ARG; }
     // SDP: 's' blocks of positive order
     const bool sdp = b->p.ns > 0, lp = b->kind == Kind::LP, eq = b->neq > 0, cones = b->p.nq > 0;
+    int rc = 0;
     if (b->kind == Kind::CPL)
-        return with_flags([&](auto SDP, auto CONES, auto EQ) {
+        rc = with_flags([&](auto SDP, auto CONES, auto EQ) {
             return solve_cpl<EQ, false, CONES, SDP>(b, maxiters, abstol, reltol, feastol);
         }, sdp, cones, eq);
-    if (b->cpl_loop())                            // GP, CP, QC: the epigraph problem, 'l' rows only
-        return eq ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
-                  : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
-    return with_flags([&](auto SDP, auto LP, auto EQ, auto CONES) {
-        return solve<CONES, EQ, LP, SDP>(b, maxiters, abstol, reltol, feastol);
-    }, sdp, lp, eq, cones);
+    else if (b->cpl_loop())                       // GP, CP, QC: the epigraph problem, 'l' rows only
+        rc = eq ? solve_cpl<true>(b, maxiters, abstol, reltol, feastol)
+                : solve_cpl<false>(b, maxiters, abstol, reltol, feastol);
+    else
+        rc = with_flags([&](auto SDP, auto LP, auto EQ, auto CONES) {
+            return solve<CONES, EQ, LP, SDP>(b, maxiters, abstol, reltol, feastol);
+        }, sdp, lp, eq, cones);
+    b->solved = rc == 0;
+    return rc;
+}
+
+int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                       double *uz, double *dP, double *dG, double *dA, int space) {
+    if (!b) { set_error("batch_adjoint: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QP || b->p.nq > 0 || b->p.ns > 0) {
+        set_error("batch_adjoint: only QP batches whose rows are all 'l' are differentiated");
+        return CVXB_E_UNSUP;
+    }
+    if (!b->solved) { set_error("batch_adjoint: no completed cvxb_batch_solve since the last load"); return CVXB_E_ARG; }
+    CVXB_CUDA(cudaSetDevice(b->device));
+    cudaStream_t st = b->st;
+    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq;
+    const Ptrs &p = b->p;
+    // host space: every given array staged on the device (inputs uploaded, outputs copied back); device: in place
+    Staged s_gx, s_gy, s_gz, s_ux, s_uy, s_uz, s_dP, s_dG, s_dA;
+    auto stage = [&](Staged &s, const double *a, size_t len, bool in) -> int {
+        if (a && len) CVXB_TRY(s.in(a, B * len, space, st, in));
+        return 0;
+    };
+    CVXB_TRY(stage(s_gx, gx, n, true)); CVXB_TRY(stage(s_gy, gy, pq, true)); CVXB_TRY(stage(s_gz, gz, m, true));
+    CVXB_TRY(stage(s_ux, ux, n, false)); CVXB_TRY(stage(s_uy, uy, pq, false)); CVXB_TRY(stage(s_uz, uz, m, false));
+    CVXB_TRY(stage(s_dP, dP, n * n, false)); CVXB_TRY(stage(s_dG, dG, m * n, false));
+    CVXB_TRY(stage(s_dA, dA, pq * n, false));
+    b->Bact = b->B;
+    CVXB_CUDA(cudaMemcpyAsync(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+    k_adj_rhs<<<(unsigned)B, 256, 0, st>>>(p, s_gx.dev, s_gy.dev, s_gz.dev, b->d_perm.p); count_launch();
+    CVXB_TRY(batch_factor(b));
+    CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
+    // one step of iterative refinement on the full KKT system: W'W spans many orders of magnitude at a converged
+    // iterate, and the reduced solve alone loses digits to it.  r = g - M u, then u += M^{-1} r with the same factor
+    const int Bi = (int)B, ni = (int)n, mi = (int)m, pi = (int)pq;
+    k_adj_uz<<<(unsigned)B, 256, 0, st>>>(p); count_launch();
+    GemvBatch gP; gP.batch = Bi; gP.sA = b->sP; gP.sx = ni; gP.sy = ni;
+    CVXB_TRY(gemv_t(ni, ni, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.rx, st, gP));
+    if (pq) {
+        GemvBatch gt; gt.batch = Bi; gt.sA = b->sA; gt.sx = pi; gt.sy = ni;
+        CVXB_TRY(gemv_t(pi, ni, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.rx, st, gt));
+        GemvBatch gn; gn.batch = Bi; gn.sA = b->sA; gn.sx = ni; gn.sy = pi;
+        CVXB_TRY(gemv_n(pi, ni, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.ry, b->gemv_ws.p, st, gn));
+    }
+    if (m) {
+        GemvBatch gt; gt.batch = Bi; gt.sA = b->sG; gt.sx = mi; gt.sy = ni;
+        CVXB_TRY(gemv_t(mi, ni, b->G.p, b->ldg, nullptr, p.dz, -1.0, 1.0, p.rx, st, gt));
+        GemvBatch gn; gn.batch = Bi; gn.sA = b->sG; gn.sx = ni; gn.sy = mi;
+        CVXB_TRY(gemv_n(mi, ni, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.rz, b->gemv_ws.p, st, gn));
+    }
+    k_adj_res<<<(unsigned)B, 256, 0, st>>>(p); count_launch();
+    CVXB_TRY(batch_solve(b, p.rx, n, p.ry, pq));
+    k_adj_vecs<<<(unsigned)B, 256, 0, st>>>(p, s_ux.dev, s_uy.dev, s_uz.dev, b->d_perm.p, b->d_info.p);
+    count_launch();
+    if (s_dP.dev || s_dG.dev || s_dA.dev) {
+        k_adj_grad<<<dim3((unsigned)((n + ADJ_TJ - 1) / ADJ_TJ), (unsigned)B), 256, 0, st>>>(
+            p, s_dP.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
+        count_launch();
+    }
+    CVXB_LAUNCH_CHECK();
+    for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dG, &s_dA}) CVXB_TRY(s->out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {

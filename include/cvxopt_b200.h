@@ -387,6 +387,25 @@ int cvxb_batch_results(cvxb_batch *b, double *x, double *s, double *z, int *stat
                        int *iters, double *pobj, double *dobj, int space);
 /* y: nprob x p, the multipliers of A x = b in the caller's problem order (as x, s, z); nothing when p = 0 */
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space);
+/* Derivatives of the last solve's results with respect to the problem data, for a loss L with gradients gx = dL/dx
+ * (nprob x n), gy = dL/dy (nprob x p) and gz = dL/dz (nprob x m).  At the returned iterate it solves
+ *     [P A' G'; A 0 0; G 0 -W'W] [ux; uy; uz] = [gx; gy; gz],   W'W = diag(s / z),
+ * with one more factorisation of the reduced KKT matrix and one step of iterative refinement on the full system, and
+ * writes ux (nprob x n), uy (nprob x p), uz (nprob x m) and
+ *     dP = -(ux x' + x ux') / 2   (n x n column-major per problem, both triangles: the gradient over symmetric P),
+ *     dG = -(z ux' + uz x')        (m x n column-major per problem, as cvxb_batch_load's G),
+ *     dA = -(y ux' + uy x')        (p x n column-major per problem, as cvxb_batch_load_eq's A);
+ * dL/dq = -ux, dL/dh = uz and dL/db = uy.  Every array is in the caller's problem order and in `space`.  A NULL input
+ * is zero; a NULL output is not written and its work is skipped.  A problem whose status is not 1 (optimal), or whose
+ * KKT matrix has no Cholesky factor at that iterate, gets NaN in all its outputs.  The scaling comes from the returned
+ * s and z alone, so the outputs are a function of the results; cvxb_batch_results is unchanged afterwards and a
+ * re-solve computes the same results.  Each call factors again.
+ * QP batches whose rows are all 'l' only (cvxb_batch_create, cvxb_batch_create_eq with dims {'l': m}); any other batch
+ * is CVXB_E_UNSUP.  A batch without a completed cvxb_batch_solve since its last cvxb_batch_load or
+ * cvxb_batch_load_eq is CVXB_E_ARG.  CVXB_DEVICE allocates nothing; CVXB_HOST stages each given array in temporary
+ * device memory, at most nprob * (2 (n + p + m) + n (n + m + p)) doubles in all. */
+int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                       double *uz, double *dP, double *dG, double *dA, int space);
 /* CUDA-event time of the last cvxb_batch_solve and the number of lock-step iterations run */
 int cvxb_batch_stats(cvxb_batch *b, double *solve_ms, int *iterations);
 /* kernel of the factorisations' SYRK in the last solve: 1 fp64 DMMA, 2 int8 slices (as cvxb_kkt_syrk_path) */
