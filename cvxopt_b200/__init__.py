@@ -23,15 +23,15 @@ __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolv
            "CPBatch", "CPBatchGroup", "cp_batch",
            "CPLBatch", "CPLBatchGroup", "cpl_batch",
            "SDPCPLBatch", "SDPCPLBatchGroup", "sdp_cpl_batch",
-           "QCQPBatch", "QCQPBatchGroup", "qcqp_batch", "qp_layer",
+           "QCQPBatch", "QCQPBatchGroup", "qcqp_batch", "qp_layer", "qcqp_layer",
            "device_count", "launch_count"]
 
 
 def __getattr__(name):
-    # qp_layer imports torch, which `import cvxopt_b200` does not need otherwise
-    if name == "qp_layer":
-        from .layer import qp_layer
-        return qp_layer
+    # the layers import torch, which `import cvxopt_b200` does not need otherwise
+    if name in ("qp_layer", "qcqp_layer"):
+        from . import layer
+        return getattr(layer, name)
     raise AttributeError("module 'cvxopt_b200' has no attribute %r" % name)
 
 

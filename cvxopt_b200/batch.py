@@ -167,15 +167,16 @@ def _sdp_dims(dims, m=None):
 
 
 ADJOINT_KEYS = ("P", "q", "G", "h", "A", "b")
+QCQP_ADJOINT_KEYS = ("P", "q", "r", "G", "h", "A", "b")
 
 
-def _adjoint_args(gx, gy, gz, want, B, n, p, m):
+def _adjoint_args(gx, gy, gz, want, B, n, p, m, keys=ADJOINT_KEYS):
     """the gradients gx (B, n), gy (B, p), gz (B, m) as contiguous float64 arrays (None stays None) and `want` as a
-    tuple of ADJOINT_KEYS; a wrong shape or an unknown key is a TypeError"""
+    tuple of `keys`; a wrong shape or an unknown key is a TypeError"""
     want = tuple(want)
-    unknown = [k for k in want if k not in ADJOINT_KEYS]
+    unknown = [k for k in want if k not in keys]
     if unknown:
-        raise TypeError("want: unknown keys %s; the keys are %s" % (unknown, ADJOINT_KEYS))
+        raise TypeError("want: unknown keys %s; the keys are %s" % (unknown, keys))
     gs = []
     for name, a, k in (("gx", gx, n), ("gy", gy, p), ("gz", gz, m)):
         if a is not None:
@@ -445,9 +446,11 @@ class QPBatchGroup:
         out["status"] = [STATUS[int(k)] for k in out["status_code"]]
         return out
 
+    _adjoint_keys = ADJOINT_KEYS         # the keys each part's adjoint takes in `want`
+
     def adjoint(self, gx, gy=None, gz=None, want=ADJOINT_KEYS):
         """QPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
-        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m)
+        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m, self._adjoint_keys)
         out = {}
         for ix, part in zip(self.idx, self.parts):
             r = part.adjoint(*(None if a is None else a[ix] for a in gs), want=want)
@@ -1033,21 +1036,58 @@ class QCQPBatch(CPBatch):
         # per problem the (nK n) x n column-major stack [P_0; ...; P_mnl]: column j holds P_0[:, j], P_1[:, j], ...
         Pcm = np.ascontiguousarray(np.transpose(P, (0, 3, 1, 2)))
         Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
-        _lib.check(self._lib.cvxb_batch_load_qcqp(self._h, Pcm.ctypes.data, q.ctypes.data, r.ctypes.data,
-                                                  x0.ctypes.data, Gcm.ctypes.data if self.ml else None,
-                                                  h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_qcqp")
-        self._load_eq(Acm, bv, _lib.HOST)
+        self.load_ptr(Pcm.ctypes.data, q.ctypes.data, r.ctypes.data, x0.ctypes.data,
+                      Gcm.ctypes.data if self.ml else None, h.ctypes.data if self.ml else None, _lib.HOST, Acm, bv)
+
+    def load_ptr(self, P, q, r, x0, G, h, space=_lib.DEVICE, A=None, b=None):
+        """cvxb_batch_load_qcqp on raw addresses in `space` (device-resident callers): P the (mnl + 1) n x n
+        column-major stack per problem, q, r, x0 (None: 0), G ml x n column-major, h; A p x n column-major and b"""
+        _lib.check(self._lib.cvxb_batch_load_qcqp(self._h, P, q, r, x0, G, h, space), "batch_load_qcqp")
+        self._load_eq(A, b, space)
+
+    def adjoint(self, gx, gy=None, gz=None, want=QCQP_ADJOINT_KEYS):
+        """derivatives of the last solve's results for a loss L with gradients gx = dL/dx (B, n), gy = dL/dy (B, p)
+        and gz = dL/dz (B, mnl + ml, laid out as [znl, zl]), None meaning zero (cvxb_batch_adjoint_qcqp).  Returns
+        host arrays for the keys in `want`, each dL/d(that input) in load()'s layout: P (B, mnl + 1, n, n, each block
+        symmetric), q (B, mnl + 1, n), r (B, mnl + 1), G (B, ml, n), h (B, ml), A (B, p, n) and b (B, p).  A problem
+        whose status is not 'optimal' gets NaN.  A batch not solved since its last load raises ValueError."""
+        B, n, m, p, ml, nK = self.B, self.n, self.m, self.p, self.ml, self.mnl + 1
+        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m, QCQP_ADJOINT_KEYS)
+        # C's outputs uy, uz (h: its 'l' rows), dP, dq, dr, dG, dA; dP, dG and dA column-major per problem
+        shapes = {"b": (B, p), "h": (B, m), "P": (B, n, nK, n), "q": (B, nK, n), "r": (B, nK), "G": (B, n, ml),
+                  "A": (B, n, p)}
+        bufs = {k: np.empty(shapes[k]) for k in want}
+        ptrs = [None if a is None else a.ctypes.data for a in gs] + [None]
+        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("b", "h", "P", "q", "r", "G", "A")]
+        self.adjoint_ptr(*ptrs, space=_lib.HOST)
+        out = {}
+        for k, v in bufs.items():
+            out[k] = (np.ascontiguousarray(v.transpose(0, 2, 3, 1)) if k == "P" else v[:, self.mnl:] if k == "h" else
+                      np.ascontiguousarray(v.transpose(0, 2, 1)) if k in ("G", "A") else v)
+        return out
+
+    def adjoint_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dq=None, dr=None, dG=None,
+                    dA=None, space=_lib.DEVICE):
+        """cvxb_batch_adjoint_qcqp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_adjoint_qcqp(self._h, gx, gy, gz, ux, uy, uz, dP, dq, dr, dG, dA, space),
+                   "batch_adjoint_qcqp")
 
 
 class QCQPBatchGroup(CPBatchGroup):
     """QPBatchGroup's interleaved sub-batches, solved concurrently on their own streams, for convex QCQPs; nothing
     calls back to the host, so the sub-batches never wait on each other"""
 
+    _adjoint_keys = QCQP_ADJOINT_KEYS
+
     def _part(self):
         return lambda nprob, n, m, device, dims, p=0: QCQPBatch(nprob, n, self._mnl, self._ml, p, device)
 
     def load(self, P, q, r, x0, G, h, A=None, b=None):
         self._load_sliced((P, q, r, x0, G, h), A, b)
+
+    def adjoint(self, gx, gy=None, gz=None, want=QCQP_ADJOINT_KEYS):
+        """QCQPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
+        return super().adjoint(gx, gy, gz, want)
 
 
 def _qcqp_args(P, q, r, G, h, dims, A, b, x0):

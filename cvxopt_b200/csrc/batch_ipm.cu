@@ -2187,6 +2187,80 @@ __global__ void __launch_bounds__(256) k_adj_grad(Ptrs p, double *dP, double *dG
                             [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
 }
 
+// ---- the adjoint of a QCQP batch's solution (cvxb_batch_adjoint_qcqp) ----
+// The same derivation with f_i(x) = x'P_i x / 2 + q_i'x + r_i: at the returned iterate, with the objective's multiplier
+// z_0 = 1, the KKT matrix is the QP's with H = P_0 + sum_i znl_i P_i in place of P and [Df; G] in place of G, Df's rows
+// (P_i x + q_i)'.  Row i of the constraint residual is f_i(x) + s_i, whose derivatives in q_i, r_i and P_i are x', 1
+// and x x' / 2; so beyond the QP's gradients dL/dP_i = -(znl_i (ux x' + x ux') + uznl_i x x') / 2, dL/dq_i =
+// -(znl_i ux + uznl_i x) and dL/dr_i = -uznl_i for i >= 1, and dL/dr_0 = 0.
+// The operator at x, once gp_products has left u = [P_0 x; ...; P_mnl x] in yv: H into all of P (the refinement's P
+// GEMV reads both triangles) and Df_i = u_i + q_i into G's rows [0, mnl), q from the slot's state row.  Thread e of a
+// slot forms H's entry e and Df's entry e, grid (ceil(max(n², mnl n) / 256), B).  The stack is mirrored at load, so
+// H(i, j) and H(j, i) are the same sum
+__global__ void __launch_bounds__(256) k_adj_qc_op(Ptrs p, GPPtrs g, CPPtrs c) {
+    const int b = blockIdx.y, n = p.n, mnl = g.mnl;
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const double *z = p.z + (long long)b * p.m;
+    if (e < (long long)n * n) {
+        const long long i = e % n, j = e / n;
+        const double *pe = g.G + (long long)b * g.sG + p.m + i + j * g.ldg;
+        double a = pe[0];
+        for (int k = 1; k < g.nK; ++k) a += z[k - 1] * pe[(long long)k * n];
+        c.P[(long long)b * c.sP + i + j * c.ldp] = a;
+    }
+    if (e < (long long)mnl * n) {
+        const long long i = e % mnl, j = e / mnl;
+        const double *u = g.yv + (long long)b * g.sumK, *qv = g.g + (long long)b * p.L;
+        g.G[(long long)b * g.sG + i + j * g.ldg] = u[(i + 1) * n + j] + qv[(i + 1) * n + j];
+    }
+}
+// o[(c nK + k) rows + i] = f(i, k, c) for the nj columns c of nK stacked rows x nj column-major blocks, contiguous in
+// memory: adj_store with the block index k stepped alongside (c, i)
+template <class F> __device__ __forceinline__ void adj_store_stack(double *o, int rows, int nK, int nj, bool bad, F f) {
+    const int qs = blockDim.x / rows, rs = blockDim.x % rows, qc = qs / nK, qk = qs % nK;
+    const int t = threadIdx.x / rows;
+    int c = t / nK, k = t % nK, i = threadIdx.x % rows;
+    while (c < nj) {
+        o[((long long)c * nK + k) * rows + i] = bad ? NAN : f(i, k, c);
+        i += rs; k += qk; c += qc;
+        if (i >= rows) { i -= rows; ++k; }
+        if (k >= nK) { k -= nK; ++c; }
+    }
+}
+// dP's nK blocks, dq, dr, dG and dA (nullptr: not written) of problem perm[b] in one pass over columns [j0, j0 +
+// ADJ_TJ), grid (ceil(n / ADJ_TJ), B), as k_adj_grad: dP per problem the (nK n) x n column-major stack, dq nK x n, dr
+// nK (by the CTA of the first tile), dG over the 'l' rows only (rows mnl.. of z and uz)
+__global__ void __launch_bounds__(256) k_adj_qc_grad(Ptrs p, GPPtrs g, double *dP, double *dq, double *dr, double *dG,
+                                                     double *dA, const int *perm, const int *info) {
+    const int b = blockIdx.y, j0 = blockIdx.x * ADJ_TJ, nj = min(ADJ_TJ, p.n - j0), n = p.n, m = p.m, pq = p.neq;
+    const int nK = g.nK, ml = m - g.mnl;
+    const long long on = (long long)b * n, om = (long long)b * m, oq = (long long)b * pq, k = perm[b];
+    const double *__restrict__ x = p.x + on, *__restrict__ ux = p.dx + on;
+    const double *__restrict__ z = p.z + om, *__restrict__ uz = p.bzp + om;
+    const double *__restrict__ y = p.y + oq, *__restrict__ uy = p.dy + oq;
+    __shared__ double xs[ADJ_TJ], uxs[ADJ_TJ];
+    if (threadIdx.x < nj) { xs[threadIdx.x] = x[j0 + threadIdx.x]; uxs[threadIdx.x] = ux[j0 + threadIdx.x]; }
+    __syncthreads();
+    const bool bad = adj_bad(p, info, b);
+    // rounded products, no FMA: every term is the same in (i, j) and (j, i), so each block is bitwise symmetric
+    if (dP) adj_store_stack(dP + (k * n + j0) * nK * n, n, nK, nj, bad, [&](int i, int l, int c) {
+        const double s = __dadd_rn(__dmul_rn(ux[i], xs[c]), __dmul_rn(x[i], uxs[c]));
+        if (l == 0) return -0.5 * s;
+        return -0.5 * __dadd_rn(__dmul_rn(z[l - 1], s), __dmul_rn(uz[l - 1], __dmul_rn(x[i], xs[c])));
+    });
+    if (dq)
+        for (int e = threadIdx.x; e < nK * nj; e += blockDim.x) {
+            const int l = e / nj, c = e % nj;
+            dq[(k * nK + l) * n + j0 + c] = bad ? NAN : l == 0 ? -uxs[c] : -(z[l - 1] * uxs[c] + uz[l - 1] * xs[c]);
+        }
+    if (dr && blockIdx.x == 0)
+        for (int l = threadIdx.x; l < nK; l += blockDim.x) dr[k * nK + l] = bad ? NAN : l == 0 ? 0.0 : -uz[l - 1];
+    if (dG && ml) adj_store(dG + (k * n + j0) * ml, ml, nj, bad,
+                            [&](int i, int c) { return -(z[g.mnl + i] * uxs[c] + uz[g.mnl + i] * xs[c]); });
+    if (dA && pq) adj_store(dA + (k * n + j0) * pq, pq, nj, bad,
+                            [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
+}
+
 // the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
 enum class Kind { QP, LP, GP, CP, CPL, QC };
 }  // namespace
@@ -2789,11 +2863,16 @@ int solve(cvxb_batch *b, int maxiters, double abstol, double reltol, double feas
 // ---- geometric programs: the lock-step cpl (cvxprog.py:622-1356) of gp's epigraph problem ----
 // F(x) over the active slots at x (slot k at x + k*sx): yv = F x, then k_gp_eval (full: with Df, H's rows and weights).
 // QC: yv = [P_0 x; ...; P_mnl x], then k_qc_eval (full: with Df; trial: with newrx's nonlinear part)
+// yv = F x over the active slots (slot k at x + k*sx); QC: [P_0 x; ...; P_mnl x]
+int gp_products(cvxb_batch *b, const double *x, long long sx) {
+    const GPPtrs &g = b->gq;
+    GemvBatch gf; gf.batch = b->Bact; gf.sA = g.sG; gf.sx = sx; gf.sy = g.sumK;
+    return gemv_n(g.sumK, b->n, g.G + b->m, g.ldg, nullptr, x, 1.0, 0.0, g.yv, b->gemv_ws.p, b->st, gf);
+}
 int gp_eval(cvxb_batch *b, const double *x, long long sx, bool full, int trial) {
     const GPPtrs &g = b->gq;
     const int B = b->Bact;
-    GemvBatch gf; gf.batch = B; gf.sA = g.sG; gf.sx = sx; gf.sy = g.sumK;
-    CVXB_TRY(gemv_n(g.sumK, b->n, g.G + b->m, g.ldg, nullptr, x, 1.0, 0.0, g.yv, b->gemv_ws.p, b->st, gf));
+    CVXB_TRY(gp_products(b, x, sx));
     if (b->kind == Kind::QC) {
         if (full) k_qc_eval<true><<<B, 256, 0, b->st>>>(b->p, g, b->cq);
         else k_qc_eval<false><<<B, 256, 0, b->st>>>(b->p, g, b->cq);
@@ -3620,31 +3699,42 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
     return rc;
 }
 
-int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
-                       double *uz, double *dP, double *dG, double *dA, int space) {
-    if (!b) { set_error("batch_adjoint: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QP || b->p.nq > 0 || b->p.ns > 0) {
-        set_error("batch_adjoint: only QP batches whose rows are all 'l' are differentiated");
-        return CVXB_E_UNSUP;
-    }
-    if (!b->solved) { set_error("batch_adjoint: no completed cvxb_batch_solve since the last load"); return CVXB_E_ARG; }
+namespace {
+// the gradient outputs of an adjoint call (nullptr: not written); dq and dr are a QCQP batch's only
+struct AdjGrads {
+    double *dP = nullptr, *dq = nullptr, *dr = nullptr, *dG = nullptr, *dA = nullptr;
+};
+// the adjoint of a solved QP or QC batch (the entry points check the kind and the solve): the right-hand side, for a
+// QC batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement step on the full
+// system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG ml x n per problem
+int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                  double *uz, AdjGrads d, int space) {
     CVXB_CUDA(cudaSetDevice(b->device));
     cudaStream_t st = b->st;
-    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq;
+    const bool qc = b->kind == Kind::QC;
+    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = qc ? b->gq.nK : 1, ml = qc ? m - b->gq.mnl : m;
     const Ptrs &p = b->p;
     // host space: every given array staged on the device (inputs uploaded, outputs copied back); device: in place
-    Staged s_gx, s_gy, s_gz, s_ux, s_uy, s_uz, s_dP, s_dG, s_dA;
+    Staged s_gx, s_gy, s_gz, s_ux, s_uy, s_uz, s_dP, s_dq, s_dr, s_dG, s_dA;
     auto stage = [&](Staged &s, const double *a, size_t len, bool in) -> int {
         if (a && len) CVXB_TRY(s.in(a, B * len, space, st, in));
         return 0;
     };
     CVXB_TRY(stage(s_gx, gx, n, true)); CVXB_TRY(stage(s_gy, gy, pq, true)); CVXB_TRY(stage(s_gz, gz, m, true));
     CVXB_TRY(stage(s_ux, ux, n, false)); CVXB_TRY(stage(s_uy, uy, pq, false)); CVXB_TRY(stage(s_uz, uz, m, false));
-    CVXB_TRY(stage(s_dP, dP, n * n, false)); CVXB_TRY(stage(s_dG, dG, m * n, false));
-    CVXB_TRY(stage(s_dA, dA, pq * n, false));
+    CVXB_TRY(stage(s_dP, d.dP, nK * n * n, false));
+    if (qc) { CVXB_TRY(stage(s_dq, d.dq, nK * n, false)); CVXB_TRY(stage(s_dr, d.dr, nK, false)); }
+    CVXB_TRY(stage(s_dG, d.dG, ml * n, false));
+    CVXB_TRY(stage(s_dA, d.dA, pq * n, false));
     b->Bact = b->B;
     CVXB_CUDA(cudaMemcpyAsync(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
     k_adj_rhs<<<(unsigned)B, 256, 0, st>>>(p, s_gx.dev, s_gy.dev, s_gz.dev, b->d_perm.p); count_launch();
+    if (qc) {
+        CVXB_TRY(gp_products(b, p.x, n));
+        const long long work = std::max(n * n, (size_t)b->gq.mnl * n);
+        k_adj_qc_op<<<dim3((unsigned)((work + 255) / 256), (unsigned)B), 256, 0, st>>>(p, b->gq, b->cq);
+        count_launch();
+    }
     CVXB_TRY(batch_factor(b));
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
     // one step of iterative refinement on the full KKT system: W'W spans many orders of magnitude at a converged
@@ -3669,15 +3759,44 @@ int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const 
     CVXB_TRY(batch_solve(b, p.rx, n, p.ry, pq));
     k_adj_vecs<<<(unsigned)B, 256, 0, st>>>(p, s_ux.dev, s_uy.dev, s_uz.dev, b->d_perm.p, b->d_info.p);
     count_launch();
-    if (s_dP.dev || s_dG.dev || s_dA.dev) {
-        k_adj_grad<<<dim3((unsigned)((n + ADJ_TJ - 1) / ADJ_TJ), (unsigned)B), 256, 0, st>>>(
-            p, s_dP.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
+    if (s_dP.dev || s_dq.dev || s_dr.dev || s_dG.dev || s_dA.dev) {
+        const dim3 grid((unsigned)((n + ADJ_TJ - 1) / ADJ_TJ), (unsigned)B);
+        if (qc) k_adj_qc_grad<<<grid, 256, 0, st>>>(p, b->gq, s_dP.dev, s_dq.dev, s_dr.dev, s_dG.dev, s_dA.dev,
+                                                    b->d_perm.p, b->d_info.p);
+        else k_adj_grad<<<grid, 256, 0, st>>>(p, s_dP.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
         count_launch();
     }
     CVXB_LAUNCH_CHECK();
-    for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dG, &s_dA}) CVXB_TRY(s->out(st));
+    for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dq, &s_dr, &s_dG, &s_dA}) CVXB_TRY(s->out(st));
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;
+}
+}  // namespace
+
+int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                       double *uz, double *dP, double *dG, double *dA, int space) {
+    if (!b) { set_error("batch_adjoint: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QP || b->p.nq > 0 || b->p.ns > 0) {
+        set_error("batch_adjoint: only QP batches whose rows are all 'l' are differentiated");
+        return CVXB_E_UNSUP;
+    }
+    if (!b->solved) { set_error("batch_adjoint: no completed cvxb_batch_solve since the last load"); return CVXB_E_ARG; }
+    return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, nullptr, nullptr, dG, dA}, space);
+}
+
+int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
+                            double *uy, double *uz, double *dP, double *dq, double *dr, double *dG, double *dA,
+                            int space) {
+    if (!b) { set_error("batch_adjoint_qcqp: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QC) {
+        set_error("batch_adjoint_qcqp: only QCQP batches (cvxb_batch_create_qcqp) are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (!b->solved) {
+        set_error("batch_adjoint_qcqp: no completed cvxb_batch_solve since the last load");
+        return CVXB_E_ARG;
+    }
+    return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, dq, dr, dG, dA}, space);
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {

@@ -538,6 +538,32 @@ int cvxb_batch_create_qcqp(cvxb_batch **out, int nprob, int n, int mnl, int ml, 
  * cvxb_batch_load_eq. */
 int cvxb_batch_load_qcqp(cvxb_batch *b, const double *P, const double *q, const double *r, const double *x0,
                          const double *G, const double *h, int space);
+/* Derivatives of a QCQP batch's last solve, cvxb_batch_adjoint's counterpart, for a loss L with gradients gx = dL/dx
+ * (nprob x n), gy = dL/dy (nprob x p) and gz = dL/dz (nprob x m, m = mnl + ml, laid out as the results' [znl; zl]).
+ * At the returned iterate, with the objective's multiplier z0 = 1, H = P0 + sum_i znl_i Pi, Df the mnl x n matrix of
+ * rows (Pi x + qi)' (i = 1..mnl) and D = diag(s / z), it solves
+ *     [H A' Df' G'; A 0 0 0; Df 0 -Dnl 0; G 0 0 -Dl] [ux; uy; uznl; uzl] = [gx; gy; gznl; gzl]
+ * with one more factorisation of the reduced KKT matrix and one step of iterative refinement on the full system, and
+ * writes ux (nprob x n), uy (nprob x p), uz = [uznl; uzl] (nprob x m) and the gradients dL/d(input):
+ *     dP: per problem the (mnl + 1) n x n column-major stack of cvxb_batch_load_qcqp's P, both triangles of each
+ *         block (the gradient over symmetric Pi, bitwise symmetric): dP0 = -(ux x' + x ux') / 2 and
+ *         dPi = -(znl_i (ux x' + x ux') + uznl_i x x') / 2;
+ *     dq: nprob x (mnl + 1) x n: dq0 = -ux, dqi = -(znl_i ux + uznl_i x);
+ *     dr: nprob x (mnl + 1): dr0 = 0, dri = -uznl_i;
+ *     dG = -(zl ux' + uzl x')  (ml x n column-major per problem, the 'l' rows only),
+ *     dA = -(y ux' + uy x')    (p x n column-major per problem);
+ * dL/dh = uzl and dL/db = uy.  Every array is in the caller's problem order and in `space`.  A NULL input is zero; a
+ * NULL output is not written and its work is skipped: without dP, dq, dr, dG and dA the gradient kernel does not run.
+ * A problem whose status is not 1 (optimal), or whose KKT matrix has no Cholesky factor at that iterate, gets NaN in
+ * all its outputs, dr0 included.  The outputs are a function of the results and the data; cvxb_batch_results is
+ * unchanged afterwards and a re-solve computes the same results.  QCQP batches only (cvxb_batch_create_qcqp): any
+ * other batch is CVXB_E_UNSUP, and cvxb_batch_adjoint refuses a QCQP batch.  A batch without a completed
+ * cvxb_batch_solve since its last cvxb_batch_load_qcqp or cvxb_batch_load_eq is CVXB_E_ARG.  CVXB_DEVICE allocates
+ * nothing; CVXB_HOST stages each given array in temporary device memory, at most nprob * (2 (n + p + m) + nK n² +
+ * nK n + nK + ml n + p n) doubles in all, nK = mnl + 1. */
+int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
+                            double *uy, double *uz, double *dP, double *dq, double *dr, double *dG, double *dA,
+                            int space);
 
 #ifdef __cplusplus
 }
