@@ -26,6 +26,7 @@ from . import _lib
 STATUS = {0: "running", 1: "optimal", 2: "unknown", 3: "unknown", 4: "primal infeasible", 5: "dual infeasible"}
 DEFAULTS = dict(maxiters=100, abstol=1e-7, reltol=1e-6, feastol=1e-7)   # coneprog.py:436-456
 BATCH_MAX = 65535        # CVXB_BATCH_MAX: problems per cvxb_batch handle
+BATCH_SMAX = 32          # CVXB_BATCH_SMAX: the largest 's' order of a batch
 
 
 def _batch_dims(dims, m=None):
@@ -168,6 +169,7 @@ def _sdp_dims(dims, m=None):
 
 ADJOINT_KEYS = ("P", "q", "G", "h", "A", "b")
 QCQP_ADJOINT_KEYS = ("P", "q", "r", "G", "h", "A", "b")
+CONELP_ADJOINT_KEYS = ("c", "G", "h", "A", "b")
 
 
 def _adjoint_args(gx, gy, gz, want, B, n, p, m, keys=ADJOINT_KEYS):
@@ -324,6 +326,31 @@ class QPBatch:
         """cvxb_batch_adjoint on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
         _lib.check(self._lib.cvxb_batch_adjoint(self._h, gx, gy, gz, ux, uy, uz, dP, dG, dA, space), "batch_adjoint")
 
+    _cone_keys = ADJOINT_KEYS            # the keys adjoint_cone takes in `want` (a cone LP: CONELP_ADJOINT_KEYS)
+
+    def adjoint_cone(self, gx, gy=None, gz=None, want=None):
+        """adjoint's derivatives on any QP or cone LP batch, with 'q' cones and 's' blocks (cvxb_batch_adjoint_cone).
+        gz (B, m) and the returned h (B, m) and G (B, m, n) are laid out as h, each 's' block unpacked column-major:
+        only the symmetric part of gz's blocks enters, and the outputs' blocks hold the same value in both triangles.
+        want: keys of ADJOINT_KEYS, of CONELP_ADJOINT_KEYS on a cone LP batch (c for q, no P); None: all of them."""
+        B, n, m, p = self.B, self.n, self.m, self.p
+        keys = self._cone_keys
+        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, B, n, p, m, keys)
+        # C's outputs ux, uy, uz, dP, dG, dA; the matrices column-major per problem
+        shapes = {"q": (B, n), "c": (B, n), "b": (B, p), "h": (B, m), "P": (B, n, n), "G": (B, n, m), "A": (B, n, p)}
+        bufs = {k: np.empty(shapes[k]) for k in want}
+        ptrs = [None if a is None else a.ctypes.data for a in gs]
+        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("c" if self._lp else "q", "b", "h", "P", "G", "A")]
+        self.adjoint_cone_ptr(*ptrs, space=_lib.HOST)
+        return {k: -v if k in ("q", "c") else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
+                for k, v in bufs.items()}
+
+    def adjoint_cone_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dG=None, dA=None,
+                         space=_lib.DEVICE):
+        """cvxb_batch_adjoint_cone on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_adjoint_cone(self._h, gx, gy, gz, ux, uy, uz, dP, dG, dA, space),
+                   "batch_adjoint_cone")
+
     def stats(self):
         ms, it = C.c_double(), C.c_int()
         self._lib.cvxb_batch_stats(self._h, C.byref(ms), C.byref(it))
@@ -447,6 +474,7 @@ class QPBatchGroup:
         return out
 
     _adjoint_keys = ADJOINT_KEYS         # the keys each part's adjoint takes in `want`
+    _cone_keys = ADJOINT_KEYS            # and its adjoint_cone
 
     def adjoint(self, gx, gy=None, gz=None, want=ADJOINT_KEYS):
         """QPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
@@ -454,6 +482,17 @@ class QPBatchGroup:
         out = {}
         for ix, part in zip(self.idx, self.parts):
             r = part.adjoint(*(None if a is None else a[ix] for a in gs), want=want)
+            for k, v in r.items():
+                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
+        return out
+
+    def adjoint_cone(self, gx, gy=None, gz=None, want=None):
+        """QPBatch.adjoint_cone on every part with its slice of the gradients, the results in problem order"""
+        keys = self._cone_keys
+        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, self.B, self.n, self.p, self.m, keys)
+        out = {}
+        for ix, part in zip(self.idx, self.parts):
+            r = part.adjoint_cone(*(None if a is None else a[ix] for a in gs), want=want)
             for k, v in r.items():
                 out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
         return out
@@ -477,6 +516,7 @@ class ConeLPBatch(QPBatch):
     results()["status"] is one of 'optimal', 'primal infeasible', 'dual infeasible' or 'unknown', with NaN where
     conelp returns None."""
     _lp = True
+    _cone_keys = CONELP_ADJOINT_KEYS
 
     def load(self, c, G, h, A=None, b=None):
         c = np.ascontiguousarray(np.asarray(c, dtype=np.float64))
@@ -500,6 +540,7 @@ class ConeLPBatch(QPBatch):
 
 class ConeLPBatchGroup(QPBatchGroup):
     """QPBatchGroup's interleaved sub-batches, solved concurrently, for cone LPs"""
+    _cone_keys = CONELP_ADJOINT_KEYS
 
     @staticmethod
     def _part():

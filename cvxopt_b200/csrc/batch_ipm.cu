@@ -1166,13 +1166,14 @@ __global__ void __launch_bounds__(SB_T) k_s_build_gs(Ptrs p, const double *G, do
         __syncthreads();
     }
 }
-// NT scaling at iteration 0 (misc.py:374-417): s = Ls Ls', z = Lz Lz', Lz' Ls = U diag(lambda) V',
+// NT scaling (misc.py:374-417): s = Ls Ls', z = Lz Lz', Lz' Ls = U diag(lambda) V',
 // r = Lz^{-T} U diag(lambda)^{1/2}, rti = Lz U diag(lambda)^{-1/2}.  part[3] = 1 when a factorisation failed.
-__global__ void __launch_bounds__(SB_T) k_s_nt_compute(Ptrs p) {
+// ALL: every slot (the adjoint's scaling at the returned iterate); else the slots still running
+template <bool ALL> __device__ __forceinline__ void s_nt_compute(const Ptrs &p) {
     SB_SETUP
     SB_PART;
     __shared__ double Ls[SMX], Lz[SMX], U[SMX], V[SMX], lam[CVXB_BATCH_SMAX];
-    if (S.done) return;
+    if (!ALL && S.done) return;
     s_load(Ls, p.s + om + so, ms);
     s_load(Lz, p.z + om + so, ms);
     bool ok = s_chol(Ls, ms);
@@ -1196,6 +1197,8 @@ __global__ void __launch_bounds__(SB_T) k_s_nt_compute(Ptrs p) {
     for (int i = threadIdx.x; i < ms; i += SB_T) p.lmbda[om + so + i * (ms + 1)] = ok ? lam[i] : NAN;
     if (tid == 0) part[3] = ok ? 0.0 : 1.0;        // a failed Cholesky or SVD stops the problem (k_update)
 }
+// at iteration 0
+__global__ void __launch_bounds__(SB_T) k_s_nt_compute(Ptrs p) { s_nt_compute<false>(p); }
 // the starting point's smallest eigenvalues (misc.max_step, coneprog.py:707, :737): s (unpacked), z (bzp, packed)
 __global__ void __launch_bounds__(SB_T) k_s_eig_start(Ptrs p) {
     SB_SETUP
@@ -2185,6 +2188,95 @@ __global__ void __launch_bounds__(256) k_adj_grad(Ptrs p, double *dP, double *dG
                            [&](int i, int c) { return -(z[i] * uxs[c] + uz[i] * xs[c]); });
     if (dA && pq) adj_store(dA + (k * n + j0) * pq, pq, nj, bad,
                             [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
+}
+
+// ---- the adjoint of a cone QP or cone LP batch's solution (cvxb_batch_adjoint_cone) ----
+// On the central path s o z = mu e, and its linearisation L(z) ds + L(s) dz = 0 gives ds = -L(z)^{-1} L(s) dz; s and z
+// share a Jordan frame there, where L(z)^{-1} L(s) is the NT scaling's W'W.  So the adjoint is the 'l' one with W'W the
+// NT scaling of the returned s and z, and a cone LP's is the same with P = 0.  The 'l' kernels above run on every row
+// as before and these fix the cone rows around them: d = di = 0 there, so k_adj_res leaves 0 in those rows, and once
+// stage 3 has zeroed them in bzp k_adj_vecs takes uz = dz.  'q' cones one per warp (W = beta (2 v v' - J), symmetric);
+// 's' blocks in k_adj_s, with r and rti from k_adj_s_nt.
+//   stage 0, after k_adj_rhs: each cone's scaling (v, beta; lmbda is scratch) and bzp := W^{-T} g; each 's' block of rz
+//            := sym(g), which k_s_wtz then scales into bzp
+//   stage 1, after k_adj_uz: dz := W^{-1} bzp; a failed 's' scaling (part[3]) sets info, so the problem gets NaN
+//   stage 2, after k_adj_res: bzp := W^{-T} rz + W dz = W^{-T} (gz - G ux + W'W uz), the refinement's right-hand side
+//   stage 3, after the refinement solve and k_adj_s: dz += W^{-1} bzp, then bzp := 0 on the cone rows
+// ds is scratch throughout
+__global__ void k_adj_cone(Ptrs p, int *info, int stage) {
+    PB_SETUP
+    double *rz = p.rz + om, *bzp = p.bzp + om, *dz = p.dz + om, *ds = p.ds + om;
+    double *v = p.v + oc - p.ml, *beta = p.beta + oc;
+    if (stage == 0) {
+        for (int i = p.ml + tid; i < p.m; i += nt) { p.d[om + i] = 0.0; p.di[om + i] = 0.0; }
+        for (int k = 0; k < p.ns; ++k) {
+            const int ms = p.sinfo[5 * k], so = p.sinfo[5 * k + 1];
+            for (int e = tid; e < ms * ms; e += nt) {
+                const int i = e % ms, j = e / ms;
+                if (i > j) {
+                    const double a = 0.5 * (rz[so + e] + rz[so + j + i * ms]);
+                    rz[so + e] = a; rz[so + j + i * ms] = a;
+                }
+            }
+        }
+        FOR_CONES(o, len) {
+            q_nt_compute(wt, p.s + om + o, p.z + om + o, v + o, p.lmbda + om + o, beta + k_, len);
+            __syncwarp();
+            q_scale(wt, v + o, beta[k_], rz + o, bzp + o, len, true);
+        }
+    } else if (stage == 1) {
+        FOR_CONES(o, len) q_scale(wt, v + o, beta[k_], bzp + o, dz + o, len, true);
+        if (tid == 0)
+            for (int k = 0; k < p.ns; ++k) if (p.spart[((long long)b * p.ns + k) * 4 + 3] != 0.0) info[b] = 1;
+    } else if (stage == 2) {
+        FOR_CONES(o, len) {
+            q_scale(wt, v + o, beta[k_], rz + o, bzp + o, len, true);
+            q_scale(wt, v + o, beta[k_], dz + o, ds + o, len, false);
+            __syncwarp();
+            FOR_LANE(i, len) bzp[o + i] += ds[o + i];
+        }
+    } else {
+        FOR_CONES(o, len) {
+            q_scale(wt, v + o, beta[k_], bzp + o, ds + o, len, true);
+            __syncwarp();
+            FOR_LANE(i, len) dz[o + i] += ds[o + i];
+        }
+        __syncthreads();
+        for (int i = p.ml + tid; i < p.m; i += nt) bzp[i] = 0.0;
+    }
+}
+// the NT scaling of every slot's returned s and z, done or not (k_s_nt_compute skips done slots)
+__global__ void __launch_bounds__(SB_T) k_adj_s_nt(Ptrs p) { s_nt_compute<true>(p); }
+// the 's' blocks of the adjoint, one CTA per (block, slot): mode 0 (after the first solve) dz := W^{-1} bzp =
+// rti unpack(bzp) rti', mode 2 (after the refinement solve) dz += the same; mode 1 (after k_adj_res) bzp :=
+// pack(W^{-T} rz + W dz) = pack(rti' rz rti + r' dz r).  dz is written from its lower triangle, so both of its
+// triangles, and those of uz, dh and dG after it, hold the same values
+__global__ void __launch_bounds__(SB_T) k_adj_s(Ptrs p, int mode) {
+    SB_SETUP
+    __shared__ double R[SMX], X[SMX], Y[SMX], T[SMX];
+    if (mode == 1) {
+        s_load(X, p.rz + om + so, ms);
+        SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+        __syncthreads();
+        s_congr(Y, R, X, T, true, ms);
+        s_load(X, p.dz + om + so, ms);
+        SB_FOR(e, ms) R[e] = p.sr[oc + sro + e];
+        __syncthreads();
+        s_congr(X, R, X, T, true, ms);
+        SB_FOR(e, ms) Y[e] += X[e];
+        __syncthreads();
+        s_store_packed(p.bzp + om + sp, Y, ms);
+        return;
+    }
+    s_load_packed(X, p.bzp + om + sp, ms);
+    SB_FOR(e, ms) R[e] = p.srti[oc + sro + e];
+    __syncthreads();
+    s_congr(Y, R, X, T, false, ms);
+    SB_FOR(e, ms) {
+        const int i = e % ms, j = e / ms;
+        const double u = Y[i >= j ? e : j + i * ms];
+        p.dz[om + so + e] = mode == 2 ? p.dz[om + so + e] + u : u;
+    }
 }
 
 // ---- the adjoint of a QCQP batch's solution (cvxb_batch_adjoint_qcqp) ----
@@ -3704,14 +3796,39 @@ namespace {
 struct AdjGrads {
     double *dP = nullptr, *dq = nullptr, *dr = nullptr, *dG = nullptr, *dA = nullptr;
 };
-// the adjoint of a solved QP or QC batch (the entry points check the kind and the solve): the right-hand side, for a
-// QC batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement step on the full
-// system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG ml x n per problem
+// kkt_chol2's switch at the adjoint's factorisation (misc.py:1421-1447), once batch_factor has run: a problem whose
+// S is singular there factors S + A'A, next to those the solve already switched.  Without P, at a converged iterate
+// whose W'W spans many orders of magnitude, G' W^{-1} W^{-T} G is numerically singular when fewer than n rows are
+// active, which a cone LP's vertex has with equality rows.  aw0: the solve's aw (slot order), for batch_adjoint to
+// restore; empty when every factorisation succeeded and nothing changed
+int adj_switch(cvxb_batch *b, std::vector<double> &aw0) {
+    cudaStream_t st = b->st;
+    const int B = b->B, pq = b->neq;
+    std::vector<int> info(B);
+    CVXB_CUDA(cudaMemcpyAsync(info.data(), b->d_info.p, B * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    if (std::none_of(info.begin(), info.end(), [](int v) { return v > 0; })) return 0;
+    aw0.resize((size_t)B * pq);
+    CVXB_CUDA(cudaMemcpyAsync(aw0.data(), b->p.aw, aw0.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i < B; ++i) info[i] = info[i] > 0 || aw0[(size_t)i * pq] != 0.0;   // k_switch's flags
+    CVXB_CUDA(cudaMemcpyAsync(b->d_pairs.p, info.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+    k_switch<<<(unsigned)B, 256, 0, st>>>(b->p.aw, b->d_pairs.p, pq); count_launch();
+    b->switched = true;
+    return batch_factor(b);
+}
+
+// the adjoint of a solved QP, cone LP or QC batch (the entry points check the kind and the solve): the right-hand side,
+// for a QC batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement step on the full
+// system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG ml x n per
+// problem.  With 'q' cones or 's' blocks k_adj_cone and the 's' kernels fix the cone rows between the 'l' steps; a
+// cone LP has no P (its entry point refuses dP)
 int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                   double *uz, AdjGrads d, int space) {
     CVXB_CUDA(cudaSetDevice(b->device));
     cudaStream_t st = b->st;
-    const bool qc = b->kind == Kind::QC;
+    const bool qc = b->kind == Kind::QC, lp = b->kind == Kind::LP;
+    const bool cones = b->p.nq > 0 || b->p.ns > 0, sdp = b->p.ns > 0;
     const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = qc ? b->gq.nK : 1, ml = qc ? m - b->gq.mnl : m;
     const Ptrs &p = b->p;
     // host space: every given array staged on the device (inputs uploaded, outputs copied back); device: in place
@@ -3729,6 +3846,12 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
     b->Bact = b->B;
     CVXB_CUDA(cudaMemcpyAsync(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
     k_adj_rhs<<<(unsigned)B, 256, 0, st>>>(p, s_gx.dev, s_gy.dev, s_gz.dev, b->d_perm.p); count_launch();
+    const dim3 sg(p.ns, (unsigned)B);                  // one CTA per ('s' block, slot)
+    if (cones) { k_adj_cone<<<(unsigned)B, 256, 0, st>>>(p, b->d_info.p, 0); count_launch(); }
+    if (sdp) {
+        k_adj_s_nt<<<sg, SB_T, 0, st>>>(p); count_launch();
+        k_s_wtz<<<sg, SB_T, 0, st>>>(p, p.rz, (long long)m, nullptr, 0, 0); count_launch();
+    }
     if (qc) {
         CVXB_TRY(gp_products(b, p.x, n));
         const long long work = std::max(n * n, (size_t)b->gq.mnl * n);
@@ -3736,27 +3859,39 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
         count_launch();
     }
     CVXB_TRY(batch_factor(b));
+    std::vector<double> aw0;                             // the solve's aw when adj_switch changed it
+    const bool switched0 = b->switched;
+    if (pq && (lp || cones)) CVXB_TRY(adj_switch(b, aw0));
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
     // one step of iterative refinement on the full KKT system: W'W spans many orders of magnitude at a converged
     // iterate, and the reduced solve alone loses digits to it.  r = g - M u, then u += M^{-1} r with the same factor
     const int Bi = (int)B, ni = (int)n, mi = (int)m, pi = (int)pq;
     k_adj_uz<<<(unsigned)B, 256, 0, st>>>(p); count_launch();
-    GemvBatch gP; gP.batch = Bi; gP.sA = b->sP; gP.sx = ni; gP.sy = ni;
-    CVXB_TRY(gemv_t(ni, ni, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.rx, st, gP));
+    // the info that k_adj_cone sets for a failed 's' scaling is the factorisation's, so it goes after batch_factor
+    if (cones) { k_adj_cone<<<(unsigned)B, 256, 0, st>>>(p, b->d_info.p, 1); count_launch(); }
+    if (sdp) { k_adj_s<<<sg, SB_T, 0, st>>>(p, 0); count_launch(); }
+    if (!lp) {
+        GemvBatch gP; gP.batch = Bi; gP.sA = b->sP; gP.sx = ni; gP.sy = ni;
+        CVXB_TRY(gemv_t(ni, ni, b->P.p, b->ldp, nullptr, p.dx, -1.0, 1.0, p.rx, st, gP));
+    }
     if (pq) {
         GemvBatch gt; gt.batch = Bi; gt.sA = b->sA; gt.sx = pi; gt.sy = ni;
         CVXB_TRY(gemv_t(pi, ni, b->A.p, b->lda, nullptr, p.dy, -1.0, 1.0, p.rx, st, gt));
         GemvBatch gn; gn.batch = Bi; gn.sA = b->sA; gn.sx = ni; gn.sy = pi;
         CVXB_TRY(gemv_n(pi, ni, b->A.p, b->lda, nullptr, p.dx, -1.0, 1.0, p.ry, b->gemv_ws.p, st, gn));
     }
-    if (m) {
+    if (m) {                                           // 's' blocks: G' trisc(uz), the G the solver reads (rw)
         GemvBatch gt; gt.batch = Bi; gt.sA = b->sG; gt.sx = mi; gt.sy = ni;
-        CVXB_TRY(gemv_t(mi, ni, b->G.p, b->ldg, nullptr, p.dz, -1.0, 1.0, p.rx, st, gt));
+        CVXB_TRY(gemv_t(mi, ni, b->G.p, b->ldg, p.rw, p.dz, -1.0, 1.0, p.rx, st, gt));
         GemvBatch gn; gn.batch = Bi; gn.sA = b->sG; gn.sx = ni; gn.sy = mi;
         CVXB_TRY(gemv_n(mi, ni, b->G.p, b->ldg, nullptr, p.dx, -1.0, 1.0, p.rz, b->gemv_ws.p, st, gn));
     }
     k_adj_res<<<(unsigned)B, 256, 0, st>>>(p); count_launch();
+    if (p.nq) { k_adj_cone<<<(unsigned)B, 256, 0, st>>>(p, b->d_info.p, 2); count_launch(); }
+    if (sdp) { k_adj_s<<<sg, SB_T, 0, st>>>(p, 1); count_launch(); }
     CVXB_TRY(batch_solve(b, p.rx, n, p.ry, pq));
+    if (sdp) { k_adj_s<<<sg, SB_T, 0, st>>>(p, 2); count_launch(); }
+    if (cones) { k_adj_cone<<<(unsigned)B, 256, 0, st>>>(p, b->d_info.p, 3); count_launch(); }
     k_adj_vecs<<<(unsigned)B, 256, 0, st>>>(p, s_ux.dev, s_uy.dev, s_uz.dev, b->d_perm.p, b->d_info.p);
     count_launch();
     if (s_dP.dev || s_dq.dev || s_dr.dev || s_dG.dev || s_dA.dev) {
@@ -3768,6 +3903,10 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
     }
     CVXB_LAUNCH_CHECK();
     for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dq, &s_dr, &s_dG, &s_dA}) CVXB_TRY(s->out(st));
+    if (!aw0.empty()) {                                  // the solver's state as the solve left it
+        CVXB_CUDA(cudaMemcpyAsync(p.aw, aw0.data(), aw0.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        b->switched = switched0;
+    }
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;
 }
@@ -3797,6 +3936,21 @@ int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, c
         return CVXB_E_ARG;
     }
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, dq, dr, dG, dA}, space);
+}
+
+int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
+                            double *uy, double *uz, double *dP, double *dG, double *dA, int space) {
+    if (!b) { set_error("batch_adjoint_cone: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QP && b->kind != Kind::LP) {
+        set_error("batch_adjoint_cone: only QP and cone LP batches are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (b->kind == Kind::LP && dP) { set_error("batch_adjoint_cone: a cone LP has no P: dP must be NULL"); return CVXB_E_ARG; }
+    if (!b->solved) {
+        set_error("batch_adjoint_cone: no completed cvxb_batch_solve since the last load");
+        return CVXB_E_ARG;
+    }
+    return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, nullptr, nullptr, dG, dA}, space);
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {

@@ -3,9 +3,11 @@
     x, y, z, status = qp_layer(P, q, G, h, A, b)   solves   minimize 1/2 x'P x + q'x  s.t.  G x <= h,  A x = b
     x, y, znl, zl, status = qcqp_layer(P, q, r, G, h, A, b)   solves   minimize f_0(x)  s.t.  f_i(x) <= 0 (i >= 1),
         G x <= h,  A x = b,   f_i(x) = x'P_i x / 2 + q_i'x + r_i
+    x, y, z, status = coneqp_layer(P, q, G, h, dims, A, b)   solves   minimize 1/2 x'P x + q'x  s.t.  G x + s = h,
+        s in the cone of dims ('l', 'q', 's'),  A x = b;   conelp_layer(c, G, h, dims, A, b) the same with P = 0
 
 for B problems at once with qp_batch's and qcqp_batch's algorithms, and their backward runs the library's adjoint
-(cvxb_batch_adjoint, cvxb_batch_adjoint_qcqp): one more factorisation and solve of the KKT system at the returned
+(cvxb_batch_adjoint, cvxb_batch_adjoint_qcqp, cvxb_batch_adjoint_cone): one more factorisation and solve of the KKT system at the returned
 iterate, then the gradients written by one kernel.  Nothing leaves the device.  The gradient of each P is the symmetric
 one (the solvers read only lower triangles), so a P built as S + S' or from an expanded tensor gets the right gradient
 from autograd.  A problem whose status is not optimal (status != 1) gets NaN gradients.
@@ -15,7 +17,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .batch import QCQPBatchGroup, QPBatchGroup
+from .batch import BATCH_SMAX, ConeLPBatchGroup, QCQPBatchGroup, QPBatchGroup, SDPBatchGroup, SDPQPBatchGroup
 
 
 def _typed(named):
@@ -52,12 +54,14 @@ def _dims(dims, m, layer):
             raise TypeError("dims['l'] = %d does not match G's %d rows" % (int(dims.get("l", 0)), m))
 
 
-def _on_device(named, P):
+def _on_device(named):
+    """every tensor of `named` on one CUDA device, the first one's"""
+    first, ref = named[0]
     for name, t in named:
         if t.device.type != "cuda":
             raise TypeError("%s must be a CUDA tensor" % name)
-        if t.device != P.device:
-            raise TypeError("%s is on %s, P on %s" % (name, t.device, P.device))
+        if t.device != ref.device:
+            raise TypeError("%s is on %s, %s on %s" % (name, t.device, first, ref.device))
 
 
 def _check(P, q, G, h, A, b, dims):
@@ -76,7 +80,7 @@ def _check(P, q, G, h, A, b, dims):
         raise TypeError("q must have shape (%d, %d)" % (B, n))
     m, p = _constraint_rows(B, n, G, h, A, b)
     _dims(dims, m, "qp_layer")
-    _on_device(named, P)
+    _on_device(named)
     return B, n, m, p
 
 
@@ -102,8 +106,35 @@ def _check_qcqp(P, q, r, G, h, A, b, x0, dims):
         raise TypeError("x0 must have shape (%d, %d)" % (B, n))
     ml, p = _constraint_rows(B, n, G, h, A, b)
     _dims(dims, ml, "qcqp_layer")
-    _on_device(named, P)
+    _on_device(named)
     return B, nK - 1, n, ml, p
+
+
+def _check_cone(P, q, G, h, dims, A, b):
+    """coneqp_layer's and conelp_layer's _check (P None: a cone LP, q its c): every refusal before any device work.
+    dims must count G's rows: 'l' + sum 'q' + sum of each 's' order squared.  Returns B, n, m, p"""
+    if (A is None) != (b is None):
+        raise TypeError("'A' and 'b' must be given together")
+    qn = "c" if P is None else "q"
+    named = ([] if P is None else [("P", P)]) + [(qn, q), ("G", G), ("h", h)] + \
+        ([("A", A), ("b", b)] if A is not None else [])
+    _typed(named)
+    if q.dim() != 2 or q.shape[0] < 1 or q.shape[1] < 1:
+        raise TypeError("%s must have shape (B, n) with B and n positive" % qn)
+    B, n = q.shape
+    if P is not None and tuple(P.shape) != (B, n, n):
+        raise TypeError("P must have shape (%d, %d, %d)" % (B, n, n))
+    m, p = _constraint_rows(B, n, G, h, A, b)
+    if not isinstance(dims, dict) or not set(dims) <= {"l", "q", "s"}:
+        raise TypeError("dims must be a dictionary with keys 'l', 'q' and 's'")
+    if int(dims.get("l", 0)) < 0 or any(int(k) < 1 for k in dims.get("q", [])) or \
+            any(not 0 <= int(k) <= BATCH_SMAX for k in dims.get("s", [])):
+        raise TypeError("dims: 'l' must be nonnegative, each 'q' size at least 1, each 's' order in 0..%d" % BATCH_SMAX)
+    cdim = int(dims.get("l", 0)) + sum(int(k) for k in dims.get("q", [])) + sum(int(k) ** 2 for k in dims.get("s", []))
+    if cdim != m:
+        raise TypeError("dims has %d rows ('l' + sum 'q' + sum 's'²), G and h have %d" % (cdim, m))
+    _on_device(named)
+    return B, n, m, p
 
 
 def _rows(t, it):
@@ -208,26 +239,67 @@ class _QPLayer(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gz, _gstatus):
-        B, n, m, p = ctx.shapes
-        need = dict(zip(("P", "q", "G", "h", "A", "b"), ctx.needs_input_grad[:6]))
-        dev = gx.device if gx is not None else gz.device if gz is not None else gy.device
-        # C's outputs ux, uy, uz, dP, dG, dA in problem order; the matrices column-major per problem
-        shapes = {"q": (n,), "b": (p,), "h": (m,), "P": (n, n), "G": (n, m), "A": (n, p)}
-        shapes = {k: s for k, s in shapes.items() if need[k] and (p or k not in ("b", "A"))}
-        out = _adjoint(ctx, (gx, gy if p else None, gz if m else None), shapes,
-                       lambda part, g, o: part.adjoint_ptr(*g, *(o.get(k) for k in ("q", "b", "h", "P", "G", "A")),
-                                                           space=_lib.DEVICE), dev)
-        f64 = dict(dtype=torch.float64, device=dev)
-        grads = {"q": lambda t: -t, "b": lambda t: t, "h": lambda t: t}
-        res = []
-        for key in ("P", "q", "G", "h", "A", "b"):
-            if key not in out:
-                res.append(torch.zeros((B, 0) if key == "b" else (B, 0, n), **f64) if need[key] else None)
-            elif key in grads:
-                res.append(grads[key](out[key]))
-            else:
-                res.append(out[key].transpose(1, 2))
-        return (*res, None, None)
+        return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_ptr), None, None)
+
+
+def _qp_grads(ctx, gx, gy, gz, adjoint):
+    """the gradients of P, q, G, h, A and b for qp_layer and the cone layers (a cone LP: P None, q its c) from those of
+    x, y and z; adjoint(part) is the part's adjoint_ptr or adjoint_cone_ptr"""
+    B, n, m, p = ctx.shapes
+    need = dict(zip(("P", "q", "G", "h", "A", "b"), ctx.needs_input_grad[:6]))
+    dev = gx.device if gx is not None else gz.device if gz is not None else gy.device
+    # C's outputs ux, uy, uz, dP, dG, dA in problem order; the matrices column-major per problem
+    shapes = {"q": (n,), "b": (p,), "h": (m,), "P": (n, n), "G": (n, m), "A": (n, p)}
+    shapes = {k: s for k, s in shapes.items() if need[k] and (p or k not in ("b", "A"))}
+    out = _adjoint(ctx, (gx, gy if p else None, gz if m else None), shapes,
+                   lambda part, g, o: adjoint(part)(*g, *(o.get(k) for k in ("q", "b", "h", "P", "G", "A")),
+                                                    space=_lib.DEVICE), dev)
+    f64 = dict(dtype=torch.float64, device=dev)
+    grads = {"q": lambda t: -t, "b": lambda t: t, "h": lambda t: t}
+    res = []
+    for key in ("P", "q", "G", "h", "A", "b"):
+        if key not in out:
+            res.append(torch.zeros((B, 0) if key == "b" else (B, 0, n), **f64) if need[key] else None)
+        elif key in grads:
+            res.append(grads[key](out[key]))
+        else:
+            res.append(out[key].transpose(1, 2))
+    return res
+
+
+class _ConeLayer(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, P, q, G, h, A, b, dims, nsub, options):
+        B, n, m, p = ctx.shapes = _check_cone(P, q, G, h, dims, A, b)
+        dev = q.device
+        device = dev.index if dev.index is not None else torch.cuda.current_device()
+        # the layouts the library loads: P, G and A column-major per problem
+        data = {"q": q.contiguous(), "G": G.transpose(1, 2).contiguous(), "h": h.contiguous()}
+        if P is not None:
+            data["P"] = P.transpose(1, 2).contiguous()
+        if p:
+            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
+        if P is not None:            # coneqp_batch's group
+            grp, head = SDPQPBatchGroup(B, n, dims, p, device, nsub), ("P", "q", "G", "h")
+        elif dims.get("s"):          # sdp_batch's
+            grp, head = SDPBatchGroup(B, n, dims, p, device, nsub), ("q", "G", "h")
+        else:                        # conelp_batch's
+            grp = ConeLPBatchGroup(B, n, m, device, nsub, {"l": dims.get("l", 0), "q": dims.get("q", [])}, p)
+            head = ("q", "G", "h")
+        try:
+            its, x, _, z, y, status = _solve(
+                grp, data, lambda part, a: part.load_ptr(*(a[k] for k in head), _lib.DEVICE, a.get("A"), a.get("b")),
+                options, dev, (n, m, p))
+        except BaseException:
+            grp.close()
+            raise
+        _keep(ctx, grp, its, ctx.needs_input_grad[:6])
+        return x, y, z, status
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gx, gy, gz, _gstatus):
+        return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_cone_ptr), None, None, None)
 
 
 class _QCQPLayer(torch.autograd.Function):
@@ -320,3 +392,33 @@ def qcqp_layer(P, q, r, G=None, h=None, A=None, b=None, x0=None, nsub=None, **op
     that need no gradient get none and cost nothing.  The solved batch is kept on the device from forward to backward,
     and freed by backward."""
     return _QCQPLayer.apply(P, q, r, G, h, A, b, x0, nsub, dict(options))
+
+
+def coneqp_layer(P, q, G, h, dims, A=None, b=None, nsub=None, **options):
+    """Solve B cone QPs  minimize 1/2 x'P x + q'x  s.t.  G x + s = h,  s in C,  A x = b  on the GPU, differentiably
+    (coneqp_batch's algorithm: solvers.coneqp's).
+
+    P (B, n, n), q (B, n), G (B, m, n), h (B, m), A (B, p, n) and b (B, p): CUDA float64 tensors on one device; A and
+    b are optional and given together.  dims: the cone C shared by every problem, {'l': ml, 'q': [...], 's': [...]}
+    ('s' orders at most 32), with m = ml + sum 'q' + sum of the 's' orders squared.  G's and h's rows are the 'l' rows,
+    each 'q' cone, then each 's' block unpacked column-major; only an 's' block's lower triangle is read.  Returns
+    (x, y, z, status_code): x (B, n), y (B, p), z (B, m) laid out as h with symmetric 's' blocks, and the int32 status
+    per problem (1 optimal).  nsub: sub-batches solved concurrently, as qp_batch's.  options: maxiters, abstol,
+    reltol, feastol, refinement.  Shape, dtype, device and dims errors are TypeErrors raised before any device work.
+
+    Backward (once: no double backward) returns dL/dP (symmetric), dL/dq, dL/dG, dL/dh, dL/dA and dL/db from the
+    gradients of x, y and z (cvxb_batch_adjoint_cone), with NaN for problems whose status is not 1.  An 's' block of
+    z's gradient enters through its symmetric part, and the 's' blocks of dL/dh and of each column of dL/dG are the
+    gradient over symmetric matrices, the same value in both triangles: a G whose 's' columns are built as X + X' gets
+    the right gradient from autograd.  The solved batch is kept on the device from forward to backward."""
+    return _ConeLayer.apply(P, q, G, h, A, b, dims, nsub, dict(options))
+
+
+def conelp_layer(c, G, h, dims, A=None, b=None, nsub=None, **options):
+    """Solve B cone LPs  minimize c'x  s.t.  G x + s = h,  s in C,  A x = b  on the GPU, differentiably
+    (conelp_batch's algorithm, sdp_batch's with 's' blocks: solvers.conelp's).
+
+    c (B, n) and the rest as coneqp_layer's, which this is with P = 0.  Returns (x, y, z, status_code); a problem
+    found infeasible (status 4 or 5) gets NaN gradients like any status other than 1.  Backward returns dL/dc, dL/dG,
+    dL/dh, dL/dA and dL/db with coneqp_layer's conventions."""
+    return _ConeLayer.apply(None, c, G, h, A, b, dims, nsub, dict(options))

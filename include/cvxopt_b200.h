@@ -564,6 +564,30 @@ int cvxb_batch_load_qcqp(cvxb_batch *b, const double *P, const double *q, const 
 int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
                             double *uy, double *uz, double *dP, double *dq, double *dr, double *dG, double *dA,
                             int space);
+/* Derivatives of a cone QP or cone LP batch's last solve, cvxb_batch_adjoint's counterpart for batches with 'q' cones
+ * and 's' blocks.  At the returned iterate it solves
+ *     [P A' G'; A 0 0; G 0 -W'W] [ux; uy; uz] = [gx; gy; gz]
+ * with W the Nesterov-Todd scaling of the returned s and z: diag(s / z) on the 'l' rows, W = beta (2 v v' - J) on a
+ * 'q' cone, W'W(X) = r r' X r r' on an 's' block; P = 0 for a cone LP.  It factors the reduced KKT matrix once more,
+ * takes one step of iterative refinement on the full system, and writes ux, uy, uz, dP, dG and dA with
+ * cvxb_batch_adjoint's formulas and layouts: dL/dq (dL/dc) = -ux, dL/dh = uz, dL/db = uy.  This is the interior-point
+ * linearisation at the returned iterate, exact on the central path; at a degenerate solution it is not the derivative
+ * of the solution map.
+ * 's' blocks: every 's' block of gz, uz and each column of dG is unpacked column-major, as the results' z, and the
+ * pairing is the trace inner product, dL = sum over all unpacked entries of g * d.  Only the symmetric part
+ * (gz + gz') / 2 of a gz block enters, so a gradient given on one triangle and its transpose give the same outputs.
+ * Both triangles of uz's and dG's 's' blocks hold the same value, the gradient over symmetric matrices (as dP for P,
+ * whose lower triangle alone is read), so a G whose 's' columns are built as X + X' gets the right gradient.
+ * Accepts every QP batch (cvxb_batch_create, _cones, _eq, _sdp_qp) and every cone LP batch (cvxb_batch_create_lp,
+ * _sdp); GP, CP, cpl and QCQP batches are CVXB_E_UNSUP.  dP must be NULL on a cone LP batch (CVXB_E_ARG).  A NULL
+ * input is zero; a NULL output is not written and its work is skipped.  A problem whose status is not 1 (optimal: a
+ * cone LP's infeasibility certificates included), whose KKT matrix has no Cholesky factor at that iterate, or whose
+ * 's' scaling fails there (a block Cholesky factor or the SVD) gets NaN in all its outputs.  On a QP batch with 'l'
+ * rows only it is cvxb_batch_adjoint, bit for bit.  cvxb_batch_results is unchanged afterwards and a re-solve
+ * computes the same results.  A batch without a completed cvxb_batch_solve since its last load is CVXB_E_ARG.
+ * CVXB_DEVICE allocates nothing; CVXB_HOST stages as cvxb_batch_adjoint does. */
+int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
+                            double *uy, double *uz, double *dP, double *dG, double *dA, int space);
 
 #ifdef __cplusplus
 }
