@@ -170,6 +170,7 @@ def _sdp_dims(dims, m=None):
 ADJOINT_KEYS = ("P", "q", "G", "h", "A", "b")
 QCQP_ADJOINT_KEYS = ("P", "q", "r", "G", "h", "A", "b")
 CONELP_ADJOINT_KEYS = ("c", "G", "h", "A", "b")
+GP_ADJOINT_KEYS = ("F", "g", "G", "h", "A", "b")
 
 
 def _adjoint_args(gx, gy, gz, want, B, n, p, m, keys=ADJOINT_KEYS):
@@ -751,10 +752,37 @@ class GPBatch(QPBatch):
         Acm, bv = self._host_eq(A, b)
         Fcm = np.ascontiguousarray(np.transpose(F, (0, 2, 1)))
         Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
-        _lib.check(self._lib.cvxb_batch_load_gp(self._h, Fcm.ctypes.data, g.ctypes.data,
-                                                Gcm.ctypes.data if self.ml else None,
-                                                h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_gp")
-        self._load_eq(Acm, bv, _lib.HOST)
+        self.load_ptr(Fcm.ctypes.data, g.ctypes.data, Gcm.ctypes.data if self.ml else None,
+                      h.ctypes.data if self.ml else None, _lib.HOST, Acm, bv)
+
+    def load_ptr(self, F, g, G, h, space=_lib.DEVICE, A=None, b=None):
+        """cvxb_batch_load_gp on raw addresses in `space` (device-resident callers): F sum K x n column-major per
+        problem, g, G ml x n column-major and h (None when ml = 0); A p x n column-major and b"""
+        _lib.check(self._lib.cvxb_batch_load_gp(self._h, F, g, G, h, space), "batch_load_gp")
+        self._load_eq(A, b, space)
+
+    def adjoint_gp(self, gx, gy=None, gz=None, want=GP_ADJOINT_KEYS):
+        """derivatives of the last solve's results for a loss L with gradients gx = dL/dx (B, n), gy = dL/dy (B, p)
+        and gz = dL/dz (B, mnl + ml, laid out as [znl, zl]), None meaning zero (cvxb_batch_adjoint_gp).  Returns host
+        arrays for the keys in `want`, each dL/d(that input) in load()'s layout: F (B, sum K, n), g (B, sum K),
+        G (B, ml, n), h (B, ml), A (B, p, n) and b (B, p).  A problem whose status is not 'optimal' gets NaN.  A batch
+        not solved since its last load raises ValueError."""
+        B, n, m, p, ml, S = self.B, self.n, self.m, self.p, self.ml, sum(self.K)
+        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m, GP_ADJOINT_KEYS)
+        # C's outputs uy, uz (h: its 'l' rows), dF, dg, dG, dA; dF, dG and dA column-major per problem
+        shapes = {"b": (B, p), "h": (B, m), "F": (B, n, S), "g": (B, S), "G": (B, n, ml), "A": (B, n, p)}
+        bufs = {k: np.empty(shapes[k]) for k in want}
+        ptrs = [None if a is None else a.ctypes.data for a in gs] + [None]
+        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("b", "h", "F", "g", "G", "A")]
+        self.adjoint_gp_ptr(*ptrs, space=_lib.HOST)
+        return {k: v[:, self.mnl:] if k == "h" else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
+                for k, v in bufs.items()}
+
+    def adjoint_gp_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dF=None, dg=None, dG=None,
+                       dA=None, space=_lib.DEVICE):
+        """cvxb_batch_adjoint_gp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_adjoint_gp(self._h, gx, gy, gz, ux, uy, uz, dF, dg, dG, dA, space),
+                   "batch_adjoint_gp")
 
     def stats(self):
         out = super().stats()
@@ -774,6 +802,16 @@ class GPBatchGroup(QPBatchGroup):
 
     def load(self, F, g, G, h, A=None, b=None):
         self._load_sliced((F, g, G, h), A, b)
+
+    def adjoint_gp(self, gx, gy=None, gz=None, want=GP_ADJOINT_KEYS):
+        """GPBatch.adjoint_gp on every part with its slice of the gradients, the results in problem order"""
+        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m, GP_ADJOINT_KEYS)
+        out = {}
+        for ix, part in zip(self.idx, self.parts):
+            r = part.adjoint_gp(*(None if a is None else a[ix] for a in gs), want=want)
+            for k, v in r.items():
+                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
+        return out
 
     def stats(self):
         out = super().stats()

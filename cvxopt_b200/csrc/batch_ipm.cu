@@ -1443,13 +1443,14 @@ template <bool CONES, bool SDP = false> __global__ void k_gp_init(Ptrs p, GPPtrs
 }
 // F(x) of gp (:2102-2153) for block i of slot b, grid (nK, Bact): yv holds F x on entry; y := softmax(F x + g),
 // f_i = max + log sum exp, w = z_i y (z_i from z, or from the trial point's nz).  FULL: also Df_i = Fi' y (grad f0 or
-// row i - 1 of G), H's rows sqrt(y_k)(F_k - Df_i) and their weights z_i.  trial: only slots still searching
-template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) {
+// row i - 1 of G), H's rows sqrt(y_k)(F_k - Df_i) and their weights z_i.  trial: only slots still searching.
+// ADJ (k_adj_gp_op, FULL): every slot, z_0 = 1, and neither w nor grad f0, which the adjoint does not read
+template <bool FULL, bool ADJ> __device__ __forceinline__ void gp_eval_body(const Ptrs &p, const GPPtrs &g, int trial) {
     const int i = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, nt = blockDim.x;
     const int lane = tid & 31, warp = tid >> 5, nwarp = nt >> 5;
     __shared__ double sh[32];
     const GPScal &T = gp_scal(g, (long long)b * p.L);
-    if (p.sc[b].done || (trial && T.searching == 0.0)) return;
+    if (!ADJ && (p.sc[b].done || (trial && T.searching == 0.0))) return;
     const int k0 = g.koff[i], K = g.koff[i + 1] - k0;
     const long long ok = (long long)b * g.sumK + k0;
     const double *F = g.G + (long long)b * g.sG + p.m + k0, *gv = g.g + (long long)b * p.L + k0;
@@ -1462,10 +1463,11 @@ template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) {
     sum = block_sum(sum, sh);
     const double r = 1.0 / sum;
     const double *zs = trial ? g.nz : p.z;
-    const double zi = i == 0 ? (trial ? T.nz0 : T.z0) : zs[(long long)b * p.m + i - 1];
+    const double zi = i == 0 ? (ADJ ? 1.0 : trial ? T.nz0 : T.z0) : zs[(long long)b * p.m + i - 1];
     for (int k = tid; k < K; k += nt) {
         const double v = y[k] * r;
-        y[k] = v; g.wv[ok + k] = zi * v;
+        y[k] = v;
+        if (!ADJ) g.wv[ok + k] = zi * v;
         if (FULL) g.hw[ok + k] = zi;
     }
     if (tid == 0) g.fv[(long long)b * g.nK + i] = mx + log(sum);
@@ -1478,12 +1480,13 @@ template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) {
         for (int k = lane; k < K; k += 32) a += Fj[k] * y[k];
         a = warp_sum(a);
         if (lane == 0) {
-            if (i == 0) g.gf0[(long long)b * p.n + j] = a;
+            if (i == 0) { if (!ADJ) g.gf0[(long long)b * p.n + j] = a; }
             else g.G[(long long)b * g.sG + (i - 1) + (long long)j * g.ldg] = a;
         }
         for (int k = lane; k < K; k += 32) hr[k + (long long)j * g.ldh] = sqrt(y[k]) * (Fj[k] - a);
     }
 }
+template <bool FULL> __global__ void k_gp_eval(Ptrs p, GPPtrs g, int trial) { gp_eval_body<FULL, false>(p, g, trial); }
 // residuals, part 1 (:668-691): rx = 0 (the GEMVs add Df'znl + G'zl + A'y), rxt = 1 - z0; rz = s + f on the
 // nonlinear rows, s - h on the 'l' rows (G x follows); rznl's epigraph row s0 + f0 - t; EQ: ry = b (A x - ry follows).
 // Without the epigraph row (EPI false, a cpl batch): rx = c, and f has no objective entry
@@ -2353,6 +2356,61 @@ __global__ void __launch_bounds__(256) k_adj_qc_grad(Ptrs p, GPPtrs g, double *d
                             [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
 }
 
+// ---- the adjoint of a GP batch's solution (cvxb_batch_adjoint_gp) ----
+// The QCQP's derivation with f_i(x) = lse(F_i x + g_i): at the returned iterate, with z_0 = 1, pi_i = softmax(F_i x +
+// g_i) and Sigma_i = diag(pi_i) - pi_i pi_i', the KKT matrix has H = sum_i z_i F_i' Sigma_i F_i and Df's rows
+// pi_i' F_i.  For a parameter t of f_i, dL/dt = -(z_i d_t(ux' grad f_i) + uz_i d_t f_i); with w_i = F_i ux and v_i =
+// Sigma_i w_i = pi_i o (w_i - pi_i' w_i) that is dL/dg_i = -(z_i v_i + uz_i pi_i) and dL/dF_i = dL/dg_i x' -
+// z_i pi_i ux', uz_0 = 0.  A monomial row (K_i = 1: pi = 1, Sigma = 0) gets the QP's dh and dG with h = -g.
+// The operator at x, once gp_products has left F x in yv: k_gp_eval<true>'s body on every slot with z_0 = 1, so pi in
+// yv, Df into G's rows [0, mnl), f into fv, and H's rows and their weights z_i in Hr and hw for gp_hessian
+__global__ void k_adj_gp_op(Ptrs p, GPPtrs g) { gp_eval_body<true, true>(p, g, 0); }
+// once the batched GEMV has left w = F ux in wv, grid (nK, B): block i of slot b reduces pi_i' w_i and replaces w_i by
+// dL/dg_i in wv, stored into problem perm[b]'s row of dg (nullptr: not written), S = sum K per problem
+__global__ void k_adj_gp_dg(Ptrs p, GPPtrs g, double *dg, const int *perm, const int *info) {
+    const int i = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, nt = blockDim.x;
+    __shared__ double sh[32];
+    const int k0 = g.koff[i], K = g.koff[i + 1] - k0;
+    const long long ok = (long long)b * g.sumK + k0, om = (long long)b * p.m;
+    const double *pi = g.yv + ok;
+    double *w = g.wv + ok;
+    double t = 0.0;
+    for (int k = tid; k < K; k += nt) t += pi[k] * w[k];
+    t = block_sum(t, sh);
+    const double zi = i == 0 ? 1.0 : p.z[om + i - 1], uzi = i == 0 ? 0.0 : p.bzp[om + i - 1];
+    const bool bad = adj_bad(p, info, b);
+    double *o = dg ? dg + (long long)perm[b] * g.sumK + k0 : nullptr;
+    for (int k = tid; k < K; k += nt) {
+        const double v = -(zi * (pi[k] * (w[k] - t)) + uzi * pi[k]);
+        w[k] = v;
+        if (o) o[k] = bad ? NAN : v;
+    }
+}
+// dF, dG and dA (nullptr: not written) of problem perm[b] over columns [j0, j0 + ADJ_TJ), grid (ceil(n / ADJ_TJ), B),
+// as k_adj_grad: dF per problem the S x n column-major F of cvxb_batch_load_gp, row k dg_k x' - hw_k pi_k ux' from
+// k_adj_gp_dg's dg in wv; dG over the 'l' rows only (rows mnl.. of z and uz)
+__global__ void __launch_bounds__(256) k_adj_gp_grad(Ptrs p, GPPtrs g, double *dF, double *dG, double *dA,
+                                                     const int *perm, const int *info) {
+    const int b = blockIdx.y, j0 = blockIdx.x * ADJ_TJ, nj = min(ADJ_TJ, p.n - j0), n = p.n, m = p.m, pq = p.neq;
+    const int S = g.sumK, ml = m - g.mnl;
+    const long long on = (long long)b * n, om = (long long)b * m, oq = (long long)b * pq, ok = (long long)b * S;
+    const long long k = perm[b];
+    const double *__restrict__ x = p.x + on, *__restrict__ ux = p.dx + on;
+    const double *__restrict__ z = p.z + om, *__restrict__ uz = p.bzp + om;
+    const double *__restrict__ y = p.y + oq, *__restrict__ uy = p.dy + oq;
+    const double *__restrict__ dgv = g.wv + ok, *__restrict__ pi = g.yv + ok, *__restrict__ hw = g.hw + ok;
+    __shared__ double xs[ADJ_TJ], uxs[ADJ_TJ];
+    if (threadIdx.x < nj) { xs[threadIdx.x] = x[j0 + threadIdx.x]; uxs[threadIdx.x] = ux[j0 + threadIdx.x]; }
+    __syncthreads();
+    const bool bad = adj_bad(p, info, b);
+    if (dF) adj_store(dF + (k * n + j0) * S, S, nj, bad,
+                      [&](int i, int c) { return dgv[i] * xs[c] - hw[i] * pi[i] * uxs[c]; });
+    if (dG && ml) adj_store(dG + (k * n + j0) * ml, ml, nj, bad,
+                            [&](int i, int c) { return -(z[g.mnl + i] * uxs[c] + uz[g.mnl + i] * xs[c]); });
+    if (dA && pq) adj_store(dA + (k * n + j0) * pq, pq, nj, bad,
+                            [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
+}
+
 // the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
 enum class Kind { QP, LP, GP, CP, CPL, QC };
 }  // namespace
@@ -2999,8 +3057,9 @@ int gp_rx(cvxb_batch *b, const double *z, const double *y, double *r, bool full)
     return 0;
 }
 // H = sum_i z_i Fi'(diag(yi) - yi yi')Fi from k_gp_eval's rows (the reference's syrk with alpha = z[i], :2141-2150),
-// lower triangle; mirrored when the refinement's residual multiplies by it
-int gp_hessian(cvxb_batch *b) {
+// lower triangle; mirrored when the refinement's residual multiplies by it, and always for the adjoint (mirror), whose
+// refinement step multiplies by H whatever the solve's refinement setting
+int gp_hessian(cvxb_batch *b, bool mirror = false) {
     const GPPtrs &g = b->gq;
     GemmDesc h;
     h.M = b->n; h.N = b->n; h.K = g.sumK;
@@ -3011,7 +3070,7 @@ int gp_hessian(cvxb_batch *b) {
     h.lower_only = true; h.batch = b->Bact;
     if (b->B == 1) h.splitk_ws = b->cw.splitk_ws.p;
     CVXB_TRY(dmma_gemm(h, b->st));
-    if (b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, b->st));
+    if (mirror || b->p.refinement) CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, b->st));
     return 0;
 }
 // a QC batch's H = z0 P_0 + sum_i z_i P_i at the iterates, mirrored when the refinement's residual multiplies by it
@@ -3792,9 +3851,11 @@ int cvxb_batch_solve(cvxb_batch *b, int maxiters, double abstol, double reltol, 
 }
 
 namespace {
-// the gradient outputs of an adjoint call (nullptr: not written); dq and dr are a QCQP batch's only
+// the gradient outputs of an adjoint call (nullptr: not written); dq and dr are a QCQP batch's only, dF and dg a GP
+// batch's
 struct AdjGrads {
     double *dP = nullptr, *dq = nullptr, *dr = nullptr, *dG = nullptr, *dA = nullptr;
+    double *dF = nullptr, *dg = nullptr;
 };
 // kkt_chol2's switch at the adjoint's factorisation (misc.py:1421-1447), once batch_factor has run: a problem whose
 // S is singular there factors S + A'A, next to those the solve already switched.  Without P, at a converged iterate
@@ -3818,21 +3879,24 @@ int adj_switch(cvxb_batch *b, std::vector<double> &aw0) {
     return batch_factor(b);
 }
 
-// the adjoint of a solved QP, cone LP or QC batch (the entry points check the kind and the solve): the right-hand side,
-// for a QC batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement step on the full
-// system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG ml x n per
-// problem.  With 'q' cones or 's' blocks k_adj_cone and the 's' kernels fix the cone rows between the 'l' steps; a
-// cone LP has no P (its entry point refuses dP)
+// the adjoint of a solved QP, cone LP, QC or GP batch (the entry points check the kind and the solve): the right-hand
+// side, for a QC or GP batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement
+// step on the full system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG
+// ml x n per problem.  GP: dF is S x n, dg S and dG ml x n per problem; the call overwrites P, G's Df rows, yv, wv, Hr,
+// hw and fv, all of which a solve rewrites before it reads them.  With 'q' cones or 's' blocks k_adj_cone and the 's'
+// kernels fix the cone rows between the 'l' steps; a cone LP has no P (its entry point refuses dP)
 int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                   double *uz, AdjGrads d, int space) {
     CVXB_CUDA(cudaSetDevice(b->device));
     cudaStream_t st = b->st;
-    const bool qc = b->kind == Kind::QC, lp = b->kind == Kind::LP;
+    const bool qc = b->kind == Kind::QC, lp = b->kind == Kind::LP, gp = b->kind == Kind::GP;
     const bool cones = b->p.nq > 0 || b->p.ns > 0, sdp = b->p.ns > 0;
-    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = qc ? b->gq.nK : 1, ml = qc ? m - b->gq.mnl : m;
+    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = qc ? b->gq.nK : 1;
+    const size_t ml = qc || gp ? m - b->gq.mnl : m, S = gp ? b->gq.sumK : 0;
     const Ptrs &p = b->p;
+    const GPPtrs &g = b->gq;
     // host space: every given array staged on the device (inputs uploaded, outputs copied back); device: in place
-    Staged s_gx, s_gy, s_gz, s_ux, s_uy, s_uz, s_dP, s_dq, s_dr, s_dG, s_dA;
+    Staged s_gx, s_gy, s_gz, s_ux, s_uy, s_uz, s_dP, s_dq, s_dr, s_dG, s_dA, s_dF, s_dg;
     auto stage = [&](Staged &s, const double *a, size_t len, bool in) -> int {
         if (a && len) CVXB_TRY(s.in(a, B * len, space, st, in));
         return 0;
@@ -3841,6 +3905,7 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
     CVXB_TRY(stage(s_ux, ux, n, false)); CVXB_TRY(stage(s_uy, uy, pq, false)); CVXB_TRY(stage(s_uz, uz, m, false));
     CVXB_TRY(stage(s_dP, d.dP, nK * n * n, false));
     if (qc) { CVXB_TRY(stage(s_dq, d.dq, nK * n, false)); CVXB_TRY(stage(s_dr, d.dr, nK, false)); }
+    if (gp) { CVXB_TRY(stage(s_dF, d.dF, S * n, false)); CVXB_TRY(stage(s_dg, d.dg, S, false)); }
     CVXB_TRY(stage(s_dG, d.dG, ml * n, false));
     CVXB_TRY(stage(s_dA, d.dA, pq * n, false));
     b->Bact = b->B;
@@ -3858,10 +3923,16 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
         k_adj_qc_op<<<dim3((unsigned)((work + 255) / 256), (unsigned)B), 256, 0, st>>>(p, b->gq, b->cq);
         count_launch();
     }
+    if (gp) {
+        CVXB_TRY(gp_products(b, p.x, n));
+        k_adj_gp_op<<<dim3((unsigned)g.nK, (unsigned)B), 256, 0, st>>>(p, g); count_launch();
+        CVXB_TRY(gp_hessian(b, true));
+    }
     CVXB_TRY(batch_factor(b));
     std::vector<double> aw0;                             // the solve's aw when adj_switch changed it
     const bool switched0 = b->switched;
-    if (pq && (lp || cones)) CVXB_TRY(adj_switch(b, aw0));
+    // a GP whose terms are all monomials is an LP, and S can be singular at its vertices as at a cone LP's
+    if (pq && (lp || cones || gp)) CVXB_TRY(adj_switch(b, aw0));
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
     // one step of iterative refinement on the full KKT system: W'W spans many orders of magnitude at a converged
     // iterate, and the reduced solve alone loses digits to it.  r = g - M u, then u += M^{-1} r with the same factor
@@ -3894,15 +3965,27 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
     if (cones) { k_adj_cone<<<(unsigned)B, 256, 0, st>>>(p, b->d_info.p, 3); count_launch(); }
     k_adj_vecs<<<(unsigned)B, 256, 0, st>>>(p, s_ux.dev, s_uy.dev, s_uz.dev, b->d_perm.p, b->d_info.p);
     count_launch();
-    if (s_dP.dev || s_dq.dev || s_dr.dev || s_dG.dev || s_dA.dev) {
-        const dim3 grid((unsigned)((n + ADJ_TJ - 1) / ADJ_TJ), (unsigned)B);
+    const dim3 grid((unsigned)((n + ADJ_TJ - 1) / ADJ_TJ), (unsigned)B);
+    if (gp) {
+        if (s_dF.dev || s_dg.dev) {                      // w = F ux into wv (yv holds pi), then dg in its place
+            GemvBatch gw; gw.batch = Bi; gw.sA = g.sG; gw.sx = ni; gw.sy = g.sumK;
+            CVXB_TRY(gemv_n(g.sumK, ni, g.G + m, g.ldg, nullptr, p.dx, 1.0, 0.0, g.wv, b->gemv_ws.p, st, gw));
+            k_adj_gp_dg<<<dim3((unsigned)g.nK, (unsigned)B), 256, 0, st>>>(p, g, s_dg.dev, b->d_perm.p,
+                                                                           b->d_info.p);
+            count_launch();
+        }
+        if (s_dF.dev || s_dG.dev || s_dA.dev) {
+            k_adj_gp_grad<<<grid, 256, 0, st>>>(p, g, s_dF.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
+            count_launch();
+        }
+    } else if (s_dP.dev || s_dq.dev || s_dr.dev || s_dG.dev || s_dA.dev) {
         if (qc) k_adj_qc_grad<<<grid, 256, 0, st>>>(p, b->gq, s_dP.dev, s_dq.dev, s_dr.dev, s_dG.dev, s_dA.dev,
                                                     b->d_perm.p, b->d_info.p);
         else k_adj_grad<<<grid, 256, 0, st>>>(p, s_dP.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
         count_launch();
     }
     CVXB_LAUNCH_CHECK();
-    for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dq, &s_dr, &s_dG, &s_dA}) CVXB_TRY(s->out(st));
+    for (Staged *s : {&s_ux, &s_uy, &s_uz, &s_dP, &s_dq, &s_dr, &s_dG, &s_dA, &s_dF, &s_dg}) CVXB_TRY(s->out(st));
     if (!aw0.empty()) {                                  // the solver's state as the solve left it
         CVXB_CUDA(cudaMemcpyAsync(p.aw, aw0.data(), aw0.size() * sizeof(double), cudaMemcpyHostToDevice, st));
         b->switched = switched0;
@@ -3936,6 +4019,22 @@ int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, c
         return CVXB_E_ARG;
     }
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, dq, dr, dG, dA}, space);
+}
+
+int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                          double *uz, double *dF, double *dg, double *dG, double *dA, int space) {
+    if (!b) { set_error("batch_adjoint_gp: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::GP) {
+        set_error("batch_adjoint_gp: only GP batches (cvxb_batch_create_gp) are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (!b->solved) {
+        set_error("batch_adjoint_gp: no completed cvxb_batch_solve since the last load");
+        return CVXB_E_ARG;
+    }
+    AdjGrads d;
+    d.dF = dF; d.dg = dg; d.dG = dG; d.dA = dA;
+    return batch_adjoint(b, gx, gy, gz, ux, uy, uz, d, space);
 }
 
 int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,

@@ -5,10 +5,12 @@
         G x <= h,  A x = b,   f_i(x) = x'P_i x / 2 + q_i'x + r_i
     x, y, z, status = coneqp_layer(P, q, G, h, dims, A, b)   solves   minimize 1/2 x'P x + q'x  s.t.  G x + s = h,
         s in the cone of dims ('l', 'q', 's'),  A x = b;   conelp_layer(c, G, h, dims, A, b) the same with P = 0
+    x, y, znl, zl, status = gp_layer(K, F, g, G, h, A, b)   solves   minimize lse(F_0 x + g_0)  s.t.
+        lse(F_i x + g_i) <= 0 (i >= 1),  G x <= h,  A x = b   (a geometric program in log form)
 
-for B problems at once with qp_batch's and qcqp_batch's algorithms, and their backward runs the library's adjoint
-(cvxb_batch_adjoint, cvxb_batch_adjoint_qcqp, cvxb_batch_adjoint_cone): one more factorisation and solve of the KKT system at the returned
-iterate, then the gradients written by one kernel.  Nothing leaves the device.  The gradient of each P is the symmetric
+for B problems at once with qp_batch's, qcqp_batch's and gp_batch's algorithms, and their backward runs the library's
+adjoint (cvxb_batch_adjoint, cvxb_batch_adjoint_qcqp, cvxb_batch_adjoint_cone, cvxb_batch_adjoint_gp): one more
+factorisation and solve of the KKT system at the returned iterate, then the gradients written by one kernel.  Nothing leaves the device.  The gradient of each P is the symmetric
 one (the solvers read only lower triangles), so a P built as S + S' or from an expanded tensor gets the right gradient
 from autograd.  A problem whose status is not optimal (status != 1) gets NaN gradients.
 """
@@ -17,7 +19,8 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .batch import BATCH_SMAX, ConeLPBatchGroup, QCQPBatchGroup, QPBatchGroup, SDPBatchGroup, SDPQPBatchGroup
+from .batch import (BATCH_SMAX, ConeLPBatchGroup, GPBatchGroup, QCQPBatchGroup, QPBatchGroup, SDPBatchGroup,
+                    SDPQPBatchGroup)
 
 
 def _typed(named):
@@ -135,6 +138,28 @@ def _check_cone(P, q, G, h, dims, A, b):
         raise TypeError("dims has %d rows ('l' + sum 'q' + sum 's'²), G and h have %d" % (cdim, m))
     _on_device(named)
     return B, n, m, p
+
+
+def _check_gp(K, F, g, G, h, A, b):
+    """gp_layer's _check, K with gp_batch's message: every refusal before any device work.  Returns B, n, ml, p"""
+    if type(K) is not list or not K or [k for k in K if type(k) is not int or k <= 0]:
+        raise TypeError("'K' must be a list of positive integers")
+    if (A is None) != (b is None):
+        raise TypeError("'A' and 'b' must be given together")
+    if (G is None) != (h is None):
+        raise TypeError("'G' and 'h' must be given together")
+    named = [("F", F), ("g", g)] + ([("G", G), ("h", h)] if G is not None else []) + \
+        ([("A", A), ("b", b)] if A is not None else [])
+    _typed(named)
+    S = sum(K)
+    if F.dim() != 3 or F.shape[1] != S or F.shape[0] < 1 or F.shape[2] < 1:
+        raise TypeError("F must have shape (B, %d, n) with B and n positive (sum K = %d rows)" % (S, S))
+    B, n = F.shape[0], F.shape[2]
+    if tuple(g.shape) != (B, S):
+        raise TypeError("g must have shape (%d, %d)" % (B, S))
+    ml, p = _constraint_rows(B, n, G, h, A, b)
+    _on_device(named)
+    return B, n, ml, p
 
 
 def _rows(t, it):
@@ -359,6 +384,62 @@ class _QCQPLayer(torch.autograd.Function):
         return (*res, None, None, None)
 
 
+class _GPLayer(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, K, F, g, G, h, A, b, nsub, options):
+        B, n, ml, p = _check_gp(K, F, g, G, h, A, b)
+        mnl = len(K) - 1
+        ctx.shapes = B, n, sum(K), mnl, ml, p
+        dev = F.device
+        # the layouts the library loads: F, G and A column-major per problem
+        data = {"F": F.transpose(1, 2).contiguous(), "g": g.contiguous()}
+        if ml:
+            data.update(G=G.transpose(1, 2).contiguous(), h=h.contiguous())
+        if p:
+            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
+        grp = GPBatchGroup(B, n, K, ml, p, dev.index if dev.index is not None else torch.cuda.current_device(), nsub)
+        try:
+            its, x, _, z, y, status = _solve(
+                grp, data, lambda part, a: part.load_ptr(a["F"], a["g"], a.get("G"), a.get("h"), _lib.DEVICE,
+                                                         a.get("A"), a.get("b")),
+                options, dev, (n, mnl + ml, p))
+        except BaseException:
+            grp.close()
+            raise
+        _keep(ctx, grp, its, ctx.needs_input_grad[1:7])
+        return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gx, gy, gznl, gzl, _gstatus):
+        B, n, S, mnl, ml, p = ctx.shapes
+        m = mnl + ml
+        need = dict(zip(("F", "g", "G", "h", "A", "b"), ctx.needs_input_grad[1:7]))
+        dev = next(t.device for t in (gx, gy, gznl, gzl) if t is not None)
+        f64 = dict(dtype=torch.float64, device=dev)
+        gz = None
+        if m and (gznl is not None or gzl is not None):
+            gz = torch.cat([torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml))], 1)
+        # C's outputs uy, uz (h: its 'l' rows), dF, dg, dG, dA in problem order; dF, dG, dA column-major
+        shapes = {"b": (p,), "h": (m,), "F": (n, S), "g": (S,), "G": (n, ml), "A": (n, p)}
+        shapes = {k: s for k, s in shapes.items() if need[k] and (ml or k not in ("G", "h")) and
+                  (p or k not in ("A", "b"))}
+        out = _adjoint(ctx, (gx, gy if p else None, gz), shapes,
+                       lambda part, g, o: part.adjoint_gp_ptr(*g, None, *(o.get(k) for k in
+                                                                          ("b", "h", "F", "g", "G", "A")),
+                                                              space=_lib.DEVICE), dev)
+        view = {"F": lambda t: t.transpose(1, 2), "h": lambda t: t[:, mnl:], "G": lambda t: t.transpose(1, 2),
+                "A": lambda t: t.transpose(1, 2)}
+        empty = {"G": (B, 0, n), "h": (B, 0), "A": (B, 0, n), "b": (B, 0)}
+        res = []
+        for key in ("F", "g", "G", "h", "A", "b"):
+            if key in out:
+                res.append(view.get(key, lambda t: t)(out[key]))
+            else:
+                res.append(torch.zeros(empty[key], **f64) if need[key] else None)
+        return (None, *res, None, None)
+
+
 def qp_layer(P, q, G, h, A=None, b=None, nsub=None, **options):
     """Solve B dense QPs  minimize 1/2 x'P x + q'x  s.t.  G x <= h,  A x = b  on the GPU, differentiably.
 
@@ -422,3 +503,27 @@ def conelp_layer(c, G, h, dims, A=None, b=None, nsub=None, **options):
     found infeasible (status 4 or 5) gets NaN gradients like any status other than 1.  Backward returns dL/dc, dL/dG,
     dL/dh, dL/dA and dL/db with coneqp_layer's conventions."""
     return _ConeLayer.apply(None, c, G, h, A, b, dims, nsub, dict(options))
+
+
+def gp_layer(K, F, g, G=None, h=None, A=None, b=None, nsub=None, **options):
+    """Solve B geometric programs in log form  minimize lse(F_0 x + g_0)  s.t.  lse(F_i x + g_i) <= 0 (i = 1..mnl),
+    G x <= h,  A x = b,  lse(u) = log sum exp(u),  on the GPU, differentiably (gp_batch's algorithm: solvers.gp's).
+
+    K: the block sizes of F shared by every problem, a list of mnl + 1 positive ints.  F (B, sum K, n), g (B, sum K),
+    G (B, ml, n), h (B, ml), A (B, p, n), b (B, p): CUDA float64 tensors on one device; G and h, A and b are optional
+    and given in pairs.  Returns (x, y, znl, zl, status_code): x (B, n), the multipliers y (B, p) of A x = b, znl
+    (B, mnl) of the posynomial constraints and zl (B, ml) of G x <= h, and the int32 status per problem (1 optimal).
+    nsub: sub-batches solved concurrently, as qp_batch's.  options: maxiters, abstol, reltol, feastol, refinement.
+    Shape, dtype, device and K errors are TypeErrors raised before any device work.
+
+    A log-log convex layer: a posynomial sum_k c_k prod_j u_j^F_kj with coefficients c > 0 in the variables u = exp(x)
+    is lse(F x + log c), so the coefficients enter as g = torch.log(c) and autograd carries the gradient on to c:
+
+        x, y, znl, zl, status = gp_layer(K, F, torch.log(c), G, h)
+        u = torch.exp(x)
+
+    Backward (once: no double backward) returns dL/dF, dL/dg, dL/dG, dL/dh, dL/dA and dL/db from the gradients of x,
+    y, znl and zl (cvxb_batch_adjoint_gp), with NaN for problems whose status is not 1; K gets none.  Inputs that need
+    no gradient get none and cost nothing.  The solved batch is kept on the device from forward to backward, and
+    freed by backward."""
+    return _GPLayer.apply(K, F, g, G, h, A, b, nsub, dict(options))

@@ -588,6 +588,31 @@ int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, c
  * CVXB_DEVICE allocates nothing; CVXB_HOST stages as cvxb_batch_adjoint does. */
 int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
                             double *uy, double *uz, double *dP, double *dG, double *dA, int space);
+/* Derivatives of a GP batch's last solve, cvxb_batch_adjoint_qcqp's counterpart, for a loss L with gradients gx =
+ * dL/dx (nprob x n), gy = dL/dy (nprob x p) and gz = dL/dz (nprob x m, m = mnl + ml, laid out as the results' [znl;
+ * zl]).  At the returned iterate, with the objective's multiplier z0 = 1, pi_i = softmax(Fi x + gi), Sigma_i =
+ * diag(pi_i) - pi_i pi_i', H = sum_{i=0..mnl} z_i Fi' Sigma_i Fi, Df the mnl x n matrix of rows pi_i' Fi (i = 1..mnl)
+ * and D = diag(s / z), it solves
+ *     [H A' Df' G'; A 0 0 0; Df 0 -Dnl 0; G 0 0 -Dl] [ux; uy; uznl; uzl] = [gx; gy; gznl; gzl]
+ * with one more factorisation of the reduced KKT matrix (S + A'A where S is singular there, as kkt_chol2 does) and one
+ * step of iterative refinement on the full system, and writes ux (nprob x n), uy (nprob x p), uz = [uznl; uzl]
+ * (nprob x m) and the gradients dL/d(input), with w_i = Fi ux, v_i = pi_i o (w_i - pi_i'w_i) and uz_0 = 0:
+ *     dg: nprob x S (S = sum K), block i -(z_i v_i + uz_i pi_i);
+ *     dF: per problem S x n column-major, ld S, as cvxb_batch_load_gp's F: block i dg_i x' - z_i pi_i ux';
+ *     dG = -(zl ux' + uzl x')  (ml x n column-major per problem, the 'l' rows only),
+ *     dA = -(y ux' + uy x')    (p x n column-major per problem);
+ * dL/dh = uzl and dL/db = uy.  A monomial block (K_i = 1) gets exactly the QP adjoint's dG and dh of the row Fi x <= -gi.
+ * Every array is in the caller's problem order and in `space`.  A NULL input is zero; a NULL output is not written and
+ * its work is skipped: without dF, dg, dG and dA no gradient kernel runs.  A problem whose status is not 1 (optimal;
+ * status 3 from a line-search step that underflowed included), or whose KKT matrix has no Cholesky factor at that
+ * iterate, gets NaN in all its outputs.  The outputs are a function of the results and the data; cvxb_batch_results is
+ * unchanged afterwards and a re-solve computes the same results.  GP batches only (cvxb_batch_create_gp): any other
+ * batch is CVXB_E_UNSUP, and cvxb_batch_adjoint, _qcqp and _cone refuse a GP batch.  A batch without a completed
+ * cvxb_batch_solve since its last cvxb_batch_load_gp or cvxb_batch_load_eq is CVXB_E_ARG.  CVXB_DEVICE allocates
+ * nothing; CVXB_HOST stages each given array in temporary device memory, at most nprob * (2 (n + p + m) + S n + S +
+ * ml n + p n) doubles in all. */
+int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                          double *uz, double *dF, double *dg, double *dG, double *dA, int space);
 
 #ifdef __cplusplus
 }
