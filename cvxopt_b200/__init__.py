@@ -24,13 +24,13 @@ __all__ = ["kkt_chol", "kkt_chol2", "kkt_ldl2", "kkt_qr", "KKTChol", "cp_kktsolv
            "CPLBatch", "CPLBatchGroup", "cpl_batch",
            "SDPCPLBatch", "SDPCPLBatchGroup", "sdp_cpl_batch",
            "QCQPBatch", "QCQPBatchGroup", "qcqp_batch", "qp_layer", "qcqp_layer",
-           "coneqp_layer", "conelp_layer", "gp_layer",
+           "coneqp_layer", "conelp_layer", "gp_layer", "cp_layer", "cpl_layer",
            "device_count", "launch_count"]
 
 
 def __getattr__(name):
     # the layers import torch, which `import cvxopt_b200` does not need otherwise
-    if name in ("qp_layer", "qcqp_layer", "coneqp_layer", "conelp_layer", "gp_layer"):
+    if name in ("qp_layer", "qcqp_layer", "coneqp_layer", "conelp_layer", "gp_layer", "cp_layer", "cpl_layer"):
         from . import layer
         return getattr(layer, name)
     raise AttributeError("module 'cvxopt_b200' has no attribute %r" % name)

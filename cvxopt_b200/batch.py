@@ -171,6 +171,8 @@ ADJOINT_KEYS = ("P", "q", "G", "h", "A", "b")
 QCQP_ADJOINT_KEYS = ("P", "q", "r", "G", "h", "A", "b")
 CONELP_ADJOINT_KEYS = ("c", "G", "h", "A", "b")
 GP_ADJOINT_KEYS = ("F", "g", "G", "h", "A", "b")
+CP_ADJOINT_KEYS = ("ux", "uznl", "G", "h", "A", "b")
+CPL_ADJOINT_KEYS = CP_ADJOINT_KEYS + ("c",)
 
 
 def _adjoint_args(gx, gy, gz, want, B, n, p, m, keys=ADJOINT_KEYS):
@@ -907,9 +909,51 @@ class CPBatch(QPBatch):
             raise TypeError("problem shapes do not match the batch")
         Acm, bv = self._host_eq(A, b)
         Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
-        _lib.check(self._lib.cvxb_batch_load_cp(self._h, x0.ctypes.data, Gcm.ctypes.data if self.ml else None,
-                                                h.ctypes.data if self.ml else None, _lib.HOST), "batch_load_cp")
-        self._load_eq(Acm, bv, _lib.HOST)
+        self.load_ptr(x0.ctypes.data, Gcm.ctypes.data if self.ml else None, h.ctypes.data if self.ml else None,
+                      _lib.HOST, Acm, bv)
+
+    def load_ptr(self, x0, G, h, space=_lib.DEVICE, A=None, b=None):
+        """cvxb_batch_load_cp on raw addresses in `space` (device-resident callers): x0, G ml x n column-major and h
+        (None when ml = 0); A p x n column-major and b"""
+        _lib.check(self._lib.cvxb_batch_load_cp(self._h, x0, G, h, space), "batch_load_cp")
+        self._load_eq(A, b, space)
+
+    _cp_keys = CP_ADJOINT_KEYS           # the keys adjoint_cp takes in `want` (a cpl batch's add c)
+
+    def adjoint_cp(self, gx, gy=None, gz=None, want=None):
+        """derivatives of the last solve's results for a loss L with gradients gx = dL/dx (B, n), gy = dL/dy (B, p)
+        and gz = dL/dz (B, mnl + ml, laid out as [znl, zl]), None meaning zero (cvxb_batch_adjoint_cp).  F is called
+        once more, at the returned x.  Returns host arrays for the keys in `want` (None: all of them): the adjoint
+        solution's ux (B, n) and uznl (B, mnl), which give a parameter t of F its dL/dt = -d_t[ux' Df' zk + uk' f]
+        (zk = [1; znl] and uk = [0; uznl] here, znl and uznl on a cpl batch), and dL/d(input) in load()'s layout:
+        G (B, ml, n), h (B, ml), A (B, p, n), b (B, p) and, on a cpl batch, c (B, n).  A problem whose status is not
+        'optimal', or whose F(x, z) there is not finite, gets NaN.  An exception raised in F comes out unchanged; a
+        batch not solved since its last load raises ValueError, and a QCQP batch NotImplementedError."""
+        B, n, m, p, mnl, ml = self.B, self.n, self.m, self.p, self.mnl, self.ml
+        keys = self._cp_keys
+        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, B, n, p, m, keys)
+        # C's outputs ux, uy, uz (uznl and h: its rows), dG, dA; dG and dA column-major per problem
+        ux = np.empty((B, n)) if {"ux", "c"} & set(want) else None
+        uz = np.empty((B, m)) if {"uznl", "h"} & set(want) else None
+        bufs = {k: np.empty(s) for k, s in (("b", (B, p)), ("G", (B, n, ml)), ("A", (B, n, p))) if k in want}
+        ptrs = [None if a is None else a.ctypes.data for a in gs + [ux, bufs.get("b"), uz, bufs.get("G"),
+                                                                    bufs.get("A")]]
+        self.adjoint_cp_ptr(*ptrs, space=_lib.HOST)
+        got = {"ux": ux, "c": None if ux is None else -ux, "uznl": None if uz is None else uz[:, :mnl],
+               "h": None if uz is None else uz[:, mnl:], "b": bufs.get("b")}
+        got.update({k: np.ascontiguousarray(bufs[k].transpose(0, 2, 1)) for k in ("G", "A") if k in bufs})
+        return {k: np.ascontiguousarray(got[k]) for k in want}
+
+    def adjoint_cp_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dG=None, dA=None,
+                       space=_lib.DEVICE):
+        """cvxb_batch_adjoint_cp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL.
+        An exception raised in F comes out unchanged, as from solve()"""
+        self._err = None
+        rc = self._lib.cvxb_batch_adjoint_cp(self._h, gx, gy, gz, ux, uy, uz, dG, dA, space)
+        err, self._err = self._err, None
+        if err is not None:
+            raise err
+        _lib.check(rc, "batch_adjoint_cp")
 
     def set_F(self, F):
         """F(x, idx=idx) -> (f, Df) and F(x, z, idx=idx) -> (f, Df, H), as cp_batch takes it.  The callback runs F on
@@ -1006,6 +1050,17 @@ class CPBatchGroup(QPBatchGroup):
 
     def load(self, x0, G, h, A=None, b=None):
         self._load_sliced((x0, G, h), A, b)
+
+    def adjoint_cp(self, gx, gy=None, gz=None, want=None):
+        """CPBatch.adjoint_cp on every part with its slice of the gradients, the results in problem order"""
+        keys = self.parts[0]._cp_keys
+        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, self.B, self.n, self.p, self.m, keys)
+        out = {}
+        for ix, part in zip(self.idx, self.parts):
+            r = part.adjoint_cp(*(None if a is None else a[ix] for a in gs), want=want)
+            for k, v in r.items():
+                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
+        return out
 
     def stats(self):
         out = super().stats()
@@ -1237,10 +1292,16 @@ class CPLBatch(CPBatch):
             raise TypeError("problem shapes do not match the batch")
         Acm, bv = self._host_eq(A, b)
         Gcm = np.ascontiguousarray(np.transpose(G, (0, 2, 1)))
-        _lib.check(self._lib.cvxb_batch_load_cpl(self._h, c.ctypes.data, x0.ctypes.data,
-                                                 Gcm.ctypes.data if cd else None, h.ctypes.data if cd else None,
-                                                 _lib.HOST), "batch_load_cpl")
-        self._load_eq(Acm, bv, _lib.HOST)
+        self.load_ptr(c.ctypes.data, x0.ctypes.data, Gcm.ctypes.data if cd else None, h.ctypes.data if cd else None,
+                      _lib.HOST, Acm, bv)
+
+    def load_ptr(self, c, x0, G, h, space=_lib.DEVICE, A=None, b=None):
+        """cvxb_batch_load_cpl on raw addresses in `space` (device-resident callers): c, x0, G cdim x n column-major
+        and h (None when cdim = 0); A p x n column-major and b"""
+        _lib.check(self._lib.cvxb_batch_load_cpl(self._h, c, x0, G, h, space), "batch_load_cpl")
+        self._load_eq(A, b, space)
+
+    _cp_keys = CPL_ADJOINT_KEYS
 
 
 class CPLBatchGroup(CPBatchGroup):

@@ -1952,24 +1952,27 @@ template <bool EPI = true> __global__ void k_cp_zpack(Ptrs p, GPPtrs g, CPPtrs c
 // Df[0] into gf0, Df[1:] into G's rows [0, mnl) and H's lower triangle into P's, by 32 x 32 tiles through shared
 // memory (H row-major, P column-major).  Trial, only the problems still searching: newrx's nonlinear part
 // Df'[nz0; nz[:mnl]] into nrx (the GEMVs add G'newzl + A'newy).  EPI false (a cpl batch): Df is Df[:mnl], all of it
-// goes into G, and newrx starts from c.  256 threads
-template <bool FULL, bool EPI = true> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GPPtrs g, CPPtrs c) {
+// goes into G, and newrx starts from c.  256 threads.
+// ADJ (k_adj_cp_take, FULL): every slot, done or not; neither fv nor gf0, which the adjoint does not read; and
+// flag[b] := 1 when f, Df or H's lower triangle has a non-finite entry, else 0
+template <bool FULL, bool EPI, bool ADJ>
+__device__ __forceinline__ void cp_take_body(const Ptrs &p, const GPPtrs &g, const CPPtrs &c, int *flag) {
     GP_SETUP
-    if (S.done || (!FULL && T.searching == 0.0)) return;
+    if (!ADJ && (S.done || (!FULL && T.searching == 0.0))) return;
     const int n = p.n, nK = g.nK;
     const double *f = c.f + (long long)b * nK, *Df = c.Df + (long long)b * nK * n;
-    for (int i = tid; i < nK; i += nt) g.fv[(long long)b * nK + i] = f[i];
+    if (!ADJ) for (int i = tid; i < nK; i += nt) g.fv[(long long)b * nK + i] = f[i];
     if (!FULL) {
         for (int j = tid; j < n; j += nt)
             g.nrx[on + j] = EPI ? cp_dfz(Df, n, nK, T.nz0, g.nz + om, j) : cpl_dfz(Df, n, nK, p.q[on + j], g.nz + om, j);
         return;
     }
-    if (tid == 0) {
+    if (!ADJ && tid == 0) {
         bool fin = true;
         for (int i = 0; i < nK; ++i) fin = fin && isfinite(f[i]);
         if (!fin) atomicMin(c.bad, c.idx[b]);
     }
-    if (EPI) for (int j = tid; j < n; j += nt) g.gf0[on + j] = Df[j];
+    if (EPI && !ADJ) for (int j = tid; j < n; j += nt) g.gf0[on + j] = Df[j];
     double *G = g.G + (long long)b * g.sG;
     for (long long e = tid; e < (long long)g.mnl * n; e += nt) {
         const long long i = e % g.mnl, j = e / g.mnl;
@@ -1992,6 +1995,17 @@ template <bool FULL, bool EPI = true> __global__ void __launch_bounds__(256) k_c
                 if (i < n && i >= j) P[i + (long long)j * c.ldp] = tile[tx][q];
             }
         }
+    if (ADJ) {                                         // f, Df and H's lower triangle, read again in one flat pass
+        bool fin = true;
+        for (int i = tid; i < nK; i += nt) fin = fin && isfinite(f[i]);
+        for (long long e = tid; e < (long long)nK * n; e += nt) fin = fin && isfinite(Df[e]);
+        for (long long e = tid; e < (long long)n * n; e += nt) fin = fin && (e % n > e / n || isfinite(H[e]));
+        const int bad = __syncthreads_or(!fin);
+        if (tid == 0) flag[b] = bad ? 1 : 0;
+    }
+}
+template <bool FULL, bool EPI = true> __global__ void __launch_bounds__(256) k_cp_take(Ptrs p, GPPtrs g, CPPtrs c) {
+    cp_take_body<FULL, EPI, false>(p, g, c, nullptr);
 }
 // rx += Df'[z0; z[:mnl]] (EPI false: Df'z[:mnl]) at the iterates, from the callback's Df (after k_gp_res_begin; the
 // GEMVs add G'zl + A'y)
@@ -2409,6 +2423,30 @@ __global__ void __launch_bounds__(256) k_adj_gp_grad(Ptrs p, GPPtrs g, double *d
                             [&](int i, int c) { return -(z[g.mnl + i] * uxs[c] + uz[g.mnl + i] * xs[c]); });
     if (dA && pq) adj_store(dA + (k * n + j0) * pq, pq, nj, bad,
                             [&](int i, int c) { return -(y[i] * uxs[c] + uy[i] * xs[c]); });
+}
+
+// ---- the adjoint of a CP or cpl batch's solution (cvxb_batch_adjoint_cp) ----
+// The QCQP's derivation with the caller's f: at the returned iterate, with zk = [1; znl] (cp's epigraph problem) or
+// zk = znl (cpl), the KKT matrix has H = sum_i zk_i grad² f_i and Df's rows grad f_i' (i = 1..mnl), both from one call
+// of the caller's F(x, zk); a cpl batch's cone rows get the cone adjoint's W'W.  For a parameter t of F, dL/dt =
+// -d_t[ux' Df' zk + uk' f] with uk = [0; uznl] (cpl: uznl), which the caller forms from ux and uz; the library writes
+// ux, uy, uz, dG and dA (k_adj_qc_grad without its P_i outputs).
+// The z of that call on every slot (k_cp_zpack skips done slots, and after a solve every slot is done)
+__global__ void k_adj_cp_zpack(Ptrs p, GPPtrs g, CPPtrs c, int epi) {
+    const long long b = blockIdx.x;
+    const double *z = p.z + b * p.m;
+    double *zc = c.z + b * g.nK;
+    for (int i = threadIdx.x; i < g.nK; i += blockDim.x) zc[i] = epi ? (i == 0 ? 1.0 : z[i - 1]) : z[i];
+}
+// the operator at x once the callback has run: Df into G's rows [0, mnl), H's lower triangle into P and each slot's
+// non-finite flag into flag (cp_take_body<true, EPI, true>)
+template <bool EPI> __global__ void __launch_bounds__(256) k_adj_cp_take(Ptrs p, GPPtrs g, CPPtrs c, int *flag) {
+    cp_take_body<true, EPI, true>(p, g, c, flag);
+}
+// after the adjoint's last factorisation: a slot whose F(x, zk) was not finite fails it, so adj_bad gives it NaN
+__global__ void k_adj_cp_flag(int *info, const int *flag, int B) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < B && flag[b]) info[b] = 1;
 }
 
 // the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
@@ -3083,11 +3121,11 @@ int qc_hessian(cvxb_batch *b) {
     return 0;
 }
 // the caller's F over the active slots at x (slot k at x + k*n); full: at the iterates, with z = [z0; z[:mnl]] and H
-int cp_call(cvxb_batch *b, const double *x, bool full) {
+int cp_call(cvxb_batch *b, const double *x, bool full, const char *fn = "batch_solve") {
     const CPPtrs &c = b->cq;
     const int rc = b->cfn(b->cctx, b->Bact, full ? 1 : 0, x, full ? c.z : nullptr, c.idx, c.f, c.Df,
                           full ? c.H : nullptr, (void *)b->st);
-    if (rc != 0) { set_error("batch_solve: the evaluation callback returned %d", rc); return CVXB_E_ARG; }
+    if (rc != 0) { set_error("%s: the evaluation callback returned %d", fn, rc); return CVXB_E_ARG; }
     return 0;
 }
 // F(x, z[:mnl]) at the iterates: f into fv, grad f0 into gf0, Df[1:] into G's rows [0, mnl); CP also H into P
@@ -3883,16 +3921,20 @@ int adj_switch(cvxb_batch *b, std::vector<double> &aw0) {
 // side, for a QC or GP batch its operator at x (H in P, Df in G's rows [0, mnl)), the reduced solve, one refinement
 // step on the full system, then ux, uy, uz and the gradients.  QC: dP is the (nK n) x n stack, dq nK x n, dr nK and dG
 // ml x n per problem.  GP: dF is S x n, dg S and dG ml x n per problem; the call overwrites P, G's Df rows, yv, wv, Hr,
-// hw and fv, all of which a solve rewrites before it reads them.  With 'q' cones or 's' blocks k_adj_cone and the 's'
-// kernels fix the cone rows between the 'l' steps; a cone LP has no P (its entry point refuses dP)
+// hw and fv, all of which a solve rewrites before it reads them.  CP and cpl: the caller's F(x, zk) once, through the
+// callback, on every slot in its caller-order index; dG is ml x n per problem (k_adj_qc_grad's), and the call
+// overwrites P, G's Df rows, the callback's buffers, cpi and d_done (each slot's non-finite flag).  With 'q' cones or
+// 's' blocks k_adj_cone and the 's' kernels fix the cone rows between the 'l' steps; a cone LP has no P (its entry
+// point refuses dP)
 int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                   double *uz, AdjGrads d, int space) {
     CVXB_CUDA(cudaSetDevice(b->device));
     cudaStream_t st = b->st;
     const bool qc = b->kind == Kind::QC, lp = b->kind == Kind::LP, gp = b->kind == Kind::GP;
+    const bool cp = b->calls_back(), epi = b->kind == Kind::CP;
     const bool cones = b->p.nq > 0 || b->p.ns > 0, sdp = b->p.ns > 0;
     const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = qc ? b->gq.nK : 1;
-    const size_t ml = qc || gp ? m - b->gq.mnl : m, S = gp ? b->gq.sumK : 0;
+    const size_t ml = qc || gp || cp ? m - b->gq.mnl : m, S = gp ? b->gq.sumK : 0;
     const Ptrs &p = b->p;
     const GPPtrs &g = b->gq;
     // host space: every given array staged on the device (inputs uploaded, outputs copied back); device: in place
@@ -3928,11 +3970,25 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
         k_adj_gp_op<<<dim3((unsigned)g.nK, (unsigned)B), 256, 0, st>>>(p, g); count_launch();
         CVXB_TRY(gp_hessian(b, true));
     }
+    if (cp) {                                            // F(x, zk): H, Df and the flags; P mirrored for the refinement
+        CVXB_TRY(cp_upload_idx(b));
+        k_adj_cp_zpack<<<(unsigned)B, 32, 0, st>>>(p, g, b->cq, epi ? 1 : 0); count_launch();
+        CVXB_TRY(cp_call(b, p.x, true, "batch_adjoint_cp"));
+        if (epi) k_adj_cp_take<true><<<(unsigned)B, 256, 0, st>>>(p, g, b->cq, b->d_done.p);
+        else k_adj_cp_take<false><<<(unsigned)B, 256, 0, st>>>(p, g, b->cq, b->d_done.p);
+        count_launch();
+        CVXB_TRY(symmetrize_lower(b->n, b->P.p, b->ldp, b->Bact, b->sP, st));
+    }
     CVXB_TRY(batch_factor(b));
     std::vector<double> aw0;                             // the solve's aw when adj_switch changed it
     const bool switched0 = b->switched;
-    // a GP whose terms are all monomials is an LP, and S can be singular at its vertices as at a cone LP's
-    if (pq && (lp || cones || gp)) CVXB_TRY(adj_switch(b, aw0));
+    // a GP whose terms are all monomials is an LP, and S can be singular at its vertices as at a cone LP's; so can a
+    // CP or cpl batch's, whose f the caller chooses
+    if (pq && (lp || cones || gp || cp)) CVXB_TRY(adj_switch(b, aw0));
+    if (cp) {
+        k_adj_cp_flag<<<(unsigned)((B + 255) / 256), 256, 0, st>>>(b->d_info.p, b->d_done.p, (int)B);
+        count_launch();
+    }
     CVXB_TRY(batch_solve(b, p.dx, n, p.dy, pq));
     // one step of iterative refinement on the full KKT system: W'W spans many orders of magnitude at a converged
     // iterate, and the reduced solve alone loses digits to it.  r = g - M u, then u += M^{-1} r with the same factor
@@ -3979,7 +4035,8 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
             count_launch();
         }
     } else if (s_dP.dev || s_dq.dev || s_dr.dev || s_dG.dev || s_dA.dev) {
-        if (qc) k_adj_qc_grad<<<grid, 256, 0, st>>>(p, b->gq, s_dP.dev, s_dq.dev, s_dr.dev, s_dG.dev, s_dA.dev,
+        // CP and cpl: dG over rows mnl.. and dA only, whose formulas are the QC batch's
+        if (qc || cp) k_adj_qc_grad<<<grid, 256, 0, st>>>(p, b->gq, s_dP.dev, s_dq.dev, s_dr.dev, s_dG.dev, s_dA.dev,
                                                     b->d_perm.p, b->d_info.p);
         else k_adj_grad<<<grid, 256, 0, st>>>(p, s_dP.dev, s_dG.dev, s_dA.dev, b->d_perm.p, b->d_info.p);
         count_launch();
@@ -4034,6 +4091,23 @@ int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, con
     }
     AdjGrads d;
     d.dF = dF; d.dg = dg; d.dG = dG; d.dA = dA;
+    return batch_adjoint(b, gx, gy, gz, ux, uy, uz, d, space);
+}
+
+int cvxb_batch_adjoint_cp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                          double *uz, double *dG, double *dA, int space) {
+    if (!b) { set_error("batch_adjoint_cp: batch is NULL"); return CVXB_E_ARG; }
+    if (!b->calls_back()) {
+        set_error("batch_adjoint_cp: only CP and cpl batches (cvxb_batch_create_cp, _cpl, _sdp_cpl) are "
+                  "differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (!b->solved) {
+        set_error("batch_adjoint_cp: no completed cvxb_batch_solve since the last load");
+        return CVXB_E_ARG;
+    }
+    AdjGrads d;
+    d.dG = dG; d.dA = dA;
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, d, space);
 }
 

@@ -7,20 +7,24 @@
         s in the cone of dims ('l', 'q', 's'),  A x = b;   conelp_layer(c, G, h, dims, A, b) the same with P = 0
     x, y, znl, zl, status = gp_layer(K, F, g, G, h, A, b)   solves   minimize lse(F_0 x + g_0)  s.t.
         lse(F_i x + g_i) <= 0 (i >= 1),  G x <= h,  A x = b   (a geometric program in log form)
+    x, y, znl, zl, status = cp_layer(F, params, G, h, A, b)   solves   minimize f_0(x)  s.t.  f_i(x) <= 0 (i >= 1),
+        G x <= h,  A x = b  with the caller's F(x; params);   cpl_layer(c, F, params, G, h, dims, A, b) minimises c'x
+        with 'l', 'q' and 's' cones
 
-for B problems at once with qp_batch's, qcqp_batch's and gp_batch's algorithms, and their backward runs the library's
-adjoint (cvxb_batch_adjoint, cvxb_batch_adjoint_qcqp, cvxb_batch_adjoint_cone, cvxb_batch_adjoint_gp): one more
-factorisation and solve of the KKT system at the returned iterate, then the gradients written by one kernel.  Nothing leaves the device.  The gradient of each P is the symmetric
-one (the solvers read only lower triangles), so a P built as S + S' or from an expanded tensor gets the right gradient
-from autograd.  A problem whose status is not optimal (status != 1) gets NaN gradients.
+for B problems at once with qp_batch's, qcqp_batch's, gp_batch's, cp_batch's and cpl_batch's algorithms, and their
+backward runs the library's adjoint (cvxb_batch_adjoint, _qcqp, _cone, _gp, _cp): one more factorisation and solve of
+the KKT system at the returned iterate, then the gradients written by one kernel.  Nothing leaves the device.  The
+gradient of each P is the symmetric one (the solvers read only lower triangles), so a P built as S + S' or from an
+expanded tensor gets the right gradient from autograd.  A problem whose status is not optimal (status != 1) gets NaN
+gradients.
 """
 import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .batch import (BATCH_SMAX, ConeLPBatchGroup, GPBatchGroup, QCQPBatchGroup, QPBatchGroup, SDPBatchGroup,
-                    SDPQPBatchGroup)
+from .batch import (BATCH_SMAX, ConeLPBatchGroup, CPBatchGroup, CPLBatchGroup, GPBatchGroup, QCQPBatchGroup,
+                    QPBatchGroup, SDPBatchGroup, SDPCPLBatchGroup, SDPQPBatchGroup)
 
 
 def _typed(named):
@@ -527,3 +531,208 @@ def gp_layer(K, F, g, G=None, h=None, A=None, b=None, nsub=None, **options):
     no gradient get none and cost nothing.  The solved batch is kept on the device from forward to backward, and
     freed by backward."""
     return _GPLayer.apply(K, F, g, G, h, A, b, nsub, dict(options))
+
+
+def _check_cp(F, params, c, G, h, dims, A, b, cpl):
+    """cp_layer's and cpl_layer's _check (cpl: c given, dims with 'l', 'q' and 's'), F() called once: every refusal
+    before any device work.  Returns B, n, mnl, ml, p, x0 (a contiguous float64 tensor on the inputs' device), the
+    dims the group takes (None: 'l' rows only) and params as a tuple"""
+    if not callable(F):
+        raise TypeError("F must be callable")
+    if not isinstance(params, (tuple, list)):
+        raise TypeError("params must be a tuple of tensors")
+    params = tuple(params)
+    if (A is None) != (b is None):
+        raise TypeError("'A' and 'b' must be given together")
+    if (G is None) != (h is None):
+        raise TypeError("'G' and 'h' must be given together")
+    named = ([("c", c)] if cpl else []) + ([("G", G), ("h", h)] if G is not None else []) + \
+        ([("A", A), ("b", b)] if A is not None else []) + [("params[%d]" % i, t) for i, t in enumerate(params)]
+    _typed(named)
+    try:
+        mnl, x0 = F()
+    except Exception:
+        raise ValueError("function call 'F()' failed") from None
+    if type(mnl) is not int or mnl < 0:
+        raise TypeError("the first output of F() must be a nonnegative integer")
+    if not isinstance(x0, torch.Tensor):
+        x0 = torch.as_tensor(np.asarray(x0))
+    if x0.dtype != torch.float64 or x0.dim() != 2 or x0.shape[0] < 1 or x0.shape[1] < 1:
+        raise TypeError("x0, F()'s second output, must be a float64 tensor of shape (B, n) with B and n positive")
+    B, n = x0.shape
+    if cpl and tuple(c.shape) != (B, n):
+        raise TypeError("c must have shape (%d, %d), as x0" % (B, n))
+    for name, t in named:
+        if name.startswith("params") and (t.dim() < 1 or t.shape[0] != B):
+            raise TypeError("%s must have leading dimension B = %d" % (name, B))
+    ml, p = _constraint_rows(B, n, G, h, A, b)
+    gdims = None
+    if not cpl:
+        _dims(dims, ml, "cp_layer")
+    else:
+        if dims is None:
+            dims = {"l": ml}
+        if not isinstance(dims, dict) or not set(dims) <= {"l", "q", "s"}:
+            raise TypeError("dims must be a dictionary with keys 'l', 'q' and 's'")
+        if int(dims.get("l", 0)) < 0 or any(int(k) < 1 for k in dims.get("q", [])) or \
+                any(not 0 <= int(k) <= BATCH_SMAX for k in dims.get("s", [])):
+            raise TypeError("dims: 'l' must be nonnegative, each 'q' size at least 1, each 's' order in 0..%d"
+                            % BATCH_SMAX)
+        gdims = {"l": int(dims.get("l", 0)), "q": [int(k) for k in dims.get("q", [])],
+                 "s": [int(k) for k in dims.get("s", [])]}
+        cdim = gdims["l"] + sum(gdims["q"]) + sum(k * k for k in gdims["s"])
+        if cdim != ml:
+            raise TypeError("dims has %d rows ('l' + sum 'q' + sum 's'²), G and h have %d" % (cdim, ml))
+    if p > n:
+        raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
+    if cpl and mnl + ml == 0:
+        raise ValueError("cpl needs at least one constraint row (mnl + cdim = 0): its merit weight 1 / gap is undefined")
+    if named:
+        _on_device(named)
+    dev = named[0][1].device if named else x0.device
+    if dev.type != "cuda":
+        raise TypeError("x0 must be a CUDA tensor when no other tensor is given")
+    return B, n, mnl, ml, p, x0.to(dev).contiguous(), gdims, params
+
+
+class _CPLayer(torch.autograd.Function):
+    # inputs: F, c (None: cp_layer), G, h, A, b, the checked shapes and dims, nsub, options, then the params one by one
+    @staticmethod
+    def forward(ctx, F, c, G, h, A, b, info, nsub, options, *params):
+        B, n, mnl, ml, p, x0, dims = info
+        cpl = c is not None
+        dev = x0.device
+        device = dev.index if dev.index is not None else torch.cuda.current_device()
+        ctx.shapes = B, n, mnl, ml, p, cpl
+        # F sees the params detached; the data in the layouts the library loads: G and A column-major per problem
+        det = tuple(t.detach() for t in params)
+
+        def Fd(x=None, z=None, idx=None):
+            return F(x, idx=idx, params=det) if z is None else F(x, z, idx=idx, params=det)
+        data = {"x0": x0}
+        if cpl:
+            data["c"] = c.contiguous()
+        if ml:
+            data.update(G=G.transpose(1, 2).contiguous(), h=h.contiguous())
+        if p:
+            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
+        if not cpl:
+            grp = CPBatchGroup(B, n, mnl, ml, p, device, nsub)
+            load = lambda part, a: part.load_ptr(a["x0"], a.get("G"), a.get("h"), _lib.DEVICE,  # noqa: E731
+                                                 a.get("A"), a.get("b"))
+        else:
+            grp = (SDPCPLBatchGroup if dims["s"] else CPLBatchGroup)(B, n, mnl, dims, p, device, nsub)
+            load = lambda part, a: part.load_ptr(a["c"], a["x0"], a.get("G"), a.get("h"), _lib.DEVICE,  # noqa: E731
+                                                 a.get("A"), a.get("b"))
+        try:
+            grp.set_F(Fd)
+            its, x, _, z, y, status = _solve(grp, data, load, options, dev, (n, mnl + ml, p))
+        except BaseException:
+            grp.close()
+            raise
+        needs = ctx.needs_input_grad
+        _keep(ctx, grp, its, needs[1:6] + needs[9:])
+        if any(needs[9:]):                   # the theta call's point and multipliers, and the detached params
+            ctx.F, ctx.params, ctx.x, ctx.znl = F, det, x.clone(), z[:, :mnl].clone()
+        return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gx, gy, gznl, gzl, _gstatus):
+        B, n, mnl, ml, p, cpl = ctx.shapes
+        m = mnl + ml
+        needs = ctx.needs_input_grad
+        need = dict(zip(("c", "G", "h", "A", "b"), needs[1:6]))
+        needp = needs[9:]
+        theta = any(needp)
+        dev = next(t.device for t in (gx, gy, gznl, gzl) if t is not None)
+        f64 = dict(dtype=torch.float64, device=dev)
+        gz = None
+        if m and (gznl is not None or gzl is not None):
+            gz = torch.cat([torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml))], 1)
+        # C's outputs ux, uy, uz ([uznl; h]), dG, dA in problem order; dG and dA column-major
+        shapes = {"ux": (n,) if need["c"] or theta else None, "b": (p,) if need["b"] and p else None,
+                  "uz": (m,) if m and ((need["h"] and ml) or (theta and mnl)) else None,
+                  "G": (n, ml) if need["G"] and ml else None, "A": (n, p) if need["A"] and p else None}
+        shapes = {k: s for k, s in shapes.items() if s is not None}
+        out = _adjoint(ctx, (gx, gy if p else None, gz), shapes,
+                       lambda part, g, o: part.adjoint_cp_ptr(*g, *(o.get(k) for k in ("ux", "b", "uz", "G", "A")),
+                                                              space=_lib.DEVICE), dev)
+        res = {"c": -out["ux"] if need["c"] else None}
+        for key, full, view in (("G", (B, ml, n), lambda t: t.transpose(1, 2)), ("h", (B, ml), lambda t: t[:, mnl:]),
+                                ("A", (B, p, n), lambda t: t.transpose(1, 2)), ("b", (B, p), lambda t: t)):
+            src = out.get("uz" if key == "h" else key)
+            res[key] = None if not need[key] else view(src) if src is not None else torch.zeros(full, **f64)
+        dparams = [None] * len(needp)
+        if theta:
+            dparams = _theta_grads(ctx, out["ux"], out["uz"][:, :mnl] if mnl else torch.zeros((B, 0), **f64),
+                                   cpl, needp)
+        return (None, res["c"], res["G"], res["h"], res["A"], res["b"], None, None, None, *dparams)
+
+
+def _theta_grads(ctx, ux, uznl, cpl, needp):
+    """dL/dtheta = -d_theta[ux' Df(x; theta)' zk + uk' f(x; theta)] for the params that need it (zk = [1; znl], uk =
+    [0; uznl]; cpl: znl and uznl), from one call F(x, idx=arange(B), params=...) with those params as fresh leaves"""
+    x, znl = ctx.x, ctx.znl
+    B = x.shape[0]
+    if cpl:
+        zk, uk = znl, uznl
+    else:
+        zk = torch.cat([torch.ones((B, 1), dtype=x.dtype, device=x.device), znl], 1)
+        uk = torch.cat([torch.zeros((B, 1), dtype=x.dtype, device=x.device), uznl], 1)
+    with torch.enable_grad():
+        leaves = tuple(t.detach().requires_grad_(nd) for t, nd in zip(ctx.params, needp))
+        f, Df = ctx.F(x, idx=torch.arange(B, device=x.device), params=leaves)[:2]
+        phi = (Df * (zk[:, :, None] * ux[:, None, :])).sum() + (uk * f).sum()
+        wrt = [t for t, nd in zip(leaves, needp) if nd]
+        # phi depends on none of them when F uses none of the params that need a gradient, or when f and Df are
+        # empty (a cpl problem with mnl = 0): every such param gets zeros
+        got = iter(torch.autograd.grad(phi, wrt, allow_unused=True) if phi.requires_grad else [None] * len(wrt))
+    out = []
+    for t, nd in zip(leaves, needp):
+        if not nd:
+            out.append(None)
+            continue
+        g = next(got)
+        out.append(torch.zeros_like(t) if g is None else -g)
+    return out
+
+
+def cp_layer(F, params=(), G=None, h=None, A=None, b=None, nsub=None, **options):
+    """Solve B smooth convex programs  minimize f_0(x; theta)  s.t.  f_i(x; theta) <= 0 (i = 1..mnl),  G x <= h,
+    A x = b  on the GPU, differentiably (cp_batch's algorithm: solvers.cp's), with f written by the caller in torch.
+
+    F is cp_batch's F with one more keyword, the parameters theta:
+      F() -> (mnl, x0): mnl shared by the batch, x0 (B, n) float64 strictly inside dom f; no gradient reaches x0;
+      F(x, idx=idx, params=params) -> (f, Df): f (k, mnl + 1), Df (k, mnl + 1, n) at the k points x of the problems
+          idx (int64 indices into the batch);
+      F(x, z, idx=idx, params=params) -> (f, Df, H): also H (k, n, n) = sum_i z_i grad² f_i(x), lower triangle read.
+    params: a tuple of CUDA float64 tensors with leading dimension B, which F indexes with idx.  G (B, ml, n),
+    h (B, ml), A (B, p, n), b (B, p): CUDA float64 tensors on the params' device, optional and given in pairs.
+    Returns (x, y, znl, zl, status_code) as qcqp_layer.  nsub: sub-batches solved concurrently, as qp_batch's.
+    options: maxiters, abstol, reltol, feastol, refinement, and dims ({'l': ml} only: 'q' and 's' cones raise
+    NotImplementedError).  Shape, dtype and device errors are TypeErrors raised before any device work.
+
+    Backward (once: no double backward) runs cvxb_batch_adjoint_cp, which calls F(x, z) once more per sub-batch, and
+    returns dL/dG, dL/dh, dL/dA, dL/db and, for a param that needs one, dL/dparam = -d_param[ux' Df' zk + uk' f] with
+    zk = [1; znl] and uk = [0; uznl], from one more call F(x, idx=arange(B), params=...) under autograd; a param F does
+    not use gets zeros.  Problems whose status is not 1 get NaN.  Inputs that need no gradient get none and cost
+    nothing: without a param that needs one, F is not called for theta.  The solved batch is kept on the device from
+    forward to backward, and freed by backward.  F must return the same values for the same point; it runs on the
+    library's stream and may see its rows in any order."""
+    dims = options.pop("dims", None)
+    B, n, mnl, ml, p, x0, _, params = _check_cp(F, params, None, G, h, dims, A, b, False)
+    return _CPLayer.apply(F, None, G, h, A, b, (B, n, mnl, ml, p, x0, None), nsub, dict(options), *params)
+
+
+def cpl_layer(c, F, params=(), G=None, h=None, dims=None, A=None, b=None, nsub=None, **options):
+    """Solve B convex problems  minimize c'x  s.t.  f_i(x; theta) <= 0 (i = 1..mnl),  G x + s = h,  s in C,  A x = b
+    on the GPU, differentiably (cpl_batch's algorithm, sdp_cpl_batch's with 's' blocks: solvers.cpl's).
+
+    F is cp_layer's without the objective row: f (k, mnl), Df (k, mnl, n), z (k, mnl).  c (B, n); G and h with dims
+    {'l': ml, 'q': [...], 's': [...]} as coneqp_layer's ('s' orders at most 32, each block unpacked column-major, only
+    its lower triangle read); dims None is {'l': rows of G}.  Returns (x, y, znl, zl, status_code), zl laid out as h
+    with symmetric 's' blocks.  Backward returns dL/dc = -ux, dL/dG, dL/dh, dL/dA, dL/db with coneqp_layer's 's'
+    conventions, and dL/dparam as cp_layer's with zk = znl and uk = uznl.  The rest is cp_layer's."""
+    B, n, mnl, ml, p, x0, gdims, params = _check_cp(F, params, c, G, h, dims, A, b, True)
+    return _CPLayer.apply(F, c, G, h, A, b, (B, n, mnl, ml, p, x0, gdims), nsub, dict(options), *params)

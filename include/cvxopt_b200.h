@@ -613,6 +613,34 @@ int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, c
  * ml n + p n) doubles in all. */
 int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                           double *uz, double *dF, double *dg, double *dG, double *dA, int space);
+/* Derivatives of a CP or cpl batch's last solve (cvxb_batch_create_cp, _cpl and _sdp_cpl: 'l', 'q' and 's' rows), for
+ * a loss L with gradients gx = dL/dx (nprob x n), gy = dL/dy (nprob x p) and gz = dL/dz (nprob x m, m = mnl + ml,
+ * laid out as the results' [znl; zl]).  At the returned iterate, with zk = [1; znl] for a CP batch (the objective's
+ * multiplier z0 = 1, as the QCQP adjoint takes it) and zk = znl for a cpl batch, the batch's callback is called once
+ * more, F(x, zk) on every problem, and gives H = sum_i zk_i grad² f_i and Df, the mnl x n matrix of rows grad f_i'
+ * (i = 1..mnl).  With D = diag(s / z) on the nonlinear and 'l' rows and W'W the NT scaling of the returned s and z on
+ * the 'q' and 's' rows (cvxb_batch_adjoint_cone's), it solves
+ *     [H A' Df' G'; A 0 0 0; Df 0 -Dnl 0; G 0 0 -W'W] [ux; uy; uznl; uzl] = [gx; gy; gznl; gzl]
+ * with one more factorisation of the reduced KKT matrix (S + A'A where S is singular there, as kkt_chol2 does) and one
+ * step of iterative refinement on the full system, and writes ux (nprob x n), uy (nprob x p), uz = [uznl; uzl]
+ * (nprob x m) and
+ *     dG = -(zl ux' + uzl x')  (ml x n column-major per problem, the rows of G only),
+ *     dA = -(y ux' + uy x')    (p x n column-major per problem);
+ * dL/dh = uzl, dL/db = uy and, for a cpl batch, dL/dc = -ux.  An 's' block follows cvxb_batch_adjoint_cone: only the
+ * symmetric part of gz's block enters, and both triangles of uz's and dG's block hold the same value.  For a
+ * parameter t of F the caller forms dL/dt = -d_t[ux' Df(x; t)' zk + uk' f(x; t)] with uk = [0; uznl] (cpl: uznl),
+ * x, z, ux and uz held constant, so uz's nonlinear rows are needed for that.  Every array is in the caller's problem
+ * order and in `space`.  A NULL input is zero; a NULL output is not written: without dG and dA no gradient kernel
+ * runs.  A problem whose status is not 1, whose F(x, zk) has a non-finite entry in f, Df or H's lower triangle, or
+ * whose KKT matrix has no Cholesky factor at that iterate, gets NaN in all its outputs.  A callback that returns
+ * nonzero makes the call CVXB_E_ARG, with the solver's state as the solve left it.  cvxb_batch_results is unchanged
+ * afterwards and a re-solve computes the same results.  CP and cpl batches only: any other batch, a QCQP batch
+ * included, is CVXB_E_UNSUP, and cvxb_batch_adjoint, _qcqp, _cone and _gp refuse CP and cpl batches.  A batch
+ * without a completed cvxb_batch_solve since its last load is CVXB_E_ARG.  CVXB_DEVICE allocates nothing;
+ * CVXB_HOST stages each given array in temporary device memory, at most nprob * (2 (n + p + m) + ml n + p n)
+ * doubles in all. */
+int cvxb_batch_adjoint_cp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
+                          double *uz, double *dG, double *dA, int space);
 
 #ifdef __cplusplus
 }
