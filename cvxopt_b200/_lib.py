@@ -154,6 +154,10 @@ _SIGS = {
     "cvxb_batch_adjoint_cone": (C.c_int, [C.c_void_p] + [C.c_void_p] * 9 + [C.c_int]),
     "cvxb_batch_adjoint_gp": (C.c_int, [C.c_void_p] + [C.c_void_p] * 10 + [C.c_int]),
     "cvxb_batch_adjoint_cp": (C.c_int, [C.c_void_p] + [C.c_void_p] * 8 + [C.c_int]),
+    "cvxb_batch_tangent": (C.c_int, [C.c_void_p] + [C.c_void_p] * 9 + [C.c_int]),
+    "cvxb_batch_tangent_qcqp": (C.c_int, [C.c_void_p] + [C.c_void_p] * 10 + [C.c_int]),
+    "cvxb_batch_tangent_gp": (C.c_int, [C.c_void_p] + [C.c_void_p] * 9 + [C.c_int]),
+    "cvxb_batch_tangent_cp": (C.c_int, [C.c_void_p] + [C.c_void_p] * 10 + [C.c_int]),
     "cvxb_batch_set_cp_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "cvxb_batch_create_cpl": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                         C.c_int]),

@@ -192,6 +192,37 @@ def _adjoint_args(gx, gy, gz, want, B, n, p, m, keys=ADJOINT_KEYS):
     return gs, want
 
 
+def _tangent_in(B, named):
+    """data directions `named` ((name, array or None, per-problem shape, axes to the library's layout or None)) ->
+    contiguous float64 host arrays in the library's layouts (None stays None); a wrong shape or dtype is a TypeError"""
+    out = []
+    for name, a, shape, axes in named:
+        if a is not None:
+            a = np.asarray(a)
+            if a.dtype.kind != "f":
+                raise TypeError("%s must be a float array, not %s" % (name, a.dtype))
+            if a.shape != (B,) + tuple(shape):
+                raise TypeError("%s must have shape %s" % (name, (B,) + tuple(shape)))
+            a = a.astype(np.float64, copy=False)
+            a = np.ascontiguousarray(a if axes is None else a.transpose(axes))
+        out.append(a)
+    return out
+
+
+def _tangent_out(lib_call, B, widths):
+    """host outputs dx, dy, dz of widths (n, p, m), filled by lib_call(dx, dy, dz addresses) -> (dx, dy, dz)"""
+    outs = [np.empty((B, w)) for w in widths]
+    lib_call(*(o.ctypes.data for o in outs))
+    return tuple(outs)
+
+
+def _ptrs(arrays):
+    return [None if a is None else a.ctypes.data for a in arrays]
+
+
+_T2 = (0, 2, 1)          # a (B, rows, n) direction to rows x n column-major per problem
+
+
 class QPBatch:
     """dims: the reference's cone dimensions dict ('l' and 'q' only); m must equal its cdim.  None: {'l': m}.
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
@@ -354,6 +385,22 @@ class QPBatch:
         _lib.check(self._lib.cvxb_batch_adjoint_cone(self._h, gx, gy, gz, ux, uy, uz, dP, dG, dA, space),
                    "batch_adjoint_cone")
 
+    def tangent(self, dP=None, dq=None, dG=None, dh=None, dA=None, db=None):
+        """forward-mode derivatives of the last solve's results along the data direction (dP, dq, dG, dh, dA, db) in
+        load()'s shapes, None meaning zero (cvxb_batch_tangent): returns host arrays dx (B, n), dy (B, p) and dz
+        (B, m), z's 's' blocks unpacked as h's.  A non-symmetric dP, and 's' blocks of dh and dG's columns, enter
+        through their symmetric parts.  Every QP batch; a cone LP batch takes dc in place of dq and no dP.  A problem
+        whose status is not 'optimal' gets NaN; a batch not solved since its last load raises ValueError."""
+        B, n, m, p = self.B, self.n, self.m, self.p
+        d = _tangent_in(B, [("dP", dP, (n, n), _T2), ("dq", dq, (n,), None), ("dG", dG, (m, n), _T2),
+                            ("dh", dh, (m,), None), ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
+        return _tangent_out(lambda *o: self.tangent_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+
+    def tangent_ptr(self, dP=None, dq=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
+                    space=_lib.DEVICE):
+        """cvxb_batch_tangent on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_tangent(self._h, dP, dq, dG, dh, dA, db, dx, dy, dz, space), "batch_tangent")
+
     def stats(self):
         ms, it = C.c_double(), C.c_int()
         self._lib.cvxb_batch_stats(self._h, C.byref(ms), C.byref(it))
@@ -500,6 +547,24 @@ class QPBatchGroup:
                 out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
         return out
 
+    def _tangent_parts(self, method, dirs):
+        """the parts' `method` with their slices of the directions dirs -> dx, dy, dz in problem order"""
+        dirs = [None if a is None else np.asarray(a) for a in dirs]
+        if any(a is not None and (a.ndim < 1 or a.shape[0] != self.B) for a in dirs):
+            raise TypeError("every direction must have leading dimension B = %d" % self.B)
+        out = None
+        for ix, part in zip(self.idx, self.parts):
+            r = getattr(part, method)(*(None if a is None else a[ix] for a in dirs))
+            if out is None:
+                out = [np.empty((self.B,) + v.shape[1:]) for v in r]
+            for o, v in zip(out, r):
+                o[ix] = v
+        return tuple(out)
+
+    def tangent(self, dP=None, dq=None, dG=None, dh=None, dA=None, db=None):
+        """QPBatch.tangent on every part with its slice of the direction, the results in problem order"""
+        return self._tangent_parts("tangent", (dP, dq, dG, dh, dA, db))
+
     def stats(self):
         st = [b.stats() for b in self.parts]
         return {"solve_ms": max(s["solve_ms"] for s in st),
@@ -540,6 +605,13 @@ class ConeLPBatch(QPBatch):
         _lib.check(self._lib.cvxb_batch_load_lp(self._h, c, G, h, space), "batch_load_lp")
         self._load_eq(A, b, space)
 
+    def tangent(self, dc=None, dG=None, dh=None, dA=None, db=None):
+        """QPBatch.tangent along (dc, dG, dh, dA, db): a cone LP has no P"""
+        B, n, m, p = self.B, self.n, self.m, self.p
+        d = _tangent_in(B, [("dc", dc, (n,), None), ("dG", dG, (m, n), _T2), ("dh", dh, (m,), None),
+                            ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
+        return _tangent_out(lambda *o: self.tangent_ptr(None, *_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+
 
 class ConeLPBatchGroup(QPBatchGroup):
     """QPBatchGroup's interleaved sub-batches, solved concurrently, for cone LPs"""
@@ -551,6 +623,10 @@ class ConeLPBatchGroup(QPBatchGroup):
 
     def load(self, c, G, h, A=None, b=None):
         self._load_sliced((c, G, h), A, b)
+
+    def tangent(self, dc=None, dG=None, dh=None, dA=None, db=None):
+        """ConeLPBatch.tangent on every part with its slice of the direction, the results in problem order"""
+        return self._tangent_parts("tangent", (dc, dG, dh, dA, db))
 
 
 def _lp_shapes(c, G, h, dims, A, b):
@@ -786,6 +862,21 @@ class GPBatch(QPBatch):
         _lib.check(self._lib.cvxb_batch_adjoint_gp(self._h, gx, gy, gz, ux, uy, uz, dF, dg, dG, dA, space),
                    "batch_adjoint_gp")
 
+    def tangent_gp(self, dF=None, dg=None, dG=None, dh=None, dA=None, db=None):
+        """forward-mode derivatives of the last solve's results along the direction (dF, dg, dG, dh, dA, db) in
+        load()'s shapes, None meaning zero (cvxb_batch_tangent_gp): returns host arrays dx (B, n), dy (B, p) and dz
+        (B, mnl + ml, laid out as [znl, zl]).  A problem whose status is not 'optimal' gets NaN"""
+        B, n, m, p, ml, S = self.B, self.n, self.m, self.p, self.ml, sum(self.K)
+        d = _tangent_in(B, [("dF", dF, (S, n), _T2), ("dg", dg, (S,), None), ("dG", dG, (ml, n), _T2),
+                            ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
+        return _tangent_out(lambda *o: self.tangent_gp_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+
+    def tangent_gp_ptr(self, dF=None, dg=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
+                       space=_lib.DEVICE):
+        """cvxb_batch_tangent_gp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
+        _lib.check(self._lib.cvxb_batch_tangent_gp(self._h, dF, dg, dG, dh, dA, db, dx, dy, dz, space),
+                   "batch_tangent_gp")
+
     def stats(self):
         out = super().stats()
         out["line_search_rounds"] = self._lib.cvxb_batch_ls_rounds(self._h)
@@ -804,6 +895,10 @@ class GPBatchGroup(QPBatchGroup):
 
     def load(self, F, g, G, h, A=None, b=None):
         self._load_sliced((F, g, G, h), A, b)
+
+    def tangent_gp(self, dF=None, dg=None, dG=None, dh=None, dA=None, db=None):
+        """GPBatch.tangent_gp on every part with its slice of the direction, the results in problem order"""
+        return self._tangent_parts("tangent_gp", (dF, dg, dG, dh, dA, db))
 
     def adjoint_gp(self, gx, gy=None, gz=None, want=GP_ADJOINT_KEYS):
         """GPBatch.adjoint_gp on every part with its slice of the gradients, the results in problem order"""
@@ -955,6 +1050,32 @@ class CPBatch(QPBatch):
             raise err
         _lib.check(rc, "batch_adjoint_cp")
 
+    def tangent_cp(self, dc=None, tx=None, tf=None, dG=None, dh=None, dA=None, db=None):
+        """forward-mode derivatives of the last solve's results along dc (B, n, a cpl batch only), dG (B, ml, n), dh
+        (B, ml), dA (B, p, n), db (B, p) and a direction dt of F's parameters t, which enters through tx = d_t[Df(x;
+        t)' zk] dt (B, n) and tf = d_t[f_nl(x; t)] dt (B, mnl) at the returned x (zk = [1; znl], cpl: znl); None
+        means zero (cvxb_batch_tangent_cp).  F is called once more, at the returned x.  Returns host arrays dx (B, n),
+        dy (B, p) and dz (B, mnl + ml, laid out as [znl, zl]).  A problem whose status is not 'optimal', or whose
+        F(x, z) there is not finite, gets NaN.  An exception raised in F comes out unchanged"""
+        B, n, m, p, mnl, ml = self.B, self.n, self.m, self.p, self.mnl, self.ml
+        if dc is not None and self._epi:
+            raise TypeError("a cp batch has no c: its objective is f_0, and F's parameters enter through tx and tf")
+        d = _tangent_in(B, [("dc", dc, (n,), None), ("tx", tx, (n,), None), ("tf", tf, (mnl,), None),
+                            ("dG", dG, (ml, n), _T2), ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2),
+                            ("db", db, (p,), None)])
+        return _tangent_out(lambda *o: self.tangent_cp_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+
+    def tangent_cp_ptr(self, dc=None, tx=None, tf=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None,
+                       dz=None, space=_lib.DEVICE):
+        """cvxb_batch_tangent_cp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL.
+        An exception raised in F comes out unchanged"""
+        self._err = None
+        rc = self._lib.cvxb_batch_tangent_cp(self._h, dc, tx, tf, dG, dh, dA, db, dx, dy, dz, space)
+        err, self._err = self._err, None
+        if err is not None:
+            raise err
+        _lib.check(rc, "batch_tangent_cp")
+
     def set_F(self, F):
         """F(x, idx=idx) -> (f, Df) and F(x, z, idx=idx) -> (f, Df, H), as cp_batch takes it.  The callback runs F on
         the batch's stream and copies what it returns into the handle's buffers; an exception in F is kept and
@@ -1050,6 +1171,10 @@ class CPBatchGroup(QPBatchGroup):
 
     def load(self, x0, G, h, A=None, b=None):
         self._load_sliced((x0, G, h), A, b)
+
+    def tangent_cp(self, dc=None, tx=None, tf=None, dG=None, dh=None, dA=None, db=None):
+        """CPBatch.tangent_cp on every part with its slice of the direction, the results in problem order"""
+        return self._tangent_parts("tangent_cp", (dc, tx, tf, dG, dh, dA, db))
 
     def adjoint_cp(self, gx, gy=None, gz=None, want=None):
         """CPBatch.adjoint_cp on every part with its slice of the gradients, the results in problem order"""
@@ -1206,6 +1331,24 @@ class QCQPBatch(CPBatch):
         _lib.check(self._lib.cvxb_batch_adjoint_qcqp(self._h, gx, gy, gz, ux, uy, uz, dP, dq, dr, dG, dA, space),
                    "batch_adjoint_qcqp")
 
+    def tangent(self, dP=None, dq=None, dr=None, dG=None, dh=None, dA=None, db=None):
+        """forward-mode derivatives of the last solve's results along the direction (dP, dq, dr, dG, dh, dA, db) in
+        load()'s shapes, None meaning zero (cvxb_batch_tangent_qcqp): returns host arrays dx (B, n), dy (B, p) and dz
+        (B, mnl + ml, laid out as [znl, zl]).  A non-symmetric dP_i enters through its symmetric part.  A problem
+        whose status is not 'optimal' gets NaN"""
+        B, n, m, p, ml, nK = self.B, self.n, self.m, self.p, self.ml, self.mnl + 1
+        d = _tangent_in(B, [("dP", dP, (nK, n, n), (0, 3, 1, 2)), ("dq", dq, (nK, n), None), ("dr", dr, (nK,), None),
+                            ("dG", dG, (ml, n), _T2), ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2),
+                            ("db", db, (p,), None)])
+        return _tangent_out(lambda *o: self.tangent_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+
+    def tangent_ptr(self, dP=None, dq=None, dr=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
+                    space=_lib.DEVICE):
+        """cvxb_batch_tangent_qcqp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None:
+        NULL"""
+        _lib.check(self._lib.cvxb_batch_tangent_qcqp(self._h, dP, dq, dr, dG, dh, dA, db, dx, dy, dz, space),
+                   "batch_tangent_qcqp")
+
 
 class QCQPBatchGroup(CPBatchGroup):
     """QPBatchGroup's interleaved sub-batches, solved concurrently on their own streams, for convex QCQPs; nothing
@@ -1222,6 +1365,10 @@ class QCQPBatchGroup(CPBatchGroup):
     def adjoint(self, gx, gy=None, gz=None, want=QCQP_ADJOINT_KEYS):
         """QCQPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
         return super().adjoint(gx, gy, gz, want)
+
+    def tangent(self, dP=None, dq=None, dr=None, dG=None, dh=None, dA=None, db=None):
+        """QCQPBatch.tangent on every part with its slice of the direction, the results in problem order"""
+        return self._tangent_parts("tangent", (dP, dq, dr, dG, dh, dA, db))
 
 
 def _qcqp_args(P, q, r, G, h, dims, A, b, x0):

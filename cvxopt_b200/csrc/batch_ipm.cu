@@ -2449,6 +2449,184 @@ __global__ void k_adj_cp_flag(int *info, const int *flag, int B) {
     if (b < B && flag[b]) info[b] = 1;
 }
 
+// ---- the tangent of a batch's solution (cvxb_batch_tangent, _qcqp, _gp, _cp) ----
+// The adjoint's matrix M is symmetric, so the derivative of (x, y, z) along a data direction d is M^{-1} r(d): the
+// same factorisation, solves and refinement as the adjoint with g = r.  r is the derivative of the KKT residual at the
+// returned iterate with the sign that puts it on the right-hand side: rx = -d(grad_x L), ry = db - dA x, rz = dh -
+// dG x, and on the nonlinear rows -d f_i.  The kernels below form r from the caller's d (problem order, nullptr: zero)
+// and the slot's x, y and z, one CTA of TAN_T threads per slot, into problem perm[b]'s rows of rx, ry and rz; each
+// matrix of d is read once, and no sum depends on the launch: the tangent is bit-identical across compaction and
+// sub-batches.
+constexpr int TAN_T = 256, TAN_RQ = 4, TAN_RC = 32 * TAN_RQ;   // threads, rows per lane, rows per chunk
+// One pass over the rows x cols column-major matrix a (ld lda), chunks of TAN_RC rows, the warps over its columns:
+// COLS: cs[j] += sum_i zf(i) a(i, j), the column sums by the lanes of warp j % nwarp (cs is global, and every pass
+// gives column j to the same warp, so its updates need no fence between passes); ROWS: rowf(i, sum_j a(i, j) xs[j])
+// once per row, the warps' partial sums added in warp order in part (TAN_RC doubles per warp).  a == nullptr is
+// zero: rowf(i, 0) only.  Every thread of the CTA calls it; zf's values are read at the start of a chunk and rowf runs
+// between two barriers, so rowf may overwrite what zf reads
+template <bool COLS, bool ROWS, class Z, class R>
+__device__ __forceinline__ void tan_pass(const double *__restrict__ a, long long lda, int rows, int cols,
+                                         const double *xs, Z zf, double *cs, R rowf, double *part) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = blockDim.x >> 5;
+    if (!a) {
+        if (ROWS) {
+            for (int i = tid; i < rows; i += blockDim.x) rowf(i, 0.0);
+            __syncthreads();
+        }
+        return;
+    }
+    for (int r0 = 0; r0 < rows; r0 += TAN_RC) {
+        double acc[TAN_RQ], zv[TAN_RQ];
+#pragma unroll
+        for (int q = 0; q < TAN_RQ; ++q) {
+            const int i = r0 + lane + 32 * q;
+            acc[q] = 0.0;
+            zv[q] = COLS && i < rows ? zf(i) : 0.0;
+        }
+        for (int j = warp; j < cols; j += nwarp) {
+            const double *aj = a + (long long)j * lda;
+            const double xj = ROWS ? xs[j] : 0.0;
+            double s = 0.0;
+#pragma unroll
+            for (int q = 0; q < TAN_RQ; ++q) {
+                const int i = r0 + lane + 32 * q;
+                if (i < rows) {
+                    const double v = aj[i];
+                    if (ROWS) acc[q] += v * xj;
+                    if (COLS) s += zv[q] * v;
+                }
+            }
+            if (COLS) {
+                s = warp_sum(s);
+                if (lane == 0) cs[j] += s;
+            }
+        }
+        if (ROWS) {
+#pragma unroll
+            for (int q = 0; q < TAN_RQ; ++q) part[warp * TAN_RC + lane + 32 * q] = acc[q];
+            __syncthreads();
+            for (int t = tid; t < TAN_RC && r0 + t < rows; t += blockDim.x) {
+                double v = 0.0;
+                for (int w = 0; w < nwarp; ++w) v += part[w * TAN_RC + t];
+                rowf(r0 + t, v);
+            }
+            __syncthreads();
+        }
+    }
+}
+// the caller's direction, problem order; which arrays a kind reads is its kernel's
+struct TanIn {
+    const double *dP, *dq, *dr, *dF, *dg, *tx, *tf, *dG, *dh, *dA, *db;
+};
+#define TAN_SETUP                                                                                      \
+    const int b = blockIdx.x, tid = threadIdx.x, nt = blockDim.x, n = p.n, m = p.m, pq = p.neq;        \
+    const long long k = perm[b];                                                                       \
+    const double *x = p.x + (long long)b * n, *y = p.y + (long long)b * pq, *z = p.z + (long long)b * m; \
+    double *rx = tx_ + k * n, *ry = ty_ + k * pq, *rz = tz_ + k * m;                                   \
+    __shared__ double part[TAN_T / 32 * TAN_RC];                                                       \
+    (void)y;
+// the linear rows, shared by every kind once rx holds the rest of -rx: rx += dA'y + dG'zl, ry = db - dA x, rzl = dh -
+// dG x over the ml = m - mnl rows of G (zl and rzl from row mnl of z and rz), then rx := -rx
+__device__ __forceinline__ void tan_linear(const Ptrs &p, const TanIn &d, long long k, int mnl, const double *x,
+                                           const double *y, const double *z, double *rx, double *ry, double *rz,
+                                           double *part) {
+    const int n = p.n, pq = p.neq, ml = p.m - mnl;
+    if (pq) tan_pass<true, true>(d.dA ? d.dA + k * pq * n : nullptr, pq, pq, n, x, [&](int i) { return y[i]; }, rx,
+                                 [&](int i, double t) { ry[i] = (d.db ? d.db[k * pq + i] : 0.0) - t; }, part);
+    if (ml) tan_pass<true, true>(d.dG ? d.dG + k * ml * n : nullptr, ml, ml, n, x, [&](int i) { return z[mnl + i]; },
+                                 rx, [&](int i, double t) { rz[mnl + i] = (d.dh ? d.dh[k * ml + i] : 0.0) - t; }, part);
+    __syncthreads();
+    for (int j = threadIdx.x; j < n; j += blockDim.x) rx[j] = -rx[j];
+}
+// QP, cone QP and cone LP (c in dq, dP nullptr): rx = -(sym(dP) x + dq + dA'y + dG'z)
+__global__ void __launch_bounds__(TAN_T) k_tan_rhs(Ptrs p, TanIn d, double *tx_, double *ty_, double *tz_,
+                                                   const int *perm) {
+    TAN_SETUP
+    for (int j = tid; j < n; j += nt) rx[j] = d.dq ? d.dq[k * n + j] : 0.0;
+    __syncthreads();
+    if (d.dP) tan_pass<true, true>(d.dP + k * n * n, n, n, n, x, [&](int i) { return 0.5 * x[i]; }, rx,
+                                   [&](int i, double t) { rx[i] += 0.5 * t; }, part);
+    tan_linear(p, d, k, 0, x, y, z, rx, ry, rz, part);
+}
+// QCQP, zk = [1; znl]: rx = -(sum_l zk_l (sym(dP_l) x + dq_l) + dA'y + dG'zl), rznl_l = -(x'dP_l x / 2 + dq_l'x +
+// dr_l); dP per problem the (nK n) x n column-major stack, dq nK x n, dr nK
+__global__ void __launch_bounds__(TAN_T) k_tan_rhs_qc(Ptrs p, GPPtrs g, TanIn d, double *tx_, double *ty_,
+                                                      double *tz_, const int *perm) {
+    TAN_SETUP
+    const int nK = g.nK;
+    __shared__ double sh[32];
+    for (int j = tid; j < n; j += nt) {
+        double a = 0.0;
+        if (d.dq) {
+            a = d.dq[k * nK * n + j];
+            for (int l = 1; l < nK; ++l) a += z[l - 1] * d.dq[(k * nK + l) * n + j];
+        }
+        rx[j] = a;
+    }
+    __syncthreads();
+    for (int l = 0; l < nK; ++l) {
+        const double zl = l == 0 ? 1.0 : z[l - 1];
+        double a = 0.0;                                  // this thread's share of x'dP_l x / 2 + dq_l'x
+        if (d.dP) tan_pass<true, true>(d.dP + k * nK * n * n + (long long)l * n, (long long)nK * n, n, n, x,
+                                       [&](int i) { return 0.5 * zl * x[i]; }, rx,
+                                       [&](int i, double t) { rx[i] += 0.5 * zl * t; a += 0.5 * x[i] * t; }, part);
+        if (l == 0) continue;
+        if (d.dq) for (int i = tid; i < n; i += nt) a += d.dq[(k * nK + l) * n + i] * x[i];
+        a = block_sum(a, sh);
+        if (tid == 0) rz[l - 1] = -(a + (d.dr ? d.dr[k * nK + l] : 0.0));
+    }
+    tan_linear(p, d, k, g.mnl, x, y, z, rx, ry, rz, part);
+}
+// GP, pi_i = softmax(F_i x + g_i), w_i = dF_i x + dg_i, z_0 = 1: rx = -(sum_i z_i (dF_i'pi_i + F_i'Sigma_i w_i) +
+// dA'y + dG'zl), rznl_i = -pi_i'w_i; dF per problem S x n column-major, dg S.  The slot's F x + g, pi, then z_i pi,
+// w and z_i Sigma_i w_i in yv and wv (scratch that the adjoint and a solve rewrite before they read it)
+__global__ void __launch_bounds__(TAN_T) k_tan_rhs_gp(Ptrs p, GPPtrs g, TanIn d, double *tx_, double *ty_,
+                                                      double *tz_, const int *perm) {
+    TAN_SETUP
+    const int S = g.sumK, nK = g.nK;
+    const double *Fb = g.G + (long long)b * g.sG + m, *gv = g.g + (long long)b * p.L;
+    double *pi = g.yv + (long long)b * S, *w = g.wv + (long long)b * S;
+    __shared__ double sh[32];
+    auto none = [](int) { return 0.0; };
+    tan_pass<false, true>(Fb, g.ldg, S, n, x, none, nullptr, [&](int r, double t) { pi[r] = t + gv[r]; }, part);
+    for (int i = 0; i < nK; ++i) {                       // softmax per block, gp_eval_body's
+        const int k0 = g.koff[i], K = g.koff[i + 1] - k0;
+        const double zi = i == 0 ? 1.0 : z[i - 1];
+        double mx = -INFINITY;
+        for (int r = tid; r < K; r += nt) mx = fmax(mx, pi[k0 + r]);
+        mx = -block_min(-mx, sh);
+        double sum = 0.0;
+        for (int r = tid; r < K; r += nt) { const double e = exp(pi[k0 + r] - mx); pi[k0 + r] = e; sum += e; }
+        const double inv = 1.0 / block_sum(sum, sh);
+        for (int r = tid; r < K; r += nt) { const double v = pi[k0 + r] * inv; pi[k0 + r] = v; w[k0 + r] = zi * v; }
+    }
+    for (int j = tid; j < n; j += nt) rx[j] = 0.0;
+    __syncthreads();
+    tan_pass<true, true>(d.dF ? d.dF + k * S * n : nullptr, S, S, n, x, [&](int r) { return w[r]; }, rx,
+                         [&](int r, double t) { w[r] = t + (d.dg ? d.dg[k * S + r] : 0.0); }, part);
+    for (int i = 0; i < nK; ++i) {                       // t_i = pi_i'w_i, then w := z_i Sigma_i w_i
+        const int k0 = g.koff[i], K = g.koff[i + 1] - k0;
+        const double zi = i == 0 ? 1.0 : z[i - 1];
+        double t = 0.0;
+        for (int r = tid; r < K; r += nt) t += pi[k0 + r] * w[k0 + r];
+        t = block_sum(t, sh);
+        if (i > 0 && tid == 0) rz[i - 1] = -t;
+        for (int r = tid; r < K; r += nt) w[k0 + r] = zi * (pi[k0 + r] * (w[k0 + r] - t));
+    }
+    __syncthreads();
+    tan_pass<true, false>(Fb, g.ldg, S, n, x, [&](int r) { return w[r]; }, rx, [](int, double) {}, part);
+    tan_linear(p, d, k, g.mnl, x, y, z, rx, ry, rz, part);
+}
+// CP and cpl, from the caller's theta terms: rx = -(dc + tx + dA'y + dG'zl), rznl = -tf (tx n, tf mnl per problem)
+__global__ void __launch_bounds__(TAN_T) k_tan_rhs_cp(Ptrs p, GPPtrs g, TanIn d, double *tx_, double *ty_,
+                                                      double *tz_, const int *perm) {
+    TAN_SETUP
+    for (int j = tid; j < n; j += nt) rx[j] = (d.dq ? d.dq[k * n + j] : 0.0) + (d.tx ? d.tx[k * n + j] : 0.0);
+    for (int i = tid; i < g.mnl; i += nt) rz[i] = d.tf ? -d.tf[k * g.mnl + i] : 0.0;
+    __syncthreads();
+    tan_linear(p, d, k, g.mnl, x, y, z, rx, ry, rz, part);
+}
+
 // the problem family of a batch: coneqp, conelp, gp, cp, cpl or a convex QCQP (cp with the library's F)
 enum class Kind { QP, LP, GP, CP, CPL, QC };
 }  // namespace
@@ -4050,6 +4228,55 @@ int batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const doubl
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;
 }
+
+// the tangent of a solved batch along d (the entry points check the kind and the solve): r(d) into the outputs (a NULL
+// output's part of r into temporary device memory), then batch_adjoint with g = r, which reads g before it writes u
+int batch_tangent(cvxb_batch *b, TanIn d, double *dx, double *dy, double *dz, int space) {
+    CVXB_CUDA(cudaSetDevice(b->device));
+    cudaStream_t st = b->st;
+    const bool qc = b->kind == Kind::QC, gp = b->kind == Kind::GP, cp = b->calls_back();
+    const size_t B = b->B, n = b->n, m = b->m, pq = b->neq, nK = b->gq.nK, mnl = b->gq.mnl;
+    const size_t ml = qc || gp || cp ? m - mnl : m, S = gp ? b->gq.sumK : 0;
+    Staged s_dP, s_dq, s_dr, s_dF, s_dg, s_tx, s_tf, s_dG, s_dh, s_dA, s_db, s_dx, s_dy, s_dz;
+    auto in = [&](Staged &s, const double *a, size_t len, const double *&o) -> int {
+        o = nullptr;
+        if (a && len) { CVXB_TRY(s.in(a, B * len, space, st)); o = s.dev; }
+        return 0;
+    };
+    TanIn t{};
+    const size_t sq = qc ? nK : 1;                       // P and q blocks per problem
+    CVXB_TRY(in(s_dP, d.dP, sq * n * n, t.dP)); CVXB_TRY(in(s_dq, d.dq, sq * n, t.dq));
+    if (qc) CVXB_TRY(in(s_dr, d.dr, nK, t.dr));
+    if (gp) { CVXB_TRY(in(s_dF, d.dF, S * n, t.dF)); CVXB_TRY(in(s_dg, d.dg, S, t.dg)); }
+    if (cp) { CVXB_TRY(in(s_tx, d.tx, n, t.tx)); CVXB_TRY(in(s_tf, d.tf, mnl, t.tf)); }
+    CVXB_TRY(in(s_dG, d.dG, ml * n, t.dG)); CVXB_TRY(in(s_dh, d.dh, ml, t.dh));
+    CVXB_TRY(in(s_dA, d.dA, pq * n, t.dA)); CVXB_TRY(in(s_db, d.db, pq, t.db));
+    Scratch<double> tmp;                                 // r's parts whose outputs are NULL
+    const size_t tn = (dx ? 0 : n) + (dy ? 0 : pq) + (dz ? 0 : m);
+    if (tn) CVXB_TRY(tmp.alloc(B * tn));
+    double *next = tmp.p;
+    auto out = [&](Staged &s, double *a, size_t len, double *&o) -> int {
+        if (!a) { o = next; next += B * len; return 0; }
+        CVXB_TRY(s.in(a, B * len, space, st, false));
+        o = s.dev;
+        return 0;
+    };
+    double *rx, *ry, *rz;
+    CVXB_TRY(out(s_dx, dx, n, rx)); CVXB_TRY(out(s_dy, dy, pq, ry)); CVXB_TRY(out(s_dz, dz, m, rz));
+    CVXB_CUDA(cudaMemcpyAsync(b->d_perm.p, b->perm.data(), B * sizeof(int), cudaMemcpyHostToDevice, st));
+    const Ptrs &p = b->p;
+    if (qc) k_tan_rhs_qc<<<(unsigned)B, TAN_T, 0, st>>>(p, b->gq, t, rx, ry, rz, b->d_perm.p);
+    else if (gp) k_tan_rhs_gp<<<(unsigned)B, TAN_T, 0, st>>>(p, b->gq, t, rx, ry, rz, b->d_perm.p);
+    else if (cp) k_tan_rhs_cp<<<(unsigned)B, TAN_T, 0, st>>>(p, b->gq, t, rx, ry, rz, b->d_perm.p);
+    else k_tan_rhs<<<(unsigned)B, TAN_T, 0, st>>>(p, t, rx, ry, rz, b->d_perm.p);
+    count_launch();
+    CVXB_LAUNCH_CHECK();
+    CVXB_TRY(batch_adjoint(b, rx, ry, rz, dx ? rx : nullptr, dy ? ry : nullptr, dz ? rz : nullptr, AdjGrads{},
+                           CVXB_DEVICE));
+    for (Staged *s : {&s_dx, &s_dy, &s_dz}) CVXB_TRY(s->out(st));
+    CVXB_CUDA(cudaStreamSynchronize(st));
+    return 0;
+}
 }  // namespace
 
 int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
@@ -4124,6 +4351,75 @@ int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, c
         return CVXB_E_ARG;
     }
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, nullptr, nullptr, dG, dA}, space);
+}
+
+namespace {
+// the checks every tangent entry point makes after its kind's
+int tangent_solved(cvxb_batch *b, const char *what) {
+    if (b->solved) return 0;
+    set_error("%s: no completed cvxb_batch_solve since the last load", what);
+    return CVXB_E_ARG;
+}
+}  // namespace
+
+int cvxb_batch_tangent(cvxb_batch *b, const double *dP, const double *dq, const double *dG, const double *dh,
+                       const double *dA, const double *db, double *dx, double *dy, double *dz, int space) {
+    if (!b) { set_error("batch_tangent: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QP && b->kind != Kind::LP) {
+        set_error("batch_tangent: only QP and cone LP batches are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (b->kind == Kind::LP && dP) { set_error("batch_tangent: a cone LP has no P: dP must be NULL"); return CVXB_E_ARG; }
+    CVXB_TRY(tangent_solved(b, "batch_tangent"));
+    TanIn d{};
+    d.dP = dP; d.dq = dq; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
+    return batch_tangent(b, d, dx, dy, dz, space);
+}
+
+int cvxb_batch_tangent_qcqp(cvxb_batch *b, const double *dP, const double *dq, const double *dr, const double *dG,
+                            const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
+                            int space) {
+    if (!b) { set_error("batch_tangent_qcqp: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::QC) {
+        set_error("batch_tangent_qcqp: only QCQP batches (cvxb_batch_create_qcqp) are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    CVXB_TRY(tangent_solved(b, "batch_tangent_qcqp"));
+    TanIn d{};
+    d.dP = dP; d.dq = dq; d.dr = dr; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
+    return batch_tangent(b, d, dx, dy, dz, space);
+}
+
+int cvxb_batch_tangent_gp(cvxb_batch *b, const double *dF, const double *dg, const double *dG, const double *dh,
+                          const double *dA, const double *db, double *dx, double *dy, double *dz, int space) {
+    if (!b) { set_error("batch_tangent_gp: batch is NULL"); return CVXB_E_ARG; }
+    if (b->kind != Kind::GP) {
+        set_error("batch_tangent_gp: only GP batches (cvxb_batch_create_gp) are differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    CVXB_TRY(tangent_solved(b, "batch_tangent_gp"));
+    TanIn d{};
+    d.dF = dF; d.dg = dg; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
+    return batch_tangent(b, d, dx, dy, dz, space);
+}
+
+int cvxb_batch_tangent_cp(cvxb_batch *b, const double *dc, const double *tx, const double *tf, const double *dG,
+                          const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
+                          int space) {
+    if (!b) { set_error("batch_tangent_cp: batch is NULL"); return CVXB_E_ARG; }
+    if (!b->calls_back()) {
+        set_error("batch_tangent_cp: only CP and cpl batches (cvxb_batch_create_cp, _cpl, _sdp_cpl) are "
+                  "differentiated here");
+        return CVXB_E_UNSUP;
+    }
+    if (b->kind == Kind::CP && dc) {
+        set_error("batch_tangent_cp: a CP batch has no c (its objective is f_0): dc must be NULL");
+        return CVXB_E_ARG;
+    }
+    CVXB_TRY(tangent_solved(b, "batch_tangent_cp"));
+    TanIn d{};
+    d.dq = dc; d.tx = tx; d.tf = tf; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
+    return batch_tangent(b, d, dx, dy, dz, space);
 }
 
 int cvxb_batch_results_y(cvxb_batch *b, double *y, int space) {

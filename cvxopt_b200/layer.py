@@ -17,6 +17,12 @@ the KKT system at the returned iterate, then the gradients written by one kernel
 gradient of each P is the symmetric one (the solvers read only lower triangles), so a P built as S + S' or from an
 expanded tensor gets the right gradient from autograd.  A problem whose status is not optimal (status != 1) gets NaN
 gradients.
+
+Every layer also has forward mode: under torch.autograd.forward_ad, dual inputs give dual x, y and z (znl and zl),
+from the library's tangent (cvxb_batch_tangent, _qcqp, _gp, _cp), the same factorisation and solves as backward
+with a right-hand side formed on the device from the input tangents.  A non-symmetric tangent of P enters through
+its symmetric part.  In cp_layer and cpl_layer the params' tangents enter through one more call of F.  status carries
+no tangent.
 """
 import numpy as np
 import torch
@@ -212,13 +218,42 @@ def _solve(grp, data, load, options, dev, widths):
     return its, x, s, z, y, torch.from_numpy(status).to(dev)
 
 
-def _keep(ctx, grp, its, needs):
-    """the solved group stays on the device for backward when some input needs a gradient"""
-    if any(needs):
+def _keep(ctx, grp, its, needs, fw=False):
+    """the solved group stays on the device for backward when some input needs a gradient, and for jvp when some
+    input carries a forward-mode tangent (fw)"""
+    if any(needs) or fw:
         ctx.grp, ctx.its = grp, its
     else:
         grp.close()
     ctx.set_materialize_grads(False)
+
+
+def _has_tangent(*ts):
+    """whether a tensor of ts carries a forward-mode tangent (torch.autograd.forward_ad)"""
+    return any(isinstance(t, torch.Tensor) and torch.autograd.forward_ad.unpack_dual(t).tangent is not None
+               for t in ts)
+
+
+def _tangent(ctx, dirs, widths, call, dev, needs):
+    """the tangent of every part of the kept group along its rows of dirs (name -> tensor in the library's layout;
+    None: zero), into dx, dy, dz (widths n, p, m) in problem order: call(part, direction addresses, output
+    addresses).  Frees the group unless backward will need it (some input needs a gradient)"""
+    grp, its = ctx.grp, ctx.its
+    f64 = dict(dtype=torch.float64, device=dev)
+    out = [torch.empty((grp.B, w), **f64) for w in widths]
+    try:
+        for it, part in zip(its, grp.parts):
+            d = {k: _rows(t, it) for k, t in dirs.items() if t is not None}
+            o = out if it is None else [torch.empty((part.B, w), **f64) for w in widths]
+            torch.cuda.current_stream(dev).synchronize()      # the slices are written, the new blocks free
+            call(part, {k: t.data_ptr() for k, t in d.items()}, [t.data_ptr() for t in o])
+            if it is not None:
+                for full, t in zip(out, o):
+                    full.index_copy_(0, it, t)
+    finally:
+        if not any(needs):
+            grp.close()
+    return out
 
 
 def _adjoint(ctx, grads, shapes, call, dev):
@@ -245,6 +280,7 @@ def _adjoint(ctx, grads, shapes, call, dev):
 class _QPLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, P, q, G, h, A, b, nsub, options):
+        options_fw = options.pop("_fw")
         B, n, m, p = ctx.shapes = _check(P, q, G, h, A, b, options.pop("dims", None))
         dev = P.device
         # the layouts the library loads: P, G and A column-major per problem
@@ -262,13 +298,18 @@ class _QPLayer(torch.autograd.Function):
         except BaseException:
             grp.close()
             raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:6])
+        _keep(ctx, grp, its, ctx.needs_input_grad[:6], options_fw)
+        ctx.dev = dev
         return x, y, z, status
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gz, _gstatus):
         return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_ptr), None, None)
+
+    @staticmethod
+    def jvp(ctx, dP, dq, dG, dh, dA, db, _nsub, _options):
+        return (*_qp_tangent(ctx, dP, dq, dG, dh, dA, db), None)
 
 
 def _qp_grads(ctx, gx, gy, gz, adjoint):
@@ -296,9 +337,25 @@ def _qp_grads(ctx, gx, gy, gz, adjoint):
     return res
 
 
+def _qp_tangent(ctx, dP, dq, dG, dh, dA, db):
+    """the tangents of x, y and z for qp_layer and the cone layers (a cone LP: dP None, dq its dc) along the inputs'
+    forward-mode tangents (None: zero), through each part's tangent_ptr"""
+    B, n, m, p = ctx.shapes
+    dev = ctx.dev
+    # the layouts the library loads: P, G and A column-major per problem
+    dirs = {"P": None if dP is None else dP.transpose(1, 2), "q": dq,
+            "G": None if dG is None or not m else dG.transpose(1, 2), "h": dh if m else None,
+            "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
+    return _tangent(ctx, dirs, (n, p, m),
+                    lambda part, d, o: part.tangent_ptr(*(d.get(k) for k in ("P", "q", "G", "h", "A", "b")), *o,
+                                                        space=_lib.DEVICE),
+                    dev, ctx.needs_input_grad[:6])
+
+
 class _ConeLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, P, q, G, h, A, b, dims, nsub, options):
+        options_fw = options.pop("_fw")
         B, n, m, p = ctx.shapes = _check_cone(P, q, G, h, dims, A, b)
         dev = q.device
         device = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -322,7 +379,8 @@ class _ConeLayer(torch.autograd.Function):
         except BaseException:
             grp.close()
             raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:6])
+        _keep(ctx, grp, its, ctx.needs_input_grad[:6], options_fw)
+        ctx.dev = dev
         return x, y, z, status
 
     @staticmethod
@@ -330,10 +388,15 @@ class _ConeLayer(torch.autograd.Function):
     def backward(ctx, gx, gy, gz, _gstatus):
         return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_cone_ptr), None, None, None)
 
+    @staticmethod
+    def jvp(ctx, dP, dq, dG, dh, dA, db, _dims, _nsub, _options):
+        return (*_qp_tangent(ctx, dP, dq, dG, dh, dA, db), None)
+
 
 class _QCQPLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, P, q, r, G, h, A, b, x0, nsub, options):
+        fw = options.pop("_fw")
         B, mnl, n, ml, p = ctx.shapes = _check_qcqp(P, q, r, G, h, A, b, x0, options.pop("dims", None))
         dev = P.device
         # the layouts the library loads: per problem P's (mnl + 1) n x n column-major stack, G and A column-major
@@ -354,7 +417,8 @@ class _QCQPLayer(torch.autograd.Function):
         except BaseException:
             grp.close()
             raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:7])
+        _keep(ctx, grp, its, ctx.needs_input_grad[:7], fw)
+        ctx.dev = dev
         return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
 
     @staticmethod
@@ -387,10 +451,24 @@ class _QCQPLayer(torch.autograd.Function):
                 res.append(torch.zeros(empty[key], **f64) if need[key] else None)
         return (*res, None, None, None)
 
+    @staticmethod
+    def jvp(ctx, dP, dq, dr, dG, dh, dA, db, _dx0, _nsub, _options):
+        B, mnl, n, ml, p = ctx.shapes
+        # the layouts the library loads: P's (mnl + 1) n x n column-major stack, G and A column-major
+        dirs = {"P": None if dP is None else dP.permute(0, 3, 1, 2), "q": dq, "r": dr,
+                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
+                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
+        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
+                              lambda part, d, o: part.tangent_ptr(*(d.get(k) for k in ("P", "q", "r", "G", "h", "A",
+                                                                                       "b")), *o, space=_lib.DEVICE),
+                              ctx.dev, ctx.needs_input_grad[:7])
+        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+
 
 class _GPLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, K, F, g, G, h, A, b, nsub, options):
+        fw = options.pop("_fw")
         B, n, ml, p = _check_gp(K, F, g, G, h, A, b)
         mnl = len(K) - 1
         ctx.shapes = B, n, sum(K), mnl, ml, p
@@ -410,7 +488,8 @@ class _GPLayer(torch.autograd.Function):
         except BaseException:
             grp.close()
             raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[1:7])
+        _keep(ctx, grp, its, ctx.needs_input_grad[1:7], fw)
+        ctx.dev = dev
         return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
 
     @staticmethod
@@ -443,6 +522,20 @@ class _GPLayer(torch.autograd.Function):
                 res.append(torch.zeros(empty[key], **f64) if need[key] else None)
         return (None, *res, None, None)
 
+    @staticmethod
+    def jvp(ctx, _dK, dF, dg, dG, dh, dA, db, _nsub, _options):
+        B, n, S, mnl, ml, p = ctx.shapes
+        # the layouts the library loads: F, G and A column-major per problem
+        dirs = {"F": None if dF is None else dF.transpose(1, 2), "g": dg,
+                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
+                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
+        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
+                              lambda part, d, o: part.tangent_gp_ptr(*(d.get(k) for k in ("F", "g", "G", "h", "A",
+                                                                                          "b")), *o,
+                                                                     space=_lib.DEVICE),
+                              ctx.dev, ctx.needs_input_grad[1:7])
+        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+
 
 def qp_layer(P, q, G, h, A=None, b=None, nsub=None, **options):
     """Solve B dense QPs  minimize 1/2 x'P x + q'x  s.t.  G x <= h,  A x = b  on the GPU, differentiably.
@@ -457,7 +550,7 @@ def qp_layer(P, q, G, h, A=None, b=None, nsub=None, **options):
     Backward (once: no double backward) returns dL/dP (symmetric), dL/dq, dL/dG, dL/dh, dL/dA and dL/db from the
     gradients of x, y and z, with NaN for problems whose status is not 1.  Inputs that need no gradient get none and
     cost nothing.  The solved batch is kept on the device from forward to backward, and freed by backward."""
-    return _QPLayer.apply(P, q, G, h, A, b, nsub, dict(options))
+    return _QPLayer.apply(P, q, G, h, A, b, nsub, dict(options, _fw=_has_tangent(P, q, G, h, A, b)))
 
 
 def qcqp_layer(P, q, r, G=None, h=None, A=None, b=None, x0=None, nsub=None, **options):
@@ -476,7 +569,8 @@ def qcqp_layer(P, q, r, G=None, h=None, A=None, b=None, x0=None, nsub=None, **op
     dL/db from the gradients of x, y, znl and zl, with NaN for problems whose status is not 1; x0 gets none.  Inputs
     that need no gradient get none and cost nothing.  The solved batch is kept on the device from forward to backward,
     and freed by backward."""
-    return _QCQPLayer.apply(P, q, r, G, h, A, b, x0, nsub, dict(options))
+    return _QCQPLayer.apply(P, q, r, G, h, A, b, x0, nsub,
+                            dict(options, _fw=_has_tangent(P, q, r, G, h, A, b)))
 
 
 def coneqp_layer(P, q, G, h, dims, A=None, b=None, nsub=None, **options):
@@ -496,7 +590,7 @@ def coneqp_layer(P, q, G, h, dims, A=None, b=None, nsub=None, **options):
     z's gradient enters through its symmetric part, and the 's' blocks of dL/dh and of each column of dL/dG are the
     gradient over symmetric matrices, the same value in both triangles: a G whose 's' columns are built as X + X' gets
     the right gradient from autograd.  The solved batch is kept on the device from forward to backward."""
-    return _ConeLayer.apply(P, q, G, h, A, b, dims, nsub, dict(options))
+    return _ConeLayer.apply(P, q, G, h, A, b, dims, nsub, dict(options, _fw=_has_tangent(P, q, G, h, A, b)))
 
 
 def conelp_layer(c, G, h, dims, A=None, b=None, nsub=None, **options):
@@ -506,7 +600,7 @@ def conelp_layer(c, G, h, dims, A=None, b=None, nsub=None, **options):
     c (B, n) and the rest as coneqp_layer's, which this is with P = 0.  Returns (x, y, z, status_code); a problem
     found infeasible (status 4 or 5) gets NaN gradients like any status other than 1.  Backward returns dL/dc, dL/dG,
     dL/dh, dL/dA and dL/db with coneqp_layer's conventions."""
-    return _ConeLayer.apply(None, c, G, h, A, b, dims, nsub, dict(options))
+    return _ConeLayer.apply(None, c, G, h, A, b, dims, nsub, dict(options, _fw=_has_tangent(c, G, h, A, b)))
 
 
 def gp_layer(K, F, g, G=None, h=None, A=None, b=None, nsub=None, **options):
@@ -530,7 +624,7 @@ def gp_layer(K, F, g, G=None, h=None, A=None, b=None, nsub=None, **options):
     y, znl and zl (cvxb_batch_adjoint_gp), with NaN for problems whose status is not 1; K gets none.  Inputs that need
     no gradient get none and cost nothing.  The solved batch is kept on the device from forward to backward, and
     freed by backward."""
-    return _GPLayer.apply(K, F, g, G, h, A, b, nsub, dict(options))
+    return _GPLayer.apply(K, F, g, G, h, A, b, nsub, dict(options, _fw=_has_tangent(F, g, G, h, A, b)))
 
 
 def _check_cp(F, params, c, G, h, dims, A, b, cpl):
@@ -600,6 +694,7 @@ class _CPLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, F, c, G, h, A, b, info, nsub, options, *params):
         B, n, mnl, ml, p, x0, dims = info
+        fw = options.pop("_fw")
         cpl = c is not None
         dev = x0.device
         device = dev.index if dev.index is not None else torch.cuda.current_device()
@@ -631,9 +726,10 @@ class _CPLayer(torch.autograd.Function):
             grp.close()
             raise
         needs = ctx.needs_input_grad
-        _keep(ctx, grp, its, needs[1:6] + needs[9:])
-        if any(needs[9:]):                   # the theta call's point and multipliers, and the detached params
+        _keep(ctx, grp, its, needs[1:6] + needs[9:], fw)
+        if any(needs[9:]) or fw:             # the theta call's point and multipliers, and the detached params
             ctx.F, ctx.params, ctx.x, ctx.znl = F, det, x.clone(), z[:, :mnl].clone()
+        ctx.dev = dev
         return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
 
     @staticmethod
@@ -668,6 +764,51 @@ class _CPLayer(torch.autograd.Function):
             dparams = _theta_grads(ctx, out["ux"], out["uz"][:, :mnl] if mnl else torch.zeros((B, 0), **f64),
                                    cpl, needp)
         return (None, res["c"], res["G"], res["h"], res["A"], res["b"], None, None, None, *dparams)
+
+    @staticmethod
+    def jvp(ctx, _dF, dc, dG, dh, dA, db, _dinfo, _nsub, _options, *dparams):
+        B, n, mnl, ml, p, cpl = ctx.shapes
+        needs = ctx.needs_input_grad
+        tx = tf = None
+        if any(t is not None for t in dparams):
+            tx, tf = _theta_tangents(ctx, dparams, cpl)
+        # the layouts the library loads: G and A column-major per problem
+        dirs = {"c": dc if cpl else None, "tx": tx, "tf": tf if mnl else None,
+                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
+                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
+        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
+                              lambda part, d, o: part.tangent_cp_ptr(*(d.get(k) for k in ("c", "tx", "tf", "G", "h",
+                                                                                          "A", "b")), *o,
+                                                                     space=_lib.DEVICE),
+                              ctx.dev, needs[1:6] + needs[9:])
+        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+
+
+def _theta_tangents(ctx, dparams, cpl):
+    """tx = d_theta[Df(x; theta)' zk] dtheta and tf = d_theta[f_nl(x; theta)] dtheta at the returned x, x and z held
+    constant (zk = [1; znl], f_nl = f[:, 1:]; cpl: znl and f), from one call F(x, idx=arange(B), params=...): the
+    directional derivative as the gradient in u of <J'u, dtheta>, J'u by reverse mode (a dual level cannot be opened
+    inside jvp)"""
+    x, znl = ctx.x, ctx.znl
+    B = x.shape[0]
+    zk = znl if cpl else torch.cat([torch.ones((B, 1), dtype=x.dtype, device=x.device), znl], 1)
+    with torch.enable_grad():
+        leaves = tuple(t.detach().requires_grad_(d is not None) for t, d in zip(ctx.params, dparams))
+        f, Df = ctx.F(x, idx=torch.arange(B, device=x.device), params=leaves)[:2]
+        outs = ((Df * zk[:, :, None]).sum(1), f if cpl else f[:, 1:])
+        us = tuple(torch.zeros_like(o, requires_grad=True) for o in outs)
+        wrt = [(t, d) for t, d in zip(leaves, dparams) if d is not None]
+        diff = [o for o in outs if o.requires_grad]
+        if not diff:                     # F uses none of the params with a tangent
+            return torch.zeros_like(outs[0]), torch.zeros_like(outs[1])
+        vjp = torch.autograd.grad([o for o in outs if o.requires_grad], [t for t, _ in wrt],
+                                  [u for o, u in zip(outs, us) if o.requires_grad], create_graph=True,
+                                  allow_unused=True)
+        s = sum((g * d).sum() for g, (_, d) in zip(vjp, wrt) if g is not None)
+        if not isinstance(s, torch.Tensor) or not s.requires_grad:
+            return torch.zeros_like(outs[0]), torch.zeros_like(outs[1])
+        got = torch.autograd.grad(s, us, allow_unused=True)
+    return tuple((torch.zeros_like(o) if g is None else g).detach() for o, g in zip(outs, got))
 
 
 def _theta_grads(ctx, ux, uznl, cpl, needp):
@@ -722,7 +863,8 @@ def cp_layer(F, params=(), G=None, h=None, A=None, b=None, nsub=None, **options)
     library's stream and may see its rows in any order."""
     dims = options.pop("dims", None)
     B, n, mnl, ml, p, x0, _, params = _check_cp(F, params, None, G, h, dims, A, b, False)
-    return _CPLayer.apply(F, None, G, h, A, b, (B, n, mnl, ml, p, x0, None), nsub, dict(options), *params)
+    return _CPLayer.apply(F, None, G, h, A, b, (B, n, mnl, ml, p, x0, None), nsub,
+                          dict(options, _fw=_has_tangent(G, h, A, b, *params)), *params)
 
 
 def cpl_layer(c, F, params=(), G=None, h=None, dims=None, A=None, b=None, nsub=None, **options):
@@ -735,4 +877,5 @@ def cpl_layer(c, F, params=(), G=None, h=None, dims=None, A=None, b=None, nsub=N
     with symmetric 's' blocks.  Backward returns dL/dc = -ux, dL/dG, dL/dh, dL/dA, dL/db with coneqp_layer's 's'
     conventions, and dL/dparam as cp_layer's with zk = znl and uk = uznl.  The rest is cp_layer's."""
     B, n, mnl, ml, p, x0, gdims, params = _check_cp(F, params, c, G, h, dims, A, b, True)
-    return _CPLayer.apply(F, c, G, h, A, b, (B, n, mnl, ml, p, x0, gdims), nsub, dict(options), *params)
+    return _CPLayer.apply(F, c, G, h, A, b, (B, n, mnl, ml, p, x0, gdims), nsub,
+                          dict(options, _fw=_has_tangent(c, G, h, A, b, *params)), *params)

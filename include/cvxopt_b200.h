@@ -642,6 +642,43 @@ int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, con
 int cvxb_batch_adjoint_cp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                           double *uz, double *dG, double *dA, int space);
 
+/* Forward-mode derivatives (tangents) of a batch's last solve: how x, y and z move when the data move along a
+ * direction d.  At the returned iterate, with the matrix M that the matching adjoint solves with (its scaling, H, Df
+ * and D), they solve M [dx; dy; dz] = r(d) with the same factorisation, solves and refinement step as the adjoint,
+ * and write dx (nprob x n), dy (nprob x p) and dz (nprob x m, on the nonlinear kinds [dznl; dzl] laid out as the
+ * results' z).  With sym(X) = (X + X') / 2, r(d) is
+ *     QP, cone QP and cone LP (P = 0, q = c):  rx = -(sym(dP) x + dq + dA'y + dG'z),  ry = db - dA x,  rz = dh - dG x;
+ *     QCQP, zk = [1; znl]:  rx = -(sum_{i=0..mnl} zk_i (sym(dPi) x + dqi) + dA'y + dG'zl),
+ *                           rznl_i = -(x'dPi x / 2 + dqi'x + dri),  ry and rzl as above;
+ *     GP, z_0 = 1, pi_i = softmax(Fi x + gi), Sigma_i = diag(pi_i) - pi_i pi_i', w_i = dFi x + dgi:
+ *                           rx = -(sum_{i=0..mnl} z_i (dFi'pi_i + Fi'Sigma_i w_i) + dA'y + dG'zl), rznl_i = -pi_i'w_i;
+ *     CP and cpl:  rx = -(dc + tx + dA'y + dG'zl),  rznl = -tf,  with the caller's terms of F's parameters t at the
+ *                  returned x, x and z held constant: tx = d_t[Df(x; t)' zk] dt (nprob x n) and tf = d_t[f_nl(x; t)] dt
+ *                  (nprob x mnl), zk = [1; znl] for cp and znl for cpl; dc on a cpl batch only.
+ * Every input has the layout of the matching load call, in the caller's problem order: P, G, A and F column-major per
+ * problem, a QCQP's dP the (mnl + 1) n x n stack and dq (mnl + 1) x n, dG the rows of G only (ml rows on the
+ * nonlinear kinds), a cone LP's dc in dq.  M is symmetric, so for every g, <g, (dx, dy, dz)> = <adjoint(g), d> with
+ * the entrywise pairing of the adjoint's outputs with d, for any d: a non-symmetric dP, and 's' blocks of dh and of
+ * dG's columns, enter through their symmetric parts, and dz's 's' blocks are symmetric.  The contract is the matching
+ * adjoint's: a NULL input is zero and a NULL output is not written; a problem whose status is not 1, whose
+ * factorisation fails there or (CP) whose F(x, zk) is not finite gets NaN in all its outputs; a failing callback makes
+ * the call CVXB_E_ARG; cvxb_batch_results is unchanged afterwards and a re-solve computes the same results.
+ * cvxb_batch_tangent takes every batch cvxb_batch_adjoint_cone takes (dP NULL on a cone LP, else CVXB_E_ARG);
+ * _qcqp QCQP batches, _gp GP batches and _cp CP, cpl and sdp cpl batches (dc NULL on a CP batch, else CVXB_E_ARG).
+ * Another kind is CVXB_E_UNSUP, and a batch without a completed cvxb_batch_solve since its last load CVXB_E_ARG.
+ * r is formed in the outputs, so CVXB_DEVICE with dx, dy and dz given allocates nothing (a NULL output's part of r
+ * takes temporary device memory); CVXB_HOST stages each given array in temporary device memory. */
+int cvxb_batch_tangent(cvxb_batch *b, const double *dP, const double *dq, const double *dG, const double *dh,
+                       const double *dA, const double *db, double *dx, double *dy, double *dz, int space);
+int cvxb_batch_tangent_qcqp(cvxb_batch *b, const double *dP, const double *dq, const double *dr, const double *dG,
+                            const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
+                            int space);
+int cvxb_batch_tangent_gp(cvxb_batch *b, const double *dF, const double *dg, const double *dG, const double *dh,
+                          const double *dA, const double *db, double *dx, double *dy, double *dz, int space);
+int cvxb_batch_tangent_cp(cvxb_batch *b, const double *dc, const double *tx, const double *tf, const double *dG,
+                          const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
+                          int space);
+
 #ifdef __cplusplus
 }
 #endif
