@@ -209,18 +209,34 @@ def _tangent_in(B, named):
     return out
 
 
-def _tangent_out(lib_call, B, widths):
-    """host outputs dx, dy, dz of widths (n, p, m), filled by lib_call(dx, dy, dz addresses) -> (dx, dy, dz)"""
-    outs = [np.empty((B, w)) for w in widths]
-    lib_call(*(o.ctypes.data for o in outs))
-    return tuple(outs)
-
-
 def _ptrs(arrays):
     return [None if a is None else a.ctypes.data for a in arrays]
 
 
-_T2 = (0, 2, 1)          # a (B, rows, n) direction to rows x n column-major per problem
+_T2 = (0, 2, 1)          # a (B, rows, n) matrix to rows x n column-major per problem
+
+# Every derivative call takes its kind's own block, which each batch class declares as `_block`, and then this linear
+# tail, which all kinds share.  An entry is (the tangent's name for it, its per-problem shape as load() takes it, from
+# the batch's n, m, p, mnl and K, the axes to the library's layout or None, whether the adjoint writes dL/d(the name
+# without its first letter) itself).  The tangent reads every entry in order; the adjoint writes ux, uy, uz, then the
+# entries it writes in order, and its other keys come from ux, uy and uz by _FROM_U.  A QP is the case mnl = 0.
+_TAIL = (("dG", lambda b: (b.m - b.mnl, b.n), _T2, True), ("dh", lambda b: (b.m - b.mnl,), None, False),
+         ("dA", lambda b: (b.p, b.n), _T2, True), ("db", lambda b: (b.p,), None, False))
+
+# the adjoint's gradients from its ux, uy and uz: key -> (which of the three, the gradient from it).  dL/dq = dL/dc =
+# -ux, dL/db = uy, dL/dh = uz's rows after the mnl nonlinear ones, and the CP adjoint's ux and uznl (uz's first rows)
+_FROM_U = {"q": (0, lambda u, mnl: -u), "c": (0, lambda u, mnl: -u), "ux": (0, lambda u, mnl: u),
+           "b": (1, lambda u, mnl: u), "h": (2, lambda u, mnl: u[:, mnl:]), "uznl": (2, lambda u, mnl: u[:, :mnl])}
+
+
+def _lib_shape(shape, axes):
+    """a per-problem shape in the library's layout: the axes of the (B,) + shape array, None: as it is"""
+    return shape if axes is None else tuple(((0,) + tuple(shape))[a] for a in axes[1:])
+
+
+def _inverse(axes):
+    """the axes back from the library's layout"""
+    return tuple(axes.index(k) for k in range(len(axes)))
 
 
 class QPBatch:
@@ -228,6 +244,8 @@ class QPBatch:
     p: equality rows A x = b per problem (load() then takes A (B, p, n) and b (B, p))."""
     _lp = False              # ConeLPBatch: a batch of cone LPs
     _sdp = False             # SDPBatch, SDPQPBatch: dims may hold 's' blocks
+    mnl = 0                  # rows of nonlinear constraints before G's: none in a QP or cone LP
+    _block = (("dP", lambda b: (b.n, b.n), _T2, True), ("dq", lambda b: (b.n,), None, False))
 
     def __init__(self, nprob, n, m, device=0, dims=None, p=0):
         if not isinstance(p, (int, np.integer)) or isinstance(p, bool):
@@ -342,18 +360,7 @@ class QPBatch:
         P (B, n, n, symmetric), q (B, n), G (B, m, n), h (B, m), A (B, p, n) and b (B, p), each dL/d(that input).
         A problem whose status is not 'optimal' gets NaN.  QP batches whose rows are all 'l' only: any other batch
         raises NotImplementedError, and a batch not solved since its last load raises ValueError."""
-        B, n, m, p = self.B, self.n, self.m, self.p
-        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m)
-        # C's outputs ux, uy, uz, dP, dG, dA; the matrices column-major per problem
-        shapes = {"q": (B, n), "b": (B, p), "h": (B, m), "P": (B, n, n), "G": (B, n, m), "A": (B, n, p)}
-        bufs = {k: np.empty(shapes[k]) for k in want}
-        ptrs = [None if a is None else a.ctypes.data for a in gs]
-        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("q", "b", "h", "P", "G", "A")]
-        self.adjoint_ptr(*ptrs, space=_lib.HOST)
-        out = {}
-        for k, v in bufs.items():
-            out[k] = -v if k == "q" else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
-        return out
+        return self._adjoint(self.adjoint_ptr, QPBatch._block, ADJOINT_KEYS, gx, gy, gz, want)
 
     def adjoint_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dG=None, dA=None,
                     space=_lib.DEVICE):
@@ -367,17 +374,8 @@ class QPBatch:
         gz (B, m) and the returned h (B, m) and G (B, m, n) are laid out as h, each 's' block unpacked column-major:
         only the symmetric part of gz's blocks enters, and the outputs' blocks hold the same value in both triangles.
         want: keys of ADJOINT_KEYS, of CONELP_ADJOINT_KEYS on a cone LP batch (c for q, no P); None: all of them."""
-        B, n, m, p = self.B, self.n, self.m, self.p
         keys = self._cone_keys
-        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, B, n, p, m, keys)
-        # C's outputs ux, uy, uz, dP, dG, dA; the matrices column-major per problem
-        shapes = {"q": (B, n), "c": (B, n), "b": (B, p), "h": (B, m), "P": (B, n, n), "G": (B, n, m), "A": (B, n, p)}
-        bufs = {k: np.empty(shapes[k]) for k in want}
-        ptrs = [None if a is None else a.ctypes.data for a in gs]
-        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("c" if self._lp else "q", "b", "h", "P", "G", "A")]
-        self.adjoint_cone_ptr(*ptrs, space=_lib.HOST)
-        return {k: -v if k in ("q", "c") else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
-                for k, v in bufs.items()}
+        return self._adjoint(self.adjoint_cone_ptr, QPBatch._block, keys, gx, gy, gz, keys if want is None else want)
 
     def adjoint_cone_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dG=None, dA=None,
                          space=_lib.DEVICE):
@@ -391,15 +389,35 @@ class QPBatch:
         (B, m), z's 's' blocks unpacked as h's.  A non-symmetric dP, and 's' blocks of dh and dG's columns, enter
         through their symmetric parts.  Every QP batch; a cone LP batch takes dc in place of dq and no dP.  A problem
         whose status is not 'optimal' gets NaN; a batch not solved since its last load raises ValueError."""
-        B, n, m, p = self.B, self.n, self.m, self.p
-        d = _tangent_in(B, [("dP", dP, (n, n), _T2), ("dq", dq, (n,), None), ("dG", dG, (m, n), _T2),
-                            ("dh", dh, (m,), None), ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
-        return _tangent_out(lambda *o: self.tangent_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+        return self._tangent(self.tangent_ptr, QPBatch._block, (dP, dq, dG, dh, dA, db))
 
     def tangent_ptr(self, dP=None, dq=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
                     space=_lib.DEVICE):
         """cvxb_batch_tangent on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL"""
         _lib.check(self._lib.cvxb_batch_tangent(self._h, dP, dq, dG, dh, dA, db, dx, dy, dz, space), "batch_tangent")
+
+    def _adjoint(self, ptr, block, keys, gx, gy, gz, want):
+        """the adjoint call `ptr` (an *_ptr) of the kind whose own block is `block`, with the gradients gx, gy, gz and
+        `want` among `keys` -> {key: host array in load()'s layout}"""
+        B = self.B
+        gs, want = _adjoint_args(gx, gy, gz, want, B, self.n, self.p, self.m, keys)
+        own = {name[1:]: (shape(self), axes) for name, shape, axes, writes in block + _TAIL if writes}
+        us = [np.empty((B, w)) if any(_FROM_U[k][0] == i for k in want if k not in own) else None
+              for i, w in enumerate((self.n, self.p, self.m))]
+        outs = {k: np.empty((B,) + _lib_shape(*own[k])) for k in own if k in want}
+        ptr(*_ptrs(gs + us + [outs.get(k) for k in own]), space=_lib.HOST)
+        got = {k: v if own[k][1] is None else v.transpose(_inverse(own[k][1])) for k, v in outs.items()}
+        return {k: np.ascontiguousarray(got[k] if k in got else _FROM_U[k][1](us[_FROM_U[k][0]], self.mnl))
+                for k in want}
+
+    def _tangent(self, ptr, block, dirs):
+        """the tangent call `ptr` (a *_ptr) of the kind whose own block is `block` along dirs, the caller's arrays for
+        block + _TAIL (None: zero) -> host dx (B, n), dy (B, p), dz (B, m)"""
+        d = _tangent_in(self.B, [(name, a, shape(self), axes)
+                                 for (name, shape, axes, _), a in zip(block + _TAIL, dirs)])
+        out = [np.empty((self.B, w)) for w in (self.n, self.p, self.m)]
+        ptr(*_ptrs(d + out), space=_lib.HOST)
+        return tuple(out)
 
     def stats(self):
         ms, it = C.c_double(), C.c_int()
@@ -528,21 +546,20 @@ class QPBatchGroup:
 
     def adjoint(self, gx, gy=None, gz=None, want=ADJOINT_KEYS):
         """QPBatch.adjoint on every part with its slice of the gradients, the results in problem order"""
-        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m, self._adjoint_keys)
-        out = {}
-        for ix, part in zip(self.idx, self.parts):
-            r = part.adjoint(*(None if a is None else a[ix] for a in gs), want=want)
-            for k, v in r.items():
-                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
-        return out
+        return self._adjoint_parts("adjoint", self._adjoint_keys, gx, gy, gz, want)
 
     def adjoint_cone(self, gx, gy=None, gz=None, want=None):
         """QPBatch.adjoint_cone on every part with its slice of the gradients, the results in problem order"""
         keys = self._cone_keys
-        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, self.B, self.n, self.p, self.m, keys)
+        return self._adjoint_parts("adjoint_cone", keys, gx, gy, gz, keys if want is None else want)
+
+    def _adjoint_parts(self, method, keys, gx, gy, gz, want):
+        """the parts' adjoint `method` with their slices of the gradients, `want` among `keys` -> {key: array} in
+        problem order"""
+        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m, keys)
         out = {}
         for ix, part in zip(self.idx, self.parts):
-            r = part.adjoint_cone(*(None if a is None else a[ix] for a in gs), want=want)
+            r = getattr(part, method)(*(None if a is None else a[ix] for a in gs), want=want)
             for k, v in r.items():
                 out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
         return out
@@ -585,6 +602,7 @@ class ConeLPBatch(QPBatch):
     conelp returns None."""
     _lp = True
     _cone_keys = CONELP_ADJOINT_KEYS
+    _block = (QPBatch._block[0], ("dc", lambda b: (b.n,), None, False))      # P is never given: its address is NULL
 
     def load(self, c, G, h, A=None, b=None):
         c = np.ascontiguousarray(np.asarray(c, dtype=np.float64))
@@ -607,10 +625,7 @@ class ConeLPBatch(QPBatch):
 
     def tangent(self, dc=None, dG=None, dh=None, dA=None, db=None):
         """QPBatch.tangent along (dc, dG, dh, dA, db): a cone LP has no P"""
-        B, n, m, p = self.B, self.n, self.m, self.p
-        d = _tangent_in(B, [("dc", dc, (n,), None), ("dG", dG, (m, n), _T2), ("dh", dh, (m,), None),
-                            ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
-        return _tangent_out(lambda *o: self.tangent_ptr(None, *_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+        return self._tangent(self.tangent_ptr, ConeLPBatch._block, (None, dc, dG, dh, dA, db))
 
 
 class ConeLPBatchGroup(QPBatchGroup):
@@ -806,6 +821,7 @@ class GPBatch(QPBatch):
     gp's epigraph problem.  K (block sizes of F, mnl = len(K) - 1), ml rows of G and p rows of A are shared by the
     batch.  load() takes F (B, sum K, n), g (B, sum K), G (B, ml, n), h (B, ml) and, with p > 0, A (B, p, n), b (B, p).
     results()' s and z are [snl; sl] and [znl; zl] (mnl + ml columns); its primal objective is gp's t."""
+    _block = (("dF", lambda b: (sum(b.K), b.n), _T2, True), ("dg", lambda b: (sum(b.K),), None, True))
 
     def __init__(self, nprob, n, K, ml, p=0, device=0):
         K = [int(k) for k in K]
@@ -845,16 +861,7 @@ class GPBatch(QPBatch):
         arrays for the keys in `want`, each dL/d(that input) in load()'s layout: F (B, sum K, n), g (B, sum K),
         G (B, ml, n), h (B, ml), A (B, p, n) and b (B, p).  A problem whose status is not 'optimal' gets NaN.  A batch
         not solved since its last load raises ValueError."""
-        B, n, m, p, ml, S = self.B, self.n, self.m, self.p, self.ml, sum(self.K)
-        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m, GP_ADJOINT_KEYS)
-        # C's outputs uy, uz (h: its 'l' rows), dF, dg, dG, dA; dF, dG and dA column-major per problem
-        shapes = {"b": (B, p), "h": (B, m), "F": (B, n, S), "g": (B, S), "G": (B, n, ml), "A": (B, n, p)}
-        bufs = {k: np.empty(shapes[k]) for k in want}
-        ptrs = [None if a is None else a.ctypes.data for a in gs] + [None]
-        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("b", "h", "F", "g", "G", "A")]
-        self.adjoint_gp_ptr(*ptrs, space=_lib.HOST)
-        return {k: v[:, self.mnl:] if k == "h" else np.ascontiguousarray(v.transpose(0, 2, 1)) if v.ndim == 3 else v
-                for k, v in bufs.items()}
+        return self._adjoint(self.adjoint_gp_ptr, GPBatch._block, GP_ADJOINT_KEYS, gx, gy, gz, want)
 
     def adjoint_gp_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dF=None, dg=None, dG=None,
                        dA=None, space=_lib.DEVICE):
@@ -866,10 +873,7 @@ class GPBatch(QPBatch):
         """forward-mode derivatives of the last solve's results along the direction (dF, dg, dG, dh, dA, db) in
         load()'s shapes, None meaning zero (cvxb_batch_tangent_gp): returns host arrays dx (B, n), dy (B, p) and dz
         (B, mnl + ml, laid out as [znl, zl]).  A problem whose status is not 'optimal' gets NaN"""
-        B, n, m, p, ml, S = self.B, self.n, self.m, self.p, self.ml, sum(self.K)
-        d = _tangent_in(B, [("dF", dF, (S, n), _T2), ("dg", dg, (S,), None), ("dG", dG, (ml, n), _T2),
-                            ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2), ("db", db, (p,), None)])
-        return _tangent_out(lambda *o: self.tangent_gp_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+        return self._tangent(self.tangent_gp_ptr, GPBatch._block, (dF, dg, dG, dh, dA, db))
 
     def tangent_gp_ptr(self, dF=None, dg=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
                        space=_lib.DEVICE):
@@ -902,13 +906,7 @@ class GPBatchGroup(QPBatchGroup):
 
     def adjoint_gp(self, gx, gy=None, gz=None, want=GP_ADJOINT_KEYS):
         """GPBatch.adjoint_gp on every part with its slice of the gradients, the results in problem order"""
-        gs, want = _adjoint_args(gx, gy, gz, want, self.B, self.n, self.p, self.m, GP_ADJOINT_KEYS)
-        out = {}
-        for ix, part in zip(self.idx, self.parts):
-            r = part.adjoint_gp(*(None if a is None else a[ix] for a in gs), want=want)
-            for k, v in r.items():
-                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
-        return out
+        return self._adjoint_parts("adjoint_gp", GP_ADJOINT_KEYS, gx, gy, gz, want)
 
     def stats(self):
         out = super().stats()
@@ -971,6 +969,17 @@ class _DevArray:
         self.__cuda_array_interface__ = {"data": (ptr, False), "shape": shape, "typestr": typestr, "version": 2}
 
 
+def _calling_F(b, call, name, *args):
+    """the library call call(b's handle, *args), which may run b's F: an exception F raised comes out unchanged, else
+    the return code is checked (any batch: the library refuses the kinds without F)"""
+    b._err = None
+    rc = call(b._h, *args)
+    err, b._err = b._err, None
+    if err is not None:
+        raise err
+    _lib.check(rc, name)
+
+
 class CPBatch(QPBatch):
     """B smooth convex programs (cvxb_batch_create_cp): B x solvers.cp(F, G, h, dims={'l': ml}, A, b), the GP batch's
     lock-step cpl on cp's epigraph problem with F evaluated by the caller's batched F on the device.  mnl, ml rows of
@@ -978,6 +987,9 @@ class CPBatch(QPBatch):
     A (B, p, n), b (B, p); set_F() takes cp_batch's F.  `index` is each problem's index in the caller's order, passed to
     F as idx.  results()' s and z are [snl; sl] and [znl; zl]; its primal objective is cp's t."""
     _epi = 1                 # rows of F's f and Df before the mnl: cp's objective (CPLBatch: none)
+    # dc (a cpl batch only) and F's parameter terms tx and tf; the adjoint writes none of them
+    _block = (("dc", lambda b: (b.n,), None, False), ("tx", lambda b: (b.n,), None, False),
+              ("tf", lambda b: (b.mnl,), None, False))
 
     def __init__(self, nprob, n, mnl, ml, p=0, device=0, index=None):
         self._lib = _lib.load()
@@ -1024,31 +1036,14 @@ class CPBatch(QPBatch):
         G (B, ml, n), h (B, ml), A (B, p, n), b (B, p) and, on a cpl batch, c (B, n).  A problem whose status is not
         'optimal', or whose F(x, z) there is not finite, gets NaN.  An exception raised in F comes out unchanged; a
         batch not solved since its last load raises ValueError, and a QCQP batch NotImplementedError."""
-        B, n, m, p, mnl, ml = self.B, self.n, self.m, self.p, self.mnl, self.ml
         keys = self._cp_keys
-        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, B, n, p, m, keys)
-        # C's outputs ux, uy, uz (uznl and h: its rows), dG, dA; dG and dA column-major per problem
-        ux = np.empty((B, n)) if {"ux", "c"} & set(want) else None
-        uz = np.empty((B, m)) if {"uznl", "h"} & set(want) else None
-        bufs = {k: np.empty(s) for k, s in (("b", (B, p)), ("G", (B, n, ml)), ("A", (B, n, p))) if k in want}
-        ptrs = [None if a is None else a.ctypes.data for a in gs + [ux, bufs.get("b"), uz, bufs.get("G"),
-                                                                    bufs.get("A")]]
-        self.adjoint_cp_ptr(*ptrs, space=_lib.HOST)
-        got = {"ux": ux, "c": None if ux is None else -ux, "uznl": None if uz is None else uz[:, :mnl],
-               "h": None if uz is None else uz[:, mnl:], "b": bufs.get("b")}
-        got.update({k: np.ascontiguousarray(bufs[k].transpose(0, 2, 1)) for k in ("G", "A") if k in bufs})
-        return {k: np.ascontiguousarray(got[k]) for k in want}
+        return self._adjoint(self.adjoint_cp_ptr, CPBatch._block, keys, gx, gy, gz, keys if want is None else want)
 
     def adjoint_cp_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dG=None, dA=None,
                        space=_lib.DEVICE):
         """cvxb_batch_adjoint_cp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL.
         An exception raised in F comes out unchanged, as from solve()"""
-        self._err = None
-        rc = self._lib.cvxb_batch_adjoint_cp(self._h, gx, gy, gz, ux, uy, uz, dG, dA, space)
-        err, self._err = self._err, None
-        if err is not None:
-            raise err
-        _lib.check(rc, "batch_adjoint_cp")
+        _calling_F(self, self._lib.cvxb_batch_adjoint_cp, "batch_adjoint_cp", gx, gy, gz, ux, uy, uz, dG, dA, space)
 
     def tangent_cp(self, dc=None, tx=None, tf=None, dG=None, dh=None, dA=None, db=None):
         """forward-mode derivatives of the last solve's results along dc (B, n, a cpl batch only), dG (B, ml, n), dh
@@ -1057,24 +1052,16 @@ class CPBatch(QPBatch):
         means zero (cvxb_batch_tangent_cp).  F is called once more, at the returned x.  Returns host arrays dx (B, n),
         dy (B, p) and dz (B, mnl + ml, laid out as [znl, zl]).  A problem whose status is not 'optimal', or whose
         F(x, z) there is not finite, gets NaN.  An exception raised in F comes out unchanged"""
-        B, n, m, p, mnl, ml = self.B, self.n, self.m, self.p, self.mnl, self.ml
         if dc is not None and self._epi:
             raise TypeError("a cp batch has no c: its objective is f_0, and F's parameters enter through tx and tf")
-        d = _tangent_in(B, [("dc", dc, (n,), None), ("tx", tx, (n,), None), ("tf", tf, (mnl,), None),
-                            ("dG", dG, (ml, n), _T2), ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2),
-                            ("db", db, (p,), None)])
-        return _tangent_out(lambda *o: self.tangent_cp_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+        return self._tangent(self.tangent_cp_ptr, CPBatch._block, (dc, tx, tf, dG, dh, dA, db))
 
     def tangent_cp_ptr(self, dc=None, tx=None, tf=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None,
                        dz=None, space=_lib.DEVICE):
         """cvxb_batch_tangent_cp on raw addresses in `space`, laid out as include/cvxopt_b200.h states; None: NULL.
         An exception raised in F comes out unchanged"""
-        self._err = None
-        rc = self._lib.cvxb_batch_tangent_cp(self._h, dc, tx, tf, dG, dh, dA, db, dx, dy, dz, space)
-        err, self._err = self._err, None
-        if err is not None:
-            raise err
-        _lib.check(rc, "batch_tangent_cp")
+        _calling_F(self, self._lib.cvxb_batch_tangent_cp, "batch_tangent_cp", dc, tx, tf, dG, dh, dA, db, dx, dy, dz,
+                   space)
 
     def set_F(self, F):
         """F(x, idx=idx) -> (f, Df) and F(x, z, idx=idx) -> (f, Df, H), as cp_batch takes it.  The callback runs F on
@@ -1179,13 +1166,7 @@ class CPBatchGroup(QPBatchGroup):
     def adjoint_cp(self, gx, gy=None, gz=None, want=None):
         """CPBatch.adjoint_cp on every part with its slice of the gradients, the results in problem order"""
         keys = self.parts[0]._cp_keys
-        gs, want = _adjoint_args(gx, gy, gz, keys if want is None else want, self.B, self.n, self.p, self.m, keys)
-        out = {}
-        for ix, part in zip(self.idx, self.parts):
-            r = part.adjoint_cp(*(None if a is None else a[ix] for a in gs), want=want)
-            for k, v in r.items():
-                out.setdefault(k, np.empty((self.B,) + v.shape[1:]))[ix] = v
-        return out
+        return self._adjoint_parts("adjoint_cp", keys, gx, gy, gz, keys if want is None else want)
 
     def stats(self):
         out = super().stats()
@@ -1275,6 +1256,9 @@ class QCQPBatch(CPBatch):
     mnl, ml rows of G and p rows of A are shared by the batch.  load() takes P (B, mnl + 1, n, n), of which only each
     P_i's lower triangle is read, q (B, mnl + 1, n), r (B, mnl + 1), x0 (B, n) or None for 0, G (B, ml, n), h (B, ml)
     and, with p > 0, A (B, p, n), b (B, p).  results() are CPBatch's."""
+    # P per problem the (mnl + 1) n x n column-major stack [P_0; ...; P_mnl]: column j holds P_0[:, j], P_1[:, j], ...
+    _block = (("dP", lambda b: (b.mnl + 1, b.n, b.n), (0, 3, 1, 2), True),
+              ("dq", lambda b: (b.mnl + 1, b.n), None, True), ("dr", lambda b: (b.mnl + 1,), None, True))
 
     def _create(self):
         return self._lib.cvxb_batch_create_qcqp(C.byref(self._h), self.B, self.n, self.mnl, self.ml, self.p,
@@ -1310,20 +1294,7 @@ class QCQPBatch(CPBatch):
         host arrays for the keys in `want`, each dL/d(that input) in load()'s layout: P (B, mnl + 1, n, n, each block
         symmetric), q (B, mnl + 1, n), r (B, mnl + 1), G (B, ml, n), h (B, ml), A (B, p, n) and b (B, p).  A problem
         whose status is not 'optimal' gets NaN.  A batch not solved since its last load raises ValueError."""
-        B, n, m, p, ml, nK = self.B, self.n, self.m, self.p, self.ml, self.mnl + 1
-        gs, want = _adjoint_args(gx, gy, gz, want, B, n, p, m, QCQP_ADJOINT_KEYS)
-        # C's outputs uy, uz (h: its 'l' rows), dP, dq, dr, dG, dA; dP, dG and dA column-major per problem
-        shapes = {"b": (B, p), "h": (B, m), "P": (B, n, nK, n), "q": (B, nK, n), "r": (B, nK), "G": (B, n, ml),
-                  "A": (B, n, p)}
-        bufs = {k: np.empty(shapes[k]) for k in want}
-        ptrs = [None if a is None else a.ctypes.data for a in gs] + [None]
-        ptrs += [bufs[k].ctypes.data if k in bufs else None for k in ("b", "h", "P", "q", "r", "G", "A")]
-        self.adjoint_ptr(*ptrs, space=_lib.HOST)
-        out = {}
-        for k, v in bufs.items():
-            out[k] = (np.ascontiguousarray(v.transpose(0, 2, 3, 1)) if k == "P" else v[:, self.mnl:] if k == "h" else
-                      np.ascontiguousarray(v.transpose(0, 2, 1)) if k in ("G", "A") else v)
-        return out
+        return self._adjoint(self.adjoint_ptr, QCQPBatch._block, QCQP_ADJOINT_KEYS, gx, gy, gz, want)
 
     def adjoint_ptr(self, gx=None, gy=None, gz=None, ux=None, uy=None, uz=None, dP=None, dq=None, dr=None, dG=None,
                     dA=None, space=_lib.DEVICE):
@@ -1336,11 +1307,7 @@ class QCQPBatch(CPBatch):
         load()'s shapes, None meaning zero (cvxb_batch_tangent_qcqp): returns host arrays dx (B, n), dy (B, p) and dz
         (B, mnl + ml, laid out as [znl, zl]).  A non-symmetric dP_i enters through its symmetric part.  A problem
         whose status is not 'optimal' gets NaN"""
-        B, n, m, p, ml, nK = self.B, self.n, self.m, self.p, self.ml, self.mnl + 1
-        d = _tangent_in(B, [("dP", dP, (nK, n, n), (0, 3, 1, 2)), ("dq", dq, (nK, n), None), ("dr", dr, (nK,), None),
-                            ("dG", dG, (ml, n), _T2), ("dh", dh, (ml,), None), ("dA", dA, (p, n), _T2),
-                            ("db", db, (p,), None)])
-        return _tangent_out(lambda *o: self.tangent_ptr(*_ptrs(d), *o, space=_lib.HOST), B, (n, p, m))
+        return self._tangent(self.tangent_ptr, QCQPBatch._block, (dP, dq, dr, dG, dh, dA, db))
 
     def tangent_ptr(self, dP=None, dq=None, dr=None, dG=None, dh=None, dA=None, db=None, dx=None, dy=None, dz=None,
                     space=_lib.DEVICE):

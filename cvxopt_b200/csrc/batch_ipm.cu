@@ -4279,43 +4279,44 @@ int batch_tangent(cvxb_batch *b, TanIn d, double *dx, double *dy, double *dz, in
 }
 }  // namespace
 
+namespace {
+// the checks every derivative entry point makes, in this order: a batch (b not NULL), of a kind the entry point
+// differentiates (ok, else the refusal unsup), without an argument its kind lacks (bad, else the refusal arg), solved
+// since its last load.  ok and bad are evaluated by the caller, so they test b before they read it
+int deriv_checks(cvxb_batch *b, const char *what, bool ok, const char *unsup, bool bad = false,
+                 const char *arg = nullptr) {
+    if (!b) { set_error("%s: batch is NULL", what); return CVXB_E_ARG; }
+    if (!ok) { set_error("%s: %s", what, unsup); return CVXB_E_UNSUP; }
+    if (bad) { set_error("%s: %s", what, arg); return CVXB_E_ARG; }
+    if (b->solved) return 0;
+    set_error("%s: no completed cvxb_batch_solve since the last load", what);
+    return CVXB_E_ARG;
+}
+const char *const QC_ONLY = "only QCQP batches (cvxb_batch_create_qcqp) are differentiated here";
+const char *const GP_ONLY = "only GP batches (cvxb_batch_create_gp) are differentiated here";
+const char *const CP_ONLY = "only CP and cpl batches (cvxb_batch_create_cp, _cpl, _sdp_cpl) are differentiated here";
+const char *const CONE_ONLY = "only QP and cone LP batches are differentiated here";
+bool qp_or_lp(const cvxb_batch *b) { return b && (b->kind == Kind::QP || b->kind == Kind::LP); }
+bool lp_with_dP(const cvxb_batch *b, const double *dP) { return b && b->kind == Kind::LP && dP; }
+}  // namespace
+
 int cvxb_batch_adjoint(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                        double *uz, double *dP, double *dG, double *dA, int space) {
-    if (!b) { set_error("batch_adjoint: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QP || b->p.nq > 0 || b->p.ns > 0) {
-        set_error("batch_adjoint: only QP batches whose rows are all 'l' are differentiated");
-        return CVXB_E_UNSUP;
-    }
-    if (!b->solved) { set_error("batch_adjoint: no completed cvxb_batch_solve since the last load"); return CVXB_E_ARG; }
+    CVXB_TRY(deriv_checks(b, "batch_adjoint", b && b->kind == Kind::QP && b->p.nq == 0 && b->p.ns == 0,
+                          "only QP batches whose rows are all 'l' are differentiated"));
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, nullptr, nullptr, dG, dA}, space);
 }
 
 int cvxb_batch_adjoint_qcqp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
                             double *uy, double *uz, double *dP, double *dq, double *dr, double *dG, double *dA,
                             int space) {
-    if (!b) { set_error("batch_adjoint_qcqp: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QC) {
-        set_error("batch_adjoint_qcqp: only QCQP batches (cvxb_batch_create_qcqp) are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (!b->solved) {
-        set_error("batch_adjoint_qcqp: no completed cvxb_batch_solve since the last load");
-        return CVXB_E_ARG;
-    }
+    CVXB_TRY(deriv_checks(b, "batch_adjoint_qcqp", b && b->kind == Kind::QC, QC_ONLY));
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, dq, dr, dG, dA}, space);
 }
 
 int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                           double *uz, double *dF, double *dg, double *dG, double *dA, int space) {
-    if (!b) { set_error("batch_adjoint_gp: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::GP) {
-        set_error("batch_adjoint_gp: only GP batches (cvxb_batch_create_gp) are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (!b->solved) {
-        set_error("batch_adjoint_gp: no completed cvxb_batch_solve since the last load");
-        return CVXB_E_ARG;
-    }
+    CVXB_TRY(deriv_checks(b, "batch_adjoint_gp", b && b->kind == Kind::GP, GP_ONLY));
     AdjGrads d;
     d.dF = dF; d.dg = dg; d.dG = dG; d.dA = dA;
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, d, space);
@@ -4323,16 +4324,7 @@ int cvxb_batch_adjoint_gp(cvxb_batch *b, const double *gx, const double *gy, con
 
 int cvxb_batch_adjoint_cp(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux, double *uy,
                           double *uz, double *dG, double *dA, int space) {
-    if (!b) { set_error("batch_adjoint_cp: batch is NULL"); return CVXB_E_ARG; }
-    if (!b->calls_back()) {
-        set_error("batch_adjoint_cp: only CP and cpl batches (cvxb_batch_create_cp, _cpl, _sdp_cpl) are "
-                  "differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (!b->solved) {
-        set_error("batch_adjoint_cp: no completed cvxb_batch_solve since the last load");
-        return CVXB_E_ARG;
-    }
+    CVXB_TRY(deriv_checks(b, "batch_adjoint_cp", b && b->calls_back(), CP_ONLY));
     AdjGrads d;
     d.dG = dG; d.dA = dA;
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, d, space);
@@ -4340,37 +4332,15 @@ int cvxb_batch_adjoint_cp(cvxb_batch *b, const double *gx, const double *gy, con
 
 int cvxb_batch_adjoint_cone(cvxb_batch *b, const double *gx, const double *gy, const double *gz, double *ux,
                             double *uy, double *uz, double *dP, double *dG, double *dA, int space) {
-    if (!b) { set_error("batch_adjoint_cone: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QP && b->kind != Kind::LP) {
-        set_error("batch_adjoint_cone: only QP and cone LP batches are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (b->kind == Kind::LP && dP) { set_error("batch_adjoint_cone: a cone LP has no P: dP must be NULL"); return CVXB_E_ARG; }
-    if (!b->solved) {
-        set_error("batch_adjoint_cone: no completed cvxb_batch_solve since the last load");
-        return CVXB_E_ARG;
-    }
+    CVXB_TRY(deriv_checks(b, "batch_adjoint_cone", qp_or_lp(b), CONE_ONLY, lp_with_dP(b, dP),
+                          "a cone LP has no P: dP must be NULL"));
     return batch_adjoint(b, gx, gy, gz, ux, uy, uz, AdjGrads{dP, nullptr, nullptr, dG, dA}, space);
 }
 
-namespace {
-// the checks every tangent entry point makes after its kind's
-int tangent_solved(cvxb_batch *b, const char *what) {
-    if (b->solved) return 0;
-    set_error("%s: no completed cvxb_batch_solve since the last load", what);
-    return CVXB_E_ARG;
-}
-}  // namespace
-
 int cvxb_batch_tangent(cvxb_batch *b, const double *dP, const double *dq, const double *dG, const double *dh,
                        const double *dA, const double *db, double *dx, double *dy, double *dz, int space) {
-    if (!b) { set_error("batch_tangent: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QP && b->kind != Kind::LP) {
-        set_error("batch_tangent: only QP and cone LP batches are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (b->kind == Kind::LP && dP) { set_error("batch_tangent: a cone LP has no P: dP must be NULL"); return CVXB_E_ARG; }
-    CVXB_TRY(tangent_solved(b, "batch_tangent"));
+    CVXB_TRY(deriv_checks(b, "batch_tangent", qp_or_lp(b), CONE_ONLY, lp_with_dP(b, dP),
+                          "a cone LP has no P: dP must be NULL"));
     TanIn d{};
     d.dP = dP; d.dq = dq; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
     return batch_tangent(b, d, dx, dy, dz, space);
@@ -4379,12 +4349,7 @@ int cvxb_batch_tangent(cvxb_batch *b, const double *dP, const double *dq, const 
 int cvxb_batch_tangent_qcqp(cvxb_batch *b, const double *dP, const double *dq, const double *dr, const double *dG,
                             const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
                             int space) {
-    if (!b) { set_error("batch_tangent_qcqp: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::QC) {
-        set_error("batch_tangent_qcqp: only QCQP batches (cvxb_batch_create_qcqp) are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    CVXB_TRY(tangent_solved(b, "batch_tangent_qcqp"));
+    CVXB_TRY(deriv_checks(b, "batch_tangent_qcqp", b && b->kind == Kind::QC, QC_ONLY));
     TanIn d{};
     d.dP = dP; d.dq = dq; d.dr = dr; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
     return batch_tangent(b, d, dx, dy, dz, space);
@@ -4392,12 +4357,7 @@ int cvxb_batch_tangent_qcqp(cvxb_batch *b, const double *dP, const double *dq, c
 
 int cvxb_batch_tangent_gp(cvxb_batch *b, const double *dF, const double *dg, const double *dG, const double *dh,
                           const double *dA, const double *db, double *dx, double *dy, double *dz, int space) {
-    if (!b) { set_error("batch_tangent_gp: batch is NULL"); return CVXB_E_ARG; }
-    if (b->kind != Kind::GP) {
-        set_error("batch_tangent_gp: only GP batches (cvxb_batch_create_gp) are differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    CVXB_TRY(tangent_solved(b, "batch_tangent_gp"));
+    CVXB_TRY(deriv_checks(b, "batch_tangent_gp", b && b->kind == Kind::GP, GP_ONLY));
     TanIn d{};
     d.dF = dF; d.dg = dg; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
     return batch_tangent(b, d, dx, dy, dz, space);
@@ -4406,17 +4366,8 @@ int cvxb_batch_tangent_gp(cvxb_batch *b, const double *dF, const double *dg, con
 int cvxb_batch_tangent_cp(cvxb_batch *b, const double *dc, const double *tx, const double *tf, const double *dG,
                           const double *dh, const double *dA, const double *db, double *dx, double *dy, double *dz,
                           int space) {
-    if (!b) { set_error("batch_tangent_cp: batch is NULL"); return CVXB_E_ARG; }
-    if (!b->calls_back()) {
-        set_error("batch_tangent_cp: only CP and cpl batches (cvxb_batch_create_cp, _cpl, _sdp_cpl) are "
-                  "differentiated here");
-        return CVXB_E_UNSUP;
-    }
-    if (b->kind == Kind::CP && dc) {
-        set_error("batch_tangent_cp: a CP batch has no c (its objective is f_0): dc must be NULL");
-        return CVXB_E_ARG;
-    }
-    CVXB_TRY(tangent_solved(b, "batch_tangent_cp"));
+    CVXB_TRY(deriv_checks(b, "batch_tangent_cp", b && b->calls_back(), CP_ONLY, b && b->kind == Kind::CP && dc,
+                          "a CP batch has no c (its objective is f_0): dc must be NULL"));
     TanIn d{};
     d.dq = dc; d.tx = tx; d.tf = tf; d.dG = dG; d.dh = dh; d.dA = dA; d.db = db;
     return batch_tangent(b, d, dx, dy, dz, space);

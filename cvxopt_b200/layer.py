@@ -29,8 +29,9 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .batch import (BATCH_SMAX, ConeLPBatchGroup, CPBatchGroup, CPLBatchGroup, GPBatchGroup, QCQPBatchGroup,
-                    QPBatchGroup, SDPBatchGroup, SDPCPLBatchGroup, SDPQPBatchGroup)
+from .batch import (_FROM_U, _TAIL, BATCH_SMAX, ConeLPBatchGroup, CPBatch, CPBatchGroup, CPLBatchGroup, GPBatch,
+                    GPBatchGroup, QCQPBatch, QCQPBatchGroup, QPBatch, QPBatchGroup, SDPBatchGroup, SDPCPLBatchGroup,
+                    SDPQPBatchGroup, _inverse, _lib_shape)
 
 
 def _typed(named):
@@ -138,16 +139,24 @@ def _check_cone(P, q, G, h, dims, A, b):
     if P is not None and tuple(P.shape) != (B, n, n):
         raise TypeError("P must have shape (%d, %d, %d)" % (B, n, n))
     m, p = _constraint_rows(B, n, G, h, A, b)
+    _cone_dims(dims, m)
+    _on_device(named)
+    return B, n, m, p
+
+
+def _cone_dims(dims, m):
+    """the cone layers' and cpl_layer's dims, checked against the m rows of G and h -> dims with int entries"""
     if not isinstance(dims, dict) or not set(dims) <= {"l", "q", "s"}:
         raise TypeError("dims must be a dictionary with keys 'l', 'q' and 's'")
     if int(dims.get("l", 0)) < 0 or any(int(k) < 1 for k in dims.get("q", [])) or \
             any(not 0 <= int(k) <= BATCH_SMAX for k in dims.get("s", [])):
         raise TypeError("dims: 'l' must be nonnegative, each 'q' size at least 1, each 's' order in 0..%d" % BATCH_SMAX)
-    cdim = int(dims.get("l", 0)) + sum(int(k) for k in dims.get("q", [])) + sum(int(k) ** 2 for k in dims.get("s", []))
+    dims = {"l": int(dims.get("l", 0)), "q": [int(k) for k in dims.get("q", [])],
+            "s": [int(k) for k in dims.get("s", [])]}
+    cdim = dims["l"] + sum(dims["q"]) + sum(k * k for k in dims["s"])
     if cdim != m:
         raise TypeError("dims has %d rows ('l' + sum 'q' + sum 's'²), G and h have %d" % (cdim, m))
-    _on_device(named)
-    return B, n, m, p
+    return dims
 
 
 def _check_gp(K, F, g, G, h, A, b):
@@ -177,9 +186,21 @@ def _rows(t, it):
     return (t if it is None else t.index_select(0, it)).contiguous()
 
 
+def _device(t):
+    """the index of t's CUDA device"""
+    return t.device.index if t.device.index is not None else torch.cuda.current_device()
+
+
+def _layout(ts, block):
+    """tensors ts in load()'s shapes, one per entry of block + _TAIL (block: a batch class's own block), as views in the
+    library's layouts.  An absent or empty one (ml = 0, p = 0) is None: the library takes it as NULL"""
+    return [None if t is None or not t.numel() else t if axes is None else t.permute(axes)
+            for t, (_, _, axes, _) in zip(ts, block + _TAIL)]
+
+
 def _solve(grp, data, load, options, dev, widths):
-    """each part of grp loads its rows of `data` (name -> tensor in the library's layout) through load(part,
-    addresses), the group solves, and the results come back in problem order.  widths: n, m, p.  Returns the parts'
+    """each part of grp loads its rows of `data` (tensors in the library's layouts, None: NULL) through load(part,
+    *addresses), the group solves, and the results come back in problem order.  widths: n, m, p.  Returns the parts'
     row indices on the device (None: all rows), x, s, z, y and the status codes"""
     B = grp.B
     n, m, p = widths
@@ -187,11 +208,11 @@ def _solve(grp, data, load, options, dev, widths):
     keep = []
 
     def loader(r, ix, part):
-        sl = {k: _rows(t, its[r]) for k, t in data.items()}
+        sl = [None if t is None else _rows(t, its[r]) for t in data]
         keep.append(sl)
         # the library reads on its own stream: torch's writes of the slices must be complete
         torch.cuda.current_stream(dev).synchronize()
-        load(part, {k: t.data_ptr() for k, t in sl.items()})
+        load(part, *(None if t is None else t.data_ptr() for t in sl))
     grp.load_ptr_sliced(loader)
     del keep
     grp.solve(**options)
@@ -228,25 +249,51 @@ def _keep(ctx, grp, its, needs, fw=False):
     ctx.set_materialize_grads(False)
 
 
+def _forward(ctx, grp, data, load, options, needs, fw, F=None):
+    """a layer's forward: the new group grp (F: its set_F, for cp and cpl) solves `data`, _layout's views made
+    contiguous, each part loaded by load(part, *addresses), and stays on the device for backward (needs: the inputs'
+    needs_input_grad) and jvp (fw); an error closes it.  ctx.shapes is (B, n, mnl, ml, p).  Returns x, y, z and the
+    status codes"""
+    B, n, mnl, ml, p = ctx.shapes
+    try:
+        if F is not None:
+            grp.set_F(F)
+        its, x, _, z, y, status = _solve(grp, [None if t is None else t.contiguous() for t in data], load, options,
+                                         ctx.dev, (n, mnl + ml, p))
+    except BaseException:
+        grp.close()
+        raise
+    _keep(ctx, grp, its, needs, fw)
+    return x, y, z, status
+
+
+def _split(z, mnl):
+    """z = [znl; zl] (or its tangent) as znl and zl, each a tensor of its own"""
+    return z[:, :mnl].clone(), z[:, mnl:].clone()
+
+
 def _has_tangent(*ts):
     """whether a tensor of ts carries a forward-mode tangent (torch.autograd.forward_ad)"""
     return any(isinstance(t, torch.Tensor) and torch.autograd.forward_ad.unpack_dual(t).tangent is not None
                for t in ts)
 
 
-def _tangent(ctx, dirs, widths, call, dev, needs):
-    """the tangent of every part of the kept group along its rows of dirs (name -> tensor in the library's layout;
-    None: zero), into dx, dy, dz (widths n, p, m) in problem order: call(part, direction addresses, output
-    addresses).  Frees the group unless backward will need it (some input needs a gradient)"""
+def _tangent(ctx, dirs, method, needs):
+    """the tangent of every part of the kept group along its rows of dirs (tensors in the library's layouts, None:
+    zero) by part.method (a tangent *_ptr), into dx, dy, dz in problem order.  Frees the group unless backward will
+    need it (some input needs a gradient)"""
+    B, n, mnl, ml, p = ctx.shapes
     grp, its = ctx.grp, ctx.its
-    f64 = dict(dtype=torch.float64, device=dev)
-    out = [torch.empty((grp.B, w), **f64) for w in widths]
+    f64 = dict(dtype=torch.float64, device=ctx.dev)
+    widths = (n, p, mnl + ml)
+    out = [torch.empty((B, w), **f64) for w in widths]
     try:
         for it, part in zip(its, grp.parts):
-            d = {k: _rows(t, it) for k, t in dirs.items() if t is not None}
+            d = [None if t is None else _rows(t, it) for t in dirs]
             o = out if it is None else [torch.empty((part.B, w), **f64) for w in widths]
-            torch.cuda.current_stream(dev).synchronize()      # the slices are written, the new blocks free
-            call(part, {k: t.data_ptr() for k, t in d.items()}, [t.data_ptr() for t in o])
+            torch.cuda.current_stream(ctx.dev).synchronize()      # the slices are written, the new blocks free
+            getattr(part, method)(*(None if t is None else t.data_ptr() for t in d), *(t.data_ptr() for t in o),
+                                  space=_lib.DEVICE)
             if it is not None:
                 for full, t in zip(out, o):
                     full.index_copy_(0, it, t)
@@ -256,213 +303,146 @@ def _tangent(ctx, dirs, widths, call, dev, needs):
     return out
 
 
-def _adjoint(ctx, grads, shapes, call, dev):
-    """the adjoint of every part of the kept group with its rows of grads (gx, gy, gz; None: zero), into the outputs
-    `shapes` (key -> per-problem shape) in problem order: call(part, gradient addresses, key -> output address).
-    Frees the group"""
+def _adjoint(ctx, grads, shapes, method):
+    """the adjoint of every part of the kept group with its rows of grads (gx, gy, gz; None: zero) by part.method (an
+    adjoint *_ptr), into outputs of the per-problem `shapes` in the call's order (None: NULL) in problem order.  Frees
+    the group"""
     grp, its = ctx.grp, ctx.its
-    f64 = dict(dtype=torch.float64, device=dev)
-    out = {k: torch.empty((grp.B,) + s, **f64) for k, s in shapes.items()}
+    f64 = dict(dtype=torch.float64, device=ctx.dev)
+    out = [None if s is None else torch.empty((grp.B,) + s, **f64) for s in shapes]
     try:
         for it, part in zip(its, grp.parts):
             g = [None if t is None else _rows(t, it) for t in grads]
-            o = out if it is None else {k: torch.empty((part.B,) + s, **f64) for k, s in shapes.items()}
-            torch.cuda.current_stream(dev).synchronize()      # the slices are written, the new blocks free
-            call(part, [None if t is None else t.data_ptr() for t in g], {k: t.data_ptr() for k, t in o.items()})
+            o = out if it is None else [None if s is None else torch.empty((part.B,) + s, **f64) for s in shapes]
+            torch.cuda.current_stream(ctx.dev).synchronize()      # the slices are written, the new blocks free
+            getattr(part, method)(*(None if t is None else t.data_ptr() for t in g + o), space=_lib.DEVICE)
             if it is not None:
-                for k, t in o.items():
-                    out[k].index_copy_(0, it, t)
+                for full, t in zip(out, o):
+                    if t is not None:
+                        full.index_copy_(0, it, t)
     finally:
         grp.close()
     return out
 
 
-class _QPLayer(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, P, q, G, h, A, b, nsub, options):
-        options_fw = options.pop("_fw")
-        B, n, m, p = ctx.shapes = _check(P, q, G, h, A, b, options.pop("dims", None))
-        dev = P.device
-        # the layouts the library loads: P, G and A column-major per problem
-        data = {"P": P.transpose(1, 2).contiguous(), "q": q.contiguous(), "G": G.transpose(1, 2).contiguous(),
-                "h": h.contiguous()}
-        if p:
-            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
-        grp = QPBatchGroup(B, n, m, dev.index if dev.index is not None else torch.cuda.current_device(), nsub,
-                           p=p)
-        try:
-            its, x, _, z, y, status = _solve(
-                grp, data, lambda part, a: part.load_ptr(a["P"], a["q"], a["G"], a["h"], _lib.DEVICE,
-                                                         a.get("A"), a.get("b")),
-                options, dev, (n, m, p))
-        except BaseException:
-            grp.close()
-            raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:6], options_fw)
-        ctx.dev = dev
-        return x, y, z, status
+def _grads(ctx, method, block, needs, gx, gy, gznl, gzl, theta=False):
+    """a layer's backward: the gradients of its inputs, one per entry of block + _TAIL (needs: which need one), from
+    those of x, y, znl and zl (None: zero) by the kept group's adjoint `method`, which writes ux, uy, uz and then the
+    entries marked as written.  Those come as views in load()'s layouts, the others by _FROM_U; an empty input that
+    needs a gradient gets zeros, one that needs none gets None.  With theta, ux and uznl follow for _theta_grads.
+    Frees the group"""
+    B, n, mnl, ml, p = ctx.shapes
+    f64 = dict(dtype=torch.float64, device=ctx.dev)
+    part = ctx.grp.parts[0]
+    inputs = [(name[1:], (B,) + shape(part), axes, writes) for name, shape, axes, writes in block + _TAIL]
+    want = {k for (k, s, _, _), nd in zip(inputs, needs) if nd and all(s)}
+    want |= {"ux", "uznl"} if theta and mnl else {"ux"} if theta else set()
+    own = [(k, s, axes) for k, s, axes, writes in inputs if writes]
+    fromu = {_FROM_U[k][0] for k in want if k not in {k for k, _, _ in own}}
+    shapes = [(w,) if i in fromu else None for i, w in enumerate((n, p, mnl + ml))]
+    shapes += [_lib_shape(s[1:], axes) if k in want else None for k, s, axes in own]
+    gz = None
+    if mnl + ml and (gznl is not None or gzl is not None):
+        gz = [torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml)) if k]
+        gz = gz[0] if len(gz) == 1 else torch.cat(gz, 1)
+    out = _adjoint(ctx, (gx, gy if p else None, gz), shapes, method)
+    u, got = out[:3], dict(zip((k for k, _, _ in own), out[3:]))
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, gx, gy, gz, _gstatus):
-        return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_ptr), None, None)
-
-    @staticmethod
-    def jvp(ctx, dP, dq, dG, dh, dA, db, _nsub, _options):
-        return (*_qp_tangent(ctx, dP, dq, dG, dh, dA, db), None)
-
-
-def _qp_grads(ctx, gx, gy, gz, adjoint):
-    """the gradients of P, q, G, h, A and b for qp_layer and the cone layers (a cone LP: P None, q its c) from those of
-    x, y and z; adjoint(part) is the part's adjoint_ptr or adjoint_cone_ptr"""
-    B, n, m, p = ctx.shapes
-    need = dict(zip(("P", "q", "G", "h", "A", "b"), ctx.needs_input_grad[:6]))
-    dev = gx.device if gx is not None else gz.device if gz is not None else gy.device
-    # C's outputs ux, uy, uz, dP, dG, dA in problem order; the matrices column-major per problem
-    shapes = {"q": (n,), "b": (p,), "h": (m,), "P": (n, n), "G": (n, m), "A": (n, p)}
-    shapes = {k: s for k, s in shapes.items() if need[k] and (p or k not in ("b", "A"))}
-    out = _adjoint(ctx, (gx, gy if p else None, gz if m else None), shapes,
-                   lambda part, g, o: adjoint(part)(*g, *(o.get(k) for k in ("q", "b", "h", "P", "G", "A")),
-                                                    space=_lib.DEVICE), dev)
-    f64 = dict(dtype=torch.float64, device=dev)
-    grads = {"q": lambda t: -t, "b": lambda t: t, "h": lambda t: t}
+    def from_u(k):
+        return _FROM_U[k][1](u[_FROM_U[k][0]], mnl)
     res = []
-    for key in ("P", "q", "G", "h", "A", "b"):
-        if key not in out:
-            res.append(torch.zeros((B, 0) if key == "b" else (B, 0, n), **f64) if need[key] else None)
-        elif key in grads:
-            res.append(grads[key](out[key]))
+    for (k, s, axes, writes), nd in zip(inputs, needs):
+        if not nd:
+            res.append(None)
+        elif not all(s):
+            res.append(torch.zeros(s, **f64))
+        elif writes:
+            res.append(got[k] if axes is None else got[k].permute(_inverse(axes)))
         else:
-            res.append(out[key].transpose(1, 2))
+            res.append(from_u(k))
+    if theta:
+        res += [from_u("ux"), from_u("uznl") if mnl else torch.zeros((B, 0), **f64)]
     return res
 
 
-def _qp_tangent(ctx, dP, dq, dG, dh, dA, db):
-    """the tangents of x, y and z for qp_layer and the cone layers (a cone LP: dP None, dq its dc) along the inputs'
-    forward-mode tangents (None: zero), through each part's tangent_ptr"""
-    B, n, m, p = ctx.shapes
-    dev = ctx.dev
-    # the layouts the library loads: P, G and A column-major per problem
-    dirs = {"P": None if dP is None else dP.transpose(1, 2), "q": dq,
-            "G": None if dG is None or not m else dG.transpose(1, 2), "h": dh if m else None,
-            "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
-    return _tangent(ctx, dirs, (n, p, m),
-                    lambda part, d, o: part.tangent_ptr(*(d.get(k) for k in ("P", "q", "G", "h", "A", "b")), *o,
-                                                        space=_lib.DEVICE),
-                    dev, ctx.needs_input_grad[:6])
+def _load_qp(part, P, q, G, h, A, b):
+    """a QP or cone LP part's load_ptr (a cone LP: P None)"""
+    part.load_ptr(*((q, G, h) if P is None else (P, q, G, h)), _lib.DEVICE, A, b)
 
 
-class _ConeLayer(torch.autograd.Function):
+class _QPLayer(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, P, q, G, h, A, b, dims, nsub, options):
-        options_fw = options.pop("_fw")
-        B, n, m, p = ctx.shapes = _check_cone(P, q, G, h, dims, A, b)
-        dev = q.device
-        device = dev.index if dev.index is not None else torch.cuda.current_device()
-        # the layouts the library loads: P, G and A column-major per problem
-        data = {"q": q.contiguous(), "G": G.transpose(1, 2).contiguous(), "h": h.contiguous()}
-        if P is not None:
-            data["P"] = P.transpose(1, 2).contiguous()
-        if p:
-            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
-        if P is not None:            # coneqp_batch's group
-            grp, head = SDPQPBatchGroup(B, n, dims, p, device, nsub), ("P", "q", "G", "h")
-        elif dims.get("s"):          # sdp_batch's
-            grp, head = SDPBatchGroup(B, n, dims, p, device, nsub), ("q", "G", "h")
-        else:                        # conelp_batch's
-            grp = ConeLPBatchGroup(B, n, m, device, nsub, {"l": dims.get("l", 0), "q": dims.get("q", [])}, p)
-            head = ("q", "G", "h")
-        try:
-            its, x, _, z, y, status = _solve(
-                grp, data, lambda part, a: part.load_ptr(*(a[k] for k in head), _lib.DEVICE, a.get("A"), a.get("b")),
-                options, dev, (n, m, p))
-        except BaseException:
-            grp.close()
-            raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:6], options_fw)
-        ctx.dev = dev
-        return x, y, z, status
+    def forward(ctx, P, q, G, h, A, b, nsub, options):
+        fw = options.pop("_fw")
+        B, n, m, p = _check(P, q, G, h, A, b, options.pop("dims", None))
+        ctx.shapes, ctx.dev = (B, n, 0, m, p), P.device
+        data = _layout((P, q, G, h, A, b), QPBatch._block)
+        grp = QPBatchGroup(B, n, m, _device(P), nsub, p=p)
+        return _forward(ctx, grp, data, _load_qp, options, ctx.needs_input_grad[:6], fw)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gz, _gstatus):
-        return (*_qp_grads(ctx, gx, gy, gz, lambda part: part.adjoint_cone_ptr), None, None, None)
+        return (*_grads(ctx, "adjoint_ptr", QPBatch._block, ctx.needs_input_grad[:6], gx, gy, None, gz), None, None)
+
+    @staticmethod
+    def jvp(ctx, dP, dq, dG, dh, dA, db, _nsub, _options):
+        dirs = _layout((dP, dq, dG, dh, dA, db), QPBatch._block)
+        return (*_tangent(ctx, dirs, "tangent_ptr", ctx.needs_input_grad[:6]), None)
+
+
+class _ConeLayer(torch.autograd.Function):
+    # a cone LP: P None and q its c, in dq's place as the library takes it
+    @staticmethod
+    def forward(ctx, P, q, G, h, A, b, dims, nsub, options):
+        fw = options.pop("_fw")
+        B, n, m, p = _check_cone(P, q, G, h, dims, A, b)
+        ctx.shapes, ctx.dev = (B, n, 0, m, p), q.device
+        data = _layout((P, q, G, h, A, b), QPBatch._block)
+        if P is not None:            # coneqp_batch's group
+            grp = SDPQPBatchGroup(B, n, dims, p, _device(q), nsub)
+        elif dims.get("s"):          # sdp_batch's
+            grp = SDPBatchGroup(B, n, dims, p, _device(q), nsub)
+        else:                        # conelp_batch's
+            grp = ConeLPBatchGroup(B, n, m, _device(q), nsub, {"l": dims.get("l", 0), "q": dims.get("q", [])}, p)
+        return _forward(ctx, grp, data, _load_qp, options, ctx.needs_input_grad[:6], fw)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gx, gy, gz, _gstatus):
+        return (*_grads(ctx, "adjoint_cone_ptr", QPBatch._block, ctx.needs_input_grad[:6], gx, gy, None, gz), None,
+                None, None)
 
     @staticmethod
     def jvp(ctx, dP, dq, dG, dh, dA, db, _dims, _nsub, _options):
-        return (*_qp_tangent(ctx, dP, dq, dG, dh, dA, db), None)
+        dirs = _layout((dP, dq, dG, dh, dA, db), QPBatch._block)
+        return (*_tangent(ctx, dirs, "tangent_ptr", ctx.needs_input_grad[:6]), None)
 
 
 class _QCQPLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, P, q, r, G, h, A, b, x0, nsub, options):
         fw = options.pop("_fw")
-        B, mnl, n, ml, p = ctx.shapes = _check_qcqp(P, q, r, G, h, A, b, x0, options.pop("dims", None))
-        dev = P.device
-        # the layouts the library loads: per problem P's (mnl + 1) n x n column-major stack, G and A column-major
-        data = {"P": P.permute(0, 3, 1, 2).contiguous(), "q": q.contiguous(), "r": r.contiguous()}
-        if x0 is not None:
-            data["x0"] = x0.contiguous()
-        if ml:
-            data.update(G=G.transpose(1, 2).contiguous(), h=h.contiguous())
-        if p:
-            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
-        grp = QCQPBatchGroup(B, n, mnl, ml, p, dev.index if dev.index is not None else torch.cuda.current_device(),
-                             nsub)
-        try:
-            its, x, _, z, y, status = _solve(
-                grp, data, lambda part, a: part.load_ptr(a["P"], a["q"], a["r"], a.get("x0"), a.get("G"), a.get("h"),
-                                                         _lib.DEVICE, a.get("A"), a.get("b")),
-                options, dev, (n, mnl + ml, p))
-        except BaseException:
-            grp.close()
-            raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[:7], fw)
-        ctx.dev = dev
-        return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
+        B, mnl, n, ml, p = _check_qcqp(P, q, r, G, h, A, b, x0, options.pop("dims", None))
+        ctx.shapes, ctx.dev = (B, n, mnl, ml, p), P.device
+        data = _layout((P, q, r, G, h, A, b), QCQPBatch._block) + [x0]
+        grp = QCQPBatchGroup(B, n, mnl, ml, p, _device(P), nsub)
+        x, y, z, status = _forward(
+            ctx, grp, data, lambda part, P, q, r, G, h, A, b, x0: part.load_ptr(P, q, r, x0, G, h, _lib.DEVICE, A, b),
+            options, ctx.needs_input_grad[:7], fw)
+        return (x, y, *_split(z, mnl), status)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gznl, gzl, _gstatus):
-        B, mnl, n, ml, p = ctx.shapes
-        nK, m = mnl + 1, mnl + ml
-        need = dict(zip(("P", "q", "r", "G", "h", "A", "b"), ctx.needs_input_grad[:7]))
-        dev = next(t.device for t in (gx, gy, gznl, gzl) if t is not None)
-        f64 = dict(dtype=torch.float64, device=dev)
-        gz = None
-        if m and (gznl is not None or gzl is not None):
-            gz = torch.cat([torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml))], 1)
-        # C's outputs uy, uz (h: its 'l' rows), dP, dq, dr, dG, dA in problem order; dP, dG, dA column-major
-        shapes = {"b": (p,), "h": (m,), "P": (n, nK, n), "q": (nK, n), "r": (nK,), "G": (n, ml), "A": (n, p)}
-        shapes = {k: s for k, s in shapes.items() if need[k] and (ml or k not in ("G", "h")) and
-                  (p or k not in ("A", "b"))}
-        out = _adjoint(ctx, (gx, gy if p else None, gz), shapes,
-                       lambda part, g, o: part.adjoint_ptr(*g, None, *(o.get(k) for k in
-                                                                       ("b", "h", "P", "q", "r", "G", "A")),
-                                                           space=_lib.DEVICE), dev)
-        view = {"P": lambda t: t.permute(0, 2, 3, 1), "h": lambda t: t[:, mnl:], "G": lambda t: t.transpose(1, 2),
-                "A": lambda t: t.transpose(1, 2)}
-        empty = {"G": (B, 0, n), "h": (B, 0), "A": (B, 0, n), "b": (B, 0)}
-        res = []
-        for key in ("P", "q", "r", "G", "h", "A", "b"):
-            if key in out:
-                res.append(view.get(key, lambda t: t)(out[key]))
-            else:
-                res.append(torch.zeros(empty[key], **f64) if need[key] else None)
-        return (*res, None, None, None)
+        return (*_grads(ctx, "adjoint_ptr", QCQPBatch._block, ctx.needs_input_grad[:7], gx, gy, gznl, gzl), None,
+                None, None)
 
     @staticmethod
     def jvp(ctx, dP, dq, dr, dG, dh, dA, db, _dx0, _nsub, _options):
-        B, mnl, n, ml, p = ctx.shapes
-        # the layouts the library loads: P's (mnl + 1) n x n column-major stack, G and A column-major
-        dirs = {"P": None if dP is None else dP.permute(0, 3, 1, 2), "q": dq, "r": dr,
-                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
-                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
-        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
-                              lambda part, d, o: part.tangent_ptr(*(d.get(k) for k in ("P", "q", "r", "G", "h", "A",
-                                                                                       "b")), *o, space=_lib.DEVICE),
-                              ctx.dev, ctx.needs_input_grad[:7])
-        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+        dirs = _layout((dP, dq, dr, dG, dh, dA, db), QCQPBatch._block)
+        dx, dy, dz = _tangent(ctx, dirs, "tangent_ptr", ctx.needs_input_grad[:7])
+        return (dx, dy, *_split(dz, ctx.shapes[2]), None)
 
 
 class _GPLayer(torch.autograd.Function):
@@ -471,70 +451,25 @@ class _GPLayer(torch.autograd.Function):
         fw = options.pop("_fw")
         B, n, ml, p = _check_gp(K, F, g, G, h, A, b)
         mnl = len(K) - 1
-        ctx.shapes = B, n, sum(K), mnl, ml, p
-        dev = F.device
-        # the layouts the library loads: F, G and A column-major per problem
-        data = {"F": F.transpose(1, 2).contiguous(), "g": g.contiguous()}
-        if ml:
-            data.update(G=G.transpose(1, 2).contiguous(), h=h.contiguous())
-        if p:
-            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
-        grp = GPBatchGroup(B, n, K, ml, p, dev.index if dev.index is not None else torch.cuda.current_device(), nsub)
-        try:
-            its, x, _, z, y, status = _solve(
-                grp, data, lambda part, a: part.load_ptr(a["F"], a["g"], a.get("G"), a.get("h"), _lib.DEVICE,
-                                                         a.get("A"), a.get("b")),
-                options, dev, (n, mnl + ml, p))
-        except BaseException:
-            grp.close()
-            raise
-        _keep(ctx, grp, its, ctx.needs_input_grad[1:7], fw)
-        ctx.dev = dev
-        return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
+        ctx.shapes, ctx.dev = (B, n, mnl, ml, p), F.device
+        data = _layout((F, g, G, h, A, b), GPBatch._block)
+        grp = GPBatchGroup(B, n, K, ml, p, _device(F), nsub)
+        x, y, z, status = _forward(
+            ctx, grp, data, lambda part, F, g, G, h, A, b: part.load_ptr(F, g, G, h, _lib.DEVICE, A, b), options,
+            ctx.needs_input_grad[1:7], fw)
+        return (x, y, *_split(z, mnl), status)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gznl, gzl, _gstatus):
-        B, n, S, mnl, ml, p = ctx.shapes
-        m = mnl + ml
-        need = dict(zip(("F", "g", "G", "h", "A", "b"), ctx.needs_input_grad[1:7]))
-        dev = next(t.device for t in (gx, gy, gznl, gzl) if t is not None)
-        f64 = dict(dtype=torch.float64, device=dev)
-        gz = None
-        if m and (gznl is not None or gzl is not None):
-            gz = torch.cat([torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml))], 1)
-        # C's outputs uy, uz (h: its 'l' rows), dF, dg, dG, dA in problem order; dF, dG, dA column-major
-        shapes = {"b": (p,), "h": (m,), "F": (n, S), "g": (S,), "G": (n, ml), "A": (n, p)}
-        shapes = {k: s for k, s in shapes.items() if need[k] and (ml or k not in ("G", "h")) and
-                  (p or k not in ("A", "b"))}
-        out = _adjoint(ctx, (gx, gy if p else None, gz), shapes,
-                       lambda part, g, o: part.adjoint_gp_ptr(*g, None, *(o.get(k) for k in
-                                                                          ("b", "h", "F", "g", "G", "A")),
-                                                              space=_lib.DEVICE), dev)
-        view = {"F": lambda t: t.transpose(1, 2), "h": lambda t: t[:, mnl:], "G": lambda t: t.transpose(1, 2),
-                "A": lambda t: t.transpose(1, 2)}
-        empty = {"G": (B, 0, n), "h": (B, 0), "A": (B, 0, n), "b": (B, 0)}
-        res = []
-        for key in ("F", "g", "G", "h", "A", "b"):
-            if key in out:
-                res.append(view.get(key, lambda t: t)(out[key]))
-            else:
-                res.append(torch.zeros(empty[key], **f64) if need[key] else None)
-        return (None, *res, None, None)
+        return (None, *_grads(ctx, "adjoint_gp_ptr", GPBatch._block, ctx.needs_input_grad[1:7], gx, gy, gznl, gzl),
+                None, None)
 
     @staticmethod
     def jvp(ctx, _dK, dF, dg, dG, dh, dA, db, _nsub, _options):
-        B, n, S, mnl, ml, p = ctx.shapes
-        # the layouts the library loads: F, G and A column-major per problem
-        dirs = {"F": None if dF is None else dF.transpose(1, 2), "g": dg,
-                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
-                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
-        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
-                              lambda part, d, o: part.tangent_gp_ptr(*(d.get(k) for k in ("F", "g", "G", "h", "A",
-                                                                                          "b")), *o,
-                                                                     space=_lib.DEVICE),
-                              ctx.dev, ctx.needs_input_grad[1:7])
-        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+        dirs = _layout((dF, dg, dG, dh, dA, db), GPBatch._block)
+        dx, dy, dz = _tangent(ctx, dirs, "tangent_gp_ptr", ctx.needs_input_grad[1:7])
+        return (dx, dy, *_split(dz, ctx.shapes[2]), None)
 
 
 def qp_layer(P, q, G, h, A=None, b=None, nsub=None, **options):
@@ -664,19 +599,7 @@ def _check_cp(F, params, c, G, h, dims, A, b, cpl):
     if not cpl:
         _dims(dims, ml, "cp_layer")
     else:
-        if dims is None:
-            dims = {"l": ml}
-        if not isinstance(dims, dict) or not set(dims) <= {"l", "q", "s"}:
-            raise TypeError("dims must be a dictionary with keys 'l', 'q' and 's'")
-        if int(dims.get("l", 0)) < 0 or any(int(k) < 1 for k in dims.get("q", [])) or \
-                any(not 0 <= int(k) <= BATCH_SMAX for k in dims.get("s", [])):
-            raise TypeError("dims: 'l' must be nonnegative, each 'q' size at least 1, each 's' order in 0..%d"
-                            % BATCH_SMAX)
-        gdims = {"l": int(dims.get("l", 0)), "q": [int(k) for k in dims.get("q", [])],
-                 "s": [int(k) for k in dims.get("s", [])]}
-        cdim = gdims["l"] + sum(gdims["q"]) + sum(k * k for k in gdims["s"])
-        if cdim != ml:
-            raise TypeError("dims has %d rows ('l' + sum 'q' + sum 's'²), G and h have %d" % (cdim, ml))
+        gdims = _cone_dims({"l": ml} if dims is None else dims, ml)
     if p > n:
         raise ValueError("Rank(A) < p or Rank([H(x); A; Df(x); G]) < n")
     if cpl and mnl + ml == 0:
@@ -695,93 +618,44 @@ class _CPLayer(torch.autograd.Function):
     def forward(ctx, F, c, G, h, A, b, info, nsub, options, *params):
         B, n, mnl, ml, p, x0, dims = info
         fw = options.pop("_fw")
-        cpl = c is not None
-        dev = x0.device
-        device = dev.index if dev.index is not None else torch.cuda.current_device()
-        ctx.shapes = B, n, mnl, ml, p, cpl
-        # F sees the params detached; the data in the layouts the library loads: G and A column-major per problem
+        ctx.shapes, ctx.dev, ctx.cpl = (B, n, mnl, ml, p), x0.device, c is not None
+        # F sees the params detached
         det = tuple(t.detach() for t in params)
 
         def Fd(x=None, z=None, idx=None):
             return F(x, idx=idx, params=det) if z is None else F(x, z, idx=idx, params=det)
-        data = {"x0": x0}
-        if cpl:
-            data["c"] = c.contiguous()
-        if ml:
-            data.update(G=G.transpose(1, 2).contiguous(), h=h.contiguous())
-        if p:
-            data.update(A=A.transpose(1, 2).contiguous(), b=b.contiguous())
-        if not cpl:
-            grp = CPBatchGroup(B, n, mnl, ml, p, device, nsub)
-            load = lambda part, a: part.load_ptr(a["x0"], a.get("G"), a.get("h"), _lib.DEVICE,  # noqa: E731
-                                                 a.get("A"), a.get("b"))
+        data = _layout((c, G, h, A, b), CPBatch._block[:1]) + [x0]
+        if c is None:
+            grp = CPBatchGroup(B, n, mnl, ml, p, _device(x0), nsub)
         else:
-            grp = (SDPCPLBatchGroup if dims["s"] else CPLBatchGroup)(B, n, mnl, dims, p, device, nsub)
-            load = lambda part, a: part.load_ptr(a["c"], a["x0"], a.get("G"), a.get("h"), _lib.DEVICE,  # noqa: E731
-                                                 a.get("A"), a.get("b"))
-        try:
-            grp.set_F(Fd)
-            its, x, _, z, y, status = _solve(grp, data, load, options, dev, (n, mnl + ml, p))
-        except BaseException:
-            grp.close()
-            raise
+            grp = (SDPCPLBatchGroup if dims["s"] else CPLBatchGroup)(B, n, mnl, dims, p, _device(x0), nsub)
         needs = ctx.needs_input_grad
-        _keep(ctx, grp, its, needs[1:6] + needs[9:], fw)
+        x, y, z, status = _forward(
+            ctx, grp, data, lambda part, c, G, h, A, b, x0: part.load_ptr(*(() if c is None else (c,)), x0, G, h,
+                                                                          _lib.DEVICE, A, b),
+            options, needs[1:6] + needs[9:], fw, Fd)
         if any(needs[9:]) or fw:             # the theta call's point and multipliers, and the detached params
             ctx.F, ctx.params, ctx.x, ctx.znl = F, det, x.clone(), z[:, :mnl].clone()
-        ctx.dev = dev
-        return x, y, z[:, :mnl].clone(), z[:, mnl:].clone(), status
+        return (x, y, *_split(z, mnl), status)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gx, gy, gznl, gzl, _gstatus):
-        B, n, mnl, ml, p, cpl = ctx.shapes
-        m = mnl + ml
-        needs = ctx.needs_input_grad
-        need = dict(zip(("c", "G", "h", "A", "b"), needs[1:6]))
-        needp = needs[9:]
+        needp = ctx.needs_input_grad[9:]
         theta = any(needp)
-        dev = next(t.device for t in (gx, gy, gznl, gzl) if t is not None)
-        f64 = dict(dtype=torch.float64, device=dev)
-        gz = None
-        if m and (gznl is not None or gzl is not None):
-            gz = torch.cat([torch.zeros((B, k), **f64) if t is None else t for t, k in ((gznl, mnl), (gzl, ml))], 1)
-        # C's outputs ux, uy, uz ([uznl; h]), dG, dA in problem order; dG and dA column-major
-        shapes = {"ux": (n,) if need["c"] or theta else None, "b": (p,) if need["b"] and p else None,
-                  "uz": (m,) if m and ((need["h"] and ml) or (theta and mnl)) else None,
-                  "G": (n, ml) if need["G"] and ml else None, "A": (n, p) if need["A"] and p else None}
-        shapes = {k: s for k, s in shapes.items() if s is not None}
-        out = _adjoint(ctx, (gx, gy if p else None, gz), shapes,
-                       lambda part, g, o: part.adjoint_cp_ptr(*g, *(o.get(k) for k in ("ux", "b", "uz", "G", "A")),
-                                                              space=_lib.DEVICE), dev)
-        res = {"c": -out["ux"] if need["c"] else None}
-        for key, full, view in (("G", (B, ml, n), lambda t: t.transpose(1, 2)), ("h", (B, ml), lambda t: t[:, mnl:]),
-                                ("A", (B, p, n), lambda t: t.transpose(1, 2)), ("b", (B, p), lambda t: t)):
-            src = out.get("uz" if key == "h" else key)
-            res[key] = None if not need[key] else view(src) if src is not None else torch.zeros(full, **f64)
-        dparams = [None] * len(needp)
-        if theta:
-            dparams = _theta_grads(ctx, out["ux"], out["uz"][:, :mnl] if mnl else torch.zeros((B, 0), **f64),
-                                   cpl, needp)
-        return (None, res["c"], res["G"], res["h"], res["A"], res["b"], None, None, None, *dparams)
+        g = _grads(ctx, "adjoint_cp_ptr", CPBatch._block[:1], ctx.needs_input_grad[1:6], gx, gy, gznl, gzl, theta)
+        dparams = _theta_grads(ctx, *g[5:], ctx.cpl, needp) if theta else [None] * len(needp)
+        return (None, *g[:5], None, None, None, *dparams)
 
     @staticmethod
     def jvp(ctx, _dF, dc, dG, dh, dA, db, _dinfo, _nsub, _options, *dparams):
-        B, n, mnl, ml, p, cpl = ctx.shapes
         needs = ctx.needs_input_grad
         tx = tf = None
         if any(t is not None for t in dparams):
-            tx, tf = _theta_tangents(ctx, dparams, cpl)
-        # the layouts the library loads: G and A column-major per problem
-        dirs = {"c": dc if cpl else None, "tx": tx, "tf": tf if mnl else None,
-                "G": None if dG is None or not ml else dG.transpose(1, 2), "h": dh if ml else None,
-                "A": None if dA is None or not p else dA.transpose(1, 2), "b": db if p else None}
-        dx, dy, dz = _tangent(ctx, dirs, (n, p, mnl + ml),
-                              lambda part, d, o: part.tangent_cp_ptr(*(d.get(k) for k in ("c", "tx", "tf", "G", "h",
-                                                                                          "A", "b")), *o,
-                                                                     space=_lib.DEVICE),
-                              ctx.dev, needs[1:6] + needs[9:])
-        return dx, dy, dz[:, :mnl].clone(), dz[:, mnl:].clone(), None
+            tx, tf = _theta_tangents(ctx, dparams, ctx.cpl)
+        dirs = _layout((dc, tx, tf, dG, dh, dA, db), CPBatch._block)
+        dx, dy, dz = _tangent(ctx, dirs, "tangent_cp_ptr", needs[1:6] + needs[9:])
+        return (dx, dy, *_split(dz, ctx.shapes[2]), None)
 
 
 def _theta_tangents(ctx, dparams, cpl):
