@@ -3,7 +3,7 @@ NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -Wno-unused-function
 SRC := cvxopt_b200/csrc
-OBJ := $(SRC)/gemm_dmma.o $(SRC)/chol.o $(SRC)/cone.o $(SRC)/kkt_api.o $(SRC)/blocks_api.o $(SRC)/batch_ipm.o $(SRC)/cone_vec.o $(SRC)/ozaki_syrk.o $(SRC)/nt_scaling.o $(SRC)/kkt_qr.o $(SRC)/kkt_ldl.o
+OBJ := $(SRC)/gemm_dmma.o $(SRC)/chol.o $(SRC)/cone.o $(SRC)/kkt_api.o $(SRC)/blocks_api.o $(SRC)/batch_ipm.o $(SRC)/cone_vec.o $(SRC)/ozaki_syrk.o $(SRC)/nt_scaling.o $(SRC)/kkt_qr.o $(SRC)/kkt_ldl.o $(SRC)/kkt_sparse.o
 LIB := cvxopt_b200/libcvxopt_b200.so
 # CPython extension mirroring cvxopt.misc_solvers over the C ABI (host side of the drop-in boundary)
 PYTHON ?= python

@@ -57,6 +57,9 @@ _SIGS = {
     "cvxb_sync": (C.c_int, []),
     "cvxb_kkt_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(Dims),
                                   C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]),
+    "cvxb_kkt_create_sparse": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(Dims), C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_int]),
     "cvxb_kkt_destroy": (None, [C.c_void_p]),
     "cvxb_kkt_reset": (C.c_int, [C.c_void_p]),
     "cvxb_kkt_set_method": (C.c_int, [C.c_void_p, C.c_int, C.c_double]),

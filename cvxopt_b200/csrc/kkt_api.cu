@@ -200,7 +200,7 @@ int kkt_unpack_z(cvxb_kkt *k, double *zd) {
 // 'q' and 's' rows of Gs = pack(W^{-T} G)                       (misc.py:1267-1272, :1614-1616)
 int kkt_scale_pack_G(cvxb_kkt *k, double *dst, long long ldd) {
     const ConeLayout &c = k->cone;
-    const double *Gq = k->G + c.mnl + c.ml;
+    const double *Gq = kkt_G_qs(k);
     if (c.nq > 0) CVXB_TRY(scale_q(c, k->W, Gq, k->ldg, dst, ldd, k->n, true, k->st));
     if (c.ns > 0) {
         // W^{-T} on an 's' block: rti' * mat(x) * rti  (trans 'T', inverse 'I'), then pack2
@@ -220,7 +220,8 @@ static int chol_solve(cvxb_kkt *k, double *xd, double *ydv) {
     const double *K = k->Kmat.p, *inv = k->inv.p, *Gs = k->Gs.p;
     double *bzp = k->bzp.p, *ws = k->gemv_ws.p;
     // x := x + Gs' bzp                                            (misc.py:1311)
-    if (c.ml > 0) CVXB_TRY(gemv_t(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, bzp + c.mnl, 1.0, 1.0, xd, st));
+    if (c.ml > 0 && k->sp) CVXB_TRY(kkt_sparse_mv(k, true, k->W.di, bzp + c.mnl, 1.0, 1.0, xd));
+    else if (c.ml > 0) CVXB_TRY(gemv_t(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, bzp + c.mnl, 1.0, 1.0, xd, st));
     if (c.mnl > 0) CVXB_TRY(gemv_t(c.mnl, n, Gs, k->ldgs, nullptr, bzp, 1.0, 1.0, xd, st));
     if (k->nrest - c.mnl > 0)
         CVXB_TRY(gemv_t(k->nrest - c.mnl, n, Gs + c.mnl, k->ldgs, nullptr, bzp + c.mnl + c.ml, 1.0, 1.0, xd, st));
@@ -242,7 +243,8 @@ static int chol_solve(cvxb_kkt *k, double *xd, double *ydv) {
         CVXB_TRY(trsv_lower(n, K, (int)ldk, inv, xd, true, k->cw, st));                    // x := L^{-T} x
     }
     // bzp := Gs x - bzp                                           (misc.py:1344)
-    if (c.ml > 0) CVXB_TRY(gemv_n(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, xd, 1.0, -1.0, bzp + c.mnl, ws, st));
+    if (c.ml > 0 && k->sp) CVXB_TRY(kkt_sparse_mv(k, false, k->W.di, xd, 1.0, -1.0, bzp + c.mnl));
+    else if (c.ml > 0) CVXB_TRY(gemv_n(c.ml, n, k->G + c.mnl, k->ldg, k->W.di, xd, 1.0, -1.0, bzp + c.mnl, ws, st));
     if (c.mnl > 0) CVXB_TRY(gemv_n(c.mnl, n, Gs, k->ldgs, nullptr, xd, 1.0, -1.0, bzp, ws, st));
     if (k->nrest - c.mnl > 0)
         CVXB_TRY(gemv_n(k->nrest - c.mnl, n, Gs + c.mnl, k->ldgs, nullptr, xd, 1.0, -1.0, bzp + c.mnl + c.ml, ws, st));
@@ -281,6 +283,93 @@ int trsm_lower_left(int n, const double *L, long long ldl, const double *inv, do
     return 0;
 }
 
+}  // namespace cvxb
+
+namespace {
+// checks of the arguments every create shares, before the device is touched
+int kkt_check_args(cvxb_kkt **out, int n, int p, const double *A, int lda) {
+    if (!out) { set_error("kkt_create: out is NULL"); return CVXB_E_ARG; }
+    *out = nullptr;
+    if (n < 0 || p < 0) { set_error("kkt_create: negative size"); return CVXB_E_ARG; }
+    if (p > 0 && (!A || lda < p)) { set_error("kkt_create: A must be p x n with lda >= p"); return CVXB_E_ARG; }
+    if (p > n) { set_error("kkt_create: Rank(A) < p (p > n)"); return CVXB_E_ARG; }
+    return 0;
+}
+
+// a handle on `device` with its cone layout, stream, events and Cholesky workspace; no matrix yet
+int kkt_open(std::unique_ptr<cvxb_kkt> &k, int n, int p, const cvxb_dims *dims, int device) {
+    CVXB_TRY(check_device(device));
+    k.reset(new cvxb_kkt());
+    k->device = device; k->n = n; k->p = p;
+    k->i8_mode = ozaki_mode();
+    CVXB_TRY(k->cone.init(dims));
+    CVXB_CUDA(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
+    for (cudaEvent_t *e : {&k->e0, &k->e1, &k->e2, &k->e3, &k->t0, &k->t1, &k->m0, &k->m1})
+        CVXB_CUDA(cudaEventCreate(e));
+    CVXB_TRY(chol_work_create(k->cw));
+    return 0;
+}
+
+// everything after G: K, the packed rows, A and the vectors
+int kkt_alloc(cvxb_kkt *k, const double *A, int lda, int space) {
+    const ConeLayout &c = k->cone;
+    const int n = k->n, p = k->p;
+    const size_t nn = (size_t)(n > 0 ? n : 1);
+    CVXB_TRY(k->Kmat.alloc((size_t)kkt_ldk(k) * nn));
+    const int nblk = (n + NB - 1) / NB + 1;
+    CVXB_TRY(k->inv.alloc((size_t)2 * nblk * NB * NB));   // inv + inv' blocks
+    k->nrest = c.mnl + c.sumq + c.sump;
+    if (k->nrest > 0) {
+        k->ldgs = (k->nrest + 1) & ~1;
+        CVXB_TRY(k->Gs.alloc((size_t)k->ldgs * nn));
+    }
+    if (c.sums2 > 0) {
+        CVXB_TRY(k->Gunp.alloc((size_t)c.sums2 * nn));
+        // workspace for the congruences: symmetric copies + intermediate, chunked over columns
+        size_t per_col = (size_t)2 * c.maxs * c.maxs;
+        size_t cols = (size_t)n < 1 ? 1 : (size_t)n;
+        size_t want = per_col * cols;
+        const size_t cap = (size_t)1 << 29;            // 4 GiB of doubles at most
+        if (want > cap) want = (cap / per_col ? cap / per_col : 1) * per_col;
+        CVXB_TRY(k->swork.alloc(want));
+    }
+    if (c.mnl > 0) CVXB_TRY(k->Dfbuf.alloc((size_t)c.mnl * nn));
+    if (p > 0) {
+        k->lda_eq = (p + 1) & ~1;
+        k->ldas = (n + 1) & ~1;
+        k->ldkp = (p + 1) & ~1;
+        CVXB_TRY(k->Aeq.alloc((size_t)k->lda_eq * nn));
+        CVXB_TRY(k->Asct.alloc((size_t)k->ldas * p));
+        CVXB_TRY(k->Kp.alloc((size_t)k->ldkp * p));
+        CVXB_TRY(k->invp.alloc((size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB));
+        CVXB_TRY(k->yd.alloc((size_t)p));
+        CVXB_TRY(upload_matrix(k->Aeq.p, k->lda_eq, A, lda, p, n, space, k->st));
+    }
+    CVXB_TRY(k->W.alloc(c));
+    const size_t cd = (size_t)(c.cdim > 0 ? c.cdim : 1);
+    CVXB_TRY(k->bzp.alloc(cd));
+    CVXB_TRY(k->zin.alloc(cd));
+    CVXB_TRY(k->zt.alloc(cd));
+    CVXB_TRY(k->xv.alloc(nn));
+    CVXB_TRY(k->yv.alloc(cd > nn ? cd : nn));
+    CVXB_TRY(k->gemv_ws.alloc(kkt_gemv_ws_doubles(k)));
+    CVXB_CUDA(cudaStreamSynchronize(k->st));
+    return 0;
+}
+}  // namespace
+
+namespace cvxb {
+size_t kkt_gemv_ws_doubles(const cvxb_kkt *k) {
+    const ConeLayout &c = k->cone;
+    const int n = k->n, p = k->p;
+    // the dense rows gemv_n runs on: all of them, or all but the sparse 'l' rows
+    const int rows = k->sp ? c.cdim - c.ml : c.cdim;
+    const size_t nn = (size_t)(n > 0 ? n : 1), cd = (size_t)(rows > 0 ? rows : 1);
+    size_t w1 = cd * (size_t)gemv_n_chunks(n), w2 = nn * (size_t)gemv_n_chunks(p > 0 ? p : 1);
+    const size_t w3 = (size_t)(p > 0 ? p : 1) * (size_t)gemv_n_chunks(n);      // A operator
+    if (w3 > w1) w1 = w3;
+    return w1 > w2 ? w1 : w2;
+}
 }  // namespace cvxb
 
 cvxb_kkt::~cvxb_kkt() {
@@ -325,25 +414,14 @@ int cvxb_sync(void) { CVXB_CUDA(cudaDeviceSynchronize()); return 0; }
 // --------------------------------------------------------------------- create
 int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const double *G,
                     int ldg, const double *A, int lda, int space, int device) {
-    if (!out) { set_error("kkt_create: out is NULL"); return CVXB_E_ARG; }
-    *out = nullptr;
-    if (n < 0 || p < 0) { set_error("kkt_create: negative size"); return CVXB_E_ARG; }
-    if (p > 0 && (!A || lda < p)) { set_error("kkt_create: A must be p x n with lda >= p"); return CVXB_E_ARG; }
-    if (p > n) { set_error("kkt_create: Rank(A) < p (p > n)"); return CVXB_E_ARG; }
-    CVXB_TRY(check_device(device));
-    std::unique_ptr<cvxb_kkt> k(new cvxb_kkt());
-    k->device = device; k->n = n; k->p = p;
-    k->i8_mode = ozaki_mode();
-    CVXB_TRY(k->cone.init(dims));
+    CVXB_TRY(kkt_check_args(out, n, p, A, lda));
+    std::unique_ptr<cvxb_kkt> k;
+    CVXB_TRY(kkt_open(k, n, p, dims, device));
     const ConeLayout &c = k->cone;
     if (c.cdim > 0 && (!G || ldg < (c.cdim > 1 ? c.cdim : 1))) {
         set_error("kkt_create: G must be cdim x n with ldg >= cdim (cdim=%d, ldg=%d)", c.cdim, ldg);
         return CVXB_E_ARG;
     }
-    CVXB_CUDA(cudaStreamCreateWithFlags(&k->st, cudaStreamNonBlocking));
-    for (cudaEvent_t *e : {&k->e0, &k->e1, &k->e2, &k->e3, &k->t0, &k->t1, &k->m0, &k->m1})
-        CVXB_CUDA(cudaEventCreate(e));
-    CVXB_TRY(chol_work_create(k->cw));
     const size_t nn = (size_t)(n > 0 ? n : 1);
     if (space == CVXB_DEVICE) {
         k->G = G; k->ldg = ldg;
@@ -354,50 +432,58 @@ int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const d
         k->G = k->Gown.p;
         CVXB_TRY(upload_matrix(k->Gown.p, k->ldg, G, ldg, c.cdim, n, CVXB_HOST, k->st));
     }
-    CVXB_TRY(k->Kmat.alloc((size_t)kkt_ldk(k.get()) * nn));
-    const int nblk = (n + NB - 1) / NB + 1;
-    CVXB_TRY(k->inv.alloc((size_t)2 * nblk * NB * NB));   // inv + inv' blocks
-    k->nrest = c.mnl + c.sumq + c.sump;
-    if (k->nrest > 0) {
-        k->ldgs = (k->nrest + 1) & ~1;
-        CVXB_TRY(k->Gs.alloc((size_t)k->ldgs * nn));
+    CVXB_TRY(kkt_alloc(k.get(), A, lda, space));
+    *out = k.release();
+    return 0;
+}
+
+int cvxb_kkt_create_sparse(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const long long *rowptr,
+                           const int *colind, const double *val, long long nnz, const double *A, int lda,
+                           int space, int device) {
+    CVXB_TRY(kkt_check_args(out, n, p, A, lda));
+    // the whole CSR is checked on the host, before the device is touched
+    if (!dims || dims->mnl < 0 || dims->ml < 0 || dims->nq < 0 || dims->ns < 0 ||
+        (dims->nq > 0 && !dims->q) || (dims->ns > 0 && !dims->s)) {
+        set_error("kkt_create_sparse: dims is NULL or has a negative dimension");
+        return CVXB_E_ARG;
     }
-    if (c.sums2 > 0) {
-        CVXB_TRY(k->Gunp.alloc((size_t)c.sums2 * nn));
-        // workspace for the congruences: symmetric copies + intermediate, chunked over columns
-        size_t per_col = (size_t)2 * c.maxs * c.maxs;
-        size_t cols = (size_t)n < 1 ? 1 : (size_t)n;
-        size_t want = per_col * cols;
-        const size_t cap = (size_t)1 << 29;            // 4 GiB of doubles at most
-        if (want > cap) want = (cap / per_col ? cap / per_col : 1) * per_col;
-        CVXB_TRY(k->swork.alloc(want));
+    long long cdim = (long long)dims->mnl + dims->ml;
+    for (int i = 0; i < dims->nq; ++i) cdim += dims->q[i];
+    for (int i = 0; i < dims->ns; ++i) cdim += (long long)dims->s[i] * dims->s[i];
+    if (!rowptr) { set_error("kkt_create_sparse: rowptr is NULL"); return CVXB_E_ARG; }
+    if (nnz < 0) { set_error("kkt_create_sparse: nnz = %lld is negative", nnz); return CVXB_E_ARG; }
+    if (nnz > 0 && (!colind || !val)) { set_error("kkt_create_sparse: colind or val is NULL"); return CVXB_E_ARG; }
+    if (rowptr[0] != 0) { set_error("kkt_create_sparse: rowptr[0] = %lld, must be 0", rowptr[0]); return CVXB_E_ARG; }
+    for (long long r = 0; r < cdim; ++r)
+        if (rowptr[r + 1] < rowptr[r]) {
+            set_error("kkt_create_sparse: rowptr is not monotone: rowptr[%lld] = %lld > rowptr[%lld] = %lld", r,
+                      rowptr[r], r + 1, rowptr[r + 1]);
+            return CVXB_E_ARG;
+        }
+    if (rowptr[cdim] != nnz) {
+        set_error("kkt_create_sparse: rowptr[cdim] = %lld differs from nnz = %lld", rowptr[cdim], nnz);
+        return CVXB_E_ARG;
     }
-    if (c.mnl > 0) CVXB_TRY(k->Dfbuf.alloc((size_t)c.mnl * nn));
-    if (p > 0) {
-        k->lda_eq = (p + 1) & ~1;
-        k->ldas = (n + 1) & ~1;
-        k->ldkp = (p + 1) & ~1;
-        CVXB_TRY(k->Aeq.alloc((size_t)k->lda_eq * nn));
-        CVXB_TRY(k->Asct.alloc((size_t)k->ldas * p));
-        CVXB_TRY(k->Kp.alloc((size_t)k->ldkp * p));
-        CVXB_TRY(k->invp.alloc((size_t)2 * ((p + NB - 1) / NB + 1) * NB * NB));
-        CVXB_TRY(k->yd.alloc((size_t)p));
-        CVXB_TRY(upload_matrix(k->Aeq.p, k->lda_eq, A, lda, p, n, space, k->st));
+    if (dims->mnl > 0 && rowptr[dims->mnl] != 0) {
+        set_error("kkt_create_sparse: rows [0, mnl) belong to Df and must be empty");
+        return CVXB_E_ARG;
     }
-    CVXB_TRY(k->W.alloc(c));
-    const size_t cd = (size_t)(c.cdim > 0 ? c.cdim : 1);
-    CVXB_TRY(k->bzp.alloc(cd));
-    CVXB_TRY(k->zin.alloc(cd));
-    CVXB_TRY(k->zt.alloc(cd));
-    CVXB_TRY(k->xv.alloc(nn));
-    CVXB_TRY(k->yv.alloc(cd > nn ? cd : nn));
-    {
-        size_t w1 = cd * (size_t)gemv_n_chunks(n), w2 = nn * (size_t)gemv_n_chunks(p > 0 ? p : 1);
-        const size_t w3 = (size_t)(p > 0 ? p : 1) * (size_t)gemv_n_chunks(n);      // A operator
-        if (w3 > w1) w1 = w3;
-        CVXB_TRY(k->gemv_ws.alloc(w1 > w2 ? w1 : w2));
-    }
-    CVXB_CUDA(cudaStreamSynchronize(k->st));
+    for (long long r = 0; r < cdim; ++r)
+        for (long long q = rowptr[r]; q < rowptr[r + 1]; ++q) {
+            if (colind[q] < 0 || colind[q] >= n) {
+                set_error("kkt_create_sparse: column index %d in row %lld is outside [0, n = %d)", colind[q], r, n);
+                return CVXB_E_ARG;
+            }
+            if (q > rowptr[r] && colind[q] <= colind[q - 1]) {
+                set_error("kkt_create_sparse: the columns of row %lld are %s (%d after %d)", r,
+                          colind[q] == colind[q - 1] ? "duplicate" : "unsorted", colind[q], colind[q - 1]);
+                return CVXB_E_ARG;
+            }
+        }
+    std::unique_ptr<cvxb_kkt> k;
+    CVXB_TRY(kkt_open(k, n, p, dims, device));
+    CVXB_TRY(kkt_sparse_load(k.get(), rowptr, colind, val));
+    CVXB_TRY(kkt_alloc(k.get(), A, lda, space));
     *out = k.release();
     return 0;
 }
@@ -414,7 +500,12 @@ int cvxb_kkt_set_method(cvxb_kkt *k, int method, double kktreg) {
     if (k->method != 0 || k->factored) { set_error("set_method: call once, right after create"); return CVXB_E_ARG; }
     CVXB_CUDA(cudaSetDevice(k->device));
     if (method == 0) return 0;
-    if (method == 1) { CVXB_TRY(kkt_qr_setup(k)); k->method = 1; return 0; }
+    if (method == 1) {
+        if (k->sp) CVXB_TRY(kkt_sparse_densify(k));      // the QR route needs the dense W^{-T} G
+        CVXB_TRY(kkt_qr_setup(k));
+        k->method = 1;
+        return 0;
+    }
     if (method == 2) { CVXB_TRY(kkt_ldl_setup(k, kktreg)); k->method = 2; return 0; }
     set_error("set_method: unknown method %d", method);
     return CVXB_E_ARG;
@@ -512,7 +603,12 @@ int cvxb_kkt_factor(cvxb_kkt *k, const cvxb_scaling *Wp, const double *H, int ld
             return 0;
         };
         k->syrk_path = 0;
-        if (c.ml > 0 && n > 0 && ozaki_use(k->i8_mode, n, c.ml, k->oz_work)) {
+        if (c.ml > 0 && n > 0 && k->sp) {
+            // K = H + G_l' diag(di)^2 G_l from the sparse 'l' rows; the dense terms below add onto it
+            CVXB_TRY(kkt_sparse_syrk(k, Hptr, ldH, k->W.di2, K, ldk));
+            have = true;
+            k->syrk_path = 3;
+        } else if (c.ml > 0 && n > 0 && ozaki_use(k->i8_mode, n, c.ml, k->oz_work)) {
             // G_l' diag(di)^2 G_l + H from nine int8 slices per entry (exact products, fp64-level result)
             ozaki_time_mma(k->m0, k->m1);
             CVXB_TRY(ozaki_syrk(n, c.ml, k->G + c.mnl, k->ldg, k->W.di, Hptr, ldH, 1.0, K, ldk, 9, 0,
@@ -678,7 +774,6 @@ int cvxb_kkt_gemv_G(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
     const ConeLayout &c = k->cone;
     const int n = k->n, m = c.cdim - c.mnl;
     cudaStream_t st = k->st;
-    const double *Gp = k->G + c.mnl;
     const bool tr = (trans == 'T' || trans == 't');
     const int nx = tr ? m : n, ny = tr ? n : m;
     const double *xd = x; double *yd = y;
@@ -689,8 +784,22 @@ int cvxb_kkt_gemv_G(cvxb_kkt *k, const double *x, double *y, double alpha, doubl
         if (beta != 0.0) CVXB_TRY(xfer_vec(yb, y, ny, CVXB_HOST, true, st));
         xd = xb; yd = yb;
     }
-    if (tr) CVXB_TRY(gemv_t(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, st));
-    else    CVXB_TRY(gemv_n(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, k->gemv_ws.p, st));
+    if (k->sp) {
+        // sparse 'l' rows, then the dense 'q' and 's' rows below them
+        const int ml = c.ml, mr = m - c.ml;
+        if (tr) {
+            double b = beta;
+            if (ml > 0) { CVXB_TRY(kkt_sparse_mv(k, true, nullptr, xd, alpha, b, yd)); b = 1.0; }
+            if (mr > 0 || ml == 0) CVXB_TRY(gemv_t(mr, n, k->Gown.p, k->ldg, nullptr, xd + ml, alpha, b, yd, st));
+        } else {
+            if (ml > 0) CVXB_TRY(kkt_sparse_mv(k, false, nullptr, xd, alpha, beta, yd));
+            if (mr > 0) CVXB_TRY(gemv_n(mr, n, k->Gown.p, k->ldg, nullptr, xd, alpha, beta, yd + ml, k->gemv_ws.p, st));
+        }
+    } else {
+        const double *Gp = k->G + c.mnl;
+        if (tr) CVXB_TRY(gemv_t(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, st));
+        else    CVXB_TRY(gemv_n(m, n, Gp, k->ldg, nullptr, xd, alpha, beta, yd, k->gemv_ws.p, st));
+    }
     if (space != CVXB_DEVICE) CVXB_TRY(xfer_vec(y, yd, ny, CVXB_HOST, false, st));
     CVXB_CUDA(cudaStreamSynchronize(st));
     return 0;

@@ -39,6 +39,21 @@ struct LdlState {
     DevBuf<double> u;           // N right-hand side
     double kktreg = 0.0;
 };
+
+// the 'l' rows of G kept sparse on the device (cvxb_kkt_create_sparse, kkt_sparse.cu).  Two copies of the pattern, so
+// that G x and G' y both run as row-by-row sums, without atomics.
+struct SparseL {
+    long long nnz = 0;
+    DevBuf<long long> rowptr;   // ml + 1: CSR of G_l
+    DevBuf<int> colind;         // nnz, sorted within each row
+    DevBuf<double> val;         // nnz
+    DevBuf<long long> colptr;   // n + 1: CSR of G_l' (the CSC view of G_l)
+    DevBuf<int> rowind;         // nnz, sorted within each column
+    DevBuf<double> tval;        // nnz
+    DevBuf<long long> tpos;     // nnz: index in val of the same entry, where the row's columns >= this one start
+    DevBuf<int> bnd;            // nchunk + 1 column boundaries: warp w of the SYRK owns columns [bnd[w], bnd[w+1])
+    int nchunk = 0;
+};
 }  // namespace cvxb
 
 struct cvxb_kkt {
@@ -48,6 +63,8 @@ struct cvxb_kkt {
     const double *G = nullptr;   // cdim x n, rows [mnl, cdim) hold G (rows [0,mnl) belong to Df)
     DevBuf<double> Gown;         // backs G when it came from the host; a device G stays the caller's
     long long ldg = 0;
+    // sparse 'l' rows (cvxb_kkt_create_sparse): G is unused, and Gown holds only the 'q' and 's' rows (ld ldg)
+    std::unique_ptr<cvxb::SparseL> sp;
     DevBuf<double> Hres;         // resident H (symmetrised), or empty
     DevBuf<double> Hbuf;         // per-call H upload buffer (lazy)
     DevBuf<double> Kmat;         // n x n: normal equations, then its Cholesky factor (lower)
@@ -83,7 +100,8 @@ struct cvxb_kkt {
     // H100 the fp64 DMMA kernel is the faster of the two at every size measured (DESIGN.md).
     int i8_mode = 0;
     DevBuf<char> oz_work;
-    int syrk_path = 0;           // kernel of the last factor's 'l'-row SYRK: 0 none, 1 fp64 DMMA, 2 int8 slices
+    int syrk_path = 0;           // kernel of the last factor's 'l'-row SYRK: 0 none, 1 fp64 DMMA, 2 int8 slices,
+                                 // 3 sparse (kkt_sparse.cu)
     // factorisation route: 0 Cholesky of the reduced system (kkt_chol / kkt_chol2), 1 QR (kkt_qr), 2 LDL' of the
     // 2x2 system (kkt_ldl2).  Set once after create (cvxb_kkt_set_method), with the state of that route.
     int method = 0;
@@ -112,4 +130,20 @@ int kkt_qr_setup(cvxb_kkt *k);
 int kkt_ldl_factor(cvxb_kkt *k);
 int kkt_ldl_solve(cvxb_kkt *k, double *xd, double *yd);
 int kkt_ldl_setup(cvxb_kkt *k, double kktreg);
+// first 'q' row of G (ld k->ldg); the 's' rows follow it
+inline const double *kkt_G_qs(const cvxb_kkt *k) {
+    return k->sp ? k->Gown.p : k->G + k->cone.mnl + k->cone.ml;
+}
+// sparse 'l' rows (kkt_sparse.cu).  kkt_sparse_load: rowptr/colind/val are the validated host CSR of all cdim rows;
+// it keeps the 'l' rows sparse, or densifies them when the dense SYRK is the faster path.
+int kkt_sparse_load(cvxb_kkt *k, const long long *rowptr, const int *colind, const double *val);
+// turn a sparse handle into a dense one: rows [mnl, cdim) of a new dense G, on the device
+int kkt_sparse_densify(cvxb_kkt *k);
+// K (lower) := D + G_l' diag(w) G_l, D lower (ld ldd) or zero when D is NULL
+int kkt_sparse_syrk(cvxb_kkt *k, const double *D, long long ldd, const double *w, double *K, long long ldk);
+// y := alpha diag(w) G_l x + beta y (trans false, y has ml entries) or alpha G_l' diag(w) x + beta y (trans true,
+// y has n entries); w may be NULL
+int kkt_sparse_mv(cvxb_kkt *k, bool trans, const double *w, const double *x, double alpha, double beta, double *y);
+// doubles of gemv_n workspace the handle needs
+size_t kkt_gemv_ws_doubles(const cvxb_kkt *k);
 }  // namespace cvxb

@@ -13,8 +13,13 @@ Usage with an unmodified CVXOPT (the plugin boundary, coneprog.py:323-344 /
 solver-owned vectors in place with (ux, uy, W*uz), exactly like the reference
 closure.  Any object exposing the buffer protocol with fp64 column-major data
 works (cvxopt.matrix, numpy F-ordered arrays); cvxopt itself is not imported.
+
+G, A, H and Df may also be sparse: a cvxopt `spmatrix` (recognised by its `CCS`
+and `size` attributes) or any scipy.sparse matrix.  The 'l' rows of G stay
+sparse on the device; everything else is densified once (INTEGRATION.md §1).
 """
 import ctypes as C
+import sys
 
 import numpy as np
 
@@ -36,6 +41,60 @@ def _mat(a, name="matrix"):
     if not arr.flags.f_contiguous:
         arr = np.asfortranarray(arr)
     return arr
+
+
+def is_sparse(a):
+    """a cvxopt spmatrix (duck-typed: the package never imports cvxopt) or a scipy.sparse matrix"""
+    if hasattr(a, "CCS") and hasattr(a, "size"):
+        return True
+    sps = sys.modules.get("scipy.sparse")      # a scipy.sparse matrix exists only once scipy.sparse is imported
+    return sps is not None and sps.issparse(a)
+
+
+def to_csr(a, name="matrix"):
+    """spmatrix or scipy.sparse -> ((rows, cols), rowptr int64, colind int32, val float64), canonical CSR: columns
+    sorted within each row, duplicate entries summed (in their order of appearance), explicit zeros kept."""
+    if hasattr(a, "CCS") and hasattr(a, "size"):
+        rows, cols = (int(k) for k in a.size)
+        colptr, rowind, vals = a.CCS
+        colptr = np.asarray(colptr, dtype=np.int64).ravel()
+        r = np.asarray(rowind, dtype=np.int64).ravel()
+        c = np.repeat(np.arange(cols, dtype=np.int64), np.diff(colptr))
+        v = np.asarray(vals).ravel()
+    else:
+        coo = a.tocoo()
+        rows, cols = (int(k) for k in coo.shape)
+        r = np.asarray(coo.row, dtype=np.int64)
+        c = np.asarray(coo.col, dtype=np.int64)
+        v = np.asarray(coo.data)
+    if v.dtype.kind not in "iuf":
+        raise TypeError("%s must be a real 'd' matrix" % name)
+    v = v.astype(np.float64)
+    if r.size != v.size or c.size != v.size:
+        raise TypeError("%s: inconsistent sparse storage" % name)
+    if r.size and (r.min() < 0 or r.max() >= rows or c.min() < 0 or c.max() >= cols):
+        raise TypeError("%s: an index is outside its %d x %d shape" % (name, rows, cols))
+    order = np.lexsort((c, r))                   # stable: duplicates stay in their order of appearance
+    r, c, v = r[order], c[order], v[order]
+    if r.size:
+        first = np.ones(r.size, dtype=bool)
+        first[1:] = (r[1:] != r[:-1]) | (c[1:] != c[:-1])
+        starts = np.flatnonzero(first)
+        v = np.add.reduceat(v, starts)
+        r, c = r[starts], c[starts]
+    rowptr = np.zeros(rows + 1, dtype=np.int64)
+    np.cumsum(np.bincount(r, minlength=rows), out=rowptr[1:])
+    return (rows, cols), rowptr, np.ascontiguousarray(c, dtype=np.int32), np.ascontiguousarray(v)
+
+
+def _dense(a, name="matrix"):
+    """_mat, for sparse input too: a sparse matrix is densified"""
+    if not is_sparse(a):
+        return _mat(a, name)
+    (rows, cols), rowptr, colind, val = to_csr(a, name)
+    out = np.zeros((rows, cols), order="F")
+    out[np.repeat(np.arange(rows), np.diff(rowptr)), colind] = val
+    return out
 
 
 def _vec_inplace(a, n, name):
@@ -119,8 +178,15 @@ class KKTChol:
     def __init__(self, G, dims, A=None, mnl=0, H=None, device=0, method="chol", kktreg=0.0):
         self._lib = _lib.load()
         self._h = C.c_void_p()
-        Gm = _mat(G, "G")
-        self.n = Gm.shape[1]
+        # a sparse G keeps its 'l' rows sparse; the QR route needs the dense W^{-T} G and densifies all of G, as the
+        # reference does
+        sparse = is_sparse(G) and method != "qr"
+        if sparse:
+            gshape, rowptr, colind, val = to_csr(G, "G")
+        else:
+            Gm = _dense(G, "G")
+            gshape = Gm.shape
+        self.n = gshape[1]
         self.dims = {"l": int(dims["l"]), "q": [int(k) for k in dims["q"]],
                      "s": [int(k) for k in dims["s"]]}
         self.mnl = int(mnl)
@@ -129,21 +195,30 @@ class KKTChol:
             p = 0
             Am = None
         else:
-            Am = _mat(A, "A")
+            Am = _dense(A, "A")
             p = Am.shape[0]
             if p and Am.shape[1] != self.n:
                 raise TypeError("A must have %d columns" % self.n)
         self.p = p
         # the reference allocates Gs as (cdim, n) and copies G into rows mnl: (misc.py:1252,1270)
-        if Gm.shape[0] != self.cdim - self.mnl:
+        if gshape[0] != self.cdim - self.mnl:
             raise TypeError("G must be a 'd' matrix of size (%d, %d)" % (self.cdim - self.mnl, self.n))
-        if self.mnl:
-            full = np.zeros((self.cdim, self.n), order="F")
-            full[self.mnl:, :] = Gm
-            Gm = full
-        rc = self._lib.cvxb_kkt_create(
-            C.byref(self._h), self.n, p, C.byref(self._cd), Gm.ctypes.data, max(1, Gm.shape[0]),
-            Am.ctypes.data if (Am is not None and p) else None, max(1, p), _lib.HOST, device)
+        Ap = Am.ctypes.data if (Am is not None and p) else None
+        if sparse:
+            # rows [0, mnl) of the factory's G belong to Df: empty rows of the CSR
+            rowptr = np.ascontiguousarray(np.concatenate([np.zeros(self.mnl, dtype=np.int64), rowptr]))
+            rc = self._lib.cvxb_kkt_create_sparse(
+                C.byref(self._h), self.n, p, C.byref(self._cd), rowptr.ctypes.data,
+                colind.ctypes.data if colind.size else None, val.ctypes.data if val.size else None,
+                int(val.size), Ap, max(1, p), _lib.HOST, device)
+        else:
+            if self.mnl:
+                full = np.zeros((self.cdim, self.n), order="F")
+                full[self.mnl:, :] = Gm
+                Gm = full
+            rc = self._lib.cvxb_kkt_create(
+                C.byref(self._h), self.n, p, C.byref(self._cd), Gm.ctypes.data, max(1, Gm.shape[0]),
+                Ap, max(1, p), _lib.HOST, device)
         _lib.check(rc, "kkt_chol")
         self.method = method
         if method != "chol":
@@ -160,7 +235,7 @@ class KKTChol:
 
     # -- resident H ---------------------------------------------------------
     def set_H(self, H):
-        Hm = _mat(H, "H")
+        Hm = _dense(H, "H")
         if Hm.shape != (self.n, self.n):
             raise TypeError("H must be a 'd' matrix of size (%d, %d)" % (self.n, self.n))
         _lib.check(self._lib.cvxb_kkt_set_H(self._h, Hm.ctypes.data, max(1, self.n), _lib.HOST), "set_H")
@@ -177,7 +252,7 @@ class KKTChol:
         if H is None or H is self._H_resident:
             use_res = 1 if self._H_resident is not None else 0
         else:
-            Hm = _mat(H, "H")
+            Hm = _dense(H, "H")
             if Hm.shape != (self.n, self.n):
                 raise TypeError("H must be a 'd' matrix of size (%d, %d)" % (self.n, self.n))
             keep.append(Hm)
@@ -186,7 +261,7 @@ class KKTChol:
         if self.mnl:
             if Df is None:
                 raise TypeError("Df is required when mnl > 0")
-            Dm = _mat(Df, "Df")
+            Dm = _dense(Df, "Df")
             if Dm.shape != (self.mnl, self.n):
                 raise TypeError("Df must be a 'd' matrix of size (%d, %d)" % (self.mnl, self.n))
             keep.append(Dm)
@@ -280,8 +355,8 @@ class KKTChol:
         return out
 
     def syrk_path(self):
-        """'none' | 'dmma' | 'int8': the kernel that computed the last factor's 'l'-row SYRK"""
-        return ("none", "dmma", "int8")[self._lib.cvxb_kkt_syrk_path(self._h)]
+        """'none' | 'dmma' | 'int8' | 'sparse': the kernel that computed the last factor's 'l'-row SYRK"""
+        return ("none", "dmma", "int8", "sparse")[self._lib.cvxb_kkt_syrk_path(self._h)]
 
     def qr_passes(self):
         """QR route: 2 = Cholesky-QR with re-orthogonalisation, 3 = the shifted variant took over"""

@@ -86,6 +86,18 @@ int  cvxb_sync(void);
 int cvxb_kkt_create(cvxb_kkt **out, int n, int p, const cvxb_dims *dims,
                     const double *G, int ldg, const double *A, int lda,
                     int space, int device);
+/* The same factory for a sparse G: cdim x n in CSR form with 0-based indices, rows [0, mnl) empty (they belong to
+ * Df).  rowptr (cdim + 1 entries), colind and val (nnz each) are HOST arrays whatever `space` is; `space` applies to A.
+ * The columns of each row must be sorted and distinct.  Every check is made before the device is touched: rowptr[0] != 0,
+ * a decreasing rowptr, rowptr[cdim] != nnz, a column outside [0, n), unsorted or duplicate columns in a row, and
+ * entries in rows [0, mnl) return CVXB_E_ARG with the fault named in cvxb_last_error().
+ * The 'l' rows stay sparse on the device (a CSR copy and a CSR copy of their transpose) and their SYRK and GEMVs run
+ * on sparse kernels; when sum over 'l' rows of nnz(row)^2 is too large against ml n^2 for that to pay, they are
+ * densified once here and take the dense path (cvxb_kkt_syrk_path tells which).  The 'q' and 's' rows are kept dense.
+ * Every other call works on this handle as on a dense one; route 1 (QR) densifies the 'l' rows first. */
+int cvxb_kkt_create_sparse(cvxb_kkt **out, int n, int p, const cvxb_dims *dims, const long long *rowptr,
+                           const int *colind, const double *val, long long nnz, const double *A, int lda,
+                           int space, int device);
 void cvxb_kkt_destroy(cvxb_kkt *k);
 
 /* Factorisation route of this factory, chosen once right after cvxb_kkt_create:
@@ -132,7 +144,8 @@ int cvxb_kkt_trace(cvxb_kkt *k, unsigned long long *out, int nsteps);
 int cvxb_kkt_last_breakdown(cvxb_kkt *k, double *ms3);
 /* which kernel computed the 'l'-row SYRK of the last factor: 0 none (ml == 0), 1 fp64 DMMA
  * (mma.sync.m16n8k4.f64, the default), 2 int8 slices on wgmma s8 (CVXB_OZAKI=2 always, =1 for large problems;
- * falls back to 1 when the slice workspace does not fit in device memory) */
+ * falls back to 1 when the slice workspace does not fit in device memory), 3 the sparse kernel of a
+ * cvxb_kkt_create_sparse handle that kept its 'l' rows sparse */
 int cvxb_kkt_syrk_path(cvxb_kkt *k);
 /* int8-slice path only: CUDA-event time of the MMA launches of the last factor's SYRK, without the two slicing kernels
  * (0 on the DMMA path); bench.py's roofline line divides the int8 operations by this */
